@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """bench.py — learner transitions/s for the Ape-X hot path (sample + gather +
-target + priority update, inside a full learner step) on N B200s.
+target + priority update, inside a full learner step) on N H100s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
 
@@ -49,12 +49,12 @@ ALG_BYTES_PER_TRANSITION_GATHER = 2 * 28224 + 4 + 4 + 1   # SURVEY.md §8d: 56 4
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=1000)
+    ap.add_argument("--steps", type=int, default=None, help="timed steps (default: 1000 for apex, 40 for r2d2 / impala)")
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default="apex", choices=["apex", "r2d2", "impala"],
                     help="apex = BASELINE.json configs[1] (the headline the driver runs); r2d2 / impala = configs[2] / "
-                         "configs[3] (secondary lines, same JSON contract; --steps defaults apply to apex only)")
+                         "configs[3] (secondary lines, same JSON contract)")
     ap.add_argument("--log2pool", type=int, default=14, help="r2d2: log2 of distinct stored sequences (payload pool)")
     ap.add_argument("--log2rollouts", type=int, default=15, help="impala: log2 of rollouts kept per GPU")
     ap.add_argument("--log2n", type=int, default=20, help="log2 of replay slots per GPU")
@@ -66,7 +66,7 @@ def parse():
     ap.add_argument("--inline-wgrad", action="store_true", help="weight gradients inline in backward instead of on a side stream")
     ap.add_argument("--serial-forwards", action="store_true", help="the three forward passes of a step on one stream")
     ap.add_argument("--unfused-tail", action="store_true", help="dueling tail as separate PyTorch ops instead of csrc/dueling.cu")
-    ap.add_argument("--cublas-dense", action="store_true", help="dense heads as cuBLAS fp32 GEMMs instead of the 3xTF32 tcgen05 kernel (csrc/gemm.cu)")
+    ap.add_argument("--cublas-dense", action="store_true", help="dense heads as cuBLAS fp32 GEMMs instead of the 3xTF32 wgmma kernel (csrc/gemm.cu)")
     ap.add_argument("--torch-optim", action="store_true", help="torch.optim.RMSprop instead of the fused kernel")
     ap.add_argument("--no-cudnn-benchmark", action="store_true", help="leave cuDNN's algorithm choice to its heuristics")
     ap.add_argument("--blaslt", action="store_true", help="route fp32 GEMMs through cuBLASLt")
@@ -79,8 +79,14 @@ def parse():
                     help="profiling aid: only the device-resident loop (no per-kernel timing, e2e or CPU baseline); "
                          "the line it prints is NOT a bench result")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write what the last one returned (Learner.fused_step of the workload, "
+                         "e.g. sampled indices, new priorities, loss scalars, gradient norm) as DIR/<name>.npy")
     ap.add_argument("--cpu-steps", type=int, default=48)
-    return ap.parse_args()
+    a = ap.parse_args()
+    if a.steps is None:
+        a.steps = 1000 if a.workload == "apex" else 40     # the secondary steps are milliseconds long
+    return a
 
 
 # --------------------------------------------------------------------------- #
@@ -244,8 +250,8 @@ def workload_config(args, world):
             "record_bytes": ALG_BYTES_PER_TRANSITION_GATHER,
             "parallelism": f"replay-sharded dp{world}" if world > 1 else "single GPU",
             "l2": "inputs >> L2: every step gathers random rows of a 59 GB payload (no L2 flush needed)",
-            "network": "dueling DQN of cfg/ape_x.json; conv_1 forward and weight gradient fused with the gather on tcgen05 "
-                       "(int8 digits, fp32-exact), dense heads as 3xTF32 tcgen05 GEMMs at fp32 accuracy, fused dueling tail; "
+            "network": "dueling DQN of cfg/ape_x.json; conv_1 forward and weight gradient fused with the gather on wgmma "
+                       "(int8 digits, fp32-exact), dense heads as 3xTF32 wgmma GEMMs at fp32 accuracy, fused dueling tail; "
                        "conv_2/conv_3 in cuDNN at PyTorch's default precision (TF32 convs) = what the reference runs"}
 
 
@@ -297,7 +303,7 @@ def secondary_workload(args):
     torch.cuda.set_device(dev)
     torch.backends.cudnn.benchmark = not args.no_cudnn_benchmark
     lib = _lib.load()
-    steps = args.steps if args.steps != 1000 else 40
+    steps = args.steps
     warm = max(3, min(args.warmup, 5))
     g = torch.Generator(device=dev); g.manual_seed(0xB200 + 7)
     peaks = {}
@@ -305,7 +311,7 @@ def secondary_workload(args):
         peaks = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
 
     if args.workload == "r2d2":
         from distributed_rl_b200 import r2d2
@@ -343,7 +349,7 @@ def secondary_workload(args):
               "record_bytes": unit_bytes, "burn_in": cfg.MEM, "n_step": cfg.UNROLL_STEP,
               "l2": "inputs >> L2: every step reads 64 random 2.26 MB sequences of a 37 GB payload",
               "network": "conv stack -> LSTM(3136,512) -> dueling heads of cfg/r2d2.json; conv_1 (all 80x64 frames, online + "
-                         "target) fused with the in-place gather on tcgen05; conv_2/3 + LSTM cuDNN; heads 3xTF32 tcgen05; Adam"}
+                         "target) fused with the in-place gather on wgmma; conv_2/3 + LSTM cuDNN; heads 3xTF32 wgmma; Adam"}
         conv_rows, c_out, nets = (T - cfg.MEM) * B, 32, 2
     else:
         from distributed_rl_b200 import impala
@@ -374,7 +380,7 @@ def secondary_workload(args):
               "l2": f"inputs >> L2: every step reads {B} random 593 KB rollouts of a {cap * unit_bytes / 1e9:.1f} GB payload",
               "network": "the reference's runnable policy (cfg/impala.json: conv 8x8s4-16, 4x4s2-32, MLP 2592-256-7): its "
                          "'ResNet-small' (baseNetwork.py:796-820) is broken upstream (SURVEY §8d C4); conv_1 of all "
-                         "21 x 1024 frames fused with the in-place gather on tcgen05 (C_OUT=16)"}
+                         "21 x 1024 frames fused with the in-place gather on wgmma (C_OUT=16)"}
         conv_rows, c_out, nets = (T + 1) * B, 16, 1
 
     def timed_region(k):
@@ -395,6 +401,8 @@ def secondary_workload(args):
     c0 = lib.b2rl_launch_count()
     ms, out = timed_region(steps)
     launches = lib.b2rl_launch_count() - c0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, out)
     clock_info = clocks.stop()
     value = units * (T if args.workload == "r2d2" else T) * steps / (ms / 1e3)
 
@@ -419,10 +427,10 @@ def secondary_workload(args):
     alg = conv_rows * (28224 + nets * 400 * c_out * 4)
     c_ach = alg / (c_us * 1e-6) / 1e9
     data_path = units * unit_bytes / ((ms / steps) * 1e-3) / 1e9
-    roofline = {"kernel": f"k_conv1_fused<{nets},{c_out}> — fused in-place gather + im2col + tcgen05 conv_1 over one step's "
+    roofline = {"kernel": f"k_conv1_fused<{nets},{c_out}> — fused in-place gather + im2col + wgmma conv_1 over one step's "
                           f"{conv_rows} frame stacks", "bound": "hbm", "achieved": c_ach, "peak": peak, "unit": "GB/s",
                 "frac": c_ach / peak, "traffic": None, "launch_us": c_us, "algorithmic_bytes_per_launch": alg,
-                "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "fallback 6650",
+                "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "H100 SXM data sheet, 3350 GB/s",
                 "whole_step_data_path": {"bytes_per_unit": unit_bytes, "units_per_step": units,
                                          "achieved_GBs": data_path, "frac": data_path / peak,
                                          "note": "SURVEY §8d per-unit gather bytes x units / step time: the step is bound by the "
@@ -483,6 +491,17 @@ def secondary_workload(args):
 # --------------------------------------------------------------------------- #
 # our arm                                                                       #
 # --------------------------------------------------------------------------- #
+def dump_outputs(d, out):
+    """One .npy per returned array: integers as float64 (exact below 2^53), floating point as float32 / float64."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    for name, v in out.items():
+        a = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
+        a = a.astype(np.float32 if a.dtype in (np.float16, np.float32) else np.float64)
+        np.save(os.path.join(d, name + ".npy"), a)
+
+
 def main():
     args = parse()
     if args.workload != "apex":
@@ -570,6 +589,8 @@ def main():
     clock_info = clocks.stop() if clocks else None
     value = B * world * args.steps / (ms / 1e3)
     scal = out["scalars"].tolist()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out)
 
     if args.quick:
         if rank == 0:
@@ -600,8 +621,8 @@ def main():
         peaks = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)" if peaks else "fallback 6650"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)" if peaks else "H100 SXM data sheet, 3350 GB/s"
     outb = store.alloc_batch(B)
     gather_us = time_graph(lambda ix: store.gather(ix, outb))
     g_ach = ALG_BYTES_PER_TRANSITION_GATHER * B / (gather_us * 1e-6) / 1e9
@@ -624,12 +645,11 @@ def main():
                                        "frac": c_ach / peak, "int8_TOPS": ops / (c_us * 1e-6) / 1e12,
                                        "note": "reads 28 224 B per sampled s' directly from the replay payload "
                                                "(no staging copy) and writes conv_1 activations of both networks"}
-        roofline = {"kernel": "k_conv1_fused<2> — fused TMA gather + im2col + tcgen05 conv_1 (online+target) of s'",
+        roofline = {"kernel": "k_conv1_fused<2> — fused TMA gather + im2col + wgmma conv_1 (online+target) of s'",
                     "bound": "hbm", "achieved": c_ach, "peak": peak, "unit": "GB/s", "frac": c_ach / peak,
                     "peak_source": peak_src, "traffic": None, "launch_us": c_us, "algorithmic_bytes_per_launch": alg,
                     "note": "algorithmic bytes = sampled frames read (SURVEY §8d: 28 224 B per frame stack) + the two "
-                            "fp32 NHWC activation maps written; currently epilogue/issue-bound, not HBM-bound "
-                            "(tensor pipe 21.6 % active, profiles/r01_conv1.md)"}
+                            "fp32 NHWC activation maps written"}
     if cfg.FUSED_CONV1 and learner._conv1_ready():
         # fused gather + conv_1 weight gradient: reads B frame stacks + dL/dy (B x 400 x 32 fp32), writes 8192 floats
         alg_w = B * (28224 + 400 * 32 * 4)
@@ -646,7 +666,7 @@ def main():
         from distributed_rl_b200 import linear as LIN
         # the forward call of the step: the online network's two passes run as ONE M = 2B GEMM (BATCHED_ONLINE)
         batched = bool(cfg.BATCHED_ONLINE and cfg.PARALLEL_FORWARDS and cfg.FUSED_CONV1)
-        tpeak = float(peaks.get("bf16_tflops", 1719.3))
+        tpeak = float(peaks.get("bf16_tflops", 989.0))
 
         def time_gemm(Mg, Ng, Kg):
             xa = LIN.split_pack(torch.randn(Mg, Kg, device=dev), False, False)
@@ -669,9 +689,9 @@ def main():
             u1, f1, a1 = time_gemm(B, Ng, Kg)
             kernels["k_gemm_tf32x3(M=B, target-net call)"] = {"launch_us": u1, "algorithmic_flops_per_launch": f1,
                                                               "achieved_TFLOPs": a1, "frac": a1 / tpeak, "shape_MNK": [B, Ng, Kg]}
-        roofline = {"kernel": "k_gemm_tf32x3 — fp32-accurate dense heads as 3xTF32 tcgen05 GEMM (largest share of the step)",
+        roofline = {"kernel": "k_gemm_tf32x3 — fp32-accurate dense heads as 3xTF32 wgmma GEMM (largest share of the step)",
                     "bound": "tensor", "achieved": t_ach, "peak": tpeak, "unit": "TFLOP/s", "frac": t_ach / tpeak,
-                    "peak_source": "measured (MEASURED_PEAKS.json bf16_tflops, burst)" if peaks else "fallback 1719.3",
+                    "peak_source": "measured (MEASURED_PEAKS.json bf16_tflops, burst)" if peaks else "H100 SXM data sheet, dense BF16 989 TFLOP/s",
                     "traffic": None, "launch_us": g_us, "algorithmic_flops_per_launch": alg_fl, "shape_MNK": [Mg, Ng, Kg],
                     "note": "achieved counts the fp32 GEMM's 2MNK flops once; the tensor pipe executes 3x that in TF32 "
                             "(tf32_TFLOPs_executed), whose dense peak is bf16/2 — see kernels[k_gemm_tf32x3]"}
@@ -748,17 +768,6 @@ def main():
         "achieved_GBs": (b_sample + b_update) * B / ((s_us + upd[str(B)]["launch_us"]) * 1e-6) / 1e9,
         "frac": (b_sample + b_update) * B / ((s_us + upd[str(B)]["launch_us"]) * 1e-6) / 1e9 / peak,
         "bound": "latency (dependent loads), not bandwidth: 129 KB per launch cannot occupy HBM"}
-    prof = os.path.join(REPO, "profiles", "r02_traffic.json")
-    if os.path.isfile(prof):
-        try:
-            tr = json.load(open(prof))
-            key = next((k for k in ("k_gemm_tf32x3", "k_conv1_fused<2>", "k_gather_bulk") if k in kernels and k in tr),
-                       None)
-            roofline["traffic"] = tr.get(key) if key else None
-            roofline["traffic_source"] = "profiles/r02_traffic.json (dram__bytes_read.sum + dram__bytes_write.sum of one " \
-                                         "ncu --set full capture of this kernel, per launch; not re-measured in this run)"
-        except Exception:
-            pass
 
     # ---- e2e: public API, host buffers in, scalars out -----------------------------------
     from distributed_rl_b200.hostmem import pinned_like, pinned_empty   # pinned pages on the GPU's NUMA node

@@ -86,7 +86,7 @@ def load() -> C.CDLL:
     if not os.path.isfile(LIB_PATH):
         raise B2RLError(
             f"{LIB_PATH} is missing — build it with `python -m distributed_rl_b200.build` "
-            "(nvcc, sm_100a).  There is deliberately no CPU fallback for the product path.")
+            "(nvcc, sm_90a).  There is deliberately no CPU fallback for the product path.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         try:

@@ -152,7 +152,7 @@ class DenseStack(nn.Sequential):
     def _layer(self, layer, x):
         if (self.dense_3xtf32 and isinstance(layer, nn.Linear) and layer.bias is None and x.is_cuda and x.dim() == 2
                 and x.dtype == torch.float32 and layer.out_features >= 64 and layer.in_features >= 64):
-            from .linear import linear3x          # fp32 SIMT sgemm -> 3xTF32 tcgen05 GEMM at fp32 accuracy
+            from .linear import linear3x          # fp32 SIMT sgemm -> 3xTF32 wgmma GEMM at fp32 accuracy
             return linear3x(x, layer.weight)
         return layer(x)
 

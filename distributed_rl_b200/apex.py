@@ -51,14 +51,14 @@ class ApexConfig:
         "centered": True})
     MODEL: dict = field(default_factory=lambda: default_apex_model())
     CHANNELS_LAST: bool = True      # NHWC activations/weights: cuDNN's TF32 kernels skip their layout transposes
-    FUSED_CONV1: bool = True        # gather + conv_1 on the tcgen05 tensor cores (csrc/conv1.cu) in fused_step
+    FUSED_CONV1: bool = True        # gather + conv_1 on the wgmma tensor cores (csrc/conv1.cu) in fused_step
     FUSED_OPTIM: bool = True        # RMSprop + zero_grad + grad-norm in one launch (csrc/optim.cu)
     EARLY_HEAD_UPDATE: bool = True  # RMSprop of the dense heads as soon as their gradients are final (no clipping in :123-138)
     CUDNN_BENCHMARK: bool = True    # let cuDNN time its conv_2/conv_3 algorithms once (no precision change)
     DEFERRED_WGRAD: bool = True      # weight gradients on a side stream, off the critical path of backward
     PARALLEL_FORWARDS: bool = True   # the three forward passes of a step on three streams (fork/join inside the graph)
     FUSED_DUELING_TAIL: bool = True  # heads' second layers + dueling combine in one kernel (csrc/dueling.cu)
-    DENSE_3XTF32: bool = True       # dense heads as 3xTF32 tcgen05 GEMMs at fp32 accuracy (csrc/gemm.cu)
+    DENSE_3XTF32: bool = True       # dense heads as 3xTF32 wgmma GEMMs at fp32 accuracy (csrc/gemm.cu)
     BATCHED_ONLINE: bool = True     # the online net's two passes (s with grad, s' without) as ONE B = 2*BATCHSIZE call
 
     @staticmethod

@@ -1,4 +1,4 @@
-// Shared declarations for libb2rl (sm_100a).  Built with -fmad=false so every
+// Shared declarations for libb2rl (sm_90a).  Built with -fmad=false so every
 // fp32/fp64 operation is individually rounded, which is what makes the kernels
 // bit-comparable with the numpy oracle (oracle/oracle.py).
 #pragma once

@@ -1,4 +1,4 @@
-// Fused gather + first convolution of the Q-network on the 5th-gen tensor cores.
+// Fused gather + first convolution of the Q-network on the Hopper tensor cores (wgmma).
 //
 //   y[k, oy, ox, co] = relu?( (1/255) * sum_{c,ky,kx} W[co, c, ky, kx] * frame[idx[k]][c, 4oy+ky, 4ox+kx] )
 //
@@ -7,38 +7,30 @@
 // (online + target) in ONE pass over the sampled uint8 frame stacks.  It replaces,
 // for the consumer of the gather, the staging copy + fp32 conversion + cuDNN conv
 // (APE_X/Learner.py:61-67,78,85,87): the sampled rows go HBM -> SMEM (TMA bulk copy)
-// -> im2col in SMEM -> tcgen05.mma -> TMEM -> registers -> NHWC fp32 activations, and
-// the uint8 frames are never written back to HBM.
+// -> im2col in SMEM -> wgmma -> registers -> NHWC fp32 activations, and the uint8
+// frames are never written back to HBM.
 //
-// Arithmetic (DESIGN.md §4.6): the pixels are exact uint8, so the MMA runs in
-// kind::i8 (u8 x s8 -> s32, exact).  fp32 weights are split per output channel into
-// four signed 7-bit digits, W = s * (q0 + q1/2^7 + q2/2^14 + q3/2^21) (+- s*2^-22),
-// which are four groups of 32 columns of the same MMA (N = 128 per network).  The
-// epilogue recombines the exact integer sums in fp32, so the result equals an fp32
-// convolution to ~2 ulp — tighter than cuDNN's TF32 path the reference would run.
+// Arithmetic (DESIGN.md §4.6): the pixels are exact uint8, so the MMA runs on u8 x s8 -> s32
+// (exact).  fp32 weights are split per output channel into four signed 7-bit digits,
+// W = s * (q0 + q1/2^7 + q2/2^14 + q3/2^21) (+- s*2^-22), which are four groups of C_OUT
+// columns of the same MMA (N = 128 per network).  The epilogue recombines the exact integer
+// sums in fp32, so the result equals an fp32 convolution to ~2 ulp — tighter than cuDNN's
+// TF32 path the reference would run.
 //
-// (A bf16 x 3-term variant with a single fp32 accumulator was tried: it needs 48 MMA
-// instructions per tile instead of 8 and twice the im2col bytes, and measured 1.4-1.6x slower —
-// tcgen05.mma issue costs ~70 cycles per instruction here; profiles/r01_conv1.md.)
-//
-// Warp roles per CTA (persistent, one CTA per SM, 28 warps):
-//   warp 0       TMA loader: weights once, then one 28 224-byte frame stack per item
-//   warp 1       MMA issuer (one elected thread): 8 x tcgen05.mma (K = 32) per 128-row tile
-//   warp 2       TMEM allocator
-//   warps 4-11   im2col producers: SMEM frame -> 128B-swizzled K-major A tile (uint8);
+// Warp roles per CTA (persistent, one CTA per SM, 17 warps):
+//   warps 0-7    two consumer warpgroups, 64 rows of every 128-row tile each: per network
+//                8 x wgmma m64nNk32 (N = 4 * C_OUT), then recombine digits -> scale -> ReLU ->
+//                NHWC stores straight from the accumulator fragment
+//   warps 8-15   im2col producers: SMEM frame -> 128B-swizzled K-major A tile (uint8);
 //                thread = (tile row, channel pair)
-//   warps 12-27  epilogue, four groups of 4 (one warp per TMEM lane quarter = four epilogue warps per SM
-//                sub-partition; a single warp per sub-partition was dependent-issue-latency bound at ~2.2 k
-//                cycles per tile, profiles/r02_conv1.md).  The accumulator is buffered 4 / n_nets deep in
-//                TMEM and group g takes network g % n_nets of the tiles in buffer g / n_nets:
-//                tcgen05.ld -> recombine digits -> scale -> ReLU -> swizzled SMEM block -> stores of
-//                full 64-byte segments (16 channels at a time, 72 registers per thread)
+//   warp 16      TMA loader: weights once, then one 28 224-byte frame stack per item
 #include "common.cuh"
-
-#include <stdlib.h>
+#include "hopper.cuh"
 
 namespace b2rl {
 namespace conv1 {
+
+using namespace sm90;
 
 constexpr int C_IN = 4, HW = 84, KS = 8, STRIDE = 4, OHW = 20;
 constexpr int C_OUT_MAX = 32;                      // output channels: 32 (Ape-X / R2D2) or 16 (IMPALA), a template parameter
@@ -49,87 +41,11 @@ constexpr int TILE_M = 128;
 constexpr int TILES = (POS + TILE_M - 1) / TILE_M; // 4 (the last one has 16 valid rows)
 constexpr int NSPLIT = 4;
 constexpr int A_STAGES = 2;
-constexpr int EPI_WARPS = 16;
-constexpr int STAGE_OUT_BYTES = EPI_WARPS * 32 * 64;   // epilogue staging: 16 warps x 32 rows x 64 B
 constexpr int A_TILE_BYTES = TILE_M * K_TOTAL;     // 32 768: 2 K-chunks x 128 rows x 128 B
 constexpr int A_CHUNK_BYTES = TILE_M * 128;        // 16 384
 constexpr int RAW_STRIDE = 28288;                  // FRAME_BYTES rounded up to 128
-constexpr int THREADS = 896;                       // 28 warps: 3 role warps, 1 spare, 8 producers, 16 epilogue
-constexpr int PRODUCERS = 256;
-
-// ---- PTX wrappers -----------------------------------------------------------
-__device__ __forceinline__ uint32_t sptr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* b, uint32_t c) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(sptr(b)), "r"(c));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* b, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sptr(b)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* b) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(sptr(b)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* b, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "W_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra D_%=;\n\t"
-      "bra W_%=;\n\t"
-      "D_%=:\n\t}" ::"r"(sptr(b)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   sptr(dst)), "l"(src), "r"(bytes), "r"(sptr(bar)) : "memory");
-}
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(sptr(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], u8 x s8 -> s32
-__device__ __forceinline__ void tc_mma_i8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc),
-      "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, int32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tc_ld8(uint32_t taddr, int32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-}
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, float a, float b, float c, float d) {
-  asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-__device__ __forceinline__ float4 ld_shared_v4(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
-  return v;
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, 128-byte swizzle SMEM matrix descriptor (cute::UMMA::SmemDescriptor, sm_100):
-//   [0,14) start address >> 4 | [16,30) LBO >> 4 (= 1 for swizzled K-major) | [32,46) SBO >> 4
-//   (= 1024 B between 8-row groups) | [46,48) version = 1 | [61,64) layout = SWIZZLE_128B (2)
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): c_format S32 (2) @4, a_format u8 (0) @7,
-// b_format s8 (1) @10, K-major A and B, N>>3 @17, M>>4 @24.
-__host__ __device__ constexpr uint32_t make_idesc(int n) {
-  return (2u << 4) | (0u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(TILE_M >> 4) << 24);
-}
+constexpr int CONSUMERS = 256, PRODUCERS = 256;
+constexpr int THREADS = CONSUMERS + PRODUCERS + 32;
 
 // Byte offset of element (row n, k) inside a K-major SW128 operand with `rows` rows:
 // [chunk = k/128][n/8][n%8][16-byte unit ^ (n%8)][byte]
@@ -194,35 +110,31 @@ struct Params {
   const float* scale;        // [n_nets][32] = s_c / 255
   float* out;                // [n_nets][n][400][32] fp32 (NHWC)
   int relu;
-  long long* dbg;            // optional [gridDim.x][16] cycle counters (B2RL_CONV1_DBG=1), else nullptr
 };
 
-// PROBE = per-role cycle counters (B2RL_CONV1_DBG=1); compiled out of the production instantiation
-template <bool PROBE>
-__device__ __forceinline__ long long pclk() {
-  if constexpr (PROBE) return clock64();
-  else return 0;
-}
+template <int N> struct Acc;
+template <> struct Acc<128> {
+  int32_t d[64];
+  __device__ __forceinline__ void mma(uint64_t a, uint64_t b, uint32_t acc) { mma_u8s8_n128(d, a, b, acc); }
+};
+template <> struct Acc<64> {
+  int32_t d[32];
+  __device__ __forceinline__ void mma(uint64_t a, uint64_t b, uint32_t acc) { mma_u8s8_n64(d, a, b, acc); }
+};
 
-template <int N_NETS, int C_OUT, bool PROBE>
+template <int N_NETS, int C_OUT>
 __global__ void __launch_bounds__(THREADS, 1)
 k_conv1_fused(const __grid_constant__ Params P) {
   constexpr int N_PER_NET = NSPLIT * C_OUT;            // MMA columns per network: 128 (64 for 16 channels)
-  constexpr int N_TOTAL = N_NETS * N_PER_NET;          // MMA N: 64 .. 256
-  constexpr int ROW_BYTES = C_OUT * 4;                 // one output position of one network
-  constexpr int B_BYTES = N_TOTAL * K_TOTAL;           // 32 / 64 KiB
-  constexpr int NBUF = 4 / N_NETS;                     // accumulator buffers in TMEM: 4 (one network) / 2
-  constexpr uint32_t TMEM_COLS = NBUF * N_TOTAL;       // 4 * N_PER_NET = 512 (32 channels) / 256 columns
+  constexpr int N_TOTAL = N_NETS * N_PER_NET;          // rows of the packed weights: 64 .. 256
+  constexpr int B_BYTES = N_TOTAL * K_TOTAL;           // 16 .. 64 KiB
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // SWIZZLE_128B atoms must be 1024-byte aligned in the shared window: align by hand (1 KiB slack reserved)
   uint8_t* smem = smem_raw + ((1024u - (sptr(smem_raw) & 1023u)) & 1023u);
   uint8_t* sB = smem;
   uint8_t* sA = smem + B_BYTES;
   uint8_t* sRaw = sA + A_STAGES * A_TILE_BYTES;
-  uint8_t* sOut = sRaw + 2 * RAW_STRIDE;       // per-epilogue-warp 4 KiB transpose buffers
-  __shared__ __align__(8) uint64_t b_full, raw_full[2], raw_empty[2], a_full[A_STAGES], a_empty[A_STAGES],
-      t_full[4], t_empty[4];
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t b_full, raw_full[2], raw_empty[2], a_full[A_STAGES], a_empty[A_STAGES];
   __shared__ float s_scale[2 * C_OUT_MAX];
   if (threadIdx.x < N_NETS * C_OUT) s_scale[threadIdx.x] = P.scale[threadIdx.x] * (1.0f / 128.0f);   // exact
 
@@ -230,106 +142,46 @@ k_conv1_fused(const __grid_constant__ Params P) {
   if (threadIdx.x == 0) {
     mbar_init(&b_full, 1);
     for (int i = 0; i < 2; ++i) { mbar_init(&raw_full[i], 1); mbar_init(&raw_empty[i], PRODUCERS); }
-    for (int i = 0; i < A_STAGES; ++i) { mbar_init(&a_full[i], PRODUCERS); mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < NBUF; ++i) { mbar_init(&t_full[i], 1); mbar_init(&t_empty[i], N_NETS * 128); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    fence_async_smem();
+    for (int i = 0; i < A_STAGES; ++i) { mbar_init(&a_full[i], PRODUCERS); mbar_init(&a_empty[i], CONSUMERS); }
+    mbar_init_fence();
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sptr(&s_tmem)),
-                 "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = s_tmem;
-  // Work is split by (frame stack, 128-row tile) unit, not by frame stack: 512 stacks over 148 CTAs would be
-  // 4 vs 3.46 stacks (16 vs 13.8 tiles); a CTA takes a contiguous run of units and loads every stack it touches.
+  // Work is split by (frame stack, 128-row tile) unit, not by frame stack: 512 stacks over 132 CTAs would be
+  // 4 vs 3.88 stacks (16 vs 15.5 tiles); a CTA takes a contiguous run of units and loads every stack it touches.
   const int64_t units = P.n * TILES;
   const int64_t u0 = units * blockIdx.x / gridDim.x, u1 = units * (blockIdx.x + 1) / gridDim.x;
   const int64_t k_first = u0 / TILES, k_end = (u1 + TILES - 1) / TILES;   // stacks [k_first, k_end)
-  const long long k_begin = pclk<PROBE>();
 
-  if (warp == 0) {
+  if (warp == (CONSUMERS + PRODUCERS) / 32) {
     // ------------------------------ TMA loader ------------------------------
     if (lane == 0) {
       mbar_expect_tx(&b_full, B_BYTES);
       constexpr int LOAD_CHUNK = (B_BYTES < 32768) ? B_BYTES : 32768;
       for (int off = 0; off < B_BYTES; off += LOAD_CHUNK) bulk_g2s(sB + off, P.bq + off, LOAD_CHUNK, &b_full);
       int it = 0;
-      long long d0 = 0;
       for (int64_t k = k_first; k < k_end; ++k, ++it) {
         const int s = it & 1;
-        const long long c0 = pclk<PROBE>();
         mbar_wait(&raw_empty[s], ((it >> 1) & 1) ^ 1);
-        d0 += pclk<PROBE>() - c0;
         int64_t row = P.idx ? P.idx[k] : k;
         row = row < 0 ? 0 : (row >= P.capacity ? P.capacity - 1 : row);
         mbar_expect_tx(&raw_full[s], FRAME_BYTES);
         bulk_g2s(sRaw + s * RAW_STRIDE, P.frames + row * FRAME_BYTES, FRAME_BYTES, &raw_full[s]);
       }
-      if (PROBE) P.dbg[blockIdx.x * 16 + 0] = d0;
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer ------------------------------
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(N_TOTAL);
-      mbar_wait(&b_full, 0);
-      tc_fence_after();
-      int at = 0;   // A-tile counter
-      long long d1 = 0, d2 = 0, d3 = 0;
-      for (int64_t k = k_first; k < k_end; ++k) {
-        const int t_lo = (int)max((int64_t)0, u0 - k * TILES), t_hi = (int)min((int64_t)TILES, u1 - k * TILES);
-        for (int t = t_lo; t < t_hi; ++t, ++at) {
-          const int stage = at % A_STAGES, acc = at % NBUF;
-          const long long c0 = pclk<PROBE>();
-          mbar_wait(&t_empty[acc], ((at / NBUF) & 1) ^ 1);
-          const long long c1 = pclk<PROBE>();
-          mbar_wait(&a_full[stage], (at / A_STAGES) & 1);
-          const long long c2 = pclk<PROBE>();
-          tc_fence_after();
-          const uint32_t a_base = sptr(sA + stage * A_TILE_BYTES), b_base = sptr(sB);
-          const uint32_t d = tmem + (uint32_t)(acc * N_TOTAL);
-#pragma unroll
-          for (int kk = 0; kk < K_TOTAL / 32; ++kk) {
-            const uint64_t ad = make_desc(a_base + (kk >> 2) * A_CHUNK_BYTES + (kk & 3) * 32);
-            const uint64_t bd = make_desc(b_base + (kk >> 2) * (N_TOTAL * 128) + (kk & 3) * 32);
-            tc_mma_i8(d, ad, bd, idesc, kk > 0 ? 1u : 0u);
-          }
-          tc_commit(&a_empty[stage]);   // SMEM stage reusable once these MMAs have read it
-          tc_commit(&t_full[acc]);      // accumulator complete
-          d1 += c1 - c0;
-          d2 += c2 - c1;
-          d3 += pclk<PROBE>() - c2;
-        }
-      }
-      if (PROBE) {
-        P.dbg[blockIdx.x * 16 + 1] = d1;
-        P.dbg[blockIdx.x * 16 + 2] = d2;
-        P.dbg[blockIdx.x * 16 + 3] = d3;
-      }
-    }
-  } else if (warp >= 4 && warp < 12) {
+  } else if (warp >= CONSUMERS / 32) {
     // --------------------------- im2col producers ---------------------------
-    const int pt = threadIdx.x - 128;            // 0..255
+    const int pt = threadIdx.x - CONSUMERS;      // 0..255
     const int r_local = pt & (TILE_M - 1);       // A-tile row
     const int chalf = pt >> 7;                   // this thread converts channels 2*chalf, 2*chalf+1 (one K chunk)
-    const bool probe = PROBE && pt == 0;
     int at = 0, it = 0;
-    long long d4 = 0, d5 = 0, d6 = 0, d7 = 0;
     for (int64_t k = k_first; k < k_end; ++k, ++it) {
       const int s = it & 1;
-      long long c0 = pclk<PROBE>();
       mbar_wait(&raw_full[s], (it >> 1) & 1);
-      d4 += pclk<PROBE>() - c0;
       const uint8_t* raw = sRaw + s * RAW_STRIDE;
       const int t_lo = (int)max((int64_t)0, u0 - k * TILES), t_hi = (int)min((int64_t)TILES, u1 - k * TILES);
       for (int t = t_lo; t < t_hi; ++t, ++at) {
         const int stage = at % A_STAGES;
-        c0 = pclk<PROBE>();
         mbar_wait(&a_empty[stage], ((at / A_STAGES) & 1) ^ 1);
-        const long long c1 = pclk<PROBE>();
         const int p = t * TILE_M + r_local;
         if (p < POS) {
           const int oy = p / OHW, ox = p - oy * OHW;
@@ -350,131 +202,81 @@ k_conv1_fused(const __grid_constant__ Params P) {
             }
           }
         }
-        const long long c2 = pclk<PROBE>();
         fence_async_smem();            // generic-proxy writes -> visible to the tensor core (async proxy)
         mbar_arrive(&a_full[stage]);
-        d5 += c1 - c0;
-        d6 += c2 - c1;
-        d7 += pclk<PROBE>() - c2;
       }
       mbar_arrive(&raw_empty[s]);      // this thread is done reading the raw frame
     }
-    if (probe) {
-      P.dbg[blockIdx.x * 16 + 4] = d4;
-      P.dbg[blockIdx.x * 16 + 5] = d5;
-      P.dbg[blockIdx.x * 16 + 6] = d6;
-      P.dbg[blockIdx.x * 16 + 7] = d7;
-    }
-  } else if (warp >= 12) {
-    // ------------------------------- epilogue -------------------------------
-    // 16 warps = 4 groups of 4 (one warp per TMEM lane quarter, i.e. four epilogue warps per SM sub-partition,
-    // so one warp's dependent-issue latency is covered by the other three).  Group g takes network g % N_NETS
-    // of every tile whose accumulator buffer is g / N_NETS: with one network the four groups rotate over four
-    // buffers, with two networks two buffers x two networks.
-    const int wq = warp & 3;                     // TMEM lane quarter this warp may access
-    const int eg = (warp - 12) >> 2;             // epilogue group 0..3
-    const int net = eg % N_NETS, slot = eg / N_NETS;
-    const int r_local = wq * 32 + lane;
-    const bool probe_e = PROBE && r_local == 0 && eg == 0;
-    uint8_t* stg = sOut + ((warp - 12) * 2048); // this warp's 32 rows x 64 B (16 channels), 16-byte units XOR-swizzled
+  } else {
+    // ------------------------- consumers: wgmma + epilogue -------------------------
+    // Warpgroup wg owns rows [64 wg, 64 wg + 64) of every tile; the networks run one after the other so that one
+    // accumulator (N_PER_NET / 2 registers) is live at a time.  Thread fragment (hopper.cuh): rows r and r + 8,
+    // columns 8j + 2(lane % 4) + {0, 1}; column d * C_OUT + co is digit d of channel co, so every thread holds
+    // all four digits of its channels.
+    const int wg = warp >> 2;
     const float relu_floor = P.relu ? 0.0f : -INFINITY;
-    // staging offsets: a thread writes its own row (lane) and later reads row i*8 + lane/4, unit lane%4
-    const uint32_t st_row = sptr(stg) + lane * 64, st_sw = (lane >> 1) & 3;
-    const uint32_t ld_off = sptr(stg) + (lane >> 2) * 64 + (((lane & 3) ^ ((lane >> 3) & 3)) << 4);
-    const int g_off = (lane >> 2) * ROW_BYTES + (lane & 3) * 16;      // byte offset of that unit inside the warp's block
-    int at = 0, own = 0;
-    long long d8 = 0, d9 = 0, d11 = 0, d12 = 0;
+    const int r_in = (warp & 3) * 16 + (lane >> 2);            // row inside the warpgroup's 64
+    const int c_in = 2 * (lane & 3);
+    mbar_wait(&b_full, 0);
+    int at = 0;
     for (int64_t k = k_first; k < k_end; ++k) {
       const int t_lo = (int)max((int64_t)0, u0 - k * TILES), t_hi = (int)min((int64_t)TILES, u1 - k * TILES);
       for (int t = t_lo; t < t_hi; ++t, ++at) {
-        if (at % NBUF != slot) continue;
-        const long long c0 = pclk<PROBE>();
-        mbar_wait(&t_full[slot], own & 1);
-        ++own;
-        const long long c1 = pclk<PROBE>();
-        tc_fence_after();
-        const uint32_t tbase = tmem + ((uint32_t)(wq * 32) << 16) + (uint32_t)(slot * N_TOTAL + net * N_PER_NET);
-        const int rows_valid = POS - (t * TILE_M + wq * 32);   // rows of this warp's block that exist (<= 0: none)
-        uint8_t* obase = reinterpret_cast<uint8_t*>(
-            P.out + (((int64_t)net * P.n + k) * POS + (t * TILE_M + wq * 32)) * C_OUT);
+        const int stage = at % A_STAGES;
+        mbar_wait(&a_full[stage], (at / A_STAGES) & 1);
+        const int p0 = t * TILE_M + wg * 64;                    // first output position of this warpgroup's rows
+        if (p0 >= POS) {                                        // the last tile's upper half holds no positions
+          mbar_arrive(&a_empty[stage]);
+          continue;
+        }
+        const uint32_t a_base = sptr(sA + stage * A_TILE_BYTES) + wg * (64 * 128), b_base = sptr(sB);
+#pragma unroll 1
+        for (int net = 0; net < N_NETS; ++net) {
+          Acc<N_PER_NET> acc;
+          wg_fence();
 #pragma unroll
-        for (int h = 0; h < C_OUT / 16; ++h) {
+          for (int kk = 0; kk < K_TOTAL / 32; ++kk) {
+            const uint64_t ad = make_desc(a_base + (kk >> 2) * A_CHUNK_BYTES + (kk & 3) * 32);
+            const uint64_t bd = make_desc(b_base + (kk >> 2) * (N_TOTAL * 128) + net * (N_PER_NET * 128) + (kk & 3) * 32);
+            acc.mma(ad, bd, kk > 0 ? 1u : 0u);
+          }
+          wg_commit();
+          wg_wait<0>();
+          wg_fence_regs(acc.d);
+          if (net == N_NETS - 1) mbar_arrive(&a_empty[stage]);   // SMEM stage reusable: every MMA has read it
+          const float* sc = s_scale + net * C_OUT;
 #pragma unroll
-          for (int c8 = 0; c8 < 2; ++c8) {
-            int32_t q0[8], q1[8], q2[8], q3[8];
-            const uint32_t col = tbase + h * 16 + c8 * 8;
-            const long long e0 = pclk<PROBE>();
-            tc_ld8(col + 0 * C_OUT, q0);
-            tc_ld8(col + 1 * C_OUT, q1);
-            tc_ld8(col + 2 * C_OUT, q2);
-            tc_ld8(col + 3 * C_OUT, q3);
-            tc_wait_ld();
-            d11 += pclk<PROBE>() - e0;
-            const float* sc = s_scale + net * C_OUT + h * 16 + c8 * 8;
+          for (int h = 0; h < 2; ++h) {
+            const int p = p0 + r_in + 8 * h;
+            if (p >= POS) continue;
+            float* orow = P.out + (((int64_t)net * P.n + k) * POS + p) * C_OUT;
 #pragma unroll
-            for (int g = 0; g < 2; ++g) {
-              float y[4];
+            for (int jj = 0; jj < C_OUT / 8; ++jj) {
+              float y[2];
 #pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int i = g * 4 + e;
+              for (int c = 0; c < 2; ++c) {
+                const int i = 4 * jj + 2 * h + c;                 // digit d sits C_OUT / 8 fragment columns further
+                const int32_t q0 = acc.d[i], q1 = acc.d[i + C_OUT / 2], q2 = acc.d[i + C_OUT], q3 = acc.d[i + 3 * C_OUT / 2];
                 // digits are recombined pairwise in exact integer arithmetic (|u| < 2^31):
                 //   u = q0*2^7 + q1,  t = q2*2^7 + q3,   sum = (u + t*2^-14) * 2^-7
                 // one fp32 rounding per conversion (2^-24 relative), then one FMA and the scale.
-                const float fu = (float)(q0[i] * 128 + q1[i]);
-                const float ft = (float)(q2[i] * 128 + q3[i]);
-                const float v = __fmaf_rn(ft, 1.0f / 16384.0f, fu) * sc[i];   // sc already holds s_c / (255 * 2^7)
-                y[e] = fmaxf(v, relu_floor);
+                const float fu = (float)(q0 * 128 + q1);
+                const float ft = (float)(q2 * 128 + q3);
+                const float v = __fmaf_rn(ft, 1.0f / 16384.0f, fu) * sc[8 * jj + c_in + c];   // sc holds s_c / (255 * 2^7)
+                y[c] = fmaxf(v, relu_floor);
               }
-              const uint32_t unit = c8 * 2 + g;      // 16-byte unit of this row's 64-byte half
-              st_shared_v4(st_row + ((unit ^ st_sw) << 4), y[0], y[1], y[2], y[3]);
+              *reinterpret_cast<float2*>(orow + 8 * jj + c_in) = make_float2(y[0], y[1]);
             }
           }
-          __syncwarp();
-          // 32 rows x 64 B of this half: every store instruction writes eight full 64-byte segments
-          // (the whole block is contiguous when C_OUT = 16)
-          if (rows_valid >= 32) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float4 v = ld_shared_v4(ld_off + i * 512);
-              *reinterpret_cast<float4*>(obase + g_off + h * 64 + i * 8 * ROW_BYTES) = v;
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              if (i * 8 + (lane >> 2) < rows_valid) {
-                const float4 v = ld_shared_v4(ld_off + i * 512);
-                *reinterpret_cast<float4*>(obase + g_off + h * 64 + i * 8 * ROW_BYTES) = v;
-              }
-            }
-          }
-          __syncwarp();
         }
-        tc_fence_before();
-        mbar_arrive(&t_empty[slot]);
-        d8 += c1 - c0;
-        d9 += pclk<PROBE>() - c1;
-        if (own == 1) d12 = c1 - k_begin;
       }
     }
-    if (probe_e) {
-      P.dbg[blockIdx.x * 16 + 8] = d8;
-      P.dbg[blockIdx.x * 16 + 9] = d9;
-      P.dbg[blockIdx.x * 16 + 11] = d11;
-      P.dbg[blockIdx.x * 16 + 12] = d12;
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (PROBE && threadIdx.x == 0) P.dbg[blockIdx.x * 16 + 10] = pclk<PROBE>() - k_begin;
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS));
   }
 }
 
 template <int N_NETS, int C_OUT>
 constexpr size_t smem_bytes() {
-  return (size_t)N_NETS * NSPLIT * C_OUT * K_TOTAL + (size_t)A_STAGES * A_TILE_BYTES + 2 * (size_t)RAW_STRIDE +
-         (size_t)STAGE_OUT_BYTES + 1024;
+  return (size_t)N_NETS * NSPLIT * C_OUT * K_TOTAL + (size_t)A_STAGES * A_TILE_BYTES + 2 * (size_t)RAW_STRIDE + 1024;
 }
 
 }  // namespace conv1
@@ -513,25 +315,20 @@ extern "C" int b2rl_conv1_pack_jobs(const float* const* w_dev, const int32_t* ne
   return B2RL_OK;
 }
 
-template <int N_NETS, int C_OUT, bool PROBE>
-static cudaError_t conv1_launch_p(const conv1::Params& P, unsigned grid, cudaStream_t st) {
+template <int N_NETS, int C_OUT>
+static cudaError_t conv1_launch(const conv1::Params& P, unsigned grid, cudaStream_t st) {
   static bool attr[64] = {false};
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
   if (!attr[dev & 63]) {
-    e = cudaFuncSetAttribute(conv1::k_conv1_fused<N_NETS, C_OUT, PROBE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    e = cudaFuncSetAttribute(conv1::k_conv1_fused<N_NETS, C_OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)conv1::smem_bytes<N_NETS, C_OUT>());
     if (e != cudaSuccess) return e;
     attr[dev & 63] = true;
   }
-  conv1::k_conv1_fused<N_NETS, C_OUT, PROBE><<<grid, conv1::THREADS, conv1::smem_bytes<N_NETS, C_OUT>(), st>>>(P);
+  conv1::k_conv1_fused<N_NETS, C_OUT><<<grid, conv1::THREADS, conv1::smem_bytes<N_NETS, C_OUT>(), st>>>(P);
   return cudaSuccess;
-}
-
-template <int N_NETS, int C_OUT>
-static cudaError_t conv1_launch(const conv1::Params& P, unsigned grid, cudaStream_t st) {
-  return P.dbg ? conv1_launch_p<N_NETS, C_OUT, true>(P, grid, st) : conv1_launch_p<N_NETS, C_OUT, false>(P, grid, st);
 }
 
 extern "C" int b2rl_conv1_fused(const uint8_t* frames_dev, int64_t capacity, const int64_t* idx_dev, int64_t n,
@@ -549,10 +346,7 @@ extern "C" int b2rl_conv1_fused(const uint8_t* frames_dev, int64_t capacity, con
   B2RL_CUDA(cudaGetDevice(&dev));
   static int sms[64] = {0};
   if (!sms[dev & 63]) B2RL_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-  static long long* dbg_buf = nullptr;
-  if (getenv("B2RL_CONV1_DBG") && !dbg_buf) B2RL_CUDA(cudaMalloc(&dbg_buf, 256 * 16 * sizeof(long long)));
-  if (dbg_buf) B2RL_CUDA(cudaMemsetAsync(dbg_buf, 0, 256 * 16 * sizeof(long long), (cudaStream_t)stream));
-  conv1::Params P{frames_dev, idx_dev, n, capacity, bq_dev, scale_dev, out_dev, relu, dbg_buf};
+  conv1::Params P{frames_dev, idx_dev, n, capacity, bq_dev, scale_dev, out_dev, relu};
   const int64_t units = n * conv1::TILES;
   const unsigned grid = (unsigned)((units < sms[dev & 63]) ? units : sms[dev & 63]);
   cudaStream_t st = (cudaStream_t)stream;
@@ -562,15 +356,5 @@ extern "C" int b2rl_conv1_fused(const uint8_t* frames_dev, int64_t capacity, con
   B2RL_CUDA(e);
   count_launch();
   B2RL_CHECK_LAUNCH();
-  if (dbg_buf) {   // profiling aid: per-role cycle counters of CTA 0 (synchronous; never set in production)
-    long long h[16];
-    B2RL_CUDA(cudaMemcpy(h, dbg_buf, sizeof(h), cudaMemcpyDeviceToHost));
-    static const char* names[13] = {"loader:wait raw_empty", "mma:wait t_empty", "mma:wait a_full", "mma:issue+commit",
-                                    "prod:wait raw_full", "prod:wait a_empty", "prod:build", "prod:fence+arrive",
-                                    "epi:wait t_full", "epi:work", "roles total (CTA 0)", "epi:tcgen05.ld+wait",
-                                    "first accumulator ready at"};
-    for (int i = 0; i < 13; ++i)
-      fprintf(stderr, "[conv1 dbg] n_nets %d n %lld %-24s %lld\n", n_nets, (long long)n, names[i], h[i]);
-  }
   return B2RL_OK;
 }

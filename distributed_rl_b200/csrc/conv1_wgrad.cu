@@ -1,4 +1,4 @@
-// Fused gather + weight gradient of the first convolution on the 5th-gen tensor cores.
+// Fused gather + weight gradient of the first convolution on the Hopper tensor cores (wgmma).
 //
 //   dW[co, c, ky, kx] = (1/255) * sum_{k, oy, ox} gy[k, oy, ox, co] * frame[idx[k]][c, 4oy+ky, 4ox+kx]
 //
@@ -6,10 +6,10 @@
 // APE_X/Learner.py:123-138).  The input of conv_1 is data, so only dL/dW is needed.  The unfused
 // path gathers the sampled uint8 rows, converts them to fp32 NHWC (58 MB for a batch of 512) and runs
 // cuDNN's fp32 wgrad; here the sampled rows go HBM -> SMEM (TMA bulk copy) -> transposed im2col
-// (patch element x output position, uint8) -> tcgen05.mma -> TMEM, and are never staged in HBM.
+// (patch element x output position, uint8) -> wgmma -> registers, and are never staged in HBM.
 //
 // Arithmetic: the GEMM is D[e = (c,ky,kx)][co] = sum_p A[e][p] * G[co][p] with p = (k, oy, ox).
-// A holds exact uint8 pixels, so the MMA runs in kind::i8.  The fp32 output gradient is written as
+// A holds exact uint8 pixels, so the MMA runs on u8 x s8 -> s32.  The fp32 output gradient is written as
 // four balanced base-256 digits (int8) against a per-(CTA, channel) power-of-two scale s > max|gy| / 127,
 //     gy = s * (q0 + q1/2^8 + q2/2^16 + q3/2^24)     (exact for |gy| >= s, else rounded at s * 2^-24),
 // the digits being four groups of C_OUT rows of the B operand (N = 4*C_OUT).  Integer accumulation over
@@ -17,23 +17,25 @@
 // one fp32 rounding per pair, so every CTA partial is the sum of pixel x (32-bit fixed-point gy) to
 // ~1 ulp.  Partials of the CTAs are summed in fp64 by k_conv1_wgrad_reduce (deterministic, no atomics).
 //
-// Warp roles per CTA (persistent, one CTA per SM, 20 warps):
-//   warp 0        TMA loader: one 28 224-byte frame stack per item
-//   warp 1        MMA issuer (one elected thread): 2 x tcgen05.mma (M = 128 each) per 32-position K step
-//   warp 2        TMEM allocator
-//   warps 4-11    A producers: SMEM frame -> [256 patch elements][128 positions] uint8, K-major SW128
-//   warps 12-19   B producers: gy (NHWC fp32, global) -> digits -> [4*C_OUT][128 positions] int8
+// Warp roles per CTA (persistent, one CTA per SM, 16 warps):
+//   warps 0-15    build one 128-position K chunk of both operands in SMEM, then each warpgroup issues the
+//                 wgmma m64nNk32 of its 64 patch elements (M = 256 over four warpgroups) and builds the next
+//                 chunk while they run; the accumulators stay in registers over all of the CTA's frame stacks
+//     warps 0-7   A: SMEM frame -> [256 patch elements][128 positions] uint8, K-major SW128
+//     warps 8-15  B: gy (NHWC fp32, global) -> digits -> [4*C_OUT][128 positions] int8
 //                 (warp = 8 channels x half of a chunk's 16-position units)
-//   warps 16-19   then run the epilogue once: TMEM -> int64 recombination -> partial[cta][co][e]
+//   thread 0 also issues the TMA bulk copy of the next frame stack when it starts on a stack's first chunk: the
+//   buffer it overwrites was last read two stacks before, by chunks that every producer has finished
 #include "common.cuh"
-
-#include <stdlib.h>
+#include "hopper.cuh"
 
 namespace b2rl {
 namespace conv1w {
 
+using namespace sm90;
+
 constexpr int C_IN = 4, HW = 84, KS = 8, STRIDE = 4, OHW = 20;
-constexpr int E_TOTAL = C_IN * KS * KS;            // 256 patch elements = GEMM M (two halves of 128)
+constexpr int E_TOTAL = C_IN * KS * KS;            // 256 patch elements = GEMM M (four warpgroups of 64)
 constexpr int FRAME_BYTES = C_IN * HW * HW;        // 28 224
 constexpr int RAW_STRIDE = 28288;
 constexpr int POS = OHW * OHW;                     // 400 output positions per frame stack
@@ -41,64 +43,11 @@ constexpr int NSPLIT = 4;
 constexpr int KCHUNK = 128;                        // positions per pipeline stage (one 128-byte K row)
 constexpr int CHUNKS = 4;                          // 128 + 128 + 128 + 16 (+16 zero padding)
 constexpr int A_BYTES = E_TOTAL * KCHUNK;          // 32 KiB
-constexpr int STAGES = 3;
-constexpr int THREADS = 640;
+constexpr int STAGES = 3;                          // a stage is rebuilt two chunks after its MMAs were issued
 constexpr int A_PRODUCERS = 256, B_PRODUCERS = 256;
+constexpr int THREADS = A_PRODUCERS + B_PRODUCERS;
 constexpr int MAX_ITEMS_PER_CTA = 160;             // int32 accumulators: 128*255*400*T < 2^31
 
-__device__ __forceinline__ uint32_t sptr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* b, uint32_t c) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(sptr(b)), "r"(c));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* b, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sptr(b)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* b) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(sptr(b)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* b, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "W_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra D_%=;\n\t"
-      "bra W_%=;\n\t"
-      "D_%=:\n\t}" ::"r"(sptr(b)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   sptr(dst)), "l"(src), "r"(bytes), "r"(sptr(bar)) : "memory");
-}
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(sptr(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_i8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc),
-      "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, int32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// K-major SW128 descriptor and u8 x s8 -> s32 instruction descriptor: see csrc/conv1.cu
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-__host__ __device__ constexpr uint32_t make_idesc(int n) {
-  return (2u << 4) | (0u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
 // byte offset of (row, 16-byte unit) in a one-chunk K-major SW128 operand
 __device__ __forceinline__ int sw_row(int row) { return (row >> 3) * 1024 + (row & 7) * 128; }
 
@@ -109,8 +58,24 @@ struct Params {
   const float* gy;           // [n][400][C_OUT] fp32 (NHWC)
   const float* y;            // optional conv_1 output after ReLU, same layout: dL/dy is taken as gy * (y > 0); else nullptr
   float* partial;            // [gridDim.x][C_OUT][256]
-  long long* dbg;            // optional [16] cycle counters of CTA 0 (B2RL_CONV1_DBG=1), else nullptr
 };
+
+template <int N> struct Acc;
+template <> struct Acc<128> {
+  int32_t d[64];
+  __device__ __forceinline__ void mma(uint64_t a, uint64_t b, uint32_t acc) { mma_u8s8_n128(d, a, b, acc); }
+};
+template <> struct Acc<64> {
+  int32_t d[32];
+  __device__ __forceinline__ void mma(uint64_t a, uint64_t b, uint32_t acc) { mma_u8s8_n64(d, a, b, acc); }
+};
+
+// digit scale of channel co: the power of two s = 2^(e-127) > max|gy| / 127 (e clamped to [27, 227])
+__device__ __forceinline__ int digit_exponent(uint32_t absmax_bits) {
+  const float t = __uint_as_float(absmax_bits) / 127.0f;
+  const int e = (int)((__float_as_uint(t) >> 23) & 0xFF) + 1;
+  return e < 27 ? 27 : (e > 227 ? 227 : e);
+}
 
 template <int C_OUT>
 __global__ void __launch_bounds__(THREADS, 1)
@@ -118,289 +83,223 @@ k_conv1_wgrad(const __grid_constant__ Params P) {
   constexpr int N_TOTAL = NSPLIT * C_OUT;              // 128 (64 for 16 channels)
   constexpr int B_BYTES = N_TOTAL * KCHUNK;
   constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  constexpr uint32_t TMEM_COLS = 2 * N_TOTAL;          // two M halves
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (sptr(smem_raw) & 1023u)) & 1023u);
   uint8_t* sStage = smem;
-  uint8_t* sRaw = smem + STAGES * STAGE_BYTES;
-  __shared__ __align__(8) uint64_t raw_full[2], raw_empty[2], s_full[STAGES], s_empty[STAGES], acc_full;
-  __shared__ uint32_t s_tmem;
+  uint8_t* sZero = smem + STAGES * STAGE_BYTES;        // a B operand of zeros: the K steps past position 415
+  uint8_t* sRaw = sZero + B_BYTES;
+  __shared__ __align__(8) uint64_t raw_full[2];
   __shared__ uint32_t s_absmax[32];                    // per channel: bits of max |gy| over this CTA's items
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x < 32) s_absmax[threadIdx.x] = 0u;
+  for (int i = threadIdx.x; i < B_BYTES / 16; i += THREADS) reinterpret_cast<uint4*>(sZero)[i] = make_uint4(0u, 0u, 0u, 0u);
+  fence_async_smem();
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) { mbar_init(&raw_full[i], 1); mbar_init(&raw_empty[i], A_PRODUCERS); }
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&s_full[i], A_PRODUCERS + B_PRODUCERS); mbar_init(&s_empty[i], 1); }
-    mbar_init(&acc_full, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    fence_async_smem();
+    for (int i = 0; i < 2; ++i) mbar_init(&raw_full[i], 1);
+    mbar_init_fence();
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sptr(&s_tmem)),
-                 "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = s_tmem;
   const int64_t first = blockIdx.x, stride = gridDim.x;
 
-  if (warp == 0) {
-    // ------------------------------ TMA loader ------------------------------
-    if (lane == 0) {
-      int it = 0;
-      for (int64_t k = first; k < P.n; k += stride, ++it) {
-        const int s = it & 1;
-        mbar_wait(&raw_empty[s], ((it >> 1) & 1) ^ 1);
-        int64_t row = P.idx ? P.idx[k] : k;
-        row = row < 0 ? 0 : (row >= P.capacity ? P.capacity - 1 : row);
-        mbar_expect_tx(&raw_full[s], FRAME_BYTES);
-        bulk_g2s(sRaw + s * RAW_STRIDE, P.frames + row * FRAME_BYTES, FRAME_BYTES, &raw_full[s]);
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer ------------------------------
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(N_TOTAL);
-      int at = 0;
-      uint32_t started = 0;
-      for (int64_t k = first; k < P.n; k += stride) {
-        for (int j = 0; j < CHUNKS; ++j, ++at) {
-          const int stage = at % STAGES;
-          const long long c0 = clock64();
-          mbar_wait(&s_full[stage], (at / STAGES) & 1);
-          const long long c1 = clock64();
-          tc_fence_after();
-          const uint32_t a_base = sptr(sStage + stage * STAGE_BYTES), b_base = a_base + A_BYTES;
-          const int ksteps = (j < CHUNKS - 1) ? 4 : 1;   // last chunk: positions 384..399 (+16 zeros)
-          for (int ks = 0; ks < ksteps; ++ks) {
-            const uint64_t bd = make_desc(b_base + ks * 32);
-            tc_mma_i8(tmem, make_desc(a_base + ks * 32), bd, idesc, started);
-            tc_mma_i8(tmem + N_TOTAL, make_desc(a_base + 128 * 128 + ks * 32), bd, idesc, started);
-            started = 1u;
-          }
-          tc_commit(&s_empty[stage]);
-          if (P.dbg && blockIdx.x == 0) { P.dbg[0] += c1 - c0; P.dbg[1] += clock64() - c1; }
-        }
-      }
-      tc_commit(&acc_full);
-    }
-  } else if (warp >= 4) {
-    // -------- all producers first find max |gy| per channel over this CTA's items (the digit scale) --------
-    const long long t_start = clock64();
-    if (warp >= 12) {
-      // -------- the B producers first find max |gy| per channel over this CTA's items (the digit scale);
-      //          the A producers need no scale and start filling the pipeline meanwhile --------
-      const int pt = threadIdx.x - 384;                 // 0..255
-      const int c4 = (pt * 4) % C_OUT;                  // this thread always sees channels c4..c4+3 (1024 % C_OUT == 0)
-      uint4 m = make_uint4(0u, 0u, 0u, 0u);
-      for (int64_t k = first; k < P.n; k += stride) {
-        const uint4* g = reinterpret_cast<const uint4*>(P.gy + k * (int64_t)(POS * C_OUT));
-        const float4* yk = P.y ? reinterpret_cast<const float4*>(P.y + k * (int64_t)(POS * C_OUT)) : nullptr;
+  // frame stack `it` of this CTA -> raw buffer it & 1
+  auto load_frame = [&](int64_t it) {
+    const int64_t k = first + it * stride;
+    if (k >= P.n) return;
+    int64_t row = P.idx ? P.idx[k] : k;
+    row = row < 0 ? 0 : (row >= P.capacity ? P.capacity - 1 : row);
+    mbar_expect_tx(&raw_full[it & 1], FRAME_BYTES);
+    bulk_g2s(sRaw + (it & 1) * RAW_STRIDE, P.frames + row * FRAME_BYTES, FRAME_BYTES, &raw_full[it & 1]);
+  };
+  if (threadIdx.x == 0) load_frame(0);
+
+  const bool is_a = warp < A_PRODUCERS / 32;
+  // -------- the B producers first find max |gy| per channel over this CTA's items (the digit scale);
+  //          the A producers need no scale and build the first chunk meanwhile --------
+  if (!is_a) {
+    const int pt = threadIdx.x - A_PRODUCERS;         // 0..255
+    const int c4 = (pt * 4) % C_OUT;                  // this thread always sees channels c4..c4+3 (1024 % C_OUT == 0)
+    uint4 m = make_uint4(0u, 0u, 0u, 0u);
+    for (int64_t k = first; k < P.n; k += stride) {
+      const uint4* g = reinterpret_cast<const uint4*>(P.gy + k * (int64_t)(POS * C_OUT));
+      const float4* yk = P.y ? reinterpret_cast<const float4*>(P.y + k * (int64_t)(POS * C_OUT)) : nullptr;
 #pragma unroll
-        for (int i = 0; i < (POS * C_OUT / 4 + 255) / 256; ++i) {
-          const int e = pt + 256 * i;
-          if (e < POS * C_OUT / 4) {
-            uint4 v = g[e];
-            if (yk) {                                    // ReLU mask of the fused forward
-              const float4 yv = yk[e];
-              v.x = yv.x > 0.0f ? v.x : 0u; v.y = yv.y > 0.0f ? v.y : 0u;
-              v.z = yv.z > 0.0f ? v.z : 0u; v.w = yv.w > 0.0f ? v.w : 0u;
-            }
-            m.x = max(m.x, v.x & 0x7FFFFFFFu); m.y = max(m.y, v.y & 0x7FFFFFFFu);
-            m.z = max(m.z, v.z & 0x7FFFFFFFu); m.w = max(m.w, v.w & 0x7FFFFFFFu);
+      for (int i = 0; i < (POS * C_OUT / 4 + 255) / 256; ++i) {
+        const int e = pt + 256 * i;
+        if (e < POS * C_OUT / 4) {
+          uint4 v = g[e];
+          if (yk) {                                    // ReLU mask of the fused forward
+            const float4 yv = yk[e];
+            v.x = yv.x > 0.0f ? v.x : 0u; v.y = yv.y > 0.0f ? v.y : 0u;
+            v.z = yv.z > 0.0f ? v.z : 0u; v.w = yv.w > 0.0f ? v.w : 0u;
           }
+          m.x = max(m.x, v.x & 0x7FFFFFFFu); m.y = max(m.y, v.y & 0x7FFFFFFFu);
+          m.z = max(m.z, v.z & 0x7FFFFFFFu); m.w = max(m.w, v.w & 0x7FFFFFFFu);
         }
       }
-      atomicMax(&s_absmax[c4 + 0], m.x); atomicMax(&s_absmax[c4 + 1], m.y);
-      atomicMax(&s_absmax[c4 + 2], m.z); atomicMax(&s_absmax[c4 + 3], m.w);
-      asm volatile("bar.sync 1, 256;" ::: "memory");
     }
-    const bool probe = P.dbg && blockIdx.x == 0 && lane == 0 && (warp == 4 || warp == 12);
-    if (probe) P.dbg[warp == 4 ? 2 : 6] += clock64() - t_start;
-    if (warp < 12) {
-      // ------------------- A producers: transposed im2col, uint8 -------------------
-      const int aw = warp - 4;
-      int at = 0, it = 0;
-      for (int64_t k = first; k < P.n; k += stride, ++it) {
-        const int s = it & 1;
-        long long a0 = clock64();
+    atomicMax(&s_absmax[c4 + 0], m.x); atomicMax(&s_absmax[c4 + 1], m.y);
+    atomicMax(&s_absmax[c4 + 2], m.z); atomicMax(&s_absmax[c4 + 3], m.w);
+    named_sync(1, B_PRODUCERS);
+  }
+
+  // A producer mapping: warp aw = (c, ky) rows 4aw..4aw+3, lane = 4 consecutive positions
+  const int aw = warp;
+  // B producer mapping: channel group bw (8 channels), half uh of the chunk's 16-position units
+  const int bw = (warp - A_PRODUCERS / 32) & 3, uh = (warp - A_PRODUCERS / 32) >> 2;
+  const int c3 = lane & 7, pq = lane >> 3;
+  const int co = 8 * bw + c3;
+  const bool b_active = !is_a && (8 * bw) < C_OUT;
+  float inv_s24 = 16777216.0f;
+  if (b_active) inv_s24 = __uint_as_float((uint32_t)(254 - digit_exponent(s_absmax[co]) + 24) << 23);   // 2^24 / s
+
+  // chunk `at` = (item at/4, chunk at%4); a B producer issues the loads of chunk at+1 before converting chunk at
+  const int64_t n_items = (P.n - first + stride - 1) / stride;
+  const int total = (int)n_items * CHUNKS;
+  auto load_chunk = [&](int at, float (&v)[4][4]) {
+    const int j = at & 3;
+    const int64_t base = (first + (int64_t)(at >> 2) * stride) * (int64_t)(POS * C_OUT) + co;
+    const float* g = P.gy + base;
+    const int u0 = (j < CHUNKS - 1) ? uh * 4 : uh, nu = (j < CHUNKS - 1) ? 4 : 1;
+#pragma unroll
+    for (int uu = 0; uu < 4; ++uu) {
+      const int p = j * KCHUNK + (u0 + uu) * 16 + 4 * pq;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) v[uu][i] = (uu < nu && p < POS) ? g[(int64_t)(p + i) * C_OUT] : 0.0f;
+    }
+    if (P.y) {                                       // ReLU mask of the fused forward
+      const float* yk = P.y + base;
+#pragma unroll
+      for (int uu = 0; uu < 4; ++uu) {
+        const int p = j * KCHUNK + (u0 + uu) * 16 + 4 * pq;
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          if (uu < nu && p < POS && !(yk[(int64_t)(p + i) * C_OUT] > 0.0f)) v[uu][i] = 0.0f;
+      }
+    }
+  };
+  float v[4][4], vn[4][4];
+  if (b_active && total > 0) load_chunk(0, v);
+
+  const int wg = warp >> 2;                          // this warpgroup's MMA rows: patch elements [64 wg, 64 wg + 64)
+  Acc<N_TOTAL> acc;
+  for (int at = 0; at < total; ++at) {
+    const int stage = at % STAGES, j = at & 3;
+    uint8_t* st = sStage + stage * STAGE_BYTES;
+    if (is_a) {
+      // ------------------- A: transposed im2col, uint8 -------------------
+      const int it = at >> 2, s = it & 1;
+      if (j == 0) {
+        if (threadIdx.x == 0) load_frame(it + 1);
         mbar_wait(&raw_full[s], (it >> 1) & 1);
-        if (probe) P.dbg[3] += clock64() - a0;
-        const uint8_t* raw = sRaw + s * RAW_STRIDE;
-        for (int j = 0; j < CHUNKS; ++j, ++at) {
-          const int stage = at % STAGES;
-          a0 = clock64();
-          mbar_wait(&s_empty[stage], ((at / STAGES) & 1) ^ 1);
-          const long long a1 = clock64();
-          const int p0 = j * KCHUNK + 4 * lane;          // this lane's 4 consecutive positions (same oy: 20 % 4 == 0)
-          if (p0 < POS) {
-            const int oy = p0 / OHW, ox0 = p0 - oy * OHW;
-            const uint8_t* src0 = raw + (STRIDE * oy) * HW + STRIDE * ox0;
-            uint8_t* dstA = sStage + stage * STAGE_BYTES;
-            const int unit = lane >> 2, word = (lane & 3) * 4;
+      }
+      const uint8_t* raw = sRaw + s * RAW_STRIDE;
+      const int p0 = j * KCHUNK + 4 * lane;          // this lane's 4 consecutive positions (same oy: 20 % 4 == 0)
+      if (p0 < POS) {
+        const int oy = p0 / OHW, ox0 = p0 - oy * OHW;
+        const uint8_t* src0 = raw + (STRIDE * oy) * HW + STRIDE * ox0;
+        const int unit = lane >> 2, word = (lane & 3) * 4;
 #pragma unroll
-            for (int r = 0; r < 4; ++r) {
-              const int cy = aw * 4 + r;                 // (c, ky): 32 rows of 8 patch elements (kx = 0..7)
-              const int c = cy >> 3, ky = cy & 7;
-              const uint32_t* src = reinterpret_cast<const uint32_t*>(src0 + c * (HW * HW) + ky * HW);
-              // pixels 4*ox0 .. 4*ox0+19: word i holds kx = 0..3 of position p0+i, word i+1 its kx = 4..7
-              const uint32_t w0 = src[0], w1 = src[1], w2 = src[2], w3 = src[3], w4 = src[4];
-              const int e0 = c * 64 + ky * 8;
-              // 4x4 byte transposes: out[kx] = {w_a.b[kx], w_b.b[kx], w_c.b[kx], w_d.b[kx]} = positions p0..p0+3 of element kx
-              const uint32_t t0 = __byte_perm(w0, w1, 0x5140), t1 = __byte_perm(w0, w1, 0x7362);
-              const uint32_t t2 = __byte_perm(w2, w3, 0x5140), t3 = __byte_perm(w2, w3, 0x7362);
-              const uint32_t u0 = __byte_perm(w1, w2, 0x5140), u1 = __byte_perm(w1, w2, 0x7362);
-              const uint32_t u2 = __byte_perm(w3, w4, 0x5140), u3 = __byte_perm(w3, w4, 0x7362);
-              const uint32_t o[8] = {__byte_perm(t0, t2, 0x5410), __byte_perm(t0, t2, 0x7632),
-                                     __byte_perm(t1, t3, 0x5410), __byte_perm(t1, t3, 0x7632),
-                                     __byte_perm(u0, u2, 0x5410), __byte_perm(u0, u2, 0x7632),
-                                     __byte_perm(u1, u3, 0x5410), __byte_perm(u1, u3, 0x7632)};
+        for (int r = 0; r < 4; ++r) {
+          const int cy = aw * 4 + r;                 // (c, ky): 32 rows of 8 patch elements (kx = 0..7)
+          const int c = cy >> 3, ky = cy & 7;
+          const uint32_t* src = reinterpret_cast<const uint32_t*>(src0 + c * (HW * HW) + ky * HW);
+          // pixels 4*ox0 .. 4*ox0+19: word i holds kx = 0..3 of position p0+i, word i+1 its kx = 4..7
+          const uint32_t w0 = src[0], w1 = src[1], w2 = src[2], w3 = src[3], w4 = src[4];
+          const int e0 = c * 64 + ky * 8;
+          // 4x4 byte transposes: out[kx] = {w_a.b[kx], w_b.b[kx], w_c.b[kx], w_d.b[kx]} = positions p0..p0+3 of element kx
+          const uint32_t t0 = __byte_perm(w0, w1, 0x5140), t1 = __byte_perm(w0, w1, 0x7362);
+          const uint32_t t2 = __byte_perm(w2, w3, 0x5140), t3 = __byte_perm(w2, w3, 0x7362);
+          const uint32_t u0 = __byte_perm(w1, w2, 0x5140), u1 = __byte_perm(w1, w2, 0x7362);
+          const uint32_t u2 = __byte_perm(w3, w4, 0x5140), u3 = __byte_perm(w3, w4, 0x7362);
+          const uint32_t o[8] = {__byte_perm(t0, t2, 0x5410), __byte_perm(t0, t2, 0x7632),
+                                 __byte_perm(t1, t3, 0x5410), __byte_perm(t1, t3, 0x7632),
+                                 __byte_perm(u0, u2, 0x5410), __byte_perm(u0, u2, 0x7632),
+                                 __byte_perm(u1, u3, 0x5410), __byte_perm(u1, u3, 0x7632)};
 #pragma unroll
-              for (int kx = 0; kx < 8; ++kx) {           // row e0 + kx: (e & 7) == kx
-                *reinterpret_cast<uint32_t*>(dstA + sw_row(e0 + kx) + ((unit ^ kx) << 4) + word) = o[kx];
-              }
-            }
+          for (int kx = 0; kx < 8; ++kx) {           // row e0 + kx: (e & 7) == kx
+            *reinterpret_cast<uint32_t*>(st + sw_row(e0 + kx) + ((unit ^ kx) << 4) + word) = o[kx];
           }
-          const long long a2 = clock64();
-          fence_async_smem();
-          mbar_arrive(&s_full[stage]);
-          if (probe) { P.dbg[4] += a1 - a0; P.dbg[5] += a2 - a1; P.dbg[13] += clock64() - a2; }
         }
-        mbar_arrive(&raw_empty[s]);
       }
     } else {
-      // ------------------- B producers: gy -> four signed 7-bit digits -------------------
-      const int bw = (warp - 12) & 3, uh = (warp - 12) >> 2;      // channel group, half of the chunk's units
-      const int c3 = lane & 7, pq = lane >> 3;
-      const int co = 8 * bw + c3;
-      const bool active = (8 * bw) < C_OUT;
-      float inv_s24 = 16777216.0f;
-      if (active) {
-        const float t = __uint_as_float(s_absmax[co]) / 127.0f;
-        int e = (int)((__float_as_uint(t) >> 23) & 0xFF) + 1;     // s = 2^(e-127) > t
-        e = e < 27 ? 27 : (e > 227 ? 227 : e);
-        inv_s24 = __uint_as_float((uint32_t)(254 - e + 24) << 23);   // 2^24 / s
-      }
-      // chunk `at` = (item at/4, chunk at%4); the loads of chunk at+1 are issued before chunk at is converted
-      const int64_t n_items = (P.n - first + stride - 1) / stride;
-      const int total = (int)n_items * CHUNKS;
-      auto load_chunk = [&](int at, float (&v)[4][4]) {
-        const int j = at & 3;
-        const int64_t base = (first + (int64_t)(at >> 2) * stride) * (int64_t)(POS * C_OUT) + co;
-        const float* g = P.gy + base;
-        const int u0 = (j < CHUNKS - 1) ? uh * 4 : uh, nu = (j < CHUNKS - 1) ? 4 : 1;
+      // ------------------- B: gy -> four signed 7-bit digits -------------------
+      // this warp's units of the chunk: 4 of 8 (last chunk: unit 0 = positions 384..399, unit 1 = zeros)
+      const int u0 = (j < CHUNKS - 1) ? uh * 4 : uh, nu = (j < CHUNKS - 1) ? 4 : 1;
+      if (b_active && at + 1 < total) load_chunk(at + 1, vn);
+      if (b_active) {
+        uint8_t* dstB = st + A_BYTES;
 #pragma unroll
         for (int uu = 0; uu < 4; ++uu) {
-          const int p = j * KCHUNK + (u0 + uu) * 16 + 4 * pq;
+          if (uu >= nu) break;
+          // X = gy / s * 2^24 as an int32 (exact: power-of-two scale, |X| <= 127 * 2^24); balanced base-256 digits
+          // via the bias 0x00808080: the three low bytes come out as q + 128, the top byte is q0 itself.
+          uint32_t Y[4];
 #pragma unroll
-          for (int i = 0; i < 4; ++i) v[uu][i] = (uu < nu && p < POS) ? g[(int64_t)(p + i) * C_OUT] : 0.0f;
+          for (int i = 0; i < 4; ++i) Y[i] = (uint32_t)__float2int_rn(v[uu][i] * inv_s24) + 0x00808080u;
+          // 4x4 byte transpose: digit d of the four positions packed into one word
+          const uint32_t t0 = __byte_perm(Y[0], Y[1], 0x5140), t1 = __byte_perm(Y[0], Y[1], 0x7362);
+          const uint32_t t2 = __byte_perm(Y[2], Y[3], 0x5140), t3 = __byte_perm(Y[2], Y[3], 0x7362);
+          const uint32_t d3 = __byte_perm(t0, t2, 0x5410) ^ 0x80808080u, d2 = __byte_perm(t0, t2, 0x7632) ^ 0x80808080u;
+          const uint32_t d1 = __byte_perm(t1, t3, 0x5410) ^ 0x80808080u, d0 = __byte_perm(t1, t3, 0x7632);
+          const int off = (((u0 + uu) ^ c3) << 4) + pq * 4;    // rows d*C_OUT + co: (row & 7) == c3
+          *reinterpret_cast<uint32_t*>(dstB + sw_row(0 * C_OUT + co) + off) = d0;
+          *reinterpret_cast<uint32_t*>(dstB + sw_row(1 * C_OUT + co) + off) = d1;
+          *reinterpret_cast<uint32_t*>(dstB + sw_row(2 * C_OUT + co) + off) = d2;
+          *reinterpret_cast<uint32_t*>(dstB + sw_row(3 * C_OUT + co) + off) = d3;
         }
-        if (P.y) {                                       // ReLU mask of the fused forward
-          const float* yk = P.y + base;
-#pragma unroll
-          for (int uu = 0; uu < 4; ++uu) {
-            const int p = j * KCHUNK + (u0 + uu) * 16 + 4 * pq;
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              if (uu < nu && p < POS && !(yk[(int64_t)(p + i) * C_OUT] > 0.0f)) v[uu][i] = 0.0f;
-          }
-        }
-      };
-      float v[4][4], vn[4][4];
-      if (active && total > 0) load_chunk(0, v);
-      for (int at = 0; at < total; ++at) {
-        const int stage = at % STAGES, j = at & 3;
-        // this warp's units of the chunk: 4 of 8 (last chunk: unit 0 = positions 384..399, unit 1 = zeros)
-        const int u0 = (j < CHUNKS - 1) ? uh * 4 : uh, nu = (j < CHUNKS - 1) ? 4 : 1;
-        if (active && at + 1 < total) load_chunk(at + 1, vn);
-        const long long b0 = clock64();
-        mbar_wait(&s_empty[stage], ((at / STAGES) & 1) ^ 1);
-        const long long b1 = clock64();
-        if (active) {
-          uint8_t* dstB = sStage + stage * STAGE_BYTES + A_BYTES;
-#pragma unroll
-          for (int uu = 0; uu < 4; ++uu) {
-            if (uu >= nu) break;
-            // X = gy / s * 2^24 as an int32 (exact: power-of-two scale, |X| <= 127 * 2^24); balanced base-256 digits
-            // via the bias 0x00808080: the three low bytes come out as q + 128, the top byte is q0 itself.
-            uint32_t Y[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) Y[i] = (uint32_t)__float2int_rn(v[uu][i] * inv_s24) + 0x00808080u;
-            // 4x4 byte transpose: digit d of the four positions packed into one word
-            const uint32_t t0 = __byte_perm(Y[0], Y[1], 0x5140), t1 = __byte_perm(Y[0], Y[1], 0x7362);
-            const uint32_t t2 = __byte_perm(Y[2], Y[3], 0x5140), t3 = __byte_perm(Y[2], Y[3], 0x7362);
-            const uint32_t d3 = __byte_perm(t0, t2, 0x5410) ^ 0x80808080u, d2 = __byte_perm(t0, t2, 0x7632) ^ 0x80808080u;
-            const uint32_t d1 = __byte_perm(t1, t3, 0x5410) ^ 0x80808080u, d0 = __byte_perm(t1, t3, 0x7632);
-            const int off = (((u0 + uu) ^ c3) << 4) + pq * 4;    // rows d*C_OUT + co: (row & 7) == c3
-            *reinterpret_cast<uint32_t*>(dstB + sw_row(0 * C_OUT + co) + off) = d0;
-            *reinterpret_cast<uint32_t*>(dstB + sw_row(1 * C_OUT + co) + off) = d1;
-            *reinterpret_cast<uint32_t*>(dstB + sw_row(2 * C_OUT + co) + off) = d2;
-            *reinterpret_cast<uint32_t*>(dstB + sw_row(3 * C_OUT + co) + off) = d3;
-          }
-        }
-        const long long b2 = clock64();
-        fence_async_smem();
-        mbar_arrive(&s_full[stage]);
-        if (probe) { P.dbg[7] += b1 - b0; P.dbg[8] += b2 - b1; P.dbg[12] += clock64() - b2; }
-#pragma unroll
-        for (int uu = 0; uu < 4; ++uu)
-#pragma unroll
-          for (int i = 0; i < 4; ++i) v[uu][i] = vn[uu][i];
       }
-      if (warp >= 16) {
-        // ------------------------------- epilogue (once) -------------------------------
-        const int wq = warp & 3;
-        const long long e0 = clock64();
-        mbar_wait(&acc_full, 0);
-        const long long e1 = clock64();
-        tc_fence_after();
-        float my_scale = 0.0f;                               // lane = channel: s * 2^-8 / 255
-        if (lane < C_OUT) {
-          const float t = __uint_as_float(s_absmax[lane]) / 127.0f;
-          int ex = (int)((__float_as_uint(t) >> 23) & 0xFF) + 1;
-          ex = ex < 27 ? 27 : (ex > 227 ? 227 : ex);
-          my_scale = __uint_as_float((uint32_t)(ex - 8) << 23) / 255.0f;
-        }
-        float* out = P.partial + (int64_t)blockIdx.x * (C_OUT * E_TOTAL);
-#pragma unroll 1
-        for (int h = 0; h < 2; ++h) {
-          const int e = h * 128 + wq * 32 + lane;
-          const uint32_t tbase = tmem + ((uint32_t)(wq * 32) << 16) + (uint32_t)(h * N_TOTAL);
-#pragma unroll 1
-          for (int cg = 0; cg < C_OUT / 16; ++cg) {
-            int32_t q0[16], q1[16], q2[16], q3[16];
-            tc_ld16(tbase + 0 * C_OUT + cg * 16, q0);
-            tc_ld16(tbase + 1 * C_OUT + cg * 16, q1);
-            tc_ld16(tbase + 2 * C_OUT + cg * 16, q2);
-            tc_ld16(tbase + 3 * C_OUT + cg * 16, q3);
-            tc_wait_ld();
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const int cc = cg * 16 + i;
-              // digit sums recombined pairwise in exact int64, one fp32 rounding per half, one FMA, the scale
-              const float fu = (float)((long long)q0[i] * 256 + (long long)q1[i]);
-              const float ft = (float)((long long)q2[i] * 256 + (long long)q3[i]);
-              out[cc * E_TOTAL + e] = __fmaf_rn(ft, 1.0f / 65536.0f, fu) * __shfl_sync(0xffffffffu, my_scale, cc);
-            }
-          }
-        }
-        if (P.dbg && blockIdx.x == 0 && warp == 16 && lane == 0) { P.dbg[9] += e1 - e0; P.dbg[10] += clock64() - e1; P.dbg[11] += clock64() - t_start; }
+      for (int uu = 0; uu < 4; ++uu)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) v[uu][i] = vn[uu][i];
+    }
+    fence_async_smem();                              // generic-proxy writes -> visible to the tensor core
+    // The chunk is complete once every producer is here.  Passing this barrier also means every warpgroup has
+    // waited for the MMAs of chunk at - 2, which read the stage that chunk at + 1 will overwrite (STAGES = 3).
+    named_sync(2, THREADS);
+    const uint32_t a_base = sptr(st) + wg * (64 * 128), b_base = sptr(st + A_BYTES);
+    // last chunk: positions 384..399 (+16 zeros) in K step 0; its other K steps multiply by the zero operand, which
+    // keeps the wgmma sequence free of branches (a divergent path would serialize every wgmma of the kernel)
+    const uint32_t b_tail = (j < CHUNKS - 1) ? b_base : sptr(sZero);
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks)
+      acc.mma(make_desc(a_base + ks * 32), make_desc((ks == 0 ? b_base : b_tail) + ks * 32), (at | ks) ? 1u : 0u);
+    wg_commit();
+    wg_wait<1>();
+  }
+  wg_wait<0>();
+  wg_fence_regs(acc.d);
+
+  // ------------------------------- epilogue -------------------------------
+  // fragment (hopper.cuh): patch elements e and e + 8, columns 8j + 2(lane % 4) + {0, 1}; column d * C_OUT + co is
+  // digit d of channel co
+  if (total == 0) return;
+  float* out = P.partial + (int64_t)blockIdx.x * (C_OUT * E_TOTAL);
+  const int e_base = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+  for (int jj = 0; jj < C_OUT / 8; ++jj) {
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      const int cc = 8 * jj + 2 * (lane & 3) + c;
+      const float scale = __uint_as_float((uint32_t)(digit_exponent(s_absmax[cc]) - 8) << 23) / 255.0f;   // s * 2^-8 / 255
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int i = 4 * jj + 2 * h + c;
+        const int32_t q0 = acc.d[i], q1 = acc.d[i + C_OUT / 2], q2 = acc.d[i + C_OUT], q3 = acc.d[i + 3 * C_OUT / 2];
+        // digit sums recombined pairwise in exact int64, one fp32 rounding per half, one FMA, the scale
+        const float fu = (float)((long long)q0 * 256 + (long long)q1);
+        const float ft = (float)((long long)q2 * 256 + (long long)q3);
+        out[cc * E_TOTAL + e_base + 8 * h] = __fmaf_rn(ft, 1.0f / 65536.0f, fu) * scale;
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS));
   }
 }
 
 // dW[i] (+)= sum over CTAs of partial[cta][i] in fp64, fixed order (deterministic, no atomics).
 // Block = 32 outputs x 8 slices of the partials: slice j adds partials j, j+8, ... (about 19 independent coalesced
-// loads per thread instead of a 148-long chain: the kernel is L2-latency bound), then the 8 slices are added in order.
+// loads per thread instead of a 132-long chain: the kernel is L2-latency bound), then the 8 slices are added in order.
 constexpr int RED_SLICES = 8;
 __global__ void __launch_bounds__(32 * RED_SLICES)
 k_conv1_wgrad_reduce(const float* __restrict__ partial, int n_parts, int numel, int accumulate, float* __restrict__ out) {
@@ -427,7 +326,7 @@ k_conv1_wgrad_reduce(const float* __restrict__ partial, int n_parts, int numel, 
 
 template <int C_OUT>
 constexpr size_t smem_bytes() {
-  return (size_t)STAGES * (A_BYTES + NSPLIT * C_OUT * KCHUNK) + 2 * (size_t)RAW_STRIDE + 1024;
+  return (size_t)STAGES * (A_BYTES + NSPLIT * C_OUT * KCHUNK) + 2 * (size_t)RAW_STRIDE + NSPLIT * C_OUT * KCHUNK + 1024;
 }
 
 }  // namespace conv1w
@@ -473,15 +372,12 @@ extern "C" int b2rl_conv1_wgrad(const uint8_t* frames_dev, int64_t capacity, con
   if (!sms[dev & 63]) B2RL_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
   cudaStream_t st = (cudaStream_t)stream;
   const int numel = c_out * conv1w::E_TOTAL;
-  static long long* dbg_buf = nullptr;
-  if (getenv("B2RL_CONV1_DBG") && !dbg_buf) B2RL_CUDA(cudaMalloc(&dbg_buf, 16 * sizeof(long long)));
-  if (dbg_buf) B2RL_CUDA(cudaMemsetAsync(dbg_buf, 0, 16 * sizeof(long long), st));
   const int64_t per_launch = (int64_t)sms[dev & 63] * conv1w::MAX_ITEMS_PER_CTA;   // int32 accumulator bound
   for (int64_t off = 0; off < n; off += per_launch) {
     const int64_t m = (n - off < per_launch) ? n - off : per_launch;
     conv1w::Params P{frames_dev, idx_dev ? idx_dev + off : nullptr, m, capacity,
                      gy_dev + off * (int64_t)(conv1w::POS * c_out),
-                     y_relu_dev ? y_relu_dev + off * (int64_t)(conv1w::POS * c_out) : nullptr, workspace_dev, dbg_buf};
+                     y_relu_dev ? y_relu_dev + off * (int64_t)(conv1w::POS * c_out) : nullptr, workspace_dev};
     if (!idx_dev) P.frames = frames_dev + off * conv1w::FRAME_BYTES, P.capacity = capacity - off;
     const unsigned grid = (unsigned)((m < sms[dev & 63]) ? m : sms[dev & 63]);
     B2RL_CUDA(c_out == 32 ? wgrad_launch<32>(P, grid, st) : wgrad_launch<16>(P, grid, st));
@@ -491,14 +387,6 @@ extern "C" int b2rl_conv1_wgrad(const uint8_t* frames_dev, int64_t capacity, con
         workspace_dev, (int)grid, numel, (accumulate || off > 0) ? 1 : 0, gw_dev);
     count_launch();
     B2RL_CHECK_LAUNCH();
-  }
-  if (dbg_buf) {   // profiling aid: per-role cycle counters of CTA 0 (synchronous; never set in production)
-    long long h[16];
-    B2RL_CUDA(cudaMemcpy(h, dbg_buf, sizeof(h), cudaMemcpyDeviceToHost));
-    static const char* names[14] = {"mma:wait s_full", "mma:issue+commit", "A:prescan", "A:wait raw_full", "A:wait s_empty",
-                                    "A:build", "B:prescan", "B:wait s_empty", "B:build", "epi:wait acc", "epi:work",
-                                    "producers total", "B:fence+arrive", "A:fence+arrive"};
-    for (int i = 0; i < 14; ++i) fprintf(stderr, "[conv1 wgrad dbg] n %lld %-20s %lld\n", (long long)n, names[i], h[i]);
   }
   return B2RL_OK;
 }

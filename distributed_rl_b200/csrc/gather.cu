@@ -232,7 +232,7 @@ k_gather_small(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int64
 }
 
 // LDG.128/STG.128 reference implementation of the big-row gather (kept for the
-// A/B comparison in profiles/, selectable with B2RL_GATHER=ldg).
+// A/B comparison with the bulk-copy gather, selectable with B2RL_GATHER=ldg).
 __global__ void __launch_bounds__(256)
 k_gather_ldg(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int64_t row_bytes,
              const int64_t* __restrict__ idx, int64_t n, int64_t capacity) {
@@ -386,7 +386,7 @@ extern "C" int b2rl_replay_fill_hash(b2rl_replay* h, int64_t n, uint32_t seed, v
     const int64_t words = n * ((h->field_bytes[f] + 3) / 4);
     if (words == 0) continue;
     int64_t blocks = (words + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;   // 32 CTAs per SM of an H100
     k_fill_hash<<<(unsigned)blocks, 256, 0, st>>>(h->field[f], h->field_bytes[f], n, seed,
                                                   (uint32_t)f * 0x9E3779B9U);
     count_launch();

@@ -1,123 +1,33 @@
 // fp32-accurate dense layers on the tensor cores: C[M][N] (+)= A[M][K] * B[N][K]^T with 3xTF32.
 //
 // The dense heads of the Q-network (3136 -> 512, twice; cfg/ape_x.json:52-71) run as cuBLAS fp32
-// SIMT GEMMs at PyTorch's default precision and are 31 % of the learner step (DESIGN.md §6b).
+// SIMT GEMMs at PyTorch's default precision and are the largest share of the learner step (DESIGN.md §6b).
 // TF32 alone (10-bit mantissa) is not what the reference computes, so every fp32 operand is split
 //      x = hi + lo,   hi = rn_tf32(x),  lo = x - hi   (exact in fp32)
-// and the product is formed as  hi*hi + hi*lo + lo*hi  on tcgen05 (kind::tf32, fp32 accumulation in
-// TMEM); the dropped lo*lo term is 2^-22 relative.  SURVEY.md §8f rank 2 ("TF32x3 policy").
+// and the product is formed as  hi*hi + hi*lo + lo*hi  with wgmma (tf32 inputs, fp32 accumulation in
+// registers); the dropped lo*lo term is 2^-22 relative.  SURVEY.md §8f rank 2 ("TF32x3 policy").
 //
 //   k_split_pack   fp32 matrix (optionally transposed) -> {hi, lo} operand images in exactly the
 //                  128B-swizzled, K-major tile layout the MMA reads, so the GEMM's loader is a
 //                  plain cp.async.bulk per tile (no tensor map, no SM-side staging)
-//   k_gemm_tf32x3  one CTA per (m-tile 128, n-tile 256, K-split): TMA loader warp, one MMA-issuing
-//                  thread (12 x tcgen05.mma per 32-float K chunk), 4 epilogue warps that store the tile
-//                  (or, when K is split, this split's partial tile) with coalesced 512-byte stores
+//   k_gemm_tf32x3  one CTA per (m-tile 128, n-tile 256, K-split): a TMA loader warp and two consumer
+//                  warpgroups (64 rows each, 12 x wgmma m64n256k8 per 32-float K chunk) that store the tile
+//                  (or, when K is split, this split's partial tile) straight from their accumulators
 //   k_splitk_reduce sums the K-split partials in split order: the result is deterministic (no atomics)
 #include "common.cuh"
-
-#include <stdlib.h>
+#include "hopper.cuh"
 
 namespace b2rl {
 namespace gemm {
+
+using namespace sm90;
 
 constexpr int TM = 128, TN = 256, KC = 32;          // tile rows of A / of B, floats per K chunk (128 B)
 constexpr int A_TILE = TM * 128, B_TILE = TN * 128;  // bytes of one {term, k-chunk} tile: 16 KiB / 32 KiB
 constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;       // hi+lo of both operands: 96 KiB
 constexpr int STAGES = 2;
-constexpr int THREADS = 224;                         // warp 0 loader, 1 MMA, 2 TMEM alloc, 3-6 epilogue
-
-__device__ __forceinline__ uint32_t sptr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* b, uint32_t c) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(sptr(b)), "r"(c));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* b, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sptr(b)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* b, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "W_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra D_%=;\n\t"
-      "bra W_%=;\n\t"
-      "D_%=:\n\t}" ::"r"(sptr(b)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   sptr(dst)), "l"(src), "r"(bytes), "r"(sptr(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(sptr(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc),
-      "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// K-major SW128 descriptor (see csrc/conv1.cu): SBO = 1024 B, LBO = 16 B, version 1, layout SWIZZLE_128B
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-// c_format F32 (1) @4, a_format TF32 (2) @7, b_format TF32 (2) @10, N>>3 @17, M>>4 @24
-constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-
-
-// ---- cta_group::2 helpers (CTA pair: one 256-row MMA over two SMs) ---------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same CTA-relative address in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* b, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(sptr(b)), "r"(rank) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* b, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "W_%=:\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra D_%=;\n\t"
-      "bra W_%=;\n\t"
-      "D_%=:\n\t}" ::"r"(sptr(b)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tc_commit2(uint64_t* bar) {   // arrives on `bar` of BOTH CTAs of the pair
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   sptr(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void tc_mma_tf32_2cta(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc),
-      "r"(idesc), "r"(accumulate) : "memory");
-}
-// M = 256 over the pair, N = 256
-constexpr uint32_t IDESC2 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)((2 * TM) >> 4) << 24);
-constexpr int STAGE2 = 2 * A_TILE + B_TILE;          // A hi+lo (my 128 rows) + my HALF of B hi+lo: 64 KiB
-constexpr int STAGES2 = 3;
+constexpr int CONSUMERS = 256;                       // warpgroups 0-1: MMA + epilogue
+constexpr int THREADS = CONSUMERS + 32;              // warp 8: TMA loader
 
 // ---- operand packing ---------------------------------------------------------
 // Image layout: [term 0=hi,1=lo][k_chunk][row_tile][row_in_tile][128 B, 16-byte units XOR (row & 7)]
@@ -304,8 +214,7 @@ __global__ void __launch_bounds__(THREADS, 1)
 k_gemm_tf32x3(const __grid_constant__ Params P) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (sptr(smem_raw) & 1023u)) & 1023u);
-  __shared__ __align__(8) uint64_t full[STAGES], empty[STAGES], acc_full;
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t full[STAGES], empty[STAGES];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t mt = blockIdx.x, nt = blockIdx.y;
   // K range of this split
@@ -315,237 +224,71 @@ k_gemm_tf32x3(const __grid_constant__ Params P) {
   const int64_t nk = k1 - k0;   // > 0: the host never launches an empty trailing split (gemm_splits)
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(&acc_full, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], CONSUMERS); }
+    mbar_init_fence();
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sptr(&s_tmem)), "n"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = s_tmem;
+  if (nk <= 0) return;
 
-  if (nk > 0) {
-    const int64_t a_term = P.k_chunks * P.m_tiles * (TM * 32);   // floats between the hi and lo images
-    const int64_t b_term = P.k_chunks * P.n_tiles * (TN * 32);
-    if (warp == 0) {
-      if (lane == 0) {
-        for (int64_t i = 0; i < nk; ++i) {
-          const int s = (int)(i % STAGES);
-          mbar_wait(&empty[s], ((i / STAGES) & 1) ^ 1);
-          const int64_t kc = k0 + i;
-          const float* a_hi = P.a + (kc * P.m_tiles + mt) * (TM * 32);
-          const float* b_hi = P.b + (kc * P.n_tiles + nt) * (TN * 32);
-          uint8_t* st = smem + (size_t)s * STAGE;
-          mbar_expect_tx(&full[s], STAGE);
-          bulk_g2s(st, a_hi, A_TILE, &full[s]);
-          bulk_g2s(st + A_TILE, a_hi + a_term, A_TILE, &full[s]);
-          bulk_g2s(st + 2 * A_TILE, b_hi, B_TILE, &full[s]);
-          bulk_g2s(st + 2 * A_TILE + B_TILE, b_hi + b_term, B_TILE, &full[s]);
-        }
-      }
-    } else if (warp == 1) {
-      if (lane == 0) {
-        for (int64_t i = 0; i < nk; ++i) {
-          const int s = (int)(i % STAGES);
-          mbar_wait(&full[s], (i / STAGES) & 1);
-          tc_fence_after();
-          const uint32_t base = sptr(smem + (size_t)s * STAGE);
-          const uint32_t a_hi = base, a_lo = base + A_TILE, b_hi = base + 2 * A_TILE, b_lo = b_hi + B_TILE;
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint32_t o = ks * 32;
-            tc_mma_tf32(tmem, make_desc(a_lo + o), make_desc(b_hi + o), IDESC, (i | ks) ? 1u : 0u);   // small terms first
-            tc_mma_tf32(tmem, make_desc(a_hi + o), make_desc(b_lo + o), IDESC, 1u);
-            tc_mma_tf32(tmem, make_desc(a_hi + o), make_desc(b_hi + o), IDESC, 1u);
-          }
-          tc_commit(&empty[s]);
-        }
-        tc_commit(&acc_full);
-      }
-    } else if (warp >= 3) {
-      // ------------------------------- epilogue -------------------------------
-      const int wq = warp & 3;                          // TMEM lane quarter (warps 3..6 -> 3,0,1,2)
-      mbar_wait(&acc_full, 0);
-      tc_fence_after();
-      uint8_t* stg = smem + (size_t)wq * 4096;          // pipeline SMEM is idle now: 32 rows x 128 B per warp
-      const int64_t row0 = mt * TM + wq * 32;
-      const uint32_t tbase = tmem + ((uint32_t)(wq * 32) << 16);
-      for (int c0 = 0; c0 < TN; c0 += 32) {
-        uint32_t v0[16], v1[16];
-        tc_ld16(tbase + c0, v0);
-        tc_ld16(tbase + c0 + 16, v1);
-        tc_wait_ld();
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          *reinterpret_cast<uint4*>(stg + lane * 128 + ((g ^ (lane & 7)) << 4)) =
-              make_uint4(v0[4 * g], v0[4 * g + 1], v0[4 * g + 2], v0[4 * g + 3]);
-          *reinterpret_cast<uint4*>(stg + lane * 128 + (((4 + g) ^ (lane & 7)) << 4)) =
-              make_uint4(v1[4 * g], v1[4 * g + 1], v1[4 * g + 2], v1[4 * g + 3]);
-        }
-        __syncwarp();
-        const int64_t col0 = nt * TN + c0;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int off = (i * 32 + lane) * 16;
-          const int row = off >> 7, unit = (off >> 4) & 7;
-          const int64_t m = row0 + row, n = col0 + unit * 4;
-          float* dst = P.c + ((int64_t)blockIdx.z * P.M + m) * P.ldc + n;
-          if (m < P.M && n + 3 < P.N) {
-            *reinterpret_cast<float4*>(dst) =
-                *reinterpret_cast<const float4*>(stg + row * 128 + ((unit ^ (row & 7)) << 4));
-          } else if (m < P.M && n < P.N) {
-            const float* x = reinterpret_cast<const float*>(stg + row * 128 + ((unit ^ (row & 7)) << 4));
-            for (int e = 0; e < 4 && n + e < P.N; ++e) dst[e] = x[e];
-          }
-        }
-        __syncwarp();
+  if (warp == CONSUMERS / 32) {
+    // ------------------------------ TMA loader ------------------------------
+    if (lane == 0) {
+      const int64_t a_term = P.k_chunks * P.m_tiles * (TM * 32);   // floats between the hi and lo images
+      const int64_t b_term = P.k_chunks * P.n_tiles * (TN * 32);
+      for (int64_t i = 0; i < nk; ++i) {
+        const int s = (int)(i % STAGES);
+        mbar_wait(&empty[s], ((i / STAGES) & 1) ^ 1);
+        const int64_t kc = k0 + i;
+        const float* a_hi = P.a + (kc * P.m_tiles + mt) * (TM * 32);
+        const float* b_hi = P.b + (kc * P.n_tiles + nt) * (TN * 32);
+        uint8_t* st = smem + (size_t)s * STAGE;
+        mbar_expect_tx(&full[s], STAGE);
+        bulk_g2s(st, a_hi, A_TILE, &full[s]);
+        bulk_g2s(st + A_TILE, a_hi + a_term, A_TILE, &full[s]);
+        bulk_g2s(st + 2 * A_TILE, b_hi, B_TILE, &full[s]);
+        bulk_g2s(st + 2 * A_TILE + B_TILE, b_hi + b_term, B_TILE, &full[s]);
       }
     }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(256));
-  }
-}
 
-
-// ---- the same GEMM on CTA pairs (tcgen05 cta_group::2) ------------------------------------------------------------
-// Two CTAs of a cluster own m-tiles 2c and 2c+1 of the same n-tile and K split.  The leader (rank 0) issues ONE
-// M = 256 MMA per step for both; A comes from each CTA's own shared memory (its 128 rows) and every CTA holds only
-// its HALF of the B tile (128 of the 256 rows), which the pair's tensor cores share.  Per SM and K chunk 64 KiB are
-// staged instead of 96 KiB, for the same MMA work per SM: the single-CTA kernel is bound by exactly that
-// (shared-memory fill + operand reads per SM; tensor pipe 49 % active, DESIGN.md §4.9), and the freed space buys a
-// third pipeline stage.  Barriers: every CTA's loader arms its LOCAL full barrier (tx bytes); a relay thread per CTA
-// forwards "my stage is full" to the leader's pair barrier (count 2, remote arrive); the leader's tcgen05.commit is
-// multicast to both CTAs' empty / accumulator barriers.
-__global__ void __launch_bounds__(THREADS, 1)
-k_gemm_tf32x3_2cta(const __grid_constant__ Params P) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (sptr(smem_raw) & 1023u)) & 1023u);
-  __shared__ __align__(8) uint64_t full[STAGES2], pair_full[STAGES2], empty[STAGES2], acc_full;
-  __shared__ uint32_t s_tmem;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t crank = cluster_ctarank();
-  const int64_t mt = blockIdx.x, nt = blockIdx.y;     // blockIdx.x = 2 * pair + crank
-  const int64_t per = (P.k_chunks + P.splits - 1) / P.splits;
-  const int64_t k0 = (int64_t)blockIdx.z * per;
-  const int64_t k1 = (k0 + per < P.k_chunks) ? k0 + per : P.k_chunks;
-  const int64_t nk = k1 - k0;
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES2; ++i) { mbar_init(&full[i], 1); mbar_init(&pair_full[i], 2); mbar_init(&empty[i], 1); }
-    mbar_init(&acc_full, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  cluster_sync_all();                 // both CTAs' barriers exist before anything can arrive at them
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sptr(&s_tmem)), "n"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = s_tmem;
-  cluster_sync_all();                 // both halves of the pair's TMEM are allocated
-
-  if (nk > 0) {
-    const int64_t a_term = P.k_chunks * P.m_tiles * (TM * 32);
-    const int64_t b_term = P.k_chunks * P.n_tiles * (TN * 32);
-    if (warp == 0) {
-      if (lane == 0) {                // loader: my A tile + my half of the B tile
-        for (int64_t i = 0; i < nk; ++i) {
-          const int s = (int)(i % STAGES2);
-          mbar_wait(&empty[s], ((i / STAGES2) & 1) ^ 1);
-          const int64_t kc = k0 + i;
-          const float* a_hi = P.a + (kc * P.m_tiles + mt) * (TM * 32);
-          const float* b_hi = P.b + (kc * P.n_tiles + nt) * (TN * 32) + (int64_t)crank * ((TN / 2) * 32);
-          uint8_t* st = smem + (size_t)s * STAGE2;
-          mbar_expect_tx(&full[s], STAGE2);
-          bulk_g2s(st, a_hi, A_TILE, &full[s]);
-          bulk_g2s(st + A_TILE, a_hi + a_term, A_TILE, &full[s]);
-          bulk_g2s(st + 2 * A_TILE, b_hi, B_TILE / 2, &full[s]);
-          bulk_g2s(st + 2 * A_TILE + B_TILE / 2, b_hi + b_term, B_TILE / 2, &full[s]);
-        }
-      }
-    } else if (warp == 2) {
-      if (lane == 0) {                // relay: my stage landed -> tell the leader's pair barrier
-        for (int64_t i = 0; i < nk; ++i) {
-          const int s = (int)(i % STAGES2);
-          mbar_wait(&full[s], (i / STAGES2) & 1);
-          mbar_arrive_remote(&pair_full[s], 0);
-        }
-      }
-    } else if (warp == 1) {
-      if (lane == 0 && crank == 0) {  // the leader issues the pair's MMAs
-        for (int64_t i = 0; i < nk; ++i) {
-          const int s = (int)(i % STAGES2);
-          mbar_wait_cluster(&pair_full[s], (i / STAGES2) & 1);
-          tc_fence_after();
-          const uint32_t base = sptr(smem + (size_t)s * STAGE2);
-          const uint32_t a_hi = base, a_lo = base + A_TILE, b_hi = base + 2 * A_TILE, b_lo = b_hi + B_TILE / 2;
+  // ------------------------- consumers: wgmma + epilogue -------------------------
+  const int wg = warp >> 2;                            // rows [64 wg, 64 wg + 64) of the tile
+  float acc[128];
+  for (int64_t i = 0; i < nk; ++i) {
+    const int s = (int)(i % STAGES);
+    mbar_wait(&full[s], (i / STAGES) & 1);
+    const uint32_t base = sptr(smem + (size_t)s * STAGE);
+    const uint32_t a_hi = base + wg * (64 * 128), a_lo = a_hi + A_TILE, b_hi = base + 2 * A_TILE, b_lo = b_hi + B_TILE;
+    wg_fence();
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint32_t o = ks * 32;
-            tc_mma_tf32_2cta(tmem, make_desc(a_lo + o), make_desc(b_hi + o), IDESC2, (i | ks) ? 1u : 0u);   // small terms first
-            tc_mma_tf32_2cta(tmem, make_desc(a_hi + o), make_desc(b_lo + o), IDESC2, 1u);
-            tc_mma_tf32_2cta(tmem, make_desc(a_hi + o), make_desc(b_hi + o), IDESC2, 1u);
-          }
-          tc_commit2(&empty[s]);      // both CTAs' stage s may be refilled
-        }
-        tc_commit2(&acc_full);        // both CTAs' halves of the accumulator are complete
-      }
-    } else if (warp >= 3) {
-      // ------------------------------- epilogue (my 128 rows) -------------------------------
-      const int wq = warp & 3;
-      mbar_wait(&acc_full, 0);
-      tc_fence_after();
-      uint8_t* stg = smem + (size_t)wq * 4096;
-      const int64_t row0 = mt * TM + wq * 32;
-      const uint32_t tbase = tmem + ((uint32_t)(wq * 32) << 16);
-      for (int c0 = 0; c0 < TN; c0 += 32) {
-        uint32_t v0[16], v1[16];
-        tc_ld16(tbase + c0, v0);
-        tc_ld16(tbase + c0 + 16, v1);
-        tc_wait_ld();
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          *reinterpret_cast<uint4*>(stg + lane * 128 + ((g ^ (lane & 7)) << 4)) =
-              make_uint4(v0[4 * g], v0[4 * g + 1], v0[4 * g + 2], v0[4 * g + 3]);
-          *reinterpret_cast<uint4*>(stg + lane * 128 + (((4 + g) ^ (lane & 7)) << 4)) =
-              make_uint4(v1[4 * g], v1[4 * g + 1], v1[4 * g + 2], v1[4 * g + 3]);
-        }
-        __syncwarp();
-        const int64_t col0 = nt * TN + c0;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int off = (i * 32 + lane) * 16;
-          const int row = off >> 7, unit = (off >> 4) & 7;
-          const int64_t m = row0 + row, n = col0 + unit * 4;
-          float* dst = P.c + ((int64_t)blockIdx.z * P.M + m) * P.ldc + n;
-          if (m < P.M && n + 3 < P.N) {
-            *reinterpret_cast<float4*>(dst) =
-                *reinterpret_cast<const float4*>(stg + row * 128 + ((unit ^ (row & 7)) << 4));
-          } else if (m < P.M && n < P.N) {
-            const float* x = reinterpret_cast<const float*>(stg + row * 128 + ((unit ^ (row & 7)) << 4));
-            for (int e = 0; e < 4 && n + e < P.N; ++e) dst[e] = x[e];
-          }
-        }
-        __syncwarp();
-      }
+    for (int ks = 0; ks < 4; ++ks) {
+      const uint32_t o = ks * 32;
+      mma_tf32_n256(acc, make_desc(a_lo + o), make_desc(b_hi + o), (i | ks) ? 1u : 0u);   // small terms first
+      mma_tf32_n256(acc, make_desc(a_hi + o), make_desc(b_lo + o), 1u);
+      mma_tf32_n256(acc, make_desc(a_hi + o), make_desc(b_hi + o), 1u);
     }
+    wg_commit();
+    wg_wait<1>();                                      // the MMAs of chunk i - 1 are done: its stage may be refilled
+    wg_fence_regs(acc);
+    if (i > 0) mbar_arrive(&empty[(i - 1) % STAGES]);
   }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                 // neither CTA frees TMEM / exits while the pair may still use it
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(256));
+  wg_wait<0>();
+  wg_fence_regs(acc);
+  // fragment (see hopper.cuh): rows r0 and r0 + 8, columns 8j + 2(lane % 4) + {0, 1}
+  const int64_t r0 = mt * TM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  float* cz = P.c + (int64_t)blockIdx.z * P.M * P.ldc;
+#pragma unroll
+  for (int j = 0; j < TN / 8; ++j) {
+    const int64_t n = nt * TN + 8 * j + 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t m = r0 + 8 * h;
+      if (m >= P.M || n >= P.N) continue;
+      float* dst = cz + m * P.ldc + n;
+      if (n + 1 < P.N) *reinterpret_cast<float2*>(dst) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      else dst[0] = acc[4 * j + 2 * h];
+    }
   }
 }
 
@@ -662,16 +405,9 @@ extern "C" int b2rl_gemm_tf32x3(const float* a_packed_dev, const float* b_packed
   B2RL_CUDA(cudaGetDevice(&dev));
   static bool attr[64] = {false};
   const size_t smem_bytes = (size_t)gemm::STAGES * gemm::STAGE + 1024;
-  const size_t smem_bytes2 = (size_t)gemm::STAGES2 * gemm::STAGE2 + 1024;
   if (!attr[dev & 63]) {
     B2RL_CUDA(cudaFuncSetAttribute(gemm::k_gemm_tf32x3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    B2RL_CUDA(cudaFuncSetAttribute(gemm::k_gemm_tf32x3_2cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes2));
     attr[dev & 63] = true;
-  }
-  static int use_2cta = -1;
-  if (use_2cta < 0) {
-    const char* e = getenv("B2RL_GEMM_2CTA");     // opt-in: measured 23.5 us vs 21.5 us for the single-CTA kernel on the
-    use_2cta = (e && e[0] == '1') ? 1 : 0;        // heads' shapes (the GEMM is overhead-bound there, DESIGN.md §4.9)
   }
   const int64_t splits = gemm_splits(M, N, K, sms);
   B2RL_REQUIRE(splits == 1 || (workspace_dev && ((uintptr_t)workspace_dev % 16) == 0),
@@ -686,17 +422,7 @@ extern "C" int b2rl_gemm_tf32x3(const float* a_packed_dev, const float* b_packed
   P.splits = (int32_t)splits;
   cudaStream_t st = (cudaStream_t)stream;
   dim3 grid((unsigned)P.m_tiles, (unsigned)P.n_tiles, (unsigned)splits);
-  if (use_2cta && (P.m_tiles % 2) == 0) {       // CTA pairs along M (tcgen05 cta_group::2)
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid; cfg.blockDim = dim3(gemm::THREADS); cfg.dynamicSmemBytes = smem_bytes2; cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    B2RL_CUDA(cudaLaunchKernelEx(&cfg, gemm::k_gemm_tf32x3_2cta, P));
-  } else {
-    gemm::k_gemm_tf32x3<<<grid, gemm::THREADS, smem_bytes, st>>>(P);
-  }
+  gemm::k_gemm_tf32x3<<<grid, gemm::THREADS, smem_bytes, st>>>(P);
   count_launch();
   B2RL_CHECK_LAUNCH();
   if (splits > 1) {

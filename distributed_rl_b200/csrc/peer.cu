@@ -5,8 +5,7 @@
 // parallelism is new work).  Per step the ranks average two gradient slices: the dense heads' (12.9 MB, launched
 // early from the weight-gradient lane, NCCL) and what is left when backward ends — the convolution stack's
 // 0.3 MB.  That second one sits on the critical path between backward and the optimizer, and is latency-bound: an
-// NCCL all-reduce of it costs 12-19 us (RING_LL at 2 ranks; two of them were 30 us of the 45 us tail in
-// profiles/r02_timeline_2gpu.txt).  Here every rank
+// NCCL all-reduce of it is a whole collective launch for little data (DESIGN.md §5).  Here every rank
 //   0. copies its slice into its own symmetric staging buffer (parity = step & 1) and publishes a per-CTA flag
 //      to every peer (st.release.sys after __threadfence_system),
 //   1. waits for the same CTA's flag of every peer (ld.acquire.sys, bounded spin),
@@ -94,7 +93,7 @@ k_peer_allreduce_mean(const __grid_constant__ Params P) {
 
 
 // ---- the LARGE slice (the dense heads' 12.9 MB): reduce-scatter + all-gather in one kernel ----------------------
-// NCCL runs this as RING_LL on one NVSwitch node — 63 us at 2 ranks and 141 us at 8 (profiles/r02_timeline_*gpu.txt),
+// NCCL runs this as RING_LL on one NVSwitch node,
 // which at 8 ranks ends only when backward does, so the heads' optimizer step behind it lands on the critical path.
 // Here the gradient bucket itself is symmetric memory, and every rank r
 //   1. publishes "my gradients are final" (per-CTA flag) and waits for the same flag of every peer,

@@ -147,7 +147,7 @@ class FlatGradBucket:
                 and gs[0]["flat"].data_ptr() == self._flat_padded.data_ptr() \
                 and os.environ.get("B2RL_PEER_ALLREDUCE_BIG"):
             # opt-in: correct (tests/mgpu_worker.py), but at 2 ranks the kernel took 111 us against NCCL's 63 us
-            # running beside backward at the lane's low priority (profiles/r02_timeline_2gpu.txt; DESIGN.md §5)
+            # running beside backward at the lane's low priority (DESIGN.md §5)
             try:
                 self._peer_big = PeerAllReduceBig(self._symm, gs[0]["flat"].numel(), self.flat.device)
             except Exception as e:

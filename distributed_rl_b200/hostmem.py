@@ -4,10 +4,8 @@ The replay server feeds the learner from host memory (decoded Redis records,
 APE_X/ReplayMemory.py:128-139).  Staging buffers are pinned so the H2D copy is a straight DMA that
 overlaps the learner step.  cudaHostAlloc places pages on the node of the allocating thread, so the
 buffers are allocated with the thread temporarily bound to the GPU's node (best effort; a no-op when
-sysfs does not expose the topology).  On the two-socket B200 test box the steady-state copy rate was
-55 GB/s from either node (tools/h2d_probe.py, profiles/r01_h2d.md) — what matters there is that the
-PCIe link needs ~0.2 s of sustained traffic to reach that rate — so the binding is a safeguard for
-hosts with a slower socket interconnect, not a measured win.
+sysfs does not expose the topology).  The binding is a safeguard for hosts with a slow socket
+interconnect, not a measured win (tools/h2d_probe.py measures the copy rate from each node).
 """
 from __future__ import annotations
 

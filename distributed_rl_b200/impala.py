@@ -44,8 +44,8 @@ class ImpalaConfig:
     LOG_W: str | None = None
     OPTIM_INFO: dict = field(default_factory=lambda: {"name": "rmsprop", "lr": 6e-4, "decay": 0})
     MODEL: dict = field(default_factory=default_impala_model)
-    FUSED_CONV1: bool = True     # conv_1 (4 -> 16 channels) of every frame through libb2rl's tcgen05 kernel
-    DENSE_3XTF32: bool = True    # the 2592 -> 256 layer as a 3xTF32 tcgen05 GEMM (csrc/gemm.cu) instead of an fp32 SIMT sgemm
+    FUSED_CONV1: bool = True     # conv_1 (4 -> 16 channels) of every frame through libb2rl's wgmma kernel
+    DENSE_3XTF32: bool = True    # the 2592 -> 256 layer as a 3xTF32 wgmma GEMM (csrc/gemm.cu) instead of an fp32 SIMT sgemm
 
     @staticmethod
     def from_configuration():

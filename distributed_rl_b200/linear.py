@@ -3,7 +3,7 @@
 The reference's dense heads are `nn.Linear(..., bias=False)` (baseline/baseNetwork.py:77-79); on the
 GPU PyTorch runs them as fp32 SIMT GEMMs.  `linear3x(x, w)` computes the same `x @ w.T` — forward,
 input gradient and weight gradient — with every operand split into two TF32 terms and three
-tcgen05 products per term pair, fp32 accumulation in TMEM (error ~2^-22 relative per product,
+wgmma products per term pair, fp32 accumulation in registers (error ~2^-22 relative per product,
 the same order as an fp32 FMA chain; tests/test_gpu_03_gemm.py pins it against fp64).
 """
 from __future__ import annotations
@@ -31,7 +31,7 @@ class WeightGradSink:
         self.device = torch.device(device)
         # two lanes: the heads' weight gradients (the big GEMM + its operand packs) and the convolution stack's.
         # On one stream the conv_2 / conv_3 weight gradients queued behind the heads' and ran alone at the very end
-        # of backward (profiles/r02_timeline.txt); on their own lane they overlap the dgrad chain.
+        # of backward; on their own lane they overlap the dgrad chain.
         # Priorities (captured into the step's graph nodes): the learner's main branch runs at -2, the convolution
         # lane at -1 (its kernels must finish before the SM-filling conv_1 weight-gradient kernel starts), the
         # heads' lane (6.4 MB GEMM operands, the early optimizer step) at 0 fills what is left.

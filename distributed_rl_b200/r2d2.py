@@ -62,8 +62,8 @@ class R2D2Config:
     PAYLOAD_POOL: int = 0        # > 0: the sum-tree has REPLAY_MEMORY_LEN slots but only this many distinct sequences
                                  #      are stored, slot s reading row s % PAYLOAD_POOL (2^20 x 2.26 MB = 2.4 TB
                                  #      does not fit HBM; SURVEY §8d C3).  Benchmark-only; ingest needs 0.
-    FUSED_CONV1: bool = True     # conv_1 of every frame through libb2rl's tcgen05 kernel (gather fused)
-    FUSED_HEADS: bool = True     # dueling heads: 3xTF32 tcgen05 GEMM + fused tail kernels (csrc/gemm.cu, csrc/dueling.cu)
+    FUSED_CONV1: bool = True     # conv_1 of every frame through libb2rl's wgmma kernel (gather fused)
+    FUSED_HEADS: bool = True     # dueling heads: 3xTF32 wgmma GEMM + fused tail kernels (csrc/gemm.cu, csrc/dueling.cu)
 
     @staticmethod
     def from_configuration():

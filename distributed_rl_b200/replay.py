@@ -403,7 +403,7 @@ def vtrace(pi_a, mu_a, value, bootstrap, reward, gamma, c_lambda, c_bar, p_bar):
     return vt, adv
 
 
-# ---- fused gather + first convolution (tcgen05) ---------------------------------
+# ---- fused gather + first convolution (wgmma) -----------------------------------
 class Conv1Pack:
     """Packed conv_1 weights of 1 or 2 networks for b2rl_conv1_fused (re-pack after every
     optimizer step of the online net / target sync: one tiny launch per network)."""

@@ -8,7 +8,7 @@ learner: pickled `[s, a, r, s', done, w, idx]`), list `update` (learner -> serve
 flags `FLAG_BATCH` (enough data to serve), `FLAG_ENOUGH` (learner has > 32 batches queued), `FLAG_REMOVE` (learner asks
 for `remove_to_fit`).
 
-What is B200-native here is the server's store: sampling, IS weights, gather and priority write-back are the HBM
+What is GPU-native here is the server's store: sampling, IS weights, gather and priority write-back are the HBM
 kernels of libb2rl (one sample launch + one TMA gather per served group of minibatches, applied updates in stream
 order); the transport stays the reference's pickled Redis lists — this mode exists so that a deployment which
 runs the reference's replay out of process keeps working, not as the fast path (the in-process `Replay` is).

@@ -1,4 +1,4 @@
-/* b2rl.h — C ABI of the B200-native learner-side replay path.
+/* b2rl.h — C ABI of the H100-native learner-side replay path.
  *
  * The reference (seungju-k1m/Distributed_RL) is pure Python and defines no
  * FFI of its own; its boundary for this path is three duck-typed Python
@@ -229,7 +229,7 @@ int b2rl_vtrace(const float* pi_a_dev, const float* mu_a_dev, const float* value
 /* Fused gather + first convolution (north-star "TMA staging of sampled transition slices
  * into shared memory for the Q-network's first GEMM"): conv_1 of cfg/ape_x.json / cfg/r2d2.json
  * (8x8, stride 4, 4 -> 32 channels, no bias; baseline/baseNetwork.py:165-172) applied to
- * frames[idx[k]] / 255 (APE_X/Learner.py:61-67,78,85,87) on the tcgen05 tensor cores, for one or
+ * frames[idx[k]] / 255 (APE_X/Learner.py:61-67,78,85,87) on the Hopper tensor cores (wgmma), for one or
  * two networks (online + target) in one pass; the sampled uint8 frames are never staged in HBM.
  * c_out = 32 (cfg/ape_x.json, cfg/r2d2.json) or 16 (cfg/impala.json:25-37).
  *   b2rl_conv1_pack   w_dev fp32 [c_out][4][8][8] of network `net` -> packed int8 digits
@@ -282,7 +282,7 @@ int b2rl_rmsprop_norm_finish(double* sumsq_scratch_dev, int32_t n_tensors, float
 
 /* The dense heads of the networks (nn.Linear, bias-free: baseline/baseNetwork.py:77-79; 3136 -> 512
  * adv/val heads cfg/ape_x.json:52-71) at fp32 accuracy on the tensor cores: every fp32 operand is
- * split into two TF32 terms and C (+)= A[M][K] * B[N][K]^T is formed from three tcgen05 products
+ * split into two TF32 terms and C (+)= A[M][K] * B[N][K]^T is formed from three wgmma products
  * with fp32 accumulation.  `split_pack` turns a row-major fp32 matrix (or its transpose) into the
  * operand image (b_role = 0: the A / M side, 1: the B / N side); `packed_floats` is the size of
  * that image in floats.  Shapes with few output tiles split K over the SMs; their partial tiles go to

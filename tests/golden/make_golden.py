@@ -16,6 +16,8 @@ Groups
   apex    APE_X/Learner.py Learner.train   (Q-values captured by wrapping forward)
   r2d2    R2D2/Learner.py Learner.train    (MEM=40, SURVEY §8a-note 1)
   impala  IMPALA/Learner.py Learner.train  (V-trace internals captured at calLoss)
+  base_agent           baseline/baseAgent.py baseAgent Q on seeded weights and input
+  run_learner_imports  the import table of run_learner.py
 """
 from __future__ import annotations
 
@@ -451,8 +453,56 @@ def gen_impala_e2e():
     print("impala_e2e.npz:", len(out), "arrays")
 
 
+def gen_base_agent():
+    """baseline/baseAgent.py baseAgent on the Ape-X cfg: Q of a seeded input under seeded weights, so that
+    tests/test_dropin_cpu.py can check GraphAgent against it without the reference."""
+    import numpy as np
+    import torch
+    from oracle import ref_harness as H
+
+    H.enter_reference("ape_x.json")
+    import configuration as C  # type: ignore
+    from baseline.baseAgent import baseAgent  # type: ignore
+
+    ref = baseAgent(C.MODEL)
+    sd = ref.state_dict()
+    names = list(sd.keys())
+    ws = seeded_weights([tuple(sd[k].shape) if sd[k].dim() > 1 else (sd[k].shape[0], 64) for k in names], 606)
+    ref.load_state_dict({k: torch.from_numpy(w if sd[k].dim() > 1 else np.ascontiguousarray(w[:, 0]))
+                         for k, w in zip(names, ws)}, strict=True)
+    x = np.random.default_rng(0xB200 + 66).random((5, 4, 84, 84), dtype=np.float32)
+    with torch.no_grad():
+        q = ref.forward([torch.from_numpy(x)])[0]
+    np.savez_compressed(os.path.join(HERE, "base_agent.npz"), names=np.array(names), q=q.numpy())
+    print("base_agent.npz: Q", tuple(q.shape))
+
+
+def gen_run_learner_imports():
+    """The import statements of the reference's run_learner.py, per ALG branch (module, name), as data."""
+    import ast
+    import json
+    from oracle import ref_harness as H
+
+    tree = ast.parse(open(os.path.join(H.REFERENCE_ROOT, "run_learner.py")).read())
+    out = {"top": [], "branches": {}}
+    for node in tree.body:
+        if isinstance(node, ast.ImportFrom):
+            out["top"] += [[node.module, a.name] for a in node.names]
+        elif isinstance(node, ast.If) and getattr(node.test, "left", None) and getattr(node.test.left, "id", "") == "ALG":
+            while isinstance(node, ast.If):
+                alg = node.test.comparators[0].value
+                out["branches"][alg] = [[n.module, a.name] for n in node.body if isinstance(n, ast.ImportFrom)
+                                        for a in n.names]
+                node = node.orelse[0] if len(node.orelse) == 1 else None
+    with open(os.path.join(HERE, "run_learner_imports.json"), "w") as f:
+        json.dump(out, f)
+        f.write("\n")
+    print("run_learner_imports.json:", out)
+
+
 GROUPS = {"tree": gen_tree, "apex": gen_apex, "r2d2": gen_r2d2, "impala": gen_impala, "apex_e2e": gen_apex_e2e,
-          "r2d2_e2e": gen_r2d2_e2e, "impala_e2e": gen_impala_e2e}
+          "r2d2_e2e": gen_r2d2_e2e, "impala_e2e": gen_impala_e2e, "base_agent": gen_base_agent,
+          "run_learner_imports": gen_run_learner_imports}
 
 if __name__ == "__main__":
     want = sys.argv[1:] or list(GROUPS)

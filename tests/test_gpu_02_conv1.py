@@ -1,4 +1,4 @@
-"""Fused gather + conv_1 (tcgen05, kind::i8 with 4-digit weight split) against an fp64
+"""Fused gather + conv_1 (wgmma u8 x s8 with 4-digit weight split) against an fp64
 convolution of the same inputs (torch CPU).  Floating-point kernel -> tolerance, stated
 per assert; the contract is 1e-5."""
 import numpy as np

@@ -1,4 +1,4 @@
-"""3xTF32 dense layer (csrc/gemm.cu, tcgen05 kind::tf32) against an fp64 matmul of the same inputs.
+"""3xTF32 dense layer (csrc/gemm.cu, wgmma tf32) against an fp64 matmul of the same inputs.
 Floating-point kernel -> tolerance, stated per assert: the error must be of the order of an fp32
 FMA chain (the cuBLAS fp32 SIMT GEMM the reference's nn.Linear runs as), far below plain TF32."""
 import pytest
@@ -170,27 +170,3 @@ def test_relu_flatten_folded_into_the_packs_matches_fp64(L):
     assert _rel(torch.cat([w1.grad, w2.grad]), wd.grad) < 5e-6
     assert (y.grad[y.detach() <= 0] == 0).all()                  # ReLU mask applied
 
-
-def test_cta_pair_variant_matches_fp64():
-    """B2RL_GEMM_2CTA=1 selects k_gemm_tf32x3_2cta (tcgen05 cta_group::2: one M=256 MMA per step over two SMs, each
-    holding half of the B tile).  Same numerics as the single-CTA kernel; run in a subprocess because the switch is
-    read once per process."""
-    import os, subprocess, sys, textwrap
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    repo = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    code = textwrap.dedent("""
-        import torch
-        from distributed_rl_b200 import linear as L
-        g = torch.Generator(device="cuda").manual_seed(5)
-        for M, N, K in ((512, 1024, 3136), (1024, 3136, 512), (256, 300, 100)):
-            x = torch.randn(M, K, device="cuda", generator=g); w = torch.randn(N, K, device="cuda", generator=g) * 0.05
-            ref = x.double() @ w.double().T
-            y = L.linear3x(x, w)
-            e = ((y.double() - ref).abs().max() / ref.abs().max()).item()
-            assert e < 5e-6, (M, N, K, e)
-        print("2CTA_OK")
-    """)
-    r = subprocess.run([sys.executable, "-c", code], cwd=repo, env=dict(os.environ, B2RL_GEMM_2CTA="1", PYTHONPATH=repo),
-                       capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0 and "2CTA_OK" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]

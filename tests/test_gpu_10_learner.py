@@ -243,7 +243,7 @@ def _first_step_gradients(apex, fused, B=64, N=8192, **kw):
 
 
 def test_fused_conv1_gradients_equal_staged_gradients(apex):
-    """The benchmarked path (tcgen05 gather+conv_1 forward and weight gradient, 3xTF32 heads, fused dueling tail,
+    """The benchmarked path (wgmma gather+conv_1 forward and weight gradient, 3xTF32 heads, fused dueling tail,
     weight gradients on the side stream) against the staged path (gathered uint8 batch -> fp32 -> cuDNN fp32 conv_1):
     same sampled slots, TD errors / priorities to fp32 noise, and every parameter's GRADIENT equal norm-wise
     (||dg|| / ||g|| <= 2e-5).  Gradients, not post-RMSprop weights: the centred RMSprop step is ~lr*sign(g)/0.22
@@ -364,7 +364,7 @@ def test_learner_train_end_to_end_vs_reference_golden(apex, golden, fused):
     """The whole reference Learner.train (run on the CPU by tests/golden/make_golden.py: 3 forwards,
     double-DQN target, clipped TD, priority, IS-weighted loss, backward, centered RMSprop) against
     distributed_rl_b200.apex.Learner.train on the GPU with the same seeded weights and minibatch.
-    `fused` routes conv_1 through the tcgen05 kernel via an in-replay batch and fused_step."""
+    `fused` routes conv_1 through the wgmma kernel via an in-replay batch and fused_step."""
     import sys, os
     sys.path.insert(0, os.path.join(os.path.dirname(__file__), "golden"))
     from make_golden import seeded_weights
