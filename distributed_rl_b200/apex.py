@@ -20,7 +20,6 @@ What changed relative to the reference, and why it is still a drop-in:
 from __future__ import annotations
 
 import pickle
-import threading
 import time
 from dataclasses import dataclass, field
 
@@ -29,6 +28,8 @@ import torch
 
 from . import replay as R
 from .agent import GraphAgent
+from .learner_common import (Conv1Gathered as _Conv1Gathered, MemoryView, ReplayThread, TargetNetLearner, conv1_packs,
+                             make_optimizer)
 
 
 @dataclass
@@ -88,54 +89,13 @@ def default_apex_model() -> dict:
     }
 
 
-def make_optimizer(info: dict, params, capturable: bool = True):
-    """baseline/utils.py getOptim (:78-132) for the optimisers the shipped configs name."""
-    name = info["name"]
-    lr, decay, eps = info["lr"], info.get("decay", 0), info.get("eps", 1e-5)
-    if name == "rmsprop":
-        return torch.optim.RMSprop(params, lr=lr, weight_decay=decay, eps=eps, momentum=info.get("momentum", 0),
-                                   alpha=info.get("alpha", 0.99), centered=info.get("centered", False),
-                                   capturable=capturable, foreach=True)
-    if name == "adam":
-        return torch.optim.Adam(params, lr=lr, weight_decay=decay, eps=eps,
-                                betas=(info.get("beta1", 0.9), info.get("beta2", 0.99)),
-                                capturable=capturable, foreach=True)
-    if name == "sgd":
-        return torch.optim.SGD(params, lr=lr, weight_decay=decay, momentum=info.get("momentum", 0))
-    raise ValueError(f"unknown optimizer {name!r}")
-
-
-class _MemoryView:
-    """What the learner reads from `Replay.memory` (APE_X/Learner.py:143,241):
-    len() and .max_weight (baseline/PER.py:80-81,129-133)."""
-
-    def __init__(self, dev_replay: R.DeviceReplay, beta: float):
-        self._r, self._beta = dev_replay, beta
-
-    def __len__(self):
-        return len(self._r)
-
-    @property
-    def max_weight(self) -> float:
-        return float(self._r.stats(self._beta)[2].item())
-
-
-class Replay(threading.Thread):
+class Replay(ReplayThread):
     """APE_X/ReplayMemory.py Replay (:19-167): same methods and attributes."""
 
     def __init__(self, cfg: ApexConfig | None = None, connect=None):
-        super().__init__(daemon=True)
-        self.cfg = cfg or ApexConfig.from_configuration()
-        self.device = torch.device(self.cfg.LEARNER_DEVICE)
+        super().__init__(cfg or ApexConfig.from_configuration(), connect)
         self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, R.APEX_FIELDS, self.device)
-        self.memory = _MemoryView(self.store, self.cfg.BETA)
-        self.connect = connect
-        self.cond = False
-        self.lock = False          # eviction handshake flag: kept for API compatibility, unused
-        self.deque = []            # pre-assembled minibatches (filled on demand)
-        self.total_frame = 0
-        self._lock = threading.Lock()
-        self._stop_evt = threading.Event()     # NOT `_stop`: that name is threading.Thread's own method
+        self.memory = MemoryView(self.store, self.cfg.BETA)
 
     # -- ingest: records are [s, a, R_n, s', done, prio] pickled by the actors ----
     def push_records(self, blobs) -> None:
@@ -195,10 +155,6 @@ class Replay(threading.Thread):
             self.store.push_commit(p)
         self.total_frame += int(torch.as_tensor(p).numel())
 
-    def stop(self) -> None:
-        """Ask the ingest thread to leave its loop (the reference's daemon thread can only die with the process)."""
-        self._stop_evt.set()
-
     def ingest(self, s, ns, a, r, d, p) -> None:
         """Steady-state ingest, one call per learner iteration (b2rl_replay_ingest_pipelined): the batch handed
         over by the previous call becomes sampleable, this one's host->device copy starts on the library's copy
@@ -206,34 +162,6 @@ class Replay(threading.Thread):
         with self._lock:
             self.store.ingest_pipelined([s, ns, a, r, d], p)
         self.total_frame += int(p.numel())
-
-    def run(self):
-        """Poll the actors' Redis list like APE_X/ReplayMemory.py:118-161: drain `experience`, push, honour the
-        learner's eviction request (`lock`, :151-160).  Minibatches are assembled on demand by sample()."""
-        if self.connect is None:
-            return
-        from .wire import drain
-        while not self._stop_evt.is_set():
-            data = drain(self.connect, "experience")
-            if data:
-                self.push_records(data)
-                self.cond = len(self.store) > self.cfg.BUFFER_SIZE
-            if self.lock:
-                self._evict_on_request()
-            if not data:
-                time.sleep(0.002)
-
-    def _evict_on_request(self) -> None:
-        """The `lock` handshake (APE_X/ReplayMemory.py:151-160, APE_X/Learner.py:189-197): once the memory is full,
-        drop queued minibatches and trim to REPLAY_MEMORY_LEN (PER.remove_to_fit, baseline/PER.py:118-127).  The
-        ring already overwrites its oldest slot on push, so there is normally nothing to trim."""
-        if len(self.store) >= self.cfg.REPLAY_MEMORY_LEN:
-            with self._lock:
-                self.deque.clear()
-                over = len(self.store) - self.cfg.REPLAY_MEMORY_LEN
-                if over > 0:
-                    self.store.evict(over)
-        self.lock = False
 
     # -- sampling -------------------------------------------------------------------
     def buffer(self, m: int = 1) -> None:
@@ -247,86 +175,18 @@ class Replay(threading.Thread):
             self.deque.append([batch["state"][sl], batch["action"][sl], batch["reward"][sl],
                                batch["next_state"][sl], batch["done"][sl], w[sl], idx[sl]])
 
-    def sample(self):
-        if len(self.deque) == 0:
-            if len(self.store) <= self.cfg.BUFFER_SIZE:
-                return False
-            self.buffer(1)
-        return self.deque.pop(0)
-
-    # -- priority write-back ----------------------------------------------------------
-    def update(self, idx, vals) -> None:
-        """Replay.update (:43-47) + _update (:49-59) -> PER.update: applied at once."""
-        if isinstance(idx, (list, tuple)):
-            idx = torch.stack([torch.as_tensor(i) for i in idx]) if len(idx) and torch.is_tensor(idx[0]) \
-                else torch.as_tensor(np.asarray(idx, np.int64))
-        vals = torch.as_tensor(vals)
-        with self._lock:
-            self.store.update(idx.to(self.device), vals.to(self.device))
-
     def _update(self):
         """Replay._update (:49-59) applies the pending write-backs; here update() has already enqueued them on
         the stream, so all that is left is to make them visible to the host."""
         torch.cuda.current_stream(self.device).synchronize()
 
 
-class _Conv1Gathered(torch.autograd.Function):
-    """conv_1 over rows `idx` of a uint8 frame table (a replay field or an explicit batch).
-    Forward: fused gather+conv on the tensor cores (or a precomputed output of the same kernel).
-    Backward: only dL/dW is needed (the input is data); cuDNN computes it from a gathered fp32
-    copy of the same rows — the one place the sampled frames are staged — or, with `fused_wgrad`
-    (default), libb2rl's fused gather + wgrad kernel computes it from the uint8 rows directly."""
-
-    fused_wgrad = True
-
-    @staticmethod
-    def forward(ctx, weight, frames, idx, pack, mem_format, store=None, y_pre=None, relu=False):
-        """relu=True: the kernel's epilogue applies the ReLU that follows conv_1 and backward applies its mask
-        inside the wgrad kernel (the caller must then skip the network's own ReLU: forward_from_conv1(y, True))."""
-        ctx.frames, ctx.store, ctx.mem_format, ctx.wshape = frames, store, mem_format, weight.shape
-        ctx.weight_param = weight
-        ctx.has_idx, ctx.relu = idx is not None, bool(relu)
-        idx_t = idx if idx is not None else torch.empty(0, dtype=torch.int64, device=frames.device)
-        if y_pre is not None:
-            y = y_pre.view_as(y_pre)
-        else:
-            y = R.conv1_fused(frames, idx, pack, relu=bool(relu))[0]
-        if relu:
-            ctx.save_for_backward(idx_t, y)
-        else:
-            ctx.save_for_backward(idx_t)
-        return y
-
-    @staticmethod
-    def backward(ctx, gy):
-        idx = ctx.saved_tensors[0]
-        y = ctx.saved_tensors[1] if ctx.relu else None
-        if _Conv1Gathered.fused_wgrad:
-            # fused gather + wgrad on the tensor cores: the sampled rows are never staged (csrc/conv1_wgrad.cu)
-            w = ctx.weight_param
-            from . import linear as _lin
-            if _lin._SINK is not None and w.grad is not None and w.grad.is_contiguous():
-                # deferred-gradient mode (grads pre-allocated, zeroed by the optimizer): the kernel's reduction adds
-                # straight into .grad — no temporary, no AccumulateGrad launch at the very end of backward
-                R.conv1_wgrad(ctx.frames, idx if ctx.has_idx else None, gy, out=w.grad, accumulate=True, relu_y=y)
-                return (None,) * len(ctx.needs_input_grad)
-            gw = R.conv1_wgrad(ctx.frames, idx if ctx.has_idx else None, gy, relu_y=y)
-            return (gw,) + (None,) * (len(ctx.needs_input_grad) - 1)
-        if y is not None:
-            gy = gy * (y > 0)
-        if not ctx.has_idx:
-            x = ctx.frames
-        elif ctx.store is not None:    # TMA bulk gather straight from the replay payload
-            x = ctx.store.gather(idx, ctx.store.alloc_batch(idx.numel(), ("state",)))["state"]
-        else:
-            x = ctx.frames.index_select(0, idx)
-        xf = (x.to(torch.float32) / 255.0).contiguous(memory_format=ctx.mem_format)
-        gw = torch.nn.grad.conv2d_weight(xf, ctx.wshape, gy.contiguous(memory_format=ctx.mem_format), stride=4)
-        return (gw,) + (None,) * (len(ctx.needs_input_grad) - 1)
-
-
-class Learner:
+class Learner(TargetNetLearner):
     """APE_X/Learner.py Learner (:20-272): train / step / run / state_dict."""
+
+    LOG_LINE = ("step:{step} // mean_value:{mean_value:.3f} // norm: {norm:.3f} // REWARD:{reward:.3f} // "
+                "NUM_MEMORY:{num_memory} // Mean_Weight:{mean_weight:.3f} // MAX_WEIGHT:{max_weight:.3f} // "
+                "TIME:{time_per_step:.5f} // loss:{loss:.5f}")
 
     def __init__(self, cfg: ApexConfig | None = None, connect=None, start_replay: bool = True,
                  writer=None):
@@ -458,10 +318,8 @@ class Learner:
         if not self.cfg.FUSED_CONV1 or self.model.first_conv_node() is None:
             return False
         if not hasattr(self, "_pack2"):
-            self._conv_name = self.model.first_conv_node()
-            c_out = getattr(self.model, self._conv_name).conv_1.out_channels
-            self._pack1 = R.Conv1Pack(1, self.device, c_out)     # online net (grad pass on s)
-            self._pack2 = R.Conv1Pack(2, self.device, c_out)     # online + target in one pass over s'
+            # _pack1: online net (grad pass on s); _pack2: online + target in one pass over s'
+            self._conv_name, self._pack1, self._pack2 = conv1_packs(self.model, self.device, 1, 2)
         return True
 
     def _streams(self):
@@ -737,36 +595,14 @@ class Learner:
         g.replay()
         return self._static
 
-    # -- parameter publication / main loop -------------------------------------------------
-    @property
-    def state_dict(self):
-        return {k: v.cpu() for k, v in self.model.state_dict().items()}
-
-    @property
-    def target_state_dict(self):
-        return {k: v.cpu() for k, v in self.target_model.state_dict().items()}
-
+    # -- main loop ---------------------------------------------------------------------------------
     def run(self, max_steps: int | None = None, log_every: int = 500):
         """Learner.run (:140-262) with the reference's cadence: wait for BUFFER_SIZE records, announce `Start`,
         hard target sync every TARGET_FREQUENCY steps, parameter publication every 50, and every `log_every`
         (500) steps the eviction request (`memory.lock`, :189-191), the `reward` drain + log line (:219-253) and a
         checkpoint of the online weights (:256-262).  Publication and checkpoints go through ParamPublisher
         (async D2H into pinned memory), so none of them stalls the learner stream."""
-        from .publish import ParamPublisher
-        from . import wire
-        while len(self.memory.memory) <= self.cfg.BUFFER_SIZE:
-            time.sleep(0.05)
-        if self.connect is not None:
-            self.connect.set("state_dict", pickle.dumps(self.state_dict))
-            self.connect.set("count", pickle.dumps(1))
-            self.connect.set("target_state_dict", pickle.dumps(self.target_state_dict))
-            self.connect.set("Start", pickle.dumps(True))
-        pub = ParamPublisher(self.model, self.connect, "state_dict", "count")
-        pub_t = ParamPublisher(self.target_model, self.connect, "target_state_dict", None)
-        ckpt_path = wire.checkpoint_path(self.cfg.LOG_W)
-        ckpt = ParamPublisher(self.model, None, None, None,
-                              on_ready=lambda sd, step: torch.save(sd, ckpt_path)) if ckpt_path else None
-        self._publishers = (pub, pub_t) + ((ckpt,) if ckpt else ())
+        pub, pub_t, ckpt = self._start()
         step = 0
         t0 = time.time()
         acc = None
@@ -787,20 +623,7 @@ class Learner:
                 self.memory.lock = True              # :189-191 eviction request, served by the ingest thread
                 if self.connect is None or not self.memory.is_alive():
                     self.memory._evict_on_request()
-                reward, n_rew = wire.drain_rewards(self.connect) if self.connect is not None else (-21.0, 0)
                 loss, mean_value, mean_w, norm = (acc / log_every).tolist()
-                dt = (time.time() - t0) / log_every
-                self.last_log = {"step": step, "mean_value": mean_value, "norm": norm, "reward": reward,
-                                 "loss": loss, "mean_weight": mean_w, "time_per_step": dt}
-                print(f"step:{step} // mean_value:{mean_value:.3f} // norm: {norm:.3f} // REWARD:{reward:.3f} // "
-                      f"NUM_MEMORY:{len(self.memory.memory)} // Mean_Weight:{mean_w:.3f} // "
-                      f"MAX_WEIGHT:{self.memory.memory.max_weight:.3f} // TIME:{dt:.5f} // loss:{loss:.5f}")
-                if self.writer is not None:
-                    if n_rew:
-                        self.writer.add_scalar("Reward", reward, step)
-                    self.writer.add_scalar("value", mean_value, step)
-                    self.writer.add_scalar("norm", norm, step)
-                if ckpt is not None:
-                    ckpt.snapshot(step)
+                self._log(step, log_every, t0, ckpt, mean_value, norm, loss=loss, mean_weight=mean_w)
                 acc, t0 = None, time.time()
         return step

@@ -6,14 +6,14 @@ baseline/utils.py ReplayMemory.sample (:310-315); the V-trace backward scan
 launch of b2rl_vtrace."""
 from __future__ import annotations
 
-import threading
 from dataclasses import dataclass, field
 
 import torch
 
 from . import replay as R
 from .agent import GraphAgent
-from .apex import make_optimizer, _Conv1Gathered
+from .learner_common import Conv1Gathered, ReplayThread, conv1_packs, make_optimizer, publishers, time_major_rows
+from .publish import ParamPublisher
 
 
 def default_impala_model() -> dict:
@@ -55,18 +55,15 @@ class ImpalaConfig:
         return ImpalaConfig(LOG_W=getattr(C, "LOG_W", None), **{k: getattr(C, k) for k in names})
 
 
-class Replay(threading.Thread):
-    """IMPALA/ReplayMemory.py Replay: batch = (s[T+1,B,28224], a[T,B], mu[T,B], r[T,B], done[B])."""
+class Replay(ReplayThread):
+    """IMPALA/ReplayMemory.py Replay: batch = (s[T+1,B,28224], a[T,B], mu[T,B], r[T,B], done[B]).  run() drains
+    `trajectory` (IMPALA/ReplayMemory.py:56-76); the learner never requests an eviction."""
+
+    LIST_KEY = "trajectory"
 
     def __init__(self, cfg: ImpalaConfig | None = None, connect=None):
-        super().__init__(daemon=True)
-        self.cfg = cfg or ImpalaConfig.from_configuration()
-        self.device = torch.device(self.cfg.LEARNER_DEVICE)
+        super().__init__(cfg or ImpalaConfig.from_configuration(), connect)
         self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, R.impala_fields(self.cfg.UNROLL_STEP), self.device)
-        self.deque = []
-        self._connect = connect
-        self._lock = threading.Lock()
-        self._stop_evt = threading.Event()
         self._rng = torch.Generator(device=self.device)        # uniform sampling stream (random.sample in the reference)
         self._rng.manual_seed(0x1A9A1A)
 
@@ -84,22 +81,6 @@ class Replay(threading.Thread):
         from .wire import decode_impala
         self.push_arrays(*decode_impala([pickle.loads(b) for b in blobs], self.cfg.UNROLL_STEP))
 
-    def stop(self) -> None:
-        self._stop_evt.set()
-
-    def run(self):
-        """IMPALA/ReplayMemory.py:56-76: drain `trajectory`, push.  Batches are assembled on demand."""
-        if self._connect is None:
-            return
-        import time
-        from .wire import drain
-        while not self._stop_evt.is_set():
-            data = drain(self._connect, "trajectory")
-            if data:
-                self.push_records(data)
-            else:
-                time.sleep(0.002)
-
     def bufferSave(self, m: int = 1):
         """IMPALA/ReplayMemory.py:30-54 with random.sample's no-replacement semantics."""
         B = self.cfg.BATCHSIZE
@@ -111,6 +92,8 @@ class Replay(threading.Thread):
             self.deque.append((b["state"][sl].transpose(0, 1).contiguous(), b["action"][sl].t().contiguous(),
                                b["mu"][sl].t().contiguous(), b["reward"][sl].t().contiguous(), b["done"][sl]))
 
+    buffer = bufferSave         # what ReplayThread.sample() calls
+
     def draw(self, n: int) -> torch.Tensor:
         """n distinct slots, uniformly (random.sample over the list of kept rollouts, baseline/utils.py:310-315).
         The kept rollouts are the ring's valid region [head - size, head): slots reserved for an ingest in flight
@@ -121,13 +104,6 @@ class Replay(threading.Thread):
         k = torch.randperm(size, device=self.device, generator=self._rng)[:n]
         tail = (head - size) % cap
         return (k + tail) % cap if tail else k
-
-    def sample(self):
-        if not self.deque:
-            if len(self.store) <= self.cfg.BUFFER_SIZE:
-                return False
-            self.bufferSave(1)
-        return self.deque.pop(0)
 
     def __len__(self):
         return len(self.store)
@@ -181,7 +157,7 @@ class Learner:
             self._t_idx = torch.arange(T + 1, device=self.device).view(T + 1, 1)
         idx = mem.draw(B)
         b = st.gather(idx, self._small)
-        rows = (idx.view(1, B) * (T + 1) + self._t_idx).reshape(-1).contiguous()
+        rows = time_major_rows(idx, self._t_idx)
         self._train_core(self._frames, rows, b["action"].t().contiguous(), b["mu"].t().contiguous(),
                          b["reward"].t().contiguous(), b["done"], step)
         return self.last
@@ -197,8 +173,7 @@ class Learner:
             if fused:
                 # one launch: conv_1 of all (T+1)*B frame stacks, uint8 -> /255 folded in, no fp32 staging
                 if not hasattr(self, "_pack1"):
-                    self._conv_name = self.model.first_conv_node()
-                    self._pack1 = R.Conv1Pack(1, dev, getattr(self.model, self._conv_name).conv_1.out_channels)
+                    self._conv_name, self._pack1 = conv1_packs(self.model, dev, 1)
                 w1 = getattr(self.model, self._conv_name).conv_1.weight
                 self._pack1.pack(0, w1)
                 y_all = R.conv1_fused(frames, rows, self._pack1, relu=False)[0]
@@ -221,7 +196,7 @@ class Learner:
         if fused:
             seq_frames = frames[:T * B] if rows is None else frames
             seq_rows = None if rows is None else rows[:T * B]
-            y = _Conv1Gathered.apply(w1, seq_frames, seq_rows, self._pack1, torch.contiguous_format, None, y_seq)
+            y = Conv1Gathered.apply(w1, seq_frames, seq_rows, self._pack1, torch.contiguous_format, None, y_seq)
             out = self.model.forward_from_conv1(y, False)[0]
         else:
             out = self.model.forward([seq])[0]
@@ -250,15 +225,10 @@ class Learner:
         the weights are snapshot on the learner stream and SET once their D2H copy has landed; if the previous
         snapshot is still in flight this step's is skipped (the actors poll every 400 env steps anyway)."""
         import time
-        from . import wire
-        from .publish import ParamPublisher
         while len(self._memory) <= self.cfg.BUFFER_SIZE:
             time.sleep(0.05)
         pub = ParamPublisher(self.model, self._connect, "params", "Count", wrap=lambda sd: (sd,))
-        ckpt_path = wire.checkpoint_path(self.cfg.LOG_W)
-        ckpt = ParamPublisher(self.model, None, None, None,
-                              on_ready=lambda sd, step: torch.save(sd, ckpt_path)) if ckpt_path else None
-        self._publishers = (pub,) + ((ckpt,) if ckpt else ())
+        self._publishers, ckpt = publishers(self.model, self.cfg.LOG_W, pub)
         t = 0
         while max_steps is None or t < max_steps:
             tr = self._memory.sample()

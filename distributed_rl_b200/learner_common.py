@@ -1,0 +1,255 @@
+"""What the Ape-X, R2D2 and IMPALA learner sides share: the optimiser factory, the replay ingest thread, the
+conv_1 autograd function and its packs, the time-major frame-row layout, and the Redis-facing pieces of
+`Learner.run` (start handshake, publishers, periodic log).  Each learner keeps its own store layout, batch
+assembly and loop body."""
+from __future__ import annotations
+
+import pickle
+import threading
+import time
+
+import numpy as np
+import torch
+
+from . import replay as R
+from . import wire
+from .publish import ParamPublisher
+
+
+def make_optimizer(info: dict, params, capturable: bool = True):
+    """baseline/utils.py getOptim (:78-132) for the optimisers the shipped configs name."""
+    name = info["name"]
+    lr, decay, eps = info["lr"], info.get("decay", 0), info.get("eps", 1e-5)
+    if name == "rmsprop":
+        return torch.optim.RMSprop(params, lr=lr, weight_decay=decay, eps=eps, momentum=info.get("momentum", 0),
+                                   alpha=info.get("alpha", 0.99), centered=info.get("centered", False),
+                                   capturable=capturable, foreach=True)
+    if name == "adam":
+        return torch.optim.Adam(params, lr=lr, weight_decay=decay, eps=eps,
+                                betas=(info.get("beta1", 0.9), info.get("beta2", 0.99)),
+                                capturable=capturable, foreach=True)
+    if name == "sgd":
+        return torch.optim.SGD(params, lr=lr, weight_decay=decay, momentum=info.get("momentum", 0))
+    raise ValueError(f"unknown optimizer {name!r}")
+
+
+class MemoryView:
+    """What the learner reads from `Replay.memory` (APE_X/Learner.py:143,241):
+    len() and .max_weight (baseline/PER.py:80-81,129-133)."""
+
+    def __init__(self, dev_replay: R.DeviceReplay, beta: float):
+        self._r, self._beta = dev_replay, beta
+
+    def __len__(self):
+        return len(self._r)
+
+    @property
+    def max_weight(self) -> float:
+        return float(self._r.stats(self._beta)[2].item())
+
+
+# -- replay ingest threads ------------------------------------------------------------------------
+class Stoppable:
+    """`stop()` for a polling loop (the reference's daemon threads can only die with the process).  The event is
+    `_stop_evt`, NOT `_stop`: that name is threading.Thread's own method."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self._stop_evt = threading.Event()
+
+    def stop(self) -> None:
+        """Ask the loop to leave."""
+        self._stop_evt.set()
+
+
+class ReplayThread(Stoppable, threading.Thread):
+    """The `Replay` thread of APE_X/ReplayMemory.py (:19-167), R2D2/ReplayMemory.py and IMPALA/ReplayMemory.py.
+    A subclass sets `self.store` (the DeviceReplay the sum-tree lives in) and provides `push_records(blobs)` and
+    `buffer(m)`, which appends m assembled minibatches to `deque`."""
+
+    LIST_KEY = "experience"     # the actors' Redis list drained by run()
+
+    def __init__(self, cfg, connect=None):
+        super().__init__(daemon=True)
+        self.cfg = cfg
+        self.device = torch.device(cfg.LEARNER_DEVICE)
+        self.connect = connect
+        self.cond = False
+        self.lock = False          # eviction request from the learner, served by run()
+        self.deque = []            # pre-assembled minibatches (filled on demand)
+        self.total_frame = 0
+        self._lock = threading.Lock()
+
+    def run(self):
+        """Poll the actors' Redis list like APE_X/ReplayMemory.py:118-161: drain `LIST_KEY`, push, honour the
+        learner's eviction request (`lock`, :151-160).  Minibatches are assembled on demand by sample()."""
+        if self.connect is None:
+            return
+        while not self._stop_evt.is_set():
+            data = wire.drain(self.connect, self.LIST_KEY)
+            if data:
+                self.push_records(data)
+                self.cond = len(self.store) > self.cfg.BUFFER_SIZE
+            if self.lock:
+                self._evict_on_request()
+            if not data:
+                time.sleep(0.002)
+
+    def _evict_on_request(self) -> None:
+        """The `lock` handshake (APE_X/ReplayMemory.py:151-160, APE_X/Learner.py:189-197): once the memory is full,
+        drop queued minibatches and trim to REPLAY_MEMORY_LEN (PER.remove_to_fit, baseline/PER.py:118-127).  The
+        ring already overwrites its oldest slot on push, so there is normally nothing to trim."""
+        if len(self.store) >= self.cfg.REPLAY_MEMORY_LEN:
+            with self._lock:
+                self.deque.clear()
+                over = len(self.store) - self.cfg.REPLAY_MEMORY_LEN
+                if over > 0:
+                    self.store.evict(over)
+        self.lock = False
+
+    def sample(self):
+        """The next queued minibatch, assembling one if none is queued; False until more than BUFFER_SIZE records
+        are stored."""
+        if not self.deque:
+            if len(self.store) <= self.cfg.BUFFER_SIZE:
+                return False
+            self.buffer(1)
+        return self.deque.pop(0)
+
+    def update(self, idx, vals) -> None:
+        """Replay.update (APE_X/ReplayMemory.py:43-59) -> PER.update, applied at once.  `idx`: a tensor, an array, or
+        a list of ints or 0-d tensors (what the reference passes)."""
+        if isinstance(idx, (list, tuple)):
+            idx = torch.stack([torch.as_tensor(i) for i in idx]) if len(idx) and torch.is_tensor(idx[0]) \
+                else torch.as_tensor(np.asarray(idx, np.int64))
+        with self._lock:
+            self.store.update(torch.as_tensor(idx).to(self.device), torch.as_tensor(vals).to(self.device))
+
+
+# -- conv_1 on libb2rl's kernels -----------------------------------------------------------------
+class Conv1Gathered(torch.autograd.Function):
+    """conv_1 over rows `idx` of a uint8 frame table (a replay field or an explicit batch).
+    Forward: fused gather+conv on the tensor cores (or a precomputed output of the same kernel).
+    Backward: only dL/dW is needed (the input is data); cuDNN computes it from a gathered fp32
+    copy of the same rows — the one place the sampled frames are staged — or, with `fused_wgrad`
+    (default), libb2rl's fused gather + wgrad kernel computes it from the uint8 rows directly."""
+
+    fused_wgrad = True
+
+    @staticmethod
+    def forward(ctx, weight, frames, idx, pack, mem_format, store=None, y_pre=None, relu=False):
+        """relu=True: the kernel's epilogue applies the ReLU that follows conv_1 and backward applies its mask
+        inside the wgrad kernel (the caller must then skip the network's own ReLU: forward_from_conv1(y, True))."""
+        ctx.frames, ctx.store, ctx.mem_format, ctx.wshape = frames, store, mem_format, weight.shape
+        ctx.weight_param = weight
+        ctx.has_idx, ctx.relu = idx is not None, bool(relu)
+        idx_t = idx if idx is not None else torch.empty(0, dtype=torch.int64, device=frames.device)
+        if y_pre is not None:
+            y = y_pre.view_as(y_pre)
+        else:
+            y = R.conv1_fused(frames, idx, pack, relu=bool(relu))[0]
+        if relu:
+            ctx.save_for_backward(idx_t, y)
+        else:
+            ctx.save_for_backward(idx_t)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        idx = ctx.saved_tensors[0]
+        y = ctx.saved_tensors[1] if ctx.relu else None
+        if Conv1Gathered.fused_wgrad:
+            # fused gather + wgrad on the tensor cores: the sampled rows are never staged (csrc/conv1_wgrad.cu)
+            w = ctx.weight_param
+            from . import linear as _lin
+            if _lin._SINK is not None and w.grad is not None and w.grad.is_contiguous():
+                # deferred-gradient mode (grads pre-allocated, zeroed by the optimizer): the kernel's reduction adds
+                # straight into .grad — no temporary, no AccumulateGrad launch at the very end of backward
+                R.conv1_wgrad(ctx.frames, idx if ctx.has_idx else None, gy, out=w.grad, accumulate=True, relu_y=y)
+                return (None,) * len(ctx.needs_input_grad)
+            gw = R.conv1_wgrad(ctx.frames, idx if ctx.has_idx else None, gy, relu_y=y)
+            return (gw,) + (None,) * (len(ctx.needs_input_grad) - 1)
+        if y is not None:
+            gy = gy * (y > 0)
+        if not ctx.has_idx:
+            x = ctx.frames
+        elif ctx.store is not None:    # TMA bulk gather straight from the replay payload
+            x = ctx.store.gather(idx, ctx.store.alloc_batch(idx.numel(), ("state",)))["state"]
+        else:
+            x = ctx.frames.index_select(0, idx)
+        xf = (x.to(torch.float32) / 255.0).contiguous(memory_format=ctx.mem_format)
+        gw = torch.nn.grad.conv2d_weight(xf, ctx.wshape, gy.contiguous(memory_format=ctx.mem_format), stride=4)
+        return (gw,) + (None,) * (len(ctx.needs_input_grad) - 1)
+
+
+def conv1_packs(model, device, *n_nets):
+    """-> (name of `model`'s first conv node, one Conv1Pack per entry of `n_nets`): each pack holds the conv_1
+    weights of that many networks (1: online; 2: online + target, run as one launch)."""
+    name = model.first_conv_node()
+    c_out = getattr(model, name).conv_1.out_channels
+    return (name,) + tuple(R.Conv1Pack(n, device, c_out) for n in n_nets)
+
+
+def time_major_rows(seq_rows: torch.Tensor, t_idx: torch.Tensor) -> torch.Tensor:
+    """Frame-table rows of the (t, b) frames in time-major order, for sequences of T frames stored as T consecutive
+    rows: row = seq_rows[b] * T + t, with t_idx = arange(T).view(T, 1) (kept by the caller: no launch per step)."""
+    return (seq_rows.view(1, -1) * t_idx.shape[0] + t_idx).reshape(-1).contiguous()
+
+
+# -- Learner.run: the Redis-facing edge ----------------------------------------------------------
+def publishers(model, log_w, *pubs):
+    """-> (`pubs` plus, when LOG_W is set, a checkpoint publisher of `model` — the tuple kept as
+    `Learner._publishers` —, that checkpoint publisher or None).  Checkpoints go to ./weight/<ALG>/<time>/weight.pth
+    (APE_X/Learner.py:256-262) once the snapshot's async D2H copy has landed."""
+    path = wire.checkpoint_path(log_w)
+    ckpt = ParamPublisher(model, None, None, None, on_ready=lambda sd, step: torch.save(sd, path)) if path else None
+    return pubs + ((ckpt,) if ckpt else ()), ckpt
+
+
+class TargetNetLearner:
+    """The parts of `Learner` that Ape-X and R2D2 share (online + target network, `Start` handshake, periodic
+    log).  Uses the learner's `cfg`, `model`, `target_model`, `memory`, `connect` and `writer`; `LOG_LINE` is the
+    learner's log line, formatted with `last_log`, `num_memory` and `max_weight`."""
+
+    LOG_LINE: str
+
+    @property
+    def state_dict(self):
+        return {k: v.cpu() for k, v in self.model.state_dict().items()}
+
+    @property
+    def target_state_dict(self):
+        return {k: v.cpu() for k, v in self.target_model.state_dict().items()}
+
+    def _start(self):
+        """Learner.run's set-up (APE_X/Learner.py:140-155, R2D2/Learner.py:217-234): wait for more than BUFFER_SIZE
+        records, publish the initial weights and announce `Start`, then build `_publishers`.
+        -> (parameter publisher, target publisher, checkpoint publisher or None)"""
+        while len(self.memory.memory) <= self.cfg.BUFFER_SIZE:
+            time.sleep(0.05)
+        if self.connect is not None:
+            self.connect.set("state_dict", pickle.dumps(self.state_dict))
+            self.connect.set("count", pickle.dumps(1))
+            self.connect.set("target_state_dict", pickle.dumps(self.target_state_dict))
+            self.connect.set("Start", pickle.dumps(True))
+        pub = ParamPublisher(self.model, self.connect, "state_dict", "count")
+        pub_t = ParamPublisher(self.target_model, self.connect, "target_state_dict", None)
+        self._publishers, ckpt = publishers(self.model, self.cfg.LOG_W, pub, pub_t)
+        return pub, pub_t, ckpt
+
+    def _log(self, step, log_every, t0, ckpt, mean_value, norm, **stats) -> None:
+        """The every-`log_every` tail (APE_X/Learner.py:219-262, R2D2/Learner.py:296-339): drain the actors'
+        `reward` list, set `last_log` (+ `stats`), print LOG_LINE, write the TensorBoard scalars and snapshot a
+        checkpoint (`ckpt`: the checkpoint publisher or None)."""
+        reward, n_rew = wire.drain_rewards(self.connect) if self.connect is not None else (-21.0, 0)
+        self.last_log = {"step": step, "mean_value": mean_value, "norm": norm, "reward": reward, **stats,
+                         "time_per_step": (time.time() - t0) / log_every}
+        mem = self.memory.memory
+        print(self.LOG_LINE.format(num_memory=len(mem), max_weight=mem.max_weight, **self.last_log))
+        if self.writer is not None:
+            if n_rew:
+                self.writer.add_scalar("Reward", reward, step)
+            self.writer.add_scalar("value", mean_value, step)
+            self.writer.add_scalar("norm", norm, step)
+        if ckpt is not None:
+            ckpt.snapshot(step)

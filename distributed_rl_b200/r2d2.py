@@ -10,14 +10,14 @@ is used here, identical whenever the reference runs at all.
 """
 from __future__ import annotations
 
-import threading
 from dataclasses import dataclass, field
 
 import torch
 
 from . import replay as R
 from .agent import GraphAgent
-from .apex import make_optimizer, _MemoryView, _Conv1Gathered
+from .learner_common import (Conv1Gathered, MemoryView, ReplayThread, TargetNetLearner, conv1_packs, make_optimizer,
+                             time_major_rows)
 
 
 def default_r2d2_model() -> dict:
@@ -74,13 +74,12 @@ class R2D2Config:
         return R2D2Config(LOG_W=getattr(C, "LOG_W", None), **{k: getattr(C, k) for k in names})
 
 
-class Replay(threading.Thread):
-    """R2D2/ReplayMemory.py Replay: batch = [(h0, h1), s, a, r, notdone, w, idx] (:118-120)."""
+class Replay(ReplayThread):
+    """R2D2/ReplayMemory.py Replay: batch = [(h0, h1), s, a, r, notdone, w, idx] (:118-120).  The reference's
+    update() is unlocked (:48-51); the device handle needs `_lock`."""
 
     def __init__(self, cfg: R2D2Config | None = None, connect=None):
-        super().__init__(daemon=True)
-        self.cfg = cfg or R2D2Config.from_configuration()
-        self.device = torch.device(self.cfg.LEARNER_DEVICE)
+        super().__init__(cfg or R2D2Config.from_configuration(), connect)
         fields = R.r2d2_fields(self.cfg.FIXED_TRAJECTORY)
         if self.cfg.PAYLOAD_POOL:
             self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, (), self.device)          # priorities only
@@ -88,11 +87,7 @@ class Replay(threading.Thread):
         else:
             self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, fields, self.device)
             self.pool = self.store
-        self.memory = _MemoryView(self.store, self.cfg.BETA)
-        self.connect, self.cond, self.lock = connect, False, False
-        self.deque, self.total_frame = [], 0
-        self._lock = threading.Lock()       # the reference's update() is unlocked (:48-51); the handle needs it
-        self._stop_evt = threading.Event()
+        self.memory = MemoryView(self.store, self.cfg.BETA)
 
     def push_arrays(self, s, a, r, h0, h1, notdone, p):
         with self._lock:
@@ -108,34 +103,6 @@ class Replay(threading.Thread):
         from .wire import decode_r2d2
         cols, p = decode_r2d2([pickle.loads(b) for b in blobs], self.cfg.FIXED_TRAJECTORY)
         self.push_arrays(*cols, p)
-
-    def stop(self) -> None:
-        self._stop_evt.set()
-
-    def run(self):
-        """R2D2/ReplayMemory.py:141-178: drain `experience`, push, serve the eviction request."""
-        if self.connect is None:
-            return
-        import time
-        from .wire import drain
-        while not self._stop_evt.is_set():
-            data = drain(self.connect, "experience")
-            if data:
-                self.push_records(data)
-                self.cond = len(self.store) > self.cfg.BUFFER_SIZE
-            if self.lock:
-                self._evict_on_request()
-            if not data:
-                time.sleep(0.002)
-
-    def _evict_on_request(self) -> None:
-        if len(self.store) >= self.cfg.REPLAY_MEMORY_LEN:       # :165-173
-            with self._lock:
-                self.deque.clear()
-                over = len(self.store) - self.cfg.REPLAY_MEMORY_LEN
-                if over > 0:
-                    self.store.evict(over)
-        self.lock = False
 
     def buffer(self, m: int = 1):
         B = self.cfg.BATCHSIZE
@@ -153,21 +120,11 @@ class Replay(threading.Thread):
         """payload row of each sampled slot (identity unless PAYLOAD_POOL)."""
         return idx % self.cfg.PAYLOAD_POOL if self.cfg.PAYLOAD_POOL else idx
 
-    def sample(self):
-        if not self.deque:
-            if len(self.store) <= self.cfg.BUFFER_SIZE:
-                return False
-            self.buffer(1)
-        return self.deque.pop(0)
 
-    def update(self, idx, vals):
-        if isinstance(idx, (list, tuple)):
-            idx = torch.stack([torch.as_tensor(i) for i in idx])
-        with self._lock:
-            self.store.update(torch.as_tensor(idx).to(self.device), torch.as_tensor(vals).to(self.device))
+class Learner(TargetNetLearner):
+    LOG_LINE = ("step:{step} // mean_value:{mean_value:.3f} // norm: {norm:.3f} // REWARD:{reward:.3f} // "
+                "NUM_MEMORY:{num_memory} // MAX_WEIGHT:{max_weight:.3f} // TIME:{time_per_step:.5f}")
 
-
-class Learner:
     def __init__(self, cfg: R2D2Config | None = None, connect=None, start_replay: bool = True, writer=None):
         self.cfg = cfg or R2D2Config.from_configuration()
         self.device = torch.device(self.cfg.LEARNER_DEVICE)
@@ -229,12 +186,10 @@ class Learner:
     def _time_major_rows(self, seq_rows, T, B):
         """Frame-table rows of the (t, b) frames in time-major order: row = seq_row[b] * T + t
         (seq_rows None: the batch itself is the table, sequence b = rows b*T ... b*T+T-1)."""
-        dev = self.device
         if not hasattr(self, "_t_idx"):
-            self._t_idx = torch.arange(T, device=dev).view(T, 1)
-            self._b_idx = torch.arange(B, device=dev).view(1, B)
-        base = self._b_idx if seq_rows is None else seq_rows.view(1, B)
-        return (base * T + self._t_idx).reshape(-1).contiguous()
+            self._t_idx = torch.arange(T, device=self.device).view(T, 1)
+            self._b_idx = torch.arange(B, device=self.device)
+        return time_major_rows(self._b_idx if seq_rows is None else seq_rows, self._t_idx)
 
     def _forward_fused(self, frames, tm_rows, T, MEM, B, A):
         """The forward passes with conv_1 on the tensor cores, reading `frames` (a uint8 (rows, 4, 84, 84) table:
@@ -242,10 +197,7 @@ class Learner:
         uint8 -> /255 conversion are folded into the kernel's gather (`tm_rows`)."""
         dev = self.device
         if not hasattr(self, "_pack2"):
-            self._conv_name = self.model.first_conv_node()
-            c_out = getattr(self.model, self._conv_name).conv_1.out_channels
-            self._pack2 = R.Conv1Pack(2, dev, c_out)
-            self._pack1 = R.Conv1Pack(1, dev, c_out)
+            self._conv_name, self._pack2, self._pack1 = conv1_packs(self.model, dev, 2, 1)
         w_on = getattr(self.model, self._conv_name).conv_1.weight
         w_tg = getattr(self.target_model, self._conv_name).conv_1.weight
         self._pack2.pack(0, w_on); self._pack2.pack(1, w_tg); self._pack1.pack(0, w_on)
@@ -261,7 +213,7 @@ class Learner:
             y_on_w, y_tg_w = R.conv1_fused(frames, rows_win, self._pack2, relu=False)
         shape = torch.tensor([L, B, -1])
         mf = torch.contiguous_format
-        y = _Conv1Gathered.apply(w_on, frames, rows_win, self._pack1, mf, None, y_on_w)
+        y = Conv1Gathered.apply(w_on, frames, rows_win, self._pack1, mf, None, y_on_w)
         q = self.model.forward_from_conv1(y, False, [shape])[0].view(L, B, A)             # :121
         with torch.no_grad():
             q_target = self.target_model.forward_from_conv1(torch.relu(y_tg_w), True, [shape])[0].view(L, B, A)
@@ -305,36 +257,13 @@ class Learner:
         self.optim.zero_grad(set_to_none=False)
         return {"p_norm": p_norm}
 
-    @property
-    def state_dict(self):
-        return {k: v.cpu() for k, v in self.model.state_dict().items()}
-
-    @property
-    def target_state_dict(self):
-        return {k: v.cpu() for k, v in self.target_model.state_dict().items()}
-
     def run(self, max_steps=None, log_every: int = 500):
         """R2D2/Learner.py:217-339: wait for BUFFER_SIZE sequences, announce `Start`, then per step sample ->
         train -> priority write-back; hard target sync every TARGET_FREQUENCY steps (+ `target_state_dict`),
         `state_dict` / `count` (= step - 50, sic :293) every 25 steps, and every 500 steps the eviction request,
         the `reward` drain + log line and a checkpoint.  Publication is asynchronous (ParamPublisher)."""
-        import pickle
         import time
-        from . import wire
-        from .publish import ParamPublisher
-        while len(self.memory.memory) <= self.cfg.BUFFER_SIZE:
-            time.sleep(0.05)
-        if self.connect is not None:                                     # :227-234
-            self.connect.set("state_dict", pickle.dumps(self.state_dict))
-            self.connect.set("count", pickle.dumps(1))
-            self.connect.set("target_state_dict", pickle.dumps(self.target_state_dict))
-            self.connect.set("Start", pickle.dumps(True))
-        pub = ParamPublisher(self.model, self.connect, "state_dict", "count")
-        pub_t = ParamPublisher(self.target_model, self.connect, "target_state_dict", None)
-        ckpt_path = wire.checkpoint_path(self.cfg.LOG_W)
-        ckpt = ParamPublisher(self.model, None, None, None,
-                              on_ready=lambda sd, step: torch.save(sd, ckpt_path)) if ckpt_path else None
-        self._publishers = (pub, pub_t) + ((ckpt,) if ckpt else ())
+        pub, pub_t, ckpt = self._start()                                # :227-234
         step, acc, t0 = 0, None, time.time()
         self.last_log = None
         while max_steps is None or step < max_steps:
@@ -360,20 +289,7 @@ class Learner:
             for p in self._publishers:
                 p.poll()
             if step % log_every == 0:                                    # :296-339
-                reward, n_rew = wire.drain_rewards(self.connect) if self.connect is not None else (-21.0, 0)
                 mean_value, norm = (acc / log_every).tolist()
-                dt = (time.time() - t0) / log_every
-                self.last_log = {"step": step, "mean_value": mean_value, "norm": norm, "reward": reward,
-                                 "time_per_step": dt}
-                print(f"step:{step} // mean_value:{mean_value:.3f} // norm: {norm:.3f} // REWARD:{reward:.3f} // "
-                      f"NUM_MEMORY:{len(self.memory.memory)} // MAX_WEIGHT:{self.memory.memory.max_weight:.3f} // "
-                      f"TIME:{dt:.5f}")
-                if self.writer is not None:
-                    if n_rew:
-                        self.writer.add_scalar("Reward", reward, step)
-                    self.writer.add_scalar("value", mean_value, step)
-                    self.writer.add_scalar("norm", norm, step)
-                if ckpt is not None:
-                    ckpt.snapshot(step)
+                self._log(step, log_every, t0, ckpt, mean_value, norm)
                 acc, t0 = None, time.time()
         return step

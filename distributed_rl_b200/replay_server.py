@@ -24,10 +24,12 @@ import torch
 
 from . import wire
 from .apex import ApexConfig
+from .learner_common import Stoppable
 
 
-class ReplayServer:
+class ReplayServer(Stoppable):
     def __init__(self, cfg: ApexConfig | None = None, connect=None, connect_push=None, m: int = 32):
+        super().__init__()
         self.cfg = cfg or ApexConfig.from_configuration()
         self.device = torch.device(self.cfg.LEARNER_DEVICE)
         from .apex import Replay
@@ -37,12 +39,8 @@ class ReplayServer:
         self.m = m                               # minibatches assembled per buffer() (the reference: 32, :66)
         self.FLAG_BATCH = self.FLAG_REMOVE = False
         self.total_transition = 0
-        self._stop_evt = threading.Event()
         if self.connect is not None:
             self.connect.set("FLAG_BATCH", pickle.dumps(False))           # :39
-
-    def stop(self) -> None:
-        self._stop_evt.set()
 
     def update(self) -> int:
         """:41-63 — apply the learner's queued priority write-backs."""
@@ -104,7 +102,7 @@ class ReplayServer:
                 time.sleep(0.002)
 
 
-class Replay_Server(threading.Thread):
+class Replay_Server(Stoppable, threading.Thread):
     """Learner-side consumer of a ReplayServer: same surface as `Replay` (sample / update / start / lock)."""
 
     def __init__(self, cfg: ApexConfig | None = None, connect=None, connect_push=None):
@@ -112,12 +110,8 @@ class Replay_Server(threading.Thread):
         self.cfg = cfg or ApexConfig.from_configuration()
         self.connect, self.connect_push = connect, connect_push if connect_push is not None else connect
         self._lock = threading.Lock()
-        self._stop_evt = threading.Event()
         self.deque, self.idx, self.vals = [], [], []
         self.lock = False
-
-    def stop(self) -> None:
-        self._stop_evt.set()
 
     def update(self, idx, vals) -> None:
         """:188-190 — queue; flushed to the server's `update` list beyond 1000 entries."""

@@ -1,6 +1,6 @@
 """Drop-in for the pieces of baseline/utils.py that are on the hot path."""
 from distributed_rl_b200.per import PrioritizedMemory  # noqa: F401
-from distributed_rl_b200.apex import make_optimizer as _mk
+from distributed_rl_b200.learner_common import make_optimizer as _mk
 
 
 def getOptim(optimData, agent, floatV=False):
