@@ -17,6 +17,17 @@ class ReplayDesc(C.Structure):
                 ("field_bytes", c_i64 * MAX_FIELDS)]
 
 
+IPC_HANDLE_BYTES = 64
+
+
+class ServeLayout(C.Structure):
+    """b2rl_serve_layout: byte offsets of the device serve ring (include/b2rl.h)."""
+    _fields_ = [("batch", c_i64), ("slots", c_i64), ("n_fields", c_i64), ("field_bytes", c_i64 * MAX_FIELDS),
+                ("field_off", c_i64 * MAX_FIELDS), ("idx_off", c_i64), ("w_off", c_i64), ("slot_bytes", c_i64),
+                ("upd_idx_off", c_i64), ("upd_prio_off", c_i64), ("upd_slot_bytes", c_i64), ("upd_base", c_i64),
+                ("total_bytes", c_i64)]
+
+
 # name -> (restype, argtypes); must list every symbol include/b2rl.h declares.
 SIGNATURES = {
     "b2rl_last_error": (C.c_char_p, []),
@@ -69,6 +80,17 @@ SIGNATURES = {
     "b2rl_dueling_backward": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b2rl_dueling_backward_w": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp]),
     "b2rl_launch_count": (c_i64, []),
+    "b2rl_serve_layout_init": (C.c_int, [c_i64, c_i32, c_i32, C.POINTER(c_i64), C.POINTER(ServeLayout)]),
+    "b2rl_serve_ring_create": (C.c_int, [c_vp, c_i64, c_i32, C.POINTER(c_vp)]),
+    "b2rl_serve_ring_layout": (C.c_int, [c_vp, C.POINTER(ServeLayout)]),
+    "b2rl_serve_ring_export": (C.c_int, [c_vp, c_vp]),
+    "b2rl_serve_ring_open": (C.c_int, [c_vp, C.POINTER(ServeLayout), c_i32, C.POINTER(c_vp)]),
+    "b2rl_serve_ring_close": (C.c_int, [c_vp]),
+    "b2rl_serve_ring_destroy": (C.c_int, [c_vp]),
+    "b2rl_serve_slot_ptrs": (C.c_int, [c_vp, c_i32, C.POINTER(c_vp), C.POINTER(c_vp)]),
+    "b2rl_serve_fill": (C.c_int, [c_vp, c_vp, c_i32, c_u64, c_f32, c_vp, c_vp]),
+    "b2rl_serve_take": (C.c_int, [c_vp, c_i32, c_vp, c_vp]),
+    "b2rl_serve_put_update": (C.c_int, [c_vp, c_i32, c_u64, c_vp, c_vp, c_i64, c_vp]),
 }
 
 _lib = None

@@ -189,7 +189,11 @@ class Learner(TargetNetLearner):
                 "TIME:{time_per_step:.5f} // loss:{loss:.5f}")
 
     def __init__(self, cfg: ApexConfig | None = None, connect=None, start_replay: bool = True,
-                 writer=None):
+                 writer=None, memory=None):
+        """`memory`: a replay served from another process (replay_server.DeviceReplayClient, or anything with the
+        `Replay` surface: sample / update / lock / memory).  run() then drives sample() -> train() -> update() with
+        the reference's cadence (APE_X/Learner.py:163-197); without it the learner owns its replay and run() steps
+        with fused_step()."""
         self.cfg = cfg or ApexConfig.from_configuration()
         self.device = torch.device(self.cfg.LEARNER_DEVICE)
         if self.cfg.CUDNN_BENCHMARK and self.device.type == "cuda":
@@ -197,13 +201,20 @@ class Learner(TargetNetLearner):
         self.build_model()
         self.build_optim()
         self.connect = connect
-        self.memory = Replay(self.cfg, connect)
-        if start_replay and connect is not None:
-            self.memory.start()
+        self._served = memory is not None
+        if self._served:
+            self.memory = memory
+            if start_replay and not memory.is_alive():
+                memory.start()
+        else:
+            self.memory = Replay(self.cfg, connect)
+            if start_replay and connect is not None:
+                self.memory.start()
         self.writer = writer
         if connect is not None:                  # :41-43 — whatever a previous run left behind is dropped
             from .wire import wipe_stale_keys
-            wipe_stale_keys(connect)
+            # ... except the keys of a replay server this learner is already attached to (its handshake lives there)
+            wipe_stale_keys(connect, keep=getattr(self.memory, "KEEP_KEYS", ()) if self._served else ())
         self.gamma_n = float(np.float32(0.99 ** self.cfg.UNROLL_STEP))  # hard-coded 0.99, :103
         self._graph = None
         self._world = 1
@@ -512,6 +523,8 @@ class Learner(TargetNetLearner):
         if self._graph is not None:
             self._graph.replay()
             return self._static
+        if self._served:
+            raise RuntimeError("fused_step() samples the learner's own replay; a served replay is driven by run()")
         B = self.cfg.BATCHSIZE
         st = self.memory.store
         fused_conv1 = self._conv1_ready()
@@ -608,9 +621,15 @@ class Learner(TargetNetLearner):
         acc = None
         self.last_log = None
         while max_steps is None or step < max_steps:
-            out = self.fused_step()
+            if self._served:
+                tot = self._served_step(step + 1, log_every)
+                if tot is None:
+                    time.sleep(0.002)                # nothing served yet (:166-170)
+                    continue
+            else:
+                out = self.fused_step()
+                tot = torch.cat([out["scalars"], out["p_norm"].reshape(1)])
             step += 1
-            tot = torch.cat([out["scalars"], out["p_norm"].reshape(1)])
             acc = tot.clone() if acc is None else acc + tot
             if step % self.cfg.TARGET_FREQUENCY == 0:
                 self.target_model.updateParameter(self.model, 1)
@@ -620,10 +639,25 @@ class Learner(TargetNetLearner):
             for p in self._publishers:
                 p.poll()
             if step % log_every == 0:
-                self.memory.lock = True              # :189-191 eviction request, served by the ingest thread
-                if self.connect is None or not self.memory.is_alive():
-                    self.memory._evict_on_request()
+                if not self._served:
+                    self.memory.lock = True          # :189-191 eviction request, served by the ingest thread
+                    if self.connect is None or not self.memory.is_alive():
+                        self.memory._evict_on_request()
                 loss, mean_value, mean_w, norm = (acc / log_every).tolist()
                 self._log(step, log_every, t0, ckpt, mean_value, norm, loss=loss, mean_weight=mean_w)
                 acc, t0 = None, time.time()
         return step
+
+    def _served_step(self, step: int, log_every: int):
+        """One iteration of the reference loop over a served replay (APE_X/Learner.py:163-197): sample, train, the
+        eviction request every `log_every` steps (that step's write-back is skipped, as there), write-back.
+        -> {loss, mean(y), mean(w), norm} as a device tensor, or None when no minibatch is ready."""
+        batch = self.memory.sample()
+        if batch is False:
+            return None
+        info, prio, idx, mean_w = self.train(batch)
+        if step % log_every == 0:
+            self.memory.lock = True
+        if self.memory.lock is False:
+            self.memory.update(idx, prio)
+        return torch.stack([info["loss"], info["mean_value"], mean_w, info["p_norm"].reshape(())])

@@ -1,4 +1,4 @@
-// Hopper (sm_90a) primitives shared by the tensor-core kernels (conv1.cu, conv1_wgrad.cu, gemm.cu):
+// Hopper (sm_90a) primitives shared by the tensor-core kernels (conv1.cu, conv1_wgrad.cu, gemm.cu) and serve.cu:
 // mbarriers, TMA bulk copies, and warpgroup MMAs (wgmma) whose operands are read from shared memory
 // through matrix descriptors and whose accumulators live in the registers of the issuing warpgroup.
 #pragma once
@@ -34,6 +34,15 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                    sptr(dst)), "l"(src), "r"(bytes), "r"(sptr(bar)) : "memory");
 }
+__device__ __forceinline__ void bulk_s2g(void* dst, const void* src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(sptr(src)), "r"(bytes)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// all but the newest N committed store groups have finished reading their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 // generic-proxy writes to shared memory -> visible to the tensor core (async proxy)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // named barrier over `threads` threads (id 0 is __syncthreads)

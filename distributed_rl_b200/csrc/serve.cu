@@ -1,0 +1,378 @@
+// Device serve ring of the stand-alone replay server (include/b2rl.h, "Device serve ring"): layout arithmetic,
+// allocation / CUDA IPC export and import, and k_serve_fill — draw + IS weights + scalar fetch + TMA bulk copy of
+// the frame rows of one minibatch into a ring slot in ONE launch.
+//
+// Replaces ReplayServer.buffer's sample -> gather -> .cpu() -> pickle -> RPUSH and Replay_Server.sample's
+// pickle.loads -> host-to-device copy (APE_X/ReplayServer.py:65-114, APE_X/ReplayMemory.py:251-257).
+#include "common.cuh"
+#include "hopper.cuh"
+#include "tree.cuh"
+
+#include <new>
+
+namespace b2rl {
+
+constexpr int SERVE_THREADS = 128;   // draws per CTA at most; warp 0's lane 0 then drives the copy engine
+constexpr int SERVE_CHUNK = 14336;   // as k_gather_bulk's default: half a frame stack per bulk copy
+constexpr int SERVE_STAGES = 16;     // 224 KiB ring of chunks
+constexpr int SERVE_LAG = 3;         // a stage is refilled once all but the newest LAG stores have drained it
+constexpr size_t SERVE_SMEM = (size_t)SERVE_CHUNK * SERVE_STAGES;
+
+struct ServeBulk {
+  const uint8_t* src[B2RL_MAX_FIELDS];   // replay field base
+  uint8_t* dst[B2RL_MAX_FIELDS];         // slot field base
+  int64_t bytes[B2RL_MAX_FIELDS];        // row bytes (multiple of 16)
+  int32_t chunks[B2RL_MAX_FIELDS];       // ceil(bytes / SERVE_CHUNK)
+  int32_t n;
+  int32_t items_per_draw;                // sum of chunks
+};
+
+// Work item t of a CTA (draw-major, then field, then chunk) -> source, destination, size.
+__device__ __forceinline__ void serve_item(const ServeBulk& P, const int64_t* s_row, int64_t k0, int64_t t,
+                                           const uint8_t*& src, uint8_t*& dst, uint32_t& bytes) {
+  const int64_t i = t / P.items_per_draw;
+  int32_t r = (int32_t)(t - i * P.items_per_draw);
+  int f = 0;
+  while (r >= P.chunks[f]) { r -= P.chunks[f]; ++f; }
+  const int64_t off = (int64_t)r * SERVE_CHUNK;
+  const int64_t rem = P.bytes[f] - off;
+  bytes = (uint32_t)(rem < SERVE_CHUNK ? rem : SERVE_CHUNK);
+  src = P.src[f] + s_row[i] * P.bytes[f] + off;
+  dst = P.dst[f] + (k0 + i) * P.bytes[f] + off;
+}
+
+// CTA c owns draws [c*per, (c+1)*per): its threads draw them (indices, weights, scalar fields), then thread 0
+// copies their bulk rows through the shared-memory ring, then the last CTA to finish writes the header.
+__global__ void __launch_bounds__(SERVE_THREADS, 1)
+k_serve_fill(const __grid_constant__ TreeView t, const __grid_constant__ ServeBulk P, SmallFields small,
+             uint64_t* __restrict__ rng_state, int64_t n, int64_t capacity, const float* __restrict__ n_valid_dev,
+             float beta, const float* __restrict__ max_w_ext, int64_t* __restrict__ idx_out,
+             float* __restrict__ w_out, uint64_t* __restrict__ header, uint64_t seq,
+             unsigned int* __restrict__ done_ticket) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  __shared__ __align__(8) uint64_t bar[SERVE_STAGES];
+  __shared__ int64_t s_row[SERVE_THREADS];
+  const int tid = threadIdx.x;
+  uint64_t seed, offset;
+  rng_stream_take(rng_state, n, seed, offset);      // every block, exactly as k_tree_sample
+  const int64_t per = (n + gridDim.x - 1) / gridDim.x;
+  const int64_t k0 = (int64_t)blockIdx.x * per;
+  const int64_t cnt = (k0 >= n) ? 0 : ((n - k0 < per) ? n - k0 : per);
+  if (tid < cnt) {
+    const int64_t k = k0 + tid;
+    double root, picked;
+    const int64_t j = tree_draw(t, philox_u01(seed, offset + (uint64_t)k), root, picked);
+    idx_out[k] = j;
+    fetch_small(small, j, k);
+    const float s32 = (float)root;
+    w_out[k] = is_weight(t, s32, __fdiv_rn((float)picked, s32), n_valid_dev, beta, max_w_ext);
+    s_row[tid] = j < 0 ? 0 : (j >= capacity ? capacity - 1 : j);   // the row b2rl_replay_gather would copy
+  }
+  if (tid == 0) {
+    for (int s = 0; s < SERVE_STAGES; ++s) sm90::mbar_init(&bar[s], 1);
+    sm90::mbar_init_fence();
+  }
+  __syncthreads();
+  if (tid == 0 && cnt > 0 && P.n > 0) {
+    const int64_t items = cnt * P.items_per_draw;
+    const int64_t pre = items < SERVE_STAGES ? items : SERVE_STAGES;
+    uint32_t phase_bits = 0;
+    int64_t loaded = 0;
+    for (; loaded < pre; ++loaded) {
+      const uint8_t* src; uint8_t* dst; uint32_t bytes;
+      serve_item(P, s_row, k0, loaded, src, dst, bytes);
+      sm90::mbar_expect_tx(&bar[loaded], bytes);
+      sm90::bulk_g2s(smem + (size_t)loaded * SERVE_CHUNK, src, bytes, &bar[loaded]);
+    }
+    int s = 0, rs = 0;
+    for (int64_t it = 0; it < items; ++it) {
+      const uint8_t* src; uint8_t* dst; uint32_t bytes;
+      serve_item(P, s_row, k0, it, src, dst, bytes);
+      sm90::mbar_wait(&bar[s], (phase_bits >> s) & 1u);
+      phase_bits ^= (1u << s);
+      sm90::bulk_s2g(dst, smem + (size_t)s * SERVE_CHUNK, bytes);
+      sm90::bulk_commit();
+      if (++s == SERVE_STAGES) s = 0;
+      if (it >= SERVE_LAG) {
+        if (loaded < items) {
+          sm90::bulk_wait_read<SERVE_LAG>();
+          const uint8_t* nsrc; uint8_t* ndst; uint32_t nbytes;
+          serve_item(P, s_row, k0, loaded, nsrc, ndst, nbytes);
+          sm90::mbar_expect_tx(&bar[rs], nbytes);
+          sm90::bulk_g2s(smem + (size_t)rs * SERVE_CHUNK, nsrc, nbytes, &bar[rs]);
+          ++loaded;
+        }
+        if (++rs == SERVE_STAGES) rs = 0;
+      }
+    }
+    sm90::bulk_wait_all();
+  }
+  // header last: written by the last CTA to get here, after every CTA's copies have completed
+  __syncthreads();
+  if (tid == 0) {
+    __threadfence();
+    if (atomicAdd(done_ticket, 1u) == gridDim.x - 1) {
+      __threadfence();
+      header[0] = seq;
+      header[1] = (uint64_t)n;
+      *done_ticket = 0u;       // re-armed for the next fill
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256)
+k_serve_put_update(uint64_t* __restrict__ header, int64_t* __restrict__ idx_dst, float* __restrict__ prio_dst,
+                   const int64_t* __restrict__ idx_src, const float* __restrict__ prio_src, int64_t n, uint64_t seq) {
+  for (int64_t k = threadIdx.x; k < n; k += blockDim.x) {
+    idx_dst[k] = idx_src[k];
+    prio_dst[k] = prio_src[k];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    header[0] = seq;
+    header[1] = (uint64_t)n;
+  }
+}
+
+}  // namespace b2rl
+
+using namespace b2rl;
+
+struct b2rl_serve_ring {
+  int device = 0;
+  bool owned = false;                  // created here (destroy) or mapped through IPC (close)
+  b2rl_serve_layout L = {};
+  uint8_t* base = nullptr;
+  unsigned int* done_ticket = nullptr; // k_serve_fill's last-CTA counter (owner only)
+};
+
+static inline int64_t align_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
+
+extern "C" int b2rl_serve_layout_init(int64_t batch, int32_t slots, int32_t n_fields, const int64_t* field_bytes,
+                                      b2rl_serve_layout* out) {
+  B2RL_REQUIRE(out != nullptr, "null out");
+  B2RL_REQUIRE(batch >= 1 && batch <= (1LL << 24), "batch out of range (1..2^24)");
+  B2RL_REQUIRE(slots >= 1 && slots <= 1024, "slots out of range (1..1024)");
+  B2RL_REQUIRE(n_fields >= 0 && n_fields <= B2RL_MAX_FIELDS, "n_fields out of range");
+  B2RL_REQUIRE(n_fields == 0 || field_bytes != nullptr, "null field_bytes");
+  b2rl_serve_layout L;
+  memset(&L, 0, sizeof(L));
+  L.batch = batch;
+  L.slots = slots;
+  L.n_fields = n_fields;
+  int64_t off = 16;                                  // header {seq, n}
+  L.idx_off = off;  off = align_up(off + 8 * batch, 16);
+  L.w_off = off;    off = align_up(off + 4 * batch, 16);
+  for (int f = 0; f < n_fields; ++f) {
+    B2RL_REQUIRE(field_bytes[f] >= 1, "field_bytes must be >= 1");
+    L.field_bytes[f] = field_bytes[f];
+    L.field_off[f] = off;
+    off = align_up(off + field_bytes[f] * batch, 16);
+  }
+  L.slot_bytes = align_up(off, 128);
+  off = 16;
+  L.upd_idx_off = off;  off = align_up(off + 8 * batch, 16);
+  L.upd_prio_off = off; off = align_up(off + 4 * batch, 16);
+  L.upd_slot_bytes = align_up(off, 128);
+  L.upd_base = (int64_t)slots * L.slot_bytes;
+  L.total_bytes = L.upd_base + (int64_t)slots * L.upd_slot_bytes;
+  *out = L;
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_serve_ring_create(b2rl_replay* h, int64_t batch, int32_t slots, b2rl_serve_ring** out) {
+  B2RL_REQUIRE(h != nullptr && out != nullptr, "null argument");
+  for (int f = 0; f < h->n_fields; ++f) {
+    const int64_t b = h->field_bytes[f];
+    B2RL_REQUIRE((b % 16 == 0 && b >= 1024) || b == 1 || b == 2 || b == 4 || b == 8,
+                 "serve ring fields must be bulk rows (multiple of 16 B, >= 1024 B) or 1/2/4/8-byte scalars");
+  }
+  b2rl_serve_layout L;
+  int rc = b2rl_serve_layout_init(batch, slots, h->n_fields, h->field_bytes, &L);
+  if (rc != B2RL_OK) return rc;
+  DeviceGuard g(h->device);
+  b2rl_serve_ring* r = new (std::nothrow) b2rl_serve_ring();
+  if (!r) { set_error("out of host memory"); return B2RL_ERR_NOMEM; }
+  r->device = h->device;
+  r->owned = true;
+  r->L = L;
+  cudaError_t e = cudaMalloc((void**)&r->base, (size_t)L.total_bytes);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&r->done_ticket, sizeof(unsigned int));
+  if (e == cudaSuccess) e = cudaMemset(r->base, 0, (size_t)L.total_bytes);
+  if (e == cudaSuccess) e = cudaMemset(r->done_ticket, 0, sizeof(unsigned int));
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {
+    set_error("serve ring of %lld bytes: %s", (long long)L.total_bytes, cudaGetErrorString(e));
+    if (r->base) cudaFree(r->base);
+    if (r->done_ticket) cudaFree(r->done_ticket);
+    delete r;
+    cudaGetLastError();
+    return B2RL_ERR_NOMEM;
+  }
+  *out = r;
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_serve_ring_layout(const b2rl_serve_ring* r, b2rl_serve_layout* out) {
+  B2RL_REQUIRE(r != nullptr && out != nullptr, "null argument");
+  *out = r->L;
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_serve_ring_export(const b2rl_serve_ring* r, void* handle_out) {
+  B2RL_REQUIRE(r != nullptr && handle_out != nullptr, "null argument");
+  B2RL_REQUIRE(r->owned, "only the ring's owner can export it");
+  static_assert(sizeof(cudaIpcMemHandle_t) == B2RL_IPC_HANDLE_BYTES, "IPC handle size");
+  DeviceGuard g(r->device);
+  cudaIpcMemHandle_t hd;
+  B2RL_CUDA(cudaIpcGetMemHandle(&hd, r->base));
+  memcpy(handle_out, &hd, sizeof(hd));
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_serve_ring_open(const void* handle, const b2rl_serve_layout* layout, int32_t device,
+                                    b2rl_serve_ring** out) {
+  B2RL_REQUIRE(handle != nullptr && layout != nullptr && out != nullptr, "null argument");
+  B2RL_REQUIRE(layout->n_fields >= 0 && layout->n_fields <= B2RL_MAX_FIELDS, "n_fields out of range");
+  b2rl_serve_layout L;
+  int rc = b2rl_serve_layout_init(layout->batch, (int32_t)layout->slots, (int32_t)layout->n_fields,
+                                  layout->field_bytes, &L);
+  if (rc != B2RL_OK) return rc;
+  B2RL_REQUIRE(memcmp(&L, layout, sizeof(L)) == 0, "layout does not match the ring arithmetic of this library");
+  int ndev = 0;
+  B2RL_CUDA(cudaGetDeviceCount(&ndev));
+  B2RL_REQUIRE(device >= 0 && device < ndev, "no such CUDA device");
+  DeviceGuard g(device);
+  cudaIpcMemHandle_t hd;
+  memcpy(&hd, handle, sizeof(hd));
+  void* p = nullptr;
+  B2RL_CUDA(cudaIpcOpenMemHandle(&p, hd, cudaIpcMemLazyEnablePeerAccess));
+  b2rl_serve_ring* r = new (std::nothrow) b2rl_serve_ring();
+  if (!r) { cudaIpcCloseMemHandle(p); set_error("out of host memory"); return B2RL_ERR_NOMEM; }
+  r->device = device;
+  r->owned = false;
+  r->L = L;
+  r->base = (uint8_t*)p;
+  *out = r;
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_serve_ring_close(b2rl_serve_ring* r) {
+  if (!r) return B2RL_OK;
+  B2RL_REQUIRE(!r->owned, "a created ring is released with b2rl_serve_ring_destroy");
+  DeviceGuard g(r->device);
+  const cudaError_t e = cudaIpcCloseMemHandle(r->base);
+  delete r;
+  B2RL_CUDA(e);
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_serve_ring_destroy(b2rl_serve_ring* r) {
+  if (!r) return B2RL_OK;
+  B2RL_REQUIRE(r->owned, "an opened ring is released with b2rl_serve_ring_close");
+  DeviceGuard g(r->device);
+  cudaDeviceSynchronize();
+  cudaFree(r->base);
+  cudaFree(r->done_ticket);
+  delete r;
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_serve_slot_ptrs(const b2rl_serve_ring* r, int32_t slot, void** batch_out, void** update_out) {
+  B2RL_REQUIRE(r != nullptr, "null ring");
+  B2RL_REQUIRE(slot >= 0 && slot < r->L.slots, "slot out of range");
+  const b2rl_serve_layout& L = r->L;
+  if (batch_out) {
+    uint8_t* s = r->base + (int64_t)slot * L.slot_bytes;
+    batch_out[0] = s;
+    batch_out[1] = s + L.idx_off;
+    batch_out[2] = s + L.w_off;
+    for (int f = 0; f < L.n_fields; ++f) batch_out[3 + f] = s + L.field_off[f];
+  }
+  if (update_out) {
+    uint8_t* u = r->base + L.upd_base + (int64_t)slot * L.upd_slot_bytes;
+    update_out[0] = u;
+    update_out[1] = u + L.upd_idx_off;
+    update_out[2] = u + L.upd_prio_off;
+  }
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, uint64_t seq, float beta,
+                               const float* max_w_dev, void* stream) {
+  B2RL_REQUIRE(h != nullptr && r != nullptr, "null argument");
+  B2RL_REQUIRE(r->owned && r->device == h->device, "fill needs the ring created for this replay, on its device");
+  B2RL_REQUIRE(slot >= 0 && slot < r->L.slots, "slot out of range");
+  B2RL_REQUIRE(r->L.n_fields == h->n_fields, "ring and replay have different fields");
+  B2RL_REQUIRE(h->size > 0, "sampling from an empty replay");
+  const b2rl_serve_layout& L = r->L;
+  void* ptrs[3 + B2RL_MAX_FIELDS];
+  int rc = b2rl_serve_slot_ptrs(r, slot, ptrs, nullptr);
+  if (rc != B2RL_OK) return rc;
+  ServeBulk P{};
+  SmallFields small{};
+  for (int f = 0; f < h->n_fields; ++f) {
+    const int64_t b = h->field_bytes[f];
+    B2RL_REQUIRE(b == L.field_bytes[f], "ring and replay have different fields");
+    if (b % 16 == 0 && b >= 1024) {
+      P.src[P.n] = h->field[f];
+      P.dst[P.n] = (uint8_t*)ptrs[3 + f];
+      P.bytes[P.n] = b;
+      P.chunks[P.n] = (int32_t)((b + SERVE_CHUNK - 1) / SERVE_CHUNK);
+      P.items_per_draw += P.chunks[P.n];
+      P.n++;
+    } else {
+      small.src[small.n] = h->field[f];
+      small.dst[small.n] = (uint8_t*)ptrs[3 + f];
+      small.bytes[small.n] = (int)b;
+      small.n++;
+    }
+  }
+  DeviceGuard g(h->device);
+  static int sms[64] = {0};
+  static bool attr_set[64] = {false};
+  const int dev = h->device & 63;
+  if (!attr_set[dev]) {
+    B2RL_CUDA(cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, h->device));
+    B2RL_CUDA(cudaFuncSetAttribute(k_serve_fill, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SERVE_SMEM));
+    attr_set[dev] = true;
+  }
+  // one CTA per SM (the shared-memory ring takes the SM), at most SERVE_THREADS draws per CTA
+  const int64_t n = L.batch;
+  int64_t grid = sms[dev] < n ? sms[dev] : n;
+  const int64_t min_grid = (n + SERVE_THREADS - 1) / SERVE_THREADS;
+  if (grid < min_grid) grid = min_grid;
+  k_serve_fill<<<(unsigned)grid, SERVE_THREADS, SERVE_SMEM, (cudaStream_t)stream>>>(
+      h->tree, P, small, h->rng_dev, n, h->capacity, h->n_valid_dev, beta, max_w_dev, (int64_t*)ptrs[1],
+      (float*)ptrs[2], (uint64_t*)ptrs[0], seq, r->done_ticket);
+  count_launch();
+  B2RL_CHECK_LAUNCH();
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_serve_take(const b2rl_serve_ring* r, int32_t slot, void* dst_dev, void* stream) {
+  B2RL_REQUIRE(r != nullptr && dst_dev != nullptr, "null argument");
+  B2RL_REQUIRE(slot >= 0 && slot < r->L.slots, "slot out of range");
+  DeviceGuard g(r->device);
+  B2RL_CUDA(cudaMemcpyAsync(dst_dev, r->base + (int64_t)slot * r->L.slot_bytes, (size_t)r->L.slot_bytes,
+                            cudaMemcpyDefault, (cudaStream_t)stream));
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_serve_put_update(b2rl_serve_ring* r, int32_t slot, uint64_t seq, const int64_t* idx_dev,
+                                     const float* prio_dev, int64_t n, void* stream) {
+  B2RL_REQUIRE(r != nullptr, "null ring");
+  B2RL_REQUIRE(slot >= 0 && slot < r->L.slots, "slot out of range");
+  B2RL_REQUIRE(n >= 0 && n <= r->L.batch, "n out of range (0..batch)");
+  B2RL_REQUIRE(n == 0 || (idx_dev != nullptr && prio_dev != nullptr), "null idx/prio");
+  void* u[3];
+  int rc = b2rl_serve_slot_ptrs(r, slot, nullptr, u);
+  if (rc != B2RL_OK) return rc;
+  DeviceGuard g(r->device);
+  k_serve_put_update<<<1, 256, 0, (cudaStream_t)stream>>>((uint64_t*)u[0], (int64_t*)u[1], (float*)u[2], idx_dev,
+                                                          prio_dev, n, seq);
+  count_launch();
+  B2RL_CHECK_LAUNCH();
+  return B2RL_OK;
+}

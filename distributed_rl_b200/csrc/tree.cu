@@ -22,6 +22,7 @@
 //   * the tree costs 4N + N/15*12 bytes instead of 32N, and a bulk build moves
 //     ~8.8N bytes (4N read, 4N leaf copy, 0.75N nodes) for 8N algorithmic
 #include "common.cuh"
+#include "tree.cuh"
 
 #include <math.h>
 #include <stdlib.h>
@@ -29,51 +30,8 @@
 namespace b2rl {
 
 // ----------------------------------------------------------------------------
-// 16-wide group arithmetic
+// 16-wide group arithmetic (ld4f / load_child_sums / descend16 live in tree.cuh)
 // ----------------------------------------------------------------------------
-// Children of node `node` of stored level k (k >= 1) live on stored level k-1 at
-// [node << bits, (node << bits) + 2^bits), bits = 4 below the top group.  Missing
-// children of a narrower top group are 0 / +inf: x + 0 == x, so the pairwise sum
-// is still the binary tree's value.
-template <bool CG>
-__device__ __forceinline__ float4 ld4f(const float* p) {
-  return CG ? __ldcg(reinterpret_cast<const float4*>(p)) : *reinterpret_cast<const float4*>(p);
-}
-template <bool CG>
-__device__ __forceinline__ double2 ld2d(const double* p) {
-  return CG ? __ldcg(reinterpret_cast<const double2*>(p)) : *reinterpret_cast<const double2*>(p);
-}
-
-template <bool CG>
-__device__ __forceinline__ void load_child_sums(const TreeView& t, int k, int64_t node, double c[16]) {
-  const int bits = (k == t.G) ? t.top_bits : 4;
-  if (k == 1) {
-    const float* p = t.leaf + (node << bits);
-    if (bits == 4) {
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float4 v = ld4f<CG>(p + 4 * q);
-        c[4 * q] = (double)v.x; c[4 * q + 1] = (double)v.y; c[4 * q + 2] = (double)v.z; c[4 * q + 3] = (double)v.w;
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) c[i] = (i < (1 << bits)) ? (double)(CG ? __ldcg(p + i) : p[i]) : 0.0;
-    }
-  } else {
-    const double* p = t.sum + t.off[k - 1] + (node << bits);
-    if (bits == 4) {
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const double2 v = ld2d<CG>(p + 2 * q);
-        c[2 * q] = v.x; c[2 * q + 1] = v.y;
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) c[i] = (i < (1 << bits)) ? (CG ? __ldcg(p + i) : p[i]) : 0.0;
-    }
-  }
-}
-
 template <bool CG>
 __device__ __forceinline__ float load_child_min(const TreeView& t, int k, int64_t node) {
   const int bits = (k == t.G) ? t.top_bits : 4;
@@ -116,42 +74,6 @@ __device__ __forceinline__ void recompute_node(const TreeView& t, int k, int64_t
   const float m = load_child_min<CG>(t, k, node);
   t.sum[t.off[k] + node] = pairwise16(c);
   t.minv[t.off[k] + node] = m;
-}
-
-// Four binary descent steps inside one 16-wide group (Node._find :53-62 applied to the
-// three recomputed levels and the stored children).  Returns the child index, updates pos,
-// and leaves the selected child's sum in `picked`.
-__device__ __forceinline__ int descend16(const double c_in[16], double& pos, double& picked) {
-  double c[16], s1[8], s2[4], s3[2];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) c[i] = c_in[i];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) s1[i] = c[2 * i] + c[2 * i + 1];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) s2[i] = s1[2 * i] + s1[2 * i + 1];
-  s3[0] = s2[0] + s2[1];
-  s3[1] = s2[2] + s2[3];
-  // The `right == 0` guard only matters when pos rounds up to the subtree total (the reference
-  // dereferences None there); it also steers a narrower top group into its zero-padded left part.
-  const bool r1 = !((pos < s3[0]) || (s3[1] == 0.0));
-  if (r1) pos = __dsub_rn(pos, s3[0]);
-  const double a2 = r1 ? s2[2] : s2[0], b2 = r1 ? s2[3] : s2[1];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) s1[i] = r1 ? s1[4 + i] : s1[i];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) c[i] = r1 ? c[8 + i] : c[i];
-  const bool r2 = !((pos < a2) || (b2 == 0.0));
-  if (r2) pos = __dsub_rn(pos, a2);
-  const double a1 = r2 ? s1[2] : s1[0], b1 = r2 ? s1[3] : s1[1];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) c[i] = r2 ? c[4 + i] : c[i];
-  const bool r3 = !((pos < a1) || (b1 == 0.0));
-  if (r3) pos = __dsub_rn(pos, a1);
-  const double a0 = r3 ? c[2] : c[0], b0 = r3 ? c[3] : c[1];
-  const bool r4 = !((pos < a0) || (b0 == 0.0));
-  if (r4) pos = __dsub_rn(pos, a0);
-  picked = r4 ? b0 : a0;
-  return (r1 ? 8 : 0) | (r2 ? 4 : 0) | (r3 ? 2 : 0) | (r4 ? 1 : 0);
 }
 
 // ----------------------------------------------------------------------------
@@ -272,76 +194,25 @@ k_build_leaves(const __grid_constant__ TreeView t, const float* __restrict__ pri
 // ----------------------------------------------------------------------------
 constexpr int SAMPLE_THREADS = 128;
 
-struct SmallFields {
-  const uint8_t* src[B2RL_MAX_FIELDS];
-  uint8_t* dst[B2RL_MAX_FIELDS];
-  int bytes[B2RL_MAX_FIELDS];
-  int n;
-};
-
 __global__ void __launch_bounds__(SAMPLE_THREADS)
 k_tree_sample(const __grid_constant__ TreeView t, const double* __restrict__ u01, uint64_t seed, uint64_t rng_offset,
               const uint64_t* __restrict__ rng_state, int64_t n, const float* __restrict__ n_valid_dev, float beta,
               const float* __restrict__ max_w_ext, int64_t* __restrict__ idx_out,
               float* __restrict__ prob_out, float* __restrict__ w_out, SmallFields small) {
   const int64_t k = (int64_t)blockIdx.x * SAMPLE_THREADS + threadIdx.x;
-  if (rng_state) {
-    // device-resident Philox stream: every block reads {seed, counter}; the LAST block to have done
-    // so advances the counter by n (and re-arms the ticket), so no separate launch is needed.
-    seed = rng_state[0];
-    rng_offset = rng_state[1];
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      __threadfence();
-      unsigned int* ticket = reinterpret_cast<unsigned int*>(const_cast<uint64_t*>(rng_state) + 2);
-      if (atomicAdd(ticket, 1u) == gridDim.x - 1) {
-        const_cast<uint64_t*>(rng_state)[1] = rng_offset + (uint64_t)n;
-        *ticket = 0u;
-      }
-    }
-  }
+  if (rng_state) rng_stream_take(const_cast<uint64_t*>(rng_state), n, seed, rng_offset);
   if (k >= n) return;
-  const double root = t.sum[t.off[t.G]];
   const double u = u01 ? u01[k] : philox_u01(seed, rng_offset + (uint64_t)k);
-  double pos = __dmul_rn(root, u);  // np.random.uniform(0, root) == root * random_sample()
-  int64_t node = 0;
-  double picked = 0.0;
-  for (int lvl = t.G; lvl >= 1; --lvl) {
-    double c[16];
-    load_child_sums<false>(t, lvl, node, c);     // 128 B (64 B on the leaf level): one dependent load per 4 levels
-    const int bits = (lvl == t.G) ? t.top_bits : 4;
-    const int ch = descend16(c, pos, picked);
-    node = (node << bits) | (int64_t)(ch & ((1 << bits) - 1));
-  }
-  const int64_t j = node;
+  double root, picked;
+  const int64_t j = tree_draw(t, u, root, picked);
   idx_out[k] = j;
-  for (int f = 0; f < small.n; ++f) {       // scalar fields of the sampled slot (a, r, done): 1/2/4/8-byte rows
-    const int b = small.bytes[f];
-    const uint8_t* s = small.src[f] + j * b;
-    uint8_t* d = small.dst[f] + k * b;
-    if (b == 4) *reinterpret_cast<uint32_t*>(d) = *reinterpret_cast<const uint32_t*>(s);
-    else if (b == 1) *d = *s;
-    else if (b == 8) *reinterpret_cast<uint64_t*>(d) = *reinterpret_cast<const uint64_t*>(s);
-    else *reinterpret_cast<uint16_t*>(d) = *reinterpret_cast<const uint16_t*>(s);
-  }
+  fetch_small(small, j, k);                 // scalar fields of the sampled slot (a, r, done)
   if (prob_out == nullptr && w_out == nullptr) return;
-  // APE_X/ReplayMemory.py:65-67, baseline/PER.py:98,129-133 — fp32 op by op.
   const float s32 = (float)root;
   const float p = (float)picked;
   const float prob = __fdiv_rn(p, s32);
   if (prob_out) prob_out[k] = prob;
-  if (w_out) {
-    const float n_valid = *n_valid_dev;   // current number of valid slots (stream-ordered, not a launch constant)
-    const float w_un = powcr(__fdiv_rn(1.0f, __fmul_rn(n_valid, prob)), beta);
-    float max_w;
-    if (max_w_ext) {
-      max_w = *max_w_ext;
-    } else {
-      const float min_prob = __fdiv_rn(t.minv[t.off[t.G]], s32);
-      max_w = powcr(__fmul_rn(n_valid, min_prob), -beta);
-    }
-    w_out[k] = __fdiv_rn(w_un, max_w);
-  }
+  if (w_out) w_out[k] = is_weight(t, s32, prob, n_valid_dev, beta, max_w_ext);
 }
 
 __global__ void k_rng_seed(uint64_t* __restrict__ rng_state, uint64_t seed, uint64_t ctr) {

@@ -12,17 +12,44 @@ What is GPU-native here is the server's store: sampling, IS weights, gather and 
 kernels of libb2rl (one sample launch + one TMA gather per served group of minibatches, applied updates in stream
 order); the transport stays the reference's pickled Redis lists — this mode exists so that a deployment which
 runs the reference's replay out of process keeps working, not as the fast path (the in-process `Replay` is).
-Lists are drained atomically (`wire.drain`), see wire.py."""
+Lists are drained atomically (`wire.drain`), see wire.py.
+
+`DeviceReplayServer` / `DeviceReplayClient` are the GPU-native transport beside them: minibatches are drawn and
+assembled by ONE kernel (`b2rl_serve_fill`) straight into a ring of device slots that the learner maps through CUDA
+IPC, and priorities come back through update slots of the same ring; no minibatch or priority touches the host.
+Redis carries only small descriptors and the handles (DESIGN.md §4.15):
+
+  key   SERVE_RING     ring IPC handle + layout + the server's events (filled[k], applied[j])   server -> learner
+  key   SERVE_CLIENT   the learner's events (released[k], written[j])                          learner -> server
+  key   SERVE_STATS    (len(replay), max IS weight), for `memory`                              server -> learner
+  key   SERVE_DETACHED the learner has unmapped the ring: the server may free it               learner -> server
+  list  BATCH_SLOT     (k, seq, n): minibatch slot k holds fill `seq`                          server -> learner
+  list  RELEASE_SLOT   (k, seq): the learner's copy out of slot k is enqueued                  learner -> server
+  list  UPDATE_SLOT    (j, seq, n): update slot j holds n (idx, priority) pairs                learner -> server
+  list  UPDATE_DONE    (j, seq): the server's tree update of slot j is enqueued                server -> learner
+
+Event invariant: an interprocess event is re-recorded only after the host-level handshake for its slot has
+completed, and a peer's stream waits on it only after reading the descriptor posted behind the record.  So every
+`cudaStreamWaitEvent` waits on the intended record, and no kernel ever waits for the other process: a missing peer
+leaves slots unserved, it cannot hang a GPU.
+
+Shutdown: the learner closes its client first (unmap, then SERVE_DETACHED); the server frees the ring only after
+that key appears.  A learner that attached with `apex.Learner(connect=..., memory=client)` keeps SERVER_KEYS out of
+its start-up wipe of stale keys."""
 from __future__ import annotations
 
+import ctypes as C
 import pickle
 import threading
 import time
+from collections import deque
 
 import numpy as np
 import torch
 
-from . import wire
+from . import _lib, wire
+from . import replay as R
+from ._lib import check
 from .apex import ApexConfig
 from .learner_common import Stoppable
 
@@ -144,3 +171,434 @@ class Replay_Server(Stoppable, threading.Thread):
                 return False
             blob = self.deque.pop(0)
         return pickle.loads(blob)
+
+
+# ---- device serve ring ----------------------------------------------------------------------------------------------
+RING_KEY, CLIENT_KEY, STATS_KEY, DETACH_KEY = "SERVE_RING", "SERVE_CLIENT", "SERVE_STATS", "SERVE_DETACHED"
+BATCH_SLOT, RELEASE_SLOT, UPDATE_SLOT, UPDATE_DONE = "BATCH_SLOT", "RELEASE_SLOT", "UPDATE_SLOT", "UPDATE_DONE"
+# What a running DeviceReplayServer reads or owns: a learner attached to it must not wipe these at start-up
+# (the server resets its own keys when it starts).
+SERVER_KEYS = (RING_KEY, CLIENT_KEY, STATS_KEY, DETACH_KEY, BATCH_SLOT, RELEASE_SLOT, UPDATE_SLOT, UPDATE_DONE,
+               "experience", "FLAG_BATCH", "FLAG_REMOVE")
+
+
+def serve_layout(batch: int, slots: int, field_bytes) -> _lib.ServeLayout:
+    """The ring geometry for a replay whose fields have these row sizes (b2rl_serve_layout_init; no CUDA call)."""
+    L = _lib.ServeLayout()
+    fb = (C.c_int64 * _lib.MAX_FIELDS)(*[int(b) for b in field_bytes])
+    check(_lib.load().b2rl_serve_layout_init(int(batch), int(slots), len(field_bytes), fb, C.byref(L)))
+    return L
+
+
+class ServeRing:
+    """The ring allocation as seen by this process: created for a DeviceReplay (the server owns it) or mapped from
+    an exported IPC handle (the learner)."""
+
+    def __init__(self, handle: C.c_void_p, device: torch.device, owned: bool):
+        self.lib = _lib.load()
+        self._h, self.device, self.owned = handle, device, owned
+        self.layout = _lib.ServeLayout()
+        check(self.lib.b2rl_serve_ring_layout(self._h, C.byref(self.layout)))
+
+    @classmethod
+    def create(cls, store: R.DeviceReplay, batch: int, slots: int) -> "ServeRing":
+        h = C.c_void_p()
+        check(_lib.load().b2rl_serve_ring_create(store._h, int(batch), int(slots), C.byref(h)))
+        return cls(h, store.device, True)
+
+    @classmethod
+    def open(cls, handle: bytes, layout: bytes, device) -> "ServeRing":
+        device = torch.device(device)
+        L = _lib.ServeLayout.from_buffer_copy(layout)
+        buf = C.create_string_buffer(bytes(handle), _lib.IPC_HANDLE_BYTES)
+        h = C.c_void_p()
+        with torch.cuda.device(device):
+            torch.zeros(1, device=device)          # the primary context the mapping lives in
+            check(_lib.load().b2rl_serve_ring_open(buf, C.byref(L), device.index, C.byref(h)))
+        return cls(h, device, False)
+
+    def export(self) -> bytes:
+        buf = C.create_string_buffer(_lib.IPC_HANDLE_BYTES)
+        check(self.lib.b2rl_serve_ring_export(self._h, buf))
+        return buf.raw
+
+    def layout_bytes(self) -> bytes:
+        return bytes(self.layout)
+
+    def slot_ptrs(self, k: int):
+        """-> (minibatch slot pointers {header, idx, w, field 0, ...}, update slot pointers {header, idx, prio})."""
+        b, u = (C.c_void_p * (3 + _lib.MAX_FIELDS))(), (C.c_void_p * 3)()
+        check(self.lib.b2rl_serve_slot_ptrs(self._h, int(k), b, u))
+        return list(b)[:3 + self.layout.n_fields], list(u)
+
+    def fill(self, store: R.DeviceReplay, k: int, seq: int, beta: float, max_w: torch.Tensor | None = None) -> None:
+        check(self.lib.b2rl_serve_fill(store._h, self._h, int(k), int(seq), float(beta),
+                                       None if max_w is None else max_w.data_ptr(), store._st()))
+
+    def take(self, k: int, dst: torch.Tensor, stream) -> None:
+        assert dst.is_contiguous() and dst.numel() * dst.element_size() >= self.layout.slot_bytes
+        check(self.lib.b2rl_serve_take(self._h, int(k), dst.data_ptr(), stream.cuda_stream))
+
+    def put_update(self, j: int, seq: int, idx: torch.Tensor, prio: torch.Tensor, stream) -> None:
+        check(self.lib.b2rl_serve_put_update(self._h, int(j), int(seq), idx.data_ptr(), prio.data_ptr(), idx.numel(),
+                                             stream.cuda_stream))
+
+    def close(self) -> None:
+        if getattr(self, "_h", None):
+            (self.lib.b2rl_serve_ring_destroy if self.owned else self.lib.b2rl_serve_ring_close)(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class ServerSlots:
+    """The server's half of the host-level handshake (no CUDA here: the device work is passed in).
+    A minibatch slot is free, or out (filled and announced, not yet released by the learner)."""
+
+    def __init__(self, connect, slots: int, batch: int):
+        self.connect, self.batch = connect, batch
+        self.free = list(range(slots))
+        self.out = {}                 # slot -> seq of the fill the learner has not released yet
+        self.seq = 0
+
+    def collect_releases(self, wait) -> int:
+        """Drain RELEASE_SLOT; `wait(k)` makes the server stream wait on released[k] (recorded by the learner before
+        it posted the descriptor) before slot k can be refilled."""
+        got = [pickle.loads(d) for d in wire.drain(self.connect, RELEASE_SLOT)]
+        for k, seq in got:
+            if self.out.get(k) != seq:
+                raise RuntimeError(f"release of slot {k} (seq {seq}) that the server did not hand out")
+            wait(k)
+            del self.out[k]
+            self.free.append(k)
+        return len(got)
+
+    def apply_updates(self, apply) -> int:
+        """Drain UPDATE_SLOT; `apply(j, n)` waits on written[j], applies the slot to the tree and records
+        applied[j]; then UPDATE_DONE hands the slots back.  -> number of priorities applied."""
+        got = [pickle.loads(d) for d in wire.drain(self.connect, UPDATE_SLOT)]
+        for j, _, n in got:
+            apply(j, n)
+        if got:
+            self.connect.rpush(UPDATE_DONE, *[pickle.dumps((j, seq)) for j, seq, _ in got])
+        return sum(n for _, _, n in got)
+
+    def fill_free(self, fill) -> int:
+        """`fill(k, seq)` fills every free slot and records filled[k]; then the descriptors go out, in fill order."""
+        blobs = []
+        while self.free:
+            k = self.free.pop(0)
+            self.seq += 1
+            fill(k, self.seq)
+            self.out[k] = self.seq
+            blobs.append(pickle.dumps((k, self.seq, self.batch)))
+        if blobs:
+            self.connect.rpush(BATCH_SLOT, *blobs)
+        return len(blobs)
+
+
+class ClientSlots:
+    """The learner's half of the handshake (no CUDA here).  Thread-safe: a polling thread may call poll()."""
+
+    def __init__(self, connect, slots: int):
+        self.connect = connect
+        self.ready = deque()          # (k, seq, n) announced by the server, not yet copied out
+        self.upd_free = list(range(slots))
+        self.upd_seq = 0
+        self._mu = threading.Lock()
+
+    def poll(self) -> None:
+        pipe = self.connect.pipeline()
+        for key in (BATCH_SLOT, UPDATE_DONE):
+            pipe.lrange(key, 0, -1)
+            pipe.delete(key)
+        r = pipe.execute()
+        filled, done = r[0] or [], r[2] or []
+        with self._mu:
+            self.ready.extend(pickle.loads(d) for d in filled)
+            self.upd_free.extend(pickle.loads(d)[0] for d in done)
+
+    def take(self, copy):
+        """The oldest filled slot: `copy(k)` waits on filled[k], copies the slot out and records released[k]; then
+        RELEASE_SLOT hands it back.  -> (k, seq, n), or None when nothing is filled."""
+        with self._mu:
+            if not self.ready:
+                return None
+            k, seq, n = self.ready.popleft()
+        copy(k)
+        self.connect.rpush(RELEASE_SLOT, pickle.dumps((k, seq)))
+        return k, seq, n
+
+    def put_update(self, write, n: int) -> bool:
+        """A free update slot j: `write(j, seq)` waits on applied[j], writes the slot and records written[j]; then
+        UPDATE_SLOT announces it.  False when every update slot is still with the server."""
+        with self._mu:
+            if not self.upd_free:
+                return False
+            j = self.upd_free.pop(0)
+            self.upd_seq += 1
+            seq = self.upd_seq
+        write(j, seq)
+        self.connect.rpush(UPDATE_SLOT, pickle.dumps((j, seq, n)))
+        return True
+
+
+def _ipc_events(device: torch.device, n: int):
+    """n interprocess events on `device` and their IPC handles (torch creates an event lazily, on the current
+    device: the handles are taken inside the device guard)."""
+    with torch.cuda.device(device):
+        ev = [torch.cuda.Event(interprocess=True) for _ in range(n)]
+        return ev, [e.ipc_handle() for e in ev]
+
+
+class DeviceReplayServer(Stoppable):
+    """The stand-alone replay server over a device ring (APE_X/ReplayServer.py:20-160): the same `experience` ingest,
+    eviction on FLAG_REMOVE and FLAG_BATCH as `ReplayServer`, but each served minibatch is one `b2rl_serve_fill`
+    launch into a ring slot the learner maps through CUDA IPC.  Keeps up to `slots` filled minibatches ahead of the
+    learner and applies arriving update slots in stream order.  Run it in its own process (CUDA IPC cannot map a
+    handle into the process that exported it)."""
+
+    STATS_EVERY = 0.1             # seconds between SERVE_STATS refreshes (each costs a device sync)
+
+    def __init__(self, cfg: ApexConfig | None = None, connect=None, slots: int = 4):
+        super().__init__()
+        self.cfg = cfg or ApexConfig.from_configuration()
+        self.device = torch.device(self.cfg.LEARNER_DEVICE)
+        from .apex import Replay
+        self._ingest = Replay(self.cfg, connect=None)      # never started: its record decoder + pinned staging + store
+        self.store = self._ingest.store
+        self.device = self.store.device
+        self.connect = connect
+        self.ring = ServeRing.create(self.store, self.cfg.BATCHSIZE, slots)
+        self.slots = ServerSlots(connect, slots, self.cfg.BATCHSIZE)
+        (self.filled, filled_h), (self.applied, applied_h) = _ipc_events(self.device, slots), _ipc_events(self.device, slots)
+        self.released = self.written = None                # the learner's events, once it has attached
+        self._upd = [self.ring.slot_ptrs(j)[1] for j in range(slots)]
+        self.FLAG_BATCH = False
+        self.total_transition = 0
+        self._stats_t = 0.0
+        connect.delete(BATCH_SLOT, RELEASE_SLOT, UPDATE_SLOT, UPDATE_DONE, CLIENT_KEY, STATS_KEY, DETACH_KEY)
+        connect.set("FLAG_BATCH", pickle.dumps(False))
+        connect.set(RING_KEY, pickle.dumps({
+            "handle": self.ring.export(), "layout": self.ring.layout_bytes(), "device": self.device.index,
+            "filled": filled_h, "applied": applied_h}))
+
+    def _stream(self):
+        return torch.cuda.current_stream(self.device)
+
+    def _peer_events(self):
+        """The learner's released / written events (SERVE_CLIENT is set before the learner posts any descriptor)."""
+        if self.released is None:
+            blob = self.connect.get(CLIENT_KEY)
+            if blob is None:
+                raise RuntimeError("a descriptor arrived before the learner published its events")
+            info = pickle.loads(blob)
+            dev = torch.device("cuda", info["device"])
+            self.released = [torch.cuda.Event.from_ipc_handle(dev, h) for h in info["released"]]
+            self.written = [torch.cuda.Event.from_ipc_handle(dev, h) for h in info["written"]]
+        return self.released, self.written
+
+    def _wait_released(self, k: int) -> None:
+        self._stream().wait_event(self._peer_events()[0][k])
+
+    def _apply(self, j: int, n: int) -> None:
+        st = self._stream()
+        st.wait_event(self._peer_events()[1][j])
+        _, idx, prio = self._upd[j]
+        check(self.store.lib.b2rl_tree_update(self.store._h, idx, prio, int(n), st.cuda_stream))
+        self.applied[j].record(st)
+
+    def _fill(self, k: int, seq: int) -> None:
+        self.ring.fill(self.store, k, seq, self.cfg.BETA)
+        self.filled[k].record(self._stream())
+
+    def _publish_stats(self, force: bool) -> None:
+        now = time.time()
+        if force or now - self._stats_t > self.STATS_EVERY:
+            mw = float(self.store.stats(self.cfg.BETA)[2].item()) if len(self.store) else 0.0
+            self.connect.set(STATS_KEY, pickle.dumps((len(self.store), mw)))
+            self._stats_t = now
+
+    def serve_once(self) -> dict:
+        """One iteration of run(): ingest, take back released slots, apply update slots, refill free slots, evict."""
+        k = self.cfg.BUFFER_SIZE
+        if len(self.store) > k and not self.FLAG_BATCH:
+            self.FLAG_BATCH = True
+            self.connect.set("FLAG_BATCH", pickle.dumps(True))
+        data = wire.drain(self.connect, "experience")
+        if data:
+            self._ingest.push_records(data)
+            self.total_transition += len(data)
+        released = self.slots.collect_releases(self._wait_released)
+        applied = self.slots.apply_updates(self._apply)
+        filled = self.slots.fill_free(self._fill) if len(self.store) > k else 0
+        if len(self.store) >= self.cfg.REPLAY_MEMORY_LEN:
+            cond = self.connect.get("FLAG_REMOVE")
+            if cond is not None and pickle.loads(cond):
+                over = len(self.store) - self.cfg.REPLAY_MEMORY_LEN
+                if over > 0:
+                    self.store.evict(over)
+                self.connect.set("FLAG_REMOVE", pickle.dumps(False))
+        self._publish_stats(bool(data))
+        return {"ingested": len(data), "filled": filled, "released": released, "updates_applied": applied}
+
+    def run(self):
+        while not self._stop_evt.is_set():
+            st = self.serve_once()
+            if not (st["ingested"] or st["filled"] or st["released"] or st["updates_applied"]):
+                time.sleep(0.0005)
+
+    def close(self, timeout: float = 60.0) -> bool:
+        """Free the ring once the learner has unmapped it.  If a learner attached, wait (up to `timeout` s) for its
+        SERVE_DETACHED, which DeviceReplayClient.close() sets after unmapping.  Without it the ring is NOT freed —
+        a learner may still be copying out of a slot — and is released with this process.  -> True when freed."""
+        torch.cuda.synchronize(self.device)
+        if self.released is not None or self.connect.get(CLIENT_KEY) is not None:
+            t0 = time.time()
+            while self.connect.get(DETACH_KEY) is None:
+                if time.time() - t0 > timeout:
+                    self.ring._h = None          # left mapped: freed with the process, never under a reader
+                    return False
+                time.sleep(0.01)
+        self.ring.close()
+        return True
+
+
+class ServedMemory:
+    """`Replay.memory` of a DeviceReplayClient: len() and .max_weight as the server last published them."""
+
+    def __init__(self, connect):
+        self._connect = connect
+
+    def _stats(self):
+        blob = self._connect.get(STATS_KEY)
+        return pickle.loads(blob) if blob is not None else (0, 0.0)
+
+    def __len__(self):
+        return int(self._stats()[0])
+
+    @property
+    def max_weight(self) -> float:
+        return float(self._stats()[1])
+
+
+class DeviceReplayClient(Stoppable, threading.Thread):
+    """Learner-side consumer of a DeviceReplayServer with the `Replay` surface (start / stop / sample / update / lock /
+    memory; APE_X/ReplayMemory.py:170-257).  sample() returns `[s, a, r, s', done, w, idx]` as CUDA tensors on the
+    learner's device, copied out of the ring (a peer copy when the server is on another GPU)."""
+
+    KEEP_KEYS = SERVER_KEYS       # what apex.Learner(connect=..., memory=this) leaves in place at start-up
+
+    def __init__(self, cfg: ApexConfig | None = None, connect=None, timeout: float = 60.0):
+        super().__init__(daemon=True)
+        self.cfg = cfg or ApexConfig.from_configuration()
+        self.device = torch.device(self.cfg.LEARNER_DEVICE)
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.connect = connect
+        self.lock = False
+        t0 = time.time()
+        while (blob := connect.get(RING_KEY)) is None:
+            if time.time() - t0 > timeout:
+                raise TimeoutError(f"no replay server published {RING_KEY} within {timeout} s")
+            time.sleep(0.01)
+        info = pickle.loads(blob)
+        self.ring = ServeRing.open(info["handle"], info["layout"], self.device)
+        L = self.ring.layout
+        self.fields = R.APEX_FIELDS
+        if [L.field_bytes[i] for i in range(L.n_fields)] != [f.nbytes for f in self.fields]:
+            raise RuntimeError("the server's ring does not carry the Ape-X record fields")
+        srv = torch.device("cuda", info["device"])
+        self.filled = [torch.cuda.Event.from_ipc_handle(srv, h) for h in info["filled"]]
+        self.applied = [torch.cuda.Event.from_ipc_handle(srv, h) for h in info["applied"]]
+        (self.released, released_h), (self.written, written_h) = _ipc_events(self.device, L.slots), \
+            _ipc_events(self.device, L.slots)
+        connect.set(CLIENT_KEY, pickle.dumps({"device": self.device.index, "released": released_h,
+                                              "written": written_h}))
+        self.slots = ClientSlots(connect, L.slots)
+        self.memory = ServedMemory(connect)
+        self._pending = deque()      # priority write-backs waiting for a free update slot
+        self.last_served = None      # descriptor (k, seq, n) of the last served slot
+        self.last_header = None      # its header {seq, n} as copied out: a device int64[2]
+
+    def poll_once(self) -> None:
+        self.slots.poll()
+        if self.lock:                                   # eviction request -> the server's flag
+            self.connect.set("FLAG_REMOVE", pickle.dumps(True))
+            self.lock = False
+
+    def run(self):
+        while not self._stop_evt.is_set():
+            self.poll_once()
+            time.sleep(0.0005)
+
+    def _views(self, buf: torch.Tensor):
+        L, B = self.ring.layout, self.ring.layout.batch
+
+        def view(off, nbytes, dtype, shape):
+            return buf[off:off + nbytes].view(dtype).view(shape)
+        out = {f.name: view(L.field_off[i], B * f.nbytes, f.dtype, (B,) + tuple(f.shape))
+               for i, f in enumerate(self.fields)}
+        return (view(0, 16, torch.int64, (2,)), view(L.idx_off, 8 * B, torch.int64, (B,)),
+                view(L.w_off, 4 * B, torch.float32, (B,)), out)
+
+    def sample(self):
+        """Replay_Server.sample (APE_X/ReplayMemory.py:251-257): the oldest filled slot, copied into fresh
+        learner-local memory on the current stream; False when nothing is filled."""
+        cur = torch.cuda.current_stream(self.device)
+        got = []
+
+        def copy(k):
+            buf = torch.empty(self.ring.layout.slot_bytes, dtype=torch.uint8, device=self.device)
+            cur.wait_event(self.filled[k])
+            self.ring.take(k, buf, cur)
+            self.released[k].record(cur)
+            got.append(buf)
+        if self.lock or not self.slots.ready:
+            self.poll_once()
+        desc = self.slots.take(copy)
+        if desc is None:
+            return False
+        header, idx, w, b = self._views(got[0])
+        self.last_served, self.last_header = desc, header
+        return [b["state"], b["action"], b["reward"], b["next_state"], b["done"], w, idx]
+
+    def update(self, idx, vals) -> None:
+        """Replay_Server.update (APE_X/ReplayMemory.py:188-190): the write-back goes to free update slots of the
+        ring (at most B pairs each) and is applied by the server in stream order.  `idx`: a tensor, an array, or a
+        list of ints or 0-d tensors."""
+        if isinstance(idx, (list, tuple)):
+            idx = torch.stack([torch.as_tensor(i) for i in idx]) if len(idx) and torch.is_tensor(idx[0]) \
+                else torch.as_tensor(np.asarray(idx, np.int64))
+        idx = torch.as_tensor(idx).to(device=self.device, dtype=torch.int64).reshape(-1).contiguous()
+        vals = torch.as_tensor(vals).to(device=self.device, dtype=torch.float32).reshape(-1).contiguous()
+        assert idx.numel() == vals.numel()
+        B = self.ring.layout.batch
+        for a in range(0, idx.numel(), B):
+            self._pending.append((idx[a:a + B], vals[a:a + B]))
+        self._flush_updates()
+
+    def _flush_updates(self) -> None:
+        cur = torch.cuda.current_stream(self.device)
+        while self._pending:
+            i, v = self._pending[0]
+
+            def write(j, seq):
+                cur.wait_event(self.applied[j])        # the server's tree update has read the slot's last contents
+                self.ring.put_update(j, seq, i, v, cur)
+                self.written[j].record(cur)
+            if not self.slots.put_update(write, i.numel()):
+                self.slots.poll()
+                if not self.slots.put_update(write, i.numel()):
+                    return                              # every update slot is with the server: retried next time
+            self._pending.popleft()
+
+    def close(self) -> None:
+        """Unmap the ring, then tell the server (SERVE_DETACHED) that it may free it."""
+        torch.cuda.synchronize(self.device)
+        self.ring.close()
+        self.connect.set(DETACH_KEY, pickle.dumps(True))

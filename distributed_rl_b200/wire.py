@@ -36,11 +36,15 @@ def drain(connect, key: str) -> list:
     return list(pipe.execute()[0] or [])
 
 
-def wipe_stale_keys(connect) -> int:
+def wipe_stale_keys(connect, keep=()) -> int:
     """Learner.__init__ (APE_X/Learner.py:41-43, R2D2/Learner.py:54,63-64): drop whatever a previous run
-    left in the database (stale `experience`, `Start`, parameters ...)."""
+    left in the database (stale `experience`, `Start`, parameters ...).  `keep`: key names that belong to a
+    process which is already running beside the learner (a replay server) and are left alone."""
     names = connect.scan()
     keys = list(names[-1]) if names else []
+    if keep:
+        keep = set(keep)
+        keys = [k for k in keys if (k.decode() if isinstance(k, bytes) else k) not in keep]
     if keys:
         connect.delete(*keys)
     return len(keys)

@@ -327,6 +327,72 @@ int b2rl_dueling_backward(const float* h_dev, const float* gq_dev, int64_t M, in
 int b2rl_dueling_backward_w(const float* h_dev, const float* row_ws_dev, int64_t M, int64_t H, int64_t A,
                             float* gwa_dev, float* gwv_dev, void* stream);
 
+/* Device serve ring: the stand-alone replay server's minibatch transport without the host
+ * (APE_X/ReplayServer.py:41-114 serves pickled minibatches over the Redis list `BATCH` and applies the
+ * pickled `update` list; APE_X/ReplayMemory.py:170-257 is the learner-side consumer).  ONE cudaMalloc
+ * allocation owned by the server process holds `slots` minibatch slots followed by `slots` update slots:
+ *   minibatch slot: header {uint64 seq, int64 n} | idx int64[B] | w fp32[B] | field f: B rows of
+ *                   field_bytes[f] (the replay's fields in order)
+ *   update slot:    header {uint64 seq, int64 n} | idx int64[B] | prio fp32[B]
+ * Every array starts on a 16-byte boundary, every slot on a 128-byte boundary.  The learner process maps the
+ * allocation through CUDA IPC (on the same GPU or a peer GPU); the handshake that orders the two processes'
+ * streams is host-level (Redis descriptors + interprocess CUDA events): nothing on the device waits for the
+ * other process. */
+#define B2RL_IPC_HANDLE_BYTES 64
+typedef struct b2rl_serve_ring b2rl_serve_ring; /* opaque */
+typedef struct {
+  int64_t batch;                          /* B: transitions per minibatch slot          */
+  int64_t slots;                          /* K: minibatch slots (and as many update slots) */
+  int64_t n_fields;
+  int64_t field_bytes[B2RL_MAX_FIELDS];
+  int64_t field_off[B2RL_MAX_FIELDS];     /* field f's B rows inside a minibatch slot   */
+  int64_t idx_off, w_off;                 /* inside a minibatch slot (header at 0)      */
+  int64_t slot_bytes;                     /* stride of the minibatch slots              */
+  int64_t upd_idx_off, upd_prio_off;      /* inside an update slot (header at 0)        */
+  int64_t upd_slot_bytes;                 /* stride of the update slots                 */
+  int64_t upd_base;                       /* offset of update slot 0 (= slots * slot_bytes) */
+  int64_t total_bytes;
+} b2rl_serve_layout;
+
+/* The layout of a ring for a replay with these fields (host arithmetic only, no CUDA call): the slot geometry
+ * the ReplayServer's `BATCH` blobs carry, APE_X/ReplayServer.py:65-114. */
+int b2rl_serve_layout_init(int64_t batch, int32_t slots, int32_t n_fields, const int64_t* field_bytes,
+                           b2rl_serve_layout* out);
+/* ReplayServer.__init__ (APE_X/ReplayServer.py:20-39): allocate the ring for replay `h` on h's device (headers
+ * zeroed).  Every field must be a bulk row (a multiple of 16 bytes, >= 1024) or a 1/2/4/8-byte scalar. */
+int b2rl_serve_ring_create(b2rl_replay* h, int64_t batch, int32_t slots, b2rl_serve_ring** out);
+/* The ring's layout (what a learner needs besides the IPC handle to open it; APE_X/ReplayMemory.py:170-186). */
+int b2rl_serve_ring_layout(const b2rl_serve_ring* r, b2rl_serve_layout* out);
+/* cudaIpcGetMemHandle of the ring's allocation: B2RL_IPC_HANDLE_BYTES bytes to handle_out (stands in for the
+ * Redis connection the consumer opens, APE_X/ReplayMemory.py:170-186). */
+int b2rl_serve_ring_export(const b2rl_serve_ring* r, void* handle_out);
+/* Replay_Server.__init__ (APE_X/ReplayMemory.py:170-186), learner side: map an exported ring into this process
+ * on `device` (cudaIpcOpenMemHandle with lazy peer access: the server may sit on another GPU).  `layout` must be
+ * the server's; it is checked against the arithmetic of b2rl_serve_layout_init.  Release with
+ * b2rl_serve_ring_close; a ring made by b2rl_serve_ring_create is released with b2rl_serve_ring_destroy. */
+int b2rl_serve_ring_open(const void* handle, const b2rl_serve_layout* layout, int32_t device, b2rl_serve_ring** out);
+int b2rl_serve_ring_close(b2rl_serve_ring* r);
+int b2rl_serve_ring_destroy(b2rl_serve_ring* r);
+/* Device pointers of slot k's arrays (the members of one `BATCH` blob, APE_X/ReplayServer.py:95-114, and of one
+ * `update` entry, :41-63), valid in this process: batch_out[0..2+n_fields] = {header, idx, w, field 0, ...},
+ * update_out[0..2] = {header, idx, prio}.  Either may be NULL. */
+int b2rl_serve_slot_ptrs(const b2rl_serve_ring* r, int32_t slot, void** batch_out, void** update_out);
+/* ReplayServer.buffer (APE_X/ReplayServer.py:65-114) for one minibatch, in ONE launch: B draws from h's
+ * device-resident Philox stream with the descent and IS-weight arithmetic of b2rl_tree_sample_fetch (the
+ * counter advances by B), idx / w / scalar fields written by the drawing threads, the bulk rows copied HBM ->
+ * SMEM -> slot with TMA bulk copies as b2rl_replay_gather does, and the header {seq, B} written last.  The slot
+ * equals b2rl_tree_sample_fetch + b2rl_replay_gather from the same RNG state, bit for bit.  max_w_dev: as for
+ * b2rl_tree_sample. */
+int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, uint64_t seq, float beta,
+                    const float* max_w_dev, void* stream);
+/* Replay_Server.sample (APE_X/ReplayMemory.py:251-257) without the unpickle: copy minibatch slot k (slot_bytes,
+ * header included) to dst_dev with one cudaMemcpyAsync on `stream` (a peer copy when the ring is on another GPU). */
+int b2rl_serve_take(const b2rl_serve_ring* r, int32_t slot, void* dst_dev, void* stream);
+/* Replay_Server.update (APE_X/ReplayMemory.py:188-190, flushed to `update` at :241-249): write n <= B (idx,
+ * priority) pairs and the header {seq, n} into update slot j, one launch on `stream`. */
+int b2rl_serve_put_update(b2rl_serve_ring* r, int32_t slot, uint64_t seq, const int64_t* idx_dev,
+                          const float* prio_dev, int64_t n, void* stream);
+
 /* Number of kernels this library has launched in this process (bench.py's
  * `gpu_launches`). */
 int64_t b2rl_launch_count(void);

@@ -1,0 +1,200 @@
+"""Stand-alone replay server transports, Ape-X at batch B: served minibatches/s and learner steps/s for
+  redis   ReplayServer -> pickled `BATCH` list -> Replay_Server (host arrays, copied to the device by train())
+  ring    DeviceReplayServer -> device serve ring (CUDA IPC) -> DeviceReplayClient
+  fused   the in-process learner: Learner.fused_step() on its own replay (no server)
+
+    python tools/bench_serve.py [--slots-store 65536] [--batch 512] [--steps 200] [--warmup 20] [--repeats 3]
+
+The server runs in a `spawn` child on --server-device, the learner here on cuda:0; the control plane is a Redis
+server (--redis HOST) or, by default, the in-memory Redis stand-in of the tests hosted by a multiprocessing manager
+(tests/shared_redis.py).  The stand-in moves the Redis-pickle arm's 29 MB minibatches through a Python socket and is
+much slower than a Redis server: that arm is then a lower bound, not a representative baseline.  With both processes on ONE GPU
+they share its SMs, so the served figures are a lower bound for a server with a GPU of its own.  Timings: host
+clock around `steps` iterations that end in a device synchronise, after `warmup` iterations; every arm is repeated
+`repeats` times in alternation and each run is reported.  Prints one JSON line."""
+from __future__ import annotations
+
+import argparse
+import json
+import multiprocessing as mp
+import os
+import pickle
+import subprocess
+import sys
+import time
+
+REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+for p in (REPO, os.path.join(REPO, "tests")):
+    if p not in sys.path:
+        sys.path.insert(0, p)
+
+from shared_redis import RedisManager, Shim  # noqa: E402
+
+
+def _connect(args, proxy):
+    """The control plane: a Redis server when --redis HOST is given, else the manager-hosted stand-in."""
+    if args["redis"]:
+        import redis
+        return redis.StrictRedis(host=args["redis"], port=6379)
+    return Shim(proxy)
+
+
+def _cfg(args, device):
+    from distributed_rl_b200 import apex
+    return apex.ApexConfig(BATCHSIZE=args["batch"], REPLAY_MEMORY_LEN=args["store"], BUFFER_SIZE=0,
+                           LEARNER_DEVICE=device)
+
+
+def _fill(store, n):
+    import torch
+    store.fill_hash(n, seed=0xB200)
+    store.build(torch.rand(n, generator=torch.Generator().manual_seed(0)).to(store.device) + 1e-3)
+
+
+def _server_main(kind, proxy, args, stop):
+    """Serve until `stop`: the ring server keeps its slots full; the Redis server keeps <= 8 pickled batches queued."""
+    from distributed_rl_b200.replay_server import DeviceReplayServer, ReplayServer
+    conn = _connect(args, proxy)
+    cfg = _cfg(args, args["server_device"])
+    if kind == "ring":
+        srv = DeviceReplayServer(cfg, conn, slots=args["ring_slots"])
+        _fill(srv.store, args["store"])
+        while not stop.is_set():
+            st = srv.serve_once()
+            if not (st["filled"] or st["released"] or st["updates_applied"]):
+                time.sleep(0.0002)
+        srv.close()
+    else:
+        srv = ReplayServer(cfg, conn, conn, m=1)
+        _fill(srv.store, args["store"])
+        conn.set("SERVE_STATS", pickle.dumps((args["store"], 1.0)))
+        while not stop.is_set():
+            busy = srv.update()
+            if conn.llen("BATCH") < 8:
+                srv.buffer()
+                busy = True
+            if not busy:
+                time.sleep(0.0002)
+
+
+def _timed(fn, steps, warmup, dev):
+    import torch
+    for _ in range(warmup):
+        fn()
+    torch.cuda.synchronize(dev)
+    t0 = time.perf_counter()
+    for _ in range(steps):
+        fn()
+    torch.cuda.synchronize(dev)
+    return steps / (time.perf_counter() - t0)
+
+
+def _served_arm(kind, args):
+    import torch
+    from distributed_rl_b200 import apex
+    from distributed_rl_b200.replay_server import DeviceReplayClient, Replay_Server
+    ctx = mp.get_context("spawn")
+    mgr = RedisManager(ctx=ctx)
+    mgr.start()
+    stop, child, client = ctx.Event(), None, None
+    dev = torch.device("cuda:0")
+    try:
+        proxy = mgr.Redis()
+        conn = _connect(args, proxy)
+        child = ctx.Process(target=_server_main, args=(kind, proxy, args, stop))
+        child.start()
+        cfg = _cfg(args, "cuda:0")
+        cfg.CUDNN_BENCHMARK = True
+        if kind == "ring":
+            client = DeviceReplayClient(cfg, conn, timeout=300.0)
+        else:
+            client = Replay_Server(cfg, conn, conn)
+            client.start()
+        L = apex.Learner(cfg, connect=None, start_replay=False, memory=client)
+
+        def next_batch():
+            while (b := client.sample()) is False:
+                time.sleep(0.0001)
+            return b
+
+        def serve_only():
+            b = next_batch()
+            if kind == "redis":          # what train() would do first: the batch onto the device
+                b[0] = torch.as_tensor(b[0]).to(dev, non_blocking=True)
+                b[3] = torch.as_tensor(b[3]).to(dev, non_blocking=True)
+
+        def step():
+            b = next_batch()
+            info, prio, idx, _ = L.train(b)
+            client.update(idx if kind == "ring" else list(idx.tolist()), prio)
+        served = _timed(serve_only, args["steps"], args["warmup"], dev)
+        steps = _timed(step, args["steps"], args["warmup"], dev)
+        return {"served_minibatches_per_s": served, "learner_steps_per_s": steps}
+    finally:
+        stop.set()
+        if client is not None:
+            client.stop()
+            if kind == "ring":
+                client.close()
+            else:
+                client.join(timeout=10)        # the polling thread must not outlive the manager
+        if child is not None:
+            child.join(timeout=60)
+            if child.is_alive():
+                child.terminate()
+                child.join()
+        mgr.shutdown()
+
+
+def _fused_arm(args):
+    import torch
+    from distributed_rl_b200 import apex
+    cfg = _cfg(args, "cuda:0")
+    L = apex.Learner(cfg, connect=None, start_replay=False)
+    _fill(L.memory.store, args["store"])
+    rate = _timed(L.fused_step, args["steps"], args["warmup"], torch.device("cuda:0"))
+    del L
+    torch.cuda.empty_cache()
+    return {"served_minibatches_per_s": None, "learner_steps_per_s": rate}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--slots-store", type=int, default=65536, help="replay slots (2^16 = 3.7 GB)")
+    ap.add_argument("--batch", type=int, default=512)
+    ap.add_argument("--ring-slots", type=int, default=4)
+    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--repeats", type=int, default=3)
+    ap.add_argument("--server-device", default="cuda:0")
+    ap.add_argument("--arms", default="redis,ring,fused")
+    ap.add_argument("--redis", default=None, help="host of a Redis server for the control plane (default: an "
+                    "in-memory stand-in in a manager process, which makes the Redis-pickle arm far slower than a "
+                    "Redis server would)")
+    a = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        sys.exit("bench_serve.py measures on a CUDA device; none is available")
+    args = {"store": a.slots_store, "batch": a.batch, "ring_slots": a.ring_slots, "steps": a.steps,
+            "warmup": a.warmup, "server_device": a.server_device, "redis": a.redis}
+    runs = {k: [] for k in a.arms.split(",")}
+    for _ in range(a.repeats):
+        for k in runs:
+            runs[k].append(_fused_arm(args) if k == "fused" else _served_arm(k, args))
+            print(json.dumps({"arm": k, **runs[k][-1]}), file=sys.stderr, flush=True)
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+    except Exception:
+        q = []
+    same = a.server_device == "cuda:0"
+    print(json.dumps({"workload": "apex_serve", "batch": a.batch, "store_slots": a.slots_store,
+                      "server_device": a.server_device, "learner_device": "cuda:0",
+                      "control_plane": f"redis://{a.redis}" if a.redis else "in-memory stand-in (manager process)",
+                      "note": "server and learner share one GPU: served figures are a lower bound" if same else
+                      "server and learner on separate GPUs",
+                      "gpus": q, "runs": runs}))
+
+
+if __name__ == "__main__":
+    main()
