@@ -1,0 +1,137 @@
+// TMA row copy shared by k_gather_bulk (gather.cu) and k_serve_fill (serve.cu): whole replay rows of the bulk
+// fields go HBM -> SMEM -> HBM through the TMA engine's 1-D bulk copies, driven by one thread over a ring of
+// shared-memory stages.  The SMs only issue descriptors; the payload never touches the register file.
+//
+// Work item = (draw k, field, chunk); a chunk is at most CHUNK bytes of one row, and items are numbered
+// draw-major, then field, then chunk.  The driving thread keeps a ring of BULK_RING_BYTES / CHUNK stages:
+//   load(item) : cp.async.bulk global -> smem, completes on mbarrier[stage]
+//   store(item): cp.async.bulk smem -> global (bulk_group)
+// and refills the stage of item t - LAG once all but the newest LAG store groups have finished reading SMEM.
+#pragma once
+#include "common.cuh"
+#include "hopper.cuh"
+
+namespace b2rl {
+
+constexpr int BULK_RING_BYTES = 229376;   // 224 KiB of dynamic shared memory per CTA; stages = BULK_RING_BYTES / CHUNK
+
+// A field is copied as bulk rows when its row is at least 1 KiB and a whole number of 16-byte units (the
+// granularity of a bulk copy); smaller rows cost more in descriptors than they move.
+inline bool is_bulk_row(int64_t row_bytes) { return row_bytes >= 1024 && row_bytes % 16 == 0; }
+
+__host__ __device__ __forceinline__ int64_t clamp_row(int64_t r, int64_t capacity) {
+  return r < 0 ? 0 : (r >= capacity ? capacity - 1 : r);
+}
+
+struct BulkField {
+  const uint8_t* src;   // replay field base
+  uint8_t* dst;         // output base
+  int64_t row_bytes;    // is_bulk_row
+  int32_t chunks;       // ceil(row_bytes / CHUNK)
+  int32_t pad;
+};
+
+struct BulkRows {
+  BulkField f[B2RL_MAX_FIELDS];
+  int64_t items_per_row;   // sum of chunks over the fields
+  int32_t n;               // fields
+  int32_t pad;
+
+  void add(const uint8_t* src, uint8_t* dst, int64_t row_bytes, int chunk) {
+    f[n] = BulkField{src, dst, row_bytes, (int32_t)((row_bytes + chunk - 1) / chunk), 0};
+    items_per_row += f[n].chunks;
+    ++n;
+  }
+};
+
+// Walks a contiguous range of items without divisions; `row` is the replay row of draw k.
+template <int CHUNK>
+struct ItemCursor {
+  int64_t k, row;
+  int32_t f, c;
+  template <class RowOf>
+  __device__ __forceinline__ void init(const BulkRows& T, const RowOf& row_of, int64_t item) {
+    k = item / T.items_per_row;
+    int32_t r = (int32_t)(item - k * T.items_per_row);
+    f = 0;
+    while (r >= T.f[f].chunks) { r -= T.f[f].chunks; ++f; }
+    c = r;
+    row = row_of(k);
+  }
+  __device__ __forceinline__ void get(const BulkRows& T, int64_t dst_k0, const uint8_t*& src, uint8_t*& dst,
+                                      uint32_t& bytes) const {
+    const int64_t off = (int64_t)c * CHUNK;
+    const int64_t rem = T.f[f].row_bytes - off;
+    bytes = (uint32_t)(rem < CHUNK ? rem : CHUNK);
+    src = T.f[f].src + row * T.f[f].row_bytes + off;
+    dst = T.f[f].dst + (dst_k0 + k) * T.f[f].row_bytes + off;
+  }
+  template <class RowOf>
+  __device__ __forceinline__ void next(const BulkRows& T, const RowOf& row_of, bool more) {
+    if (++c == T.f[f].chunks) {
+      c = 0;
+      if (++f == T.n) {
+        f = 0;
+        ++k;
+        if (more) row = row_of(k);
+      }
+    }
+  }
+};
+
+// Run by ONE thread of the CTA, which needs BULK_RING_BYTES of dynamic shared memory: copies items
+// [first, first + items) of table T (items >= 1).  Draw k reads replay row row_of(k) and writes output row
+// dst_k0 + k.
+template <int CHUNK, int LAG, class RowOf>
+__device__ __forceinline__ void copy_rows(const BulkRows& T, const RowOf& row_of, int64_t dst_k0, int64_t first,
+                                          int64_t items) {
+  constexpr int STAGES = BULK_RING_BYTES / CHUNK;
+  static_assert(STAGES <= 32 && STAGES > LAG + 1, "ring geometry");
+  extern __shared__ __align__(128) uint8_t smem[];
+  __shared__ __align__(8) uint64_t bar[STAGES];
+  for (int s = 0; s < STAGES; ++s) sm90::mbar_init(&bar[s], 1);
+  sm90::mbar_init_fence();
+
+  uint32_t phase_bits = 0;  // bit s = parity to wait for on stage s
+  ItemCursor<CHUNK> ld, stc;   // load cursor runs ahead of the store cursor
+  ld.init(T, row_of, first);
+  stc = ld;
+  int64_t loaded = 0;
+  // prologue: fill the ring
+  const int64_t pre = items < STAGES ? items : STAGES;
+  for (; loaded < pre; ++loaded) {
+    const uint8_t* src; uint8_t* dst; uint32_t bytes;
+    ld.get(T, dst_k0, src, dst, bytes);
+    sm90::mbar_expect_tx(&bar[loaded], bytes);
+    sm90::bulk_g2s(smem + (size_t)loaded * CHUNK, src, bytes, &bar[loaded]);
+    ld.next(T, row_of, loaded + 1 < items);
+  }
+  int s = 0;            // stage of item t
+  int rs = 0;           // stage to recycle next (item t - LAG)
+  for (int64_t t = 0; t < items; ++t) {
+    const uint8_t* src; uint8_t* dst; uint32_t bytes;
+    stc.get(T, dst_k0, src, dst, bytes);
+    sm90::mbar_wait(&bar[s], (phase_bits >> s) & 1u);
+    phase_bits ^= (1u << s);
+    sm90::bulk_s2g(dst, smem + (size_t)s * CHUNK, bytes);
+    sm90::bulk_commit();
+    stc.next(T, row_of, t + 1 < items);
+    if (++s == STAGES) s = 0;
+    // refill the stage used LAG items ago once its store has drained SMEM
+    if (t >= LAG) {
+      if (loaded < items) {
+        sm90::bulk_wait_read<LAG>();   // all but the newest LAG store groups have finished reading SMEM
+        const uint8_t* nsrc; uint8_t* ndst; uint32_t nbytes;
+        ld.get(T, dst_k0, nsrc, ndst, nbytes);
+        sm90::mbar_expect_tx(&bar[rs], nbytes);
+        sm90::bulk_g2s(smem + (size_t)rs * CHUNK, nsrc, nbytes, &bar[rs]);
+        ++loaded;
+        ld.next(T, row_of, loaded < items);
+      }
+      if (++rs == STAGES) rs = 0;
+    }
+  }
+  sm90::bulk_wait_all();
+}
+
+}  // namespace b2rl

@@ -56,6 +56,28 @@ struct DeviceGuard {
   int target = -1;
 };
 
+// Multiprocessor count of device `dev`, queried once per device.
+inline cudaError_t sm_count(int dev, int* out) {
+  static int sms[64] = {0};
+  if (!sms[dev & 63]) {
+    const cudaError_t e = cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) return e;
+  }
+  *out = sms[dev & 63];
+  return cudaSuccess;
+}
+
+// Lets kernel K use `bytes` of dynamic shared memory on device `dev` (beyond the default 48 KiB); the attribute
+// is set once per kernel and device.
+template <auto K>
+cudaError_t set_max_dynamic_smem(int dev, size_t bytes) {
+  static bool done[64] = {false};
+  if (done[dev & 63]) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (e == cudaSuccess) done[dev & 63] = true;
+  return e;
+}
+
 // ---- device helpers --------------------------------------------------------
 
 // x^e for fp32 operands: evaluated in fp64, rounded once ("powcr", DESIGN.md §3).

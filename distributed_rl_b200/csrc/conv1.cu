@@ -317,16 +317,11 @@ extern "C" int b2rl_conv1_pack_jobs(const float* const* w_dev, const int32_t* ne
 
 template <int N_NETS, int C_OUT>
 static cudaError_t conv1_launch(const conv1::Params& P, unsigned grid, cudaStream_t st) {
-  static bool attr[64] = {false};
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess)
+    e = set_max_dynamic_smem<conv1::k_conv1_fused<N_NETS, C_OUT>>(dev, conv1::smem_bytes<N_NETS, C_OUT>());
   if (e != cudaSuccess) return e;
-  if (!attr[dev & 63]) {
-    e = cudaFuncSetAttribute(conv1::k_conv1_fused<N_NETS, C_OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)conv1::smem_bytes<N_NETS, C_OUT>());
-    if (e != cudaSuccess) return e;
-    attr[dev & 63] = true;
-  }
   conv1::k_conv1_fused<N_NETS, C_OUT><<<grid, conv1::THREADS, conv1::smem_bytes<N_NETS, C_OUT>(), st>>>(P);
   return cudaSuccess;
 }
@@ -344,11 +339,11 @@ extern "C" int b2rl_conv1_fused(const uint8_t* frames_dev, int64_t capacity, con
                "frames, packed weights and output must be 16-byte aligned");
   int dev = 0;
   B2RL_CUDA(cudaGetDevice(&dev));
-  static int sms[64] = {0};
-  if (!sms[dev & 63]) B2RL_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
+  int sms = 0;
+  B2RL_CUDA(sm_count(dev, &sms));
   conv1::Params P{frames_dev, idx_dev, n, capacity, bq_dev, scale_dev, out_dev, relu};
   const int64_t units = n * conv1::TILES;
-  const unsigned grid = (unsigned)((units < sms[dev & 63]) ? units : sms[dev & 63]);
+  const unsigned grid = (unsigned)((units < sms) ? units : sms);
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e;
   if (c_out == 32) e = (n_nets == 1) ? conv1_launch<1, 32>(P, grid, st) : conv1_launch<2, 32>(P, grid, st);

@@ -336,16 +336,10 @@ using namespace b2rl;
 
 template <int C_OUT>
 static cudaError_t wgrad_launch(const conv1w::Params& P, unsigned grid, cudaStream_t st) {
-  static bool attr[64] = {false};
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = set_max_dynamic_smem<conv1w::k_conv1_wgrad<C_OUT>>(dev, conv1w::smem_bytes<C_OUT>());
   if (e != cudaSuccess) return e;
-  if (!attr[dev & 63]) {
-    e = cudaFuncSetAttribute(conv1w::k_conv1_wgrad<C_OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)conv1w::smem_bytes<C_OUT>());
-    if (e != cudaSuccess) return e;
-    attr[dev & 63] = true;
-  }
   conv1w::k_conv1_wgrad<C_OUT><<<grid, conv1w::THREADS, conv1w::smem_bytes<C_OUT>(), st>>>(P);
   return cudaSuccess;
 }
@@ -353,7 +347,7 @@ static cudaError_t wgrad_launch(const conv1w::Params& P, unsigned grid, cudaStre
 extern "C" int64_t b2rl_conv1_wgrad_workspace_floats(int32_t c_out) {
   int dev = 0, sms = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return -1;
-  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return -1;
+  if (sm_count(dev, &sms) != cudaSuccess) return -1;
   return (int64_t)sms * c_out * conv1w::E_TOTAL;
 }
 
@@ -368,18 +362,18 @@ extern "C" int b2rl_conv1_wgrad(const uint8_t* frames_dev, int64_t capacity, con
                "frames, gy and y must be 16-byte aligned");
   int dev = 0;
   B2RL_CUDA(cudaGetDevice(&dev));
-  static int sms[64] = {0};
-  if (!sms[dev & 63]) B2RL_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
+  int sms = 0;
+  B2RL_CUDA(sm_count(dev, &sms));
   cudaStream_t st = (cudaStream_t)stream;
   const int numel = c_out * conv1w::E_TOTAL;
-  const int64_t per_launch = (int64_t)sms[dev & 63] * conv1w::MAX_ITEMS_PER_CTA;   // int32 accumulator bound
+  const int64_t per_launch = (int64_t)sms * conv1w::MAX_ITEMS_PER_CTA;   // int32 accumulator bound
   for (int64_t off = 0; off < n; off += per_launch) {
     const int64_t m = (n - off < per_launch) ? n - off : per_launch;
     conv1w::Params P{frames_dev, idx_dev ? idx_dev + off : nullptr, m, capacity,
                      gy_dev + off * (int64_t)(conv1w::POS * c_out),
                      y_relu_dev ? y_relu_dev + off * (int64_t)(conv1w::POS * c_out) : nullptr, workspace_dev};
     if (!idx_dev) P.frames = frames_dev + off * conv1w::FRAME_BYTES, P.capacity = capacity - off;
-    const unsigned grid = (unsigned)((m < sms[dev & 63]) ? m : sms[dev & 63]);
+    const unsigned grid = (unsigned)((m < sms) ? m : sms);
     B2RL_CUDA(c_out == 32 ? wgrad_launch<32>(P, grid, st) : wgrad_launch<16>(P, grid, st));
     count_launch();
     B2RL_CHECK_LAUNCH();

@@ -4,59 +4,12 @@
 // Replaces Replay.buffer's deepcopy + pickle.loads + np.stack
 // (APE_X/ReplayMemory.py:61-116, baseline/PER.py:113) — the dominant CPU cost
 // of the reference path (SURVEY.md §3.1).
-#include "common.cuh"
+#include "bulk_rows.cuh"
 
 namespace b2rl {
 
 // ----------------------------------------------------------------------------
-// mbarrier / bulk-copy PTX wrappers (sm_90+; SASS: UBLKCP / SYNCS)
-// ----------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t}" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void bulk_s2g(void* gdst, const void* smem_src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst),
-               "r"(smem_u32(smem_src)), "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-// ----------------------------------------------------------------------------
-// Bulk gather.  Work item = (field, sample k, chunk c); a chunk is at most CHUNK
-// bytes of one row.  Thread 0 of each CTA drives a ring of GATHER_SMEM / CHUNK stages:
-//   load(item) : cp.async.bulk global -> smem, completes on mbarrier[stage]
-//   store(item): cp.async.bulk smem -> global (bulk_group)
-// The SMs only issue descriptors; the payload never touches the register file.
+// Bulk gather: the TMA row copy of bulk_rows.cuh over the minibatch, each CTA on a contiguous item range.
 // CHUNK = 14 KiB (half a frame stack, 16 stages) measured best: stores of the first
 // chunks overlap the loads of the later ones, and the single driving thread is not
 // yet issue-bound (8 KiB chunks were 10 % slower, 28 KiB chunks 2 % slower).
@@ -64,171 +17,70 @@ __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wa
 // the samples, so one launch assembles the whole minibatch.
 // ----------------------------------------------------------------------------
 constexpr int GATHER_THREADS = 64;
-constexpr int GATHER_SMEM = 229376;  // 224 KiB ring; stages = GATHER_SMEM / CHUNK
 
-struct GatherField {
+struct SmallField {
   const uint8_t* src;   // field base
   uint8_t* dst;         // output base
-  int64_t row_bytes;    // multiple of 16 for bulk fields
-  int32_t chunks;       // ceil(row_bytes / CHUNK)
-  int32_t pad;
+  int64_t row_bytes;
 };
 struct GatherParams {
-  GatherField f[B2RL_MAX_FIELDS];    // bulk (TMA) fields
-  GatherField s[B2RL_MAX_FIELDS];    // small fields, copied by warp 1
-  int32_t n_fields;
+  BulkRows bulk;                       // bulk (TMA) fields
+  SmallField s[B2RL_MAX_FIELDS];       // small fields, copied by warp 1
   int32_t n_small;
   int64_t n;            // samples
   int64_t capacity;
-  int64_t items_per_sample;  // sum of chunks over bulk fields
-  int64_t total_items;
+  int64_t total_items;  // bulk.items_per_row * n
 };
 
-// Walks the CTA's contiguous item range (sample-major, then field, then chunk) without divisions.
-template <int CHUNK>
-struct ItemCursor {
-  int64_t k, row;
-  int32_t f, c;
-  __device__ __forceinline__ void init(const GatherParams& P, const int64_t* __restrict__ idx, int64_t item) {
-    k = item / P.items_per_sample;
-    int32_t r = (int32_t)(item - k * P.items_per_sample);
-    f = 0;
-    while (r >= P.f[f].chunks) { r -= P.f[f].chunks; ++f; }
-    c = r;
-    row = clamp_row(P, idx[k]);
+template <typename U>
+__device__ __forceinline__ void gather_units(const U* __restrict__ src, U* __restrict__ dst, int64_t units_per_row,
+                                             const int64_t* __restrict__ idx, int64_t capacity, int64_t k0,
+                                             int64_t k1, int64_t u, int64_t step) {
+  for (u += k0 * units_per_row; u < k1 * units_per_row; u += step) {
+    const int64_t k = u / units_per_row, w = u - k * units_per_row;
+    dst[u] = src[clamp_row(idx[k], capacity) * units_per_row + w];
   }
-  static __device__ __forceinline__ int64_t clamp_row(const GatherParams& P, int64_t r) {
-    return r < 0 ? 0 : (r >= P.capacity ? P.capacity - 1 : r);
-  }
-  __device__ __forceinline__ void get(const GatherParams& P, const uint8_t*& src, uint8_t*& dst,
-                                      uint32_t& bytes) const {
-    const int64_t off = (int64_t)c * CHUNK;
-    const int64_t rem = P.f[f].row_bytes - off;
-    bytes = (uint32_t)(rem < CHUNK ? rem : CHUNK);
-    src = P.f[f].src + row * P.f[f].row_bytes + off;
-    dst = P.f[f].dst + k * P.f[f].row_bytes + off;
-  }
-  __device__ __forceinline__ void next(const GatherParams& P, const int64_t* __restrict__ idx, bool more) {
-    if (++c == P.f[f].chunks) {
-      c = 0;
-      if (++f == P.n_fields) {
-        f = 0;
-        ++k;
-        if (more) row = clamp_row(P, idx[k]);
-      }
-    }
-  }
-};
+}
+
+// Rows [k0, k1) of a small field's output <- their clamped replay rows, in 4-byte words when the row is a whole
+// number of words, else in bytes.  The caller's threads take units u, u + step, ... of the range.
+__device__ __forceinline__ void gather_small_rows(const uint8_t* src, uint8_t* dst, int64_t row_bytes,
+                                                  const int64_t* __restrict__ idx, int64_t capacity, int64_t k0,
+                                                  int64_t k1, int64_t u, int64_t step) {
+  if ((row_bytes & 3) == 0)
+    gather_units(reinterpret_cast<const uint32_t*>(src), reinterpret_cast<uint32_t*>(dst), row_bytes >> 2, idx,
+                 capacity, k0, k1, u, step);
+  else
+    gather_units(src, dst, row_bytes, idx, capacity, k0, k1, u, step);
+}
 
 template <int CHUNK, int LAG>
 __global__ void __launch_bounds__(GATHER_THREADS, 1)
 k_gather_bulk(const __grid_constant__ GatherParams P, const int64_t* __restrict__ idx) {
-  constexpr int STAGES = GATHER_SMEM / CHUNK;
-  static_assert(STAGES <= 32 && STAGES > LAG + 1, "ring geometry");
-  extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ __align__(8) uint64_t bar[STAGES];
-
   if (threadIdx.x >= 32) {
     // ---- warp 1: scalar fields of samples [k0, k1) ------------------------------------
-    const int lane = threadIdx.x - 32;
     const int64_t per = (P.n + gridDim.x - 1) / gridDim.x;
     const int64_t k0 = (int64_t)blockIdx.x * per;
     const int64_t k1 = (k0 + per < P.n) ? k0 + per : P.n;
-    for (int f = 0; f < P.n_small; ++f) {
-      const int64_t rb = P.s[f].row_bytes;
-      if ((rb & 3) == 0) {
-        const int64_t words = rb >> 2;
-        for (int64_t u = lane; u < (k1 - k0) * words; u += 32) {
-          const int64_t k = k0 + u / words, w = u % words;
-          int64_t row = idx[k];
-          row = row < 0 ? 0 : (row >= P.capacity ? P.capacity - 1 : row);
-          reinterpret_cast<uint32_t*>(P.s[f].dst)[k * words + w] =
-              reinterpret_cast<const uint32_t*>(P.s[f].src)[row * words + w];
-        }
-      } else {
-        for (int64_t u = lane; u < (k1 - k0) * rb; u += 32) {
-          const int64_t k = k0 + u / rb, b = u % rb;
-          int64_t row = idx[k];
-          row = row < 0 ? 0 : (row >= P.capacity ? P.capacity - 1 : row);
-          P.s[f].dst[k * rb + b] = P.s[f].src[row * rb + b];
-        }
-      }
-    }
+    for (int f = 0; f < P.n_small; ++f)
+      gather_small_rows(P.s[f].src, P.s[f].dst, P.s[f].row_bytes, idx, P.capacity, k0, k1, threadIdx.x - 32, 32);
     return;
   }
-  if (threadIdx.x != 0 || P.total_items == 0) return;  // a single thread drives the copy engine
-  for (int s = 0; s < STAGES; ++s) mbar_init(&bar[s], 1);
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-
+  if (threadIdx.x != 0) return;  // a single thread drives the copy engine
   // items of this CTA: a contiguous range, so consecutive items share idx[] cache lines
   const int64_t per_cta = (P.total_items + gridDim.x - 1) / gridDim.x;
   const int64_t first = (int64_t)blockIdx.x * per_cta;
   if (first >= P.total_items) return;
   const int64_t my_items = (P.total_items - first < per_cta) ? P.total_items - first : per_cta;
-  uint32_t phase_bits = 0;  // bit s = parity to wait for on stage s
-
-  ItemCursor<CHUNK> ld, stc;   // load cursor runs ahead of the store cursor
-  ld.init(P, idx, first);
-  stc = ld;
-  int64_t loaded = 0;
-  // prologue: fill the ring
-  const int64_t pre = my_items < STAGES ? my_items : STAGES;
-  for (; loaded < pre; ++loaded) {
-    const uint8_t* src; uint8_t* dst; uint32_t bytes;
-    ld.get(P, src, dst, bytes);
-    mbar_expect_tx(&bar[loaded], bytes);
-    bulk_g2s(smem + (size_t)loaded * CHUNK, src, bytes, &bar[loaded]);
-    ld.next(P, idx, loaded + 1 < my_items);
-  }
-  int s = 0;            // stage of item t
-  int rs = 0;           // stage to recycle next (item t - LAG)
-  for (int64_t t = 0; t < my_items; ++t) {
-    const uint8_t* src; uint8_t* dst; uint32_t bytes;
-    stc.get(P, src, dst, bytes);
-    mbar_wait(&bar[s], (phase_bits >> s) & 1u);
-    phase_bits ^= (1u << s);
-    bulk_s2g(dst, smem + (size_t)s * CHUNK, bytes);
-    bulk_commit();
-    stc.next(P, idx, t + 1 < my_items);
-    if (++s == STAGES) s = 0;
-    // refill the stage used LAG items ago once its store has drained SMEM
-    if (t >= LAG) {
-      if (loaded < my_items) {
-        bulk_wait_read<LAG>();   // all but the newest LAG store groups have finished reading SMEM
-        const uint8_t* nsrc; uint8_t* ndst; uint32_t nbytes;
-        ld.get(P, nsrc, ndst, nbytes);
-        mbar_expect_tx(&bar[rs], nbytes);
-        bulk_g2s(smem + (size_t)rs * CHUNK, nsrc, nbytes, &bar[rs]);
-        ++loaded;
-        ld.next(P, idx, loaded < my_items);
-      }
-      if (++rs == STAGES) rs = 0;
-    }
-  }
-  bulk_wait_all();
+  copy_rows<CHUNK, LAG>(P.bulk, [&](int64_t k) { return clamp_row(idx[k], P.capacity); }, 0, first, my_items);
 }
 
 // Generic fallback / small fields: one thread per (sample, 4-byte word or byte).
 __global__ void __launch_bounds__(256)
 k_gather_small(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int64_t row_bytes,
                const int64_t* __restrict__ idx, int64_t n, int64_t capacity) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if ((row_bytes & 3) == 0) {
-    const int64_t words = row_bytes >> 2;
-    if (t >= n * words) return;
-    const int64_t k = t / words, w = t - k * words;
-    int64_t row = idx[k];
-    row = row < 0 ? 0 : (row >= capacity ? capacity - 1 : row);
-    reinterpret_cast<uint32_t*>(dst)[k * words + w] =
-        reinterpret_cast<const uint32_t*>(src)[row * words + w];
-  } else {
-    if (t >= n * row_bytes) return;
-    const int64_t k = t / row_bytes, b = t - k * row_bytes;
-    int64_t row = idx[k];
-    row = row < 0 ? 0 : (row >= capacity ? capacity - 1 : row);
-    dst[k * row_bytes + b] = src[row * row_bytes + b];
-  }
+  gather_small_rows(src, dst, row_bytes, idx, capacity, 0, n, (int64_t)blockIdx.x * blockDim.x + threadIdx.x,
+                    (int64_t)gridDim.x * blockDim.x);
 }
 
 // LDG.128/STG.128 reference implementation of the big-row gather (kept for the
@@ -238,8 +90,7 @@ k_gather_ldg(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int64_t
              const int64_t* __restrict__ idx, int64_t n, int64_t capacity) {
   const int64_t k = blockIdx.x;
   if (k >= n) return;
-  int64_t row = idx[k];
-  row = row < 0 ? 0 : (row >= capacity ? capacity - 1 : row);
+  const int64_t row = clamp_row(idx[k], capacity);
   const int4* s = reinterpret_cast<const int4*>(src + row * row_bytes);
   int4* d = reinterpret_cast<int4*>(dst + k * row_bytes);
   const int64_t nv = row_bytes >> 4;
@@ -316,28 +167,19 @@ extern "C" int b2rl_replay_gather(b2rl_replay* h, const int64_t* idx_dev, int64_
   GatherParams P{};
   P.n = n;
   P.capacity = h->capacity;
-  int nb = 0, ns = 0;
   for (int f = 0; f < h->n_fields; ++f) {
     uint8_t* out = (uint8_t*)out_fields_dev[f];
     if (out == nullptr) continue;
     const int64_t rb = h->field_bytes[f];
     const bool big = rb >= 1024;
-    const bool aligned16 = (rb % 16 == 0) && ((uintptr_t)out % 16 == 0) && ((uintptr_t)h->field[f] % 16 == 0);
-    if (big && aligned16 && gather_mode() == 0) {
-      P.f[nb].src = h->field[f];
-      P.f[nb].dst = out;
-      P.f[nb].row_bytes = rb;
-      P.f[nb].chunks = (int32_t)((rb + gather_chunk() - 1) / gather_chunk());
-      P.items_per_sample += P.f[nb].chunks;
-      ++nb;
-    } else if (big && aligned16) {
+    const bool bulk = is_bulk_row(rb) && ((uintptr_t)out % 16 == 0) && ((uintptr_t)h->field[f] % 16 == 0);
+    if (bulk && gather_mode() == 0) {
+      P.bulk.add(h->field[f], out, rb, gather_chunk());
+    } else if (bulk) {
       k_gather_ldg<<<(unsigned)n, 256, 0, st>>>(h->field[f], out, rb, idx_dev, n, h->capacity);
       count_launch();
     } else if (!big && ((rb % 4 != 0) || (((uintptr_t)out % 4 == 0) && ((uintptr_t)h->field[f] % 4 == 0)))) {
-      P.s[ns].src = h->field[f];
-      P.s[ns].dst = out;
-      P.s[ns].row_bytes = rb;
-      ++ns;
+      P.s[P.n_small++] = SmallField{h->field[f], out, rb};
     } else {
       const int64_t units = (rb % 4 == 0 && (uintptr_t)out % 4 == 0) ? n * (rb / 4) : n * rb;
       k_gather_small<<<(unsigned)((units + 255) / 256), 256, 0, st>>>(h->field[f], out, rb, idx_dev, n,
@@ -345,31 +187,21 @@ extern "C" int b2rl_replay_gather(b2rl_replay* h, const int64_t* idx_dev, int64_
       count_launch();
     }
   }
-  if (nb > 0 || ns > 0) {
-    P.n_fields = nb;
-    P.n_small = ns;
-    P.total_items = P.items_per_sample * n;
-    static int sms[64] = {0};
-    static bool attr_set[64] = {false};
+  if (P.bulk.n > 0 || P.n_small > 0) {
+    P.total_items = P.bulk.items_per_row * n;
     const int dev = h->device;
-    const size_t smem_bytes = (size_t)GATHER_SMEM;
-    if (!attr_set[dev & 63]) {
-      B2RL_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-      B2RL_CUDA(cudaFuncSetAttribute(k_gather_bulk<28672, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)smem_bytes));
-      B2RL_CUDA(cudaFuncSetAttribute(k_gather_bulk<14336, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)smem_bytes));
-      B2RL_CUDA(cudaFuncSetAttribute(k_gather_bulk<8192, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)smem_bytes));
-      attr_set[dev & 63] = true;
-    }
-    int64_t grid = sms[dev & 63];
+    int sms = 0;
+    B2RL_CUDA(sm_count(dev, &sms));
+    B2RL_CUDA((set_max_dynamic_smem<k_gather_bulk<28672, 1>>(dev, BULK_RING_BYTES)));
+    B2RL_CUDA((set_max_dynamic_smem<k_gather_bulk<14336, 3>>(dev, BULK_RING_BYTES)));
+    B2RL_CUDA((set_max_dynamic_smem<k_gather_bulk<8192, 6>>(dev, BULK_RING_BYTES)));
+    int64_t grid = sms;
     const int64_t work = P.total_items > n ? P.total_items : n;
     if (grid > work) grid = work;
     switch (gather_chunk()) {
-      case 28672: k_gather_bulk<28672, 1><<<(unsigned)grid, GATHER_THREADS, smem_bytes, st>>>(P, idx_dev); break;
-      case 8192:  k_gather_bulk<8192, 6><<<(unsigned)grid, GATHER_THREADS, smem_bytes, st>>>(P, idx_dev); break;
-      default:    k_gather_bulk<14336, 3><<<(unsigned)grid, GATHER_THREADS, smem_bytes, st>>>(P, idx_dev); break;
+      case 28672: k_gather_bulk<28672, 1><<<(unsigned)grid, GATHER_THREADS, BULK_RING_BYTES, st>>>(P, idx_dev); break;
+      case 8192:  k_gather_bulk<8192, 6><<<(unsigned)grid, GATHER_THREADS, BULK_RING_BYTES, st>>>(P, idx_dev); break;
+      default:    k_gather_bulk<14336, 3><<<(unsigned)grid, GATHER_THREADS, BULK_RING_BYTES, st>>>(P, idx_dev); break;
     }
     count_launch();
   }
@@ -397,6 +229,37 @@ extern "C" int b2rl_replay_fill_hash(b2rl_replay* h, int64_t n, uint32_t seed, v
   return publish_size(h, st);
 }
 
+// Record i of fields_src -> ring slot (start + i) % capacity, i < n; a NULL field is skipped.
+static int copy_ring_range(b2rl_replay* h, const void* const* fields_src, int64_t start, int64_t n,
+                           cudaStream_t st) {
+  const int64_t first = (start + n <= h->capacity) ? n : (h->capacity - start);  // before the wrap
+  for (int f = 0; f < h->n_fields; ++f) {
+    const uint8_t* src = (const uint8_t*)fields_src[f];
+    if (src == nullptr) continue;
+    const int64_t rb = h->field_bytes[f];
+    B2RL_CUDA(cudaMemcpyAsync(h->field[f] + start * rb, src, (size_t)(first * rb), cudaMemcpyDefault, st));
+    if (first < n)
+      B2RL_CUDA(cudaMemcpyAsync(h->field[f], src + first * rb, (size_t)((n - first) * rb), cudaMemcpyDefault, st));
+  }
+  return B2RL_OK;
+}
+
+// The n records at head become sampleable with the device priorities prios_dev; head moves past them.
+static int publish(b2rl_replay* h, const float* prios_dev, int64_t n, cudaStream_t st) {
+  h->size = (h->size + n > h->capacity) ? h->capacity : h->size + n;   // published by the update kernel itself
+  int rc = b2rl_tree_update_impl(h, nullptr, h->head, prios_dev, 0.0f, n, st, true);
+  if (rc != B2RL_OK) return rc;
+  h->head = (h->head + n) % h->capacity;
+  return B2RL_OK;
+}
+
+// The n slots at head are about to be overwritten: their records can no longer be sampled.
+static int retire(b2rl_replay* h, int64_t n, cudaStream_t st) {
+  const int64_t overwritten = h->size + n - h->capacity;
+  if (overwritten > 0) h->size -= overwritten;
+  return b2rl_tree_update_impl(h, nullptr, h->head, nullptr, 0.0f, n, st, overwritten > 0);
+}
+
 extern "C" int b2rl_replay_push(b2rl_replay* h, const void* const* fields_src, const float* prios,
                                 int64_t n, void* stream) {
   B2RL_REQUIRE(h != nullptr, "null handle");
@@ -406,23 +269,10 @@ extern "C" int b2rl_replay_push(b2rl_replay* h, const void* const* fields_src, c
   B2RL_REQUIRE(h->n_fields == 0 || fields_src != nullptr, "null fields");
   DeviceGuard g(h->device);
   cudaStream_t st = (cudaStream_t)stream;
-  const int64_t head = h->head;
-  const int64_t first = (head + n <= h->capacity) ? n : (h->capacity - head);  // before the wrap
-  for (int f = 0; f < h->n_fields; ++f) {
-    const uint8_t* src = (const uint8_t*)fields_src[f];
-    if (src == nullptr) continue;
-    const int64_t rb = h->field_bytes[f];
-    B2RL_CUDA(cudaMemcpyAsync(h->field[f] + head * rb, src, (size_t)(first * rb), cudaMemcpyDefault, st));
-    if (first < n)
-      B2RL_CUDA(cudaMemcpyAsync(h->field[f], src + first * rb, (size_t)((n - first) * rb),
-                                cudaMemcpyDefault, st));
-  }
-  B2RL_CUDA(cudaMemcpyAsync(h->scratch_val, prios, (size_t)n * sizeof(float), cudaMemcpyDefault, st));
-  h->size = (h->size + n > h->capacity) ? h->capacity : h->size + n;   // published by the update kernel itself
-  int rc = b2rl_tree_update_impl(h, nullptr, head, h->scratch_val, 0.0f, n, st, true);
+  int rc = copy_ring_range(h, fields_src, h->head, n, st);
   if (rc != B2RL_OK) return rc;
-  h->head = (head + n) % h->capacity;
-  return B2RL_OK;
+  B2RL_CUDA(cudaMemcpyAsync(h->scratch_val, prios, (size_t)n * sizeof(float), cudaMemcpyDefault, st));
+  return publish(h, h->scratch_val, n, st);
 }
 
 extern "C" int b2rl_replay_reserve(b2rl_replay* h, int64_t n, int64_t* start_slot, void* stream) {
@@ -430,9 +280,7 @@ extern "C" int b2rl_replay_reserve(b2rl_replay* h, int64_t n, int64_t* start_slo
   B2RL_REQUIRE(n >= 1 && n <= h->capacity, "n out of range (1..capacity)");
   B2RL_REQUIRE(h->reserved == 0, "a reservation is already pending (call b2rl_replay_commit first)");
   DeviceGuard g(h->device);
-  const int64_t overwritten = h->size + n - h->capacity;     // records that become unsampleable now
-  if (overwritten > 0) h->size -= overwritten;
-  int rc = b2rl_tree_update_impl(h, nullptr, h->head, nullptr, 0.0f, n, (cudaStream_t)stream, overwritten > 0);
+  int rc = retire(h, n, (cudaStream_t)stream);
   if (rc != B2RL_OK) return rc;
   h->reserved = n;
   if (start_slot) *start_slot = h->head;
@@ -444,17 +292,7 @@ extern "C" int b2rl_replay_copy_payload(b2rl_replay* h, const void* const* field
   B2RL_REQUIRE(h != nullptr && fields_src != nullptr, "null argument");
   B2RL_REQUIRE(n >= 1 && n <= h->capacity && start_slot >= 0 && start_slot < h->capacity, "range out of bounds");
   DeviceGuard g(h->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t first = (start_slot + n <= h->capacity) ? n : (h->capacity - start_slot);
-  for (int f = 0; f < h->n_fields; ++f) {
-    const uint8_t* src = (const uint8_t*)fields_src[f];
-    if (src == nullptr) continue;
-    const int64_t rb = h->field_bytes[f];
-    B2RL_CUDA(cudaMemcpyAsync(h->field[f] + start_slot * rb, src, (size_t)(first * rb), cudaMemcpyDefault, st));
-    if (first < n)
-      B2RL_CUDA(cudaMemcpyAsync(h->field[f], src + first * rb, (size_t)((n - first) * rb), cudaMemcpyDefault, st));
-  }
-  return B2RL_OK;
+  return copy_ring_range(h, fields_src, start_slot, n, (cudaStream_t)stream);
 }
 
 extern "C" int b2rl_replay_commit(b2rl_replay* h, const float* prios, int64_t n, void* stream) {
@@ -463,10 +301,8 @@ extern "C" int b2rl_replay_commit(b2rl_replay* h, const float* prios, int64_t n,
   DeviceGuard g(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   B2RL_CUDA(cudaMemcpyAsync(h->scratch_val, prios, (size_t)n * sizeof(float), cudaMemcpyDefault, st));
-  h->size = (h->size + n > h->capacity) ? h->capacity : h->size + n;
-  int rc = b2rl_tree_update_impl(h, nullptr, h->head, h->scratch_val, 0.0f, n, st, true);
+  int rc = publish(h, h->scratch_val, n, st);
   if (rc != B2RL_OK) return rc;
-  h->head = (h->head + n) % h->capacity;
   h->reserved = 0;
   return B2RL_OK;
 }
@@ -491,11 +327,8 @@ extern "C" int b2rl_replay_ingest_pipelined(b2rl_replay* h, const void* const* f
   if (h->pipe_n > 0) {                      // 1. publish the batch in flight
     B2RL_REQUIRE(h->reserved == h->pipe_n, "pipelined ingest mixed with reserve/commit");
     B2RL_CUDA(cudaStreamWaitEvent(st, h->ev_copied, 0));
-    const int64_t m = h->pipe_n;
-    h->size = (h->size + m > h->capacity) ? h->capacity : h->size + m;
-    int rc = b2rl_tree_update_impl(h, nullptr, h->head, h->pipe_prios, 0.0f, m, st, true);
+    int rc = publish(h, h->pipe_prios, h->pipe_n, st);
     if (rc != B2RL_OK) return rc;
-    h->head = (h->head + m) % h->capacity;
     h->reserved = 0;
     h->pipe_n = 0;
     // the copy stream must not overwrite pipe_prios before this update has read it
@@ -512,27 +345,15 @@ extern "C" int b2rl_replay_ingest_pipelined(b2rl_replay* h, const void* const* f
     B2RL_CUDA(cudaMalloc((void**)&h->pipe_prios, sizeof(float) * (size_t)n));
     h->pipe_cap = n;
   }
-  // 2. retire the slots about to be overwritten (they can no longer be sampled)
-  const int64_t overwritten = h->size + n - h->capacity;
-  if (overwritten > 0) h->size -= overwritten;
-  int rc = b2rl_tree_update_impl(h, nullptr, h->head, nullptr, 0.0f, n, st, overwritten > 0);
+  int rc = retire(h, n, st);                // 2. retire the slots about to be overwritten
   if (rc != B2RL_OK) return rc;
   h->reserved = n;
   h->pipe_n = n;
   // 3. payload + priorities on the copy stream, behind the retirement
   B2RL_CUDA(cudaEventRecord(h->ev_reserved, st));
   B2RL_CUDA(cudaStreamWaitEvent(h->ingest_stream, h->ev_reserved, 0));
-  const int64_t start = h->head;
-  const int64_t first = (start + n <= h->capacity) ? n : (h->capacity - start);
-  for (int f = 0; f < h->n_fields; ++f) {
-    const uint8_t* src = (const uint8_t*)fields_src[f];
-    if (src == nullptr) continue;
-    const int64_t rb = h->field_bytes[f];
-    B2RL_CUDA(cudaMemcpyAsync(h->field[f] + start * rb, src, (size_t)(first * rb), cudaMemcpyDefault, h->ingest_stream));
-    if (first < n)
-      B2RL_CUDA(cudaMemcpyAsync(h->field[f], src + first * rb, (size_t)((n - first) * rb), cudaMemcpyDefault,
-                                h->ingest_stream));
-  }
+  rc = copy_ring_range(h, fields_src, h->head, n, h->ingest_stream);
+  if (rc != B2RL_OK) return rc;
   B2RL_CUDA(cudaMemcpyAsync(h->pipe_prios, prios_src, (size_t)n * sizeof(float), cudaMemcpyDefault, h->ingest_stream));
   B2RL_CUDA(cudaEventRecord(h->ev_copied, h->ingest_stream));
   return B2RL_OK;

@@ -381,9 +381,7 @@ static int64_t gemm_splits(int64_t M, int64_t N, int64_t K, int sms) {
 static int gemm_sms(int* out) {
   int dev = 0;
   B2RL_CUDA(cudaGetDevice(&dev));
-  static int sms[64] = {0};
-  if (!sms[dev & 63]) B2RL_CUDA(cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-  *out = sms[dev & 63];
+  B2RL_CUDA(sm_count(dev, out));
   return B2RL_OK;
 }
 
@@ -403,12 +401,8 @@ extern "C" int b2rl_gemm_tf32x3(const float* a_packed_dev, const float* b_packed
   if (int rc = gemm_sms(&sms)) return rc;
   int dev = 0;
   B2RL_CUDA(cudaGetDevice(&dev));
-  static bool attr[64] = {false};
   const size_t smem_bytes = (size_t)gemm::STAGES * gemm::STAGE + 1024;
-  if (!attr[dev & 63]) {
-    B2RL_CUDA(cudaFuncSetAttribute(gemm::k_gemm_tf32x3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    attr[dev & 63] = true;
-  }
+  B2RL_CUDA(set_max_dynamic_smem<gemm::k_gemm_tf32x3>(dev, smem_bytes));
   const int64_t splits = gemm_splits(M, N, K, sms);
   B2RL_REQUIRE(splits == 1 || (workspace_dev && ((uintptr_t)workspace_dev % 16) == 0),
                "this shape splits K: pass b2rl_gemm_workspace_floats() floats of 16-byte aligned workspace");

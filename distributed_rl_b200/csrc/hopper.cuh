@@ -1,5 +1,5 @@
-// Hopper (sm_90a) primitives shared by the tensor-core kernels (conv1.cu, conv1_wgrad.cu, gemm.cu) and serve.cu:
-// mbarriers, TMA bulk copies, and warpgroup MMAs (wgmma) whose operands are read from shared memory
+// Hopper (sm_90a) primitives shared by the tensor-core kernels (conv1.cu, conv1_wgrad.cu, gemm.cu) and the TMA row
+// copy of bulk_rows.cuh (k_gather_bulk, k_serve_fill): mbarriers, TMA bulk copies, and warpgroup MMAs (wgmma) whose operands are read from shared memory
 // through matrix descriptors and whose accumulators live in the registers of the issuing warpgroup.
 #pragma once
 #include <stdint.h>

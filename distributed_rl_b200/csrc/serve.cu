@@ -4,8 +4,7 @@
 //
 // Replaces ReplayServer.buffer's sample -> gather -> .cpu() -> pickle -> RPUSH and Replay_Server.sample's
 // pickle.loads -> host-to-device copy (APE_X/ReplayServer.py:65-114, APE_X/ReplayMemory.py:251-257).
-#include "common.cuh"
-#include "hopper.cuh"
+#include "bulk_rows.cuh"
 #include "tree.cuh"
 
 #include <new>
@@ -13,44 +12,16 @@
 namespace b2rl {
 
 constexpr int SERVE_THREADS = 128;   // draws per CTA at most; warp 0's lane 0 then drives the copy engine
-constexpr int SERVE_CHUNK = 14336;   // as k_gather_bulk's default: half a frame stack per bulk copy
-constexpr int SERVE_STAGES = 16;     // 224 KiB ring of chunks
-constexpr int SERVE_LAG = 3;         // a stage is refilled once all but the newest LAG stores have drained it
-constexpr size_t SERVE_SMEM = (size_t)SERVE_CHUNK * SERVE_STAGES;
-
-struct ServeBulk {
-  const uint8_t* src[B2RL_MAX_FIELDS];   // replay field base
-  uint8_t* dst[B2RL_MAX_FIELDS];         // slot field base
-  int64_t bytes[B2RL_MAX_FIELDS];        // row bytes (multiple of 16)
-  int32_t chunks[B2RL_MAX_FIELDS];       // ceil(bytes / SERVE_CHUNK)
-  int32_t n;
-  int32_t items_per_draw;                // sum of chunks
-};
-
-// Work item t of a CTA (draw-major, then field, then chunk) -> source, destination, size.
-__device__ __forceinline__ void serve_item(const ServeBulk& P, const int64_t* s_row, int64_t k0, int64_t t,
-                                           const uint8_t*& src, uint8_t*& dst, uint32_t& bytes) {
-  const int64_t i = t / P.items_per_draw;
-  int32_t r = (int32_t)(t - i * P.items_per_draw);
-  int f = 0;
-  while (r >= P.chunks[f]) { r -= P.chunks[f]; ++f; }
-  const int64_t off = (int64_t)r * SERVE_CHUNK;
-  const int64_t rem = P.bytes[f] - off;
-  bytes = (uint32_t)(rem < SERVE_CHUNK ? rem : SERVE_CHUNK);
-  src = P.src[f] + s_row[i] * P.bytes[f] + off;
-  dst = P.dst[f] + (k0 + i) * P.bytes[f] + off;
-}
 
 // CTA c owns draws [c*per, (c+1)*per): its threads draw them (indices, weights, scalar fields), then thread 0
-// copies their bulk rows through the shared-memory ring, then the last CTA to finish writes the header.
+// copies their bulk rows with the TMA row copy of bulk_rows.cuh (k_gather_bulk's default geometry: 14 KiB chunks,
+// 16 stages, lag 3), then the last CTA to finish writes the header.
 __global__ void __launch_bounds__(SERVE_THREADS, 1)
-k_serve_fill(const __grid_constant__ TreeView t, const __grid_constant__ ServeBulk P, SmallFields small,
+k_serve_fill(const __grid_constant__ TreeView t, const __grid_constant__ BulkRows P, SmallFields small,
              uint64_t* __restrict__ rng_state, int64_t n, int64_t capacity, const float* __restrict__ n_valid_dev,
              float beta, const float* __restrict__ max_w_ext, int64_t* __restrict__ idx_out,
              float* __restrict__ w_out, uint64_t* __restrict__ header, uint64_t seq,
              unsigned int* __restrict__ done_ticket) {
-  extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ __align__(8) uint64_t bar[SERVE_STAGES];
   __shared__ int64_t s_row[SERVE_THREADS];
   const int tid = threadIdx.x;
   uint64_t seed, offset;
@@ -66,47 +37,11 @@ k_serve_fill(const __grid_constant__ TreeView t, const __grid_constant__ ServeBu
     fetch_small(small, j, k);
     const float s32 = (float)root;
     w_out[k] = is_weight(t, s32, __fdiv_rn((float)picked, s32), n_valid_dev, beta, max_w_ext);
-    s_row[tid] = j < 0 ? 0 : (j >= capacity ? capacity - 1 : j);   // the row b2rl_replay_gather would copy
-  }
-  if (tid == 0) {
-    for (int s = 0; s < SERVE_STAGES; ++s) sm90::mbar_init(&bar[s], 1);
-    sm90::mbar_init_fence();
+    s_row[tid] = clamp_row(j, capacity);   // the row b2rl_replay_gather would copy
   }
   __syncthreads();
-  if (tid == 0 && cnt > 0 && P.n > 0) {
-    const int64_t items = cnt * P.items_per_draw;
-    const int64_t pre = items < SERVE_STAGES ? items : SERVE_STAGES;
-    uint32_t phase_bits = 0;
-    int64_t loaded = 0;
-    for (; loaded < pre; ++loaded) {
-      const uint8_t* src; uint8_t* dst; uint32_t bytes;
-      serve_item(P, s_row, k0, loaded, src, dst, bytes);
-      sm90::mbar_expect_tx(&bar[loaded], bytes);
-      sm90::bulk_g2s(smem + (size_t)loaded * SERVE_CHUNK, src, bytes, &bar[loaded]);
-    }
-    int s = 0, rs = 0;
-    for (int64_t it = 0; it < items; ++it) {
-      const uint8_t* src; uint8_t* dst; uint32_t bytes;
-      serve_item(P, s_row, k0, it, src, dst, bytes);
-      sm90::mbar_wait(&bar[s], (phase_bits >> s) & 1u);
-      phase_bits ^= (1u << s);
-      sm90::bulk_s2g(dst, smem + (size_t)s * SERVE_CHUNK, bytes);
-      sm90::bulk_commit();
-      if (++s == SERVE_STAGES) s = 0;
-      if (it >= SERVE_LAG) {
-        if (loaded < items) {
-          sm90::bulk_wait_read<SERVE_LAG>();
-          const uint8_t* nsrc; uint8_t* ndst; uint32_t nbytes;
-          serve_item(P, s_row, k0, loaded, nsrc, ndst, nbytes);
-          sm90::mbar_expect_tx(&bar[rs], nbytes);
-          sm90::bulk_g2s(smem + (size_t)rs * SERVE_CHUNK, nsrc, nbytes, &bar[rs]);
-          ++loaded;
-        }
-        if (++rs == SERVE_STAGES) rs = 0;
-      }
-    }
-    sm90::bulk_wait_all();
-  }
+  if (tid == 0 && cnt > 0 && P.n > 0)
+    copy_rows<14336, 3>(P, [](int64_t i) { return s_row[i]; }, k0, 0, cnt * P.items_per_row);
   // header last: written by the last CTA to get here, after every CTA's copies have completed
   __syncthreads();
   if (tid == 0) {
@@ -185,7 +120,7 @@ extern "C" int b2rl_serve_ring_create(b2rl_replay* h, int64_t batch, int32_t slo
   B2RL_REQUIRE(h != nullptr && out != nullptr, "null argument");
   for (int f = 0; f < h->n_fields; ++f) {
     const int64_t b = h->field_bytes[f];
-    B2RL_REQUIRE((b % 16 == 0 && b >= 1024) || b == 1 || b == 2 || b == 4 || b == 8,
+    B2RL_REQUIRE(is_bulk_row(b) || b == 1 || b == 2 || b == 4 || b == 8,
                  "serve ring fields must be bulk rows (multiple of 16 B, >= 1024 B) or 1/2/4/8-byte scalars");
   }
   b2rl_serve_layout L;
@@ -310,18 +245,13 @@ extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot,
   void* ptrs[3 + B2RL_MAX_FIELDS];
   int rc = b2rl_serve_slot_ptrs(r, slot, ptrs, nullptr);
   if (rc != B2RL_OK) return rc;
-  ServeBulk P{};
+  BulkRows P{};
   SmallFields small{};
   for (int f = 0; f < h->n_fields; ++f) {
     const int64_t b = h->field_bytes[f];
     B2RL_REQUIRE(b == L.field_bytes[f], "ring and replay have different fields");
-    if (b % 16 == 0 && b >= 1024) {
-      P.src[P.n] = h->field[f];
-      P.dst[P.n] = (uint8_t*)ptrs[3 + f];
-      P.bytes[P.n] = b;
-      P.chunks[P.n] = (int32_t)((b + SERVE_CHUNK - 1) / SERVE_CHUNK);
-      P.items_per_draw += P.chunks[P.n];
-      P.n++;
+    if (is_bulk_row(b)) {
+      P.add(h->field[f], (uint8_t*)ptrs[3 + f], b, 14336);   // the CHUNK of k_serve_fill's copy_rows
     } else {
       small.src[small.n] = h->field[f];
       small.dst[small.n] = (uint8_t*)ptrs[3 + f];
@@ -330,20 +260,15 @@ extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot,
     }
   }
   DeviceGuard g(h->device);
-  static int sms[64] = {0};
-  static bool attr_set[64] = {false};
-  const int dev = h->device & 63;
-  if (!attr_set[dev]) {
-    B2RL_CUDA(cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, h->device));
-    B2RL_CUDA(cudaFuncSetAttribute(k_serve_fill, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SERVE_SMEM));
-    attr_set[dev] = true;
-  }
+  int sms = 0;
+  B2RL_CUDA(sm_count(h->device, &sms));
+  B2RL_CUDA(set_max_dynamic_smem<k_serve_fill>(h->device, BULK_RING_BYTES));
   // one CTA per SM (the shared-memory ring takes the SM), at most SERVE_THREADS draws per CTA
   const int64_t n = L.batch;
-  int64_t grid = sms[dev] < n ? sms[dev] : n;
+  int64_t grid = sms < n ? sms : n;
   const int64_t min_grid = (n + SERVE_THREADS - 1) / SERVE_THREADS;
   if (grid < min_grid) grid = min_grid;
-  k_serve_fill<<<(unsigned)grid, SERVE_THREADS, SERVE_SMEM, (cudaStream_t)stream>>>(
+  k_serve_fill<<<(unsigned)grid, SERVE_THREADS, BULK_RING_BYTES, (cudaStream_t)stream>>>(
       h->tree, P, small, h->rng_dev, n, h->capacity, h->n_valid_dev, beta, max_w_dev, (int64_t*)ptrs[1],
       (float*)ptrs[2], (uint64_t*)ptrs[0], seq, r->done_ticket);
   count_launch();

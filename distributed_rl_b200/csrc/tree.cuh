@@ -1,7 +1,8 @@
 // Device-side pieces of the sum-tree that more than one kernel uses: the 16-wide group loads, the radix-16
 // descent of proportional sampling, the fetch of a sampled slot's scalar fields and the IS weight.
-// k_tree_sample (tree.cu) and k_serve_fill (serve.cu) both draw through tree_draw / is_weight, so a served
-// minibatch is bit-identical to b2rl_tree_sample_fetch from the same RNG state.
+// k_tree_sample (tree.cu) and k_serve_fill (serve.cu) both draw through tree_draw / is_weight and fetch through
+// fetch_small, so a served minibatch is bit-identical to b2rl_tree_sample_fetch from the same RNG state; its frame
+// rows go through copy_rows (bulk_rows.cuh), as b2rl_replay_gather's.
 #pragma once
 #include "common.cuh"
 

@@ -54,18 +54,49 @@ from .apex import ApexConfig
 from .learner_common import Stoppable
 
 
-class ReplayServer(Stoppable):
-    def __init__(self, cfg: ApexConfig | None = None, connect=None, connect_push=None, m: int = 32):
+class _StandaloneServer(Stoppable):
+    """What the two stand-alone servers share (APE_X/ReplayServer.py:20-160): the ingest of `experience` into the
+    store, FLAG_BATCH once the store holds more than BUFFER_SIZE records, and eviction on FLAG_REMOVE."""
+
+    def __init__(self, cfg: ApexConfig | None, connect):
         super().__init__()
         self.cfg = cfg or ApexConfig.from_configuration()
         self.device = torch.device(self.cfg.LEARNER_DEVICE)
         from .apex import Replay
         self._ingest = Replay(self.cfg, connect=None)      # never started: its record decoder + pinned staging + store
         self.store = self._ingest.store
-        self.connect, self.connect_push = connect, connect_push if connect_push is not None else connect
-        self.m = m                               # minibatches assembled per buffer() (the reference: 32, :66)
-        self.FLAG_BATCH = self.FLAG_REMOVE = False
+        self.connect = connect
+        self.FLAG_BATCH = False
         self.total_transition = 0
+
+    def _ingest_experience(self) -> list:
+        """The top of serve_once(): raise FLAG_BATCH, then push the drained `experience` records. -> the records."""
+        if len(self.store) > self.cfg.BUFFER_SIZE and not self.FLAG_BATCH:
+            self.FLAG_BATCH = True
+            self.connect.set("FLAG_BATCH", pickle.dumps(True))
+        data = wire.drain(self.connect, "experience")
+        if data:
+            self._ingest.push_records(data)
+            self.total_transition += len(data)
+        return data
+
+    def _evict_on_request(self) -> None:
+        """A full store honours the learner's FLAG_REMOVE: evict down to REPLAY_MEMORY_LEN, clear the flag."""
+        if len(self.store) >= self.cfg.REPLAY_MEMORY_LEN:
+            cond = self.connect.get("FLAG_REMOVE")
+            if cond is not None and pickle.loads(cond):
+                over = len(self.store) - self.cfg.REPLAY_MEMORY_LEN
+                if over > 0:
+                    self.store.evict(over)
+                self.connect.set("FLAG_REMOVE", pickle.dumps(False))
+
+
+class ReplayServer(_StandaloneServer):
+    def __init__(self, cfg: ApexConfig | None = None, connect=None, connect_push=None, m: int = 32):
+        super().__init__(cfg, connect)
+        self.connect_push = connect_push if connect_push is not None else connect
+        self.m = m                               # minibatches assembled per buffer() (the reference: 32, :66)
+        self.FLAG_REMOVE = False
         if self.connect is not None:
             self.connect.set("FLAG_BATCH", pickle.dumps(False))           # :39
 
@@ -99,25 +130,10 @@ class ReplayServer(Stoppable):
 
     def serve_once(self) -> dict:
         """One iteration of run() (:116-160)."""
-        k = self.cfg.BUFFER_SIZE
-        if len(self.store) > k and not self.FLAG_BATCH:
-            self.FLAG_BATCH = True
-            self.connect.set("FLAG_BATCH", pickle.dumps(True))
-        data = wire.drain(self.connect, "experience")
-        pushed = 0
-        if data:
-            self._ingest.push_records(data)
-            self.total_transition += len(data)
-            if len(self.store) > k:
-                pushed = self.buffer()
+        data = self._ingest_experience()
+        pushed = self.buffer() if data and len(self.store) > self.cfg.BUFFER_SIZE else 0
         applied = self.update()
-        if len(self.store) >= self.cfg.REPLAY_MEMORY_LEN:
-            cond = self.connect.get("FLAG_REMOVE")
-            if cond is not None and pickle.loads(cond):
-                over = len(self.store) - self.cfg.REPLAY_MEMORY_LEN
-                if over > 0:
-                    self.store.evict(over)
-                self.connect.set("FLAG_REMOVE", pickle.dumps(False))
+        self._evict_on_request()
         return {"ingested": len(data), "batches_queued": pushed, "updates_applied": applied}
 
     def run(self):
@@ -355,7 +371,7 @@ def _ipc_events(device: torch.device, n: int):
         return ev, [e.ipc_handle() for e in ev]
 
 
-class DeviceReplayServer(Stoppable):
+class DeviceReplayServer(_StandaloneServer):
     """The stand-alone replay server over a device ring (APE_X/ReplayServer.py:20-160): the same `experience` ingest,
     eviction on FLAG_REMOVE and FLAG_BATCH as `ReplayServer`, but each served minibatch is one `b2rl_serve_fill`
     launch into a ring slot the learner maps through CUDA IPC.  Keeps up to `slots` filled minibatches ahead of the
@@ -365,21 +381,13 @@ class DeviceReplayServer(Stoppable):
     STATS_EVERY = 0.1             # seconds between SERVE_STATS refreshes (each costs a device sync)
 
     def __init__(self, cfg: ApexConfig | None = None, connect=None, slots: int = 4):
-        super().__init__()
-        self.cfg = cfg or ApexConfig.from_configuration()
-        self.device = torch.device(self.cfg.LEARNER_DEVICE)
-        from .apex import Replay
-        self._ingest = Replay(self.cfg, connect=None)      # never started: its record decoder + pinned staging + store
-        self.store = self._ingest.store
+        super().__init__(cfg, connect)
         self.device = self.store.device
-        self.connect = connect
         self.ring = ServeRing.create(self.store, self.cfg.BATCHSIZE, slots)
         self.slots = ServerSlots(connect, slots, self.cfg.BATCHSIZE)
         (self.filled, filled_h), (self.applied, applied_h) = _ipc_events(self.device, slots), _ipc_events(self.device, slots)
         self.released = self.written = None                # the learner's events, once it has attached
         self._upd = [self.ring.slot_ptrs(j)[1] for j in range(slots)]
-        self.FLAG_BATCH = False
-        self.total_transition = 0
         self._stats_t = 0.0
         connect.delete(BATCH_SLOT, RELEASE_SLOT, UPDATE_SLOT, UPDATE_DONE, CLIENT_KEY, STATS_KEY, DETACH_KEY)
         connect.set("FLAG_BATCH", pickle.dumps(False))
@@ -425,24 +433,11 @@ class DeviceReplayServer(Stoppable):
 
     def serve_once(self) -> dict:
         """One iteration of run(): ingest, take back released slots, apply update slots, refill free slots, evict."""
-        k = self.cfg.BUFFER_SIZE
-        if len(self.store) > k and not self.FLAG_BATCH:
-            self.FLAG_BATCH = True
-            self.connect.set("FLAG_BATCH", pickle.dumps(True))
-        data = wire.drain(self.connect, "experience")
-        if data:
-            self._ingest.push_records(data)
-            self.total_transition += len(data)
+        data = self._ingest_experience()
         released = self.slots.collect_releases(self._wait_released)
         applied = self.slots.apply_updates(self._apply)
-        filled = self.slots.fill_free(self._fill) if len(self.store) > k else 0
-        if len(self.store) >= self.cfg.REPLAY_MEMORY_LEN:
-            cond = self.connect.get("FLAG_REMOVE")
-            if cond is not None and pickle.loads(cond):
-                over = len(self.store) - self.cfg.REPLAY_MEMORY_LEN
-                if over > 0:
-                    self.store.evict(over)
-                self.connect.set("FLAG_REMOVE", pickle.dumps(False))
+        filled = self.slots.fill_free(self._fill) if len(self.store) > self.cfg.BUFFER_SIZE else 0
+        self._evict_on_request()
         self._publish_stats(bool(data))
         return {"ingested": len(data), "filled": filled, "released": released, "updates_applied": applied}
 
