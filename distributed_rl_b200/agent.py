@@ -374,29 +374,33 @@ class GraphAgent(nn.Module):
         return tuple(vals[n] for n in self._outputs)
 
     @contextlib.contextmanager
-    def packed_heads_cache(self):
+    def packed_heads_cache(self, packs: dict | None = None):
         """While active, the packed (3xTF32) forward operand of the fused heads is built once and reused by
-        every forward pass: use it around several passes between which the weights do not change."""
-        self._pack_cache = {}
+        every forward pass: use it around several passes between which the weights do not change.  `packs`:
+        operands prepack_heads() already built for these weights (e.g. on another stream), used from the start."""
+        self._pack_cache = dict(packs) if packs else {}
         try:
             yield
         finally:
             self._pack_cache = None
 
-    def prepack_heads(self, transposed: bool = False):
+    def prepack_heads(self, transposed: bool = False) -> dict:
         """Fill the packed-operand cache (inside packed_heads_cache()) without running a forward pass, so
         that passes issued on several streams afterwards only read it.  transposed=True prepares the W^T
-        operand the input-gradient GEMM of a later backward pass needs (entry "bwdT")."""
+        operand the input-gradient GEMM of a later backward pass needs (entry "bwdT").  Returns the cache
+        entries it filled, which packed_heads_cache(packs) accepts."""
+        built = {}
         if self._pack_cache is None or not (self.dense_3xtf32 and self.fuse_sibling_heads):
-            return
+            return built
         from .linear import _pack_pieces
         for group in set(self._head_groups.values()):
             duel = self._dueling.get(group) if self.fused_dueling_tail else None
             names = (duel["adv"], duel["val"]) if duel is not None else group
             ws = [next(iter(getattr(self, n).children())).weight for n in names]
             if ws[0].is_cuda and not any(w.shape[0] % 32 for w in ws[:-1]):
-                self._pack_cache.setdefault(group, {})["bwdT" if transposed else "fwd"] = \
-                    _pack_pieces([w.detach() for w in ws], transposed, True)
+                entry = built[group] = self._pack_cache.setdefault(group, {})
+                entry["bwdT" if transposed else "fwd"] = _pack_pieces([w.detach() for w in ws], transposed, True)
+        return built
 
     def _prehead_group(self):
         """(group, (C, HW)) if the first conv node ends with [Conv2d, ReLU, Flatten] and feeds ONLY one dueling head

@@ -181,6 +181,54 @@ class Replay(ReplayThread):
         torch.cuda.current_stream(self.device).synchronize()
 
 
+class _StepState:
+    """What `Learner.fused_step` keeps from one step to the next: its streams and fork/join sites, the conv_1 weight
+    packs, the weight-gradient sink, the draw buffers and the batched pass's conv_1 output.  Built once, before the
+    first step's warm-up, so that no stream, event or buffer is created inside the warm-up or the capture.
+
+    Stream priorities are captured into the graph's kernel nodes: the main branch runs at -2 and so does the target
+    network's pass (both feed the target kernel); the operand packs and the side branch (needed much later) at 0;
+    the sink's lanes at -1 (convolutions) and 0 (heads)."""
+
+    def __init__(self, L: "Learner"):
+        from .linear import SideBranch, WeightGradSink
+        cfg, dev, B = L.cfg, L.device, L.cfg.BATCHSIZE
+        self.main = torch.cuda.Stream(dev, priority=-2)
+        packs, target = torch.cuda.Stream(dev), torch.cuda.Stream(dev, priority=-2)
+
+        def branch(stream):          # without PARALLEL_FORWARDS the step runs on one stream
+            return SideBranch(stream if cfg.PARALLEL_FORWARDS else None)
+        self.conv1_packs = branch(target)         # conv_1 waits for this launch
+        self.head_packs_built = branch(packs)
+        self.target_pass = branch(target)
+        self.side = branch(packs)                 # Q_online(s') or the batched pass's action / done conversion; W^T pack
+        self.prio_update = branch(target)
+        self.max_w = SideBranch(packs)            # data parallel: the reduced max IS weight, for the next step
+        self.head_packs = None                    # (online, target) heads' forward operands of this step
+        self.pack1 = self.pack2 = self.cur = self.y_big = self.sink = None
+        if not L._conv1_ready():
+            return
+        # pack1: online net (grad pass on s); pack2: online + target in one pass over s'
+        self.conv_name, self.pack1, self.pack2 = conv1_packs(L.model, dev, 1, 2)
+        self.cur = dict(L.memory.store.alloc_batch(B, ("action", "reward", "done")),
+                        idx=torch.empty(B, dtype=torch.int64, device=dev),
+                        w=torch.empty(B, dtype=torch.float32, device=dev))
+        if cfg.PARALLEL_FORWARDS and cfg.BATCHED_ONLINE:
+            self.y_big = torch.empty((3, B, 20, 20, self.pack1.c_out), dtype=torch.float32, device=dev)
+        if cfg.DEFERRED_WGRAD and L._fused_optim:
+            self.sink = WeightGradSink(dev)
+            self.sink.grads_are_zero = True      # grads are pre-allocated and zeroed by the fused optimizer
+            getattr(L.model, self.conv_name).split_backward = True
+            if L._world > 1:
+                L._bucket.attach_sink(self.sink)
+            # Learner.step (:123-138) has no clipping: a parameter can be stepped once its own gradient is final
+            # (after its all-reduce when data parallel).  The heads (97 % of the elements) are final ~150 us
+            # before the conv stack's.
+            self.early_params = [p for n, p in L.model.named_parameters() if not n.startswith(self.conv_name + ".")]
+            self.early_ok = (cfg.EARLY_HEAD_UPDATE and bool(self.early_params)
+                             and L.optim.set_early(self.early_params))
+
+
 class Learner(TargetNetLearner):
     """APE_X/Learner.py Learner (:20-272): train / step / run / state_dict."""
 
@@ -217,6 +265,7 @@ class Learner(TargetNetLearner):
             wipe_stale_keys(connect, keep=getattr(self.memory, "KEEP_KEYS", ()) if self._served else ())
         self.gamma_n = float(np.float32(0.99 ** self.cfg.UNROLL_STEP))  # hard-coded 0.99, :103
         self._graph = None
+        self._fused = None              # _StepState, built by the first fused_step / _forward_backward_fused
         self._world = 1
         self.launches_per_step = None   # libb2rl kernels per fused step (bench.py's gpu_launches)
 
@@ -326,72 +375,53 @@ class Learner(TargetNetLearner):
 
     # -- fused gather + conv_1 path ------------------------------------------------------------
     def _conv1_ready(self) -> bool:
-        if not self.cfg.FUSED_CONV1 or self.model.first_conv_node() is None:
-            return False
-        if not hasattr(self, "_pack2"):
-            # _pack1: online net (grad pass on s); _pack2: online + target in one pass over s'
-            self._conv_name, self._pack1, self._pack2 = conv1_packs(self.model, self.device, 1, 2)
-        return True
+        return bool(self.cfg.FUSED_CONV1) and self.model.first_conv_node() is not None
 
-    def _streams(self):
-        if not hasattr(self, "_fork"):
-            # s1: operand packs (needed much later: default priority); s2: the target network's pass — as critical
-            # as the main branch (both feed the target kernel), so it gets the main branch's priority in the graph
-            self._fork = (torch.cuda.Stream(self.device), torch.cuda.Stream(self.device, priority=-2),
-                          torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event())
-            self._ev_pk, self._ev_tg, self._ev_upd = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
-            self._ev_hp, self._ev_mw = torch.cuda.Event(), torch.cuda.Event()
-        return self._fork
+    def _fused_state(self) -> "_StepState":
+        if self._fused is None:
+            self._fused = _StepState(self)
+        return self._fused
 
-    def _pack_conv1(self):
-        w_on = getattr(self.model, self._conv_name).conv_1.weight
-        w_tg = getattr(self.target_model, self._conv_name).conv_1.weight
-        R.conv1_pack_jobs([(self._pack1, 0, w_on), (self._pack2, 0, w_on), (self._pack2, 1, w_tg)])   # one launch
+    _pack2 = property(lambda self: self._fused_state().pack2)   # conv_1 weights of online + target, packed
+    _cur = property(lambda self: self._fused.cur)      # the draw of the last fused_step: idx, w, action, reward, done
 
-    def _pack_conv1_async(self):
-        """The conv_1 weight packs of this step on a side stream (they only depend on the weights): they overlap
-        the tree sample + scalar gather at the start of the step.  Returns the event the conv_1 launch waits for."""
-        s1, s2 = self._streams()[:2]
-        cur = torch.cuda.current_stream(self.device)
-        self._ev_pk.record(cur)
-        s1.wait_event(self._ev_pk)
-        s2.wait_event(self._ev_pk)
-        with torch.cuda.stream(s2):          # the high-priority side stream: conv_1 waits for these three launches
-            self._pack_conv1()
-            self._ev_pk.record(s2)
-        # The heads' forward operands (online and target: four 3136 x 512 matrices -> two packed images) are needed
-        # ~120 us into the step: built on the low-priority side stream now instead of on the main / target branches
-        # in front of their GEMMs.
-        self._head_packs = None
+    def _pack_weights(self):
+        """This step's weight packs.  They depend only on the weights, so they are forked at the start of the step
+        and overlap the tree sample + scalar gather: the conv_1 packs (one launch; conv_1 waits for it, so it runs on
+        the high-priority stream) and, for the batched online pass, the heads' forward operands of both networks
+        (four 3136 x 512 matrices -> two packed images, needed ~120 us into the step)."""
+        s = self._fused
+        w_on = getattr(self.model, s.conv_name).conv_1.weight
+        w_tg = getattr(self.target_model, s.conv_name).conv_1.weight
+        with s.conv1_packs.fork():
+            R.conv1_pack_jobs([(s.pack1, 0, w_on), (s.pack2, 0, w_on), (s.pack2, 1, w_tg)])   # one launch
         if self.cfg.PARALLEL_FORWARDS and self.cfg.BATCHED_ONLINE:
-            with torch.cuda.stream(s1):
+            with s.head_packs_built.fork():
                 with self.model.packed_heads_cache():
-                    self.model.prepack_heads()
-                    self._head_packs = dict(self.model._pack_cache)
+                    on = self.model.prepack_heads()
                 with self.target_model.packed_heads_cache():      # was ~11 us in front of the target pass's GEMM
-                    self.target_model.prepack_heads()
-                    self._head_packs_tg = dict(self.target_model._pack_cache)
-                self._ev_hp.record(s1)
-        return self._ev_pk
+                    tg = self.target_model.prepack_heads()
+            s.head_packs = (on, tg)
 
-    def _forward_backward_fused(self, idx, action, reward, done, weight, packs_done=None, update_tree=False,
+    def _forward_backward_fused(self, idx, action, reward, done, weight, prepacked=False, update_tree=False,
                                 early_update=False):
         """Same maths as _forward_backward, but s and s' are never staged as uint8/fp32 batches:
         conv_1 reads the sampled rows straight from the replay payload (b2rl_conv1_fused).
-        `packs_done`: event after which the conv_1 weight packs are valid (None: pack here).
+        `prepacked`: the caller has already issued this step's _pack_weights().
         `update_tree`: write the new priorities back on a side stream as soon as the target kernel has produced
-        them (overlapping backward); the caller then waits for `self._ev_upd` instead of calling store.update.
+        them (overlapping backward); the caller then joins `prio_update` instead of calling store.update.
         `early_update`: the caller WILL call self.step() next; the heads' part of that optimizer step may then be
         issued here, behind their weight gradients on the sink's lane, while the conv stack's backward still runs."""
+        s = self._fused_state()
         st = self.memory.store
-        w_on = getattr(self.model, self._conv_name).conv_1.weight
+        w_on = getattr(self.model, s.conv_name).conv_1.weight
+        if not prepacked:
+            self._pack_weights()
+        s.conv1_packs.join()
         notdone = None
-        if packs_done is None:
-            self._pack_conv1()
-        else:
-            torch.cuda.current_stream(self.device).wait_event(packs_done)
-        with self.model.packed_heads_cache():     # the online weights are packed once for both passes
-            if self.cfg.PARALLEL_FORWARDS and self.cfg.BATCHED_ONLINE:
+        batched = self.cfg.PARALLEL_FORWARDS and self.cfg.BATCHED_ONLINE
+        with self.model.packed_heads_cache(s.head_packs[0] if batched else None):   # online weights packed once
+            if batched:
                 # Q(s) (with grad) and Q_online(s') (without) share the online weights: every kernel after conv_1 is
                 # launch / set-up bound at B = 512 (DESIGN.md §6b), so both run as ONE B = 2*BATCHSIZE pass
                 # (conv_2, conv_3, heads' GEMM, dueling tail: one launch each instead of two).  The pass is recorded
@@ -399,119 +429,67 @@ class Learner(TargetNetLearner):
                 # outputs (first B rows: views, no kernels) through the same forward code.  Q_target(s') runs
                 # beside it on a second stream.
                 from .linear import OutputTape
-                s1, s2, e0, e1, e2 = self._streams()
-                cur = torch.cuda.current_stream(self.device)
-                early_packs = packs_done is not None and bool(getattr(self, "_head_packs", None))
-                if early_packs:
-                    self.model._pack_cache.update(self._head_packs)       # built on s1 at the start of the step
-                else:
-                    self.model.prepack_heads()
-                B = idx.numel()
-                c_out = self._pack1.c_out
-                if getattr(self, "_y_big", None) is None or self._y_big.shape[1] != B:
-                    self._y_big = torch.empty((3, B, 20, 20, c_out), dtype=torch.float32, device=self.device)
-                big = self._y_big          # [0] conv_1(s) online, [1] conv_1(s') online, [2] conv_1(s') target
+                B, c_out = idx.numel(), s.pack1.c_out
+                big = s.y_big          # [0] conv_1(s) online, [1] conv_1(s') online, [2] conv_1(s') target
+                if big.shape[1] != B:
+                    raise ValueError(f"the batched online pass is sized for BATCHSIZE = {big.shape[1]}, got {B} rows")
                 with torch.no_grad():
-                    R.conv1_fused(st.field_view("state"), idx, self._pack1, relu=True, out=big[0:1])
-                    y_tg = R.conv1_fused(st.field_view("next_state"), idx, self._pack2, relu=True, out=big[1:3])[1]
-                if early_packs:
-                    cur.wait_event(self._ev_hp)      # long done; the heads' GEMM is ~100 us away
-                e0.record(cur)
-                s1.wait_event(e0)
-                s2.wait_event(e0)
+                    R.conv1_fused(st.field_view("state"), idx, s.pack1, relu=True, out=big[0:1])
+                    y_tg = R.conv1_fused(st.field_view("next_state"), idx, s.pack2, relu=True, out=big[1:3])[1]
+                s.head_packs_built.join()      # long done; the heads' GEMM is ~100 us away
                 with torch.no_grad():
-                    with torch.cuda.stream(s2):
-                        with self.target_model.packed_heads_cache():
-                            if early_packs:
-                                self.target_model._pack_cache.update(self._head_packs_tg)
-                            qn_target = self.target_model.forward_from_conv1(y_tg, True)[0]  # :85
-                        e2.record(s2)
-                    with torch.cuda.stream(s1):
+                    with s.target_pass.fork(), self.target_model.packed_heads_cache(s.head_packs[1]):
+                        qn_target = self.target_model.forward_from_conv1(y_tg, True)[0]  # :85
+                    with s.side.fork():
                         if action.dtype != torch.int64:            # int32 replay field -> the target kernel's int64:
                             action = action.to(torch.int64)        # off the main branch (it sat in front of conv_1)
                         notdone = 1.0 - done.to(torch.float32)     # likewise (two launches in front of the target kernel)
                         self.model.prepack_heads(transposed=True)   # W^T operand of the heads' dgrad, off the main branch
-                        e1.record(s1)
                     y_both = big[0:2].view(2 * B, 20, 20, c_out).permute(0, 3, 1, 2)     # logical NCHW, physical NHWC
                     with OutputTape.record() as tape:
                         q_all = self.model.forward_from_conv1(y_both, True)[0]          # :78 and :87 in one pass
                 qn_online = q_all[B:]
-                y = _Conv1Gathered.apply(w_on, st.field_view("state"), idx, self._pack1, self._mf, st,
+                y = _Conv1Gathered.apply(w_on, st.field_view("state"), idx, s.pack1, self._mf, st,
                                          big[0].permute(0, 3, 1, 2), True)
                 with OutputTape.replay(tape.half(B)):
                     q = self.model.forward_from_conv1(y, True)[0]                       # graph only: outputs replayed
-                cur.wait_event(e1)
-                cur.wait_event(e2)
-            elif self.cfg.PARALLEL_FORWARDS:
-                # The three passes are independent until the target kernel: fork them onto three streams
-                # (captured as parallel branches of the step's CUDA graph) so their small kernels overlap.
-                s1, s2, e0, e1, e2 = self._streams()
-                cur = torch.cuda.current_stream(self.device)
+            else:
+                # Three separate passes, independent until the target kernel.  With PARALLEL_FORWARDS the two over s'
+                # fork onto two streams (parallel branches of the step's CUDA graph) so their small kernels overlap.
                 self.model.prepack_heads()
                 with torch.no_grad():
-                    y_on, y_tg = R.conv1_fused(st.field_view("next_state"), idx, self._pack2, relu=True)
-                e0.record(cur)
-                s1.wait_event(e0)
-                s2.wait_event(e0)
-                with torch.no_grad():
-                    with torch.cuda.stream(s1):
+                    y_on, y_tg = R.conv1_fused(st.field_view("next_state"), idx, s.pack2, relu=True)
+                    with s.side.fork():
                         qn_online = self.model.forward_from_conv1(y_on, True)[0]        # :87
-                        self.model.prepack_heads(transposed=True)   # W^T operand of the heads' dgrad, off the main branch
-                        e1.record(s1)
-                    with torch.cuda.stream(s2):
+                        if self.cfg.PARALLEL_FORWARDS:    # on one stream backward packs it beside its wgrad lanes
+                            self.model.prepack_heads(transposed=True)   # W^T operand of the heads' dgrad, off the main branch
+                    with s.target_pass.fork():
                         qn_target = self.target_model.forward_from_conv1(y_tg, True)[0]  # :85
-                        e2.record(s2)
-                y = _Conv1Gathered.apply(w_on, st.field_view("state"), idx, self._pack1, self._mf, st, None, True)
+                y = _Conv1Gathered.apply(w_on, st.field_view("state"), idx, s.pack1, self._mf, st, None, True)
                 q = self.model.forward_from_conv1(y, True)[0]                        # :78 (ReLU in the conv_1 epilogue)
-                cur.wait_event(e1)
-                cur.wait_event(e2)
-            else:
-                with torch.no_grad():
-                    y_on, y_tg = R.conv1_fused(st.field_view("next_state"), idx, self._pack2, relu=True)
-                    qn_online = self.model.forward_from_conv1(y_on, True)[0]        # :87
-                    qn_target = self.target_model.forward_from_conv1(y_tg, True)[0]  # :85
-                y = _Conv1Gathered.apply(w_on, st.field_view("state"), idx, self._pack1, self._mf, st, None, True)
-                q = self.model.forward_from_conv1(y, True)[0]                        # :78 (ReLU in the conv_1 epilogue)
+            s.side.join()
+            s.target_pass.join()
         if notdone is None:
             notdone = 1.0 - done.to(torch.float32)
         out = R.apex_target(q.detach(), qn_online, qn_target, action, reward, notdone, weight,
                             self.gamma_n, self.cfg.ALPHA)
         if update_tree:      # priority write-back (one CTA) next to backward instead of after the optimizer
-            s2 = self._streams()[1]
-            cur = torch.cuda.current_stream(self.device)
-            self._ev_tg.record(cur)
-            s2.wait_event(self._ev_tg)
-            with torch.cuda.stream(s2):
+            with s.prio_update.fork():
                 st.update(idx, out["prio"])
-                self._ev_upd.record(s2)
-        if self.cfg.DEFERRED_WGRAD and self._fused_optim:      # grads are pre-allocated and zeroed by the optimizer
-            if not hasattr(self, "_sink"):
-                from .linear import WeightGradSink
-                self._sink = WeightGradSink(self.device)
-                getattr(self.model, self._conv_name).split_backward = True
-                if self._world > 1:
-                    self._bucket.attach_sink(self._sink)
-                # Learner.step (:123-138) has no clipping: a parameter can be stepped once its own gradient is final
-                # (after its all-reduce when data parallel).  The heads (97 % of the elements) are final ~150 us
-                # before the conv stack's.
-                self._early_params = [p for n, p in self.model.named_parameters()
-                                      if not n.startswith(self._conv_name + ".")]
-                self._early_ok = (self.cfg.EARLY_HEAD_UPDATE and bool(self._early_params)
-                                  and self.optim.set_early(self._early_params))
-            self._sink.grads_are_zero = True      # this branch: grads pre-allocated and zeroed by the fused optimizer
-            with self._sink.active():
+        sink = s.sink
+        if sink is None:
+            q.backward(out["grad_q"])
+        else:
+            with sink.active():
                 q.backward(out["grad_q"])
-            if early_update and self._early_ok and \
-                    all(id(p) in self._sink.accumulated[0] for p in self._early_params):
+            if early_update and s.early_ok and all(id(p) in sink.accumulated[0] for p in s.early_params):
                 if self._world > 1:
                     # data parallel: the heads' all-reduce was launched from this lane when their last gradient
                     # landed; the lane waits for it, then steps them — still beside the conv stack's backward
-                    self._sink.run_on_lane(lambda: self._bucket.wait_group(0) and self.optim.step_early(), 0)
+                    sink.run_on_lane(lambda: self._bucket.wait_group(0) and self.optim.step_early(), 0)
                 else:
-                    self._sink.run_on_lane(self.optim.step_early, 0)
-            self._sink.join()
-        else:
-            q.backward(out["grad_q"])
+                    sink.run_on_lane(self.optim.step_early, 0)
+            sink.join()
         if self._world > 1:
             self._bucket.finish()
         return out
@@ -527,7 +505,10 @@ class Learner(TargetNetLearner):
             raise RuntimeError("fused_step() samples the learner's own replay; a served replay is driven by run()")
         B = self.cfg.BATCHSIZE
         st = self.memory.store
-        fused_conv1 = self._conv1_ready()
+        s = self._fused_state()
+        fused_conv1 = s.pack1 is not None
+        side = fused_conv1 and self.cfg.PARALLEL_FORWARDS
+        batched = side and self.cfg.BATCHED_ONLINE      # the batched pass converts the action itself
 
         def body():
             max_w, mw_work = None, None
@@ -537,26 +518,20 @@ class Learner(TargetNetLearner):
                 # (the reference's own max_weight is up to 16 minibatches stale, APE_X/ReplayMemory.py:61-67).
                 mw_work = self._D.all_reduce_max_(st.max_weight(self.cfg.BETA, out=self._max_w), async_op=True)
                 max_w = self._max_w_use
-            side = fused_conv1 and self.cfg.PARALLEL_FORWARDS
-            packs_done = self._pack_conv1_async() if side else None
             if fused_conv1:
+                self._pack_weights()
                 # ONE launch draws the minibatch: indices + IS weights from the sum-tree and the sampled slots'
                 # scalar fields (a, r, done); the frames are read in place by the conv_1 kernels.
                 # (Drawing the NEXT minibatch at the end of the step would hide these ~5 us too, but a ring slot
                 # overwritten by the ingest between the draw and its use would pair new frames with the old
                 # record's a / r / done — DESIGN.md §4.2.)
-                if not hasattr(self, "_cur"):
-                    self._cur = dict(st.alloc_batch(B, ("action", "reward", "done")),
-                                     idx=torch.empty(B, dtype=torch.int64, device=self.device),
-                                     w=torch.empty(B, dtype=torch.float32, device=self.device))
-                c = self._cur
+                c = s.cur
                 st.sample_fetch(B, self.cfg.BETA, c["idx"], c["w"], {k: c[k] for k in ("action", "reward", "done")},
                                 max_w=max_w)
                 idx = c["idx"]
-                batched = self.cfg.PARALLEL_FORWARDS and self.cfg.BATCHED_ONLINE      # converts the action itself
                 out = self._forward_backward_fused(idx, c["action"] if batched else c["action"].to(torch.int64),
                                                    c["reward"], c["done"], c["w"],
-                                                   packs_done=packs_done, update_tree=side, early_update=True)
+                                                   prepacked=True, update_tree=side, early_update=True)
             else:
                 idx, _, w = st.sample(B, beta=self.cfg.BETA, want_prob=False, max_w=max_w)
                 b = st.gather(idx)
@@ -564,18 +539,16 @@ class Learner(TargetNetLearner):
                                              b["next_state"], b["done"], w)
             info = self.step()
             if side:
-                torch.cuda.current_stream(self.device).wait_event(self._ev_upd)
+                s.prio_update.join()
             else:
                 st.update(idx, out["prio"])
             if mw_work is not None:
                 # the reduced maximum becomes the NEXT step's normaliser: wait + copy on a side stream (this step's
                 # draw has long read the old value), joined here at no cost instead of 5 us at the end of the step
-                s1 = self._streams()[0]
-                with torch.cuda.stream(s1):
+                with s.max_w.fork(after_current=False):
                     mw_work.wait()
                     self._max_w_use.copy_(self._max_w)
-                    self._ev_mw.record(s1)
-                torch.cuda.current_stream(self.device).wait_event(self._ev_mw)
+                s.max_w.join()
             return {"scalars": out["scalars"], "p_norm": info["p_norm"], "prio": out["prio"], "idx": idx}
 
         lib = st.lib
@@ -589,19 +562,19 @@ class Learner(TargetNetLearner):
         self.optim.zero_grad(set_to_none=False)
         # The step's main branch is captured on a HIGH-priority stream (kernel nodes inherit it): the side branches
         # (weight gradients, early optimizer step, operand packs) only fill SMs the critical chain leaves idle.
-        side = torch.cuda.Stream(self.device, priority=-2)
+        main = s.main
         # The ingest thread keeps pushing on the same replay handle: hold its lock so that no cudaMalloc /
         # cudaHostAlloc / copy of that thread lands inside the warm-up or the (global-mode) capture.
         with self.memory._lock:
-            side.wait_stream(torch.cuda.current_stream(self.device))
-            with torch.cuda.stream(side):
+            main.wait_stream(torch.cuda.current_stream(self.device))
+            with torch.cuda.stream(main):
                 for _ in range(3):   # warm-up: lazy inits (cuDNN plans, optimizer state) happen outside capture
                     body()
-            torch.cuda.current_stream(self.device).wait_stream(side)
+            torch.cuda.current_stream(self.device).wait_stream(main)
             torch.cuda.synchronize(self.device)
             g = torch.cuda.CUDAGraph()
             c0 = lib.b2rl_launch_count()
-            with torch.cuda.graph(g, stream=side):
+            with torch.cuda.graph(g, stream=main):
                 self._static = body()
             self.launches_per_step = lib.b2rl_launch_count() - c0   # recorded into the graph, replayed each step
         self._graph = g

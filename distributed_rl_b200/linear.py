@@ -8,6 +8,8 @@ the same order as an fp32 FMA chain; tests/test_gpu_03_gemm.py pins it against f
 """
 from __future__ import annotations
 
+import contextlib
+
 import torch
 
 from . import _lib
@@ -15,6 +17,37 @@ from . import _lib
 
 def _stream():
     return torch.cuda.current_stream().cuda_stream
+
+
+class SideBranch:
+    """One fork/join site of a step on a side stream.  `with branch.fork():` runs its block on `stream` behind the
+    work the current stream has queued so far (`after_current=False`: only behind what `stream` already holds);
+    `join()` makes the current stream wait for every block forked since the last join.  With `stream=None`
+    (parallelism disabled) the block runs in place and `join()` does nothing.  The events are created here, once,
+    so that forking inside a captured step creates none."""
+
+    def __init__(self, stream: torch.cuda.Stream | None):
+        self.stream = stream
+        self._forked, self._done = torch.cuda.Event(), torch.cuda.Event()
+        self._open = False
+
+    @contextlib.contextmanager
+    def fork(self, after_current: bool = True):
+        if self.stream is None:
+            yield
+            return
+        if after_current:
+            self._forked.record(torch.cuda.current_stream(self.stream.device))
+            self.stream.wait_event(self._forked)
+        with torch.cuda.stream(self.stream):
+            yield
+        self._done.record(self.stream)
+        self._open = True
+
+    def join(self) -> None:
+        if self._open:
+            torch.cuda.current_stream(self.stream.device).wait_event(self._done)
+            self._open = False
 
 
 class WeightGradSink:
@@ -35,11 +68,9 @@ class WeightGradSink:
         # Priorities (captured into the step's graph nodes): the learner's main branch runs at -2, the convolution
         # lane at -1 (its kernels must finish before the SM-filling conv_1 weight-gradient kernel starts), the
         # heads' lane (6.4 MB GEMM operands, the early optimizer step) at 0 fills what is left.
-        self.stream = torch.cuda.Stream(self.device, priority=0)
-        self.streams = (self.stream, torch.cuda.Stream(self.device, priority=-1))
-        self._fork = (torch.cuda.Event(), torch.cuda.Event())
-        self._done = (torch.cuda.Event(), torch.cuda.Event())
-        self._keep, self._pending = [], [False, False]
+        self.lanes = (SideBranch(torch.cuda.Stream(self.device, priority=0)),
+                      SideBranch(torch.cuda.Stream(self.device, priority=-1)))
+        self._keep = []
         self._lane, self.accumulated = 0, (set(), set())   # per lane: ids of the params accumulated since the last join
         self.on_ready = {}          # id(param) -> callable, invoked (side stream) after that param's grad is complete
 
@@ -48,20 +79,15 @@ class WeightGradSink:
         return _SINK is not None and all(p.grad is not None for p in params)
 
     def submit(self, fn, keep=(), lane: int = 0):
-        cur = torch.cuda.current_stream(self.device)
-        self._fork[lane].record(cur)
-        self.streams[lane].wait_event(self._fork[lane])
         self._lane = lane
-        with torch.cuda.stream(self.streams[lane]):
+        with self.lanes[lane].fork():
             fn()
         self._keep.extend(keep)
-        self._pending[lane] = True
 
     def run_on_lane(self, fn, lane: int = 0):
         """Queue fn behind what the lane already holds, without a new dependency on the caller's stream."""
-        with torch.cuda.stream(self.streams[lane]):
+        with self.lanes[lane].fork(after_current=False):
             fn()
-        self._pending[lane] = True
 
     def accumulate(self, param, grad):
         """(side stream) param.grad += grad, then the parameter's ready callback."""
@@ -81,11 +107,8 @@ class WeightGradSink:
     grads_are_zero = False
 
     def join(self):
-        for lane in (0, 1):
-            if self._pending[lane]:
-                self._done[lane].record(self.streams[lane])
-                torch.cuda.current_stream(self.device).wait_event(self._done[lane])
-                self._pending[lane] = False
+        for lane in self.lanes:
+            lane.join()
         self._keep.clear()
         self.accumulated[0].clear()
         self.accumulated[1].clear()
