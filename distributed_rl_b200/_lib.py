@@ -64,7 +64,8 @@ SIGNATURES = {
     "b2rl_conv1_wgrad_workspace_floats": (c_i64, [c_i32]),
     "b2rl_conv1_wgrad": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp]),
     "b2rl_rmsprop_step": (C.c_int, [C.POINTER(c_vp), C.POINTER(c_vp), C.POINTER(c_vp), C.POINTER(c_vp),
-                                    C.POINTER(c_i64), c_i32, c_f64, c_f64, c_f64, c_i32, c_vp, c_vp, c_vp]),
+                                    C.POINTER(c_i64), c_i32, c_f64, c_f64, c_f64, c_i32, C.POINTER(c_i64), c_vp, c_vp,
+                                    c_vp]),
     "b2rl_rmsprop_norm_finish": (C.c_int, [c_vp, c_i32, c_vp, c_vp]),
     "b2rl_peer_allreduce_max_ctas": (c_i32, []),
     "b2rl_peer_allreduce_mean": (C.c_int, [c_vp, c_vp, c_i32, c_i32, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp]),
@@ -73,10 +74,11 @@ SIGNATURES = {
     "b2rl_gemm_split_pack": (C.c_int, [c_vp, c_i64, c_i64, c_i64, c_i32, c_i32, c_vp, c_vp]),
     "b2rl_gemm_split_pack_into": (C.c_int, [c_vp, c_i64, c_i64, c_i64, c_i32, c_i32, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp]),
     "b2rl_gemm_pack_act_nhwc": (C.c_int, [c_vp, c_i64, c_i64, c_i64, c_i32, c_i32, c_vp, c_vp]),
-    "b2rl_unflatten_relu_mask": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i64, c_vp, c_vp]),
+    "b2rl_unflatten_relu_mask": (C.c_int, [c_vp, c_i64, c_i32, c_i64, c_vp, c_i64, c_i64, c_i64, c_vp, c_vp]),
     "b2rl_gemm_workspace_floats": (c_i64, [c_i64, c_i64, c_i64, c_i64]),
     "b2rl_gemm_tf32x3": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp]),
-    "b2rl_dueling_forward": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp]),
+    "b2rl_gemm_tf32x3_partials": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_vp]),
+    "b2rl_dueling_forward": (C.c_int, [c_vp, c_i32, c_i64, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]),
     "b2rl_dueling_backward": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b2rl_dueling_backward_w": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp]),
     "b2rl_launch_count": (c_i64, []),

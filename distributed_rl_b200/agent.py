@@ -237,6 +237,10 @@ class _Mean(nn.Module):
         return xs[0].mean(dim=-1, keepdim=True)
 
 
+def _refresh_after_load(module, incompatible_keys):
+    module.refresh_resident_heads()
+
+
 _NODE = {"CNN2D": ConvStack, "MLP": DenseStack, "LSTMNET": Recurrent,
          "ViewV2": lambda d: ViewAs(), "Add": lambda d: _Add(), "Substract": lambda d: _Sub(),
          "Mean": lambda d: _Mean()}
@@ -267,6 +271,12 @@ class GraphAgent(nn.Module):
         self.fuse_sibling_heads = True
         self.dense_3xtf32 = False       # first Linear of fused sibling heads via linear.linear3x (csrc/gemm.cu)
         self._pack_cache = None         # see packed_heads_cache()
+        # Persistent operand images of the fused heads' first layers ({group: {"fwd", "bwdT"?}}), see
+        # keep_resident_heads().  RULE: every write of those weights must leave the images equal to packing the new
+        # weights.  The fused optimizer does it in the update itself (FusedRMSprop.write_images); updateParameter and
+        # load_state_dict repack them (refresh_resident_heads); any other in-place write must call that too.
+        self._resident = None
+        self.register_load_state_dict_post_hook(_refresh_after_load)
         groups = {}
         for name in order:
             m = getattr(self, name)
@@ -331,11 +341,10 @@ class GraphAgent(nn.Module):
                     adv, val = getattr(self, duel["adv"]), getattr(self, duel["val"])
                     pre = x if isinstance(x, _PreHead) else None
                     if pre is not None:
-                        from .linear import relu_flat_linear3x
+                        from .linear import relu_flat_heads_dueling
                         ws = [adv.MLP_1.weight, val.MLP_1.weight]
                         cache = None if self._pack_cache is None else self._pack_cache.setdefault(group, {})
-                        h = relu_flat_linear3x(pre.y, ws, cache)
-                        vals[duel["out"]] = dueling_tail(h, adv.MLP_2.weight, val.MLP_2.weight)
+                        vals[duel["out"]] = relu_flat_heads_dueling(pre.y, ws, adv.MLP_2.weight, val.MLP_2.weight, cache)
                         for n in duel["inner"]:
                             vals[n] = None
                         continue
@@ -390,17 +399,44 @@ class GraphAgent(nn.Module):
         operand the input-gradient GEMM of a later backward pass needs (entry "bwdT").  Returns the cache
         entries it filled, which packed_heads_cache(packs) accepts."""
         built = {}
-        if self._pack_cache is None or not (self.dense_3xtf32 and self.fuse_sibling_heads):
+        if self._pack_cache is None:
             return built
         from .linear import _pack_pieces
-        for group in set(self._head_groups.values()):
+        for group, ws in self.head_pieces():
+            entry = built[group] = self._pack_cache.setdefault(group, {})
+            entry["bwdT" if transposed else "fwd"] = _pack_pieces(ws, transposed, True)
+        return built
+
+    def head_pieces(self):
+        """[(group, first-layer weights in operand order)] of the sibling head groups the 3xTF32 GEMM runs fused."""
+        if not (self.dense_3xtf32 and self.fuse_sibling_heads):
+            return []
+        out = []
+        for group in sorted(set(self._head_groups.values())):
             duel = self._dueling.get(group) if self.fused_dueling_tail else None
             names = (duel["adv"], duel["val"]) if duel is not None else group
             ws = [next(iter(getattr(self, n).children())).weight for n in names]
             if ws[0].is_cuda and not any(w.shape[0] % 32 for w in ws[:-1]):
-                entry = built[group] = self._pack_cache.setdefault(group, {})
-                entry["bwdT" if transposed else "fwd"] = _pack_pieces([w.detach() for w in ws], transposed, True)
-        return built
+                out.append((group, ws))
+        return out
+
+    def keep_resident_heads(self, transposed: bool) -> dict:
+        """Allocate and pack persistent operand images of the fused heads: "fwd" (and "bwdT", the W^T operand of
+        dL/dx, if `transposed`) per group, in the form packed_heads_cache(packs) takes.  See the rule in __init__."""
+        from .linear import _pack_pieces
+        self._resident = {group: {k: _pack_pieces(ws, k == "bwdT", True) for k in (("fwd", "bwdT") if transposed
+                                                                                else ("fwd",))}
+                          for group, ws in self.head_pieces()}
+        return self._resident
+
+    def refresh_resident_heads(self) -> None:
+        """Repack the resident images (in place: captured graphs keep reading them) from the current weights."""
+        if not self._resident:
+            return
+        from .linear import _pack_pieces
+        for group, ws in self.head_pieces():
+            for k, img in self._resident[group].items():
+                _pack_pieces(ws, k == "bwdT", True, out=img)
 
     def _prehead_group(self):
         """(group, (C, HW)) if the first conv node ends with [Conv2d, ReLU, Flatten] and feeds ONLY one dueling head
@@ -468,6 +504,7 @@ class GraphAgent(nn.Module):
             else:
                 torch._foreach_mul_(mine, 1 - tau)
                 torch._foreach_add_(mine, theirs, alpha=tau)
+        self.refresh_resident_heads()
 
     def calculateNorm(self):
         return sum(p.grad.norm(2) for p in self.parameters() if p.grad is not None)

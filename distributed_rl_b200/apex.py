@@ -205,6 +205,7 @@ class _StepState:
         self.prio_update = branch(target)
         self.max_w = SideBranch(packs)            # data parallel: the reduced max IS weight, for the next step
         self.head_packs = None                    # (online, target) heads' forward operands of this step
+        self.resident = None                      # (online, target) heads' persistent operand images, or None
         self.pack1 = self.pack2 = self.cur = self.y_big = self.sink = None
         if not L._conv1_ready():
             return
@@ -215,6 +216,19 @@ class _StepState:
                         w=torch.empty(B, dtype=torch.float32, device=dev))
         if cfg.PARALLEL_FORWARDS and cfg.BATCHED_ONLINE:
             self.y_big = torch.empty((3, B, 20, 20, self.pack1.c_out), dtype=torch.float32, device=dev)
+        if L._fused_optim:
+            # The heads' operand images live across steps: the fused optimizer rewrites the online ones whenever it
+            # steps the weights, and the target's change only at a target sync (GraphAgent.updateParameter repacks
+            # them).  torch.optim cannot maintain them: that configuration packs them every step.
+            on = L.model.keep_resident_heads(transposed=True)
+            tg = L.target_model.keep_resident_heads(transposed=False)
+            for group, ws in L.model.head_pieces():
+                off = 0
+                for w in ws:
+                    L.optim.write_images(w, on[group]["fwd"], on[group]["bwdT"],
+                                         sum(v.shape[0] for v in ws), off)
+                    off += w.shape[0]
+            self.resident = (on, tg) if on else None
         if cfg.DEFERRED_WGRAD and L._fused_optim:
             self.sink = WeightGradSink(dev)
             self.sink.grads_are_zero = True      # grads are pre-allocated and zeroed by the fused optimizer
@@ -395,7 +409,9 @@ class Learner(TargetNetLearner):
         w_tg = getattr(self.target_model, s.conv_name).conv_1.weight
         with s.conv1_packs.fork():
             R.conv1_pack_jobs([(s.pack1, 0, w_on), (s.pack2, 0, w_on), (s.pack2, 1, w_tg)])   # one launch
-        if self.cfg.PARALLEL_FORWARDS and self.cfg.BATCHED_ONLINE:
+        if s.resident is not None:
+            s.head_packs = s.resident
+        elif self.cfg.PARALLEL_FORWARDS and self.cfg.BATCHED_ONLINE:
             with s.head_packs_built.fork():
                 with self.model.packed_heads_cache():
                     on = self.model.prepack_heads()
@@ -420,7 +436,9 @@ class Learner(TargetNetLearner):
         s.conv1_packs.join()
         notdone = None
         batched = self.cfg.PARALLEL_FORWARDS and self.cfg.BATCHED_ONLINE
-        with self.model.packed_heads_cache(s.head_packs[0] if batched else None):   # online weights packed once
+        resident = s.resident is not None
+        on_packs, tg_packs = s.head_packs if (batched or resident) else (None, None)
+        with self.model.packed_heads_cache(on_packs):   # online weights packed once
             if batched:
                 # Q(s) (with grad) and Q_online(s') (without) share the online weights: every kernel after conv_1 is
                 # launch / set-up bound at B = 512 (DESIGN.md §6b), so both run as ONE B = 2*BATCHSIZE pass
@@ -438,13 +456,14 @@ class Learner(TargetNetLearner):
                     y_tg = R.conv1_fused(st.field_view("next_state"), idx, s.pack2, relu=True, out=big[1:3])[1]
                 s.head_packs_built.join()      # long done; the heads' GEMM is ~100 us away
                 with torch.no_grad():
-                    with s.target_pass.fork(), self.target_model.packed_heads_cache(s.head_packs[1]):
+                    with s.target_pass.fork(), self.target_model.packed_heads_cache(tg_packs):
                         qn_target = self.target_model.forward_from_conv1(y_tg, True)[0]  # :85
                     with s.side.fork():
                         if action.dtype != torch.int64:            # int32 replay field -> the target kernel's int64:
                             action = action.to(torch.int64)        # off the main branch (it sat in front of conv_1)
                         notdone = 1.0 - done.to(torch.float32)     # likewise (two launches in front of the target kernel)
-                        self.model.prepack_heads(transposed=True)   # W^T operand of the heads' dgrad, off the main branch
+                        if not resident:
+                            self.model.prepack_heads(transposed=True)   # W^T operand of the heads' dgrad, off the main branch
                     y_both = big[0:2].view(2 * B, 20, 20, c_out).permute(0, 3, 1, 2)     # logical NCHW, physical NHWC
                     with OutputTape.record() as tape:
                         q_all = self.model.forward_from_conv1(y_both, True)[0]          # :78 and :87 in one pass
@@ -456,14 +475,15 @@ class Learner(TargetNetLearner):
             else:
                 # Three separate passes, independent until the target kernel.  With PARALLEL_FORWARDS the two over s'
                 # fork onto two streams (parallel branches of the step's CUDA graph) so their small kernels overlap.
-                self.model.prepack_heads()
+                if not resident:
+                    self.model.prepack_heads()
                 with torch.no_grad():
                     y_on, y_tg = R.conv1_fused(st.field_view("next_state"), idx, s.pack2, relu=True)
                     with s.side.fork():
                         qn_online = self.model.forward_from_conv1(y_on, True)[0]        # :87
-                        if self.cfg.PARALLEL_FORWARDS:    # on one stream backward packs it beside its wgrad lanes
+                        if self.cfg.PARALLEL_FORWARDS and not resident:   # on one stream backward packs it beside its wgrad lanes
                             self.model.prepack_heads(transposed=True)   # W^T operand of the heads' dgrad, off the main branch
-                    with s.target_pass.fork():
+                    with s.target_pass.fork(), self.target_model.packed_heads_cache(tg_packs):
                         qn_target = self.target_model.forward_from_conv1(y_tg, True)[0]  # :85
                 y = _Conv1Gathered.apply(w_on, st.field_view("state"), idx, s.pack1, self._mf, st, None, True)
                 q = self.model.forward_from_conv1(y, True)[0]                        # :78 (ReLU in the conv_1 epilogue)

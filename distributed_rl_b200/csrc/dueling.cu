@@ -32,18 +32,59 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+constexpr int STAGE_UNROLL = 8;      // float4 loads in flight per thread while the CTA stages its rows of h
+
 // q[m][j] ; one warp per row, lane owns columns lane, lane+32, ...; the A+1 dot products are accumulated as
-// independent chains and reduced together so that the shuffle latencies overlap
+// independent chains and reduced together so that the shuffle latencies overlap.
+// h: `splits` K-split partials [split][M][2H] of the heads' first-layer GEMM, `split_stride` floats apart.  The CTA
+// first stages its ROWS_PER_CTA rows in SMEM, summing the partials in split order (the sum k_splitk_reduce forms);
+// every thread keeps STAGE_UNROLL independent float4 loads in flight per split, so the sum runs at memory speed
+// although a warp owns a whole row afterwards.  h_out (may be null) receives the summed rows.
 template <int A_MAX>
 __global__ void __launch_bounds__(ROWS_PER_CTA * 32)
-k_dueling_forward(const float* __restrict__ h, int M, int H, const float* __restrict__ wa, int A,
-                  const float* __restrict__ wv, float* __restrict__ q) {
-  extern __shared__ float s_w[];                       // [A + 1][H]: Wa rows, then Wv
+k_dueling_forward(const float* __restrict__ h, int splits, int64_t split_stride, int M, int H,
+                  const float* __restrict__ wa, int A, const float* __restrict__ wv, float* __restrict__ q,
+                  float* __restrict__ h_out) {
+  extern __shared__ float s_w[];                       // [A + 1][H]: Wa rows, then Wv; then [ROWS_PER_CTA][2H] of h
+  float* s_h = s_w + A * H + H;
   load_weights(s_w, wa, wv, A, H);
+  {
+    const int m0 = blockIdx.x * ROWS_PER_CTA;
+    const int n4 = (min(ROWS_PER_CTA, M - m0) * 2 * H) >> 2;          // float4s of this CTA's rows (contiguous)
+    const float4* src = reinterpret_cast<const float4*>(h + (int64_t)m0 * 2 * H);
+    const int64_t z4 = split_stride >> 2;
+    float4* dst = h_out ? reinterpret_cast<float4*>(h_out + (int64_t)m0 * 2 * H) : nullptr;
+    for (int i0 = threadIdx.x; i0 < n4; i0 += ROWS_PER_CTA * 32 * STAGE_UNROLL) {
+      float4 v[STAGE_UNROLL];
+#pragma unroll
+      for (int u = 0; u < STAGE_UNROLL; ++u) {
+        const int i = i0 + u * ROWS_PER_CTA * 32;
+        v[u] = (i < n4) ? src[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      for (int z = 1; z < splits; ++z) {
+#pragma unroll
+        for (int u = 0; u < STAGE_UNROLL; ++u) {
+          const int i = i0 + u * ROWS_PER_CTA * 32;
+          if (i < n4) {
+            const float4 w = src[z * z4 + i];
+            v[u].x += w.x; v[u].y += w.y; v[u].z += w.z; v[u].w += w.w;
+          }
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < STAGE_UNROLL; ++u) {
+        const int i = i0 + u * ROWS_PER_CTA * 32;
+        if (i < n4) {
+          reinterpret_cast<float4*>(s_h)[i] = v[u];
+          if (dst) dst[i] = v[u];
+        }
+      }
+    }
+  }
   __syncthreads();
   const int lane = threadIdx.x & 31, m = blockIdx.x * ROWS_PER_CTA + (threadIdx.x >> 5);
   if (m >= M) return;
-  const float* hr = h + (int64_t)m * 2 * H;
+  const float* hr = s_h + (threadIdx.x >> 5) * 2 * H;
   float s[A_MAX], val = 0.0f;
 #pragma unroll
   for (int j = 0; j < A_MAX; ++j) s[j] = 0.0f;
@@ -187,24 +228,31 @@ static cudaError_t dueling_smem(const void* fn, size_t bytes) {
                            : cudaSuccess;
 }
 
-extern "C" int b2rl_dueling_forward(const float* h_dev, int64_t M, int64_t H, const float* wa_dev, int64_t A,
-                                    const float* wv_dev, float* q_dev, void* stream) {
+extern "C" int b2rl_dueling_forward(const float* h_dev, int32_t splits, int64_t split_stride, int64_t M, int64_t H,
+                                    const float* wa_dev, int64_t A, const float* wv_dev, float* q_dev, float* h_out_dev,
+                                    void* stream) {
   if (int rc = dueling_check(h_dev, M, H, A)) return rc;
   B2RL_REQUIRE(wa_dev && wv_dev && q_dev, "null argument");
   B2RL_REQUIRE(((uintptr_t)wa_dev % 16) == 0 && ((uintptr_t)wv_dev % 16) == 0, "weights must be 16-byte aligned");
-  const size_t smem = (size_t)(A + 1) * H * sizeof(float);
+  B2RL_REQUIRE(((uintptr_t)h_dev % 16) == 0 && ((uintptr_t)h_out_dev % 16) == 0, "h must be 16-byte aligned");
+  B2RL_REQUIRE(splits >= 1 && (splits == 1 || (split_stride >= M * 2 * H && split_stride % 4 == 0)),
+               "bad split-K partials");
+  const size_t smem = (size_t)(A + 1 + 2 * dueling::ROWS_PER_CTA) * H * sizeof(float);
   const unsigned grid = (unsigned)((M + dueling::ROWS_PER_CTA - 1) / dueling::ROWS_PER_CTA);
   const unsigned block = dueling::ROWS_PER_CTA * 32;
   cudaStream_t st = (cudaStream_t)stream;
   if (A <= 8) {
     B2RL_CUDA(dueling_smem((const void*)dueling::k_dueling_forward<8>, smem));
-    dueling::k_dueling_forward<8><<<grid, block, smem, st>>>(h_dev, (int)M, (int)H, wa_dev, (int)A, wv_dev, q_dev);
+    dueling::k_dueling_forward<8><<<grid, block, smem, st>>>(h_dev, splits, split_stride, (int)M, (int)H, wa_dev,
+                                                                 (int)A, wv_dev, q_dev, h_out_dev);
   } else if (A <= 16) {
     B2RL_CUDA(dueling_smem((const void*)dueling::k_dueling_forward<16>, smem));
-    dueling::k_dueling_forward<16><<<grid, block, smem, st>>>(h_dev, (int)M, (int)H, wa_dev, (int)A, wv_dev, q_dev);
+    dueling::k_dueling_forward<16><<<grid, block, smem, st>>>(h_dev, splits, split_stride, (int)M, (int)H, wa_dev,
+                                                                 (int)A, wv_dev, q_dev, h_out_dev);
   } else {
     B2RL_CUDA(dueling_smem((const void*)dueling::k_dueling_forward<32>, smem));
-    dueling::k_dueling_forward<32><<<grid, block, smem, st>>>(h_dev, (int)M, (int)H, wa_dev, (int)A, wv_dev, q_dev);
+    dueling::k_dueling_forward<32><<<grid, block, smem, st>>>(h_dev, splits, split_stride, (int)M, (int)H, wa_dev,
+                                                                 (int)A, wv_dev, q_dev, h_out_dev);
   }
   count_launch();
   B2RL_CHECK_LAUNCH();

@@ -13,16 +13,19 @@
 //   k_gemm_tf32x3  one CTA per (m-tile 128, n-tile 256, K-split): a TMA loader warp and two consumer
 //                  warpgroups (64 rows each, 12 x wgmma m64n256k8 per 32-float K chunk) that store the tile
 //                  (or, when K is split, this split's partial tile) straight from their accumulators
-//   k_splitk_reduce sums the K-split partials in split order: the result is deterministic (no atomics)
+//   k_splitk_reduce sums the K-split partials in split order: the result is deterministic (no atomics).
+//                  b2rl_gemm_tf32x3_partials leaves the partials in memory instead, for a consumer that sums them
+//                  in the same order while it reads its input (k_dueling_forward, k_unflatten_relu_mask)
 #include "common.cuh"
 #include "hopper.cuh"
+#include "operand_image.cuh"
 
 namespace b2rl {
 namespace gemm {
 
 using namespace sm90;
 
-constexpr int TM = 128, TN = 256, KC = 32;          // tile rows of A / of B, floats per K chunk (128 B)
+constexpr int TM = 128, TN = 256, KC = image::KC;   // tile rows of A / of B, floats per K chunk (128 B)
 constexpr int A_TILE = TM * 128, B_TILE = TN * 128;  // bytes of one {term, k-chunk} tile: 16 KiB / 32 KiB
 constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;       // hi+lo of both operands: 96 KiB
 constexpr int STAGES = 2;
@@ -30,20 +33,10 @@ constexpr int CONSUMERS = 256;                       // warpgroups 0-1: MMA + ep
 constexpr int THREADS = CONSUMERS + 32;              // warp 8: TMA loader
 
 // ---- operand packing ---------------------------------------------------------
-// Image layout: [term 0=hi,1=lo][k_chunk][row_tile][row_in_tile][128 B, 16-byte units XOR (row & 7)]
-// One CTA per (32 operand rows, one K chunk); thread = (row r = tid / 8, 16-byte unit = tid % 8), so
+// Image layout: operand_image.cuh.  One CTA per (32 operand rows, one K chunk); thread = (row r = tid / 8, 16-byte unit = tid % 8), so
 // both the source row segment and the image row are one contiguous 128 B per 8 threads.
 // TRANSPOSE: the operand's rows are the source's columns; the 32x32 block goes through SMEM so that
 // the source is still read along its contiguous dimension.
-__device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
-  const uint32_t u = __float_as_uint(x);
-  uint32_t h = (u + 0x1000u) & 0xFFFFE000u;                        // round to nearest on the 13 dropped bits
-  if ((h & 0x7F800000u) == 0x7F800000u) h = u & 0xFFFFE000u;        // rounding reached inf (or x is inf/nan): truncate
-  hi = __uint_as_float(h);
-  lo = ((u & 0x7F800000u) == 0x7F800000u) ? 0.0f : x - hi;          // exact in fp32
-  if ((u & 0x7F800000u) == 0x7F800000u) hi = x;
-}
-
 template <bool TRANSPOSE>
 __global__ void __launch_bounds__(256)
 k_split_pack(const float* __restrict__ src, int src_rows, int src_cols, int64_t src_ld, int tile_rows,
@@ -77,15 +70,7 @@ k_split_pack(const float* __restrict__ src, int src_rows, int src_cols, int64_t 
   }
   const int irow = row_off + row, ikc = kc_off + kc;
   if (irow >= rows_pad) return;
-  float hi[4], lo[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) split_tf32(v[e], hi[e], lo[e]);
-  const int rt = irow / tile_rows, rr = irow - rt * tile_rows;
-  const int tiles = rows_pad / tile_rows;
-  const int64_t off = (((int64_t)ikc * tiles + rt) * tile_rows + rr) * 32 + ((unit ^ (rr & 7)) << 2);
-  const int64_t term_stride = (int64_t)k_chunks * rows_pad * 32;
-  *reinterpret_cast<float4*>(out + off) = make_float4(hi[0], hi[1], hi[2], hi[3]);
-  *reinterpret_cast<float4*>(out + term_stride + off) = make_float4(lo[0], lo[1], lo[2], lo[3]);
+  image::store_unit(out, image::offset(irow, ikc, unit, tile_rows, rows_pad), image::term_stride(k_chunks, rows_pad), v);
 }
 
 // ---- activation-side packs that fold act_3 (ReLU) + nn.Flatten into the heads' operand images ----------------
@@ -120,8 +105,7 @@ k_pack_act_nhwc(const float* __restrict__ y, int B, int HW, int C, int relu, flo
       }
     }
     __syncthreads();
-    const int rt = b / TM, rr = b - rt * TM, tiles = rows_pad / TM;
-    const int64_t term_stride = (int64_t)k_chunks * rows_pad * 32;
+    const int64_t ts = image::term_stride(k_chunks, rows_pad);
     for (int w = threadIdx.x; w < k_chunks * 8; w += 256) {
       const int kc = w >> 3, unit = w & 7;
       const int f0 = kc * KC + unit * 4;
@@ -132,12 +116,7 @@ k_pack_act_nhwc(const float* __restrict__ y, int B, int HW, int C, int relu, flo
         v[e] = (b < B && f0 + e < K) ? s_act[hw * ld + c] : 0.0f;
         if (++hw == HW) { hw = 0; ++c; }
       }
-      float hi[4], lo[4];
-#pragma unroll
-      for (int e = 0; e < 4; ++e) split_tf32(v[e], hi[e], lo[e]);
-      const int64_t off = (((int64_t)kc * tiles + rt) * TM + rr) * 32 + ((unit ^ (rr & 7)) << 2);
-      *reinterpret_cast<float4*>(out + off) = make_float4(hi[0], hi[1], hi[2], hi[3]);
-      *reinterpret_cast<float4*>(out + term_stride + off) = make_float4(lo[0], lo[1], lo[2], lo[3]);
+      image::store_unit(out, image::offset(b, kc, unit, TM, rows_pad), ts, v);
     }
   } else {
     // one CTA per (chunk of 32 b's, hw): s[b][c], row stride C + 1; image rows f = c*HW + hw, contraction = b
@@ -150,20 +129,13 @@ k_pack_act_nhwc(const float* __restrict__ y, int B, int HW, int C, int relu, flo
       s_act[bb * ld + c] = v;
     }
     __syncthreads();
-    const int tiles = rows_pad / TN;
-    const int64_t term_stride = (int64_t)k_chunks * rows_pad * 32;
+    const int64_t ts = image::term_stride(k_chunks, rows_pad);
     for (int w = threadIdx.x; w < C * 8; w += 256) {
       const int c = w >> 3, unit = w & 7;
-      const int f = c * HW + hw;
-      float v[4], hi[4], lo[4];
+      float v[4];
 #pragma unroll
       for (int e = 0; e < 4; ++e) v[e] = s_act[(unit * 4 + e) * ld + c];
-#pragma unroll
-      for (int e = 0; e < 4; ++e) split_tf32(v[e], hi[e], lo[e]);
-      const int rt = f / TN, rr = f - rt * TN;
-      const int64_t off = (((int64_t)kc * tiles + rt) * TN + rr) * 32 + ((unit ^ (rr & 7)) << 2);
-      *reinterpret_cast<float4*>(out + off) = make_float4(hi[0], hi[1], hi[2], hi[3]);
-      *reinterpret_cast<float4*>(out + term_stride + off) = make_float4(lo[0], lo[1], lo[2], lo[3]);
+      image::store_unit(out, image::offset(c * HW + hw, kc, unit, TN, rows_pad), ts, v);
     }
   }
 }
@@ -171,27 +143,31 @@ k_pack_act_nhwc(const float* __restrict__ y, int B, int HW, int C, int relu, flo
 // zero rows [K, rows_pad) of the x^T image (the padding of the last row tile)
 __global__ void __launch_bounds__(256)
 k_pack_zero_rows(float* __restrict__ out, int row0, int rows_pad, int k_chunks, int tile_rows) {
-  const int tiles = rows_pad / tile_rows;
-  const int64_t term_stride = (int64_t)k_chunks * rows_pad * 32;
+  const int64_t ts = image::term_stride(k_chunks, rows_pad);
   const int n_rows = rows_pad - row0;
   const int64_t total = (int64_t)n_rows * k_chunks * 8;
+  const float zero[4] = {0.f, 0.f, 0.f, 0.f};
   for (int64_t w = (int64_t)blockIdx.x * 256 + threadIdx.x; w < total; w += (int64_t)gridDim.x * 256) {
     const int unit = (int)(w & 7);
     const int64_t q = w >> 3;
     const int kc = (int)(q / n_rows), f = row0 + (int)(q - (int64_t)kc * n_rows);
-    const int rt = f / tile_rows, rr = f - rt * tile_rows;
-    const int64_t off = (((int64_t)kc * tiles + rt) * tile_rows + rr) * 32 + ((unit ^ (rr & 7)) << 2);
-    *reinterpret_cast<float4*>(out + off) = make_float4(0.f, 0.f, 0.f, 0.f);
-    *reinterpret_cast<float4*>(out + term_stride + off) = make_float4(0.f, 0.f, 0.f, 0.f);
+    image::store_unit(out, image::offset(f, kc, unit, tile_rows, rows_pad), ts, zero);
   }
 }
 
+// gx: `splits` K-split partials of dL/dx, `split_stride` floats apart, summed here in split order (the same sum
+// k_splitk_reduce forms)
 __global__ void __launch_bounds__(256)
-k_unflatten_relu_mask(const float* __restrict__ gx, int64_t gx_ld, const float* __restrict__ y, int HW, int C,
-                      float* __restrict__ out) {
+k_unflatten_relu_mask(const float* __restrict__ gx, int64_t gx_ld, int splits, int64_t split_stride,
+                      const float* __restrict__ y, int HW, int C, float* __restrict__ out) {
   extern __shared__ float s_act[];          // gx row in f order: s[c*HW + hw]
   const int b = blockIdx.x, K = C * HW;
-  for (int i = threadIdx.x; i < K; i += 256) s_act[i] = gx[(int64_t)b * gx_ld + i];
+  const float* gr = gx + (int64_t)b * gx_ld;
+  for (int i = threadIdx.x; i < K; i += 256) {
+    float v = gr[i];
+    for (int z = 1; z < splits; ++z) v += gr[z * split_stride + i];
+    s_act[i] = v;
+  }
   __syncthreads();
   const float* yr = y + (int64_t)b * K;
   float* o = out + (int64_t)b * K;
@@ -392,6 +368,40 @@ extern "C" int64_t b2rl_gemm_workspace_floats(int64_t M, int64_t N, int64_t K, i
   return splits > 1 ? splits * M * ldc : 0;
 }
 
+// k_gemm_tf32x3 alone: C (splits == 1) or the K-split partials [split][M][ldc] stored at `out`
+static int gemm_launch(const float* a_packed_dev, const float* b_packed_dev, float* out, int64_t M, int64_t N,
+                       int64_t K, int64_t ldc, int64_t splits, cudaStream_t st) {
+  int dev = 0;
+  B2RL_CUDA(cudaGetDevice(&dev));
+  const size_t smem_bytes = (size_t)gemm::STAGES * gemm::STAGE + 1024;
+  B2RL_CUDA(set_max_dynamic_smem<gemm::k_gemm_tf32x3>(dev, smem_bytes));
+  gemm::Params P{};
+  P.a = a_packed_dev; P.b = b_packed_dev;
+  P.c = out;
+  P.M = M; P.N = N; P.ldc = ldc;
+  P.m_tiles = (M + gemm::TM - 1) / gemm::TM;
+  P.n_tiles = (N + gemm::TN - 1) / gemm::TN;
+  P.k_chunks = (K + gemm::KC - 1) / gemm::KC;
+  P.splits = (int32_t)splits;
+  dim3 grid((unsigned)P.m_tiles, (unsigned)P.n_tiles, (unsigned)splits);
+  gemm::k_gemm_tf32x3<<<grid, gemm::THREADS, smem_bytes, st>>>(P);
+  count_launch();
+  B2RL_CHECK_LAUNCH();
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_gemm_tf32x3_partials(const float* a_packed_dev, const float* b_packed_dev, float* partials_dev,
+                                         int64_t M, int64_t N, int64_t K, int64_t ldc, void* stream) {
+  B2RL_REQUIRE(a_packed_dev && b_packed_dev && partials_dev, "null argument");
+  B2RL_REQUIRE(M >= 1 && N >= 1 && K >= 1 && ldc >= N, "bad shape");
+  B2RL_REQUIRE(((uintptr_t)partials_dev % 16) == 0 && (ldc % 4) == 0,
+               "partials must be 16-byte aligned with ldc % 4 == 0");
+  int sms = 0;
+  if (int rc = gemm_sms(&sms)) return rc;
+  return gemm_launch(a_packed_dev, b_packed_dev, partials_dev, M, N, K, ldc, gemm_splits(M, N, K, sms),
+                     (cudaStream_t)stream);
+}
+
 extern "C" int b2rl_gemm_tf32x3(const float* a_packed_dev, const float* b_packed_dev, float* c_dev, int64_t M,
                                 int64_t N, int64_t K, int64_t ldc, float* workspace_dev, void* stream) {
   B2RL_REQUIRE(a_packed_dev && b_packed_dev && c_dev, "null argument");
@@ -399,26 +409,12 @@ extern "C" int b2rl_gemm_tf32x3(const float* a_packed_dev, const float* b_packed
   B2RL_REQUIRE(((uintptr_t)c_dev % 16) == 0 && (ldc % 4) == 0, "C must be 16-byte aligned with ldc % 4 == 0");
   int sms = 0;
   if (int rc = gemm_sms(&sms)) return rc;
-  int dev = 0;
-  B2RL_CUDA(cudaGetDevice(&dev));
-  const size_t smem_bytes = (size_t)gemm::STAGES * gemm::STAGE + 1024;
-  B2RL_CUDA(set_max_dynamic_smem<gemm::k_gemm_tf32x3>(dev, smem_bytes));
   const int64_t splits = gemm_splits(M, N, K, sms);
   B2RL_REQUIRE(splits == 1 || (workspace_dev && ((uintptr_t)workspace_dev % 16) == 0),
                "this shape splits K: pass b2rl_gemm_workspace_floats() floats of 16-byte aligned workspace");
-  gemm::Params P{};
-  P.a = a_packed_dev; P.b = b_packed_dev;
-  P.c = splits > 1 ? workspace_dev : c_dev;
-  P.M = M; P.N = N; P.ldc = ldc;
-  P.m_tiles = (M + gemm::TM - 1) / gemm::TM;
-  P.n_tiles = (N + gemm::TN - 1) / gemm::TN;
-  P.k_chunks = (K + gemm::KC - 1) / gemm::KC;
-  P.splits = (int32_t)splits;
   cudaStream_t st = (cudaStream_t)stream;
-  dim3 grid((unsigned)P.m_tiles, (unsigned)P.n_tiles, (unsigned)splits);
-  gemm::k_gemm_tf32x3<<<grid, gemm::THREADS, smem_bytes, st>>>(P);
-  count_launch();
-  B2RL_CHECK_LAUNCH();
+  if (int rc = gemm_launch(a_packed_dev, b_packed_dev, splits > 1 ? workspace_dev : c_dev, M, N, K, ldc, splits, st))
+    return rc;
   if (splits > 1) {
     const int64_t quads = M * (ldc >> 2);
     gemm::k_splitk_reduce<<<(unsigned)((quads + 255) / 256), 256, 0, st>>>(workspace_dev, (int)splits, M, N, ldc, c_dev);
@@ -464,13 +460,16 @@ extern "C" int b2rl_gemm_pack_act_nhwc(const float* y_dev, int64_t B, int64_t HW
 
 // The backward counterpart: dL/dy (NHWC, [B][HW][C]) = dL/dx (NCHW-flatten order, [B][gx_ld]) permuted back and
 // masked by the ReLU (y > 0) — nn.Flatten's and act_3's backward in one launch.
-extern "C" int b2rl_unflatten_relu_mask(const float* gx_dev, int64_t gx_ld, const float* y_dev, int64_t B, int64_t HW,
-                                        int64_t C, float* out_dev, void* stream) {
+extern "C" int b2rl_unflatten_relu_mask(const float* gx_dev, int64_t gx_ld, int32_t splits, int64_t split_stride,
+                                        const float* y_dev, int64_t B, int64_t HW, int64_t C, float* out_dev,
+                                        void* stream) {
   B2RL_REQUIRE(gx_dev && y_dev && out_dev, "null argument");
   B2RL_REQUIRE(B >= 1 && HW >= 1 && C >= 1 && gx_ld >= C * HW, "bad shape");
+  B2RL_REQUIRE(splits >= 1 && (splits == 1 || split_stride >= B * gx_ld), "bad split-K partials");
   const size_t smem = (size_t)C * HW * sizeof(float);
   B2RL_REQUIRE(smem <= 48 * 1024, "activation row too large for the staging tile");
-  gemm::k_unflatten_relu_mask<<<(unsigned)B, 256, smem, (cudaStream_t)stream>>>(gx_dev, gx_ld, y_dev, (int)HW, (int)C, out_dev);
+  gemm::k_unflatten_relu_mask<<<(unsigned)B, 256, smem, (cudaStream_t)stream>>>(gx_dev, gx_ld, splits, split_stride,
+                                                                              y_dev, (int)HW, (int)C, out_dev);
   count_launch();
   B2RL_CHECK_LAUNCH();
   return B2RL_OK;

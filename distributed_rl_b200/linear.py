@@ -89,6 +89,11 @@ class WeightGradSink:
         with self.lanes[lane].fork(after_current=False):
             fn()
 
+    def after_current(self, lane: int = 0):
+        """The lane's later work waits for what the current stream has queued so far."""
+        with self.lanes[lane].fork():
+            pass
+
     def accumulate(self, param, grad):
         """(side stream) param.grad += grad, then the parameter's ready callback."""
         param.grad.add_(grad)
@@ -243,13 +248,31 @@ def gemm_packed(a: torch.Tensor, b: torch.Tensor, M: int, N: int, K: int, out: t
     return out
 
 
-def _pack_pieces(mats, transpose: bool, b_role: bool) -> torch.Tensor:
+def gemm_partials(a: torch.Tensor, b: torch.Tensor, M: int, N: int, K: int):
+    """A[M][K] @ B[N][K]^T from packed operand images, left as its K-split partials (b2rl_gemm_tf32x3_partials):
+    -> (partials, splits, ldc); partial z is rows [z*M, (z+1)*M) of partials viewed [splits*M][ldc].  Summed in
+    split order they are gemm_packed's result, bit for bit."""
+    L = _lib.load()
+    ldc = (N + 3) // 4 * 4
+    n_ws = L.b2rl_gemm_workspace_floats(M, N, K, ldc)
+    splits = n_ws // (M * ldc) if n_ws else 1
+    part = torch.empty(splits * M * ldc, dtype=torch.float32, device=a.device)
+    _lib.check(L.b2rl_gemm_tf32x3_partials(a.data_ptr(), b.data_ptr(), part.data_ptr(), M, N, K, ldc, _stream()))
+    return part, splits, ldc
+
+
+def _pack_pieces(mats, transpose: bool, b_role: bool, out: torch.Tensor | None = None) -> torch.Tensor:
     """Operand image of vertically stacked matrices (transpose=False: rows stack) or of the transpose of
-    that stack (transpose=True: the pieces sit side by side along the contraction index)."""
+    that stack (transpose=True: the pieces sit side by side along the contraction index).  `out`: an existing
+    image of that shape to overwrite."""
     L = _lib.load()
     inner, total = mats[0].shape[1], sum(m.shape[0] for m in mats)
     rows, k = (inner, total) if transpose else (total, inner)
-    out = torch.empty(L.b2rl_gemm_packed_floats(rows, k, int(b_role)), dtype=torch.float32, device=mats[0].device)
+    n = L.b2rl_gemm_packed_floats(rows, k, int(b_role))
+    if out is None:
+        out = torch.empty(n, dtype=torch.float32, device=mats[0].device)
+    elif out.numel() != n or not out.is_contiguous():
+        raise ValueError("`out` is not an image of this operand")
     off = 0
     for m in mats:
         if m.stride(1) != 1:
@@ -306,6 +329,7 @@ class _Linear3x(torch.autograd.Function):
             # dx[M][K] = gy[M][N] @ W[N][K]: contraction over N, the B operand is W^T ([K rows][N])
             bt = ctx.cache.get("bwdT") if ctx.cache is not None else None     # prepared ahead (GraphAgent.prepack_heads)
             gx = gemm_packed(split_pack(gy, False, False), bt if bt is not None else _pack_pieces(ws, True, True), M, K, N)
+            _images_read()
         return (gx, None, *gws)
 
 
@@ -334,38 +358,55 @@ class _ReluFlatLinear3x(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gh):
         y, *ws = ctx.saved_tensors
-        B, C, H, W = y.shape
-        N, K = sum(w.shape[0] for w in ws), C * H * W
-        gh = gh.contiguous()
-        gy, gws = None, [None] * len(ws)
-        if any(ctx.needs_input_grad[2:]):
-            def wgrad():
-                gw = gemm_packed(split_pack(gh, True, False), pack_act_nhwc(y, True), N, K, B)
-                return list(torch.split(gw, [w.shape[0] for w in ws], 0))
-            if WeightGradSink.usable(ws):       # before dL/dy is launched: runs beside it (see _Linear3x.backward)
-                sink = _SINK
-
-                def deferred():
-                    joint = _stacked_rows([w.grad for w in ws]) if sink.grads_are_zero else None
-                    if joint is not None and not any(id(w) in sink.accumulated[0] for w in ws):
-                        # the GEMM writes dW of all sibling heads straight into their (adjacent, zero) .grad rows:
-                        # no temporary and no 6.4 MB grad.add_ per head (the heads' all-reduce starts that much earlier)
-                        gemm_packed(split_pack(gh, True, False), pack_act_nhwc(y, True), N, K, B, out=joint)
-                        for w in ws:
-                            sink.written(w)
-                    else:
-                        for w, g in zip(ws, wgrad()):
-                            sink.accumulate(w, g)
-                sink.submit(deferred, keep=(gh, y))
-            else:
-                gws = wgrad()
-        if ctx.needs_input_grad[0]:
-            bt = ctx.cache.get("bwdT") if ctx.cache is not None else None
-            gx = gemm_packed(split_pack(gh, False, False), bt if bt is not None else _pack_pieces(ws, True, True), B, K, N)
-            gy = torch.empty_like(y)                                         # channels_last like y
-            _lib.check(_lib.load().b2rl_unflatten_relu_mask(gx.data_ptr(), gx.stride(0), y.data_ptr(), B, H * W, C,
-                                                           gy.data_ptr(), _stream()))
+        gy, gws = _relu_flat_backward(y, ws, ctx.cache, gh, ctx.needs_input_grad[0], any(ctx.needs_input_grad[2:]))
         return (gy, None, *gws)
+
+
+def _relu_flat_backward(y, ws, cache, gh, need_gy: bool, need_gw: bool):
+    """Backward of h = flatten_NCHW(relu(y)) @ cat(ws, 0).T -> (dL/dy or None, [dL/dW_i or None]).  The weight
+    gradients go to the active WeightGradSink when there is one."""
+    B, C, H, W = y.shape
+    N, K = sum(w.shape[0] for w in ws), C * H * W
+    gh = gh.contiguous()
+    gy, gws = None, [None] * len(ws)
+    if need_gw:
+        def wgrad():
+            gw = gemm_packed(split_pack(gh, True, False), pack_act_nhwc(y, True), N, K, B)
+            return list(torch.split(gw, [w.shape[0] for w in ws], 0))
+        if WeightGradSink.usable(ws):       # before dL/dy is launched: runs beside it (see _Linear3x.backward)
+            sink = _SINK
+
+            def deferred():
+                joint = _stacked_rows([w.grad for w in ws]) if sink.grads_are_zero else None
+                if joint is not None and not any(id(w) in sink.accumulated[0] for w in ws):
+                    # the GEMM writes dW of all sibling heads straight into their (adjacent, zero) .grad rows:
+                    # no temporary and no 6.4 MB grad.add_ per head (the heads' all-reduce starts that much earlier)
+                    gemm_packed(split_pack(gh, True, False), pack_act_nhwc(y, True), N, K, B, out=joint)
+                    for w in ws:
+                        sink.written(w)
+                else:
+                    for w, g in zip(ws, wgrad()):
+                        sink.accumulate(w, g)
+            sink.submit(deferred, keep=(gh, y))
+        else:
+            gws = wgrad()
+    if need_gy:
+        bt = cache.get("bwdT") if cache is not None else None
+        # dL/dx stays as its K-split partials: the unflatten + ReLU-mask kernel sums them while it reads them
+        gx, splits, ld = gemm_partials(split_pack(gh, False, False), bt if bt is not None else _pack_pieces(ws, True, True),
+                                       B, K, N)
+        gy = torch.empty_like(y)                                         # channels_last like y
+        _lib.check(_lib.load().b2rl_unflatten_relu_mask(gx.data_ptr(), ld, splits, B * ld, y.data_ptr(), B, H * W, C,
+                                                       gy.data_ptr(), _stream()))
+        _images_read()
+    return gy, gws
+
+
+def _images_read():
+    """dL/dx of the heads has been issued.  The heads' lane steps their weights early (FusedRMSprop.step_early), and
+    that update rewrites the weights' resident W^T operand image the dL/dx GEMM reads: order the lane behind it."""
+    if _SINK is not None:
+        _SINK.after_current(0)
 
 
 def _stacked_rows(ts):
@@ -419,8 +460,8 @@ class _DuelingTail(torch.autograd.Function):
 
         def compute():
             q = torch.empty(M, A, dtype=torch.float32, device=h.device)
-            _lib.check(_lib.load().b2rl_dueling_forward(h.data_ptr(), M, H, wa.data_ptr(), A, wv.data_ptr(), q.data_ptr(),
-                                                        _stream()))
+            _lib.check(_lib.load().b2rl_dueling_forward(h.data_ptr(), 1, 0, M, H, wa.data_ptr(), A, wv.data_ptr(),
+                                                        q.data_ptr(), None, _stream()))
             return q
         q = taped(compute)
         ctx.save_for_backward(h, wa, wv)
@@ -429,32 +470,87 @@ class _DuelingTail(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gq):
         h, wa, wv = ctx.saved_tensors
-        M, H2 = h.shape
-        A, H = wa.shape
-        gq = gq.contiguous()
-        gh = torch.empty_like(h) if ctx.needs_input_grad[0] else None
-        need_w = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
-        L = _lib.load()
-        row_ws = torch.empty(M * (A + 1), dtype=torch.float32, device=h.device)
-        defer = need_w and WeightGradSink.usable((wa, wv))
-        gwa = torch.empty_like(wa) if need_w else None
-        gwv = torch.empty_like(wv) if need_w else None
-        # row pass (dL/dh + the per-row table) on this stream; the column pass (dL/dW) here or on the sink's stream
-        _lib.check(L.b2rl_dueling_backward(h.data_ptr(), gq.data_ptr(), M, H, wa.data_ptr(), A, wv.data_ptr(),
-                                           gh.data_ptr() if gh is not None else None,
-                                           None if (defer or not need_w) else gwa.data_ptr(),
-                                           None if (defer or not need_w) else gwv.data_ptr(), row_ws.data_ptr(), _stream()))
-        if defer:
-            sink = _SINK
+        return _dueling_backward(h, wa, wv, gq, ctx.needs_input_grad[0], ctx.needs_input_grad[1] or ctx.needs_input_grad[2])
 
-            def deferred():
-                _lib.check(L.b2rl_dueling_backward_w(h.data_ptr(), row_ws.data_ptr(), M, H, A, gwa.data_ptr(),
-                                                     gwv.data_ptr(), _stream()))
-                sink.accumulate(wa, gwa)
-                sink.accumulate(wv, gwv)
-            sink.submit(deferred, keep=(h, row_ws, gwa, gwv))
-            return gh, None, None
-        return gh, gwa, gwv
+
+def _dueling_backward(h, wa, wv, gq, need_gh: bool, need_w: bool):
+    """Backward of the dueling tail -> (dL/dh, dL/dWa, dL/dWv); each None when not needed, the weights' also when
+    the active WeightGradSink takes them."""
+    M, H2 = h.shape
+    A, H = wa.shape
+    gq = gq.contiguous()
+    gh = torch.empty_like(h) if need_gh else None
+    L = _lib.load()
+    row_ws = torch.empty(M * (A + 1), dtype=torch.float32, device=h.device)
+    defer = need_w and WeightGradSink.usable((wa, wv))
+    gwa = torch.empty_like(wa) if need_w else None
+    gwv = torch.empty_like(wv) if need_w else None
+    # row pass (dL/dh + the per-row table) on this stream; the column pass (dL/dW) here or on the sink's stream
+    _lib.check(L.b2rl_dueling_backward(h.data_ptr(), gq.data_ptr(), M, H, wa.data_ptr(), A, wv.data_ptr(),
+                                       gh.data_ptr() if gh is not None else None,
+                                       None if (defer or not need_w) else gwa.data_ptr(),
+                                       None if (defer or not need_w) else gwv.data_ptr(), row_ws.data_ptr(), _stream()))
+    if defer:
+        sink = _SINK
+
+        def deferred():
+            _lib.check(L.b2rl_dueling_backward_w(h.data_ptr(), row_ws.data_ptr(), M, H, A, gwa.data_ptr(),
+                                                 gwv.data_ptr(), _stream()))
+            sink.accumulate(wa, gwa)
+            sink.accumulate(wv, gwv)
+        sink.submit(deferred, keep=(h, row_ws, gwa, gwv))
+        return gh, None, None
+    return gh, gwa, gwv
+
+
+class _ReluFlatHeadsDueling(torch.autograd.Function):
+    """Q = dueling_tail(relu_flat_linear3x(y, ws), wa, wv) with the heads' GEMM left as its K-split partials, which
+    the dueling forward kernel sums while it stages its rows (no k_splitk_reduce launch, no h round trip through it).
+    h is written only when backward or the tape needs it.  Tape: h, then q, like the two ops it replaces.  Backward:
+    the two ops' backward bodies, in their order."""
+
+    @staticmethod
+    def forward(ctx, y, cache, need_h, wa, wv, *ws):
+        B, C, Hh, W = y.shape
+        N, K = sum(w.shape[0] for w in ws), C * Hh * W
+        A, H = wa.shape
+        b = cache.get("fwd") if cache is not None else None
+        if b is None:
+            b = _pack_pieces(ws, False, True)
+            if cache is not None:
+                cache["fwd"] = b
+        res = {}
+
+        def heads():
+            part, splits, ldc = gemm_partials(pack_act_nhwc(y, False), b, B, N, K)
+            h = torch.empty(B, N, dtype=torch.float32, device=y.device) if need_h else None
+            q = torch.empty(B, A, dtype=torch.float32, device=y.device)
+            _lib.check(_lib.load().b2rl_dueling_forward(part.data_ptr(), splits, B * ldc, B, H, wa.data_ptr(), A,
+                                                        wv.data_ptr(), q.data_ptr(),
+                                                        h.data_ptr() if h is not None else None, _stream()))
+            res["q"] = q
+            return h
+        h = taped(heads)
+        q = taped(lambda: res["q"])
+        ctx.save_for_backward(y, h, wa, wv, *ws)
+        ctx.cache = cache
+        return q
+
+    @staticmethod
+    def backward(ctx, gq):
+        y, h, wa, wv, *ws = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        need_gy, need_gws = need[0], any(need[5:])
+        gh, gwa, gwv = _dueling_backward(h, wa, wv, gq, need_gy or need_gws, need[3] or need[4])
+        gy, gws = (_relu_flat_backward(y, ws, ctx.cache, gh, need_gy, need_gws) if gh is not None
+                   else (None, [None] * len(ws)))
+        return (gy, None, None, gwa, gwv, *gws)
+
+
+def relu_flat_heads_dueling(y: torch.Tensor, ws, wa: torch.Tensor, wv: torch.Tensor, cache: dict | None = None):
+    """dueling_tail(relu_flat_linear3x(y, ws, cache), wa, wv) as one op (see _ReluFlatHeadsDueling)."""
+    need_h = torch.is_grad_enabled() or _TAPE is not None
+    return _ReluFlatHeadsDueling.apply(y, cache, need_h, wa, wv, *ws)
 
 
 def dueling_tail_supported(h: torch.Tensor, wa: torch.Tensor, wv: torch.Tensor) -> bool:

@@ -40,6 +40,19 @@ class FusedRMSprop:
         self._ga = arr(*[t.data_ptr() for t in self.grad_avg]) if self.centered else None
         self._numel = (C.c_int64 * n)(*[p.numel() for p in self.params])
         self._arr = arr
+        self._images = [(0,) * 6 for _ in self.params]     # see write_images
+        self._keep_images = []
+
+    def write_images(self, param, fwd: torch.Tensor, wt: torch.Tensor | None, total_n: int, n_off: int) -> None:
+        """From now on every update of `param` (rows x cols, row-major) also writes it into the 3xTF32 B-role operand
+        images of the weight stack it belongs to (total_n rows, `param` at row n_off): `fwd` of the stack, `wt` (may
+        be None) of its transpose — the images linear._pack_pieces(stack, False / True, True) builds.  The images
+        must be current when this is called; the update keeps them so."""
+        i = next(i for i, p in enumerate(self.params) if p is param)
+        rows, cols = param.shape
+        assert param.is_contiguous() and param.grad.is_contiguous()
+        self._images[i] = (fwd.data_ptr(), wt.data_ptr() if wt is not None else 0, rows, cols, total_n, n_off)
+        self._keep_images.extend([fwd, wt])
 
     def _launch(self, lo: int, hi: int, norm_out) -> None:
         """Update + zero_grad of tensors [lo, hi); their squared gradient norms land in scratch slots [lo, hi)."""
@@ -50,7 +63,8 @@ class FusedRMSprop:
         check(_lib.load().b2rl_rmsprop_step(
             sub(self._p), (C.c_void_p * n)(*[p.grad.data_ptr() for p in self.params[lo:hi]]), sub(self._sq),
             sub(self._ga) if self.centered else None, (C.c_int64 * n)(*self._numel[lo:hi]), n, self.lr, self.alpha,
-            self.eps, int(self.centered), self._scratch.data_ptr() + 8 * lo, norm_out,
+            self.eps, int(self.centered), (C.c_int64 * (6 * n))(*[v for im in self._images[lo:hi] for v in im]),
+            self._scratch.data_ptr() + 8 * lo, norm_out,
             torch.cuda.current_stream(self.device).cuda_stream))
 
     def set_early(self, params) -> bool:

@@ -268,11 +268,16 @@ int b2rl_conv1_wgrad(const uint8_t* frames_dev, int64_t capacity, const int64_t*
  * the reference's diagnostic "norm" sqrt(sum_i ||g_i||_2) written to grad_norm_out_dev (may be
  * NULL).  The four pointer arrays and numel are HOST arrays of n_tensors (<= 24) entries holding
  * device pointers of dense tensors with identical element order; sumsq_scratch_dev: n_tensors
- * doubles, zeroed once by the caller (the kernel re-zeroes them). */
+ * doubles, zeroed once by the caller (the kernel re-zeroes them).  images (may be NULL): a HOST array of
+ * 6 * n_tensors int64 {fwd image, W^T image, rows, cols, total_n, n_off}; a tensor whose image pointers are not both
+ * 0 is a row-major rows x cols weight (multiples of 32) of a stack of total_n rows (the sibling heads of
+ * cfg/ape_x.json:52-71) at row n_off, and the update also writes it into the stack's 3xTF32 B-role images
+ * (b2rl_gemm_split_pack_into with total_rows = total_n, total_k = cols; and its transpose, total_rows = cols,
+ * total_k = total_n), bit-equal to packing the updated weights. */
 int b2rl_rmsprop_step(float* const* params, float* const* grads, float* const* square_avg,
                       float* const* grad_avg, const int64_t* numel, int32_t n_tensors, double lr, double alpha,
-                      double eps, int32_t centered, double* sumsq_scratch_dev, float* grad_norm_out_dev,
-                      void* stream);
+                      double eps, int32_t centered, const int64_t* images, double* sumsq_scratch_dev,
+                      float* grad_norm_out_dev, void* stream);
 /* The same update issued in two parts: Learner.step (APE_X/Learner.py:123-138) has no gradient clipping, so a
  * parameter can be updated as soon as its own gradient is final — the dense heads' (97 % of the elements) while the
  * convolution stack's backward still runs.  Each part calls b2rl_rmsprop_step on its tensors with
@@ -304,20 +309,30 @@ int b2rl_gemm_split_pack_into(const float* src_dev, int64_t src_rows, int64_t sr
  * out[b][hw][c] = gx[b][c*HW + hw] * (y[b][hw][c] > 0). */
 int b2rl_gemm_pack_act_nhwc(const float* y_dev, int64_t B, int64_t HW, int64_t C, int32_t relu, int32_t transpose,
                             float* out_dev, void* stream);
-int b2rl_unflatten_relu_mask(const float* gx_dev, int64_t gx_ld, const float* y_dev, int64_t B, int64_t HW, int64_t C,
-                             float* out_dev, void* stream);
+int b2rl_unflatten_relu_mask(const float* gx_dev, int64_t gx_ld, int32_t splits, int64_t split_stride,
+                             const float* y_dev, int64_t B, int64_t HW, int64_t C, float* out_dev, void* stream);
 int64_t b2rl_gemm_workspace_floats(int64_t M, int64_t N, int64_t K, int64_t ldc);
 int b2rl_gemm_tf32x3(const float* a_packed_dev, const float* b_packed_dev, float* c_dev, int64_t M,
                      int64_t N, int64_t K, int64_t ldc, float* workspace_dev, void* stream);
+/* The heads' GEMM (nn.Linear, baseline/baseNetwork.py:77-79) without its split-K reduction: the `splits` partials
+ * (splits = b2rl_gemm_workspace_floats / (M * ldc), or 1 when that is 0) are stored as [split][M][ldc] at
+ * partials_dev, which holds max(b2rl_gemm_workspace_floats, M * ldc) floats.  Their consumer sums them in split
+ * order, which gives the bits b2rl_gemm_tf32x3 returns: b2rl_dueling_forward and b2rl_unflatten_relu_mask take
+ * (splits, split_stride = M * ldc) for that. */
+int b2rl_gemm_tf32x3_partials(const float* a_packed_dev, const float* b_packed_dev, float* partials_dev, int64_t M,
+                              int64_t N, int64_t K, int64_t ldc, void* stream);
 
 /* Tail of the dueling Q-network after the first dense layer of the two heads (cfg/ape_x.json:52-88: MLP
  * heads 3136-512-A and 3136-512-1, then the Add / Mean / Substract nodes executed by
  * baseline/baseAgent.py:287-309):  r = relu(h);  Q_j = r[:H].Wa[j] + r[H:].Wv - mean_i(r[:H].Wa[i]).
  * h_dev: [M][2H] pre-activations (advantage | value), wa_dev: [A][H], wv_dev: [H], q_dev: [M][A].
  * backward: gh_dev [M][2H] (may be NULL), gwa_dev [A][H] and gwv_dev [H] (both or neither), row_ws_dev:
- * M*(A+1) floats of scratch; sums over the batch run in a fixed order.  H % 32 == 0, H <= 1024, A <= 32. */
-int b2rl_dueling_forward(const float* h_dev, int64_t M, int64_t H, const float* wa_dev, int64_t A,
-                         const float* wv_dev, float* q_dev, void* stream);
+ * M*(A+1) floats of scratch; sums over the batch run in a fixed order.  H % 32 == 0, H <= 1024, A <= 32.
+ * forward: h_dev holds `splits` partials of h, split_stride floats apart (b2rl_gemm_tf32x3_partials; 1 and 0 for a
+ * plain h), summed in split order; h_out_dev (may be NULL) receives the summed h.  h_dev, h_out_dev 16-byte aligned. */
+int b2rl_dueling_forward(const float* h_dev, int32_t splits, int64_t split_stride, int64_t M, int64_t H,
+                         const float* wa_dev, int64_t A, const float* wv_dev, float* q_dev, float* h_out_dev,
+                         void* stream);
 int b2rl_dueling_backward(const float* h_dev, const float* gq_dev, int64_t M, int64_t H, const float* wa_dev,
                           int64_t A, const float* wv_dev, float* gh_dev, float* gwa_dev, float* gwv_dev,
                           float* row_ws_dev, void* stream);
