@@ -1,6 +1,7 @@
-// TMA row copy shared by k_gather_bulk (gather.cu) and k_serve_fill (serve.cu): whole replay rows of the bulk
-// fields go HBM -> SMEM -> HBM through the TMA engine's 1-D bulk copies, driven by one thread over a ring of
-// shared-memory stages.  The SMs only issue descriptors; the payload never touches the register file.
+// Row copies shared by k_gather_bulk (gather.cu) and k_serve_fill (serve.cu).  The TMA row copy: whole replay rows of
+// the bulk fields go HBM -> SMEM -> HBM through the TMA engine's 1-D bulk copies, driven by one thread over a ring of
+// shared-memory stages.  The SMs only issue descriptors; the payload never touches the register file.  Rows too
+// small for it are copied in words by the other threads of the CTA (copy_small_rows, at the end).
 //
 // Work item = (draw k, field, chunk); a chunk is at most CHUNK bytes of one row, and items are numbered
 // draw-major, then field, then chunk.  The driving thread keeps a ring of BULK_RING_BYTES / CHUNK stages:
@@ -132,6 +133,36 @@ __device__ __forceinline__ void copy_rows(const BulkRows& T, const RowOf& row_of
     }
   }
   sm90::bulk_wait_all();
+}
+
+// A field whose rows are neither bulk rows nor copied by the draw itself: copied by the CTA's threads in words.
+struct SmallField {
+  const uint8_t* src;   // field base
+  uint8_t* dst;         // output base
+  int64_t row_bytes;
+};
+
+template <typename U, class RowOf>
+__device__ __forceinline__ void copy_small_units(const U* __restrict__ src, U* __restrict__ dst, int64_t units_per_row,
+                                                 const RowOf& row_of, int64_t k0, int64_t k1, int64_t u,
+                                                 int64_t step) {
+  for (u += k0 * units_per_row; u < k1 * units_per_row; u += step) {
+    const int64_t k = u / units_per_row, w = u - k * units_per_row;
+    dst[u] = src[row_of(k) * units_per_row + w];
+  }
+}
+
+// Output rows [k0, k1) of a small field <- replay rows row_of(k), in 4-byte words when the row is a whole number of
+// words, else in bytes.  The caller's threads take units u, u + step, ... of the range (shared by k_gather_bulk's
+// warp 1 and k_serve_fill's warps 1..3).
+template <class RowOf>
+__device__ __forceinline__ void copy_small_rows(const SmallField& f, const RowOf& row_of, int64_t k0, int64_t k1,
+                                                int64_t u, int64_t step) {
+  if ((f.row_bytes & 3) == 0)
+    copy_small_units(reinterpret_cast<const uint32_t*>(f.src), reinterpret_cast<uint32_t*>(f.dst), f.row_bytes >> 2,
+                     row_of, k0, k1, u, step);
+  else
+    copy_small_units(f.src, f.dst, f.row_bytes, row_of, k0, k1, u, step);
 }
 
 }  // namespace b2rl

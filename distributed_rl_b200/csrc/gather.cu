@@ -18,11 +18,6 @@ namespace b2rl {
 // ----------------------------------------------------------------------------
 constexpr int GATHER_THREADS = 64;
 
-struct SmallField {
-  const uint8_t* src;   // field base
-  uint8_t* dst;         // output base
-  int64_t row_bytes;
-};
 struct GatherParams {
   BulkRows bulk;                       // bulk (TMA) fields
   SmallField s[B2RL_MAX_FIELDS];       // small fields, copied by warp 1
@@ -31,28 +26,6 @@ struct GatherParams {
   int64_t capacity;
   int64_t total_items;  // bulk.items_per_row * n
 };
-
-template <typename U>
-__device__ __forceinline__ void gather_units(const U* __restrict__ src, U* __restrict__ dst, int64_t units_per_row,
-                                             const int64_t* __restrict__ idx, int64_t capacity, int64_t k0,
-                                             int64_t k1, int64_t u, int64_t step) {
-  for (u += k0 * units_per_row; u < k1 * units_per_row; u += step) {
-    const int64_t k = u / units_per_row, w = u - k * units_per_row;
-    dst[u] = src[clamp_row(idx[k], capacity) * units_per_row + w];
-  }
-}
-
-// Rows [k0, k1) of a small field's output <- their clamped replay rows, in 4-byte words when the row is a whole
-// number of words, else in bytes.  The caller's threads take units u, u + step, ... of the range.
-__device__ __forceinline__ void gather_small_rows(const uint8_t* src, uint8_t* dst, int64_t row_bytes,
-                                                  const int64_t* __restrict__ idx, int64_t capacity, int64_t k0,
-                                                  int64_t k1, int64_t u, int64_t step) {
-  if ((row_bytes & 3) == 0)
-    gather_units(reinterpret_cast<const uint32_t*>(src), reinterpret_cast<uint32_t*>(dst), row_bytes >> 2, idx,
-                 capacity, k0, k1, u, step);
-  else
-    gather_units(src, dst, row_bytes, idx, capacity, k0, k1, u, step);
-}
 
 template <int CHUNK, int LAG>
 __global__ void __launch_bounds__(GATHER_THREADS, 1)
@@ -63,7 +36,8 @@ k_gather_bulk(const __grid_constant__ GatherParams P, const int64_t* __restrict_
     const int64_t k0 = (int64_t)blockIdx.x * per;
     const int64_t k1 = (k0 + per < P.n) ? k0 + per : P.n;
     for (int f = 0; f < P.n_small; ++f)
-      gather_small_rows(P.s[f].src, P.s[f].dst, P.s[f].row_bytes, idx, P.capacity, k0, k1, threadIdx.x - 32, 32);
+      copy_small_rows(P.s[f], [&](int64_t k) { return clamp_row(idx[k], P.capacity); }, k0, k1, threadIdx.x - 32,
+                      32);
     return;
   }
   if (threadIdx.x != 0) return;  // a single thread drives the copy engine
@@ -79,8 +53,8 @@ k_gather_bulk(const __grid_constant__ GatherParams P, const int64_t* __restrict_
 __global__ void __launch_bounds__(256)
 k_gather_small(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int64_t row_bytes,
                const int64_t* __restrict__ idx, int64_t n, int64_t capacity) {
-  gather_small_rows(src, dst, row_bytes, idx, capacity, 0, n, (int64_t)blockIdx.x * blockDim.x + threadIdx.x,
-                    (int64_t)gridDim.x * blockDim.x);
+  copy_small_rows(SmallField{src, dst, row_bytes}, [&](int64_t k) { return clamp_row(idx[k], capacity); }, 0, n,
+                  (int64_t)blockIdx.x * blockDim.x + threadIdx.x, (int64_t)gridDim.x * blockDim.x);
 }
 
 // LDG.128/STG.128 reference implementation of the big-row gather (kept for the

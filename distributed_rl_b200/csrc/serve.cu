@@ -1,6 +1,6 @@
 // Device serve ring of the stand-alone replay server (include/b2rl.h, "Device serve ring"): layout arithmetic,
-// allocation / CUDA IPC export and import, and k_serve_fill — draw + IS weights + scalar fetch + TMA bulk copy of
-// the frame rows of one minibatch into a ring slot in ONE launch.
+// allocation / CUDA IPC export and import, and k_serve_fill — draw + IS weights + scalar fetch + small-row copy +
+// TMA bulk copy of the frame rows of one minibatch into a ring slot in ONE launch.
 //
 // Replaces ReplayServer.buffer's sample -> gather -> .cpu() -> pickle -> RPUSH and Replay_Server.sample's
 // pickle.loads -> host-to-device copy (APE_X/ReplayServer.py:65-114, APE_X/ReplayMemory.py:251-257).
@@ -13,35 +13,72 @@ namespace b2rl {
 
 constexpr int SERVE_THREADS = 128;   // draws per CTA at most; warp 0's lane 0 then drives the copy engine
 
-// CTA c owns draws [c*per, (c+1)*per): its threads draw them (indices, weights, scalar fields), then thread 0
-// copies their bulk rows with the TMA row copy of bulk_rows.cuh (k_gather_bulk's default geometry: 14 KiB chunks,
-// 16 stages, lag 3), then the last CTA to finish writes the header.
+// Fields of a served record whose rows are neither bulk rows nor 1/2/4/8-byte scalars (R2D2's action and reward:
+// 80 x 4 B): copied by warps 1..3 of the CTA while thread 0 drives the TMA row copy.
+struct SmallRows {
+  SmallField f[B2RL_MAX_FIELDS];
+  int32_t n;
+};
+
+// BY_ITEMS (fewer draws than SMs): CTA c owns a contiguous range of the minibatch's copy items (draw-major, then
+// field, then 14 KiB chunk: the items of copy_rows), as k_gather_bulk's CTAs do, so the copy still spreads over
+// every SM.  Its threads draw every draw the range touches; a draw is a pure function of the Philox counter and the
+// tree, so each CTA that draws k gets the same slot.  The CTA that holds draw k's first item owns it and alone
+// writes idx[k], w[k] and its scalar and small rows.  Otherwise CTA c owns draws [c*per, (c+1)*per) whole: for Ape-X
+// B = 512 the two splits give the same partition, and the item split's extra index arithmetic measured 1.7 % slower.  Thread 0 copies the range's bulk items with the TMA row copy of bulk_rows.cuh
+// (k_gather_bulk's default geometry: 14 KiB chunks, 16 stages, lag 3), warps 1..3 copy the owned draws' small rows,
+// then the last CTA to finish writes the header.  A record without bulk fields counts one item per draw.
+template <bool BY_ITEMS>
 __global__ void __launch_bounds__(SERVE_THREADS, 1)
 k_serve_fill(const __grid_constant__ TreeView t, const __grid_constant__ BulkRows P, SmallFields small,
-             uint64_t* __restrict__ rng_state, int64_t n, int64_t capacity, const float* __restrict__ n_valid_dev,
-             float beta, const float* __restrict__ max_w_ext, int64_t* __restrict__ idx_out,
-             float* __restrict__ w_out, uint64_t* __restrict__ header, uint64_t seq,
+             const __grid_constant__ SmallRows rows, uint64_t* __restrict__ rng_state, int64_t n, int64_t capacity,
+             const float* __restrict__ n_valid_dev, float beta, const float* __restrict__ max_w_ext,
+             int64_t* __restrict__ idx_out, float* __restrict__ w_out, uint64_t* __restrict__ header, uint64_t seq,
              unsigned int* __restrict__ done_ticket) {
   __shared__ int64_t s_row[SERVE_THREADS];
   const int tid = threadIdx.x;
   uint64_t seed, offset;
   rng_stream_take(rng_state, n, seed, offset);      // every block, exactly as k_tree_sample
-  const int64_t per = (n + gridDim.x - 1) / gridDim.x;
-  const int64_t k0 = (int64_t)blockIdx.x * per;
-  const int64_t cnt = (k0 >= n) ? 0 : ((n - k0 < per) ? n - k0 : per);
-  if (tid < cnt) {
-    const int64_t k = k0 + tid;
+  const int64_t ipr = P.n > 0 ? P.items_per_row : 1;
+  // items [first, first + items); draws touched [k_lo, k_hi), owned [k_own, k_hi); k_hi - k_lo <= SERVE_THREADS
+  int64_t first, items, k_lo, k_own, k_hi;
+  if (BY_ITEMS) {
+    const int64_t total = n * ipr;
+    const int64_t per = (total + gridDim.x - 1) / gridDim.x;
+    first = (int64_t)blockIdx.x * per;
+    items = (first >= total) ? 0 : ((total - first < per) ? total - first : per);
+    k_lo = first / ipr;
+    k_own = (first + ipr - 1) / ipr;
+    k_hi = (items > 0) ? (first + items + ipr - 1) / ipr : k_lo;
+  } else {
+    const int64_t per = (n + gridDim.x - 1) / gridDim.x;
+    k_lo = k_own = (int64_t)blockIdx.x * per;
+    k_hi = (k_lo >= n) ? k_lo : ((n - k_lo < per) ? n : k_lo + per);
+    first = k_lo * ipr;
+    items = (k_hi - k_lo) * ipr;
+  }
+  if (tid < k_hi - k_lo) {
+    const int64_t k = k_lo + tid;
     double root, picked;
     const int64_t j = tree_draw(t, philox_u01(seed, offset + (uint64_t)k), root, picked);
-    idx_out[k] = j;
-    fetch_small(small, j, k);
-    const float s32 = (float)root;
-    w_out[k] = is_weight(t, s32, __fdiv_rn((float)picked, s32), n_valid_dev, beta, max_w_ext);
     s_row[tid] = clamp_row(j, capacity);   // the row b2rl_replay_gather would copy
+    if (k >= k_own) {
+      idx_out[k] = j;
+      fetch_small(small, j, k);
+      const float s32 = (float)root;
+      w_out[k] = is_weight(t, s32, __fdiv_rn((float)picked, s32), n_valid_dev, beta, max_w_ext);
+    }
   }
   __syncthreads();
-  if (tid == 0 && cnt > 0 && P.n > 0)
-    copy_rows<14336, 3>(P, [](int64_t i) { return s_row[i]; }, k0, 0, cnt * P.items_per_row);
+  if (items > 0) {
+    if (tid == 0 && P.n > 0) {
+      copy_rows<14336, 3>(P, [](int64_t i) { return s_row[i]; }, k_lo, first - k_lo * ipr, items);
+    } else if (tid >= 32) {
+      for (int f = 0; f < rows.n; ++f)
+        copy_small_rows(rows.f[f], [&](int64_t k) { return s_row[k - k_lo]; }, k_own, k_hi, tid - 32,
+                        SERVE_THREADS - 32);
+    }
+  }
   // header last: written by the last CTA to get here, after every CTA's copies have completed
   __syncthreads();
   if (tid == 0) {
@@ -118,11 +155,6 @@ extern "C" int b2rl_serve_layout_init(int64_t batch, int32_t slots, int32_t n_fi
 
 extern "C" int b2rl_serve_ring_create(b2rl_replay* h, int64_t batch, int32_t slots, b2rl_serve_ring** out) {
   B2RL_REQUIRE(h != nullptr && out != nullptr, "null argument");
-  for (int f = 0; f < h->n_fields; ++f) {
-    const int64_t b = h->field_bytes[f];
-    B2RL_REQUIRE(is_bulk_row(b) || b == 1 || b == 2 || b == 4 || b == 8,
-                 "serve ring fields must be bulk rows (multiple of 16 B, >= 1024 B) or 1/2/4/8-byte scalars");
-  }
   b2rl_serve_layout L;
   int rc = b2rl_serve_layout_init(batch, slots, h->n_fields, h->field_bytes, &L);
   if (rc != B2RL_OK) return rc;
@@ -247,29 +279,39 @@ extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot,
   if (rc != B2RL_OK) return rc;
   BulkRows P{};
   SmallFields small{};
+  SmallRows rows{};
   for (int f = 0; f < h->n_fields; ++f) {
     const int64_t b = h->field_bytes[f];
     B2RL_REQUIRE(b == L.field_bytes[f], "ring and replay have different fields");
     if (is_bulk_row(b)) {
       P.add(h->field[f], (uint8_t*)ptrs[3 + f], b, 14336);   // the CHUNK of k_serve_fill's copy_rows
-    } else {
+    } else if (b == 1 || b == 2 || b == 4 || b == 8) {
       small.src[small.n] = h->field[f];
       small.dst[small.n] = (uint8_t*)ptrs[3 + f];
       small.bytes[small.n] = (int)b;
       small.n++;
+    } else {
+      rows.f[rows.n++] = SmallField{h->field[f], (uint8_t*)ptrs[3 + f], b};
     }
   }
   DeviceGuard g(h->device);
   int sms = 0;
   B2RL_CUDA(sm_count(h->device, &sms));
-  B2RL_CUDA(set_max_dynamic_smem<k_serve_fill>(h->device, BULK_RING_BYTES));
-  // one CTA per SM (the shared-memory ring takes the SM), at most SERVE_THREADS draws per CTA
+  B2RL_CUDA(set_max_dynamic_smem<k_serve_fill<true>>(h->device, BULK_RING_BYTES));
+  B2RL_CUDA(set_max_dynamic_smem<k_serve_fill<false>>(h->device, BULK_RING_BYTES));
+  // one CTA per SM (the shared-memory ring takes the SM).  Split by items: at most one CTA per copy item, and
+  // enough CTAs that no item range touches more than SERVE_THREADS draws (a range of at most SERVE_THREADS - 2
+  // draws' items starts and ends inside at most SERVE_THREADS draws).  Split by draws: at most SERVE_THREADS each.
   const int64_t n = L.batch;
-  int64_t grid = sms < n ? sms : n;
-  const int64_t min_grid = (n + SERVE_THREADS - 1) / SERVE_THREADS;
+  const bool by_items = n < sms;
+  const int64_t work = by_items ? n * (P.n > 0 ? P.items_per_row : 1) : n;
+  int64_t grid = sms < work ? sms : work;
+  const int64_t min_grid = by_items ? (n + SERVE_THREADS - 3) / (SERVE_THREADS - 2)
+                                    : (n + SERVE_THREADS - 1) / SERVE_THREADS;
   if (grid < min_grid) grid = min_grid;
-  k_serve_fill<<<(unsigned)grid, SERVE_THREADS, BULK_RING_BYTES, (cudaStream_t)stream>>>(
-      h->tree, P, small, h->rng_dev, n, h->capacity, h->n_valid_dev, beta, max_w_dev, (int64_t*)ptrs[1],
+  auto kernel = by_items ? k_serve_fill<true> : k_serve_fill<false>;
+  kernel<<<(unsigned)grid, SERVE_THREADS, BULK_RING_BYTES, (cudaStream_t)stream>>>(
+      h->tree, P, small, rows, h->rng_dev, n, h->capacity, h->n_valid_dev, beta, max_w_dev, (int64_t*)ptrs[1],
       (float*)ptrs[2], (uint64_t*)ptrs[0], seq, r->done_ticket);
   count_launch();
   B2RL_CHECK_LAUNCH();

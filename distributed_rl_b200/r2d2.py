@@ -125,7 +125,11 @@ class Learner(TargetNetLearner):
     LOG_LINE = ("step:{step} // mean_value:{mean_value:.3f} // norm: {norm:.3f} // REWARD:{reward:.3f} // "
                 "NUM_MEMORY:{num_memory} // MAX_WEIGHT:{max_weight:.3f} // TIME:{time_per_step:.5f}")
 
-    def __init__(self, cfg: R2D2Config | None = None, connect=None, start_replay: bool = True, writer=None):
+    def __init__(self, cfg: R2D2Config | None = None, connect=None, start_replay: bool = True, writer=None,
+                 memory=None):
+        """`memory`: a replay served from another process (replay_server.DeviceReplayClient or Replay_Server built
+        with this R2D2Config, or anything with the `Replay` surface: sample / update / lock / memory).  run() drives
+        sample() -> train() -> update() either way; a served memory passes the eviction request on to its server."""
         self.cfg = cfg or R2D2Config.from_configuration()
         self.device = torch.device(self.cfg.LEARNER_DEVICE)
         self.model = GraphAgent(self.cfg.MODEL).to(self.device)
@@ -134,13 +138,20 @@ class Learner(TargetNetLearner):
             m.dense_3xtf32 = m.fused_dueling_tail = bool(self.cfg.FUSED_HEADS) and self.device.type == "cuda"
         self.optim = make_optimizer(self.cfg.OPTIM_INFO, self.model.getParameters())
         self.connect = connect
-        self.memory = Replay(self.cfg, connect)
+        self._served = memory is not None
+        if self._served:
+            self.memory = memory
+            if start_replay and not memory.is_alive():
+                memory.start()
+        else:
+            self.memory = Replay(self.cfg, connect)
+            if start_replay and connect is not None:
+                self.memory.start()                              # R2D2/Learner.py:46-48
         self.writer = writer
         if connect is not None:
-            if start_replay:
-                self.memory.start()                              # R2D2/Learner.py:46-48
             from .wire import wipe_stale_keys
-            wipe_stale_keys(connect)                             # :54,63-64
+            # :54,63-64 — except the keys of a replay server this learner is already attached to
+            wipe_stale_keys(connect, keep=getattr(self.memory, "KEEP_KEYS", ()) if self._served else ())
 
     def train(self, transition, t=0):
         c = self.cfg
@@ -274,9 +285,9 @@ class Learner(TargetNetLearner):
             info, prio, idx = self.train(batch)
             step += 1
             if step % log_every == 0:
-                self.memory.lock = True                                  # :266-268
-                if self.connect is None or not self.memory.is_alive():
-                    self.memory._evict_on_request()
+                self.memory.lock = True                                  # :266-268, that step's write-back skipped
+                if not self._served and (self.connect is None or not self.memory.is_alive()):
+                    self.memory._evict_on_request()                      # a served memory's server evicts
             if not self.memory.lock:
                 self.memory.update(idx, prio)                            # :271-274
             tot = torch.stack([info["mean_value"].reshape(()), info["p_norm"].reshape(())])

@@ -1,12 +1,13 @@
-"""Stand-alone replay mode (SURVEY.md §8 f4): `ReplayServer` (APE_X/ReplayServer.py:20-160) owns the prioritized
-replay in ITS OWN process / GPU and serves pre-assembled minibatches over the reference's Redis protocol;
-`Replay_Server` (APE_X/ReplayMemory.py:170-257) is the learner-side consumer with the `Replay` surface
-(`sample()`, `update()`, `start()`).
+"""Stand-alone replay mode (SURVEY.md §8 f4): `ReplayServer` (APE_X/ReplayServer.py:20-160,
+R2D2/ReplayServer.py:20-175) owns the prioritized replay in ITS OWN process / GPU and serves pre-assembled minibatches
+over the reference's Redis protocol; `Replay_Server` (APE_X/ReplayMemory.py:170-257, R2D2/ReplayMemory.py:187-274) is
+the learner-side consumer with the `Replay` surface (`sample()`, `update()`, `start()`).  Every server and client
+serves the record kind of its config: Ape-X transitions (`ApexConfig`) or R2D2 sequences (`R2D2Config`), see `KINDS`.
 
 Keys (the reference's): list `experience` (actors -> server), list `BATCH` on the push connection (server ->
-learner: pickled `[s, a, r, s', done, w, idx]`), list `update` (learner -> server: pickled `(idx list, priorities)`),
-flags `FLAG_BATCH` (enough data to serve), `FLAG_ENOUGH` (learner has > 32 batches queued), `FLAG_REMOVE` (learner asks
-for `remove_to_fit`).
+learner: pickled `[s, a, r, s', done, w, idx]` or `[(h0, h1), s, a, r, notdone, w, idx]`), list `update` (learner ->
+server: pickled `(idx list, priorities)`), flags `FLAG_BATCH` (enough data to serve), `FLAG_ENOUGH` (learner has more
+than 32 (Ape-X) / 18 (R2D2) batches queued), `FLAG_REMOVE` (learner asks for `remove_to_fit`).
 
 What is GPU-native here is the server's store: sampling, IS weights, gather and priority write-back are the HBM
 kernels of libb2rl (one sample launch + one TMA gather per served group of minibatches, applied updates in stream
@@ -34,8 +35,8 @@ completed, and a peer's stream waits on it only after reading the descriptor pos
 leaves slots unserved, it cannot hang a GPU.
 
 Shutdown: the learner closes its client first (unmap, then SERVE_DETACHED); the server frees the ring only after
-that key appears.  A learner that attached with `apex.Learner(connect=..., memory=client)` keeps SERVER_KEYS out of
-its start-up wipe of stale keys."""
+that key appears.  A learner that attached with `apex.Learner(connect=..., memory=client)` or
+`r2d2.Learner(connect=..., memory=client)` keeps SERVER_KEYS out of its start-up wipe of stale keys."""
 from __future__ import annotations
 
 import ctypes as C
@@ -43,6 +44,8 @@ import pickle
 import threading
 import time
 from collections import deque
+from dataclasses import dataclass
+from typing import Callable
 
 import numpy as np
 import torch
@@ -50,20 +53,63 @@ import torch
 from . import _lib, wire
 from . import replay as R
 from ._lib import check
+from . import apex, r2d2
 from .apex import ApexConfig
 from .learner_common import Stoppable
+from .r2d2 import R2D2Config
+
+
+@dataclass(frozen=True)
+class RecordKind:
+    """What the servers and clients need to know about the records they serve."""
+    name: str
+    replay: type                    # the ingest Replay: decoder of the actors' `experience` records + the store
+    fields: Callable                # cfg -> the store's fields
+    batch: Callable                 # (gathered fields, IS weights, indices) -> the learner's minibatch list
+    host: Callable                  # (field name, CPU tensor) -> what a pickled `BATCH` blob carries
+    m: int                          # minibatches per ReplayServer.buffer()
+    enough: int                     # Replay_Server raises FLAG_ENOUGH above this many queued minibatches
+
+
+def _apex_batch(b, w, idx):
+    """APE_X/ReplayServer.py:95-114: [s, a, r, s', done, w, idx]."""
+    return [b["state"], b["action"], b["reward"], b["next_state"], b["done"], w, idx]
+
+
+def _r2d2_batch(b, w, idx):
+    """R2D2/ReplayMemory.py:74-120 (r2d2.Replay.buffer): [(h0, h1), s, a, r, notdone, w, idx], h0 / h1 (1, B, 512)."""
+    return [(b["h0"].unsqueeze(0), b["h1"].unsqueeze(0)), b["state"], b["action"], b["reward"], b["notdone"], w, idx]
+
+
+KINDS = {
+    "apex": RecordKind("apex", apex.Replay, lambda cfg: R.APEX_FIELDS, _apex_batch,
+                       lambda name, t: t.numpy().astype(bool) if name == "done" else t.numpy(),
+                       m=32, enough=32),                      # APE_X/ReplayServer.py:66, APE_X/ReplayMemory.py:232
+    "r2d2": RecordKind("r2d2", r2d2.Replay, lambda cfg: R.r2d2_fields(cfg.FIXED_TRAJECTORY), _r2d2_batch,
+                       lambda name, t: t if name in ("h0", "h1") else t.numpy(),   # h0 / h1 stay torch (:100-101)
+                       m=8, enough=18),                       # R2D2/ReplayServer.py:66, R2D2/ReplayMemory.py:249
+}
+
+
+def record_kind(cfg) -> RecordKind:
+    """The kind a config describes: R2D2Config -> sequences, anything else (ApexConfig) -> transitions."""
+    return KINDS["r2d2" if isinstance(cfg, R2D2Config) else "apex"]
 
 
 class _StandaloneServer(Stoppable):
-    """What the two stand-alone servers share (APE_X/ReplayServer.py:20-160): the ingest of `experience` into the
-    store, FLAG_BATCH once the store holds more than BUFFER_SIZE records, and eviction on FLAG_REMOVE."""
+    """What the two stand-alone servers share (APE_X/ReplayServer.py:20-160, R2D2/ReplayServer.py:20-175): the
+    ingest of `experience` into the store, FLAG_BATCH once the store holds more than BUFFER_SIZE records, and
+    eviction on FLAG_REMOVE.  `cfg`: ApexConfig (the default, from `configuration`) or R2D2Config."""
 
-    def __init__(self, cfg: ApexConfig | None, connect):
+    def __init__(self, cfg: ApexConfig | R2D2Config | None, connect):
         super().__init__()
         self.cfg = cfg or ApexConfig.from_configuration()
+        if getattr(self.cfg, "PAYLOAD_POOL", 0):
+            raise ValueError("a replay server needs a store that ingests records; PAYLOAD_POOL is a benchmark store "
+                             "without ingest (set PAYLOAD_POOL = 0)")
+        self.kind = record_kind(self.cfg)
         self.device = torch.device(self.cfg.LEARNER_DEVICE)
-        from .apex import Replay
-        self._ingest = Replay(self.cfg, connect=None)      # never started: its record decoder + pinned staging + store
+        self._ingest = self.kind.replay(self.cfg, connect=None)   # never started: record decoder + staging + store
         self.store = self._ingest.store
         self.connect = connect
         self.FLAG_BATCH = False
@@ -92,10 +138,11 @@ class _StandaloneServer(Stoppable):
 
 
 class ReplayServer(_StandaloneServer):
-    def __init__(self, cfg: ApexConfig | None = None, connect=None, connect_push=None, m: int = 32):
+    def __init__(self, cfg: ApexConfig | R2D2Config | None = None, connect=None, connect_push=None,
+                 m: int | None = None):
         super().__init__(cfg, connect)
         self.connect_push = connect_push if connect_push is not None else connect
-        self.m = m                               # minibatches assembled per buffer() (the reference: 32, :66)
+        self.m = self.kind.m if m is None else m   # minibatches per buffer() (the reference: Ape-X 32, R2D2 8; :66)
         self.FLAG_REMOVE = False
         if self.connect is not None:
             self.connect.set("FLAG_BATCH", pickle.dumps(False))           # :39
@@ -115,17 +162,19 @@ class ReplayServer(_StandaloneServer):
         return len(idx_list)
 
     def buffer(self) -> int:
-        """:65-114 — sample BATCHSIZE * m, IS weights, assemble m minibatches, RPUSH them to `BATCH`."""
+        """APE_X/ReplayServer.py:65-114, R2D2/ReplayServer.py:65-136 — sample BATCHSIZE * m, IS weights, assemble m
+        minibatches, RPUSH them to `BATCH`, each once.  R2D2 minibatch k is sequences kB .. kB + B - 1, batch-major
+        (state (B, T, 4, 84, 84)), the layout r2d2.Replay.buffer hands its learner (DESIGN.md §2: the reference's
+        time-major vsplit and its second RPUSH of every blob are not reproduced)."""
         B, m = self.cfg.BATCHSIZE, self.m
         idx, _, w = self.store.sample(B * m, beta=self.cfg.BETA)
-        b = self.store.gather(idx)
-        s, ns = b["state"].cpu().numpy(), b["next_state"].cpu().numpy()
-        a, r, d = b["action"].cpu().numpy(), b["reward"].cpu().numpy(), b["done"].cpu().numpy().astype(bool)
+        b = {name: t.cpu() for name, t in self.store.gather(idx).items()}
         w, idx = w.cpu(), idx.cpu()
         blobs = []
         for k in range(m):
             sl = slice(k * B, (k + 1) * B)
-            blobs.append(pickle.dumps([s[sl], a[sl], r[sl], ns[sl], d[sl], w[sl], idx[sl]]))
+            host = {name: self.kind.host(name, t[sl]) for name, t in b.items()}
+            blobs.append(pickle.dumps(self.kind.batch(host, w[sl], idx[sl])))
         return self.connect_push.rpush("BATCH", *blobs)
 
     def serve_once(self) -> dict:
@@ -146,11 +195,14 @@ class ReplayServer(_StandaloneServer):
 
 
 class Replay_Server(Stoppable, threading.Thread):
-    """Learner-side consumer of a ReplayServer: same surface as `Replay` (sample / update / start / lock)."""
+    """Learner-side consumer of a ReplayServer: same surface as `Replay` (sample / update / start / lock).  Every
+    `BATCH` blob is queued once and unpickled once, by sample() (R2D2/ReplayMemory.py:244-246 queues each blob a
+    second time, already unpickled, which its sample() then fails to unpickle; DESIGN.md §2)."""
 
-    def __init__(self, cfg: ApexConfig | None = None, connect=None, connect_push=None):
+    def __init__(self, cfg: ApexConfig | R2D2Config | None = None, connect=None, connect_push=None):
         super().__init__(daemon=True)
         self.cfg = cfg or ApexConfig.from_configuration()
+        self.kind = record_kind(self.cfg)
         self.connect, self.connect_push = connect, connect_push if connect_push is not None else connect
         self._lock = threading.Lock()
         self.deque, self.idx, self.vals = [], [], []
@@ -167,7 +219,7 @@ class Replay_Server(Stoppable, threading.Thread):
         if data:
             with self._lock:
                 self.deque += data
-        self.connect.set("FLAG_ENOUGH", pickle.dumps(len(self.deque) > 32))       # :232-239
+        self.connect.set("FLAG_ENOUGH", pickle.dumps(len(self.deque) > self.kind.enough))   # :232-239
         if self.lock:                                                              # eviction request -> the server's flag
             self.connect.set("FLAG_REMOVE", pickle.dumps(True))
             self.lock = False
@@ -380,7 +432,7 @@ class DeviceReplayServer(_StandaloneServer):
 
     STATS_EVERY = 0.1             # seconds between SERVE_STATS refreshes (each costs a device sync)
 
-    def __init__(self, cfg: ApexConfig | None = None, connect=None, slots: int = 4):
+    def __init__(self, cfg: ApexConfig | R2D2Config | None = None, connect=None, slots: int = 4):
         super().__init__(cfg, connect)
         self.device = self.store.device
         self.ring = ServeRing.create(self.store, self.cfg.BATCHSIZE, slots)
@@ -484,13 +536,15 @@ class ServedMemory:
 class DeviceReplayClient(Stoppable, threading.Thread):
     """Learner-side consumer of a DeviceReplayServer with the `Replay` surface (start / stop / sample / update / lock /
     memory; APE_X/ReplayMemory.py:170-257).  sample() returns `[s, a, r, s', done, w, idx]` as CUDA tensors on the
-    learner's device, copied out of the ring (a peer copy when the server is on another GPU)."""
+    learner's device, copied out of the ring (a peer copy when the server is on another GPU); with an R2D2Config,
+    `[(h0, h1), s, a, r, notdone, w, idx]` as r2d2.Replay.sample returns it."""
 
-    KEEP_KEYS = SERVER_KEYS       # what apex.Learner(connect=..., memory=this) leaves in place at start-up
+    KEEP_KEYS = SERVER_KEYS       # what apex/r2d2.Learner(connect=..., memory=this) leaves in place at start-up
 
-    def __init__(self, cfg: ApexConfig | None = None, connect=None, timeout: float = 60.0):
+    def __init__(self, cfg: ApexConfig | R2D2Config | None = None, connect=None, timeout: float = 60.0):
         super().__init__(daemon=True)
         self.cfg = cfg or ApexConfig.from_configuration()
+        self.kind = record_kind(self.cfg)
         self.device = torch.device(self.cfg.LEARNER_DEVICE)
         if self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
@@ -504,9 +558,9 @@ class DeviceReplayClient(Stoppable, threading.Thread):
         info = pickle.loads(blob)
         self.ring = ServeRing.open(info["handle"], info["layout"], self.device)
         L = self.ring.layout
-        self.fields = R.APEX_FIELDS
+        self.fields = self.kind.fields(self.cfg)
         if [L.field_bytes[i] for i in range(L.n_fields)] != [f.nbytes for f in self.fields]:
-            raise RuntimeError("the server's ring does not carry the Ape-X record fields")
+            raise RuntimeError(f"the server's ring does not carry the {self.kind.name} record fields of this config")
         srv = torch.device("cuda", info["device"])
         self.filled = [torch.cuda.Event.from_ipc_handle(srv, h) for h in info["filled"]]
         self.applied = [torch.cuda.Event.from_ipc_handle(srv, h) for h in info["applied"]]
@@ -542,8 +596,8 @@ class DeviceReplayClient(Stoppable, threading.Thread):
                 view(L.w_off, 4 * B, torch.float32, (B,)), out)
 
     def sample(self):
-        """Replay_Server.sample (APE_X/ReplayMemory.py:251-257): the oldest filled slot, copied into fresh
-        learner-local memory on the current stream; False when nothing is filled."""
+        """Replay_Server.sample (APE_X/ReplayMemory.py:251-257, R2D2/ReplayMemory.py:266-274): the oldest filled
+        slot, copied into fresh learner-local memory on the current stream; False when nothing is filled."""
         cur = torch.cuda.current_stream(self.device)
         got = []
 
@@ -560,7 +614,7 @@ class DeviceReplayClient(Stoppable, threading.Thread):
             return False
         header, idx, w, b = self._views(got[0])
         self.last_served, self.last_header = desc, header
-        return [b["state"], b["action"], b["reward"], b["next_state"], b["done"], w, idx]
+        return self.kind.batch(b, w, idx)
 
     def update(self, idx, vals) -> None:
         """Replay_Server.update (APE_X/ReplayMemory.py:188-190): the write-back goes to free update slots of the

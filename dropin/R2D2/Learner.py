@@ -1,6 +1,6 @@
 """Drop-in for R2D2/Learner.py."""
-from distributed_rl_b200.r2d2 import R2D2Config, Learner as _Learner, Replay  # noqa: F401
-from distributed_rl_b200.r2d2 import Replay as Replay_Server  # noqa: F401
+from distributed_rl_b200.r2d2 import R2D2Config, Learner as _Learner  # noqa: F401
+from R2D2.ReplayMemory import Replay, Replay_Server  # noqa: F401  (R2D2/Learner.py:5)
 
 
 class Learner(_Learner):

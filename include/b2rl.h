@@ -373,8 +373,8 @@ typedef struct {
  * the ReplayServer's `BATCH` blobs carry, APE_X/ReplayServer.py:65-114. */
 int b2rl_serve_layout_init(int64_t batch, int32_t slots, int32_t n_fields, const int64_t* field_bytes,
                            b2rl_serve_layout* out);
-/* ReplayServer.__init__ (APE_X/ReplayServer.py:20-39): allocate the ring for replay `h` on h's device (headers
- * zeroed).  Every field must be a bulk row (a multiple of 16 bytes, >= 1024) or a 1/2/4/8-byte scalar. */
+/* ReplayServer.__init__ (APE_X/ReplayServer.py:20-39, R2D2/ReplayServer.py:20-39): allocate the ring for replay
+ * `h` on h's device (headers zeroed).  Any field with row_bytes >= 1 can be served. */
 int b2rl_serve_ring_create(b2rl_replay* h, int64_t batch, int32_t slots, b2rl_serve_ring** out);
 /* The ring's layout (what a learner needs besides the IPC handle to open it; APE_X/ReplayMemory.py:170-186). */
 int b2rl_serve_ring_layout(const b2rl_serve_ring* r, b2rl_serve_layout* out);
@@ -392,12 +392,14 @@ int b2rl_serve_ring_destroy(b2rl_serve_ring* r);
  * `update` entry, :41-63), valid in this process: batch_out[0..2+n_fields] = {header, idx, w, field 0, ...},
  * update_out[0..2] = {header, idx, prio}.  Either may be NULL. */
 int b2rl_serve_slot_ptrs(const b2rl_serve_ring* r, int32_t slot, void** batch_out, void** update_out);
-/* ReplayServer.buffer (APE_X/ReplayServer.py:65-114) for one minibatch, in ONE launch: B draws from h's
- * device-resident Philox stream with the descent and IS-weight arithmetic of b2rl_tree_sample_fetch (the
- * counter advances by B), idx / w / scalar fields written by the drawing threads, the bulk rows copied HBM ->
- * SMEM -> slot with TMA bulk copies as b2rl_replay_gather does, and the header {seq, B} written last.  The slot
- * equals b2rl_tree_sample_fetch + b2rl_replay_gather from the same RNG state, bit for bit.  max_w_dev: as for
- * b2rl_tree_sample. */
+/* ReplayServer.buffer (APE_X/ReplayServer.py:65-114, R2D2/ReplayServer.py:65-136) for one minibatch, in ONE
+ * launch: B draws from h's device-resident Philox stream with the descent and IS-weight arithmetic of
+ * b2rl_tree_sample_fetch (the counter advances by B), idx / w / 1-2-4-8-byte scalar fields written by the drawing
+ * threads, bulk rows (a multiple of 16 bytes, >= 1024) copied HBM -> SMEM -> slot with TMA bulk copies as
+ * b2rl_replay_gather does, every other row (e.g. R2D2's 80-step action / reward) copied in words or bytes by the
+ * other threads of the same CTAs, and the header {seq, B} written last.  The CTAs split the minibatch's copy work
+ * evenly, so a minibatch of fewer draws than SMs still uses every SM.  The slot equals b2rl_tree_sample_fetch +
+ * b2rl_replay_gather from the same RNG state, bit for bit.  max_w_dev: as for b2rl_tree_sample. */
 int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, uint64_t seq, float beta,
                     const float* max_w_dev, void* stream);
 /* Replay_Server.sample (APE_X/ReplayMemory.py:251-257) without the unpickle: copy minibatch slot k (slot_bytes,

@@ -1,9 +1,16 @@
-"""Stand-alone replay server transports, Ape-X at batch B: served minibatches/s and learner steps/s for
+"""Stand-alone replay server transports, Ape-X transitions or R2D2 sequences at batch B: served minibatches/s and
+learner steps/s for
   redis   ReplayServer -> pickled `BATCH` list -> Replay_Server (host arrays, copied to the device by train())
   ring    DeviceReplayServer -> device serve ring (CUDA IPC) -> DeviceReplayClient
   fused   the in-process learner: Learner.fused_step() on its own replay (no server)
+  fill    b2rl_serve_fill alone, in this process: CUDA events around `steps` fills into alternating ring slots, at
+          each batch of --fill-batches; bytes/s = 2 x slot bytes / fill time (each byte read once, written once)
 
-    python tools/bench_serve.py [--slots-store 65536] [--batch 512] [--steps 200] [--warmup 20] [--repeats 3]
+    python tools/bench_serve.py [--workload apex|r2d2] [--slots-store N] [--batch B] [--steps 200] [--warmup 20]
+                                [--repeats 3] [--arms redis,ring,fused,fill]
+
+Defaults per workload: Ape-X B = 512 on a 2^16-slot store (3.7 GB); R2D2 B = 64, T = 80, MEM = 20 on a 2^12-sequence
+store (9.2 GB).
 
 The server runs in a `spawn` child on --server-device, the learner here on cuda:0; the control plane is a Redis
 server (--redis HOST) or, by default, the in-memory Redis stand-in of the tests hosted by a multiprocessing manager
@@ -40,9 +47,18 @@ def _connect(args, proxy):
 
 
 def _cfg(args, device):
-    from distributed_rl_b200 import apex
+    from distributed_rl_b200 import apex, r2d2
+    if args["workload"] == "r2d2":
+        return r2d2.R2D2Config(BATCHSIZE=args["batch"], REPLAY_MEMORY_LEN=args["store"], BUFFER_SIZE=0,
+                               FIXED_TRAJECTORY=80, MEM=20, LEARNER_DEVICE=device)
     return apex.ApexConfig(BATCHSIZE=args["batch"], REPLAY_MEMORY_LEN=args["store"], BUFFER_SIZE=0,
                            LEARNER_DEVICE=device)
+
+
+def _learner(args, cfg, memory=None):
+    from distributed_rl_b200 import apex, r2d2
+    mod = r2d2 if args["workload"] == "r2d2" else apex
+    return mod.Learner(cfg, connect=None, start_replay=False, **({} if memory is None else {"memory": memory}))
 
 
 def _fill(store, n):
@@ -91,7 +107,6 @@ def _timed(fn, steps, warmup, dev):
 
 def _served_arm(kind, args):
     import torch
-    from distributed_rl_b200 import apex
     from distributed_rl_b200.replay_server import DeviceReplayClient, Replay_Server
     ctx = mp.get_context("spawn")
     mgr = RedisManager(ctx=ctx)
@@ -110,7 +125,8 @@ def _served_arm(kind, args):
         else:
             client = Replay_Server(cfg, conn, conn)
             client.start()
-        L = apex.Learner(cfg, connect=None, start_replay=False, memory=client)
+        L = _learner(args, cfg, client)
+        frames = (1,) if args["workload"] == "r2d2" else (0, 3)     # the frame arrays of the minibatch list
 
         def next_batch():
             while (b := client.sample()) is False:
@@ -120,15 +136,16 @@ def _served_arm(kind, args):
         def serve_only():
             b = next_batch()
             if kind == "redis":          # what train() would do first: the batch onto the device
-                b[0] = torch.as_tensor(b[0]).to(dev, non_blocking=True)
-                b[3] = torch.as_tensor(b[3]).to(dev, non_blocking=True)
+                for i in frames:
+                    b[i] = torch.as_tensor(b[i]).to(dev, non_blocking=True)
 
         def step():
             b = next_batch()
-            info, prio, idx, _ = L.train(b)
+            info, prio, idx = L.train(b)[:3]
             client.update(idx if kind == "ring" else list(idx.tolist()), prio)
-        served = _timed(serve_only, args["steps"], args["warmup"], dev)
-        steps = _timed(step, args["steps"], args["warmup"], dev)
+        n = args["redis_steps"] if kind == "redis" else args["steps"]
+        served = _timed(serve_only, n, args["warmup"], dev)
+        steps = _timed(step, n, args["warmup"], dev)
         return {"served_minibatches_per_s": served, "learner_steps_per_s": steps}
     finally:
         stop.set()
@@ -148,9 +165,8 @@ def _served_arm(kind, args):
 
 def _fused_arm(args):
     import torch
-    from distributed_rl_b200 import apex
     cfg = _cfg(args, "cuda:0")
-    L = apex.Learner(cfg, connect=None, start_replay=False)
+    L = _learner(args, cfg)
     _fill(L.memory.store, args["store"])
     rate = _timed(L.fused_step, args["steps"], args["warmup"], torch.device("cuda:0"))
     del L
@@ -158,16 +174,54 @@ def _fused_arm(args):
     return {"served_minibatches_per_s": None, "learner_steps_per_s": rate}
 
 
+def _fill_arm(args):
+    """b2rl_serve_fill alone: one store, a 2-slot ring per batch size, CUDA events around `steps` back-to-back
+    fills (slots alternate, as a server with a free slot would fill them)."""
+    import torch
+    from distributed_rl_b200 import replay as R
+    from distributed_rl_b200.replay_server import ServeRing, record_kind
+    cfg = _cfg(args, "cuda:0")
+    store = R.DeviceReplay(args["store"], record_kind(cfg).fields(cfg), "cuda:0")
+    _fill(store, args["store"])
+    out = {}
+    try:
+        for B in args["fill_batches"]:
+            ring = ServeRing.create(store, B, 2)
+            for i in range(args["warmup"]):
+                ring.fill(store, i % 2, i + 1, cfg.BETA)
+            st = torch.cuda.current_stream()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(st)
+            for i in range(args["steps"]):
+                ring.fill(store, i % 2, i + 1, cfg.BETA)
+            e1.record(st)
+            e1.synchronize()
+            t = e0.elapsed_time(e1) / 1e3 / args["steps"]
+            bps = 2 * ring.layout.slot_bytes / t
+            out[str(B)] = {"fill_us": t * 1e6, "slot_bytes": ring.layout.slot_bytes, "bytes_per_s": bps,
+                           "fraction_of_3.35e12": bps / 3.35e12}
+            torch.cuda.synchronize()
+            ring.close()
+    finally:
+        store.close()
+        torch.cuda.empty_cache()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--slots-store", type=int, default=65536, help="replay slots (2^16 = 3.7 GB)")
-    ap.add_argument("--batch", type=int, default=512)
+    ap.add_argument("--workload", choices=("apex", "r2d2"), default="apex")
+    ap.add_argument("--slots-store", type=int, default=None,
+                    help="replay slots (default: Ape-X 2^16 = 3.7 GB, R2D2 2^12 sequences = 9.2 GB)")
+    ap.add_argument("--batch", type=int, default=None, help="default: Ape-X 512, R2D2 64")
+    ap.add_argument("--fill-batches", default=None, help="batch sizes of the fill arm, e.g. 32,64 (default: --batch)")
+    ap.add_argument("--redis-steps", type=int, default=None, help="timed steps of the redis arm (default: --steps)")
     ap.add_argument("--ring-slots", type=int, default=4)
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--server-device", default="cuda:0")
-    ap.add_argument("--arms", default="redis,ring,fused")
+    ap.add_argument("--arms", default="redis,ring,fused", help="any of redis, ring, fused, fill")
     ap.add_argument("--redis", default=None, help="host of a Redis server for the control plane (default: an "
                     "in-memory stand-in in a manager process, which makes the Redis-pickle arm far slower than a "
                     "Redis server would)")
@@ -175,12 +229,18 @@ def main():
     import torch
     if not torch.cuda.is_available():
         sys.exit("bench_serve.py measures on a CUDA device; none is available")
-    args = {"store": a.slots_store, "batch": a.batch, "ring_slots": a.ring_slots, "steps": a.steps,
-            "warmup": a.warmup, "server_device": a.server_device, "redis": a.redis}
+    r2 = a.workload == "r2d2"
+    store = a.slots_store or (4096 if r2 else 65536)
+    batch = a.batch or (64 if r2 else 512)
+    args = {"workload": a.workload, "store": store, "batch": batch, "ring_slots": a.ring_slots, "steps": a.steps,
+            "warmup": a.warmup, "server_device": a.server_device, "redis": a.redis,
+            "redis_steps": a.redis_steps or a.steps,
+            "fill_batches": [int(x) for x in a.fill_batches.split(",")] if a.fill_batches else [batch]}
     runs = {k: [] for k in a.arms.split(",")}
+    arm = {"fused": _fused_arm, "fill": _fill_arm}
     for _ in range(a.repeats):
         for k in runs:
-            runs[k].append(_fused_arm(args) if k == "fused" else _served_arm(k, args))
+            runs[k].append(arm[k](args) if k in arm else _served_arm(k, args))
             print(json.dumps({"arm": k, **runs[k][-1]}), file=sys.stderr, flush=True)
     try:
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -188,7 +248,7 @@ def main():
     except Exception:
         q = []
     same = a.server_device == "cuda:0"
-    print(json.dumps({"workload": "apex_serve", "batch": a.batch, "store_slots": a.slots_store,
+    print(json.dumps({"workload": f"{a.workload}_serve", "batch": batch, "store_slots": store,
                       "server_device": a.server_device, "learner_device": "cuda:0",
                       "control_plane": f"redis://{a.redis}" if a.redis else "in-memory stand-in (manager process)",
                       "note": "server and learner share one GPU: served figures are a lower bound" if same else
