@@ -91,6 +91,7 @@ SIGNATURES = {
     "b2rl_serve_ring_destroy": (C.c_int, [c_vp]),
     "b2rl_serve_slot_ptrs": (C.c_int, [c_vp, c_i32, C.POINTER(c_vp), C.POINTER(c_vp)]),
     "b2rl_serve_fill": (C.c_int, [c_vp, c_vp, c_i32, c_u64, c_f32, c_vp, c_vp]),
+    "b2rl_serve_fill_uniform": (C.c_int, [c_vp, c_vp, c_i32, c_u64, c_i32, c_vp]),
     "b2rl_serve_take": (C.c_int, [c_vp, c_i32, c_vp, c_vp]),
     "b2rl_serve_put_update": (C.c_int, [c_vp, c_i32, c_u64, c_vp, c_vp, c_i64, c_vp]),
 }

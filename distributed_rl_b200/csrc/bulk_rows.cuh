@@ -28,8 +28,8 @@ struct BulkField {
   const uint8_t* src;   // replay field base
   uint8_t* dst;         // output base
   int64_t row_bytes;    // is_bulk_row
-  int32_t chunks;       // ceil(row_bytes / CHUNK)
-  int32_t pad;
+  int32_t chunks;       // ceil(row_bytes / CHUNK); time-major: steps * ceil(step_bytes / CHUNK)
+  int32_t step_bytes;   // time-major destination only: bytes of one time step of the row (a multiple of 16)
 };
 
 struct BulkRows {
@@ -43,10 +43,19 @@ struct BulkRows {
     items_per_row += f[n].chunks;
     ++n;
   }
+  // A row of `steps` time steps whose step t of draw k goes to output row t * batch + k: chunked per step, so no
+  // chunk straddles two steps and each one is a single bulk copy with a contiguous destination.
+  void add_time_major(const uint8_t* src, uint8_t* dst, int64_t row_bytes, int64_t steps, int chunk) {
+    const int64_t step = row_bytes / steps;
+    f[n] = BulkField{src, dst, row_bytes, (int32_t)(steps * ((step + chunk - 1) / chunk)), (int32_t)step};
+    items_per_row += f[n].chunks;
+    ++n;
+  }
 };
 
-// Walks a contiguous range of items without divisions; `row` is the replay row of draw k.
-template <int CHUNK>
+// Walks a contiguous range of items without divisions; `row` is the replay row of draw k.  TIME_MAJOR: the
+// destination of step t of draw k is output row t * batch + k (BulkRows::add_time_major).
+template <int CHUNK, bool TIME_MAJOR = false>
 struct ItemCursor {
   int64_t k, row;
   int32_t f, c;
@@ -60,7 +69,18 @@ struct ItemCursor {
     row = row_of(k);
   }
   __device__ __forceinline__ void get(const BulkRows& T, int64_t dst_k0, const uint8_t*& src, uint8_t*& dst,
-                                      uint32_t& bytes) const {
+                                      uint32_t& bytes, int64_t batch = 0) const {
+    if (TIME_MAJOR) {
+      const int32_t step = T.f[f].step_bytes;
+      const int32_t cps = (step + CHUNK - 1) / CHUNK;   // chunks per step
+      const int32_t t = c / cps;
+      const int64_t off = (int64_t)(c - t * cps) * CHUNK;
+      const int64_t rem = step - off;
+      bytes = (uint32_t)(rem < CHUNK ? rem : CHUNK);
+      src = T.f[f].src + row * T.f[f].row_bytes + (int64_t)t * step + off;
+      dst = T.f[f].dst + ((int64_t)t * batch + dst_k0 + k) * step + off;
+      return;
+    }
     const int64_t off = (int64_t)c * CHUNK;
     const int64_t rem = T.f[f].row_bytes - off;
     bytes = (uint32_t)(rem < CHUNK ? rem : CHUNK);
@@ -82,10 +102,10 @@ struct ItemCursor {
 
 // Run by ONE thread of the CTA, which needs BULK_RING_BYTES of dynamic shared memory: copies items
 // [first, first + items) of table T (items >= 1).  Draw k reads replay row row_of(k) and writes output row
-// dst_k0 + k.
-template <int CHUNK, int LAG, class RowOf>
+// dst_k0 + k, or with TIME_MAJOR step t of it to output row t * batch + dst_k0 + k.
+template <int CHUNK, int LAG, bool TIME_MAJOR = false, class RowOf>
 __device__ __forceinline__ void copy_rows(const BulkRows& T, const RowOf& row_of, int64_t dst_k0, int64_t first,
-                                          int64_t items) {
+                                          int64_t items, int64_t batch = 0) {
   constexpr int STAGES = BULK_RING_BYTES / CHUNK;
   static_assert(STAGES <= 32 && STAGES > LAG + 1, "ring geometry");
   extern __shared__ __align__(128) uint8_t smem[];
@@ -94,7 +114,7 @@ __device__ __forceinline__ void copy_rows(const BulkRows& T, const RowOf& row_of
   sm90::mbar_init_fence();
 
   uint32_t phase_bits = 0;  // bit s = parity to wait for on stage s
-  ItemCursor<CHUNK> ld, stc;   // load cursor runs ahead of the store cursor
+  ItemCursor<CHUNK, TIME_MAJOR> ld, stc;   // load cursor runs ahead of the store cursor
   ld.init(T, row_of, first);
   stc = ld;
   int64_t loaded = 0;
@@ -102,7 +122,7 @@ __device__ __forceinline__ void copy_rows(const BulkRows& T, const RowOf& row_of
   const int64_t pre = items < STAGES ? items : STAGES;
   for (; loaded < pre; ++loaded) {
     const uint8_t* src; uint8_t* dst; uint32_t bytes;
-    ld.get(T, dst_k0, src, dst, bytes);
+    ld.get(T, dst_k0, src, dst, bytes, batch);
     sm90::mbar_expect_tx(&bar[loaded], bytes);
     sm90::bulk_g2s(smem + (size_t)loaded * CHUNK, src, bytes, &bar[loaded]);
     ld.next(T, row_of, loaded + 1 < items);
@@ -111,7 +131,7 @@ __device__ __forceinline__ void copy_rows(const BulkRows& T, const RowOf& row_of
   int rs = 0;           // stage to recycle next (item t - LAG)
   for (int64_t t = 0; t < items; ++t) {
     const uint8_t* src; uint8_t* dst; uint32_t bytes;
-    stc.get(T, dst_k0, src, dst, bytes);
+    stc.get(T, dst_k0, src, dst, bytes, batch);
     sm90::mbar_wait(&bar[s], (phase_bits >> s) & 1u);
     phase_bits ^= (1u << s);
     sm90::bulk_s2g(dst, smem + (size_t)s * CHUNK, bytes);
@@ -123,7 +143,7 @@ __device__ __forceinline__ void copy_rows(const BulkRows& T, const RowOf& row_of
       if (loaded < items) {
         sm90::bulk_wait_read<LAG>();   // all but the newest LAG store groups have finished reading SMEM
         const uint8_t* nsrc; uint8_t* ndst; uint32_t nbytes;
-        ld.get(T, dst_k0, nsrc, ndst, nbytes);
+        ld.get(T, dst_k0, nsrc, ndst, nbytes, batch);
         sm90::mbar_expect_tx(&bar[rs], nbytes);
         sm90::bulk_g2s(smem + (size_t)rs * CHUNK, nsrc, nbytes, &bar[rs]);
         ++loaded;
@@ -163,6 +183,20 @@ __device__ __forceinline__ void copy_small_rows(const SmallField& f, const RowOf
                      row_of, k0, k1, u, step);
   else
     copy_small_units(f.src, f.dst, f.row_bytes, row_of, k0, k1, u, step);
+}
+
+// The time-major form for a row of T 4-byte steps (IMPALA's action, mu, reward): dst[t * batch + k] =
+// src[row_of(k) * T + t] for k in [k0, k1).  Each thread reads consecutive words of a row.
+template <class RowOf>
+__device__ __forceinline__ void copy_small_rows_time_major(const SmallField& f, const RowOf& row_of, int64_t k0,
+                                                           int64_t k1, int64_t batch, int64_t u, int64_t step) {
+  const uint32_t* __restrict__ src = reinterpret_cast<const uint32_t*>(f.src);
+  uint32_t* __restrict__ dst = reinterpret_cast<uint32_t*>(f.dst);
+  const int64_t T = f.row_bytes >> 2;
+  for (u += k0 * T; u < k1 * T; u += step) {
+    const int64_t k = u / T, t = u - k * T;
+    dst[t * batch + k] = src[row_of(k) * T + t];
+  }
 }
 
 }  // namespace b2rl

@@ -21,20 +21,20 @@ struct SmallRows {
 };
 
 // BY_ITEMS (fewer draws than SMs): CTA c owns a contiguous range of the minibatch's copy items (draw-major, then
-// field, then 14 KiB chunk: the items of copy_rows), as k_gather_bulk's CTAs do, so the copy still spreads over
-// every SM.  Its threads draw every draw the range touches; a draw is a pure function of the Philox counter and the
-// tree, so each CTA that draws k gets the same slot.  The CTA that holds draw k's first item owns it and alone
+// field, then chunk: the items of copy_rows), as k_gather_bulk's CTAs do, so the copy still spreads over
+// every SM.  Its threads draw every draw the range touches; a draw is a pure function of the Philox counter (and the
+// tree), so each CTA that draws k gets the same slot.  The CTA that holds draw k's first item owns it and alone
 // writes idx[k], w[k] and its scalar and small rows.  Otherwise CTA c owns draws [c*per, (c+1)*per) whole: for Ape-X
 // B = 512 the two splits give the same partition, and the item split's extra index arithmetic measured 1.7 % slower.  Thread 0 copies the range's bulk items with the TMA row copy of bulk_rows.cuh
 // (k_gather_bulk's default geometry: 14 KiB chunks, 16 stages, lag 3), warps 1..3 copy the owned draws' small rows,
 // then the last CTA to finish writes the header.  A record without bulk fields counts one item per draw.
-template <bool BY_ITEMS>
-__global__ void __launch_bounds__(SERVE_THREADS, 1)
-k_serve_fill(const __grid_constant__ TreeView t, const __grid_constant__ BulkRows P, SmallFields small,
-             const __grid_constant__ SmallRows rows, uint64_t* __restrict__ rng_state, int64_t n, int64_t capacity,
-             const float* __restrict__ n_valid_dev, float beta, const float* __restrict__ max_w_ext,
-             int64_t* __restrict__ idx_out, float* __restrict__ w_out, uint64_t* __restrict__ header, uint64_t seq,
-             unsigned int* __restrict__ done_ticket) {
+// draw(seed, offset, k, owned, row) stores the replay row of draw k in `row`; an owned draw also writes its idx / w /
+// scalars.
+// TIME_MAJOR: step t of draw k goes to output row t * n + k (bulk rows and the small rows of T 4-byte steps).
+template <bool BY_ITEMS, bool TIME_MAJOR, int CHUNK, class Draw>
+__device__ __forceinline__ void serve_fill(const BulkRows& P, const SmallRows& rows, uint64_t* __restrict__ rng_state,
+                                           int64_t n, const Draw& draw, uint64_t* __restrict__ header, uint64_t seq,
+                                           unsigned int* __restrict__ done_ticket) {
   __shared__ int64_t s_row[SERVE_THREADS];
   const int tid = threadIdx.x;
   uint64_t seed, offset;
@@ -59,24 +59,21 @@ k_serve_fill(const __grid_constant__ TreeView t, const __grid_constant__ BulkRow
   }
   if (tid < k_hi - k_lo) {
     const int64_t k = k_lo + tid;
-    double root, picked;
-    const int64_t j = tree_draw(t, philox_u01(seed, offset + (uint64_t)k), root, picked);
-    s_row[tid] = clamp_row(j, capacity);   // the row b2rl_replay_gather would copy
-    if (k >= k_own) {
-      idx_out[k] = j;
-      fetch_small(small, j, k);
-      const float s32 = (float)root;
-      w_out[k] = is_weight(t, s32, __fdiv_rn((float)picked, s32), n_valid_dev, beta, max_w_ext);
-    }
+    draw(seed, offset, k, k >= k_own, s_row[tid]);
   }
   __syncthreads();
   if (items > 0) {
     if (tid == 0 && P.n > 0) {
-      copy_rows<14336, 3>(P, [](int64_t i) { return s_row[i]; }, k_lo, first - k_lo * ipr, items);
+      copy_rows<CHUNK, 3, TIME_MAJOR>(P, [](int64_t i) { return s_row[i]; }, k_lo, first - k_lo * ipr, items, n);
     } else if (tid >= 32) {
-      for (int f = 0; f < rows.n; ++f)
-        copy_small_rows(rows.f[f], [&](int64_t k) { return s_row[k - k_lo]; }, k_own, k_hi, tid - 32,
-                        SERVE_THREADS - 32);
+      for (int f = 0; f < rows.n; ++f) {
+        if (TIME_MAJOR)
+          copy_small_rows_time_major(rows.f[f], [&](int64_t k) { return s_row[k - k_lo]; }, k_own, k_hi, n,
+                                     tid - 32, SERVE_THREADS - 32);
+        else
+          copy_small_rows(rows.f[f], [&](int64_t k) { return s_row[k - k_lo]; }, k_own, k_hi, tid - 32,
+                          SERVE_THREADS - 32);
+      }
     }
   }
   // header last: written by the last CTA to get here, after every CTA's copies have completed
@@ -90,6 +87,77 @@ k_serve_fill(const __grid_constant__ TreeView t, const __grid_constant__ BulkRow
       *done_ticket = 0u;       // re-armed for the next fill
     }
   }
+}
+
+// The prioritized fill (Ape-X, R2D2): sum-tree descent + IS weights, batch-major slot.
+template <bool BY_ITEMS>
+__global__ void __launch_bounds__(SERVE_THREADS, 1)
+k_serve_fill(const __grid_constant__ TreeView t, const __grid_constant__ BulkRows P, SmallFields small,
+             const __grid_constant__ SmallRows rows, uint64_t* __restrict__ rng_state, int64_t n, int64_t capacity,
+             const float* __restrict__ n_valid_dev, float beta, const float* __restrict__ max_w_ext,
+             int64_t* __restrict__ idx_out, float* __restrict__ w_out, uint64_t* __restrict__ header, uint64_t seq,
+             unsigned int* __restrict__ done_ticket) {
+  serve_fill<BY_ITEMS, false, 14336>(P, rows, rng_state, n,
+                                     [&](uint64_t seed, uint64_t offset, int64_t k, bool own, int64_t& row) {
+    double root, picked;
+    const int64_t j = tree_draw(t, philox_u01(seed, offset + (uint64_t)k), root, picked);
+    row = clamp_row(j, capacity);   // the row b2rl_replay_gather would copy
+    if (own) {
+      idx_out[k] = j;
+      fetch_small(small, j, k);
+      const float s32 = (float)root;
+      w_out[k] = is_weight(t, s32, __fdiv_rn((float)picked, s32), n_valid_dev, beta, max_w_ext);
+    }
+  }, header, seq, done_ticket);
+}
+
+// The uniform draw without replacement of the IMPALA fill (random.sample, baseline/utils.py:310-315): draw k of a
+// fill is slot (tail + pi(k)) mod capacity, where pi is a keyed pseudorandom permutation of [0, size): a 4-round
+// balanced Feistel network on the smallest even bit width w >= 2 with 2^w >= size, cycle-walked into [0, size).
+// The round keys are the four words of ONE Philox4x32-10 block at the fill's first counter, so a draw is a pure
+// function of (seed, counter, k) and the draws of one fill are distinct by construction.
+struct UniformDraw {
+  int64_t size;        // the valid region [tail, tail + size) mod capacity
+  int64_t tail;
+  int64_t capacity;
+  int32_t half;        // w / 2
+  uint32_t mask;       // 2^half - 1
+};
+
+constexpr int UNIFORM_CHUNK = 14112;   // half an 84x84x4 frame stack: no chunk of a time-major frame row straddles two steps
+
+__host__ __device__ __forceinline__ uint32_t feistel4(uint32_t x, const uint32_t key[4], int half, uint32_t mask) {
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const uint32_t L = x >> half, R = x & mask;
+    x = (R << half) | (L ^ (lowbias32(R ^ key[r]) & mask));
+  }
+  return x;
+}
+
+__device__ __forceinline__ int64_t uniform_row(const UniformDraw& u, const uint32_t key[4], int64_t k) {
+  uint32_t y = feistel4((uint32_t)k, key, u.half, u.mask);
+  while ((int64_t)y >= u.size) y = feistel4(y, key, u.half, u.mask);   // k < size: the walk ends on k's cycle
+  const int64_t j = u.tail + (int64_t)y;
+  return j >= u.capacity ? j - u.capacity : j;
+}
+
+template <bool BY_ITEMS>
+__global__ void __launch_bounds__(SERVE_THREADS, 1)
+k_serve_fill_uniform(const __grid_constant__ BulkRows P, SmallFields small, const __grid_constant__ SmallRows rows,
+                     uint64_t* __restrict__ rng_state, int64_t n, UniformDraw u, int64_t* __restrict__ idx_out,
+                     uint64_t* __restrict__ header, uint64_t seq, unsigned int* __restrict__ done_ticket) {
+  serve_fill<BY_ITEMS, true, UNIFORM_CHUNK>(P, rows, rng_state, n,
+                                            [&](uint64_t seed, uint64_t offset, int64_t k, bool own, int64_t& row) {
+    uint32_t key[4];
+    philox4x32_10(offset, seed, key);
+    const int64_t j = uniform_row(u, key, k);
+    row = j;
+    if (own) {
+      idx_out[k] = j;
+      fetch_small(small, j, k);
+    }
+  }, header, seq, done_ticket);
 }
 
 __global__ void __launch_bounds__(256)
@@ -266,23 +334,39 @@ extern "C" int b2rl_serve_slot_ptrs(const b2rl_serve_ring* r, int32_t slot, void
   return B2RL_OK;
 }
 
-extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, uint64_t seq, float beta,
-                               const float* max_w_dev, void* stream) {
+// What both fills check before anything is launched: the ring was created for this replay, on its device.
+static int fill_slot_ptrs(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, void** ptrs) {
   B2RL_REQUIRE(h != nullptr && r != nullptr, "null argument");
   B2RL_REQUIRE(r->owned && r->device == h->device, "fill needs the ring created for this replay, on its device");
   B2RL_REQUIRE(slot >= 0 && slot < r->L.slots, "slot out of range");
   B2RL_REQUIRE(r->L.n_fields == h->n_fields, "ring and replay have different fields");
+  for (int f = 0; f < h->n_fields; ++f)
+    B2RL_REQUIRE(h->field_bytes[f] == r->L.field_bytes[f], "ring and replay have different fields");
   B2RL_REQUIRE(h->size > 0, "sampling from an empty replay");
-  const b2rl_serve_layout& L = r->L;
+  return b2rl_serve_slot_ptrs(r, slot, ptrs, nullptr);
+}
+
+// One CTA per SM (the shared-memory ring takes the SM).  Split by items: at most one CTA per copy item, and
+// enough CTAs that no item range touches more than SERVE_THREADS draws (a range of at most SERVE_THREADS - 2
+// draws' items starts and ends inside at most SERVE_THREADS draws).  Split by draws: at most SERVE_THREADS each.
+static int64_t fill_grid(int sms, int64_t n, const BulkRows& P, bool by_items) {
+  const int64_t work = by_items ? n * (P.n > 0 ? P.items_per_row : 1) : n;
+  int64_t grid = sms < work ? sms : work;
+  const int64_t min_grid = by_items ? (n + SERVE_THREADS - 3) / (SERVE_THREADS - 2)
+                                    : (n + SERVE_THREADS - 1) / SERVE_THREADS;
+  return grid < min_grid ? min_grid : grid;
+}
+
+extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, uint64_t seq, float beta,
+                               const float* max_w_dev, void* stream) {
   void* ptrs[3 + B2RL_MAX_FIELDS];
-  int rc = b2rl_serve_slot_ptrs(r, slot, ptrs, nullptr);
+  int rc = fill_slot_ptrs(h, r, slot, ptrs);
   if (rc != B2RL_OK) return rc;
   BulkRows P{};
   SmallFields small{};
   SmallRows rows{};
   for (int f = 0; f < h->n_fields; ++f) {
     const int64_t b = h->field_bytes[f];
-    B2RL_REQUIRE(b == L.field_bytes[f], "ring and replay have different fields");
     if (is_bulk_row(b)) {
       P.add(h->field[f], (uint8_t*)ptrs[3 + f], b, 14336);   // the CHUNK of k_serve_fill's copy_rows
     } else if (b == 1 || b == 2 || b == 4 || b == 8) {
@@ -299,20 +383,64 @@ extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot,
   B2RL_CUDA(sm_count(h->device, &sms));
   B2RL_CUDA(set_max_dynamic_smem<k_serve_fill<true>>(h->device, BULK_RING_BYTES));
   B2RL_CUDA(set_max_dynamic_smem<k_serve_fill<false>>(h->device, BULK_RING_BYTES));
-  // one CTA per SM (the shared-memory ring takes the SM).  Split by items: at most one CTA per copy item, and
-  // enough CTAs that no item range touches more than SERVE_THREADS draws (a range of at most SERVE_THREADS - 2
-  // draws' items starts and ends inside at most SERVE_THREADS draws).  Split by draws: at most SERVE_THREADS each.
-  const int64_t n = L.batch;
+  const int64_t n = r->L.batch;
   const bool by_items = n < sms;
-  const int64_t work = by_items ? n * (P.n > 0 ? P.items_per_row : 1) : n;
-  int64_t grid = sms < work ? sms : work;
-  const int64_t min_grid = by_items ? (n + SERVE_THREADS - 3) / (SERVE_THREADS - 2)
-                                    : (n + SERVE_THREADS - 1) / SERVE_THREADS;
-  if (grid < min_grid) grid = min_grid;
   auto kernel = by_items ? k_serve_fill<true> : k_serve_fill<false>;
-  kernel<<<(unsigned)grid, SERVE_THREADS, BULK_RING_BYTES, (cudaStream_t)stream>>>(
+  kernel<<<(unsigned)fill_grid(sms, n, P, by_items), SERVE_THREADS, BULK_RING_BYTES, (cudaStream_t)stream>>>(
       h->tree, P, small, rows, h->rng_dev, n, h->capacity, h->n_valid_dev, beta, max_w_dev, (int64_t*)ptrs[1],
       (float*)ptrs[2], (uint64_t*)ptrs[0], seq, r->done_ticket);
+  count_launch();
+  B2RL_CHECK_LAUNCH();
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_serve_fill_uniform(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, uint64_t seq, int32_t steps,
+                                       void* stream) {
+  void* ptrs[3 + B2RL_MAX_FIELDS];
+  int rc = fill_slot_ptrs(h, r, slot, ptrs);
+  if (rc != B2RL_OK) return rc;
+  B2RL_REQUIRE(steps >= 1, "steps must be >= 1");
+  const int64_t n = r->L.batch, size = h->size, cap = h->capacity;
+  B2RL_REQUIRE(n <= size, "sample larger than population: the batch exceeds the stored records");
+  B2RL_REQUIRE(size <= (1LL << 32), "a uniform fill draws from at most 2^32 records");
+  UniformDraw u{};
+  u.size = size;
+  u.capacity = cap;
+  u.tail = ((h->head - size) % cap + cap) % cap;   // the valid region, as impala.Replay.draw takes it
+  int w = 2;
+  while ((1LL << w) < size) w += 2;
+  u.half = w / 2;
+  u.mask = (1u << u.half) - 1u;
+  BulkRows P{};
+  SmallFields small{};
+  SmallRows rows{};
+  for (int f = 0; f < h->n_fields; ++f) {
+    const int64_t b = h->field_bytes[f];
+    if (is_bulk_row(b)) {        // T + 1 steps (the frame stacks s_0 .. s_T)
+      B2RL_REQUIRE(b % (steps + 1) == 0 && (b / (steps + 1)) % 16 == 0,
+                   "a bulk row of a time-major slot must be steps + 1 rows of a multiple of 16 bytes");
+      P.add_time_major(h->field[f], (uint8_t*)ptrs[3 + f], b, steps + 1, UNIFORM_CHUNK);
+    } else if (b == 4 * (int64_t)steps) {     // T 4-byte steps (action, mu, reward)
+      rows.f[rows.n++] = SmallField{h->field[f], (uint8_t*)ptrs[3 + f], b};
+    } else if (b == 1 || b == 2 || b == 4 || b == 8) {   // a batch-major scalar (done)
+      small.src[small.n] = h->field[f];
+      small.dst[small.n] = (uint8_t*)ptrs[3 + f];
+      small.bytes[small.n] = (int)b;
+      small.n++;
+    } else {
+      B2RL_REQUIRE(false, "a time-major slot holds bulk rows of steps + 1 steps, rows of steps 4-byte words and "
+                          "1/2/4/8-byte scalars only");
+    }
+  }
+  DeviceGuard g(h->device);
+  int sms = 0;
+  B2RL_CUDA(sm_count(h->device, &sms));
+  B2RL_CUDA(set_max_dynamic_smem<k_serve_fill_uniform<true>>(h->device, BULK_RING_BYTES));
+  B2RL_CUDA(set_max_dynamic_smem<k_serve_fill_uniform<false>>(h->device, BULK_RING_BYTES));
+  const bool by_items = n < sms;
+  auto kernel = by_items ? k_serve_fill_uniform<true> : k_serve_fill_uniform<false>;
+  kernel<<<(unsigned)fill_grid(sms, n, P, by_items), SERVE_THREADS, BULK_RING_BYTES, (cudaStream_t)stream>>>(
+      P, small, rows, h->rng_dev, n, u, (int64_t*)ptrs[1], (uint64_t*)ptrs[0], seq, r->done_ticket);
   count_launch();
   B2RL_CHECK_LAUNCH();
   return B2RL_OK;

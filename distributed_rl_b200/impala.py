@@ -110,17 +110,34 @@ class Replay(ReplayThread):
 
 
 class Learner:
-    def __init__(self, cfg: ImpalaConfig | None = None, connect=None, start_replay: bool = True):
+    def __init__(self, cfg: ImpalaConfig | None = None, connect=None, start_replay: bool = True, memory=None):
+        """`memory`: a replay served from another process (replay_server.DeviceReplayClient built with this
+        ImpalaConfig, or anything with its surface: sample / memory).  run() then drives sample() -> train() on it;
+        fused_step() needs the in-process Replay."""
         self.cfg = cfg or ImpalaConfig.from_configuration()
         self.device = torch.device(self.cfg.LEARNER_DEVICE)
         self.model = GraphAgent(self.cfg.MODEL).to(self.device)
         self.model.dense_3xtf32 = bool(self.cfg.DENSE_3XTF32) and self.device.type == "cuda"
         self.mOptim = make_optimizer(self.cfg.OPTIM_INFO, self.model.getParameters())
         self._connect = connect
-        self._memory = Replay(self.cfg, connect)
-        if connect is not None and start_replay:
-            self._memory.start()                                # IMPALA/Learner.py:27-28
+        self._served = memory is not None
+        if self._served:
+            self._memory = memory
+            if start_replay and not memory.is_alive():
+                memory.start()
+        else:
+            self._memory = Replay(self.cfg, connect)
+            if connect is not None and start_replay:
+                self._memory.start()                            # IMPALA/Learner.py:27-28
         self.last = {}
+
+    @property
+    def memory(self):
+        return self._memory
+
+    def _stored(self) -> int:
+        """Rollouts in the replay: a served memory reports the server's count through `memory`."""
+        return len(self._memory.memory) if self._served else len(self._memory)
 
     def forward(self, state, action):
         """IMPALA/Learner.py:70-83: pi(a|s) of the taken action and V(s)."""
@@ -225,7 +242,7 @@ class Learner:
         the weights are snapshot on the learner stream and SET once their D2H copy has landed; if the previous
         snapshot is still in flight this step's is skipped (the actors poll every 400 env steps anyway)."""
         import time
-        while len(self._memory) <= self.cfg.BUFFER_SIZE:
+        while self._stored() <= self.cfg.BUFFER_SIZE:
             time.sleep(0.05)
         pub = ParamPublisher(self.model, self._connect, "params", "Count", wrap=lambda sd: (sd,))
         self._publishers, ckpt = publishers(self.model, self.cfg.LOG_W, pub)

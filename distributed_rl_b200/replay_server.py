@@ -2,7 +2,9 @@
 R2D2/ReplayServer.py:20-175) owns the prioritized replay in ITS OWN process / GPU and serves pre-assembled minibatches
 over the reference's Redis protocol; `Replay_Server` (APE_X/ReplayMemory.py:170-257, R2D2/ReplayMemory.py:187-274) is
 the learner-side consumer with the `Replay` surface (`sample()`, `update()`, `start()`).  Every server and client
-serves the record kind of its config: Ape-X transitions (`ApexConfig`) or R2D2 sequences (`R2D2Config`), see `KINDS`.
+serves the record kind of its config: Ape-X transitions (`ApexConfig`), R2D2 sequences (`R2D2Config`) or, on the
+device ring only, IMPALA rollouts (`ImpalaConfig`), see `KINDS`.  The reference has no IMPALA replay server, so the
+Redis-protocol pair refuses an ImpalaConfig.
 
 Keys (the reference's): list `experience` (actors -> server), list `BATCH` on the push connection (server ->
 learner: pickled `[s, a, r, s', done, w, idx]` or `[(h0, h1), s, a, r, notdone, w, idx]`), list `update` (learner ->
@@ -36,7 +38,12 @@ leaves slots unserved, it cannot hang a GPU.
 
 Shutdown: the learner closes its client first (unmap, then SERVE_DETACHED); the server frees the ring only after
 that key appears.  A learner that attached with `apex.Learner(connect=..., memory=client)` or
-`r2d2.Learner(connect=..., memory=client)` keeps SERVER_KEYS out of its start-up wipe of stale keys."""
+`r2d2.Learner(connect=..., memory=client)` keeps SERVER_KEYS out of its start-up wipe of stale keys
+(`impala.Learner` wipes no keys).
+
+IMPALA rollouts are unprioritized: the server fills a slot with `b2rl_serve_fill_uniform` (B distinct rollouts drawn
+uniformly from the valid region, written time-major so that `state` is conv_1's frame table as it lies in the slot),
+publishes a max IS weight of 0 and never receives update slots."""
 from __future__ import annotations
 
 import ctypes as C
@@ -53,8 +60,9 @@ import torch
 from . import _lib, wire
 from . import replay as R
 from ._lib import check
-from . import apex, r2d2
+from . import apex, impala, r2d2
 from .apex import ApexConfig
+from .impala import ImpalaConfig
 from .learner_common import Stoppable
 from .r2d2 import R2D2Config
 
@@ -63,12 +71,18 @@ from .r2d2 import R2D2Config
 class RecordKind:
     """What the servers and clients need to know about the records they serve."""
     name: str
-    replay: type                    # the ingest Replay: decoder of the actors' `experience` records + the store
+    replay: type                    # the ingest Replay: decoder of the actors' records + the store
     fields: Callable                # cfg -> the store's fields
     batch: Callable                 # (gathered fields, IS weights, indices) -> the learner's minibatch list
-    host: Callable                  # (field name, CPU tensor) -> what a pickled `BATCH` blob carries
+    host: Callable | None           # (field name, CPU tensor) -> what a pickled `BATCH` blob carries
     m: int                          # minibatches per ReplayServer.buffer()
     enough: int                     # Replay_Server raises FLAG_ENOUGH above this many queued minibatches
+    list_key: str = "experience"    # the actors' Redis list the server drains
+    steps: Callable | None = None   # cfg -> T for a uniform, time-major kind (IMPALA); None: prioritized, batch-major
+
+    @property
+    def prioritized(self) -> bool:
+        return self.steps is None
 
 
 def _apex_batch(b, w, idx):
@@ -81,6 +95,11 @@ def _r2d2_batch(b, w, idx):
     return [(b["h0"].unsqueeze(0), b["h1"].unsqueeze(0)), b["state"], b["action"], b["reward"], b["notdone"], w, idx]
 
 
+def _impala_batch(b, w, idx):
+    """IMPALA/ReplayMemory.py:30-54 (impala.Replay.bufferSave): (s, a, mu, r, done), s (T+1, B, 28224) time-major."""
+    return (b["state"], b["action"], b["mu"], b["reward"], b["done"])
+
+
 KINDS = {
     "apex": RecordKind("apex", apex.Replay, lambda cfg: R.APEX_FIELDS, _apex_batch,
                        lambda name, t: t.numpy().astype(bool) if name == "done" else t.numpy(),
@@ -88,20 +107,34 @@ KINDS = {
     "r2d2": RecordKind("r2d2", r2d2.Replay, lambda cfg: R.r2d2_fields(cfg.FIXED_TRAJECTORY), _r2d2_batch,
                        lambda name, t: t if name in ("h0", "h1") else t.numpy(),   # h0 / h1 stay torch (:100-101)
                        m=8, enough=18),                       # R2D2/ReplayServer.py:66, R2D2/ReplayMemory.py:249
+    "impala": RecordKind("impala", impala.Replay, lambda cfg: R.impala_fields(cfg.UNROLL_STEP), _impala_batch,
+                         None, m=1, enough=0, list_key="trajectory",           # IMPALA/ReplayMemory.py:56-76
+                         steps=lambda cfg: cfg.UNROLL_STEP),
 }
 
 
 def record_kind(cfg) -> RecordKind:
-    """The kind a config describes: R2D2Config -> sequences, anything else (ApexConfig) -> transitions."""
-    return KINDS["r2d2" if isinstance(cfg, R2D2Config) else "apex"]
+    """The kind a config describes: R2D2Config -> sequences, ImpalaConfig -> rollouts, anything else (ApexConfig)
+    -> transitions."""
+    if isinstance(cfg, R2D2Config):
+        return KINDS["r2d2"]
+    return KINDS["impala" if isinstance(cfg, ImpalaConfig) else "apex"]
+
+
+def _redis_protocol_kind(cfg) -> None:
+    """The Redis-protocol pair serves the reference's two replay servers (Ape-X, R2D2) and nothing else."""
+    if cfg is not None and not record_kind(cfg).prioritized:
+        raise ValueError(f"the Redis-protocol replay server has no {record_kind(cfg).name} mode (the reference has no "
+                         "IMPALA replay server): serve it with DeviceReplayServer / DeviceReplayClient")
 
 
 class _StandaloneServer(Stoppable):
     """What the two stand-alone servers share (APE_X/ReplayServer.py:20-160, R2D2/ReplayServer.py:20-175): the
-    ingest of `experience` into the store, FLAG_BATCH once the store holds more than BUFFER_SIZE records, and
-    eviction on FLAG_REMOVE.  `cfg`: ApexConfig (the default, from `configuration`) or R2D2Config."""
+    ingest of the actors' records (`experience`, IMPALA's `trajectory`) into the store, FLAG_BATCH once the store
+    holds more than BUFFER_SIZE records, and eviction on FLAG_REMOVE.  `cfg`: ApexConfig (the default, from
+    `configuration`), R2D2Config or ImpalaConfig."""
 
-    def __init__(self, cfg: ApexConfig | R2D2Config | None, connect):
+    def __init__(self, cfg: ApexConfig | R2D2Config | ImpalaConfig | None, connect):
         super().__init__()
         self.cfg = cfg or ApexConfig.from_configuration()
         if getattr(self.cfg, "PAYLOAD_POOL", 0):
@@ -116,11 +149,12 @@ class _StandaloneServer(Stoppable):
         self.total_transition = 0
 
     def _ingest_experience(self) -> list:
-        """The top of serve_once(): raise FLAG_BATCH, then push the drained `experience` records. -> the records."""
+        """The top of serve_once(): raise FLAG_BATCH, then push the drained records of the kind's list. -> the
+        records."""
         if len(self.store) > self.cfg.BUFFER_SIZE and not self.FLAG_BATCH:
             self.FLAG_BATCH = True
             self.connect.set("FLAG_BATCH", pickle.dumps(True))
-        data = wire.drain(self.connect, "experience")
+        data = wire.drain(self.connect, self.kind.list_key)
         if data:
             self._ingest.push_records(data)
             self.total_transition += len(data)
@@ -140,6 +174,7 @@ class _StandaloneServer(Stoppable):
 class ReplayServer(_StandaloneServer):
     def __init__(self, cfg: ApexConfig | R2D2Config | None = None, connect=None, connect_push=None,
                  m: int | None = None):
+        _redis_protocol_kind(cfg)
         super().__init__(cfg, connect)
         self.connect_push = connect_push if connect_push is not None else connect
         self.m = self.kind.m if m is None else m   # minibatches per buffer() (the reference: Ape-X 32, R2D2 8; :66)
@@ -200,6 +235,7 @@ class Replay_Server(Stoppable, threading.Thread):
     second time, already unpickled, which its sample() then fails to unpickle; DESIGN.md §2)."""
 
     def __init__(self, cfg: ApexConfig | R2D2Config | None = None, connect=None, connect_push=None):
+        _redis_protocol_kind(cfg)
         super().__init__(daemon=True)
         self.cfg = cfg or ApexConfig.from_configuration()
         self.kind = record_kind(self.cfg)
@@ -302,6 +338,10 @@ class ServeRing:
     def fill(self, store: R.DeviceReplay, k: int, seq: int, beta: float, max_w: torch.Tensor | None = None) -> None:
         check(self.lib.b2rl_serve_fill(store._h, self._h, int(k), int(seq), float(beta),
                                        None if max_w is None else max_w.data_ptr(), store._st()))
+
+    def fill_uniform(self, store: R.DeviceReplay, k: int, seq: int, steps: int) -> None:
+        """B distinct records drawn uniformly from the store's valid region, time-major over `steps` (IMPALA's T)."""
+        check(self.lib.b2rl_serve_fill_uniform(store._h, self._h, int(k), int(seq), int(steps), store._st()))
 
     def take(self, k: int, dst: torch.Tensor, stream) -> None:
         assert dst.is_contiguous() and dst.numel() * dst.element_size() >= self.layout.slot_bytes
@@ -432,7 +472,7 @@ class DeviceReplayServer(_StandaloneServer):
 
     STATS_EVERY = 0.1             # seconds between SERVE_STATS refreshes (each costs a device sync)
 
-    def __init__(self, cfg: ApexConfig | R2D2Config | None = None, connect=None, slots: int = 4):
+    def __init__(self, cfg: ApexConfig | R2D2Config | ImpalaConfig | None = None, connect=None, slots: int = 4):
         super().__init__(cfg, connect)
         self.device = self.store.device
         self.ring = ServeRing.create(self.store, self.cfg.BATCHSIZE, slots)
@@ -473,13 +513,22 @@ class DeviceReplayServer(_StandaloneServer):
         self.applied[j].record(st)
 
     def _fill(self, k: int, seq: int) -> None:
-        self.ring.fill(self.store, k, seq, self.cfg.BETA)
+        if self.kind.prioritized:
+            self.ring.fill(self.store, k, seq, self.cfg.BETA)
+        else:
+            self.ring.fill_uniform(self.store, k, seq, self.kind.steps(self.cfg))
         self.filled[k].record(self._stream())
+
+    def _can_fill(self) -> bool:
+        """More than BUFFER_SIZE records; a draw without replacement also needs at least B of them."""
+        n = len(self.store)
+        return n > self.cfg.BUFFER_SIZE and (self.kind.prioritized or n >= self.cfg.BATCHSIZE)
 
     def _publish_stats(self, force: bool) -> None:
         now = time.time()
         if force or now - self._stats_t > self.STATS_EVERY:
-            mw = float(self.store.stats(self.cfg.BETA)[2].item()) if len(self.store) else 0.0
+            prio = self.kind.prioritized and len(self.store)
+            mw = float(self.store.stats(self.cfg.BETA)[2].item()) if prio else 0.0
             self.connect.set(STATS_KEY, pickle.dumps((len(self.store), mw)))
             self._stats_t = now
 
@@ -488,7 +537,7 @@ class DeviceReplayServer(_StandaloneServer):
         data = self._ingest_experience()
         released = self.slots.collect_releases(self._wait_released)
         applied = self.slots.apply_updates(self._apply)
-        filled = self.slots.fill_free(self._fill) if len(self.store) > self.cfg.BUFFER_SIZE else 0
+        filled = self.slots.fill_free(self._fill) if self._can_fill() else 0
         self._evict_on_request()
         self._publish_stats(bool(data))
         return {"ingested": len(data), "filled": filled, "released": released, "updates_applied": applied}
@@ -537,11 +586,13 @@ class DeviceReplayClient(Stoppable, threading.Thread):
     """Learner-side consumer of a DeviceReplayServer with the `Replay` surface (start / stop / sample / update / lock /
     memory; APE_X/ReplayMemory.py:170-257).  sample() returns `[s, a, r, s', done, w, idx]` as CUDA tensors on the
     learner's device, copied out of the ring (a peer copy when the server is on another GPU); with an R2D2Config,
-    `[(h0, h1), s, a, r, notdone, w, idx]` as r2d2.Replay.sample returns it."""
+    `[(h0, h1), s, a, r, notdone, w, idx]` as r2d2.Replay.sample returns it; with an ImpalaConfig,
+    `(s, a, mu, r, done)` time-major as impala.Replay.sample returns it (`last_idx` holds the rollouts' slots)."""
 
     KEEP_KEYS = SERVER_KEYS       # what apex/r2d2.Learner(connect=..., memory=this) leaves in place at start-up
 
-    def __init__(self, cfg: ApexConfig | R2D2Config | None = None, connect=None, timeout: float = 60.0):
+    def __init__(self, cfg: ApexConfig | R2D2Config | ImpalaConfig | None = None, connect=None,
+                 timeout: float = 60.0):
         super().__init__(daemon=True)
         self.cfg = cfg or ApexConfig.from_configuration()
         self.kind = record_kind(self.cfg)
@@ -573,6 +624,7 @@ class DeviceReplayClient(Stoppable, threading.Thread):
         self._pending = deque()      # priority write-backs waiting for a free update slot
         self.last_served = None      # descriptor (k, seq, n) of the last served slot
         self.last_header = None      # its header {seq, n} as copied out: a device int64[2]
+        self.last_idx = None         # its replay slots: a device int64[B]
 
     def poll_once(self) -> None:
         self.slots.poll()
@@ -590,8 +642,12 @@ class DeviceReplayClient(Stoppable, threading.Thread):
 
         def view(off, nbytes, dtype, shape):
             return buf[off:off + nbytes].view(dtype).view(shape)
-        out = {f.name: view(L.field_off[i], B * f.nbytes, f.dtype, (B,) + tuple(f.shape))
-               for i, f in enumerate(self.fields)}
+
+        def shape(f):            # a time-major slot: step t of record k at row t * B + k; scalars stay (B,)
+            if self.kind.prioritized or not f.shape:
+                return (B,) + tuple(f.shape)
+            return (f.shape[0], B) + tuple(f.shape[1:])
+        out = {f.name: view(L.field_off[i], B * f.nbytes, f.dtype, shape(f)) for i, f in enumerate(self.fields)}
         return (view(0, 16, torch.int64, (2,)), view(L.idx_off, 8 * B, torch.int64, (B,)),
                 view(L.w_off, 4 * B, torch.float32, (B,)), out)
 
@@ -613,13 +669,15 @@ class DeviceReplayClient(Stoppable, threading.Thread):
         if desc is None:
             return False
         header, idx, w, b = self._views(got[0])
-        self.last_served, self.last_header = desc, header
+        self.last_served, self.last_header, self.last_idx = desc, header, idx
         return self.kind.batch(b, w, idx)
 
     def update(self, idx, vals) -> None:
         """Replay_Server.update (APE_X/ReplayMemory.py:188-190): the write-back goes to free update slots of the
         ring (at most B pairs each) and is applied by the server in stream order.  `idx`: a tensor, an array, or a
-        list of ints or 0-d tensors."""
+        list of ints or 0-d tensors.  An unprioritized kind (IMPALA) has no write-back."""
+        if not self.kind.prioritized:
+            raise TypeError(f"the {self.kind.name} replay is uniform: it has no priorities to write back")
         if isinstance(idx, (list, tuple)):
             idx = torch.stack([torch.as_tensor(i) for i in idx]) if len(idx) and torch.is_tensor(idx[0]) \
                 else torch.as_tensor(np.asarray(idx, np.int64))

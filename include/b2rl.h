@@ -402,6 +402,19 @@ int b2rl_serve_slot_ptrs(const b2rl_serve_ring* r, int32_t slot, void** batch_ou
  * b2rl_replay_gather from the same RNG state, bit for bit.  max_w_dev: as for b2rl_tree_sample. */
 int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, uint64_t seq, float beta,
                     const float* max_w_dev, void* stream);
+/* IMPALA's minibatch (IMPALA/ReplayMemory.py:30-54: s[T+1, B], a[T, B], mu[T, B], r[T, B], done[B]) in ONE launch:
+ * B rollouts drawn uniformly WITHOUT replacement from the ring's valid region [head - size, head), as random.sample
+ * draws them (baseline/utils.py:310-315), written TIME-MAJOR into minibatch slot `slot`.  Draw k is slot
+ * (tail + pi(k)) mod capacity, tail = (head - size) mod capacity, where pi is a permutation of [0, size): a 4-round
+ * balanced Feistel network on the smallest even bit width >= 2 covering size, cycle-walked into [0, size), with the
+ * four words of the Philox4x32-10 block of the handle's device-resident stream at its current counter as round keys
+ * (the counter advances by B).  size and head are the host-side values of b2rl_replay_size at the call.  Field
+ * layout, with steps = T: a bulk row of (T + 1) equal steps -> step t of draw k at row t * B + k; a row of T 4-byte
+ * words -> word t of draw k at t * B + k; a 1/2/4/8-byte scalar -> row k.  idx is written, w is not (uniform replay
+ * has no IS weights), the header {seq, B} last.  Same slot layout and ring as b2rl_serve_fill.  An error, and no
+ * launch, when B > size or the ring was not created for h. */
+int b2rl_serve_fill_uniform(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, uint64_t seq, int32_t steps,
+                            void* stream);
 /* Replay_Server.sample (APE_X/ReplayMemory.py:251-257) without the unpickle: copy minibatch slot k (slot_bytes,
  * header included) to dst_dev with one cudaMemcpyAsync on `stream` (a peer copy when the ring is on another GPU). */
 int b2rl_serve_take(const b2rl_serve_ring* r, int32_t slot, void* dst_dev, void* stream);

@@ -1,16 +1,19 @@
-"""Stand-alone replay server transports, Ape-X transitions or R2D2 sequences at batch B: served minibatches/s and
-learner steps/s for
-  redis   ReplayServer -> pickled `BATCH` list -> Replay_Server (host arrays, copied to the device by train())
+"""Stand-alone replay server transports, Ape-X transitions, R2D2 sequences or IMPALA rollouts at batch B: served
+minibatches/s and learner steps/s for
+  redis   ReplayServer -> pickled `BATCH` list -> Replay_Server (host arrays, copied to the device by train());
+          Ape-X and R2D2 only
   ring    DeviceReplayServer -> device serve ring (CUDA IPC) -> DeviceReplayClient
   fused   the in-process learner: Learner.fused_step() on its own replay (no server)
-  fill    b2rl_serve_fill alone, in this process: CUDA events around `steps` fills into alternating ring slots, at
-          each batch of --fill-batches; bytes/s = 2 x slot bytes / fill time (each byte read once, written once)
+  sample  IMPALA only: the in-process Replay's sample() -> Learner.train() (gather + time-major transpose per step)
+  fill    b2rl_serve_fill (IMPALA: b2rl_serve_fill_uniform) alone, in this process: CUDA events around `steps` fills
+          into alternating ring slots, at each batch of --fill-batches; bytes/s = 2 x slot bytes / fill time (each
+          byte read once, written once)
 
-    python tools/bench_serve.py [--workload apex|r2d2] [--slots-store N] [--batch B] [--steps 200] [--warmup 20]
-                                [--repeats 3] [--arms redis,ring,fused,fill]
+    python tools/bench_serve.py [--workload apex|r2d2|impala] [--slots-store N] [--batch B] [--steps 200]
+                                [--warmup 20] [--repeats 3] [--arms redis,ring,fused,sample,fill]
 
 Defaults per workload: Ape-X B = 512 on a 2^16-slot store (3.7 GB); R2D2 B = 64, T = 80, MEM = 20 on a 2^12-sequence
-store (9.2 GB).
+store (9.2 GB); IMPALA B = 32, T = 20 on a 2^11-rollout store (1.2 GB).
 
 The server runs in a `spawn` child on --server-device, the learner here on cuda:0; the control plane is a Redis
 server (--redis HOST) or, by default, the in-memory Redis stand-in of the tests hosted by a multiprocessing manager
@@ -47,7 +50,10 @@ def _connect(args, proxy):
 
 
 def _cfg(args, device):
-    from distributed_rl_b200 import apex, r2d2
+    from distributed_rl_b200 import apex, impala, r2d2
+    if args["workload"] == "impala":
+        return impala.ImpalaConfig(BATCHSIZE=args["batch"], UNROLL_STEP=20, REPLAY_MEMORY_LEN=args["store"],
+                                   BUFFER_SIZE=0, LEARNER_DEVICE=device)
     if args["workload"] == "r2d2":
         return r2d2.R2D2Config(BATCHSIZE=args["batch"], REPLAY_MEMORY_LEN=args["store"], BUFFER_SIZE=0,
                                FIXED_TRAJECTORY=80, MEM=20, LEARNER_DEVICE=device)
@@ -56,8 +62,8 @@ def _cfg(args, device):
 
 
 def _learner(args, cfg, memory=None):
-    from distributed_rl_b200 import apex, r2d2
-    mod = r2d2 if args["workload"] == "r2d2" else apex
+    from distributed_rl_b200 import apex, impala, r2d2
+    mod = {"r2d2": r2d2, "impala": impala}.get(args["workload"], apex)
     return mod.Learner(cfg, connect=None, start_replay=False, **({} if memory is None else {"memory": memory}))
 
 
@@ -65,6 +71,13 @@ def _fill(store, n):
     import torch
     store.fill_hash(n, seed=0xB200)
     store.build(torch.rand(n, generator=torch.Generator().manual_seed(0)).to(store.device) + 1e-3)
+    if "mu" in [f.name for f in store.fields]:
+        # IMPALA rollouts: Learner.train indexes the policy with the stored actions, so hashed words will not do
+        g = torch.Generator(device=store.device).manual_seed(0)
+        store.field_view("action").random_(0, 6, generator=g)          # ImpalaConfig.ACTION_SIZE
+        store.field_view("mu").uniform_(0.1, 1.0, generator=g)
+        store.field_view("reward").normal_(generator=g)
+        store.field_view("done").bernoulli_(0.9, generator=g)
 
 
 def _server_main(kind, proxy, args, stop):
@@ -141,6 +154,9 @@ def _served_arm(kind, args):
 
         def step():
             b = next_batch()
+            if args["workload"] == "impala":        # uniform replay: no priorities to write back
+                L.train(b)
+                return
             info, prio, idx = L.train(b)[:3]
             client.update(idx if kind == "ring" else list(idx.tolist()), prio)
         n = args["redis_steps"] if kind == "redis" else args["steps"]
@@ -174,6 +190,19 @@ def _fused_arm(args):
     return {"served_minibatches_per_s": None, "learner_steps_per_s": rate}
 
 
+def _sample_arm(args):
+    """IMPALA's in-process path through the learner's own replay: Replay.sample() (draw, gather, transpose to
+    time-major) -> Learner.train()."""
+    import torch
+    cfg = _cfg(args, "cuda:0")
+    L = _learner(args, cfg)
+    _fill(L.memory.store, args["store"])
+    rate = _timed(lambda: L.train(L.memory.sample()), args["steps"], args["warmup"], torch.device("cuda:0"))
+    del L
+    torch.cuda.empty_cache()
+    return {"served_minibatches_per_s": None, "learner_steps_per_s": rate}
+
+
 def _fill_arm(args):
     """b2rl_serve_fill alone: one store, a 2-slot ring per batch size, CUDA events around `steps` back-to-back
     fills (slots alternate, as a server with a free slot would fill them)."""
@@ -181,19 +210,26 @@ def _fill_arm(args):
     from distributed_rl_b200 import replay as R
     from distributed_rl_b200.replay_server import ServeRing, record_kind
     cfg = _cfg(args, "cuda:0")
-    store = R.DeviceReplay(args["store"], record_kind(cfg).fields(cfg), "cuda:0")
+    kind = record_kind(cfg)
+    store = R.DeviceReplay(args["store"], kind.fields(cfg), "cuda:0")
     _fill(store, args["store"])
     out = {}
     try:
         for B in args["fill_batches"]:
             ring = ServeRing.create(store, B, 2)
+
+            def fill(i):
+                if kind.prioritized:
+                    ring.fill(store, i % 2, i + 1, cfg.BETA)
+                else:
+                    ring.fill_uniform(store, i % 2, i + 1, kind.steps(cfg))
             for i in range(args["warmup"]):
-                ring.fill(store, i % 2, i + 1, cfg.BETA)
+                fill(i)
             st = torch.cuda.current_stream()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record(st)
             for i in range(args["steps"]):
-                ring.fill(store, i % 2, i + 1, cfg.BETA)
+                fill(i)
             e1.record(st)
             e1.synchronize()
             t = e0.elapsed_time(e1) / 1e3 / args["steps"]
@@ -210,10 +246,11 @@ def _fill_arm(args):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", choices=("apex", "r2d2"), default="apex")
+    ap.add_argument("--workload", choices=("apex", "r2d2", "impala"), default="apex")
     ap.add_argument("--slots-store", type=int, default=None,
-                    help="replay slots (default: Ape-X 2^16 = 3.7 GB, R2D2 2^12 sequences = 9.2 GB)")
-    ap.add_argument("--batch", type=int, default=None, help="default: Ape-X 512, R2D2 64")
+                    help="replay slots (default: Ape-X 2^16 = 3.7 GB, R2D2 2^12 sequences = 9.2 GB, IMPALA 2^11 "
+                         "rollouts = 1.2 GB)")
+    ap.add_argument("--batch", type=int, default=None, help="default: Ape-X 512, R2D2 64, IMPALA 32")
     ap.add_argument("--fill-batches", default=None, help="batch sizes of the fill arm, e.g. 32,64 (default: --batch)")
     ap.add_argument("--redis-steps", type=int, default=None, help="timed steps of the redis arm (default: --steps)")
     ap.add_argument("--ring-slots", type=int, default=4)
@@ -221,7 +258,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--server-device", default="cuda:0")
-    ap.add_argument("--arms", default="redis,ring,fused", help="any of redis, ring, fused, fill")
+    ap.add_argument("--arms", default=None, help="any of redis, ring, fused, sample, fill (default: Ape-X and R2D2 "
+                    "redis,ring,fused; IMPALA ring,sample,fused)")
     ap.add_argument("--redis", default=None, help="host of a Redis server for the control plane (default: an "
                     "in-memory stand-in in a manager process, which makes the Redis-pickle arm far slower than a "
                     "Redis server would)")
@@ -229,15 +267,17 @@ def main():
     import torch
     if not torch.cuda.is_available():
         sys.exit("bench_serve.py measures on a CUDA device; none is available")
-    r2 = a.workload == "r2d2"
-    store = a.slots_store or (4096 if r2 else 65536)
-    batch = a.batch or (64 if r2 else 512)
+    store = a.slots_store or {"r2d2": 4096, "impala": 2048}.get(a.workload, 65536)
+    batch = a.batch or {"r2d2": 64, "impala": 32}.get(a.workload, 512)
+    arms = a.arms or ("ring,sample,fused" if a.workload == "impala" else "redis,ring,fused")
+    if a.workload == "impala" and "redis" in arms.split(","):
+        sys.exit("IMPALA has no Redis-protocol replay server")
     args = {"workload": a.workload, "store": store, "batch": batch, "ring_slots": a.ring_slots, "steps": a.steps,
             "warmup": a.warmup, "server_device": a.server_device, "redis": a.redis,
             "redis_steps": a.redis_steps or a.steps,
             "fill_batches": [int(x) for x in a.fill_batches.split(",")] if a.fill_batches else [batch]}
-    runs = {k: [] for k in a.arms.split(",")}
-    arm = {"fused": _fused_arm, "fill": _fill_arm}
+    runs = {k: [] for k in arms.split(",")}
+    arm = {"fused": _fused_arm, "sample": _sample_arm, "fill": _fill_arm}
     for _ in range(a.repeats):
         for k in runs:
             runs[k].append(arm[k](args) if k in arm else _served_arm(k, args))
