@@ -63,6 +63,8 @@ SIGNATURES = {
     "b2rl_conv1_fused": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp]),
     "b2rl_conv1_wgrad_workspace_floats": (c_i64, [c_i32]),
     "b2rl_conv1_wgrad": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp]),
+    "b2rl_conv1_fused_table": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp]),
+    "b2rl_conv1_wgrad_table": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp]),
     "b2rl_rmsprop_step": (C.c_int, [C.POINTER(c_vp), C.POINTER(c_vp), C.POINTER(c_vp), C.POINTER(c_vp),
                                     C.POINTER(c_i64), c_i32, c_f64, c_f64, c_f64, c_i32, C.POINTER(c_i64), c_vp, c_vp,
                                     c_vp]),
@@ -93,6 +95,8 @@ SIGNATURES = {
     "b2rl_serve_fill": (C.c_int, [c_vp, c_vp, c_i32, c_u64, c_f32, c_vp, c_vp]),
     "b2rl_serve_fill_uniform": (C.c_int, [c_vp, c_vp, c_i32, c_u64, c_i32, c_vp]),
     "b2rl_serve_take": (C.c_int, [c_vp, c_i32, c_vp, c_vp]),
+    "b2rl_serve_bind": (C.c_int, [c_vp, C.POINTER(ServeLayout), c_i64, c_vp, c_vp, c_vp, C.POINTER(c_vp),
+                                  C.POINTER(c_vp), c_vp]),
     "b2rl_serve_put_update": (C.c_int, [c_vp, c_i32, c_u64, c_vp, c_vp, c_i64, c_vp]),
 }
 

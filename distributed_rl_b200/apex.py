@@ -26,6 +26,7 @@ from dataclasses import dataclass, field
 import numpy as np
 import torch
 
+from . import _lib
 from . import replay as R
 from .agent import GraphAgent
 from .learner_common import (Conv1Gathered as _Conv1Gathered, MemoryView, ReplayThread, TargetNetLearner, conv1_packs,
@@ -61,6 +62,8 @@ class ApexConfig:
     FUSED_DUELING_TAIL: bool = True  # heads' second layers + dueling combine in one kernel (csrc/dueling.cu)
     DENSE_3XTF32: bool = True       # dense heads as 3xTF32 wgmma GEMMs at fp32 accuracy (csrc/gemm.cu)
     BATCHED_ONLINE: bool = True     # the online net's two passes (s with grad, s' without) as ONE B = 2*BATCHSIZE call
+    SERVED_FUSED_STEP: bool = False  # on a served replay (DeviceReplayClient), run() steps the captured fused step on
+                                     # the bound ring slot instead of sample() -> train() -> update()
 
     @staticmethod
     def from_configuration():
@@ -206,14 +209,25 @@ class _StepState:
         self.max_w = SideBranch(packs)            # data parallel: the reduced max IS weight, for the next step
         self.head_packs = None                    # (online, target) heads' forward operands of this step
         self.resident = None                      # (online, target) heads' persistent operand images, or None
-        self.pack1 = self.pack2 = self.cur = self.y_big = self.sink = None
+        self.pack1 = self.pack2 = self.cur = self.y_big = self.sink = self.frames = None
         if not L._conv1_ready():
+            if L._served:
+                raise ValueError("SERVED_FUSED_STEP reads the ring slot's frames with the fused conv_1 kernels: the "
+                                 "model's first node must be the Atari conv_1")
             return
         # pack1: online net (grad pass on s); pack2: online + target in one pass over s'
         self.conv_name, self.pack1, self.pack2 = conv1_packs(L.model, dev, 1, 2)
-        self.cur = dict(L.memory.store.alloc_batch(B, ("action", "reward", "done")),
-                        idx=torch.empty(B, dtype=torch.int64, device=dev),
-                        w=torch.empty(B, dtype=torch.float32, device=dev))
+        idx_w = dict(idx=torch.empty(B, dtype=torch.int64, device=dev), w=torch.empty(B, dtype=torch.float32, device=dev))
+        if L._served:
+            # The draw is the server's.  Before each step, memory.acquire() binds a filled ring slot to these buffers
+            # (outside the graph): its header, idx, w, action, reward and done are copied in, and the two entries of
+            # `table` receive the addresses of its state / next_state rows, which conv_1 reads in place.
+            self.cur = dict(R.alloc_rows(R.APEX_FIELDS, B, dev, ("action", "reward", "done")), **idx_w,
+                            header=torch.zeros(2, dtype=torch.int64, device=dev))
+            self.table = torch.zeros(2, dtype=torch.int64, device=dev)
+            self.frames = {"state": R.BoundFrames(self.table, 0, B), "next_state": R.BoundFrames(self.table, 1, B)}
+        else:
+            self.cur = dict(L.memory.store.alloc_batch(B, ("action", "reward", "done")), **idx_w)
         if cfg.PARALLEL_FORWARDS and cfg.BATCHED_ONLINE:
             self.y_big = torch.empty((3, B, 20, 20, self.pack1.c_out), dtype=torch.float32, device=dev)
         if L._fused_optim:
@@ -255,8 +269,11 @@ class Learner(TargetNetLearner):
         """`memory`: a replay served from another process (replay_server.DeviceReplayClient, or anything with the
         `Replay` surface: sample / update / lock / memory).  run() then drives sample() -> train() -> update() with
         the reference's cadence (APE_X/Learner.py:163-197); without it the learner owns its replay and run() steps
-        with fused_step()."""
+        with fused_step().  With SERVED_FUSED_STEP, run() over a served memory steps fused_step() instead, on the
+        slot `memory.acquire()` binds (same cadence)."""
         self.cfg = cfg or ApexConfig.from_configuration()
+        if memory is not None and self.cfg.SERVED_FUSED_STEP:
+            self._check_served_fused(memory)
         self.device = torch.device(self.cfg.LEARNER_DEVICE)
         if self.cfg.CUDNN_BENCHMARK and self.device.type == "cuda":
             torch.backends.cudnn.benchmark = True
@@ -280,6 +297,7 @@ class Learner(TargetNetLearner):
         self.gamma_n = float(np.float32(0.99 ** self.cfg.UNROLL_STEP))  # hard-coded 0.99, :103
         self._graph = None
         self._fused = None              # _StepState, built by the first fused_step / _forward_backward_fused
+        self._bound_warm = 0            # eager warm-up steps _bound_step has run
         self._world = 1
         self.launches_per_step = None   # libb2rl kernels per fused step (bench.py's gpu_launches)
 
@@ -287,6 +305,9 @@ class Learner(TargetNetLearner):
         """Replay-sharded data parallelism (SURVEY.md §8e): every rank owns a replay shard and
         samples locally; per step one NCCL all-reduce (AVG) of the gradients, kept in ONE flat
         bucket so it is a single collective, and one MAX all-reduce of the max IS weight."""
+        if self._served and self.cfg.SERVED_FUSED_STEP:
+            raise ValueError("data parallelism samples every rank's own replay shard; a learner stepping served "
+                             "minibatches (SERVED_FUSED_STEP) has no shard")
         from . import dist as D
         self._D = D
         self._world = D.world()
@@ -429,7 +450,11 @@ class Learner(TargetNetLearner):
         `early_update`: the caller WILL call self.step() next; the heads' part of that optimizer step may then be
         issued here, behind their weight gradients on the sink's lane, while the conv stack's backward still runs."""
         s = self._fused_state()
-        st = self.memory.store
+        if self._served:        # the bound ring slot: its rows are the draws, in order
+            st, src_s, src_ns, rows = None, s.frames["state"], s.frames["next_state"], None
+        else:
+            st = self.memory.store
+            src_s, src_ns, rows = st.field_view("state"), st.field_view("next_state"), idx
         w_on = getattr(self.model, s.conv_name).conv_1.weight
         if not prepacked:
             self._pack_weights()
@@ -447,13 +472,13 @@ class Learner(TargetNetLearner):
                 # outputs (first B rows: views, no kernels) through the same forward code.  Q_target(s') runs
                 # beside it on a second stream.
                 from .linear import OutputTape
-                B, c_out = idx.numel(), s.pack1.c_out
+                B, c_out = weight.numel(), s.pack1.c_out
                 big = s.y_big          # [0] conv_1(s) online, [1] conv_1(s') online, [2] conv_1(s') target
                 if big.shape[1] != B:
                     raise ValueError(f"the batched online pass is sized for BATCHSIZE = {big.shape[1]}, got {B} rows")
                 with torch.no_grad():
-                    R.conv1_fused(st.field_view("state"), idx, s.pack1, relu=True, out=big[0:1])
-                    y_tg = R.conv1_fused(st.field_view("next_state"), idx, s.pack2, relu=True, out=big[1:3])[1]
+                    R.conv1_fused(src_s, rows, s.pack1, relu=True, out=big[0:1])
+                    y_tg = R.conv1_fused(src_ns, rows, s.pack2, relu=True, out=big[1:3])[1]
                 s.head_packs_built.join()      # long done; the heads' GEMM is ~100 us away
                 with torch.no_grad():
                     with s.target_pass.fork(), self.target_model.packed_heads_cache(tg_packs):
@@ -468,8 +493,7 @@ class Learner(TargetNetLearner):
                     with OutputTape.record() as tape:
                         q_all = self.model.forward_from_conv1(y_both, True)[0]          # :78 and :87 in one pass
                 qn_online = q_all[B:]
-                y = _Conv1Gathered.apply(w_on, st.field_view("state"), idx, s.pack1, self._mf, st,
-                                         big[0].permute(0, 3, 1, 2), True)
+                y = _Conv1Gathered.apply(w_on, src_s, rows, s.pack1, self._mf, st, big[0].permute(0, 3, 1, 2), True)
                 with OutputTape.replay(tape.half(B)):
                     q = self.model.forward_from_conv1(y, True)[0]                       # graph only: outputs replayed
             else:
@@ -478,14 +502,14 @@ class Learner(TargetNetLearner):
                 if not resident:
                     self.model.prepack_heads()
                 with torch.no_grad():
-                    y_on, y_tg = R.conv1_fused(st.field_view("next_state"), idx, s.pack2, relu=True)
+                    y_on, y_tg = R.conv1_fused(src_ns, rows, s.pack2, relu=True)
                     with s.side.fork():
                         qn_online = self.model.forward_from_conv1(y_on, True)[0]        # :87
                         if self.cfg.PARALLEL_FORWARDS and not resident:   # on one stream backward packs it beside its wgrad lanes
                             self.model.prepack_heads(transposed=True)   # W^T operand of the heads' dgrad, off the main branch
                     with s.target_pass.fork(), self.target_model.packed_heads_cache(tg_packs):
                         qn_target = self.target_model.forward_from_conv1(y_tg, True)[0]  # :85
-                y = _Conv1Gathered.apply(w_on, st.field_view("state"), idx, s.pack1, self._mf, st, None, True)
+                y = _Conv1Gathered.apply(w_on, src_s, rows, s.pack1, self._mf, st, None, True)
                 q = self.model.forward_from_conv1(y, True)[0]                        # :78 (ReLU in the conv_1 epilogue)
             s.side.join()
             s.target_pass.join()
@@ -517,12 +541,16 @@ class Learner(TargetNetLearner):
     # -- the whole hot loop iteration as one CUDA graph -----------------------------------
     def fused_step(self, use_graph: bool = True):
         """sample -> gather -> forwards -> target -> backward -> RMSprop -> priority
-        write-back (APE_X/Learner.py:165-197) with no host round trip."""
+        write-back (APE_X/Learner.py:165-197) with no host round trip.  On a served memory (SERVED_FUSED_STEP) the
+        same step on the slot the last `memory.acquire()` bound; see _bound_step."""
+        if self._served:
+            if not self.cfg.SERVED_FUSED_STEP:
+                raise RuntimeError("fused_step() samples the learner's own replay; a served replay is driven by run() "
+                                   "(or set SERVED_FUSED_STEP)")
+            return self._bound_step(use_graph)
         if self._graph is not None:
             self._graph.replay()
             return self._static
-        if self._served:
-            raise RuntimeError("fused_step() samples the learner's own replay; a served replay is driven by run()")
         B = self.cfg.BATCHSIZE
         st = self.memory.store
         s = self._fused_state()
@@ -601,6 +629,54 @@ class Learner(TargetNetLearner):
         g.replay()
         return self._static
 
+    BOUND_WARMUP = 3       # eager steps on served minibatches before the bound step is captured
+
+    def _bound_step(self, use_graph: bool = True):
+        """One step on the served minibatch `memory.acquire(cur, frames)` bound: fused_step's graph, with the draw
+        (sample_fetch) and the in-graph tree update replaced by reads of the bound buffers; the priorities leave
+        through memory.update() after the step.  The first BOUND_WARMUP calls run the step eagerly on the main stream
+        (lazy inits stay outside the capture), each on its own minibatch; the next call captures the graph, and every
+        call replays it.  The caller releases the slot after this returns: the replay is then enqueued."""
+        s = self._fused_state()
+        if self._graph is not None:
+            self._graph.replay()
+            return self._static
+        c = s.cur
+        batched = self.cfg.PARALLEL_FORWARDS and self.cfg.BATCHED_ONLINE   # the batched pass converts the action
+
+        def body():
+            self._pack_weights()
+            out = self._forward_backward_fused(c["idx"], c["action"] if batched else c["action"].to(torch.int64),
+                                               c["reward"], c["done"], c["w"], prepacked=True, early_update=True)
+            info = self.step()
+            return {"scalars": out["scalars"], "p_norm": info["p_norm"], "prio": out["prio"], "idx": c["idx"]}
+
+        lib = _lib.load()
+        if not use_graph:
+            c0 = lib.b2rl_launch_count()
+            r = body()
+            self.launches_per_step = lib.b2rl_launch_count() - c0
+            return r
+        cur = torch.cuda.current_stream(self.device)
+        if self._bound_warm < self.BOUND_WARMUP:
+            if self._bound_warm == 0:
+                self.optim.zero_grad(set_to_none=False)
+            self._bound_warm += 1
+            s.main.wait_stream(cur)
+            with torch.cuda.stream(s.main):
+                r = body()
+            cur.wait_stream(s.main)
+            return r
+        torch.cuda.synchronize(self.device)
+        g = torch.cuda.CUDAGraph()
+        c0 = lib.b2rl_launch_count()
+        with torch.cuda.graph(g, stream=s.main):
+            self._static = body()
+        self.launches_per_step = lib.b2rl_launch_count() - c0
+        self._graph = g
+        g.replay()
+        return self._static
+
     # -- main loop ---------------------------------------------------------------------------------
     def run(self, max_steps: int | None = None, log_every: int = 500):
         """Learner.run (:140-262) with the reference's cadence: wait for BUFFER_SIZE records, announce `Start`,
@@ -645,6 +721,8 @@ class Learner(TargetNetLearner):
         """One iteration of the reference loop over a served replay (APE_X/Learner.py:163-197): sample, train, the
         eviction request every `log_every` steps (that step's write-back is skipped, as there), write-back.
         -> {loss, mean(y), mean(w), norm} as a device tensor, or None when no minibatch is ready."""
+        if self.cfg.SERVED_FUSED_STEP:
+            return self._served_fused_step(step, log_every)
         batch = self.memory.sample()
         if batch is False:
             return None
@@ -654,3 +732,31 @@ class Learner(TargetNetLearner):
         if self.memory.lock is False:
             self.memory.update(idx, prio)
         return torch.stack([info["loss"], info["mean_value"], mean_w, info["p_norm"].reshape(())])
+
+    def _served_fused_step(self, step: int, log_every: int):
+        """_served_step on the captured step: bind the oldest filled slot (memory.acquire), step on it, hand the slot
+        back once the step is enqueued (memory.release: conv_1's weight gradient, in backward, is its last reader),
+        then the eviction request every `log_every` steps (that step's write-back is skipped) or the write-back.
+        -> {loss, mean(y), mean(w), norm} as a device tensor, or None when no minibatch is ready."""
+        s = self._fused_state()
+        if self.memory.acquire(s.cur, s.frames) is None:
+            return None
+        out = self.fused_step()
+        self.memory.release()
+        if step % log_every == 0:
+            self.memory.lock = True
+        if self.memory.lock is False:
+            self.memory.update(out["idx"], out["prio"])
+        return torch.cat([out["scalars"], out["p_norm"].reshape(1)])
+
+    def _check_served_fused(self, memory) -> None:
+        """What SERVED_FUSED_STEP needs, checked before anything is built."""
+        if not self.cfg.FUSED_CONV1:
+            raise ValueError("SERVED_FUSED_STEP reads the frames in the ring slot with the fused conv_1 kernels: it "
+                             "needs FUSED_CONV1")
+        if not (hasattr(memory, "acquire") and hasattr(memory, "release")):
+            raise TypeError("SERVED_FUSED_STEP needs a served memory that binds ring slots (DeviceReplayClient)")
+        batch = memory.ring.layout.batch
+        if batch != self.cfg.BATCHSIZE:
+            raise ValueError(f"the server's ring holds minibatches of {batch}; the step graph is built for "
+                             f"BATCHSIZE = {self.cfg.BATCHSIZE}")

@@ -112,6 +112,15 @@ struct Params {
   int relu;
 };
 
+// The table variant: the frame base is read from device memory when the kernel starts (`frames` is unused), so a
+// captured launch follows whatever b2rl_serve_bind last wrote into the entry (the ring slot of this step).
+struct TableParams : Params {
+  const uint8_t* const* table;   // one entry: the field base
+};
+
+__device__ __forceinline__ const uint8_t* frame_base(const Params& P) { return P.frames; }
+__device__ __forceinline__ const uint8_t* frame_base(const TableParams& P) { return *P.table; }
+
 template <int N> struct Acc;
 template <> struct Acc<128> {
   int32_t d[64];
@@ -122,9 +131,9 @@ template <> struct Acc<64> {
   __device__ __forceinline__ void mma(uint64_t a, uint64_t b, uint32_t acc) { mma_u8s8_n64(d, a, b, acc); }
 };
 
-template <int N_NETS, int C_OUT>
+template <int N_NETS, int C_OUT, class PARAMS = Params>
 __global__ void __launch_bounds__(THREADS, 1)
-k_conv1_fused(const __grid_constant__ Params P) {
+k_conv1_fused(const __grid_constant__ PARAMS P) {
   constexpr int N_PER_NET = NSPLIT * C_OUT;            // MMA columns per network: 128 (64 for 16 channels)
   constexpr int N_TOTAL = N_NETS * N_PER_NET;          // rows of the packed weights: 64 .. 256
   constexpr int B_BYTES = N_TOTAL * K_TOTAL;           // 16 .. 64 KiB
@@ -155,6 +164,7 @@ k_conv1_fused(const __grid_constant__ Params P) {
   if (warp == (CONSUMERS + PRODUCERS) / 32) {
     // ------------------------------ TMA loader ------------------------------
     if (lane == 0) {
+      const uint8_t* frames = frame_base(P);
       mbar_expect_tx(&b_full, B_BYTES);
       constexpr int LOAD_CHUNK = (B_BYTES < 32768) ? B_BYTES : 32768;
       for (int off = 0; off < B_BYTES; off += LOAD_CHUNK) bulk_g2s(sB + off, P.bq + off, LOAD_CHUNK, &b_full);
@@ -165,7 +175,7 @@ k_conv1_fused(const __grid_constant__ Params P) {
         int64_t row = P.idx ? P.idx[k] : k;
         row = row < 0 ? 0 : (row >= P.capacity ? P.capacity - 1 : row);
         mbar_expect_tx(&raw_full[s], FRAME_BYTES);
-        bulk_g2s(sRaw + s * RAW_STRIDE, P.frames + row * FRAME_BYTES, FRAME_BYTES, &raw_full[s]);
+        bulk_g2s(sRaw + s * RAW_STRIDE, frames + row * FRAME_BYTES, FRAME_BYTES, &raw_full[s]);
       }
     }
   } else if (warp >= CONSUMERS / 32) {
@@ -315,34 +325,33 @@ extern "C" int b2rl_conv1_pack_jobs(const float* const* w_dev, const int32_t* ne
   return B2RL_OK;
 }
 
-template <int N_NETS, int C_OUT>
-static cudaError_t conv1_launch(const conv1::Params& P, unsigned grid, cudaStream_t st) {
+template <int N_NETS, int C_OUT, class PARAMS>
+static cudaError_t conv1_launch(const PARAMS& P, unsigned grid, cudaStream_t st) {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e == cudaSuccess)
-    e = set_max_dynamic_smem<conv1::k_conv1_fused<N_NETS, C_OUT>>(dev, conv1::smem_bytes<N_NETS, C_OUT>());
+    e = set_max_dynamic_smem<conv1::k_conv1_fused<N_NETS, C_OUT, PARAMS>>(dev, conv1::smem_bytes<N_NETS, C_OUT>());
   if (e != cudaSuccess) return e;
-  conv1::k_conv1_fused<N_NETS, C_OUT><<<grid, conv1::THREADS, conv1::smem_bytes<N_NETS, C_OUT>(), st>>>(P);
+  conv1::k_conv1_fused<N_NETS, C_OUT, PARAMS><<<grid, conv1::THREADS, conv1::smem_bytes<N_NETS, C_OUT>(), st>>>(P);
   return cudaSuccess;
 }
 
-extern "C" int b2rl_conv1_fused(const uint8_t* frames_dev, int64_t capacity, const int64_t* idx_dev, int64_t n,
-                                const int8_t* bq_dev, const float* scale_dev, int32_t n_nets, int32_t c_out,
-                                float* out_dev, int32_t relu, void* stream) {
-  B2RL_REQUIRE(n >= 0, "negative n");
-  if (n == 0) return B2RL_OK;
-  B2RL_REQUIRE(frames_dev && bq_dev && scale_dev && out_dev, "null argument");
+// What b2rl_conv1_fused and b2rl_conv1_fused_table share once their frame source is checked.
+template <class PARAMS>
+static int conv1_fused_run(PARAMS& P, const int8_t* bq_dev, const float* scale_dev, int32_t n_nets, int32_t c_out,
+                           float* out_dev, void* stream) {
+  B2RL_REQUIRE(bq_dev && scale_dev && out_dev, "null argument");
   B2RL_REQUIRE(n_nets == 1 || n_nets == 2, "n_nets must be 1 or 2");
   B2RL_REQUIRE(c_out == 16 || c_out == 32, "c_out must be 16 or 32");
-  B2RL_REQUIRE(capacity >= 1, "capacity must be positive");
-  B2RL_REQUIRE(((uintptr_t)frames_dev % 16 == 0) && ((uintptr_t)bq_dev % 16 == 0) && ((uintptr_t)out_dev % 16 == 0),
+  B2RL_REQUIRE(P.capacity >= 1, "capacity must be positive");
+  B2RL_REQUIRE(((uintptr_t)bq_dev % 16 == 0) && ((uintptr_t)out_dev % 16 == 0),
                "frames, packed weights and output must be 16-byte aligned");
   int dev = 0;
   B2RL_CUDA(cudaGetDevice(&dev));
   int sms = 0;
   B2RL_CUDA(sm_count(dev, &sms));
-  conv1::Params P{frames_dev, idx_dev, n, capacity, bq_dev, scale_dev, out_dev, relu};
-  const int64_t units = n * conv1::TILES;
+  P.bq = bq_dev, P.scale = scale_dev, P.out = out_dev;
+  const int64_t units = P.n * conv1::TILES;
   const unsigned grid = (unsigned)((units < sms) ? units : sms);
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e;
@@ -352,4 +361,27 @@ extern "C" int b2rl_conv1_fused(const uint8_t* frames_dev, int64_t capacity, con
   count_launch();
   B2RL_CHECK_LAUNCH();
   return B2RL_OK;
+}
+
+extern "C" int b2rl_conv1_fused(const uint8_t* frames_dev, int64_t capacity, const int64_t* idx_dev, int64_t n,
+                                const int8_t* bq_dev, const float* scale_dev, int32_t n_nets, int32_t c_out,
+                                float* out_dev, int32_t relu, void* stream) {
+  B2RL_REQUIRE(n >= 0, "negative n");
+  if (n == 0) return B2RL_OK;
+  B2RL_REQUIRE(frames_dev, "null argument");
+  B2RL_REQUIRE((uintptr_t)frames_dev % 16 == 0, "frames, packed weights and output must be 16-byte aligned");
+  conv1::Params P{frames_dev, idx_dev, n, capacity, nullptr, nullptr, nullptr, relu};
+  return conv1_fused_run(P, bq_dev, scale_dev, n_nets, c_out, out_dev, stream);
+}
+
+extern "C" int b2rl_conv1_fused_table(const uint8_t* const* frame_table_dev, int64_t capacity, const int64_t* idx_dev,
+                                      int64_t n, const int8_t* bq_dev, const float* scale_dev, int32_t n_nets,
+                                      int32_t c_out, float* out_dev, int32_t relu, void* stream) {
+  B2RL_REQUIRE(n >= 0, "negative n");
+  B2RL_REQUIRE(frame_table_dev != nullptr, "null frame table");
+  B2RL_REQUIRE((uintptr_t)frame_table_dev % 8 == 0, "a frame table entry must be 8-byte aligned");
+  if (n == 0) return B2RL_OK;
+  conv1::TableParams P{};
+  P.idx = idx_dev, P.n = n, P.capacity = capacity, P.relu = relu, P.table = frame_table_dev;
+  return conv1_fused_run(P, bq_dev, scale_dev, n_nets, c_out, out_dev, stream);
 }

@@ -60,6 +60,16 @@ struct Params {
   float* partial;            // [gridDim.x][C_OUT][256]
 };
 
+// The table variant (b2rl_conv1_wgrad_table): the frame base is read from device memory when the kernel starts and
+// advanced by frame_off bytes there (`frames` is unused), so a captured launch follows the entry b2rl_serve_bind wrote.
+struct TableParams : Params {
+  const uint8_t* const* table;
+  int64_t frame_off;         // rows of the earlier launches of a split n (idx == nullptr), in bytes
+};
+
+__device__ __forceinline__ const uint8_t* frame_base(const Params& P) { return P.frames; }
+__device__ __forceinline__ const uint8_t* frame_base(const TableParams& P) { return *P.table + P.frame_off; }
+
 template <int N> struct Acc;
 template <> struct Acc<128> {
   int32_t d[64];
@@ -77,9 +87,9 @@ __device__ __forceinline__ int digit_exponent(uint32_t absmax_bits) {
   return e < 27 ? 27 : (e > 227 ? 227 : e);
 }
 
-template <int C_OUT>
+template <int C_OUT, class PARAMS = Params>
 __global__ void __launch_bounds__(THREADS, 1)
-k_conv1_wgrad(const __grid_constant__ Params P) {
+k_conv1_wgrad(const __grid_constant__ PARAMS P) {
   constexpr int N_TOTAL = NSPLIT * C_OUT;              // 128 (64 for 16 channels)
   constexpr int B_BYTES = N_TOTAL * KCHUNK;
   constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
@@ -101,6 +111,7 @@ k_conv1_wgrad(const __grid_constant__ Params P) {
   }
   __syncthreads();
   const int64_t first = blockIdx.x, stride = gridDim.x;
+  const uint8_t* frames = frame_base(P);
 
   // frame stack `it` of this CTA -> raw buffer it & 1
   auto load_frame = [&](int64_t it) {
@@ -109,7 +120,7 @@ k_conv1_wgrad(const __grid_constant__ Params P) {
     int64_t row = P.idx ? P.idx[k] : k;
     row = row < 0 ? 0 : (row >= P.capacity ? P.capacity - 1 : row);
     mbar_expect_tx(&raw_full[it & 1], FRAME_BYTES);
-    bulk_g2s(sRaw + (it & 1) * RAW_STRIDE, P.frames + row * FRAME_BYTES, FRAME_BYTES, &raw_full[it & 1]);
+    bulk_g2s(sRaw + (it & 1) * RAW_STRIDE, frames + row * FRAME_BYTES, FRAME_BYTES, &raw_full[it & 1]);
   };
   if (threadIdx.x == 0) load_frame(0);
 
@@ -334,13 +345,14 @@ constexpr size_t smem_bytes() {
 
 using namespace b2rl;
 
-template <int C_OUT>
-static cudaError_t wgrad_launch(const conv1w::Params& P, unsigned grid, cudaStream_t st) {
+template <int C_OUT, class PARAMS>
+static cudaError_t wgrad_launch(const PARAMS& P, unsigned grid, cudaStream_t st) {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
-  if (e == cudaSuccess) e = set_max_dynamic_smem<conv1w::k_conv1_wgrad<C_OUT>>(dev, conv1w::smem_bytes<C_OUT>());
+  if (e == cudaSuccess)
+    e = set_max_dynamic_smem<conv1w::k_conv1_wgrad<C_OUT, PARAMS>>(dev, conv1w::smem_bytes<C_OUT>());
   if (e != cudaSuccess) return e;
-  conv1w::k_conv1_wgrad<C_OUT><<<grid, conv1w::THREADS, conv1w::smem_bytes<C_OUT>(), st>>>(P);
+  conv1w::k_conv1_wgrad<C_OUT, PARAMS><<<grid, conv1w::THREADS, conv1w::smem_bytes<C_OUT>(), st>>>(P);
   return cudaSuccess;
 }
 
@@ -351,14 +363,15 @@ extern "C" int64_t b2rl_conv1_wgrad_workspace_floats(int32_t c_out) {
   return (int64_t)sms * c_out * conv1w::E_TOTAL;
 }
 
-extern "C" int b2rl_conv1_wgrad(const uint8_t* frames_dev, int64_t capacity, const int64_t* idx_dev, int64_t n,
-                                const float* gy_dev, const float* y_relu_dev, int32_t c_out, float* workspace_dev,
-                                float* gw_dev, int32_t accumulate, void* stream) {
-  B2RL_REQUIRE(n >= 1, "n must be positive");
-  B2RL_REQUIRE(frames_dev && gy_dev && workspace_dev && gw_dev, "null argument");
+// The launches of b2rl_conv1_wgrad and b2rl_conv1_wgrad_table.  `frames_dev` null: the frame base is the table entry
+// (read on the device, where the offset of each launch of a split n is added).
+static int wgrad_run(const uint8_t* frames_dev, const uint8_t* const* table_dev, int64_t capacity,
+                     const int64_t* idx_dev, int64_t n, const float* gy_dev, const float* y_relu_dev, int32_t c_out,
+                     float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream) {
+  B2RL_REQUIRE(gy_dev && workspace_dev && gw_dev, "null argument");
   B2RL_REQUIRE(c_out == 16 || c_out == 32, "c_out must be 16 or 32");
   B2RL_REQUIRE(capacity >= 1, "capacity must be positive");
-  B2RL_REQUIRE(((uintptr_t)frames_dev % 16 == 0) && ((uintptr_t)gy_dev % 16 == 0) && ((uintptr_t)y_relu_dev % 16 == 0),
+  B2RL_REQUIRE(((uintptr_t)gy_dev % 16 == 0) && ((uintptr_t)y_relu_dev % 16 == 0),
                "frames, gy and y must be 16-byte aligned");
   int dev = 0;
   B2RL_CUDA(cudaGetDevice(&dev));
@@ -372,9 +385,18 @@ extern "C" int b2rl_conv1_wgrad(const uint8_t* frames_dev, int64_t capacity, con
     conv1w::Params P{frames_dev, idx_dev ? idx_dev + off : nullptr, m, capacity,
                      gy_dev + off * (int64_t)(conv1w::POS * c_out),
                      y_relu_dev ? y_relu_dev + off * (int64_t)(conv1w::POS * c_out) : nullptr, workspace_dev};
-    if (!idx_dev) P.frames = frames_dev + off * conv1w::FRAME_BYTES, P.capacity = capacity - off;
+    const int64_t frame_off = idx_dev ? 0 : off * conv1w::FRAME_BYTES;
+    if (!idx_dev) P.capacity = capacity - off;
     const unsigned grid = (unsigned)((m < sms) ? m : sms);
-    B2RL_CUDA(c_out == 32 ? wgrad_launch<32>(P, grid, st) : wgrad_launch<16>(P, grid, st));
+    if (frames_dev) {
+      P.frames = frames_dev + frame_off;
+      B2RL_CUDA(c_out == 32 ? wgrad_launch<32>(P, grid, st) : wgrad_launch<16>(P, grid, st));
+    } else {
+      conv1w::TableParams T{};
+      static_cast<conv1w::Params&>(T) = P;
+      T.frames = nullptr, T.table = table_dev, T.frame_off = frame_off;
+      B2RL_CUDA(c_out == 32 ? wgrad_launch<32>(T, grid, st) : wgrad_launch<16>(T, grid, st));
+    }
     count_launch();
     B2RL_CHECK_LAUNCH();
     conv1w::k_conv1_wgrad_reduce<<<(numel + 31) / 32, dim3(32, conv1w::RED_SLICES), 0, st>>>(
@@ -383,4 +405,24 @@ extern "C" int b2rl_conv1_wgrad(const uint8_t* frames_dev, int64_t capacity, con
     B2RL_CHECK_LAUNCH();
   }
   return B2RL_OK;
+}
+
+extern "C" int b2rl_conv1_wgrad(const uint8_t* frames_dev, int64_t capacity, const int64_t* idx_dev, int64_t n,
+                                const float* gy_dev, const float* y_relu_dev, int32_t c_out, float* workspace_dev,
+                                float* gw_dev, int32_t accumulate, void* stream) {
+  B2RL_REQUIRE(n >= 1, "n must be positive");
+  B2RL_REQUIRE(frames_dev, "null argument");
+  B2RL_REQUIRE((uintptr_t)frames_dev % 16 == 0, "frames, gy and y must be 16-byte aligned");
+  return wgrad_run(frames_dev, nullptr, capacity, idx_dev, n, gy_dev, y_relu_dev, c_out, workspace_dev, gw_dev,
+                   accumulate, stream);
+}
+
+extern "C" int b2rl_conv1_wgrad_table(const uint8_t* const* frame_table_dev, int64_t capacity, const int64_t* idx_dev,
+                                      int64_t n, const float* gy_dev, const float* y_relu_dev, int32_t c_out,
+                                      float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream) {
+  B2RL_REQUIRE(n >= 1, "n must be positive");
+  B2RL_REQUIRE(frame_table_dev != nullptr, "null frame table");
+  B2RL_REQUIRE((uintptr_t)frame_table_dev % 8 == 0, "a frame table entry must be 8-byte aligned");
+  return wgrad_run(nullptr, frame_table_dev, capacity, idx_dev, n, gy_dev, y_relu_dev, c_out, workspace_dev, gw_dev,
+                   accumulate, stream);
 }

@@ -175,6 +175,34 @@ k_serve_put_update(uint64_t* __restrict__ header, int64_t* __restrict__ idx_dst,
   }
 }
 
+// k_serve_bind: hand a filled minibatch slot to a captured learner step.  The step's graph reads fixed buffers and a
+// frame table; the bind copies the slot's small arrays into those buffers (CTA j copies job j) and writes the device
+// addresses of the frame fields' rows into the table entries (CTA 0), so conv_1 reads the frames in the slot itself.
+struct BindCopy {
+  const uint8_t* src;
+  uint8_t* dst;
+  int64_t bytes;
+};
+struct BindJobs {
+  BindCopy copy[3 + B2RL_MAX_FIELDS];         // header, idx, w, then the copied fields
+  const uint8_t* addr[B2RL_MAX_FIELDS];       // rows of a frame field ...
+  const uint8_t** entry[B2RL_MAX_FIELDS];     // ... and the table entry that receives their address
+  int32_t n_entries;
+};
+
+__global__ void __launch_bounds__(256)
+k_serve_bind(const __grid_constant__ BindJobs J) {
+  if (blockIdx.x == 0 && threadIdx.x < J.n_entries) *J.entry[threadIdx.x] = J.addr[threadIdx.x];
+  const BindCopy c = J.copy[blockIdx.x];
+  if ((((uintptr_t)c.src | (uintptr_t)c.dst | (uintptr_t)c.bytes) & 15) == 0) {
+    const uint4* s = reinterpret_cast<const uint4*>(c.src);
+    uint4* d = reinterpret_cast<uint4*>(c.dst);
+    for (int64_t i = threadIdx.x; i < c.bytes / 16; i += blockDim.x) d[i] = s[i];
+  } else {
+    for (int64_t i = threadIdx.x; i < c.bytes; i += blockDim.x) c.dst[i] = c.src[i];
+  }
+}
+
 }  // namespace b2rl
 
 using namespace b2rl;
@@ -452,6 +480,38 @@ extern "C" int b2rl_serve_take(const b2rl_serve_ring* r, int32_t slot, void* dst
   DeviceGuard g(r->device);
   B2RL_CUDA(cudaMemcpyAsync(dst_dev, r->base + (int64_t)slot * r->L.slot_bytes, (size_t)r->L.slot_bytes,
                             cudaMemcpyDefault, (cudaStream_t)stream));
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_serve_bind(const void* slot_dev, const b2rl_serve_layout* layout, int64_t n,
+                               uint64_t* header_out_dev, int64_t* idx_out_dev, float* w_out_dev,
+                               void* const* fields_out_dev, void* const* table_out_dev, void* stream) {
+  B2RL_REQUIRE(slot_dev != nullptr, "null slot");
+  B2RL_REQUIRE(layout != nullptr, "null layout");
+  B2RL_REQUIRE((uintptr_t)slot_dev % 16 == 0, "the slot base must be 16-byte aligned");
+  B2RL_REQUIRE(layout->n_fields >= 0 && layout->n_fields <= B2RL_MAX_FIELDS, "n_fields out of range");
+  B2RL_REQUIRE(layout->batch == n, "the slot's batch does not match n");
+  B2RL_REQUIRE(header_out_dev && idx_out_dev && w_out_dev, "null header, idx or w buffer");
+  const uint8_t* s = (const uint8_t*)slot_dev;
+  BindJobs J{};
+  int jobs = 0;
+  J.copy[jobs++] = BindCopy{s, (uint8_t*)header_out_dev, 16};
+  J.copy[jobs++] = BindCopy{s + layout->idx_off, (uint8_t*)idx_out_dev, 8 * n};
+  J.copy[jobs++] = BindCopy{s + layout->w_off, (uint8_t*)w_out_dev, 4 * n};
+  for (int f = 0; f < layout->n_fields; ++f) {
+    void* field_out = fields_out_dev ? fields_out_dev[f] : nullptr;
+    void* entry = table_out_dev ? table_out_dev[f] : nullptr;
+    B2RL_REQUIRE(!(field_out && entry), "a field is either copied or bound in the frame table, not both");
+    if (field_out) J.copy[jobs++] = BindCopy{s + layout->field_off[f], (uint8_t*)field_out, layout->field_bytes[f] * n};
+    if (entry) {
+      B2RL_REQUIRE((uintptr_t)entry % 8 == 0, "a frame table entry must be 8-byte aligned");
+      J.addr[J.n_entries] = s + layout->field_off[f];
+      J.entry[J.n_entries++] = (const uint8_t**)entry;
+    }
+  }
+  k_serve_bind<<<jobs, 256, 0, (cudaStream_t)stream>>>(J);
+  count_launch();
+  B2RL_CHECK_LAUNCH();
   return B2RL_OK;
 }
 

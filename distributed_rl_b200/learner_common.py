@@ -128,7 +128,8 @@ class ReplayThread(Stoppable, threading.Thread):
 
 # -- conv_1 on libb2rl's kernels -----------------------------------------------------------------
 class Conv1Gathered(torch.autograd.Function):
-    """conv_1 over rows `idx` of a uint8 frame table (a replay field or an explicit batch).
+    """conv_1 over rows `idx` of a uint8 frame table (a replay field, an explicit batch, or a served ring slot bound
+    through a device-resident table entry, R.BoundFrames: backward then reads the same slot rows).
     Forward: fused gather+conv on the tensor cores (or a precomputed output of the same kernel).
     Backward: only dL/dW is needed (the input is data); cuDNN computes it from a gathered fp32
     copy of the same rows — the one place the sampled frames are staged — or, with `fused_wgrad`
@@ -169,6 +170,9 @@ class Conv1Gathered(torch.autograd.Function):
                 return (None,) * len(ctx.needs_input_grad)
             gw = R.conv1_wgrad(ctx.frames, idx if ctx.has_idx else None, gy, relu_y=y)
             return (gw,) + (None,) * (len(ctx.needs_input_grad) - 1)
+        if isinstance(ctx.frames, R.BoundFrames):
+            raise RuntimeError("conv_1 over a bound ring slot has no cuDNN weight gradient: set "
+                               "Conv1Gathered.fused_wgrad")
         if y is not None:
             gy = gy * (y > 0)
         if not ctx.has_idx:

@@ -84,6 +84,13 @@ _TYPESTR = {torch.uint8: "|u1", torch.int32: "<i4", torch.int64: "<i8", torch.fl
             torch.float64: "<f8", torch.int8: "|i1", torch.int16: "<i2", torch.float16: "<f2"}
 
 
+def alloc_rows(fields: Sequence[Field], n: int, device, names: Sequence[str] | None = None) -> dict:
+    """n uninitialised rows of each named field (all when `names` is None), with the field's dtype and shape."""
+    names = [f.name for f in fields] if names is None else list(names)
+    return {f.name: torch.empty((n,) + tuple(f.shape), dtype=f.dtype, device=device)
+            for f in fields if f.name in names}
+
+
 class DeviceReplay:
     def __init__(self, capacity: int, fields: Sequence[Field] = APEX_FIELDS, device="cuda:0"):
         self.lib = _lib.load()
@@ -330,9 +337,7 @@ class DeviceReplay:
 
     # -- gather ----------------------------------------------------------------
     def alloc_batch(self, n: int, names: Sequence[str] | None = None):
-        names = [f.name for f in self.fields] if names is None else list(names)
-        return {f.name: torch.empty((n,) + tuple(f.shape), dtype=f.dtype, device=self.device)
-                for f in self.fields if f.name in names}
+        return alloc_rows(self.fields, n, self.device, names)
 
     def gather(self, idx: torch.Tensor, out: dict | None = None) -> dict:
         n = idx.numel()
@@ -437,33 +442,59 @@ def conv1_pack_jobs(jobs) -> None:
         arr(*[p.scale.data_ptr() for p, _, _ in jobs]), n, c_out, _stream_ptr(jobs[0][0].device)))
 
 
-def conv1_fused(frames: torch.Tensor, idx, pack: Conv1Pack, relu: bool = False, out=None):
-    """frames: uint8 (rows, 4, 84, 84) contiguous (e.g. DeviceReplay.field_view("state"));
+@dataclass(frozen=True)
+class BoundFrames:
+    """A frame source whose base address lives in device memory: entry `entry` of the int64 `table` holds the
+    address of `rows` frame stacks (b2rl_serve_bind writes it when a served minibatch slot is bound).  conv1_fused /
+    conv1_wgrad read the entry when their kernels start, so a CUDA graph that captured them follows every rebind."""
+    table: torch.Tensor
+    entry: int
+    rows: int
+
+    @property
+    def device(self) -> torch.device:
+        return self.table.device
+
+    def entry_ptr(self) -> int:
+        assert self.table.dtype == torch.int64 and self.table.is_contiguous() and 0 <= self.entry < self.table.numel()
+        return self.table.data_ptr() + 8 * self.entry
+
+
+def _frame_source(frames):
+    """-> (rows, the frames' pointer or the table entry's, whether it is a table entry)."""
+    if isinstance(frames, BoundFrames):
+        return frames.rows, frames.entry_ptr(), True
+    assert frames.dtype == torch.uint8 and frames.is_contiguous() and frames[0].numel() == FRAME_STACK_BYTES
+    return frames.shape[0], frames.data_ptr(), False
+
+
+def conv1_fused(frames, idx, pack: Conv1Pack, relu: bool = False, out=None):
+    """frames: uint8 (rows, 4, 84, 84) contiguous (e.g. DeviceReplay.field_view("state")), or a BoundFrames;
     idx: int64[n] rows to take (None: all rows in order).
     -> list of n_nets tensors (n, c_out, 20, 20) fp32 in channels_last memory format."""
-    assert frames.dtype == torch.uint8 and frames.is_contiguous() and frames[0].numel() == FRAME_STACK_BYTES
-    n = frames.shape[0] if idx is None else idx.numel()
+    rows, ptr, table = _frame_source(frames)
+    n = rows if idx is None else idx.numel()
     dev = frames.device
     if out is None:
         out = torch.empty((pack.n_nets, n, 20, 20, pack.c_out), dtype=torch.float32, device=dev)
-    check(_lib.load().b2rl_conv1_fused(frames.data_ptr(), frames.shape[0], None if idx is None else idx.data_ptr(),
-                                       n, pack.bq.data_ptr(), pack.scale.data_ptr(), pack.n_nets, pack.c_out,
-                                       out.data_ptr(),
-                                       int(bool(relu)), _stream_ptr(dev)))
+    lib = _lib.load()
+    check((lib.b2rl_conv1_fused_table if table else lib.b2rl_conv1_fused)(
+        ptr, rows, None if idx is None else idx.data_ptr(), n, pack.bq.data_ptr(), pack.scale.data_ptr(), pack.n_nets,
+        pack.c_out, out.data_ptr(), int(bool(relu)), _stream_ptr(dev)))
     return [out[i].permute(0, 3, 1, 2) for i in range(pack.n_nets)]   # logical NCHW, physical NHWC
 
 
 _wgrad_ws = {}
 
 
-def conv1_wgrad(frames: torch.Tensor, idx, gy: torch.Tensor, out: torch.Tensor | None = None,
+def conv1_wgrad(frames, idx, gy: torch.Tensor, out: torch.Tensor | None = None,
                 accumulate: bool = False, relu_y: torch.Tensor | None = None) -> torch.Tensor:
     """dL/dW of conv_1 from the sampled uint8 rows and dL/dy, without staging the rows (b2rl_conv1_wgrad).
-    frames: uint8 (rows, 4, 84, 84) contiguous; idx: int64[n] or None; gy: (n, c_out, 20, 20) fp32
+    frames: uint8 (rows, 4, 84, 84) contiguous, or a BoundFrames; idx: int64[n] or None; gy: (n, c_out, 20, 20) fp32
     (made channels_last if it is not) -> (c_out, 4, 8, 8) fp32.  relu_y: the post-ReLU output of
     conv1_fused(relu=True) for the same rows; gy is then dL/d(relu output) and is masked by (y > 0) in the kernel."""
-    assert frames.dtype == torch.uint8 and frames.is_contiguous() and frames[0].numel() == FRAME_STACK_BYTES
-    n = frames.shape[0] if idx is None else idx.numel()
+    rows, ptr, table = _frame_source(frames)
+    n = rows if idx is None else idx.numel()
     c_out = gy.shape[1]
     assert gy.shape == (n, c_out, 20, 20) and gy.dtype == torch.float32
     gy = gy.contiguous(memory_format=torch.channels_last)
@@ -479,7 +510,9 @@ def conv1_wgrad(frames: torch.Tensor, idx, gy: torch.Tensor, out: torch.Tensor |
         out = torch.empty((c_out, 4, 8, 8), dtype=torch.float32, device=dev)
         accumulate = False
     assert out.is_contiguous() and out.numel() == c_out * 256
-    check(_lib.load().b2rl_conv1_wgrad(frames.data_ptr(), frames.shape[0], None if idx is None else idx.data_ptr(), n,
-                                       gy.data_ptr(), None if relu_y is None else relu_y.data_ptr(), c_out,
-                                       _wgrad_ws[key].data_ptr(), out.data_ptr(), int(bool(accumulate)), _stream_ptr(dev)))
+    lib = _lib.load()
+    check((lib.b2rl_conv1_wgrad_table if table else lib.b2rl_conv1_wgrad)(
+        ptr, rows, None if idx is None else idx.data_ptr(), n, gy.data_ptr(),
+        None if relu_y is None else relu_y.data_ptr(), c_out, _wgrad_ws[key].data_ptr(), out.data_ptr(),
+        int(bool(accumulate)), _stream_ptr(dev)))
     return out

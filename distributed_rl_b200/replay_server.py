@@ -347,6 +347,23 @@ class ServeRing:
         assert dst.is_contiguous() and dst.numel() * dst.element_size() >= self.layout.slot_bytes
         check(self.lib.b2rl_serve_take(self._h, int(k), dst.data_ptr(), stream.cuda_stream))
 
+    def bind(self, base: int, fields, out: dict, frames: dict, stream) -> None:
+        """b2rl_serve_bind: the filled slot at device address `base` (a mapped slot or a local copy of one) -> the
+        step's fixed buffers: out["header"] (int64[2]), out["idx"], out["w"] and every field named in `out` are
+        copied; every field named in `frames` (name -> R.BoundFrames) gets the address of its rows in the slot."""
+        L = self.layout
+        fo, to = (C.c_void_p * _lib.MAX_FIELDS)(), (C.c_void_p * _lib.MAX_FIELDS)()
+        for i, f in enumerate(fields):
+            if f.name in out:
+                t = out[f.name]
+                assert t.is_contiguous() and t.numel() * t.element_size() == L.batch * f.nbytes, f.name
+                fo[i] = t.data_ptr()
+            elif f.name in frames:
+                assert frames[f.name].rows == L.batch, f.name
+                to[i] = frames[f.name].entry_ptr()
+        check(self.lib.b2rl_serve_bind(base, C.byref(L), L.batch, out["header"].data_ptr(), out["idx"].data_ptr(),
+                                       out["w"].data_ptr(), fo, to, stream.cuda_stream))
+
     def put_update(self, j: int, seq: int, idx: torch.Tensor, prio: torch.Tensor, stream) -> None:
         check(self.lib.b2rl_serve_put_update(self._h, int(j), int(seq), idx.data_ptr(), prio.data_ptr(), idx.numel(),
                                              stream.cuda_stream))
@@ -430,16 +447,25 @@ class ClientSlots:
             self.ready.extend(pickle.loads(d) for d in filled)
             self.upd_free.extend(pickle.loads(d)[0] for d in done)
 
+    def acquire(self):
+        """The oldest filled slot, held by the learner until release(k, seq).  -> (k, seq, n), or None when nothing
+        is filled."""
+        with self._mu:
+            return self.ready.popleft() if self.ready else None
+
+    def release(self, k: int, seq: int) -> None:
+        """RELEASE_SLOT hands slot k back (the caller has recorded released[k] behind the slot's last reader)."""
+        self.connect.rpush(RELEASE_SLOT, pickle.dumps((k, seq)))
+
     def take(self, copy):
         """The oldest filled slot: `copy(k)` waits on filled[k], copies the slot out and records released[k]; then
         RELEASE_SLOT hands it back.  -> (k, seq, n), or None when nothing is filled."""
-        with self._mu:
-            if not self.ready:
-                return None
-            k, seq, n = self.ready.popleft()
-        copy(k)
-        self.connect.rpush(RELEASE_SLOT, pickle.dumps((k, seq)))
-        return k, seq, n
+        desc = self.acquire()
+        if desc is None:
+            return None
+        copy(desc[0])
+        self.release(*desc[:2])
+        return desc
 
     def put_update(self, write, n: int) -> bool:
         """A free update slot j: `write(j, seq)` waits on applied[j], writes the slot and records written[j]; then
@@ -613,7 +639,8 @@ class DeviceReplayClient(Stoppable, threading.Thread):
         if [L.field_bytes[i] for i in range(L.n_fields)] != [f.nbytes for f in self.fields]:
             raise RuntimeError(f"the server's ring does not carry the {self.kind.name} record fields of this config")
         srv = torch.device("cuda", info["device"])
-        self.filled = [torch.cuda.Event.from_ipc_handle(srv, h) for h in info["filled"]]
+        self.server_device = srv
+        self.filled =[torch.cuda.Event.from_ipc_handle(srv, h) for h in info["filled"]]
         self.applied = [torch.cuda.Event.from_ipc_handle(srv, h) for h in info["applied"]]
         (self.released, released_h), (self.written, written_h) = _ipc_events(self.device, L.slots), \
             _ipc_events(self.device, L.slots)
@@ -625,6 +652,11 @@ class DeviceReplayClient(Stoppable, threading.Thread):
         self.last_served = None      # descriptor (k, seq, n) of the last served slot
         self.last_header = None      # its header {seq, n} as copied out: a device int64[2]
         self.last_idx = None         # its replay slots: a device int64[B]
+        self._held = None            # (k, seq) of the slot acquire() bound in place, until release()
+        self._stage = None           # acquire() with the server on another GPU: the learner-local slot copy
+
+    def _stream(self):
+        return torch.cuda.current_stream(self.device)
 
     def poll_once(self) -> None:
         self.slots.poll()
@@ -672,6 +704,47 @@ class DeviceReplayClient(Stoppable, threading.Thread):
         self.last_served, self.last_header, self.last_idx = desc, header, idx
         return self.kind.batch(b, w, idx)
 
+    def acquire(self, out: dict, frames: dict):
+        """sample() for a captured learner step (apex.Learner with SERVED_FUSED_STEP): the oldest filled slot is bound
+        to the step's fixed buffers (ServeRing.bind) on the current stream, behind filled[k]; nothing is allocated.
+        `out`: header (int64[2]), idx, w and the fields to copy; `frames`: field name -> R.BoundFrames whose table
+        entry receives the address of that field's rows.  With the server on this GPU the slot itself is bound and
+        stays with the learner until release().  With the server on another GPU the slot is copied once into a
+        persistent learner-local buffer and released at once; that buffer is bound.  -> the descriptor (k, seq, n),
+        or None when nothing is filled."""
+        if self.lock or not self.slots.ready:
+            self.poll_once()
+        desc = self.slots.acquire()
+        if desc is None:
+            return None
+        k, seq, _ = desc
+        cur = self._stream()
+        cur.wait_event(self.filled[k])
+        if self.server_device == self.device:
+            base = self.ring.slot_ptrs(k)[0][0]
+            self._held = (k, seq)
+        else:
+            if self._stage is None:
+                self._stage = torch.empty(self.ring.layout.slot_bytes, dtype=torch.uint8, device=self.device)
+            self.ring.take(k, self._stage, cur)
+            self.released[k].record(cur)
+            self.slots.release(k, seq)
+            base = self._stage.data_ptr()
+        self.ring.bind(base, self.fields, out, frames, cur)
+        self.last_served = desc
+        return desc
+
+    def release(self) -> None:
+        """Hand back the slot acquire() bound in place: released[k] is recorded on the current stream, so call it
+        once the step that reads the slot is enqueued (conv_1's weight gradient, in backward, reads it last).  A slot
+        that was copied to the learner's GPU has already been released."""
+        if self._held is None:
+            return
+        k, seq = self._held
+        self._held = None
+        self.released[k].record(self._stream())
+        self.slots.release(k, seq)
+
     def update(self, idx, vals) -> None:
         """Replay_Server.update (APE_X/ReplayMemory.py:188-190): the write-back goes to free update slots of the
         ring (at most B pairs each) and is applied by the server in stream order.  `idx`: a tensor, an array, or a
@@ -685,12 +758,19 @@ class DeviceReplayClient(Stoppable, threading.Thread):
         vals = torch.as_tensor(vals).to(device=self.device, dtype=torch.float32).reshape(-1).contiguous()
         assert idx.numel() == vals.numel()
         B = self.ring.layout.batch
+        new = 0
         for a in range(0, idx.numel(), B):
             self._pending.append((idx[a:a + B], vals[a:a + B]))
+            new += 1
         self._flush_updates()
+        # Whatever still waits for an update slot is copied now, on the stream: the caller's tensors may be a captured
+        # step's static outputs, which its next replay overwrites.
+        for j in range(max(len(self._pending) - new, 0), len(self._pending)):
+            i, v = self._pending[j]
+            self._pending[j] = (i.clone(), v.clone())
 
     def _flush_updates(self) -> None:
-        cur = torch.cuda.current_stream(self.device)
+        cur = self._stream()
         while self._pending:
             i, v = self._pending[0]
 

@@ -262,6 +262,21 @@ int b2rl_conv1_wgrad(const uint8_t* frames_dev, int64_t capacity, const int64_t*
                      const float* gy_dev, const float* y_relu_dev, int32_t c_out, float* workspace_dev,
                      float* gw_dev, int32_t accumulate, void* stream);
 
+/* conv_1 forward and weight gradient of a learner step on a minibatch served by the stand-alone replay server
+ * (Replay_Server.sample, APE_X/ReplayMemory.py:251-257, feeding Learner.train, APE_X/Learner.py:55-121): the same
+ * kernels and results as b2rl_conv1_fused / b2rl_conv1_wgrad, but the frame base is not an argument.
+ * frame_table_dev points to ONE device-resident entry (const uint8_t*) that the kernels read when they start, e.g.
+ * written by b2rl_serve_bind, so a launch captured in a CUDA graph reads whichever slot was bound before the replay.
+ * The base it holds must be 16-byte aligned; when b2rl_conv1_wgrad_table splits a large n over several launches
+ * (idx_dev NULL) each launch adds its row offset to the loaded base on the device.  An error, and no launch, for a
+ * null or misaligned entry. */
+int b2rl_conv1_fused_table(const uint8_t* const* frame_table_dev, int64_t capacity, const int64_t* idx_dev, int64_t n,
+                           const int8_t* bq_dev, const float* scale_dev, int32_t n_nets, int32_t c_out,
+                           float* out_dev, int32_t relu, void* stream);
+int b2rl_conv1_wgrad_table(const uint8_t* const* frame_table_dev, int64_t capacity, const int64_t* idx_dev,
+                           int64_t n, const float* gy_dev, const float* y_relu_dev, int32_t c_out,
+                           float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream);
+
 /* Learner.step (APE_X/Learner.py:123-138; IMPALA/Learner.py:258-266 without the clipping) with
  * torch.optim.RMSprop's update (baseline/utils.py getOptim :124-130; centered for Ape-X,
  * cfg/ape_x.json:27-35) in ONE pass: square_avg / grad_avg / param update, gradient zeroed, and
@@ -418,6 +433,18 @@ int b2rl_serve_fill_uniform(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, ui
 /* Replay_Server.sample (APE_X/ReplayMemory.py:251-257) without the unpickle: copy minibatch slot k (slot_bytes,
  * header included) to dst_dev with one cudaMemcpyAsync on `stream` (a peer copy when the ring is on another GPU). */
 int b2rl_serve_take(const b2rl_serve_ring* r, int32_t slot, void* dst_dev, void* stream);
+/* Replay_Server.sample (APE_X/ReplayMemory.py:251-257) for a captured learner step (APE_X/Learner.py:55-121), in
+ * ONE launch on `stream`: the filled minibatch slot at slot_dev (a mapped ring slot, or a learner-local copy made
+ * with b2rl_serve_take), laid out by `layout`, is bound to the step's fixed buffers.  The header {seq, n}, idx and
+ * w are copied to header_out_dev (16 B), idx_out_dev (int64[n]) and w_out_dev (fp32[n]).  For each field f:
+ * fields_out_dev[f] != NULL receives a copy of its n rows; table_out_dev[f] != NULL (an 8-byte aligned device
+ * entry, for b2rl_conv1_fused_table / b2rl_conv1_wgrad_table) receives the device address of its rows instead, so
+ * the frames are read in the slot.  Either host array may be NULL.  An error, and no launch, for a null slot, a slot
+ * base that is not 16-byte aligned or a layout whose batch is not n.  The slot must stay unreleased until the last
+ * kernel that reads a table entry has run. */
+int b2rl_serve_bind(const void* slot_dev, const b2rl_serve_layout* layout, int64_t n, uint64_t* header_out_dev,
+                    int64_t* idx_out_dev, float* w_out_dev, void* const* fields_out_dev, void* const* table_out_dev,
+                    void* stream);
 /* Replay_Server.update (APE_X/ReplayMemory.py:188-190, flushed to `update` at :241-249): write n <= B (idx,
  * priority) pairs and the header {seq, n} into update slot j, one launch on `stream`. */
 int b2rl_serve_put_update(b2rl_serve_ring* r, int32_t slot, uint64_t seq, const int64_t* idx_dev,

@@ -3,6 +3,9 @@ minibatches/s and learner steps/s for
   redis   ReplayServer -> pickled `BATCH` list -> Replay_Server (host arrays, copied to the device by train());
           Ape-X and R2D2 only
   ring    DeviceReplayServer -> device serve ring (CUDA IPC) -> DeviceReplayClient
+  ring-fused  Ape-X only: the same ring, with the learner's captured fused step reading each minibatch in its ring
+          slot (ApexConfig.SERVED_FUSED_STEP: acquire -> graph replay -> release -> write-back); served
+          minibatches/s is acquire + release alone
   fused   the in-process learner: Learner.fused_step() on its own replay (no server)
   sample  IMPALA only: the in-process Replay's sample() -> Learner.train() (gather + time-major transpose per step)
   fill    b2rl_serve_fill (IMPALA: b2rl_serve_fill_uniform) alone, in this process: CUDA events around `steps` fills
@@ -10,7 +13,7 @@ minibatches/s and learner steps/s for
           byte read once, written once)
 
     python tools/bench_serve.py [--workload apex|r2d2|impala] [--slots-store N] [--batch B] [--steps 200]
-                                [--warmup 20] [--repeats 3] [--arms redis,ring,fused,sample,fill]
+                                [--warmup 20] [--repeats 3] [--arms redis,ring,ring-fused,fused,sample,fill]
 
 Defaults per workload: Ape-X B = 512 on a 2^16-slot store (3.7 GB); R2D2 B = 64, T = 80, MEM = 20 on a 2^12-sequence
 store (9.2 GB); IMPALA B = 32, T = 20 on a 2^11-rollout store (1.2 GB).
@@ -85,7 +88,7 @@ def _server_main(kind, proxy, args, stop):
     from distributed_rl_b200.replay_server import DeviceReplayServer, ReplayServer
     conn = _connect(args, proxy)
     cfg = _cfg(args, args["server_device"])
-    if kind == "ring":
+    if kind.startswith("ring"):
         srv = DeviceReplayServer(cfg, conn, slots=args["ring_slots"])
         _fill(srv.store, args["store"])
         while not stop.is_set():
@@ -133,7 +136,8 @@ def _served_arm(kind, args):
         child.start()
         cfg = _cfg(args, "cuda:0")
         cfg.CUDNN_BENCHMARK = True
-        if kind == "ring":
+        cfg.SERVED_FUSED_STEP = kind == "ring-fused"
+        if kind.startswith("ring"):
             client = DeviceReplayClient(cfg, conn, timeout=300.0)
         else:
             client = Replay_Server(cfg, conn, conn)
@@ -159,6 +163,19 @@ def _served_arm(kind, args):
                 return
             info, prio, idx = L.train(b)[:3]
             client.update(idx if kind == "ring" else list(idx.tolist()), prio)
+        if kind == "ring-fused":
+            s = L._fused_state()
+            count = [0]
+
+            def serve_only():            # the bind alone: acquire (wait on filled[k] + one k_serve_bind), release
+                while client.acquire(s.cur, s.frames) is None:
+                    time.sleep(0.0001)
+                client.release()
+
+            def step():                  # the eviction request never comes: every step writes back
+                count[0] += 1
+                while L._served_fused_step(count[0], 1 << 62) is None:
+                    time.sleep(0.0001)
         n = args["redis_steps"] if kind == "redis" else args["steps"]
         served = _timed(serve_only, n, args["warmup"], dev)
         steps = _timed(step, n, args["warmup"], dev)
@@ -167,7 +184,7 @@ def _served_arm(kind, args):
         stop.set()
         if client is not None:
             client.stop()
-            if kind == "ring":
+            if kind.startswith("ring"):
                 client.close()
             else:
                 client.join(timeout=10)        # the polling thread must not outlive the manager
@@ -258,7 +275,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--server-device", default="cuda:0")
-    ap.add_argument("--arms", default=None, help="any of redis, ring, fused, sample, fill (default: Ape-X and R2D2 "
+    ap.add_argument("--arms", default=None, help="any of redis, ring, ring-fused (Ape-X), fused, sample, fill (default: Ape-X and R2D2 "
                     "redis,ring,fused; IMPALA ring,sample,fused)")
     ap.add_argument("--redis", default=None, help="host of a Redis server for the control plane (default: an "
                     "in-memory stand-in in a manager process, which makes the Redis-pickle arm far slower than a "
@@ -272,6 +289,8 @@ def main():
     arms = a.arms or ("ring,sample,fused" if a.workload == "impala" else "redis,ring,fused")
     if a.workload == "impala" and "redis" in arms.split(","):
         sys.exit("IMPALA has no Redis-protocol replay server")
+    if a.workload != "apex" and "ring-fused" in arms.split(","):
+        sys.exit("the ring-fused arm is the Ape-X learner's served fused step")
     args = {"workload": a.workload, "store": store, "batch": batch, "ring_slots": a.ring_slots, "steps": a.steps,
             "warmup": a.warmup, "server_device": a.server_device, "redis": a.redis,
             "redis_steps": a.redis_steps or a.steps,
