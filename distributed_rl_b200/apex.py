@@ -20,7 +20,6 @@ What changed relative to the reference, and why it is still a drop-in:
 from __future__ import annotations
 
 import pickle
-import time
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -29,8 +28,8 @@ import torch
 from . import _lib
 from . import replay as R
 from .agent import GraphAgent
-from .learner_common import (Conv1Gathered as _Conv1Gathered, MemoryView, ReplayThread, TargetNetLearner, conv1_packs,
-                             make_optimizer)
+from .learner_common import (Conv1Gathered as _Conv1Gathered, MemoryView, ReplayThread, TargetNetLearner,
+                             _attach_replay, conv1_packs, make_optimizer)
 
 
 @dataclass
@@ -263,6 +262,8 @@ class Learner(TargetNetLearner):
     LOG_LINE = ("step:{step} // mean_value:{mean_value:.3f} // norm: {norm:.3f} // REWARD:{reward:.3f} // "
                 "NUM_MEMORY:{num_memory} // Mean_Weight:{mean_weight:.3f} // MAX_WEIGHT:{max_weight:.3f} // "
                 "TIME:{time_per_step:.5f} // loss:{loss:.5f}")
+    PUBLISH_EVERY = 50
+    LOG_STATS = ("loss", "mean_value", "mean_weight", "norm")
 
     def __init__(self, cfg: ApexConfig | None = None, connect=None, start_replay: bool = True,
                  writer=None, memory=None):
@@ -270,7 +271,7 @@ class Learner(TargetNetLearner):
         `Replay` surface: sample / update / lock / memory).  run() then drives sample() -> train() -> update() with
         the reference's cadence (APE_X/Learner.py:163-197); without it the learner owns its replay and run() steps
         with fused_step().  With SERVED_FUSED_STEP, run() over a served memory steps fused_step() instead, on the
-        slot `memory.acquire()` binds (same cadence)."""
+        slot `memory.acquire()` binds (same cadence): see _next_step."""
         self.cfg = cfg or ApexConfig.from_configuration()
         if memory is not None and self.cfg.SERVED_FUSED_STEP:
             self._check_served_fused(memory)
@@ -280,20 +281,8 @@ class Learner(TargetNetLearner):
         self.build_model()
         self.build_optim()
         self.connect = connect
-        self._served = memory is not None
-        if self._served:
-            self.memory = memory
-            if start_replay and not memory.is_alive():
-                memory.start()
-        else:
-            self.memory = Replay(self.cfg, connect)
-            if start_replay and connect is not None:
-                self.memory.start()
+        self.memory = _attach_replay(self, memory, lambda: Replay(self.cfg, connect), connect, start_replay, wipe=True)
         self.writer = writer
-        if connect is not None:                  # :41-43 — whatever a previous run left behind is dropped
-            from .wire import wipe_stale_keys
-            # ... except the keys of a replay server this learner is already attached to (its handshake lives there)
-            wipe_stale_keys(connect, keep=getattr(self.memory, "KEEP_KEYS", ()) if self._served else ())
         self.gamma_n = float(np.float32(0.99 ** self.cfg.UNROLL_STEP))  # hard-coded 0.99, :103
         self._graph = None
         self._fused = None              # _StepState, built by the first fused_step / _forward_backward_fused
@@ -543,14 +532,14 @@ class Learner(TargetNetLearner):
         """sample -> gather -> forwards -> target -> backward -> RMSprop -> priority
         write-back (APE_X/Learner.py:165-197) with no host round trip.  On a served memory (SERVED_FUSED_STEP) the
         same step on the slot the last `memory.acquire()` bound; see _bound_step."""
+        if self._graph is not None:
+            self._graph.replay()
+            return self._static
         if self._served:
             if not self.cfg.SERVED_FUSED_STEP:
                 raise RuntimeError("fused_step() samples the learner's own replay; a served replay is driven by run() "
                                    "(or set SERVED_FUSED_STEP)")
             return self._bound_step(use_graph)
-        if self._graph is not None:
-            self._graph.replay()
-            return self._static
         B = self.cfg.BATCHSIZE
         st = self.memory.store
         s = self._fused_state()
@@ -599,35 +588,16 @@ class Learner(TargetNetLearner):
                 s.max_w.join()
             return {"scalars": out["scalars"], "p_norm": info["p_norm"], "prio": out["prio"], "idx": idx}
 
-        lib = st.lib
         if self._world > 1 and self._max_w_use is None:      # first step: reduce synchronously once
             self._max_w_use = self._D.all_reduce_max_(st.max_weight(self.cfg.BETA)).clone()
         if not use_graph:
-            c0 = lib.b2rl_launch_count()
-            r = body()
-            self.launches_per_step = lib.b2rl_launch_count() - c0
-            return r
+            return self._eager_or_captured(body, False)
         self.optim.zero_grad(set_to_none=False)
-        # The step's main branch is captured on a HIGH-priority stream (kernel nodes inherit it): the side branches
-        # (weight gradients, early optimizer step, operand packs) only fill SMs the critical chain leaves idle.
-        main = s.main
         # The ingest thread keeps pushing on the same replay handle: hold its lock so that no cudaMalloc /
         # cudaHostAlloc / copy of that thread lands inside the warm-up or the (global-mode) capture.
         with self.memory._lock:
-            main.wait_stream(torch.cuda.current_stream(self.device))
-            with torch.cuda.stream(main):
-                for _ in range(3):   # warm-up: lazy inits (cuDNN plans, optimizer state) happen outside capture
-                    body()
-            torch.cuda.current_stream(self.device).wait_stream(main)
-            torch.cuda.synchronize(self.device)
-            g = torch.cuda.CUDAGraph()
-            c0 = lib.b2rl_launch_count()
-            with torch.cuda.graph(g, stream=main):
-                self._static = body()
-            self.launches_per_step = lib.b2rl_launch_count() - c0   # recorded into the graph, replayed each step
-        self._graph = g
-        g.replay()
-        return self._static
+            self._warm_up(body, 3)
+            return self._eager_or_captured(body, True)
 
     BOUND_WARMUP = 3       # eager steps on served minibatches before the bound step is captured
 
@@ -637,11 +607,7 @@ class Learner(TargetNetLearner):
         through memory.update() after the step.  The first BOUND_WARMUP calls run the step eagerly on the main stream
         (lazy inits stay outside the capture), each on its own minibatch; the next call captures the graph, and every
         call replays it.  The caller releases the slot after this returns: the replay is then enqueued."""
-        s = self._fused_state()
-        if self._graph is not None:
-            self._graph.replay()
-            return self._static
-        c = s.cur
+        c = self._fused_state().cur
         batched = self.cfg.PARALLEL_FORWARDS and self.cfg.BATCHED_ONLINE   # the batched pass converts the action
 
         def body():
@@ -651,103 +617,78 @@ class Learner(TargetNetLearner):
             info = self.step()
             return {"scalars": out["scalars"], "p_norm": info["p_norm"], "prio": out["prio"], "idx": c["idx"]}
 
+        if use_graph and self._bound_warm < self.BOUND_WARMUP:
+            if self._bound_warm == 0:
+                self.optim.zero_grad(set_to_none=False)
+            self._bound_warm += 1
+            return self._warm_up(body, 1)
+        return self._eager_or_captured(body, use_graph)
+
+    # The two callers warm up before the capture differently, on purpose.  fused_step draws its own minibatches, so
+    # its first call runs all three warm-ups and the capture, under the replay's lock (bench.py's warm-up loop counts
+    # on "3 eager warm-ups + capture" in the first call).  A bound step needs a new served slot for each warm-up, so
+    # _bound_step warms up over three calls and captures on the fourth.
+    def _eager_or_captured(self, body, use_graph: bool):
+        """`body` (one step) run eagerly, its libb2rl launches counted into `launches_per_step`; or, with
+        `use_graph`, captured into `_graph`, whose launches are counted the same way, and replayed: every later
+        fused_step replays it.  -> the step's outputs (for the graph: `_static`, its static output buffers)."""
         lib = _lib.load()
         if not use_graph:
             c0 = lib.b2rl_launch_count()
             r = body()
             self.launches_per_step = lib.b2rl_launch_count() - c0
             return r
-        cur = torch.cuda.current_stream(self.device)
-        if self._bound_warm < self.BOUND_WARMUP:
-            if self._bound_warm == 0:
-                self.optim.zero_grad(set_to_none=False)
-            self._bound_warm += 1
-            s.main.wait_stream(cur)
-            with torch.cuda.stream(s.main):
-                r = body()
-            cur.wait_stream(s.main)
-            return r
         torch.cuda.synchronize(self.device)
         g = torch.cuda.CUDAGraph()
         c0 = lib.b2rl_launch_count()
-        with torch.cuda.graph(g, stream=s.main):
+        # The step's main branch is captured on a HIGH-priority stream (kernel nodes inherit it): the side branches
+        # (weight gradients, early optimizer step, operand packs) only fill SMs the critical chain leaves idle.
+        with torch.cuda.graph(g, stream=self._fused.main):
             self._static = body()
-        self.launches_per_step = lib.b2rl_launch_count() - c0
+        self.launches_per_step = lib.b2rl_launch_count() - c0   # recorded into the graph, replayed each step
         self._graph = g
         g.replay()
         return self._static
 
-    # -- main loop ---------------------------------------------------------------------------------
-    def run(self, max_steps: int | None = None, log_every: int = 500):
-        """Learner.run (:140-262) with the reference's cadence: wait for BUFFER_SIZE records, announce `Start`,
-        hard target sync every TARGET_FREQUENCY steps, parameter publication every 50, and every `log_every`
-        (500) steps the eviction request (`memory.lock`, :189-191), the `reward` drain + log line (:219-253) and a
-        checkpoint of the online weights (:256-262).  Publication and checkpoints go through ParamPublisher
-        (async D2H into pinned memory), so none of them stalls the learner stream."""
-        pub, pub_t, ckpt = self._start()
-        step = 0
-        t0 = time.time()
-        acc = None
-        self.last_log = None
-        while max_steps is None or step < max_steps:
+    def _warm_up(self, body, n: int):
+        """`n` eager runs of `body` on the step's main stream, so that lazy inits (cuDNN plans, optimizer state)
+        happen outside the capture.  -> what the last one returned."""
+        cur, main = torch.cuda.current_stream(self.device), self._fused.main
+        main.wait_stream(cur)
+        with torch.cuda.stream(main):
+            for _ in range(n):
+                r = body()
+        cur.wait_stream(main)
+        return r
+
+    # -- one step of run() ---------------------------------------------------------------------------
+    def _next_step(self, step: int, log_every: int):
+        """One iteration of the reference loop (APE_X/Learner.py:163-197) and its write-back cadence.  In-process:
+        fused_step(), whose graph writes the priorities back.  Served: a minibatch from `memory`, then the
+        write-back; with SERVED_FUSED_STEP the oldest filled slot is bound (memory.acquire), fused_step() runs on it
+        and the slot is handed back once the step is enqueued (memory.release: conv_1's weight gradient, in
+        backward, is its last reader); otherwise sample() -> train().
+        -> {loss, mean(y), mean(w), norm} as a device tensor, or None when no minibatch is ready."""
+        if self._served and not self.cfg.SERVED_FUSED_STEP:
+            batch = self.memory.sample()
+            if batch is False:
+                return None
+            info, prio, idx, mean_w = self.train(batch)
+            tot = torch.stack([info["loss"], info["mean_value"], mean_w, info["p_norm"].reshape(())])
+        else:
             if self._served:
-                tot = self._served_step(step + 1, log_every)
-                if tot is None:
-                    time.sleep(0.002)                # nothing served yet (:166-170)
-                    continue
+                s = self._fused_state()
+                if self.memory.acquire(s.cur, s.frames) is None:
+                    return None
+                out = self.fused_step()
+                self.memory.release()
+                idx, prio = out["idx"], out["prio"]
             else:
                 out = self.fused_step()
-                tot = torch.cat([out["scalars"], out["p_norm"].reshape(1)])
-            step += 1
-            acc = tot.clone() if acc is None else acc + tot
-            if step % self.cfg.TARGET_FREQUENCY == 0:
-                self.target_model.updateParameter(self.model, 1)
-                pub_t.snapshot(step)                 # async D2H; published by a later poll()
-            if step % 50 == 0:
-                pub.snapshot(step - 50)              # :212-216, without stalling the learner stream
-            for p in self._publishers:
-                p.poll()
-            if step % log_every == 0:
-                if not self._served:
-                    self.memory.lock = True          # :189-191 eviction request, served by the ingest thread
-                    if self.connect is None or not self.memory.is_alive():
-                        self.memory._evict_on_request()
-                loss, mean_value, mean_w, norm = (acc / log_every).tolist()
-                self._log(step, log_every, t0, ckpt, mean_value, norm, loss=loss, mean_weight=mean_w)
-                acc, t0 = None, time.time()
-        return step
-
-    def _served_step(self, step: int, log_every: int):
-        """One iteration of the reference loop over a served replay (APE_X/Learner.py:163-197): sample, train, the
-        eviction request every `log_every` steps (that step's write-back is skipped, as there), write-back.
-        -> {loss, mean(y), mean(w), norm} as a device tensor, or None when no minibatch is ready."""
-        if self.cfg.SERVED_FUSED_STEP:
-            return self._served_fused_step(step, log_every)
-        batch = self.memory.sample()
-        if batch is False:
-            return None
-        info, prio, idx, mean_w = self.train(batch)
-        if step % log_every == 0:
-            self.memory.lock = True
-        if self.memory.lock is False:
-            self.memory.update(idx, prio)
-        return torch.stack([info["loss"], info["mean_value"], mean_w, info["p_norm"].reshape(())])
-
-    def _served_fused_step(self, step: int, log_every: int):
-        """_served_step on the captured step: bind the oldest filled slot (memory.acquire), step on it, hand the slot
-        back once the step is enqueued (memory.release: conv_1's weight gradient, in backward, is its last reader),
-        then the eviction request every `log_every` steps (that step's write-back is skipped) or the write-back.
-        -> {loss, mean(y), mean(w), norm} as a device tensor, or None when no minibatch is ready."""
-        s = self._fused_state()
-        if self.memory.acquire(s.cur, s.frames) is None:
-            return None
-        out = self.fused_step()
-        self.memory.release()
-        if step % log_every == 0:
-            self.memory.lock = True
-        if self.memory.lock is False:
-            self.memory.update(out["idx"], out["prio"])
-        return torch.cat([out["scalars"], out["p_norm"].reshape(1)])
+                idx, prio = None, None
+            tot = torch.cat([out["scalars"], out["p_norm"].reshape(1)])
+        self._write_back(step, log_every, idx, prio)
+        return tot
 
     def _check_served_fused(self, memory) -> None:
         """What SERVED_FUSED_STEP needs, checked before anything is built."""

@@ -12,7 +12,8 @@ import torch
 
 from . import replay as R
 from .agent import GraphAgent
-from .learner_common import Conv1Gathered, ReplayThread, conv1_packs, make_optimizer, publishers, time_major_rows
+from .learner_common import (Conv1Gathered, ReplayThread, _attach_replay, conv1_packs, make_optimizer, publishers,
+                             time_major_rows)
 from .publish import ParamPublisher
 
 
@@ -120,15 +121,8 @@ class Learner:
         self.model.dense_3xtf32 = bool(self.cfg.DENSE_3XTF32) and self.device.type == "cuda"
         self.mOptim = make_optimizer(self.cfg.OPTIM_INFO, self.model.getParameters())
         self._connect = connect
-        self._served = memory is not None
-        if self._served:
-            self._memory = memory
-            if start_replay and not memory.is_alive():
-                memory.start()
-        else:
-            self._memory = Replay(self.cfg, connect)
-            if connect is not None and start_replay:
-                self._memory.start()                            # IMPALA/Learner.py:27-28
+        self._memory = _attach_replay(self, memory, lambda: Replay(self.cfg, connect), connect, start_replay,
+                                      wipe=False)
         self.last = {}
 
     @property

@@ -1,7 +1,7 @@
-"""What the Ape-X, R2D2 and IMPALA learner sides share: the optimiser factory, the replay ingest thread, the
-conv_1 autograd function and its packs, the time-major frame-row layout, and the Redis-facing pieces of
-`Learner.run` (start handshake, publishers, periodic log).  Each learner keeps its own store layout, batch
-assembly and loop body."""
+"""What the Ape-X, R2D2 and IMPALA learner sides share: the optimiser factory, the replay ingest thread and the
+learner's replay set-up, the conv_1 autograd function and its packs, the time-major frame-row layout, and the
+Ape-X / R2D2 `Learner.run` loop with its write-back cadence (start handshake, publishers, periodic log).  Each
+learner keeps its own store layout, batch assembly and step body."""
 from __future__ import annotations
 
 import pickle
@@ -117,13 +117,37 @@ class ReplayThread(Stoppable, threading.Thread):
         return self.deque.pop(0)
 
     def update(self, idx, vals) -> None:
-        """Replay.update (APE_X/ReplayMemory.py:43-59) -> PER.update, applied at once.  `idx`: a tensor, an array, or
-        a list of ints or 0-d tensors (what the reference passes)."""
-        if isinstance(idx, (list, tuple)):
-            idx = torch.stack([torch.as_tensor(i) for i in idx]) if len(idx) and torch.is_tensor(idx[0]) \
-                else torch.as_tensor(np.asarray(idx, np.int64))
+        """Replay.update (APE_X/ReplayMemory.py:43-59) -> PER.update, applied at once.  `idx`: see _index_tensor."""
         with self._lock:
-            self.store.update(torch.as_tensor(idx).to(self.device), torch.as_tensor(vals).to(self.device))
+            self.store.update(_index_tensor(idx).to(self.device), torch.as_tensor(vals).to(self.device))
+
+
+def _index_tensor(idx) -> torch.Tensor:
+    """A write-back's replay slots as a tensor.  `idx`: a tensor, an array, or a list of ints or 0-d tensors (what
+    the reference passes)."""
+    if isinstance(idx, (list, tuple)):
+        return torch.stack([torch.as_tensor(i) for i in idx]) if len(idx) and torch.is_tensor(idx[0]) \
+            else torch.as_tensor(np.asarray(idx, np.int64))
+    return torch.as_tensor(idx)
+
+
+def _attach_replay(learner, memory, make_replay, connect, start_replay: bool, wipe: bool):
+    """The learner's replay (APE_X/Learner.py:28-29,41-43, R2D2/Learner.py:46-48,54,63-64, IMPALA/Learner.py:27-28):
+    `memory`, a replay served from another process, started unless it already runs; or, when it is None,
+    `make_replay()`, the learner's own, started when there is a Redis connection.  `wipe`: then drop whatever a
+    previous run left in the database, except the keys of a replay server this learner is attached to
+    (`memory.KEEP_KEYS`: its handshake lives there).  Sets `learner._served`.  -> the replay."""
+    learner._served = memory is not None
+    if learner._served:
+        if start_replay and not memory.is_alive():
+            memory.start()
+    else:
+        memory = make_replay()
+        if start_replay and connect is not None:
+            memory.start()
+    if wipe and connect is not None:
+        wire.wipe_stale_keys(connect, keep=getattr(memory, "KEEP_KEYS", ()) if learner._served else ())
+    return memory
 
 
 # -- conv_1 on libb2rl's kernels -----------------------------------------------------------------
@@ -211,11 +235,58 @@ def publishers(model, log_w, *pubs):
 
 
 class TargetNetLearner:
-    """The parts of `Learner` that Ape-X and R2D2 share (online + target network, `Start` handshake, periodic
-    log).  Uses the learner's `cfg`, `model`, `target_model`, `memory`, `connect` and `writer`; `LOG_LINE` is the
-    learner's log line, formatted with `last_log`, `num_memory` and `max_weight`."""
+    """The parts of `Learner` that Ape-X and R2D2 share (online + target network, run loop, write-back cadence,
+    `Start` handshake, periodic log).  Uses the learner's `cfg`, `model`, `target_model`, `memory`, `_served`,
+    `connect` and `writer`.  A learner provides `_next_step(step, log_every)` and sets `LOG_LINE`, its log line
+    formatted with `last_log`, `num_memory` and `max_weight`; `PUBLISH_EVERY`, the steps between two publications
+    of the online weights; and `LOG_STATS`, the names of the stats `_next_step` returns."""
 
     LOG_LINE: str
+    PUBLISH_EVERY: int
+    LOG_STATS: tuple
+
+    def run(self, max_steps: int | None = None, log_every: int = 500):
+        """Learner.run (APE_X/Learner.py:140-262, R2D2/Learner.py:217-339) with the reference's cadence: wait for
+        more than BUFFER_SIZE records, announce `Start`, then per step `_next_step` (retried after 2 ms, and not
+        counted, while no minibatch is ready: APE_X/Learner.py:166-170); hard target sync every TARGET_FREQUENCY
+        steps (+ `target_state_dict`, APE_X/Learner.py:207-210); `state_dict` / `count` = step - 50 every
+        PUBLISH_EVERY steps (:212-216; R2D2 publishes every 25 steps and still counts step - 50, sic
+        R2D2/Learner.py:289-293); and every `log_every` (500) steps the `reward` drain + log line and a checkpoint
+        of the online weights (APE_X/Learner.py:219-262, R2D2/Learner.py:296-339).  Publication and checkpoints go
+        through ParamPublisher (async D2H into pinned memory), so none of them stalls the learner stream."""
+        pub, pub_t, ckpt = self._start()
+        step, acc, t0 = 0, None, time.time()
+        self.last_log = None
+        while max_steps is None or step < max_steps:
+            tot = self._next_step(step + 1, log_every)
+            if tot is None:
+                time.sleep(0.002)
+                continue
+            step += 1
+            acc = tot if acc is None else acc + tot
+            if step % self.cfg.TARGET_FREQUENCY == 0:
+                self.target_model.updateParameter(self.model, 1)
+                pub_t.snapshot(step)                 # async D2H; published by a later poll()
+            if step % self.PUBLISH_EVERY == 0:
+                pub.snapshot(step - 50)
+            for p in self._publishers:
+                p.poll()
+            if step % log_every == 0:
+                self._log(step, log_every, t0, ckpt, **dict(zip(self.LOG_STATS, (acc / log_every).tolist())))
+                acc, t0 = None, time.time()
+        return step
+
+    def _write_back(self, step: int, log_every: int, idx, prio) -> None:
+        """The write-back cadence (APE_X/Learner.py:189-197, R2D2/Learner.py:266-274): every `log_every` steps the
+        eviction request (`memory.lock`), which skips that step's write-back unless it has been served by then.  An
+        in-process replay without a running ingest thread serves it inline; a served memory passes it on to its
+        server.  `prio` None: the step has written its priorities back itself."""
+        if step % log_every == 0:
+            self.memory.lock = True
+            if not self._served and (self.connect is None or not self.memory.is_alive()):
+                self.memory._evict_on_request()
+        if prio is not None and self.memory.lock is False:
+            self.memory.update(idx, prio)
 
     @property
     def state_dict(self):

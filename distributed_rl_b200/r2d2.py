@@ -16,8 +16,8 @@ import torch
 
 from . import replay as R
 from .agent import GraphAgent
-from .learner_common import (Conv1Gathered, MemoryView, ReplayThread, TargetNetLearner, conv1_packs, make_optimizer,
-                             time_major_rows)
+from .learner_common import (Conv1Gathered, MemoryView, ReplayThread, TargetNetLearner, _attach_replay, conv1_packs,
+                             make_optimizer, time_major_rows)
 
 
 def default_r2d2_model() -> dict:
@@ -124,6 +124,8 @@ class Replay(ReplayThread):
 class Learner(TargetNetLearner):
     LOG_LINE = ("step:{step} // mean_value:{mean_value:.3f} // norm: {norm:.3f} // REWARD:{reward:.3f} // "
                 "NUM_MEMORY:{num_memory} // MAX_WEIGHT:{max_weight:.3f} // TIME:{time_per_step:.5f}")
+    PUBLISH_EVERY = 25
+    LOG_STATS = ("mean_value", "norm")
 
     def __init__(self, cfg: R2D2Config | None = None, connect=None, start_replay: bool = True, writer=None,
                  memory=None):
@@ -138,20 +140,8 @@ class Learner(TargetNetLearner):
             m.dense_3xtf32 = m.fused_dueling_tail = bool(self.cfg.FUSED_HEADS) and self.device.type == "cuda"
         self.optim = make_optimizer(self.cfg.OPTIM_INFO, self.model.getParameters())
         self.connect = connect
-        self._served = memory is not None
-        if self._served:
-            self.memory = memory
-            if start_replay and not memory.is_alive():
-                memory.start()
-        else:
-            self.memory = Replay(self.cfg, connect)
-            if start_replay and connect is not None:
-                self.memory.start()                              # R2D2/Learner.py:46-48
+        self.memory = _attach_replay(self, memory, lambda: Replay(self.cfg, connect), connect, start_replay, wipe=True)
         self.writer = writer
-        if connect is not None:
-            from .wire import wipe_stale_keys
-            # :54,63-64 — except the keys of a replay server this learner is already attached to
-            wipe_stale_keys(connect, keep=getattr(self.memory, "KEEP_KEYS", ()) if self._served else ())
 
     def train(self, transition, t=0):
         c = self.cfg
@@ -268,39 +258,12 @@ class Learner(TargetNetLearner):
         self.optim.zero_grad(set_to_none=False)
         return {"p_norm": p_norm}
 
-    def run(self, max_steps=None, log_every: int = 500):
-        """R2D2/Learner.py:217-339: wait for BUFFER_SIZE sequences, announce `Start`, then per step sample ->
-        train -> priority write-back; hard target sync every TARGET_FREQUENCY steps (+ `target_state_dict`),
-        `state_dict` / `count` (= step - 50, sic :293) every 25 steps, and every 500 steps the eviction request,
-        the `reward` drain + log line and a checkpoint.  Publication is asynchronous (ParamPublisher)."""
-        import time
-        pub, pub_t, ckpt = self._start()                                # :227-234
-        step, acc, t0 = 0, None, time.time()
-        self.last_log = None
-        while max_steps is None or step < max_steps:
-            batch = self.memory.sample()
-            if batch is False:
-                time.sleep(0.002)
-                continue
-            info, prio, idx = self.train(batch)
-            step += 1
-            if step % log_every == 0:
-                self.memory.lock = True                                  # :266-268, that step's write-back skipped
-                if not self._served and (self.connect is None or not self.memory.is_alive()):
-                    self.memory._evict_on_request()                      # a served memory's server evicts
-            if not self.memory.lock:
-                self.memory.update(idx, prio)                            # :271-274
-            tot = torch.stack([info["mean_value"].reshape(()), info["p_norm"].reshape(())])
-            acc = tot if acc is None else acc + tot
-            if step % self.cfg.TARGET_FREQUENCY == 0:                    # :283-286
-                self.target_model.updateParameter(self.model, 1)
-                pub_t.snapshot(step)
-            if step % 25 == 0:                                           # :288-293
-                pub.snapshot(step - 50)
-            for p in self._publishers:
-                p.poll()
-            if step % log_every == 0:                                    # :296-339
-                mean_value, norm = (acc / log_every).tolist()
-                self._log(step, log_every, t0, ckpt, mean_value, norm)
-                acc, t0 = None, time.time()
-        return step
+    def _next_step(self, step: int, log_every: int):
+        """One iteration of run() (R2D2/Learner.py:240-274): sample -> train -> the write-back cadence.
+        -> {mean(Q), norm} as a device tensor, or None when no minibatch is ready."""
+        batch = self.memory.sample()
+        if batch is False:
+            return None
+        info, prio, idx = self.train(batch)
+        self._write_back(step, log_every, idx, prio)
+        return torch.stack([info["mean_value"].reshape(()), info["p_norm"].reshape(())])

@@ -63,7 +63,7 @@ from ._lib import check
 from . import apex, impala, r2d2
 from .apex import ApexConfig
 from .impala import ImpalaConfig
-from .learner_common import Stoppable
+from .learner_common import Stoppable, _index_tensor
 from .r2d2 import R2D2Config
 
 
@@ -683,24 +683,32 @@ class DeviceReplayClient(Stoppable, threading.Thread):
         return (view(0, 16, torch.int64, (2,)), view(L.idx_off, 8 * B, torch.int64, (B,)),
                 view(L.w_off, 4 * B, torch.float32, (B,)), out)
 
+    def _next_filled(self):
+        """The oldest filled slot, held by the learner until it is released, with the current stream made to wait on
+        its filled[k].  Polls first while the eviction request is pending or nothing is known to be filled.
+        -> (descriptor (k, seq, n), stream), or None when nothing is filled."""
+        if self.lock or not self.slots.ready:
+            self.poll_once()
+        desc = self.slots.acquire()
+        if desc is None:
+            return None
+        cur = self._stream()
+        cur.wait_event(self.filled[desc[0]])
+        return desc, cur
+
     def sample(self):
         """Replay_Server.sample (APE_X/ReplayMemory.py:251-257, R2D2/ReplayMemory.py:266-274): the oldest filled
         slot, copied into fresh learner-local memory on the current stream; False when nothing is filled."""
-        cur = torch.cuda.current_stream(self.device)
-        got = []
-
-        def copy(k):
-            buf = torch.empty(self.ring.layout.slot_bytes, dtype=torch.uint8, device=self.device)
-            cur.wait_event(self.filled[k])
-            self.ring.take(k, buf, cur)
-            self.released[k].record(cur)
-            got.append(buf)
-        if self.lock or not self.slots.ready:
-            self.poll_once()
-        desc = self.slots.take(copy)
-        if desc is None:
+        got = self._next_filled()
+        if got is None:
             return False
-        header, idx, w, b = self._views(got[0])
+        desc, cur = got
+        k, seq, _ = desc
+        buf = torch.empty(self.ring.layout.slot_bytes, dtype=torch.uint8, device=self.device)
+        self.ring.take(k, buf, cur)
+        self.released[k].record(cur)
+        self.slots.release(k, seq)
+        header, idx, w, b = self._views(buf)
         self.last_served, self.last_header, self.last_idx = desc, header, idx
         return self.kind.batch(b, w, idx)
 
@@ -712,14 +720,11 @@ class DeviceReplayClient(Stoppable, threading.Thread):
         stays with the learner until release().  With the server on another GPU the slot is copied once into a
         persistent learner-local buffer and released at once; that buffer is bound.  -> the descriptor (k, seq, n),
         or None when nothing is filled."""
-        if self.lock or not self.slots.ready:
-            self.poll_once()
-        desc = self.slots.acquire()
-        if desc is None:
+        got = self._next_filled()
+        if got is None:
             return None
+        desc, cur = got
         k, seq, _ = desc
-        cur = self._stream()
-        cur.wait_event(self.filled[k])
         if self.server_device == self.device:
             base = self.ring.slot_ptrs(k)[0][0]
             self._held = (k, seq)
@@ -751,10 +756,7 @@ class DeviceReplayClient(Stoppable, threading.Thread):
         list of ints or 0-d tensors.  An unprioritized kind (IMPALA) has no write-back."""
         if not self.kind.prioritized:
             raise TypeError(f"the {self.kind.name} replay is uniform: it has no priorities to write back")
-        if isinstance(idx, (list, tuple)):
-            idx = torch.stack([torch.as_tensor(i) for i in idx]) if len(idx) and torch.is_tensor(idx[0]) \
-                else torch.as_tensor(np.asarray(idx, np.int64))
-        idx = torch.as_tensor(idx).to(device=self.device, dtype=torch.int64).reshape(-1).contiguous()
+        idx = _index_tensor(idx).to(device=self.device, dtype=torch.int64).reshape(-1).contiguous()
         vals = torch.as_tensor(vals).to(device=self.device, dtype=torch.float32).reshape(-1).contiguous()
         assert idx.numel() == vals.numel()
         B = self.ring.layout.batch

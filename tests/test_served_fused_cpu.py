@@ -74,11 +74,11 @@ def _client(rs, conn, log, B=4, slots=2, same_gpu=True):
 
 
 def _learner(client, log, conn, rs, B=4):
-    """An apex.Learner reduced to what _served_fused_step touches; its step is logged with the RELEASE_SLOT count
-    at the time the step is enqueued."""
+    """An apex.Learner reduced to what _next_step touches on a served memory; its step is logged with the RELEASE_SLOT
+    count at the time the step is enqueued."""
     from distributed_rl_b200 import apex
     L = object.__new__(apex.Learner)
-    L.cfg = apex.ApexConfig(BATCHSIZE=B, SERVED_FUSED_STEP=True)
+    L.cfg, L._served = apex.ApexConfig(BATCHSIZE=B, SERVED_FUSED_STEP=True), True
     L.memory, L._fused = client, SimpleNamespace(cur={}, frames={})
     prio = torch.arange(B, dtype=torch.float32)
 
@@ -96,7 +96,7 @@ def test_the_slot_is_released_after_the_step_and_the_eviction_step_skips_its_wri
     srv.fill_free(lambda k, seq: None)
     c = _client(rs, conn, log)
     L = _learner(c, log, conn, rs)
-    assert L._served_fused_step(1, 2) is not None
+    assert L._next_step(1, 2) is not None
     # filled[0] is waited on before the bind; the step runs while slot 0 is still held; released[0] is recorded
     # behind the step, then RELEASE_SLOT hands the slot back; then the write-back goes to update slot 0
     assert log == [("wait", "filled0"), ("bind", 1000), ("step", 0), ("record", "released0"),
@@ -105,12 +105,12 @@ def test_the_slot_is_released_after_the_step_and_the_eviction_step_skips_its_wri
     assert [pickle.loads(d) for d in conn.lrange(rs.RELEASE_SLOT, 0, -1)] == [(0, 1)]
     assert conn.llen(rs.UPDATE_SLOT) == 1
     del log[:]
-    assert L._served_fused_step(2, 2) is not None          # step 2 % log_every == 0: the eviction request
+    assert L._next_step(2, 2) is not None                  # step 2 % log_every == 0: the eviction request
     assert log == [("wait", "filled1"), ("bind", 2000), ("step", 1), ("record", "released1")]
     assert conn.llen(rs.UPDATE_SLOT) == 1                   # no write-back for this step
     assert c.lock is True and conn.get("FLAG_REMOVE") is None
     assert [pickle.loads(d) for d in conn.lrange(rs.RELEASE_SLOT, 0, -1)] == [(0, 1), (1, 2)]
-    assert L._served_fused_step(3, 2) is None               # nothing filled; the poll raised the server's flag
+    assert L._next_step(3, 2) is None                       # nothing filled; the poll raised the server's flag
     assert pickle.loads(conn.get("FLAG_REMOVE")) is True and c.lock is False
     assert srv.collect_releases(lambda k: None) == 2 and sorted(srv.free) == [0, 1]
 
@@ -121,11 +121,11 @@ def test_a_slot_from_another_gpu_is_staged_and_released_before_the_step(rs):
     c = _client(rs, conn, log, same_gpu=False)
     c._stage = torch.empty(8, dtype=torch.uint8)           # the persistent local copy (allocated on first use)
     L = _learner(c, log, conn, rs)
-    L._served_fused_step(1, 100)
+    L._next_step(1, 100)
     stage = c._stage.data_ptr()
     assert log[:5] == [("wait", "filled0"), ("take", 0), ("record", "released0"), ("bind", stage), ("step", 1)]
     c2 = c._stage
-    L._served_fused_step(2, 100)
+    L._next_step(2, 100)
     assert c._stage is c2                                   # one buffer for every step
     assert [pickle.loads(d) for d in conn.lrange(rs.RELEASE_SLOT, 0, -1)] == [(0, 1), (1, 2)]
 

@@ -174,7 +174,7 @@ def _served_arm(kind, args):
 
             def step():                  # the eviction request never comes: every step writes back
                 count[0] += 1
-                while L._served_fused_step(count[0], 1 << 62) is None:
+                while L._next_step(count[0], 1 << 62) is None:
                     time.sleep(0.0001)
         n = args["redis_steps"] if kind == "redis" else args["steps"]
         served = _timed(serve_only, n, args["warmup"], dev)
