@@ -25,11 +25,10 @@ from dataclasses import dataclass, field
 import numpy as np
 import torch
 
-from . import _lib
 from . import replay as R
 from .agent import GraphAgent
 from .learner_common import (Conv1Gathered as _Conv1Gathered, MemoryView, ReplayThread, TargetNetLearner,
-                             _attach_replay, conv1_packs, make_optimizer)
+                             _attach_replay, check_served_fused, conv1_packs, make_optimizer)
 
 
 @dataclass
@@ -274,7 +273,7 @@ class Learner(TargetNetLearner):
         slot `memory.acquire()` binds (same cadence): see _next_step."""
         self.cfg = cfg or ApexConfig.from_configuration()
         if memory is not None and self.cfg.SERVED_FUSED_STEP:
-            self._check_served_fused(memory)
+            check_served_fused(self.cfg, memory)
         self.device = torch.device(self.cfg.LEARNER_DEVICE)
         if self.cfg.CUDNN_BENCHMARK and self.device.type == "cuda":
             torch.backends.cudnn.benchmark = True
@@ -590,24 +589,24 @@ class Learner(TargetNetLearner):
 
         if self._world > 1 and self._max_w_use is None:      # first step: reduce synchronously once
             self._max_w_use = self._D.all_reduce_max_(st.max_weight(self.cfg.BETA)).clone()
+        # The step is warmed up and captured on its HIGH-priority main stream (kernel nodes inherit it): the side
+        # branches (weight gradients, early optimizer step, operand packs) only fill SMs the critical chain leaves idle.
         if not use_graph:
-            return self._eager_or_captured(body, False)
+            return self._eager_or_captured(body, False, s.main)
         self.optim.zero_grad(set_to_none=False)
         # The ingest thread keeps pushing on the same replay handle: hold its lock so that no cudaMalloc /
         # cudaHostAlloc / copy of that thread lands inside the warm-up or the (global-mode) capture.
         with self.memory._lock:
-            self._warm_up(body, 3)
-            return self._eager_or_captured(body, True)
-
-    BOUND_WARMUP = 3       # eager steps on served minibatches before the bound step is captured
+            self._warm_up(body, 3, s.main)
+            return self._eager_or_captured(body, True, s.main)
 
     def _bound_step(self, use_graph: bool = True):
         """One step on the served minibatch `memory.acquire(cur, frames)` bound: fused_step's graph, with the draw
         (sample_fetch) and the in-graph tree update replaced by reads of the bound buffers; the priorities leave
-        through memory.update() after the step.  The first BOUND_WARMUP calls run the step eagerly on the main stream
-        (lazy inits stay outside the capture), each on its own minibatch; the next call captures the graph, and every
-        call replays it.  The caller releases the slot after this returns: the replay is then enqueued."""
-        c = self._fused_state().cur
+        through memory.update() after the step.  Warm-up, capture and replay: CapturedStep._served_step, on the main
+        stream."""
+        s = self._fused_state()
+        c = s.cur
         batched = self.cfg.PARALLEL_FORWARDS and self.cfg.BATCHED_ONLINE   # the batched pass converts the action
 
         def body():
@@ -617,49 +616,9 @@ class Learner(TargetNetLearner):
             info = self.step()
             return {"scalars": out["scalars"], "p_norm": info["p_norm"], "prio": out["prio"], "idx": c["idx"]}
 
-        if use_graph and self._bound_warm < self.BOUND_WARMUP:
-            if self._bound_warm == 0:
-                self.optim.zero_grad(set_to_none=False)
-            self._bound_warm += 1
-            return self._warm_up(body, 1)
-        return self._eager_or_captured(body, use_graph)
-
-    # The two callers warm up before the capture differently, on purpose.  fused_step draws its own minibatches, so
-    # its first call runs all three warm-ups and the capture, under the replay's lock (bench.py's warm-up loop counts
-    # on "3 eager warm-ups + capture" in the first call).  A bound step needs a new served slot for each warm-up, so
-    # _bound_step warms up over three calls and captures on the fourth.
-    def _eager_or_captured(self, body, use_graph: bool):
-        """`body` (one step) run eagerly, its libb2rl launches counted into `launches_per_step`; or, with
-        `use_graph`, captured into `_graph`, whose launches are counted the same way, and replayed: every later
-        fused_step replays it.  -> the step's outputs (for the graph: `_static`, its static output buffers)."""
-        lib = _lib.load()
-        if not use_graph:
-            c0 = lib.b2rl_launch_count()
-            r = body()
-            self.launches_per_step = lib.b2rl_launch_count() - c0
-            return r
-        torch.cuda.synchronize(self.device)
-        g = torch.cuda.CUDAGraph()
-        c0 = lib.b2rl_launch_count()
-        # The step's main branch is captured on a HIGH-priority stream (kernel nodes inherit it): the side branches
-        # (weight gradients, early optimizer step, operand packs) only fill SMs the critical chain leaves idle.
-        with torch.cuda.graph(g, stream=self._fused.main):
-            self._static = body()
-        self.launches_per_step = lib.b2rl_launch_count() - c0   # recorded into the graph, replayed each step
-        self._graph = g
-        g.replay()
-        return self._static
-
-    def _warm_up(self, body, n: int):
-        """`n` eager runs of `body` on the step's main stream, so that lazy inits (cuDNN plans, optimizer state)
-        happen outside the capture.  -> what the last one returned."""
-        cur, main = torch.cuda.current_stream(self.device), self._fused.main
-        main.wait_stream(cur)
-        with torch.cuda.stream(main):
-            for _ in range(n):
-                r = body()
-        cur.wait_stream(main)
-        return r
+        if use_graph and self._bound_warm == 0:
+            self.optim.zero_grad(set_to_none=False)
+        return self._served_step(body, use_graph, s.main)
 
     # -- one step of run() ---------------------------------------------------------------------------
     def _next_step(self, step: int, log_every: int):
@@ -690,14 +649,3 @@ class Learner(TargetNetLearner):
         self._write_back(step, log_every, idx, prio)
         return tot
 
-    def _check_served_fused(self, memory) -> None:
-        """What SERVED_FUSED_STEP needs, checked before anything is built."""
-        if not self.cfg.FUSED_CONV1:
-            raise ValueError("SERVED_FUSED_STEP reads the frames in the ring slot with the fused conv_1 kernels: it "
-                             "needs FUSED_CONV1")
-        if not (hasattr(memory, "acquire") and hasattr(memory, "release")):
-            raise TypeError("SERVED_FUSED_STEP needs a served memory that binds ring slots (DeviceReplayClient)")
-        batch = memory.ring.layout.batch
-        if batch != self.cfg.BATCHSIZE:
-            raise ValueError(f"the server's ring holds minibatches of {batch}; the step graph is built for "
-                             f"BATCHSIZE = {self.cfg.BATCHSIZE}")

@@ -12,8 +12,8 @@ import torch
 
 from . import replay as R
 from .agent import GraphAgent
-from .learner_common import (Conv1Gathered, ReplayThread, _attach_replay, conv1_packs, make_optimizer, publishers,
-                             time_major_rows)
+from .learner_common import (CapturedStep, Conv1Gathered, ReplayThread, _attach_replay, check_served_fused,
+                             conv1_packs, make_optimizer, publishers, time_major_rows)
 from .publish import ParamPublisher
 
 
@@ -47,6 +47,8 @@ class ImpalaConfig:
     MODEL: dict = field(default_factory=default_impala_model)
     FUSED_CONV1: bool = True     # conv_1 (4 -> 16 channels) of every frame through libb2rl's wgmma kernel
     DENSE_3XTF32: bool = True    # the 2592 -> 256 layer as a 3xTF32 wgmma GEMM (csrc/gemm.cu) instead of an fp32 SIMT sgemm
+    SERVED_FUSED_STEP: bool = False  # on a served replay (DeviceReplayClient), run() steps a captured step on the
+                                     # bound ring slot instead of sample() -> train()
 
     @staticmethod
     def from_configuration():
@@ -110,12 +112,15 @@ class Replay(ReplayThread):
         return len(self.store)
 
 
-class Learner:
+class Learner(CapturedStep):
     def __init__(self, cfg: ImpalaConfig | None = None, connect=None, start_replay: bool = True, memory=None):
         """`memory`: a replay served from another process (replay_server.DeviceReplayClient built with this
         ImpalaConfig, or anything with its surface: sample / memory).  run() then drives sample() -> train() on it;
-        fused_step() needs the in-process Replay."""
+        with SERVED_FUSED_STEP it steps on the slot `memory.acquire()` binds instead (see _next_step).  fused_step()
+        needs the in-process Replay."""
         self.cfg = cfg or ImpalaConfig.from_configuration()
+        if memory is not None and self.cfg.SERVED_FUSED_STEP:
+            check_served_fused(self.cfg, memory, R.impala_fields(self.cfg.UNROLL_STEP))
         self.device = torch.device(self.cfg.LEARNER_DEVICE)
         self.model = GraphAgent(self.cfg.MODEL).to(self.device)
         self.model.dense_3xtf32 = bool(self.cfg.DENSE_3XTF32) and self.device.type == "cuda"
@@ -124,6 +129,10 @@ class Learner:
         self._memory = _attach_replay(self, memory, lambda: Replay(self.cfg, connect), connect, start_replay,
                                       wipe=False)
         self.last = {}
+        self._graph = self._static = None
+        self._bound = None              # _BoundRollouts, built by the first bound step
+        self._bound_warm = 0            # eager warm-up steps on served slots
+        self.launches_per_step = None
 
     @property
     def memory(self):
@@ -173,9 +182,32 @@ class Learner:
                          b["reward"].t().contiguous(), b["done"], step)
         return self.last
 
-    def _train_core(self, frames, rows, action, mu, reward, done, step):
+    def _bound_state(self) -> "_BoundRollouts":
+        if self._bound is None:
+            self._bound = _BoundRollouts(self)
+        return self._bound
+
+    def _bound_step(self, use_graph: bool = True):
+        """One step on the served rollouts `memory.acquire(cur, frames)` bound (SERVED_FUSED_STEP): _train_core with
+        conv_1 and its weight gradient reading the slot's time-major frames through the frame table and a / mu / r /
+        done read from the bound buffers.  Warm-up, capture and replay: CapturedStep._served_step.
+        -> `last` (for the graph: its static buffers)."""
+        s = self._bound_state()
+        c = s.cur
+
+        def body():
+            self._train_core(s.frames["state"], None, c["action"], c["mu"], c["reward"], c["done"], 0,
+                             seq_frames=s.seq_frames)
+            return self.last
+
+        self.last = self._served_step(body, use_graph, s.stream)
+        return self.last
+
+    def _train_core(self, frames, rows, action, mu, reward, done, step, seq_frames=None):
         """IMPALA/Learner.py:121-235 on a uint8 frame table read in place (`rows`: time-major frame rows, None =
-        all rows in order) or, with rows == "staged", on a staged (T+1, B, 28224) batch through PyTorch's conv_1."""
+        all rows in order) or, with rows == "staged", on a staged (T+1, B, 28224) batch through PyTorch's conv_1.
+        `seq_frames`: with rows None and `frames` a bound ring slot (R.BoundFrames), the same slot's first T * B
+        rows, which the grad pass reads (a BoundFrames cannot be sliced)."""
         c = self.cfg
         T, B, A = c.UNROLL_STEP, c.BATCHSIZE, c.ACTION_SIZE
         dev = self.device
@@ -205,7 +237,8 @@ class Learner:
                                c.GAMMA, c.C_LAMBDA, c.C_VALUE, c.P_VALUE)       # :151-215 in one launch
         # calLoss (:95-119): second forward with grad (conv_1's output is reused: same weights, same frames)
         if fused:
-            seq_frames = frames[:T * B] if rows is None else frames
+            if seq_frames is None:
+                seq_frames = frames[:T * B] if rows is None else frames
             seq_rows = None if rows is None else rows[:T * B]
             y = Conv1Gathered.apply(w1, seq_frames, seq_rows, self._pack1, torch.contiguous_format, None, y_seq)
             out = self.model.forward_from_conv1(y, False)[0]
@@ -242,11 +275,9 @@ class Learner:
         self._publishers, ckpt = publishers(self.model, self.cfg.LOG_W, pub)
         t = 0
         while max_steps is None or t < max_steps:
-            tr = self._memory.sample()
-            if tr is False:
+            if not self._next_step(t):
                 time.sleep(0.2)
                 continue
-            self.train(tr, t)
             pub.snapshot(t)
             if ckpt is not None and (t + 1) % 100 == 0:
                 ckpt.snapshot(t)
@@ -254,3 +285,47 @@ class Learner:
                 p.poll()
             t += 1
         return t
+
+    def _next_step(self, t: int) -> bool:
+        """One step of run(): sample() -> train(); or, with SERVED_FUSED_STEP on a served memory, bind the oldest
+        filled slot (memory.acquire), run the bound step on it and hand the slot back once the step is enqueued
+        (memory.release: conv_1's weight gradient, in backward, is its last reader).  Uniform replay: nothing is
+        written back.  -> False when no minibatch is ready (nothing ran)."""
+        if self._served and self.cfg.SERVED_FUSED_STEP:
+            s = self._bound_state()
+            if self._memory.acquire(s.cur, s.frames) is None:
+                return False
+            self._bound_step()
+            self._memory.release()
+            return True
+        tr = self._memory.sample()
+        if tr is False:
+            return False
+        self.train(tr, t)
+        return True
+
+
+class _BoundRollouts:
+    """The buffers a served rollout slot is bound to, built once before the first warm-up, and the stream the bound
+    step is warmed up and captured on.  memory.acquire() copies the slot's header, idx, w, action / mu / reward
+    (T, B) and done (B,) into `cur` and writes the address of its `state` rows into the one-entry `table`.  The
+    server writes the slot time-major (b2rl_serve_fill_uniform), so `state` is conv_1's frame table as it lies:
+    (T+1) * B rows in order, no index array.  The grad pass reads its first T * B rows: `seq_frames`, the same table
+    entry with fewer rows."""
+
+    def __init__(self, L: "Learner"):
+        c, dev = L.cfg, L.device
+        T, B = c.UNROLL_STEP, c.BATCHSIZE
+        if L.model.first_conv_node() is None:
+            raise ValueError("SERVED_FUSED_STEP reads the ring slot's frames with the fused conv_1 kernels: the "
+                             "model's first node must be the Atari conv_1")
+        self.stream = torch.cuda.Stream(dev)
+        f = {x.name: x for x in R.impala_fields(T)}
+        self.cur = {name: torch.empty((T, B), dtype=f[name].dtype, device=dev) for name in ("action", "mu", "reward")}
+        self.cur.update(done=torch.empty(B, dtype=f["done"].dtype, device=dev),
+                        idx=torch.empty(B, dtype=torch.int64, device=dev),
+                        w=torch.empty(B, dtype=torch.float32, device=dev),
+                        header=torch.zeros(2, dtype=torch.int64, device=dev))
+        self.table = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.frames = {"state": R.BoundFrames(self.table, 0, (T + 1) * B)}
+        self.seq_frames = R.BoundFrames(self.table, 0, T * B)

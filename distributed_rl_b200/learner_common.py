@@ -1,7 +1,8 @@
 """What the Ape-X, R2D2 and IMPALA learner sides share: the optimiser factory, the replay ingest thread and the
-learner's replay set-up, the conv_1 autograd function and its packs, the time-major frame-row layout, and the
-Ape-X / R2D2 `Learner.run` loop with its write-back cadence (start handshake, publishers, periodic log).  Each
-learner keeps its own store layout, batch assembly and step body."""
+learner's replay set-up, the conv_1 autograd function and its packs, the time-major frame-row layout, the checks
+and the warm-up / capture / replay of a captured step (`CapturedStep`), and the Ape-X / R2D2 `Learner.run` loop with
+its write-back cadence (start handshake, publishers, periodic log).  Each learner keeps its own store layout, batch
+assembly and step body."""
 from __future__ import annotations
 
 import pickle
@@ -11,6 +12,7 @@ import time
 import numpy as np
 import torch
 
+from . import _lib
 from . import replay as R
 from . import wire
 from .publish import ParamPublisher
@@ -234,7 +236,82 @@ def publishers(model, log_w, *pubs):
     return pubs + ((ckpt,) if ckpt else ()), ckpt
 
 
-class TargetNetLearner:
+def check_served_fused(cfg, memory, fields=None) -> None:
+    """What SERVED_FUSED_STEP needs, checked before the learner builds anything: FUSED_CONV1 (conv_1 reads the ring
+    slot's frames through the frame table), a memory that binds ring slots (DeviceReplayClient.acquire / release), a
+    ring whose minibatches hold BATCHSIZE records and, when `fields` is given, a ring that carries those fields."""
+    if not cfg.FUSED_CONV1:
+        raise ValueError("SERVED_FUSED_STEP reads the frames in the ring slot with the fused conv_1 kernels: it "
+                         "needs FUSED_CONV1")
+    if not (hasattr(memory, "acquire") and hasattr(memory, "release")):
+        raise TypeError("SERVED_FUSED_STEP needs a served memory that binds ring slots (DeviceReplayClient)")
+    L = memory.ring.layout
+    if L.batch != cfg.BATCHSIZE:
+        raise ValueError(f"the server's ring holds minibatches of {L.batch}; the step graph is built for "
+                         f"BATCHSIZE = {cfg.BATCHSIZE}")
+    if fields is not None and [int(L.field_bytes[i]) for i in range(L.n_fields)] != [f.nbytes for f in fields]:
+        raise ValueError("the server's ring does not carry this config's record fields (field sizes "
+                         f"{[int(L.field_bytes[i]) for i in range(L.n_fields)]}, expected "
+                         f"{[f.nbytes for f in fields]})")
+
+
+class CapturedStep:
+    """One learner step run eagerly or as a CUDA graph, on a stream of the learner's (Ape-X: the step's
+    high-priority main stream; R2D2 / IMPALA: one stream of the step state).  Sets `_graph`, `_static` (the graph's
+    output buffers), `_bound_warm` and `launches_per_step`; the learner initialises them to None, None, 0, None.
+
+    The callers warm up before the capture in two ways, on purpose.  A step that draws its own minibatch (the
+    in-process `fused_step`) runs its three warm-ups and the capture in its first call, under the replay's lock
+    (bench.py's warm-up loop counts on "3 eager warm-ups + capture" in the first call).  A step on a served ring slot
+    needs a new slot for each warm-up, so `_served_step` warms up over BOUND_WARMUP calls and captures on the next."""
+
+    BOUND_WARMUP = 3       # eager steps on served minibatches before the bound step is captured
+
+    def _served_step(self, body, use_graph: bool, stream):
+        """One step on the slot `memory.acquire()` bound: the first BOUND_WARMUP calls run `body` eagerly on `stream`
+        (lazy inits stay outside the capture), each on its own minibatch; the next call captures it; every later call
+        replays the graph.  The caller releases the slot after this returns: the step is then enqueued."""
+        if self._graph is not None:
+            self._graph.replay()
+            return self._static
+        if use_graph and self._bound_warm < self.BOUND_WARMUP:
+            self._bound_warm += 1
+            return self._warm_up(body, 1, stream)
+        return self._eager_or_captured(body, use_graph, stream)
+
+    def _eager_or_captured(self, body, use_graph: bool, stream):
+        """`body` (one step) run eagerly, its libb2rl launches counted into `launches_per_step`; or, with
+        `use_graph`, captured on `stream` into `_graph`, whose launches are counted the same way, and replayed: every
+        later step replays it.  -> the step's outputs (for the graph: `_static`, its static output buffers)."""
+        lib = _lib.load()
+        if not use_graph:
+            c0 = lib.b2rl_launch_count()
+            r = body()
+            self.launches_per_step = lib.b2rl_launch_count() - c0
+            return r
+        torch.cuda.synchronize(self.device)
+        g = torch.cuda.CUDAGraph()
+        c0 = lib.b2rl_launch_count()
+        with torch.cuda.graph(g, stream=stream):
+            self._static = body()
+        self.launches_per_step = lib.b2rl_launch_count() - c0   # recorded into the graph, replayed each step
+        self._graph = g
+        g.replay()
+        return self._static
+
+    def _warm_up(self, body, n: int, stream):
+        """`n` eager runs of `body` on `stream`, so that lazy inits (cuDNN plans, optimizer state, workspaces)
+        happen outside the capture.  -> what the last one returned."""
+        cur = torch.cuda.current_stream(self.device)
+        stream.wait_stream(cur)
+        with torch.cuda.stream(stream):
+            for _ in range(n):
+                r = body()
+        cur.wait_stream(stream)
+        return r
+
+
+class TargetNetLearner(CapturedStep):
     """The parts of `Learner` that Ape-X and R2D2 share (online + target network, run loop, write-back cadence,
     `Start` handshake, periodic log).  Uses the learner's `cfg`, `model`, `target_model`, `memory`, `_served`,
     `connect` and `writer`.  A learner provides `_next_step(step, log_every)` and sets `LOG_LINE`, its log line

@@ -16,8 +16,8 @@ import torch
 
 from . import replay as R
 from .agent import GraphAgent
-from .learner_common import (Conv1Gathered, MemoryView, ReplayThread, TargetNetLearner, _attach_replay, conv1_packs,
-                             make_optimizer, time_major_rows)
+from .learner_common import (Conv1Gathered, MemoryView, ReplayThread, TargetNetLearner, _attach_replay,
+                             check_served_fused, conv1_packs, make_optimizer, time_major_rows)
 
 
 def default_r2d2_model() -> dict:
@@ -64,6 +64,8 @@ class R2D2Config:
                                  #      does not fit HBM; SURVEY §8d C3).  Benchmark-only; ingest needs 0.
     FUSED_CONV1: bool = True     # conv_1 of every frame through libb2rl's wgmma kernel (gather fused)
     FUSED_HEADS: bool = True     # dueling heads: 3xTF32 wgmma GEMM + fused tail kernels (csrc/gemm.cu, csrc/dueling.cu)
+    SERVED_FUSED_STEP: bool = False  # on a served replay (DeviceReplayClient), run() steps a captured step on the
+                                     # bound ring slot instead of sample() -> train() -> update()
 
     @staticmethod
     def from_configuration():
@@ -131,8 +133,12 @@ class Learner(TargetNetLearner):
                  memory=None):
         """`memory`: a replay served from another process (replay_server.DeviceReplayClient or Replay_Server built
         with this R2D2Config, or anything with the `Replay` surface: sample / update / lock / memory).  run() drives
-        sample() -> train() -> update() either way; a served memory passes the eviction request on to its server."""
+        sample() -> train() -> update() either way; a served memory passes the eviction request on to its server.
+        With SERVED_FUSED_STEP, run() over a served memory steps on the slot `memory.acquire()` binds instead (same
+        cadence): see _next_step."""
         self.cfg = cfg or R2D2Config.from_configuration()
+        if memory is not None and self.cfg.SERVED_FUSED_STEP:
+            check_served_fused(self.cfg, memory, R.r2d2_fields(self.cfg.FIXED_TRAJECTORY))
         self.device = torch.device(self.cfg.LEARNER_DEVICE)
         self.model = GraphAgent(self.cfg.MODEL).to(self.device)
         self.target_model = GraphAgent(self.cfg.MODEL).to(self.device)
@@ -142,6 +148,10 @@ class Learner(TargetNetLearner):
         self.connect = connect
         self.memory = _attach_replay(self, memory, lambda: Replay(self.cfg, connect), connect, start_replay, wipe=True)
         self.writer = writer
+        self._graph = self._static = None
+        self._step_state = None         # _StepState, built by the first captured or bound step
+        self._bound_warm = 0            # eager warm-up steps on served slots
+        self.launches_per_step = None
 
     def train(self, transition, t=0):
         c = self.cfg
@@ -173,16 +183,24 @@ class Learner(TargetNetLearner):
             q = self.model.forward([window, shape])[0].view(L, B, A)              # :121
             with torch.no_grad():
                 q_target = self.target_model.forward([window, shape])[0].view(L, B, A)   # :132
+        out, info = self._learn(q, q_target, action, reward, notdone, weight)
+        info["mean_value"] = out["scalars"][1]
+        info["loss"] = out["scalars"][0]
+        return info, out["prio"], idx
+
+    def _learn(self, q, q_target, action, reward, notdone, weight):
+        """The step after the forward passes (R2D2/Learner.py:110-215): the window's actions / rewards, target and
+        priority kernel, backward, then step().  `action`, `reward`: (B, T); `notdone`, `weight`: (B,).
+        -> (the target kernel's outputs, step()'s info)"""
+        c, dev = self.cfg, self.device
+        MEM = c.MEM
         act = torch.as_tensor(action).to(dev, torch.int64).t()[MEM:-1].contiguous()      # (L-1, B)
         rew = torch.as_tensor(reward).to(dev, torch.float32).t()[MEM:-1].contiguous()
         nd = torch.as_tensor(notdone).to(dev, torch.float32).contiguous()
         out = R.r2d2_target(q.detach().contiguous(), q_target.contiguous(), act, rew, nd, weight,
                             c.UNROLL_STEP, c.GAMMA, c.ALPHA, c.USE_RESCALING)
         q.backward(out["grad_q"])                               # == loss.backward(), :189-192
-        info = self.step()
-        info["mean_value"] = out["scalars"][1]
-        info["loss"] = out["scalars"][0]
-        return info, out["prio"], idx
+        return out, self.step()
 
     def _time_major_rows(self, seq_rows, T, B):
         """Frame-table rows of the (t, b) frames in time-major order: row = seq_row[b] * T + t
@@ -220,11 +238,19 @@ class Learner(TargetNetLearner):
             q_target = self.target_model.forward_from_conv1(torch.relu(y_tg_w), True, [shape])[0].view(L, B, A)
         return q, q_target
 
-    def fused_step(self):
+    def fused_step(self, use_graph: bool = False):
         """One learner step with everything resident: sample B sequence slots + IS weights from the sum-tree,
         gather only the small per-sequence fields (a, r, h0, h1, notdone: 5 KB of the 2.26 MB), run conv_1 over the
         sequences' frames IN PLACE in the replay payload (row = slot_row * T + t), target / priority kernel,
-        backward, clip + Adam, priority write-back.  No host round trip (R2D2/Learner.py:235-274 in one call)."""
+        backward, clip + Adam, priority write-back.  No host round trip (R2D2/Learner.py:235-274 in one call).
+        `use_graph`: the first call runs three eager warm-ups and captures the step as a CUDA graph (under the
+        replay's lock, so that no ingest work lands in the capture); every later call replays it.  The draw reads
+        the tree's device-resident size and Philox counter, so each replay draws a new minibatch."""
+        if self._graph is not None:
+            self._graph.replay()
+            return self._static
+        if self._served:
+            raise RuntimeError("fused_step() samples the learner's own replay; a served replay is driven by run()")
         c = self.cfg
         T, MEM, B, A = c.FIXED_TRAJECTORY, c.MEM, c.BATCHSIZE, c.ACTION_SIZE
         mem = self.memory
@@ -232,21 +258,50 @@ class Learner(TargetNetLearner):
         if not hasattr(self, "_small"):
             self._small = pool.alloc_batch(B, ("action", "reward", "h0", "h1", "notdone"))
             self._frames = pool.field_view("state").view(-1, 4, 84, 84)
-        idx, _, w = st.sample(B, beta=c.BETA, want_prob=False)
-        rows = mem.rows_of(idx)
-        b = pool.gather(rows, self._small)
-        h0, h1 = b["h0"].unsqueeze(0), b["h1"].unsqueeze(0)
-        self.model.setCellState((h0, h1))
-        self.target_model.setCellState((h0, h1))
-        q, q_target = self._forward_fused(self._frames, self._time_major_rows(rows, T, B), T, MEM, B, A)
-        act = b["action"].to(torch.int64).t()[MEM:-1].contiguous()
-        rew = b["reward"].t()[MEM:-1].contiguous()
-        out = R.r2d2_target(q.detach().contiguous(), q_target.contiguous(), act, rew, b["notdone"], w,
-                            c.UNROLL_STEP, c.GAMMA, c.ALPHA, c.USE_RESCALING)
-        q.backward(out["grad_q"])
-        info = self.step()
-        st.update(idx, out["prio"])
-        return {"scalars": out["scalars"], "p_norm": info["p_norm"], "prio": out["prio"], "idx": idx}
+
+        def body():
+            idx, _, w = st.sample(B, beta=c.BETA, want_prob=False)
+            rows = mem.rows_of(idx)
+            b = pool.gather(rows, self._small)
+            h0, h1 = b["h0"].unsqueeze(0), b["h1"].unsqueeze(0)
+            self.model.setCellState((h0, h1))
+            self.target_model.setCellState((h0, h1))
+            q, q_target = self._forward_fused(self._frames, self._time_major_rows(rows, T, B), T, MEM, B, A)
+            out, info = self._learn(q, q_target, b["action"], b["reward"], b["notdone"], w)
+            st.update(idx, out["prio"])
+            return {"scalars": out["scalars"], "p_norm": info["p_norm"], "prio": out["prio"], "idx": idx}
+
+        if not use_graph:
+            return body()
+        stream = self._state().stream
+        with mem._lock:
+            self._warm_up(body, 3, stream)
+            return self._eager_or_captured(body, True, stream)
+
+    def _state(self) -> "_StepState":
+        if self._step_state is None:
+            self._step_state = _StepState(self)
+        return self._step_state
+
+    def _bound_step(self, use_graph: bool = True):
+        """One step on the served minibatch `memory.acquire(cur, frames)` bound (SERVED_FUSED_STEP): fused_step's
+        body with the draw, the small-field gather and the tree update replaced by the bound buffers; conv_1 of the
+        burn-in, of the window and its weight gradient read the slot's frames through the frame table.  The
+        priorities leave through memory.update() after the step.  Warm-up, capture and replay:
+        CapturedStep._served_step."""
+        s = self._state()
+        c, cur = self.cfg, s.cur
+        T, MEM, B, A = c.FIXED_TRAJECTORY, c.MEM, c.BATCHSIZE, c.ACTION_SIZE
+        h0, h1 = cur["h0"].unsqueeze(0), cur["h1"].unsqueeze(0)
+
+        def body():
+            self.model.setCellState((h0, h1))
+            self.target_model.setCellState((h0, h1))
+            q, q_target = self._forward_fused(s.frames["state"], s.rows, T, MEM, B, A)
+            out, info = self._learn(q, q_target, cur["action"], cur["reward"], cur["notdone"], cur["w"])
+            return {"scalars": out["scalars"], "p_norm": info["p_norm"], "prio": out["prio"], "idx": cur["idx"]}
+
+        return self._served_step(body, use_graph, s.stream)
 
     def step(self):
         """R2D2/Learner.py:200-215: norm, clip at 40, Adam."""
@@ -259,11 +314,48 @@ class Learner(TargetNetLearner):
         return {"p_norm": p_norm}
 
     def _next_step(self, step: int, log_every: int):
-        """One iteration of run() (R2D2/Learner.py:240-274): sample -> train -> the write-back cadence.
+        """One iteration of run() (R2D2/Learner.py:240-274): sample -> train -> the write-back cadence.  With
+        SERVED_FUSED_STEP on a served memory, the oldest filled slot is bound (memory.acquire), the bound step runs
+        on it and the slot is handed back once the step is enqueued (memory.release: conv_1's weight gradient, in
+        backward, is its last reader); then the write-back.
         -> {mean(Q), norm} as a device tensor, or None when no minibatch is ready."""
+        if self._served and self.cfg.SERVED_FUSED_STEP:
+            s = self._state()
+            if self.memory.acquire(s.cur, s.frames) is None:
+                return None
+            out = self._bound_step()
+            self.memory.release()
+            self._write_back(step, log_every, out["idx"], out["prio"])
+            return torch.stack([out["scalars"][1].reshape(()), out["p_norm"].reshape(())])
         batch = self.memory.sample()
         if batch is False:
             return None
         info, prio, idx = self.train(batch)
         self._write_back(step, log_every, idx, prio)
         return torch.stack([info["mean_value"].reshape(()), info["p_norm"].reshape(())])
+
+
+class _StepState:
+    """What a captured R2D2 step keeps from one step to the next, built once before its first warm-up: the stream it
+    is warmed up and captured on and, on a served memory, the buffers a ring slot is bound to.  memory.acquire()
+    copies the slot's header, idx, w, action (B, T), reward (B, T), h0, h1 (B, 512) and notdone (B,) into `cur` and
+    writes the address of its `state` rows into the one-entry `table`.  The slot's `state` is batch-major
+    (B, T, 4, 84, 84), so frame (b, t) is row b * T + t from that address, and `rows` (the time-major order the
+    burn-in and the window read, split at MEM * B by _forward_fused) stays the same for every slot."""
+
+    def __init__(self, L: "Learner"):
+        c, dev = L.cfg, L.device
+        T, B = c.FIXED_TRAJECTORY, c.BATCHSIZE
+        self.stream = torch.cuda.Stream(dev)
+        self.cur = self.frames = self.rows = None
+        if L._served:
+            if L.model.first_conv_node() is None:
+                raise ValueError("SERVED_FUSED_STEP reads the ring slot's frames with the fused conv_1 kernels: the "
+                                 "model's first node must be the Atari conv_1")
+            self.cur = dict(R.alloc_rows(R.r2d2_fields(T), B, dev, ("action", "reward", "h0", "h1", "notdone")),
+                            idx=torch.empty(B, dtype=torch.int64, device=dev),
+                            w=torch.empty(B, dtype=torch.float32, device=dev),
+                            header=torch.zeros(2, dtype=torch.int64, device=dev))
+            self.table = torch.zeros(1, dtype=torch.int64, device=dev)
+            self.frames = {"state": R.BoundFrames(self.table, 0, B * T)}
+            self.rows = L._time_major_rows(None, T, B)

@@ -294,6 +294,28 @@ def serve_layout(batch: int, slots: int, field_bytes) -> _lib.ServeLayout:
     return L
 
 
+def bind_targets(batch: int, fields, out: dict, frames: dict):
+    """The per-field arguments of b2rl_serve_bind for a slot of `batch` records: (copy destinations, frame table
+    entries), one pointer per field, null for a field that is neither copied nor bound.  A copied field's buffer holds
+    exactly its `batch` rows.  A bound frame field holds field_bytes / FRAME_STACK_BYTES frame stacks per record
+    (Ape-X one, an R2D2 sequence T, an IMPALA rollout T + 1), so its BoundFrames must cover batch times that many
+    rows: conv_1 reads no further than the slot."""
+    fo, to = (C.c_void_p * _lib.MAX_FIELDS)(), (C.c_void_p * _lib.MAX_FIELDS)()
+    for i, f in enumerate(fields):
+        if f.name in out:
+            t = out[f.name]
+            assert t.is_contiguous() and t.numel() * t.element_size() == batch * f.nbytes, f.name
+            fo[i] = t.data_ptr()
+        elif f.name in frames:
+            stacks, rest = divmod(f.nbytes, R.FRAME_STACK_BYTES)
+            if rest or frames[f.name].rows != batch * stacks:
+                raise ValueError(f"field {f.name!r} holds {f.nbytes / R.FRAME_STACK_BYTES:g} frame stacks per record: "
+                                 f"a slot of {batch} records has {batch * f.nbytes / R.FRAME_STACK_BYTES:g} frame rows, "
+                                 f"not the {frames[f.name].rows} of its BoundFrames")
+            to[i] = frames[f.name].entry_ptr()
+    return fo, to
+
+
 class ServeRing:
     """The ring allocation as seen by this process: created for a DeviceReplay (the server owns it) or mapped from
     an exported IPC handle (the learner)."""
@@ -352,15 +374,7 @@ class ServeRing:
         step's fixed buffers: out["header"] (int64[2]), out["idx"], out["w"] and every field named in `out` are
         copied; every field named in `frames` (name -> R.BoundFrames) gets the address of its rows in the slot."""
         L = self.layout
-        fo, to = (C.c_void_p * _lib.MAX_FIELDS)(), (C.c_void_p * _lib.MAX_FIELDS)()
-        for i, f in enumerate(fields):
-            if f.name in out:
-                t = out[f.name]
-                assert t.is_contiguous() and t.numel() * t.element_size() == L.batch * f.nbytes, f.name
-                fo[i] = t.data_ptr()
-            elif f.name in frames:
-                assert frames[f.name].rows == L.batch, f.name
-                to[i] = frames[f.name].entry_ptr()
+        fo, to = bind_targets(L.batch, fields, out, frames)
         check(self.lib.b2rl_serve_bind(base, C.byref(L), L.batch, out["header"].data_ptr(), out["idx"].data_ptr(),
                                        out["w"].data_ptr(), fo, to, stream.cuda_stream))
 
@@ -713,7 +727,8 @@ class DeviceReplayClient(Stoppable, threading.Thread):
         return self.kind.batch(b, w, idx)
 
     def acquire(self, out: dict, frames: dict):
-        """sample() for a captured learner step (apex.Learner with SERVED_FUSED_STEP): the oldest filled slot is bound
+        """sample() for a captured learner step (SERVED_FUSED_STEP of apex, r2d2 or impala.Learner): the oldest filled
+        slot is bound
         to the step's fixed buffers (ServeRing.bind) on the current stream, behind filled[k]; nothing is allocated.
         `out`: header (int64[2]), idx, w and the fields to copy; `frames`: field name -> R.BoundFrames whose table
         entry receives the address of that field's rows.  With the server on this GPU the slot itself is bound and

@@ -3,17 +3,20 @@ minibatches/s and learner steps/s for
   redis   ReplayServer -> pickled `BATCH` list -> Replay_Server (host arrays, copied to the device by train());
           Ape-X and R2D2 only
   ring    DeviceReplayServer -> device serve ring (CUDA IPC) -> DeviceReplayClient
-  ring-fused  Ape-X only: the same ring, with the learner's captured fused step reading each minibatch in its ring
-          slot (ApexConfig.SERVED_FUSED_STEP: acquire -> graph replay -> release -> write-back); served
-          minibatches/s is acquire + release alone
-  fused   the in-process learner: Learner.fused_step() on its own replay (no server)
+  ring-fused  the same ring, with the learner's captured step reading each minibatch in its ring slot
+          (SERVED_FUSED_STEP: acquire -> graph replay -> release -> write-back, IMPALA without the write-back);
+          served minibatches/s is acquire + release alone
+  fused   the in-process learner: Learner.fused_step() on its own replay (no server); captured for Ape-X, eager for
+          R2D2 and IMPALA
+  fused-graph  R2D2 only: the in-process fused_step(use_graph=True), captured in its first call and replayed
   sample  IMPALA only: the in-process Replay's sample() -> Learner.train() (gather + time-major transpose per step)
   fill    b2rl_serve_fill (IMPALA: b2rl_serve_fill_uniform) alone, in this process: CUDA events around `steps` fills
           into alternating ring slots, at each batch of --fill-batches; bytes/s = 2 x slot bytes / fill time (each
           byte read once, written once)
 
     python tools/bench_serve.py [--workload apex|r2d2|impala] [--slots-store N] [--batch B] [--steps 200]
-                                [--warmup 20] [--repeats 3] [--arms redis,ring,ring-fused,fused,sample,fill]
+                                [--warmup 20] [--repeats 3]
+                                [--arms redis,ring,ring-fused,fused,fused-graph,sample,fill]
 
 Defaults per workload: Ape-X B = 512 on a 2^16-slot store (3.7 GB); R2D2 B = 64, T = 80, MEM = 20 on a 2^12-sequence
 store (9.2 GB); IMPALA B = 32, T = 20 on a 2^11-rollout store (1.2 GB).
@@ -164,7 +167,7 @@ def _served_arm(kind, args):
             info, prio, idx = L.train(b)[:3]
             client.update(idx if kind == "ring" else list(idx.tolist()), prio)
         if kind == "ring-fused":
-            s = L._fused_state()
+            s = getattr(L, {"r2d2": "_state", "impala": "_bound_state"}.get(args["workload"], "_fused_state"))()
             count = [0]
 
             def serve_only():            # the bind alone: acquire (wait on filled[k] + one k_serve_bind), release
@@ -172,8 +175,12 @@ def _served_arm(kind, args):
                     time.sleep(0.0001)
                 client.release()
 
-            def step():                  # the eviction request never comes: every step writes back
+            def step():                  # the eviction request never comes: every step writes back (not IMPALA)
                 count[0] += 1
+                if args["workload"] == "impala":
+                    while not L._next_step(count[0]):
+                        time.sleep(0.0001)
+                    return
                 while L._next_step(count[0], 1 << 62) is None:
                     time.sleep(0.0001)
         n = args["redis_steps"] if kind == "redis" else args["steps"]
@@ -196,12 +203,15 @@ def _served_arm(kind, args):
         mgr.shutdown()
 
 
-def _fused_arm(args):
+def _fused_arm(args, use_graph=False):
+    """The in-process fused_step: eager (`fused`) or, R2D2's `fused-graph`, captured in the first call and replayed
+    (the warm-up calls include the three eager warm-ups and the capture)."""
     import torch
     cfg = _cfg(args, "cuda:0")
     L = _learner(args, cfg)
     _fill(L.memory.store, args["store"])
-    rate = _timed(L.fused_step, args["steps"], args["warmup"], torch.device("cuda:0"))
+    fn = (lambda: L.fused_step(use_graph=True)) if use_graph else L.fused_step
+    rate = _timed(fn, args["steps"], args["warmup"], torch.device("cuda:0"))
     del L
     torch.cuda.empty_cache()
     return {"served_minibatches_per_s": None, "learner_steps_per_s": rate}
@@ -275,8 +285,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--server-device", default="cuda:0")
-    ap.add_argument("--arms", default=None, help="any of redis, ring, ring-fused (Ape-X), fused, sample, fill (default: Ape-X and R2D2 "
-                    "redis,ring,fused; IMPALA ring,sample,fused)")
+    ap.add_argument("--arms", default=None, help="any of redis, ring, ring-fused, fused, fused-graph (R2D2), sample, "
+                    "fill (default: Ape-X and R2D2 redis,ring,fused; IMPALA ring,sample,fused)")
     ap.add_argument("--redis", default=None, help="host of a Redis server for the control plane (default: an "
                     "in-memory stand-in in a manager process, which makes the Redis-pickle arm far slower than a "
                     "Redis server would)")
@@ -289,14 +299,16 @@ def main():
     arms = a.arms or ("ring,sample,fused" if a.workload == "impala" else "redis,ring,fused")
     if a.workload == "impala" and "redis" in arms.split(","):
         sys.exit("IMPALA has no Redis-protocol replay server")
-    if a.workload != "apex" and "ring-fused" in arms.split(","):
-        sys.exit("the ring-fused arm is the Ape-X learner's served fused step")
+    if a.workload != "r2d2" and "fused-graph" in arms.split(","):
+        sys.exit("the fused-graph arm is the R2D2 learner's captured in-process step (Ape-X's fused arm is captured "
+                 "already; IMPALA's draw cannot be captured)")
     args = {"workload": a.workload, "store": store, "batch": batch, "ring_slots": a.ring_slots, "steps": a.steps,
             "warmup": a.warmup, "server_device": a.server_device, "redis": a.redis,
             "redis_steps": a.redis_steps or a.steps,
             "fill_batches": [int(x) for x in a.fill_batches.split(",")] if a.fill_batches else [batch]}
     runs = {k: [] for k in arms.split(",")}
-    arm = {"fused": _fused_arm, "sample": _sample_arm, "fill": _fill_arm}
+    arm = {"fused": _fused_arm, "fused-graph": lambda x: _fused_arm(x, use_graph=True), "sample": _sample_arm,
+           "fill": _fill_arm}
     for _ in range(a.repeats):
         for k in runs:
             runs[k].append(arm[k](args) if k in arm else _served_arm(k, args))
