@@ -162,6 +162,12 @@ struct SmallField {
   int64_t row_bytes;
 };
 
+// The small-row fields of one launch (R2D2's action and reward: 80 x 4 B; IMPALA's action, mu and reward: T x 4 B).
+struct SmallRows {
+  SmallField f[B2RL_MAX_FIELDS];
+  int32_t n;
+};
+
 template <typename U, class RowOf>
 __device__ __forceinline__ void copy_small_units(const U* __restrict__ src, U* __restrict__ dst, int64_t units_per_row,
                                                  const RowOf& row_of, int64_t k0, int64_t k1, int64_t u,

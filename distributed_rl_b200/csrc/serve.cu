@@ -6,6 +6,7 @@
 // pickle.loads -> host-to-device copy (APE_X/ReplayServer.py:65-114, APE_X/ReplayMemory.py:251-257).
 #include "bulk_rows.cuh"
 #include "tree.cuh"
+#include "uniform.cuh"
 
 #include <new>
 
@@ -13,12 +14,8 @@ namespace b2rl {
 
 constexpr int SERVE_THREADS = 128;   // draws per CTA at most; warp 0's lane 0 then drives the copy engine
 
-// Fields of a served record whose rows are neither bulk rows nor 1/2/4/8-byte scalars (R2D2's action and reward:
-// 80 x 4 B): copied by warps 1..3 of the CTA while thread 0 drives the TMA row copy.
-struct SmallRows {
-  SmallField f[B2RL_MAX_FIELDS];
-  int32_t n;
-};
+// Fields of a served record whose rows are neither bulk rows nor 1/2/4/8-byte scalars (SmallRows) are copied by
+// warps 1..3 of the CTA while thread 0 drives the TMA row copy.
 
 // BY_ITEMS (fewer draws than SMs): CTA c owns a contiguous range of the minibatch's copy items (draw-major, then
 // field, then chunk: the items of copy_rows), as k_gather_bulk's CTAs do, so the copy still spreads over
@@ -111,36 +108,8 @@ k_serve_fill(const __grid_constant__ TreeView t, const __grid_constant__ BulkRow
   }, header, seq, done_ticket);
 }
 
-// The uniform draw without replacement of the IMPALA fill (random.sample, baseline/utils.py:310-315): draw k of a
-// fill is slot (tail + pi(k)) mod capacity, where pi is a keyed pseudorandom permutation of [0, size): a 4-round
-// balanced Feistel network on the smallest even bit width w >= 2 with 2^w >= size, cycle-walked into [0, size).
-// The round keys are the four words of ONE Philox4x32-10 block at the fill's first counter, so a draw is a pure
-// function of (seed, counter, k) and the draws of one fill are distinct by construction.
-struct UniformDraw {
-  int64_t size;        // the valid region [tail, tail + size) mod capacity
-  int64_t tail;
-  int64_t capacity;
-  int32_t half;        // w / 2
-  uint32_t mask;       // 2^half - 1
-};
-
+// The IMPALA fill: the uniform draw without replacement of uniform.cuh, time-major slot.
 constexpr int UNIFORM_CHUNK = 14112;   // half an 84x84x4 frame stack: no chunk of a time-major frame row straddles two steps
-
-__host__ __device__ __forceinline__ uint32_t feistel4(uint32_t x, const uint32_t key[4], int half, uint32_t mask) {
-#pragma unroll
-  for (int r = 0; r < 4; ++r) {
-    const uint32_t L = x >> half, R = x & mask;
-    x = (R << half) | (L ^ (lowbias32(R ^ key[r]) & mask));
-  }
-  return x;
-}
-
-__device__ __forceinline__ int64_t uniform_row(const UniformDraw& u, const uint32_t key[4], int64_t k) {
-  uint32_t y = feistel4((uint32_t)k, key, u.half, u.mask);
-  while ((int64_t)y >= u.size) y = feistel4(y, key, u.half, u.mask);   // k < size: the walk ends on k's cycle
-  const int64_t j = u.tail + (int64_t)y;
-  return j >= u.capacity ? j - u.capacity : j;
-}
 
 template <bool BY_ITEMS>
 __global__ void __launch_bounds__(SERVE_THREADS, 1)
@@ -431,33 +400,24 @@ extern "C" int b2rl_serve_fill_uniform(b2rl_replay* h, b2rl_serve_ring* r, int32
   const int64_t n = r->L.batch, size = h->size, cap = h->capacity;
   B2RL_REQUIRE(n <= size, "sample larger than population: the batch exceeds the stored records");
   B2RL_REQUIRE(size <= (1LL << 32), "a uniform fill draws from at most 2^32 records");
-  UniformDraw u{};
-  u.size = size;
-  u.capacity = cap;
-  u.tail = ((h->head - size) % cap + cap) % cap;   // the valid region, as impala.Replay.draw takes it
-  int w = 2;
-  while ((1LL << w) < size) w += 2;
-  u.half = w / 2;
-  u.mask = (1u << u.half) - 1u;
+  const UniformDraw u = uniform_draw_over(size, h->head, cap);
   BulkRows P{};
   SmallFields small{};
   SmallRows rows{};
   for (int f = 0; f < h->n_fields; ++f) {
     const int64_t b = h->field_bytes[f];
-    if (is_bulk_row(b)) {        // T + 1 steps (the frame stacks s_0 .. s_T)
-      B2RL_REQUIRE(b % (steps + 1) == 0 && (b / (steps + 1)) % 16 == 0,
-                   "a bulk row of a time-major slot must be steps + 1 rows of a multiple of 16 bytes");
+    RolloutField kind;
+    const char* bad = rollout_field(b, steps, kind);
+    B2RL_REQUIRE(bad == nullptr, bad);
+    if (kind == RolloutField::FRAMES) {
       P.add_time_major(h->field[f], (uint8_t*)ptrs[3 + f], b, steps + 1, UNIFORM_CHUNK);
-    } else if (b == 4 * (int64_t)steps) {     // T 4-byte steps (action, mu, reward)
+    } else if (kind == RolloutField::STEPS) {
       rows.f[rows.n++] = SmallField{h->field[f], (uint8_t*)ptrs[3 + f], b};
-    } else if (b == 1 || b == 2 || b == 4 || b == 8) {   // a batch-major scalar (done)
+    } else {                     // a batch-major scalar
       small.src[small.n] = h->field[f];
       small.dst[small.n] = (uint8_t*)ptrs[3 + f];
       small.bytes[small.n] = (int)b;
       small.n++;
-    } else {
-      B2RL_REQUIRE(false, "a time-major slot holds bulk rows of steps + 1 steps, rows of steps 4-byte words and "
-                          "1/2/4/8-byte scalars only");
     }
   }
   DeviceGuard g(h->device);

@@ -131,6 +131,7 @@ class Learner(CapturedStep):
         self.last = {}
         self._graph = self._static = None
         self._bound = None              # _BoundRollouts, built by the first bound step
+        self._drawn = None              # _DrawnRollouts, built by the first captured in-process step
         self._bound_warm = 0            # eager warm-up steps on served slots
         self.launches_per_step = None
 
@@ -162,11 +163,15 @@ class Learner(CapturedStep):
         else:
             self._train_core(state, "staged", action, mu, reward, done, step)
 
-    def fused_step(self, step=0):
+    def fused_step(self, step=0, use_graph=False):
         """One learner step with everything resident: draw B rollouts uniformly without replacement
         (random.sample, baseline/utils.py:310-315), gather only a / mu / r / done (244 B of the 593 KB rollout),
         run conv_1 over the rollouts' (T+1) frames IN PLACE in the replay payload (row = slot * (T+1) + t,
-        time-major), V-trace kernel, loss, backward, clip + RMSprop."""
+        time-major), V-trace kernel, loss, backward, clip + RMSprop.
+        `use_graph`: the step as a CUDA graph (_captured_step), its draw one launch of DeviceReplay.uniform_fetch
+        before each replay.  -> `last` (for the graph: its static buffers, plus `idx`)."""
+        if use_graph:
+            return self._captured_step()
         c = self.cfg
         T, B = c.UNROLL_STEP, c.BATCHSIZE
         mem = self._memory
@@ -180,6 +185,52 @@ class Learner(CapturedStep):
         rows = time_major_rows(idx, self._t_idx)
         self._train_core(self._frames, rows, b["action"].t().contiguous(), b["mu"].t().contiguous(),
                          b["reward"].t().contiguous(), b["done"], step)
+        return self.last
+
+    def _drawn_state(self) -> "_DrawnRollouts":
+        if self._drawn is None:
+            self._drawn = _DrawnRollouts(self)
+        return self._drawn
+
+    def _captured_step(self):
+        """fused_step(use_graph=True): one launch of DeviceReplay.uniform_fetch draws B rollouts into fixed buffers
+        (the draw of the served fill, on the replay's device-resident Philox stream), then _train_core runs on them
+        with conv_1 reading the frames in place through the fixed frame rows.  The draw reads the host-side size and
+        head, so it stays outside the graph.  The first call runs three eager warm-ups, each on its own draw, and
+        captures the body on a fourth; every later call is one draw plus graph.replay().  All under the replay's
+        lock.  -> `last`: the graph's static buffers, plus `idx`."""
+        if self._served:
+            raise RuntimeError("fused_step() samples the learner's own replay; a served replay is driven by run()")
+        c = self.cfg
+        T, B = c.UNROLL_STEP, c.BATCHSIZE
+        mem = self._memory
+        s = self._drawn_state()
+        cur = s.cur
+
+        def draw():
+            mem.store.uniform_fetch(B, T, cur)
+
+        def body():
+            self._train_core(s.frames, cur["rows"], cur["action"], cur["mu"], cur["reward"], cur["done"], 0)
+            self.last["idx"] = cur["idx"]
+            return self.last
+
+        def warm_up():
+            draw()
+            return body()
+
+        # The draw and the replay go to the current stream, as the eager step's draw and gather do, under the lock the
+        # replay thread's ingest (Replay.push_arrays) takes: the draw sees the slots committed before it and never
+        # those an ingest has reserved, and an ingest enqueued after this call is ordered after the step.
+        with mem._lock:
+            if self._graph is None:
+                self._warm_up(warm_up, 3, s.stream)
+                draw()
+                self.last = self._eager_or_captured(body, True, s.stream)
+            else:
+                draw()
+                self._graph.replay()
+                self.last = self._static
         return self.last
 
     def _bound_state(self) -> "_BoundRollouts":
@@ -320,12 +371,36 @@ class _BoundRollouts:
             raise ValueError("SERVED_FUSED_STEP reads the ring slot's frames with the fused conv_1 kernels: the "
                              "model's first node must be the Atari conv_1")
         self.stream = torch.cuda.Stream(dev)
-        f = {x.name: x for x in R.impala_fields(T)}
-        self.cur = {name: torch.empty((T, B), dtype=f[name].dtype, device=dev) for name in ("action", "mu", "reward")}
-        self.cur.update(done=torch.empty(B, dtype=f["done"].dtype, device=dev),
-                        idx=torch.empty(B, dtype=torch.int64, device=dev),
-                        w=torch.empty(B, dtype=torch.float32, device=dev),
+        self.cur = _rollout_buffers(T, B, dev)
+        self.cur.update(w=torch.empty(B, dtype=torch.float32, device=dev),
                         header=torch.zeros(2, dtype=torch.int64, device=dev))
         self.table = torch.zeros(1, dtype=torch.int64, device=dev)
         self.frames = {"state": R.BoundFrames(self.table, 0, (T + 1) * B)}
         self.seq_frames = R.BoundFrames(self.table, 0, T * B)
+
+
+class _DrawnRollouts:
+    """The fixed buffers of the captured in-process step (fused_step(use_graph=True)), built once before its first
+    warm-up, and the stream it is warmed up and captured on.  DeviceReplay.uniform_fetch draws into `cur`: idx (B,),
+    action / mu / reward (T, B), done (B,) and `rows`, the (T+1) * B time-major rows of the drawn rollouts' frames in
+    `frames`, the replay's `state` field with one frame stack per row (row = slot * (T+1) + t)."""
+
+    def __init__(self, L: "Learner"):
+        c, dev = L.cfg, L.device
+        T, B = c.UNROLL_STEP, c.BATCHSIZE
+        if L.model.first_conv_node() is None:
+            raise ValueError("fused_step(use_graph=True) reads the replay's frames with the fused conv_1 kernels: "
+                             "the model's first node must be the Atari conv_1")
+        self.stream = torch.cuda.Stream(dev)
+        self.cur = _rollout_buffers(T, B, dev)
+        self.cur["rows"] = torch.empty((T + 1) * B, dtype=torch.int64, device=dev)
+        self.frames = L._memory.store.field_view("state").view(-1, 4, 84, 84)
+
+
+def _rollout_buffers(T: int, B: int, dev) -> dict:
+    """A captured step's fixed rollout buffers: action / mu / reward (T, B) and done (B,) with the record's dtypes,
+    idx (B,)."""
+    f = {x.name: x for x in R.impala_fields(T)}
+    cur = {name: torch.empty((T, B), dtype=f[name].dtype, device=dev) for name in ("action", "mu", "reward")}
+    cur.update(done=torch.empty(B, dtype=f["done"].dtype, device=dev), idx=torch.empty(B, dtype=torch.int64, device=dev))
+    return cur

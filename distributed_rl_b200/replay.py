@@ -350,6 +350,29 @@ class DeviceReplay:
         check(self.lib.b2rl_replay_gather(self._h, idx.data_ptr(), n, ptrs, self._st()))
         return out
 
+    def uniform_fetch(self, n: int, steps: int, out: dict) -> dict:
+        """n distinct rollouts of `steps` steps drawn uniformly WITHOUT replacement from the valid region
+        [head - size, head) (random.sample, baseline/utils.py:310-315) on the device-resident Philox stream, with
+        the permutation of the served fill (b2rl_serve_fill_uniform), in ONE launch (b2rl_uniform_fetch) into the
+        caller's fixed buffers: out["idx"] int64[n]; each non-frame field named in `out`, rows of `steps` words
+        time-major (steps, n) and scalars (n,); out["rows"] (optional) int64[(steps + 1) * n], the rows of the
+        time-major frames in the frame field viewed as one frame stack per row.  The frames are not copied.
+        n > len(self) raises ValueError, as random.sample does, before anything is launched."""
+        if n > len(self):
+            raise ValueError("Sample larger than population")
+        ptrs = (C.c_void_p * _lib.MAX_FIELDS)()
+        for i, f in enumerate(self.fields):
+            t = out.get(f.name)
+            if t is not None:
+                assert t.is_contiguous() and t.numel() * t.element_size() == n * f.nbytes, f"bad buffer for {f.name}"
+                ptrs[i] = t.data_ptr()
+        idx, rows = out["idx"], out.get("rows")
+        assert idx.dtype == torch.int64 and idx.is_contiguous() and idx.numel() == n
+        assert rows is None or (rows.dtype == torch.int64 and rows.is_contiguous() and rows.numel() == (steps + 1) * n)
+        check(self.lib.b2rl_uniform_fetch(self._h, int(n), int(steps), idx.data_ptr(), ptrs,
+                                          None if rows is None else rows.data_ptr(), self._st()))
+        return out
+
 
 # ---- stateless target kernels -------------------------------------------------
 def _p(t):

@@ -190,6 +190,20 @@ int b2rl_tree_leaves(b2rl_replay* h, int64_t start, int64_t n, float* out_dev, v
 int b2rl_replay_gather(b2rl_replay* h, const int64_t* idx_dev, int64_t n,
                        void* const* out_fields_dev, void* stream);
 
+/* IMPALA's minibatch for a captured learner step (IMPALA/ReplayMemory.py:30-54, drawn as random.sample draws,
+ * baseline/utils.py:310-315) in ONE launch: n rollouts drawn uniformly WITHOUT replacement from the ring's valid
+ * region [head - size, head) with exactly the permutation of b2rl_serve_fill_uniform (same slots from the same
+ * device-resident Philox state, size and head; the counter advances by n), written into the caller's fixed
+ * buffers.  size and head are the host-side values of b2rl_replay_size at the call, so slots reserved by an ingest
+ * in flight are never drawn.  idx_out_dev: int64[n].  For each field f with fields_out_dev[f] != NULL (with
+ * steps = T): a row of T 4-byte words -> word t of draw k at t * n + k; a 1/2/4/8-byte scalar -> row k.  A frame
+ * field (a bulk row of T + 1 equal steps) is not copied and its entry must be NULL: frame_rows_out_dev (int64[(T+1)
+ * * n], may be NULL) receives the frame-table rows of the time-major frames instead, row t * n + k = idx[k] * (T+1)
+ * + t, for b2rl_conv1_fused / b2rl_conv1_wgrad over the field.  fields_out_dev may be NULL.  An error, and no
+ * launch, when n > size, size > 2^32 or a field is not one of those three kinds. */
+int b2rl_uniform_fetch(b2rl_replay* h, int64_t n, int32_t steps, int64_t* idx_out_dev,
+                       void* const* fields_out_dev, int64_t* frame_rows_out_dev, void* stream);
+
 /* Learner.train target section, Ape-X (APE_X/Learner.py:85-121):
  *   a* = argmax_a qn_online[b,:];  y = r + gamma_n * qn_target[b,a*] * notdone
  *   d = clamp(y - q_s[b,action[b]], -1, 1);  prio = (|d| + 1e-7)^alpha

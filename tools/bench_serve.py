@@ -8,7 +8,8 @@ minibatches/s and learner steps/s for
           served minibatches/s is acquire + release alone
   fused   the in-process learner: Learner.fused_step() on its own replay (no server); captured for Ape-X, eager for
           R2D2 and IMPALA
-  fused-graph  R2D2 only: the in-process fused_step(use_graph=True), captured in its first call and replayed
+  fused-graph  R2D2 and IMPALA: the in-process fused_step(use_graph=True), captured in its first call and replayed
+          (IMPALA: one b2rl_uniform_fetch draw launch before each replay)
   sample  IMPALA only: the in-process Replay's sample() -> Learner.train() (gather + time-major transpose per step)
   fill    b2rl_serve_fill (IMPALA: b2rl_serve_fill_uniform) alone, in this process: CUDA events around `steps` fills
           into alternating ring slots, at each batch of --fill-batches; bytes/s = 2 x slot bytes / fill time (each
@@ -204,8 +205,8 @@ def _served_arm(kind, args):
 
 
 def _fused_arm(args, use_graph=False):
-    """The in-process fused_step: eager (`fused`) or, R2D2's `fused-graph`, captured in the first call and replayed
-    (the warm-up calls include the three eager warm-ups and the capture)."""
+    """The in-process fused_step: eager (`fused`) or, R2D2's and IMPALA's `fused-graph`, captured in the first call
+    and replayed (the warm-up calls include the three eager warm-ups and the capture)."""
     import torch
     cfg = _cfg(args, "cuda:0")
     L = _learner(args, cfg)
@@ -285,7 +286,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--server-device", default="cuda:0")
-    ap.add_argument("--arms", default=None, help="any of redis, ring, ring-fused, fused, fused-graph (R2D2), sample, "
+    ap.add_argument("--arms", default=None, help="any of redis, ring, ring-fused, fused, fused-graph (R2D2, IMPALA), "
+                    "sample, "
                     "fill (default: Ape-X and R2D2 redis,ring,fused; IMPALA ring,sample,fused)")
     ap.add_argument("--redis", default=None, help="host of a Redis server for the control plane (default: an "
                     "in-memory stand-in in a manager process, which makes the Redis-pickle arm far slower than a "
@@ -299,9 +301,9 @@ def main():
     arms = a.arms or ("ring,sample,fused" if a.workload == "impala" else "redis,ring,fused")
     if a.workload == "impala" and "redis" in arms.split(","):
         sys.exit("IMPALA has no Redis-protocol replay server")
-    if a.workload != "r2d2" and "fused-graph" in arms.split(","):
-        sys.exit("the fused-graph arm is the R2D2 learner's captured in-process step (Ape-X's fused arm is captured "
-                 "already; IMPALA's draw cannot be captured)")
+    if a.workload == "apex" and "fused-graph" in arms.split(","):
+        sys.exit("the fused-graph arm is the R2D2 and IMPALA learners' captured in-process step (Ape-X's fused arm is "
+                 "captured already)")
     args = {"workload": a.workload, "store": store, "batch": batch, "ring_slots": a.ring_slots, "steps": a.steps,
             "warmup": a.warmup, "server_device": a.server_device, "redis": a.redis,
             "redis_steps": a.redis_steps or a.steps,
