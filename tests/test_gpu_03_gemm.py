@@ -103,7 +103,7 @@ def test_stacked_weights_and_cache(L):
     assert _rel(y3, x.detach().double() @ torch.cat([w2, w1]).detach().double().T) < 5e-6
 
 
-@pytest.mark.parametrize("M,H,A", [(512, 512, 6), (1, 32, 1), (37, 96, 18), (64, 1024, 32)])
+@pytest.mark.parametrize("M,H,A", [(512, 512, 6), (1, 32, 1), (37, 96, 18), (64, 1024, 32), (3840, 512, 6)])
 def test_dueling_tail_matches_pytorch(L, M, H, A):
     """csrc/dueling.cu against the unfused node sequence (ReLU, two Linear, Add, Mean, Substract) in fp64."""
     g = torch.Generator(device="cuda").manual_seed(M + H + A)

@@ -4,19 +4,47 @@ import numpy as np
 import pytest
 
 
-def test_balanced_base256_digits_via_bias_reconstruct_exactly():
-    """csrc/conv1_wgrad.cu B producers: Y = X + 0x00808080; low three bytes ^ 0x80 are int8 digits, the top byte is q0."""
-    rng = np.random.default_rng(0)
-    X = np.concatenate([rng.integers(-(127 << 24), (127 << 24) + 1, size=200000, dtype=np.int64),
-                        np.array([0, 1, -1, 127 << 24, -(127 << 24), 128, -128, 0x7F7F7F, -0x808080], np.int64)])
+def _wgrad_digits(X):
+    """csrc/conv1_wgrad.cu B producers: Y = X + 0x00808080; low three bytes ^ 0x80 are int8 digits, the top byte is q0.
+    -> (d0, d1, d2, d3), most significant first."""
     Y = (X + 0x00808080).astype(np.int64)
     assert (Y < 2 ** 31).all() and (Y >= -2 ** 31).all()          # fits the int32 the kernel uses
     Yu = Y.astype(np.int32).view(np.uint32).astype(np.uint32)
     b = [((Yu >> (8 * k)) & 0xFF).astype(np.uint8) for k in range(4)]
     d3, d2, d1 = [(x ^ 0x80).view(np.int8).astype(np.int64) for x in b[:3]]
-    d0 = b[3].view(np.int8).astype(np.int64)
+    return b[3].view(np.int8).astype(np.int64), d1, d2, d3
+
+
+def _wgrad_digit_scale(absmax):
+    """csrc/conv1_wgrad.cu digit_exponent: s = 2^(exponent(fl(max/127)) + 1), the power of two just above max/127."""
+    t = np.float32(absmax) / np.float32(127.0)
+    e = ((t.view(np.uint32) >> 23) & 0xFF) + 1
+    return np.uint32(int(e) << 23).view(np.float32)
+
+
+def test_balanced_base256_digits_via_bias_reconstruct_exactly():
+    """The four digits of _wgrad_digits give back X exactly, the leading one within [-127, 127]."""
+    rng = np.random.default_rng(0)
+    X = np.concatenate([rng.integers(-(127 << 24), (127 << 24) + 1, size=200000, dtype=np.int64),
+                        np.array([0, 1, -1, 127 << 24, -(127 << 24), 128, -128, 0x7F7F7F, -0x808080], np.int64)])
+    d0, d1, d2, d3 = _wgrad_digits(X)
     assert (np.abs(d0) <= 127).all()
     assert np.array_equal(((d0 * 256 + d1) * 256 + d2) * 256 + d3, X)
+
+
+def test_most_negative_wgrad_digits_fit_int32_column_sums():
+    """The gradient the GPU test of the accumulators' limit feeds: gy = -0x7E808080 * 2^-24 (fp32-exact; the decimal
+    -126.50196087360382 rounds to it) has digit scale 1 and the digits (-126, -128, -128, -128), the most negative
+    the bias trick forms.  A CTA's column sum of 160 items of 400 positions of pixel 255 times -128 still fits int32."""
+    gy = np.float32(-0x7E808080 * 2.0 ** -24)
+    assert float(gy) == -0x7E808080 * 2.0 ** -24 and gy == np.float32(-126.50196087360382)
+    s = _wgrad_digit_scale(abs(gy))
+    assert s == 1.0
+    X = np.array([np.rint(np.float64(gy) / np.float64(s) * 2.0 ** 24)], np.int64)
+    assert X[0] == -0x7E808080
+    assert [int(d[0]) for d in _wgrad_digits(X)] == [-126, -128, -128, -128]
+    assert -128 * 255 * 400 * 160 >= -2 ** 31
+    assert -128 * 255 * 400 * 165 < -2 ** 31                      # ... and 165 items would not
 
 
 def test_power_of_two_scale_keeps_every_gradient_within_127():
@@ -24,10 +52,7 @@ def test_power_of_two_scale_keeps_every_gradient_within_127():
     rng = np.random.default_rng(1)
     for _ in range(200):
         v = (rng.standard_normal(400) * 10.0 ** rng.uniform(-6, 3)).astype(np.float32)
-        m = np.abs(v).max()
-        t = np.float32(m) / np.float32(127.0)
-        e = ((t.view(np.uint32) >> 23) & 0xFF) + 1
-        s = np.uint32(int(e) << 23).view(np.float32)
+        s = _wgrad_digit_scale(np.abs(v).max())
         x = v.astype(np.float64) / np.float64(s) * 2.0 ** 24
         assert np.abs(x).max() <= 127 * 2 ** 24 + 16
         big = np.abs(v) >= s
