@@ -66,6 +66,10 @@ SIGNATURES = {
     "b2rl_conv1_wgrad": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp]),
     "b2rl_conv1_fused_table": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp]),
     "b2rl_conv1_wgrad_table": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp]),
+    "b2rl_conv1_fused_strided": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_vp,
+                                           c_i32, c_vp]),
+    "b2rl_conv1_wgrad_strided": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp,
+                                           c_i32, c_vp]),
     "b2rl_rmsprop_step": (C.c_int, [C.POINTER(c_vp), C.POINTER(c_vp), C.POINTER(c_vp), C.POINTER(c_vp),
                                     C.POINTER(c_i64), c_i32, c_f64, c_f64, c_f64, c_i32, C.POINTER(c_i64), c_vp, c_vp,
                                     c_vp]),

@@ -23,7 +23,9 @@
 //                NHWC stores straight from the accumulator fragment
 //   warps 8-15   im2col producers: SMEM frame -> 128B-swizzled K-major A tile (uint8);
 //                thread = (tile row, channel pair)
-//   warp 16      TMA loader: weights once, then one 28 224-byte frame stack per item
+//   warp 16      TMA loader: weights once, then one 28 224-byte frame stack per item, from base + row * row_stride
+//                (a stride of 7 056 reads the overlapping 4-frame windows of a frame strip: channel c of row r is
+//                frame r + c)
 #include "common.cuh"
 #include "hopper.cuh"
 
@@ -102,10 +104,11 @@ k_conv1_pack_jobs(const __grid_constant__ PackJobs J, int c_out) {
 }
 
 struct Params {
-  const uint8_t* frames;     // field base: rows of FRAME_BYTES
+  const uint8_t* frames;     // field base: row r is the FRAME_BYTES starting at frames + r * row_stride
   const int64_t* idx;        // sampled rows, or nullptr for rows 0..n-1
   int64_t n;                 // frame stacks to process
   int64_t capacity;          // rows in `frames` (indices are clamped)
+  int64_t row_stride;        // bytes between rows: FRAME_BYTES (stacks) or 7 056 (overlapping windows of a frame strip)
   const int8_t* bq;          // packed weights (n_nets * 128 rows, SW128 layout), n_nets*128*256 bytes
   const float* scale;        // [n_nets][32] = s_c / 255
   float* out;                // [n_nets][n][400][32] fp32 (NHWC)
@@ -175,7 +178,7 @@ k_conv1_fused(const __grid_constant__ PARAMS P) {
         int64_t row = P.idx ? P.idx[k] : k;
         row = row < 0 ? 0 : (row >= P.capacity ? P.capacity - 1 : row);
         mbar_expect_tx(&raw_full[s], FRAME_BYTES);
-        bulk_g2s(sRaw + s * RAW_STRIDE, frames + row * FRAME_BYTES, FRAME_BYTES, &raw_full[s]);
+        bulk_g2s(sRaw + s * RAW_STRIDE, frames + row * P.row_stride, FRAME_BYTES, &raw_full[s]);
       }
     }
   } else if (warp >= CONSUMERS / 32) {
@@ -336,7 +339,7 @@ static cudaError_t conv1_launch(const PARAMS& P, unsigned grid, cudaStream_t st)
   return cudaSuccess;
 }
 
-// What b2rl_conv1_fused and b2rl_conv1_fused_table share once their frame source is checked.
+// What the direct and the table frame source share once the source is checked.
 template <class PARAMS>
 static int conv1_fused_run(PARAMS& P, const int8_t* bq_dev, const float* scale_dev, int32_t n_nets, int32_t c_out,
                            float* out_dev, void* stream) {
@@ -363,25 +366,39 @@ static int conv1_fused_run(PARAMS& P, const int8_t* bq_dev, const float* scale_d
   return B2RL_OK;
 }
 
+extern "C" int b2rl_conv1_fused_strided(const uint8_t* frames_dev, const uint8_t* const* frame_table_dev,
+                                        int64_t row_stride, int64_t rows, const int64_t* idx_dev, int64_t n,
+                                        const int8_t* bq_dev, const float* scale_dev, int32_t n_nets, int32_t c_out,
+                                        float* out_dev, int32_t relu, void* stream) {
+  B2RL_REQUIRE(n >= 0, "negative n");
+  B2RL_REQUIRE((frames_dev != nullptr) != (frame_table_dev != nullptr), "exactly one of frames and frame table");
+  B2RL_REQUIRE(row_stride > 0 && row_stride % 16 == 0, "the row stride must be a positive multiple of 16 bytes");
+  B2RL_REQUIRE(frames_dev ? (uintptr_t)frames_dev % 16 == 0 : (uintptr_t)frame_table_dev % 8 == 0,
+               "frames must be 16-byte aligned, a frame table entry 8-byte aligned");
+  if (n == 0) return B2RL_OK;
+  if (frames_dev) {
+    conv1::Params P{frames_dev, idx_dev, n, rows, row_stride, nullptr, nullptr, nullptr, relu};
+    return conv1_fused_run(P, bq_dev, scale_dev, n_nets, c_out, out_dev, stream);
+  }
+  conv1::TableParams P{};
+  P.idx = idx_dev, P.n = n, P.capacity = rows, P.row_stride = row_stride, P.relu = relu, P.table = frame_table_dev;
+  return conv1_fused_run(P, bq_dev, scale_dev, n_nets, c_out, out_dev, stream);
+}
+
 extern "C" int b2rl_conv1_fused(const uint8_t* frames_dev, int64_t capacity, const int64_t* idx_dev, int64_t n,
                                 const int8_t* bq_dev, const float* scale_dev, int32_t n_nets, int32_t c_out,
                                 float* out_dev, int32_t relu, void* stream) {
   B2RL_REQUIRE(n >= 0, "negative n");
   if (n == 0) return B2RL_OK;
   B2RL_REQUIRE(frames_dev, "null argument");
-  B2RL_REQUIRE((uintptr_t)frames_dev % 16 == 0, "frames, packed weights and output must be 16-byte aligned");
-  conv1::Params P{frames_dev, idx_dev, n, capacity, nullptr, nullptr, nullptr, relu};
-  return conv1_fused_run(P, bq_dev, scale_dev, n_nets, c_out, out_dev, stream);
+  return b2rl_conv1_fused_strided(frames_dev, nullptr, conv1::FRAME_BYTES, capacity, idx_dev, n, bq_dev, scale_dev,
+                                  n_nets, c_out, out_dev, relu, stream);
 }
 
 extern "C" int b2rl_conv1_fused_table(const uint8_t* const* frame_table_dev, int64_t capacity, const int64_t* idx_dev,
                                       int64_t n, const int8_t* bq_dev, const float* scale_dev, int32_t n_nets,
                                       int32_t c_out, float* out_dev, int32_t relu, void* stream) {
-  B2RL_REQUIRE(n >= 0, "negative n");
   B2RL_REQUIRE(frame_table_dev != nullptr, "null frame table");
-  B2RL_REQUIRE((uintptr_t)frame_table_dev % 8 == 0, "a frame table entry must be 8-byte aligned");
-  if (n == 0) return B2RL_OK;
-  conv1::TableParams P{};
-  P.idx = idx_dev, P.n = n, P.capacity = capacity, P.relu = relu, P.table = frame_table_dev;
-  return conv1_fused_run(P, bq_dev, scale_dev, n_nets, c_out, out_dev, stream);
+  return b2rl_conv1_fused_strided(nullptr, frame_table_dev, conv1::FRAME_BYTES, capacity, idx_dev, n, bq_dev,
+                                  scale_dev, n_nets, c_out, out_dev, relu, stream);
 }

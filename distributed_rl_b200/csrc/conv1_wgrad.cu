@@ -52,9 +52,10 @@ constexpr int MAX_ITEMS_PER_CTA = 160;             // int32 accumulators: 128*25
 __device__ __forceinline__ int sw_row(int row) { return (row >> 3) * 1024 + (row & 7) * 128; }
 
 struct Params {
-  const uint8_t* frames;     // field base: rows of FRAME_BYTES
+  const uint8_t* frames;     // field base: row r is the FRAME_BYTES starting at frames + r * row_stride
   const int64_t* idx;        // sampled rows, or nullptr for rows 0..n-1
   int64_t n, capacity;
+  int64_t row_stride;        // bytes between rows: FRAME_BYTES (stacks) or 7 056 (overlapping windows of a frame strip)
   const float* gy;           // [n][400][C_OUT] fp32 (NHWC)
   const float* y;            // optional conv_1 output after ReLU, same layout: dL/dy is taken as gy * (y > 0); else nullptr
   float* partial;            // [gridDim.x][C_OUT][256]
@@ -120,7 +121,7 @@ k_conv1_wgrad(const __grid_constant__ PARAMS P) {
     int64_t row = P.idx ? P.idx[k] : k;
     row = row < 0 ? 0 : (row >= P.capacity ? P.capacity - 1 : row);
     mbar_expect_tx(&raw_full[it & 1], FRAME_BYTES);
-    bulk_g2s(sRaw + (it & 1) * RAW_STRIDE, frames + row * FRAME_BYTES, FRAME_BYTES, &raw_full[it & 1]);
+    bulk_g2s(sRaw + (it & 1) * RAW_STRIDE, frames + row * P.row_stride, FRAME_BYTES, &raw_full[it & 1]);
   };
   if (threadIdx.x == 0) load_frame(0);
 
@@ -363,9 +364,9 @@ extern "C" int64_t b2rl_conv1_wgrad_workspace_floats(int32_t c_out) {
   return (int64_t)sms * c_out * conv1w::E_TOTAL;
 }
 
-// The launches of b2rl_conv1_wgrad and b2rl_conv1_wgrad_table.  `frames_dev` null: the frame base is the table entry
+// The launches of every conv_1 weight-gradient entry point.  `frames_dev` null: the frame base is the table entry
 // (read on the device, where the offset of each launch of a split n is added).
-static int wgrad_run(const uint8_t* frames_dev, const uint8_t* const* table_dev, int64_t capacity,
+static int wgrad_run(const uint8_t* frames_dev, const uint8_t* const* table_dev, int64_t row_stride, int64_t capacity,
                      const int64_t* idx_dev, int64_t n, const float* gy_dev, const float* y_relu_dev, int32_t c_out,
                      float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream) {
   B2RL_REQUIRE(gy_dev && workspace_dev && gw_dev, "null argument");
@@ -382,10 +383,10 @@ static int wgrad_run(const uint8_t* frames_dev, const uint8_t* const* table_dev,
   const int64_t per_launch = (int64_t)sms * conv1w::MAX_ITEMS_PER_CTA;   // int32 accumulator bound
   for (int64_t off = 0; off < n; off += per_launch) {
     const int64_t m = (n - off < per_launch) ? n - off : per_launch;
-    conv1w::Params P{frames_dev, idx_dev ? idx_dev + off : nullptr, m, capacity,
+    conv1w::Params P{frames_dev, idx_dev ? idx_dev + off : nullptr, m, capacity, row_stride,
                      gy_dev + off * (int64_t)(conv1w::POS * c_out),
                      y_relu_dev ? y_relu_dev + off * (int64_t)(conv1w::POS * c_out) : nullptr, workspace_dev};
-    const int64_t frame_off = idx_dev ? 0 : off * conv1w::FRAME_BYTES;
+    const int64_t frame_off = idx_dev ? 0 : off * row_stride;
     if (!idx_dev) P.capacity = capacity - off;
     const unsigned grid = (unsigned)((m < sms) ? m : sms);
     if (frames_dev) {
@@ -407,22 +408,31 @@ static int wgrad_run(const uint8_t* frames_dev, const uint8_t* const* table_dev,
   return B2RL_OK;
 }
 
+extern "C" int b2rl_conv1_wgrad_strided(const uint8_t* frames_dev, const uint8_t* const* frame_table_dev,
+                                        int64_t row_stride, int64_t rows, const int64_t* idx_dev, int64_t n,
+                                        const float* gy_dev, const float* y_relu_dev, int32_t c_out,
+                                        float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream) {
+  B2RL_REQUIRE(n >= 1, "n must be positive");
+  B2RL_REQUIRE((frames_dev != nullptr) != (frame_table_dev != nullptr), "exactly one of frames and frame table");
+  B2RL_REQUIRE(row_stride > 0 && row_stride % 16 == 0, "the row stride must be a positive multiple of 16 bytes");
+  B2RL_REQUIRE(frames_dev ? (uintptr_t)frames_dev % 16 == 0 : (uintptr_t)frame_table_dev % 8 == 0,
+               "frames must be 16-byte aligned, a frame table entry 8-byte aligned");
+  return wgrad_run(frames_dev, frame_table_dev, row_stride, rows, idx_dev, n, gy_dev, y_relu_dev, c_out,
+                   workspace_dev, gw_dev, accumulate, stream);
+}
+
 extern "C" int b2rl_conv1_wgrad(const uint8_t* frames_dev, int64_t capacity, const int64_t* idx_dev, int64_t n,
                                 const float* gy_dev, const float* y_relu_dev, int32_t c_out, float* workspace_dev,
                                 float* gw_dev, int32_t accumulate, void* stream) {
-  B2RL_REQUIRE(n >= 1, "n must be positive");
   B2RL_REQUIRE(frames_dev, "null argument");
-  B2RL_REQUIRE((uintptr_t)frames_dev % 16 == 0, "frames, gy and y must be 16-byte aligned");
-  return wgrad_run(frames_dev, nullptr, capacity, idx_dev, n, gy_dev, y_relu_dev, c_out, workspace_dev, gw_dev,
-                   accumulate, stream);
+  return b2rl_conv1_wgrad_strided(frames_dev, nullptr, conv1w::FRAME_BYTES, capacity, idx_dev, n, gy_dev, y_relu_dev,
+                                  c_out, workspace_dev, gw_dev, accumulate, stream);
 }
 
 extern "C" int b2rl_conv1_wgrad_table(const uint8_t* const* frame_table_dev, int64_t capacity, const int64_t* idx_dev,
                                       int64_t n, const float* gy_dev, const float* y_relu_dev, int32_t c_out,
                                       float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream) {
-  B2RL_REQUIRE(n >= 1, "n must be positive");
   B2RL_REQUIRE(frame_table_dev != nullptr, "null frame table");
-  B2RL_REQUIRE((uintptr_t)frame_table_dev % 8 == 0, "a frame table entry must be 8-byte aligned");
-  return wgrad_run(nullptr, frame_table_dev, capacity, idx_dev, n, gy_dev, y_relu_dev, c_out, workspace_dev, gw_dev,
-                   accumulate, stream);
+  return b2rl_conv1_wgrad_strided(nullptr, frame_table_dev, conv1w::FRAME_BYTES, capacity, idx_dev, n, gy_dev,
+                                  y_relu_dev, c_out, workspace_dev, gw_dev, accumulate, stream);
 }

@@ -203,7 +203,8 @@ class Conv1Gathered(torch.autograd.Function):
             gy = gy * (y > 0)
         if not ctx.has_idx:
             x = ctx.frames
-        elif ctx.store is not None:    # TMA bulk gather straight from the replay payload
+        elif ctx.store is not None and ctx.frames.stride(0) == R.FRAME_STACK_BYTES:
+            # TMA bulk gather straight from the replay payload (whole records: never for the windows of frame strips)
             x = ctx.store.gather(idx, ctx.store.alloc_batch(idx.numel(), ("state",)))["state"]
         else:
             x = ctx.frames.index_select(0, idx)
@@ -220,10 +221,13 @@ def conv1_packs(model, device, *n_nets):
     return (name,) + tuple(R.Conv1Pack(n, device, c_out) for n in n_nets)
 
 
-def time_major_rows(seq_rows: torch.Tensor, t_idx: torch.Tensor) -> torch.Tensor:
-    """Frame-table rows of the (t, b) frames in time-major order, for sequences of T frames stored as T consecutive
-    rows: row = seq_rows[b] * T + t, with t_idx = arange(T).view(T, 1) (kept by the caller: no launch per step)."""
-    return (seq_rows.view(1, -1) * t_idx.shape[0] + t_idx).reshape(-1).contiguous()
+def time_major_rows(seq_rows: torch.Tensor, t_idx: torch.Tensor, pitch: int | None = None) -> torch.Tensor:
+    """Frame-table rows of the (t, b) frames in time-major order, for sequences of T frames whose rows start `pitch`
+    rows apart (None: T, frame stacks stored as T consecutive rows; T + 3 for the windows of frame strips,
+    R.sequence_rows): row = seq_rows[b] * pitch + t, with t_idx = arange(T).view(T, 1) (kept by the caller: no launch
+    per step)."""
+    pitch = t_idx.shape[0] if pitch is None else pitch
+    return (seq_rows.view(1, -1) * pitch + t_idx).reshape(-1).contiguous()
 
 
 # -- Learner.run: the Redis-facing edge ----------------------------------------------------------

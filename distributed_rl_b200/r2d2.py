@@ -66,6 +66,9 @@ class R2D2Config:
     FUSED_HEADS: bool = True     # dueling heads: 3xTF32 wgmma GEMM + fused tail kernels (csrc/gemm.cu, csrc/dueling.cu)
     SERVED_FUSED_STEP: bool = False  # on a served replay (DeviceReplayClient), run() steps a captured step on the
                                      # bound ring slot instead of sample() -> train() -> update()
+    FRAME_STRIP: bool = False    # store each sequence's T + 3 distinct frames instead of its T stacks (3.83x fewer
+                                 # bytes per sequence at T = 80); conv_1 reads stack t as frames t .. t + 3 in place.
+                                 # Only records whose stacks slide (every one R2D2/Player.py sends) can be stored.
 
     @staticmethod
     def from_configuration():
@@ -73,7 +76,8 @@ class R2D2Config:
         names = ("BATCHSIZE", "ACTION_SIZE", "ALPHA", "BETA", "GAMMA", "UNROLL_STEP", "FIXED_TRAJECTORY", "MEM",
                  "USE_RESCALING", "REPLAY_MEMORY_LEN", "BUFFER_SIZE", "TARGET_FREQUENCY", "LEARNER_DEVICE",
                  "REDIS_SERVER", "OPTIM_INFO", "MODEL")
-        return R2D2Config(LOG_W=getattr(C, "LOG_W", None), **{k: getattr(C, k) for k in names})
+        return R2D2Config(LOG_W=getattr(C, "LOG_W", None), FRAME_STRIP=bool(getattr(C, "FRAME_STRIP", False)),
+                          **{k: getattr(C, k) for k in names})
 
 
 class Replay(ReplayThread):
@@ -82,7 +86,7 @@ class Replay(ReplayThread):
 
     def __init__(self, cfg: R2D2Config | None = None, connect=None):
         super().__init__(cfg or R2D2Config.from_configuration(), connect)
-        fields = R.r2d2_fields(self.cfg.FIXED_TRAJECTORY)
+        fields = R.r2d2_config_fields(self.cfg)
         if self.cfg.PAYLOAD_POOL:
             self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, (), self.device)          # priorities only
             self.pool = R.DeviceReplay(self.cfg.PAYLOAD_POOL, fields, self.device)           # the stored sequences
@@ -92,6 +96,11 @@ class Replay(ReplayThread):
         self.memory = MemoryView(self.store, self.cfg.BETA)
 
     def push_arrays(self, s, a, r, h0, h1, notdone, p):
+        """`s`: (n, T, 4, 84, 84) stacks or, with FRAME_STRIP, (n, T + 3, 84, 84) strips.  With FRAME_STRIP, stacks are
+        encoded into strips first (R.encode_strips): a record whose stacks do not slide raises ValueError naming it,
+        and nothing of the batch is pushed."""
+        if self.cfg.FRAME_STRIP and tuple(s.shape[1:]) != (self.cfg.FIXED_TRAJECTORY + 3, 84, 84):
+            s = R.encode_strips(s)
         with self._lock:
             self.store.push([s, a, r, h0, h1, notdone], p)
         self.total_frame += int(torch.as_tensor(p).numel())
@@ -103,7 +112,7 @@ class Replay(ReplayThread):
             return
         import pickle
         from .wire import decode_r2d2
-        cols, p = decode_r2d2([pickle.loads(b) for b in blobs], self.cfg.FIXED_TRAJECTORY)
+        cols, p = decode_r2d2([pickle.loads(b) for b in blobs], self.cfg.FIXED_TRAJECTORY, strip=self.cfg.FRAME_STRIP)
         self.push_arrays(*cols, p)
 
     def buffer(self, m: int = 1):
@@ -111,11 +120,12 @@ class Replay(ReplayThread):
         with self._lock:
             idx, _, w = self.store.sample(B * m, beta=self.cfg.BETA)
             b = self.pool.gather(self.rows_of(idx))
+        state = R.as_stacks(b["state"])                     # strips: the zero-copy stack view
         for k in range(m):
             sl = slice(k * B, (k + 1) * B)
             h0 = b["h0"][sl].unsqueeze(0).contiguous()     # (1, B, 512) like torch.cat(..., 1) at :87-88
             h1 = b["h1"][sl].unsqueeze(0).contiguous()
-            self.deque.append([(h0, h1), b["state"][sl], b["action"][sl], b["reward"][sl], b["notdone"][sl],
+            self.deque.append([(h0, h1), state[sl], b["action"][sl], b["reward"][sl], b["notdone"][sl],
                                w[sl], idx[sl]])
 
     def rows_of(self, idx: torch.Tensor) -> torch.Tensor:
@@ -138,7 +148,7 @@ class Learner(TargetNetLearner):
         cadence): see _next_step."""
         self.cfg = cfg or R2D2Config.from_configuration()
         if memory is not None and self.cfg.SERVED_FUSED_STEP:
-            check_served_fused(self.cfg, memory, R.r2d2_fields(self.cfg.FIXED_TRAJECTORY))
+            check_served_fused(self.cfg, memory, R.r2d2_config_fields(self.cfg))
         self.device = torch.device(self.cfg.LEARNER_DEVICE)
         self.model = GraphAgent(self.cfg.MODEL).to(self.device)
         self.target_model = GraphAgent(self.cfg.MODEL).to(self.device)
@@ -166,8 +176,12 @@ class Learner(TargetNetLearner):
         state = torch.as_tensor(state).to(dev)
         fused = c.FUSED_CONV1 and state.dtype == torch.uint8 and self.model.first_conv_node() is not None
         if fused:
-            frames = state.contiguous().view(B * T, 4, 84, 84)
-            q, q_target = self._forward_fused(frames, self._time_major_rows(None, T, B), T, MEM, B, A)
+            strips = R.stacks_strips(state)
+            if strips is not None:                              # the stack view of frame strips: read the windows
+                frames, pitch = R.strip_windows(strips.contiguous()), T + 3
+            else:
+                frames, pitch = state.contiguous().view(B * T, 4, 84, 84), T
+            q, q_target = self._forward_fused(frames, self._time_major_rows(None, T, B, pitch), T, MEM, B, A)
         else:
             state = state.float() / 255.0                       # :89-90
             sv = state.permute(1, 0, 2, 3, 4).contiguous()      # time-major, :93
@@ -202,18 +216,19 @@ class Learner(TargetNetLearner):
         q.backward(out["grad_q"])                               # == loss.backward(), :189-192
         return out, self.step()
 
-    def _time_major_rows(self, seq_rows, T, B):
-        """Frame-table rows of the (t, b) frames in time-major order: row = seq_row[b] * T + t
-        (seq_rows None: the batch itself is the table, sequence b = rows b*T ... b*T+T-1)."""
+    def _time_major_rows(self, seq_rows, T, B, pitch):
+        """Frame-table rows of the (t, b) frames in time-major order: row = seq_row[b] * pitch + t (pitch T for
+        stacks, T + 3 for the windows of frame strips; seq_rows None: the batch itself is the table, sequence b's
+        rows start at b * pitch)."""
         if not hasattr(self, "_t_idx"):
             self._t_idx = torch.arange(T, device=self.device).view(T, 1)
             self._b_idx = torch.arange(B, device=self.device)
-        return time_major_rows(self._b_idx if seq_rows is None else seq_rows, self._t_idx)
+        return time_major_rows(self._b_idx if seq_rows is None else seq_rows, self._t_idx, pitch)
 
     def _forward_fused(self, frames, tm_rows, T, MEM, B, A):
         """The forward passes with conv_1 on the tensor cores, reading `frames` (a uint8 (rows, 4, 84, 84) table:
-        the staged batch or the replay payload itself) IN PLACE: the (b, t) -> time-major reordering and the
-        uint8 -> /255 conversion are folded into the kernel's gather (`tm_rows`)."""
+        the staged batch or the replay payload itself, its stacks or the windows of its strips) IN PLACE: the (b, t) ->
+        time-major reordering and the uint8 -> /255 conversion are folded into the kernel's gather (`tm_rows`)."""
         dev = self.device
         if not hasattr(self, "_pack2"):
             self._conv_name, self._pack2, self._pack1 = conv1_packs(self.model, dev, 2, 1)
@@ -257,7 +272,10 @@ class Learner(TargetNetLearner):
         st, pool = mem.store, mem.pool
         if not hasattr(self, "_small"):
             self._small = pool.alloc_batch(B, ("action", "reward", "h0", "h1", "notdone"))
-            self._frames = pool.field_view("state").view(-1, 4, 84, 84)
+            if c.FRAME_STRIP:
+                self._frames, self._pitch = R.strip_windows(pool.field_view("state")), T + 3
+            else:
+                self._frames, self._pitch = pool.field_view("state").view(-1, 4, 84, 84), T
 
         def body():
             idx, _, w = st.sample(B, beta=c.BETA, want_prob=False)
@@ -266,7 +284,7 @@ class Learner(TargetNetLearner):
             h0, h1 = b["h0"].unsqueeze(0), b["h1"].unsqueeze(0)
             self.model.setCellState((h0, h1))
             self.target_model.setCellState((h0, h1))
-            q, q_target = self._forward_fused(self._frames, self._time_major_rows(rows, T, B), T, MEM, B, A)
+            q, q_target = self._forward_fused(self._frames, self._time_major_rows(rows, T, B, self._pitch), T, MEM, B, A)
             out, info = self._learn(q, q_target, b["action"], b["reward"], b["notdone"], w)
             st.update(idx, out["prio"])
             return {"scalars": out["scalars"], "p_norm": info["p_norm"], "prio": out["prio"], "idx": idx}
@@ -340,8 +358,9 @@ class _StepState:
     is warmed up and captured on and, on a served memory, the buffers a ring slot is bound to.  memory.acquire()
     copies the slot's header, idx, w, action (B, T), reward (B, T), h0, h1 (B, 512) and notdone (B,) into `cur` and
     writes the address of its `state` rows into the one-entry `table`.  The slot's `state` is batch-major
-    (B, T, 4, 84, 84), so frame (b, t) is row b * T + t from that address, and `rows` (the time-major order the
-    burn-in and the window read, split at MEM * B by _forward_fused) stays the same for every slot."""
+    (B, T, 4, 84, 84), so frame (b, t) is row b * T + t from that address (with FRAME_STRIP, (B, T + 3, 84, 84):
+    window b * (T + 3) + t, rows 7 056 bytes apart), and `rows` (the time-major order the burn-in and the window
+    read, split at MEM * B by _forward_fused) stays the same for every slot."""
 
     def __init__(self, L: "Learner"):
         c, dev = L.cfg, L.device
@@ -352,10 +371,11 @@ class _StepState:
             if L.model.first_conv_node() is None:
                 raise ValueError("SERVED_FUSED_STEP reads the ring slot's frames with the fused conv_1 kernels: the "
                                  "model's first node must be the Atari conv_1")
-            self.cur = dict(R.alloc_rows(R.r2d2_fields(T), B, dev, ("action", "reward", "h0", "h1", "notdone")),
+            self.cur = dict(R.alloc_rows(R.r2d2_config_fields(c), B, dev, ("action", "reward", "h0", "h1", "notdone")),
                             idx=torch.empty(B, dtype=torch.int64, device=dev),
                             w=torch.empty(B, dtype=torch.float32, device=dev),
                             header=torch.zeros(2, dtype=torch.int64, device=dev))
             self.table = torch.zeros(1, dtype=torch.int64, device=dev)
-            self.frames = {"state": R.BoundFrames(self.table, 0, B * T)}
-            self.rows = L._time_major_rows(None, T, B)
+            pitch, rows, stride = R.sequence_rows(B, T, c.FRAME_STRIP)
+            self.frames = {"state": R.BoundFrames(self.table, 0, rows, stride)}
+            self.rows = L._time_major_rows(None, T, B, pitch)

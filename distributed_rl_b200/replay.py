@@ -18,6 +18,7 @@ from . import _lib
 from ._lib import ReplayDesc, check
 
 FRAME_STACK_BYTES = 4 * 84 * 84  # one (4,84,84) uint8 observation, 28 224 B
+FRAME_BYTES = 84 * 84            # one 84x84 uint8 frame, 7 056 B: the row stride of a frame strip's windows
 
 
 @dataclass(frozen=True)
@@ -44,16 +45,98 @@ APEX_FIELDS = (  # [s, a, R_n, s', done, prio]  APE_X/Player.py:252-261
 )
 
 
-def r2d2_fields(T: int = 80, hidden: int = 512):
-    """[(h0,h1), (s,a,r) x T, done, prio]  R2D2/ReplayMemory.py:70-88."""
+def r2d2_fields(T: int = 80, hidden: int = 512, strip: bool = False):
+    """[(h0,h1), (s,a,r) x T, done, prio]  R2D2/ReplayMemory.py:70-88.  `strip`: `state` holds the sequence's T + 3
+    distinct frames (T + 3, 84, 84) instead of its T stacks (T, 4, 84, 84); stack t is frames t .. t + 3."""
     return (
-        Field("state", torch.uint8, (T, 4, 84, 84)),
+        Field("state", torch.uint8, (T + 3, 84, 84) if strip else (T, 4, 84, 84)),
         Field("action", torch.int32, (T,)),
         Field("reward", torch.float32, (T,)),
         Field("h0", torch.float32, (hidden,)),
         Field("h1", torch.float32, (hidden,)),
         Field("notdone", torch.float32, ()),
     )
+
+
+def r2d2_config_fields(cfg):
+    """The R2D2 record fields of an R2D2Config: FIXED_TRAJECTORY steps, frame strips when FRAME_STRIP is set."""
+    return r2d2_fields(cfg.FIXED_TRAJECTORY, strip=bool(getattr(cfg, "FRAME_STRIP", False)))
+
+
+# ---- R2D2 frame strips: a sequence of T stacks stored as its T + 3 distinct frames ----------------------------------
+# Every R2D2 record slides: R2D2/Player.py:38-63 stacks the last four frames of one episode, so stack t + 1 is stack t
+# shifted by one frame (s[t+1][:3] == s[t][1:]).  Frames t .. t + 3 of a strip are stack t, and stack t is the
+# FRAME_STACK_BYTES that start at byte t * FRAME_BYTES of the strip: conv_1 reads it in place as one row of a view
+# whose rows are FRAME_BYTES apart.
+def sequence_rows(n_seq: int, T: int, strip: bool) -> tuple:
+    """conv_1's frame rows over `n_seq` consecutive sequences of T steps -> (row pitch per sequence, rows, row stride
+    in bytes).  Stacks: T rows per sequence, n_seq * T rows of FRAME_STACK_BYTES.  Strips: T + 3 rows per sequence
+    (the last three windows of a strip straddle into the next one and are never read), n_seq * (T + 3) - 3 rows, the
+    last of which ends at the end of the last strip."""
+    if strip:
+        return T + 3, n_seq * (T + 3) - 3, FRAME_BYTES
+    return T, n_seq * T, FRAME_STACK_BYTES
+
+
+def strip_windows(strips: torch.Tensor) -> torch.Tensor:
+    """The window view of contiguous uint8 strips (n_seq, T + 3, 84, 84): a (n_seq * (T + 3) - 3, 4, 84, 84) view
+    with strides (7056, 7056, 84, 1), whose row s * (T + 3) + t is stack t of sequence s.  Zero-copy."""
+    assert strips.dtype == torch.uint8 and strips.dim() == 4 and strips.shape[2:] == (84, 84) and strips.is_contiguous()
+    _, rows, _ = sequence_rows(strips.shape[0], strips.shape[1] - 3, True)
+    return strips.as_strided((rows, 4, 84, 84), (FRAME_BYTES, FRAME_BYTES, 84, 1))
+
+
+def strip_stacks(strips: torch.Tensor) -> torch.Tensor:
+    """The stack view of uint8 strips (B, T + 3, 84, 84) whose inner three dimensions are contiguous: a zero-copy
+    (B, T, 4, 84, 84) view whose values are the sequences' stacks."""
+    assert strips.dtype == torch.uint8 and strips.dim() == 4 and strips.shape[2:] == (84, 84) and strips[0].is_contiguous()
+    B, T = strips.shape[0], strips.shape[1] - 3
+    return strips.as_strided((B, T, 4, 84, 84), (strips.stride(0), FRAME_BYTES, FRAME_BYTES, 84, 1))
+
+
+def stacks_strips(stacks: torch.Tensor) -> torch.Tensor | None:
+    """The strips (B, T + 3, 84, 84) under a stack view made by strip_stacks, or None when `stacks` is not one."""
+    if stacks.dim() != 5 or stacks.stride()[1:] != (FRAME_BYTES, FRAME_BYTES, 84, 1):
+        return None
+    B, T = stacks.shape[0], stacks.shape[1]
+    return stacks.as_strided((B, T + 3, 84, 84), (stacks.stride(0), FRAME_BYTES, 84, 1))
+
+
+def as_stacks(state: torch.Tensor) -> torch.Tensor:
+    """R2D2 `state` rows as the learner reads them, (B, T, 4, 84, 84): strips through their stack view, stacks as
+    they are."""
+    return strip_stacks(state) if state.ndim == 4 else state
+
+
+def encode_strip(stacks, out: np.ndarray, record: int = 0) -> None:
+    """One record's T stacks (an iterable of (4, 84, 84) uint8 arrays, e.g. a (T, 4, 84, 84) array) -> its strip
+    `out` (T + 3, 84, 84): out[0:4] = s_0, out[3 + t] = s_t[3], after checking s_t[:3] == out[t:t+3].  A stack that
+    does not slide raises ValueError naming `record` (its position in the batch) and the step."""
+    T = out.shape[0] - 3
+    t = -1
+    for t, st in enumerate(stacks):
+        if t >= T:
+            raise ValueError(f"record {record}: more than {T} stacks")
+        st = np.asarray(st, np.uint8).reshape(4, 84, 84)
+        if t == 0:
+            out[0:3] = st[:3]
+        elif not np.array_equal(st[:3], out[t:t + 3]):
+            raise ValueError(f"record {record}: stack {t} is not stack {t - 1} shifted by one frame, so the sequence "
+                             "cannot be stored as a frame strip (FRAME_STRIP)")
+        out[3 + t] = st[3]
+    if t != T - 1:
+        raise ValueError(f"record {record}: {t + 1} stacks, not {T}")
+
+
+def encode_strips(stacks) -> np.ndarray:
+    """(n, T, 4, 84, 84) uint8 stacks -> (n, T + 3, 84, 84) strips (encode_strip per record).  Every record is
+    checked before anything is returned, so a caller that pushes the result pushes all of the batch or none of it."""
+    stacks = stacks.cpu().numpy() if torch.is_tensor(stacks) else np.asarray(stacks)
+    n, T = stacks.shape[:2]
+    out = np.empty((n, T + 3, 84, 84), np.uint8)
+    for i in range(n):
+        encode_strip(stacks[i], out[i], i)
+    return out
 
 
 def impala_fields(T: int = 20):
@@ -468,11 +551,14 @@ def conv1_pack_jobs(jobs) -> None:
 @dataclass(frozen=True)
 class BoundFrames:
     """A frame source whose base address lives in device memory: entry `entry` of the int64 `table` holds the
-    address of `rows` frame stacks (b2rl_serve_bind writes it when a served minibatch slot is bound).  conv1_fused /
-    conv1_wgrad read the entry when their kernels start, so a CUDA graph that captured them follows every rebind."""
+    address of `rows` frame rows, `row_stride` bytes apart (b2rl_serve_bind writes it when a served minibatch slot is
+    bound).  conv1_fused / conv1_wgrad read the entry when their kernels start, so a CUDA graph that captured them
+    follows every rebind.  `row_stride`: FRAME_STACK_BYTES for frame stacks, FRAME_BYTES for the windows of frame
+    strips (sequence_rows)."""
     table: torch.Tensor
     entry: int
     rows: int
+    row_stride: int = FRAME_STACK_BYTES
 
     @property
     def device(self) -> torch.device:
@@ -484,26 +570,29 @@ class BoundFrames:
 
 
 def _frame_source(frames):
-    """-> (rows, the frames' pointer or the table entry's, whether it is a table entry)."""
+    """-> (rows, row stride in bytes, the frames' pointer or None, the table entry's pointer or None).  A tensor's rows
+    are its first dimension, each a contiguous FRAME_STACK_BYTES; stride(0) is the row stride (the library checks
+    that it is a positive multiple of 16)."""
     if isinstance(frames, BoundFrames):
-        return frames.rows, frames.entry_ptr(), True
-    assert frames.dtype == torch.uint8 and frames.is_contiguous() and frames[0].numel() == FRAME_STACK_BYTES
-    return frames.shape[0], frames.data_ptr(), False
+        return frames.rows, frames.row_stride, None, frames.entry_ptr()
+    assert frames.dtype == torch.uint8 and frames[0].is_contiguous() and frames[0].numel() == FRAME_STACK_BYTES
+    stride = frames.stride(0) if frames.shape[0] > 1 else FRAME_STACK_BYTES   # a size-1 dimension's stride is arbitrary
+    return frames.shape[0], stride * frames.element_size(), frames.data_ptr(), None
 
 
 def conv1_fused(frames, idx, pack: Conv1Pack, relu: bool = False, out=None):
-    """frames: uint8 (rows, 4, 84, 84) contiguous (e.g. DeviceReplay.field_view("state")), or a BoundFrames;
+    """frames: uint8 (rows, 4, 84, 84) with its inner three dimensions contiguous: frame stacks (e.g.
+    DeviceReplay.field_view("state")), the windows of frame strips (strip_windows), or a BoundFrames;
     idx: int64[n] rows to take (None: all rows in order).
     -> list of n_nets tensors (n, c_out, 20, 20) fp32 in channels_last memory format."""
-    rows, ptr, table = _frame_source(frames)
+    rows, row_stride, ptr, entry = _frame_source(frames)
     n = rows if idx is None else idx.numel()
     dev = frames.device
     if out is None:
         out = torch.empty((pack.n_nets, n, 20, 20, pack.c_out), dtype=torch.float32, device=dev)
-    lib = _lib.load()
-    check((lib.b2rl_conv1_fused_table if table else lib.b2rl_conv1_fused)(
-        ptr, rows, None if idx is None else idx.data_ptr(), n, pack.bq.data_ptr(), pack.scale.data_ptr(), pack.n_nets,
-        pack.c_out, out.data_ptr(), int(bool(relu)), _stream_ptr(dev)))
+    check(_lib.load().b2rl_conv1_fused_strided(
+        ptr, entry, row_stride, rows, None if idx is None else idx.data_ptr(), n, pack.bq.data_ptr(),
+        pack.scale.data_ptr(), pack.n_nets, pack.c_out, out.data_ptr(), int(bool(relu)), _stream_ptr(dev)))
     return [out[i].permute(0, 3, 1, 2) for i in range(pack.n_nets)]   # logical NCHW, physical NHWC
 
 
@@ -513,10 +602,10 @@ _wgrad_ws = {}
 def conv1_wgrad(frames, idx, gy: torch.Tensor, out: torch.Tensor | None = None,
                 accumulate: bool = False, relu_y: torch.Tensor | None = None) -> torch.Tensor:
     """dL/dW of conv_1 from the sampled uint8 rows and dL/dy, without staging the rows (b2rl_conv1_wgrad).
-    frames: uint8 (rows, 4, 84, 84) contiguous, or a BoundFrames; idx: int64[n] or None; gy: (n, c_out, 20, 20) fp32
+    frames: as for conv1_fused; idx: int64[n] or None; gy: (n, c_out, 20, 20) fp32
     (made channels_last if it is not) -> (c_out, 4, 8, 8) fp32.  relu_y: the post-ReLU output of
     conv1_fused(relu=True) for the same rows; gy is then dL/d(relu output) and is masked by (y > 0) in the kernel."""
-    rows, ptr, table = _frame_source(frames)
+    rows, row_stride, ptr, entry = _frame_source(frames)
     n = rows if idx is None else idx.numel()
     c_out = gy.shape[1]
     assert gy.shape == (n, c_out, 20, 20) and gy.dtype == torch.float32
@@ -533,9 +622,8 @@ def conv1_wgrad(frames, idx, gy: torch.Tensor, out: torch.Tensor | None = None,
         out = torch.empty((c_out, 4, 8, 8), dtype=torch.float32, device=dev)
         accumulate = False
     assert out.is_contiguous() and out.numel() == c_out * 256
-    lib = _lib.load()
-    check((lib.b2rl_conv1_wgrad_table if table else lib.b2rl_conv1_wgrad)(
-        ptr, rows, None if idx is None else idx.data_ptr(), n, gy.data_ptr(),
+    check(_lib.load().b2rl_conv1_wgrad_strided(
+        ptr, entry, row_stride, rows, None if idx is None else idx.data_ptr(), n, gy.data_ptr(),
         None if relu_y is None else relu_y.data_ptr(), c_out, _wgrad_ws[key].data_ptr(), out.data_ptr(),
         int(bool(accumulate)), _stream_ptr(dev)))
     return out

@@ -91,8 +91,18 @@ def _apex_batch(b, w, idx):
 
 
 def _r2d2_batch(b, w, idx):
-    """R2D2/ReplayMemory.py:74-120 (r2d2.Replay.buffer): [(h0, h1), s, a, r, notdone, w, idx], h0 / h1 (1, B, 512)."""
-    return [(b["h0"].unsqueeze(0), b["h1"].unsqueeze(0)), b["state"], b["action"], b["reward"], b["notdone"], w, idx]
+    """R2D2/ReplayMemory.py:74-120 (r2d2.Replay.buffer): [(h0, h1), s, a, r, notdone, w, idx], h0 / h1 (1, B, 512),
+    s (B, T, 4, 84, 84): the stack view of frame strips."""
+    return [(b["h0"].unsqueeze(0), b["h1"].unsqueeze(0)), R.as_stacks(b["state"]), b["action"], b["reward"],
+            b["notdone"], w, idx]
+
+
+def _r2d2_host(name, t):
+    """A pickled R2D2 `BATCH` keeps the reference's format: h0 / h1 stay torch (:100-101), s is the (B, T, 4, 84, 84)
+    stack array, materialised here from frame strips."""
+    if name in ("h0", "h1"):
+        return t
+    return np.ascontiguousarray(R.as_stacks(t).numpy()) if name == "state" else t.numpy()
 
 
 def _impala_batch(b, w, idx):
@@ -104,8 +114,7 @@ KINDS = {
     "apex": RecordKind("apex", apex.Replay, lambda cfg: R.APEX_FIELDS, _apex_batch,
                        lambda name, t: t.numpy().astype(bool) if name == "done" else t.numpy(),
                        m=32, enough=32),                      # APE_X/ReplayServer.py:66, APE_X/ReplayMemory.py:232
-    "r2d2": RecordKind("r2d2", r2d2.Replay, lambda cfg: R.r2d2_fields(cfg.FIXED_TRAJECTORY), _r2d2_batch,
-                       lambda name, t: t if name in ("h0", "h1") else t.numpy(),   # h0 / h1 stay torch (:100-101)
+    "r2d2": RecordKind("r2d2", r2d2.Replay, R.r2d2_config_fields, _r2d2_batch, _r2d2_host,
                        m=8, enough=18),                       # R2D2/ReplayServer.py:66, R2D2/ReplayMemory.py:249
     "impala": RecordKind("impala", impala.Replay, lambda cfg: R.impala_fields(cfg.UNROLL_STEP), _impala_batch,
                          None, m=1, enough=0, list_key="trajectory",           # IMPALA/ReplayMemory.py:56-76
@@ -297,9 +306,10 @@ def serve_layout(batch: int, slots: int, field_bytes) -> _lib.ServeLayout:
 def bind_targets(batch: int, fields, out: dict, frames: dict):
     """The per-field arguments of b2rl_serve_bind for a slot of `batch` records: (copy destinations, frame table
     entries), one pointer per field, null for a field that is neither copied nor bound.  A copied field's buffer holds
-    exactly its `batch` rows.  A bound frame field holds field_bytes / FRAME_STACK_BYTES frame stacks per record
-    (Ape-X one, an R2D2 sequence T, an IMPALA rollout T + 1), so its BoundFrames must cover batch times that many
-    rows: conv_1 reads no further than the slot."""
+    exactly its `batch` rows.  A bound frame field's BoundFrames must cover exactly the FRAME_STACK_BYTES rows, its
+    row_stride apart, that fit in the slot's batch * field_bytes: conv_1 reads no further than the slot.  For frame
+    stacks that is batch times field_bytes / FRAME_STACK_BYTES (Ape-X one per record, an R2D2 sequence T, an IMPALA
+    rollout T + 1); for the windows of R2D2 frame strips, batch * (T + 3) - 3."""
     fo, to = (C.c_void_p * _lib.MAX_FIELDS)(), (C.c_void_p * _lib.MAX_FIELDS)()
     for i, f in enumerate(fields):
         if f.name in out:
@@ -307,11 +317,12 @@ def bind_targets(batch: int, fields, out: dict, frames: dict):
             assert t.is_contiguous() and t.numel() * t.element_size() == batch * f.nbytes, f.name
             fo[i] = t.data_ptr()
         elif f.name in frames:
-            stacks, rest = divmod(f.nbytes, R.FRAME_STACK_BYTES)
-            if rest or frames[f.name].rows != batch * stacks:
+            bf = frames[f.name]
+            span = batch * f.nbytes - R.FRAME_STACK_BYTES
+            if span < 0 or bf.rows != span // bf.row_stride + 1:
                 raise ValueError(f"field {f.name!r} holds {f.nbytes / R.FRAME_STACK_BYTES:g} frame stacks per record: "
-                                 f"a slot of {batch} records has {batch * f.nbytes / R.FRAME_STACK_BYTES:g} frame rows, "
-                                 f"not the {frames[f.name].rows} of its BoundFrames")
+                                 f"a slot of {batch} records has {max(span // bf.row_stride + 1, 0)} frame rows "
+                                 f"{bf.row_stride} bytes apart, not the {bf.rows} of its BoundFrames")
             to[i] = frames[f.name].entry_ptr()
     return fo, to
 

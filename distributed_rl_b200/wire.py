@@ -84,13 +84,16 @@ def _hidden(h, hidden: int) -> np.ndarray:
     return t.reshape(-1)[:hidden].astype(np.float32)
 
 
-def decode_r2d2(recs, T: int, hidden: int = 512):
+def decode_r2d2(recs, T: int, hidden: int = 512, strip: bool = False):
     """R2D2 records (object arrays): rec[0] = (h0, h1) each (1,1,hidden); rec[1+3t], rec[2+3t], rec[3+3t]
     = s_t (4,84,84) u8, a_t, r_t; rec[-2] = done; rec[-1] = priority.  Exactly the indexing of
     R2D2/ReplayMemory.py:70-88 (`done` becomes notdone = float(not done), :86).
+    `strip`: state is written as frame strips (n, T + 3, 84, 84) straight from the records (replay.encode_strip); a
+    record whose stacks do not slide raises ValueError naming its position, before anything is returned.
     -> ([state, action, reward, h0, h1, notdone], priorities)"""
+    from .replay import encode_strip
     n = len(recs)
-    s = np.empty((n, T, 4, 84, 84), np.uint8)
+    s = np.empty((n, T + 3, 84, 84) if strip else (n, T, 4, 84, 84), np.uint8)
     a = np.empty((n, T), np.int32)
     rw = np.empty((n, T), np.float32)
     h0 = np.empty((n, hidden), np.float32)
@@ -99,8 +102,11 @@ def decode_r2d2(recs, T: int, hidden: int = 512):
     p = np.empty(n, np.float32)
     for i, r in enumerate(recs):
         h0[i], h1[i] = _hidden(r[0][0], hidden), _hidden(r[0][1], hidden)
+        if strip:
+            encode_strip((r[1 + 3 * t] for t in range(T)), s[i], i)
         for t in range(T):
-            s[i, t] = np.asarray(r[1 + 3 * t], np.uint8).reshape(4, 84, 84)
+            if not strip:
+                s[i, t] = np.asarray(r[1 + 3 * t], np.uint8).reshape(4, 84, 84)
             a[i, t] = int(r[2 + 3 * t])
             rw[i, t] = float(r[3 + 3 * t])
         nd[i] = float(not r[-2])

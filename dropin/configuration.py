@@ -20,6 +20,7 @@ elif ALG == "R2D2":
     FIXED_TRAJECTORY = DATA["FIXED_TRAJECTORY"]
     MEM = DATA["MEM"]
     USE_RESCALING = DATA["USE_RESCALING"]
+    FRAME_STRIP = bool(DATA.get("FRAME_STRIP", False))   # not a reference key: store sequences as frame strips
 elif ALG == "IMPALA":
     C_LAMBDA = DATA["C_LAMBDA"]
     C_VALUE = DATA["C_VALUE"]

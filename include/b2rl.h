@@ -291,6 +291,24 @@ int b2rl_conv1_wgrad_table(const uint8_t* const* frame_table_dev, int64_t capaci
                            int64_t n, const float* gy_dev, const float* y_relu_dev, int32_t c_out,
                            float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream);
 
+/* conv_1 forward and weight gradient over frame rows `row_stride` bytes apart: row r is the 28 224 bytes that start
+ * at base + r * row_stride.  A stride of 28 224 reads whole frame stacks, exactly as b2rl_conv1_fused / _wgrad (and
+ * their _table forms, which call these with that stride).  A stride of 7 056 reads the overlapping 4-frame windows
+ * of an R2D2 frame strip: a sequence of T observations stored as its T + 3 distinct 84x84 frames, where stack t is
+ * frames t .. t + 3 (R2D2/Player.py:38-63 stacks the last four frames of one episode, and R2D2/ReplayMemory.py:70-88
+ * stores T such stacks per sequence).  Exactly one of frames_dev (the base, 16-byte aligned) and frame_table_dev
+ * (one device-resident entry holding the base, 8-byte aligned, as for the _table forms) is non-null.  `rows` is the
+ * number of rows indices are clamped to: the caller guarantees that row rows - 1 ends inside the allocation.  An
+ * error, and no launch, for a stride that is not a positive multiple of 16 or a null or misaligned source. */
+int b2rl_conv1_fused_strided(const uint8_t* frames_dev, const uint8_t* const* frame_table_dev, int64_t row_stride,
+                             int64_t rows, const int64_t* idx_dev, int64_t n, const int8_t* bq_dev,
+                             const float* scale_dev, int32_t n_nets, int32_t c_out, float* out_dev, int32_t relu,
+                             void* stream);
+int b2rl_conv1_wgrad_strided(const uint8_t* frames_dev, const uint8_t* const* frame_table_dev, int64_t row_stride,
+                             int64_t rows, const int64_t* idx_dev, int64_t n, const float* gy_dev,
+                             const float* y_relu_dev, int32_t c_out, float* workspace_dev, float* gw_dev,
+                             int32_t accumulate, void* stream);
+
 /* Learner.step (APE_X/Learner.py:123-138; IMPALA/Learner.py:258-266 without the clipping) with
  * torch.optim.RMSprop's update (baseline/utils.py getOptim :124-130; centered for Ape-X,
  * cfg/ape_x.json:27-35) in ONE pass: square_avg / grad_avg / param update, gradient zeroed, and
