@@ -70,6 +70,14 @@ SIGNATURES = {
                                            c_i32, c_vp]),
     "b2rl_conv1_wgrad_strided": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp,
                                            c_i32, c_vp]),
+    "b2rl_conv1_fused_planes": (C.c_int, [c_vp, c_vp, c_i32, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_vp,
+                                          c_i32, c_vp]),
+    "b2rl_conv1_wgrad_planes": (C.c_int, [c_vp, c_vp, c_i32, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp,
+                                          c_i32, c_vp]),
+    "b2rl_dedup_attach": (C.c_int, [c_vp, c_i32, c_i64, c_i64, c_u64]),
+    "b2rl_dedup_push": (C.c_int, [c_vp, c_vp, c_vp, C.POINTER(c_vp), c_vp, c_i64, c_vp]),
+    "b2rl_dedup_info": (C.c_int, [c_vp, C.POINTER(c_vp), C.POINTER(c_i64), C.POINTER(c_i64)]),
+    "b2rl_replay_gather_planes": (C.c_int, [c_vp, c_vp, c_i64, C.POINTER(c_vp), C.POINTER(c_vp), c_vp]),
     "b2rl_rmsprop_step": (C.c_int, [C.POINTER(c_vp), C.POINTER(c_vp), C.POINTER(c_vp), C.POINTER(c_vp),
                                     C.POINTER(c_i64), c_i32, c_f64, c_f64, c_f64, c_i32, C.POINTER(c_i64), c_vp, c_vp,
                                     c_vp]),

@@ -62,6 +62,11 @@ class ApexConfig:
     BATCHED_ONLINE: bool = True     # the online net's two passes (s with grad, s' without) as ONE B = 2*BATCHSIZE call
     SERVED_FUSED_STEP: bool = False  # on a served replay (DeviceReplayClient), run() steps the captured fused step on
                                      # the bound ring slot instead of sample() -> train() -> update()
+    FRAME_DEDUP: bool = False        # store every distinct frame once, in a pool of FRAMES_PER_TRANSITION frames per
+                                     # slot (R.DedupReplay, DESIGN.md §4.16): samples are the same, the replay smaller
+    FRAMES_PER_TRANSITION: float = 4.0
+    DEDUP_WINDOW: int = 1 << 20      # a frame is reused only from the last DEDUP_WINDOW frames stored (at most 1/8 of
+                                     # the pool, see dedup_geometry)
 
     @staticmethod
     def from_configuration():
@@ -70,7 +75,25 @@ class ApexConfig:
                                          "REPLAY_MEMORY_LEN", "BUFFER_SIZE", "TARGET_FREQUENCY",
                                          "LEARNER_DEVICE", "REDIS_SERVER", "OPTIM_INFO", "MODEL")}
         kw["LOG_W"] = getattr(C, "LOG_W", None)
+        for k in ("FRAME_DEDUP", "FRAMES_PER_TRANSITION", "DEDUP_WINDOW"):     # optional keys of cfg/ape_x.json
+            if hasattr(C, k):
+                kw[k] = getattr(C, k)
         return ApexConfig(**kw)
+
+
+def dedup_geometry(cfg: ApexConfig) -> tuple:
+    """(pool frames, window) of a FRAME_DEDUP replay: ceil(FRAMES_PER_TRANSITION * REPLAY_MEMORY_LEN) frames, and
+    DEDUP_WINDOW capped at an eighth of them.  A slot stays live until pool - window frames have been stored after it,
+    so the cap keeps that at least 7/8 of the pool: ~2.3 REPLAY_MEMORY_LEN records at the ~3 new frames per record
+    the reference actor sends, more than the slot ring holds."""
+    import math
+    import warnings
+    F = int(math.ceil(cfg.FRAMES_PER_TRANSITION * cfg.REPLAY_MEMORY_LEN))
+    W = min(int(cfg.DEDUP_WINDOW), F // 8)
+    if W < cfg.DEDUP_WINDOW:
+        warnings.warn(f"DEDUP_WINDOW = {cfg.DEDUP_WINDOW} frames is more than an eighth of the {F}-frame pool: the "
+                      f"frame-deduplicated replay uses a window of {W} frames", stacklevel=2)
+    return F, W
 
 
 def default_apex_model() -> dict:
@@ -95,7 +118,10 @@ class Replay(ReplayThread):
 
     def __init__(self, cfg: ApexConfig | None = None, connect=None):
         super().__init__(cfg or ApexConfig.from_configuration(), connect)
-        self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, R.APEX_FIELDS, self.device)
+        if self.cfg.FRAME_DEDUP:
+            self.store = R.DedupReplay(self.cfg.REPLAY_MEMORY_LEN, *dedup_geometry(self.cfg), device=self.device)
+        else:
+            self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, R.APEX_FIELDS, self.device)
         self.memory = MemoryView(self.store, self.cfg.BETA)
 
     # -- ingest: records are [s, a, R_n, s', done, prio] pickled by the actors ----
@@ -127,7 +153,7 @@ class Replay(ReplayThread):
             st["event"].synchronize()
         if st is None or st["cap"] < n:
             cap = max(n, 2 * (st["cap"] if st else 0), 64)
-            shape = tuple(self.store.fields[0].shape)
+            shape = tuple(R.APEX_FIELDS[0].shape)
             st = {"cap": cap, "event": torch.cuda.Event(),
                   "s": pinned_empty((cap, *shape), torch.uint8, self.device),
                   "ns": pinned_empty((cap, *shape), torch.uint8, self.device),
@@ -442,7 +468,7 @@ class Learner(TargetNetLearner):
             st, src_s, src_ns, rows = None, s.frames["state"], s.frames["next_state"], None
         else:
             st = self.memory.store
-            src_s, src_ns, rows = st.field_view("state"), st.field_view("next_state"), idx
+            src_s, src_ns, rows = st.frame_source("state"), st.frame_source("next_state"), idx
         w_on = getattr(self.model, s.conv_name).conv_1.weight
         if not prepacked:
             self._pack_weights()

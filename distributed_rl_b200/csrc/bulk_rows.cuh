@@ -30,7 +30,11 @@ struct BulkField {
   int64_t row_bytes;    // is_bulk_row
   int32_t chunks;       // ceil(row_bytes / CHUNK); time-major: steps * ceil(step_bytes / CHUNK)
   int32_t step_bytes;   // time-major destination only: bytes of one time step of the row (a multiple of 16)
+  const int32_t* planes;   // plane rows only: 8 pool ids per replay row; chunk c of a row is pool frame planes[8 row +
+  int32_t plane_base;      // plane_base + c] (src is the frame pool), so a frame stack is four PLANE_BYTES copies
 };
+
+constexpr int PLANE_BYTES = 84 * 84;   // one frame of the deduplicated Ape-X store's pool
 
 struct BulkRows {
   BulkField f[B2RL_MAX_FIELDS];
@@ -39,15 +43,22 @@ struct BulkRows {
   int32_t pad;
 
   void add(const uint8_t* src, uint8_t* dst, int64_t row_bytes, int chunk) {
-    f[n] = BulkField{src, dst, row_bytes, (int32_t)((row_bytes + chunk - 1) / chunk), 0};
+    f[n] = BulkField{src, dst, row_bytes, (int32_t)((row_bytes + chunk - 1) / chunk), 0, nullptr, 0};
     items_per_row += f[n].chunks;
+    ++n;
+  }
+  // Frame stacks assembled from a frame pool: output row k is planes plane_base .. plane_base + 3 of replay row
+  // row_of(k), one chunk per plane (the copy loop's CHUNK must be at least PLANE_BYTES).
+  void add_planes(const uint8_t* pool, const int32_t* planes, int32_t plane_base, uint8_t* dst) {
+    f[n] = BulkField{pool, dst, 4 * PLANE_BYTES, 4, 0, planes, plane_base};
+    items_per_row += 4;
     ++n;
   }
   // A row of `steps` time steps whose step t of draw k goes to output row t * batch + k: chunked per step, so no
   // chunk straddles two steps and each one is a single bulk copy with a contiguous destination.
   void add_time_major(const uint8_t* src, uint8_t* dst, int64_t row_bytes, int64_t steps, int chunk) {
     const int64_t step = row_bytes / steps;
-    f[n] = BulkField{src, dst, row_bytes, (int32_t)(steps * ((step + chunk - 1) / chunk)), (int32_t)step};
+    f[n] = BulkField{src, dst, row_bytes, (int32_t)(steps * ((step + chunk - 1) / chunk)), (int32_t)step, nullptr, 0};
     items_per_row += f[n].chunks;
     ++n;
   }
@@ -79,6 +90,12 @@ struct ItemCursor {
       bytes = (uint32_t)(rem < CHUNK ? rem : CHUNK);
       src = T.f[f].src + row * T.f[f].row_bytes + (int64_t)t * step + off;
       dst = T.f[f].dst + ((int64_t)t * batch + dst_k0 + k) * step + off;
+      return;
+    }
+    if (T.f[f].planes != nullptr) {
+      bytes = PLANE_BYTES;
+      src = T.f[f].src + (int64_t)T.f[f].planes[row * 8 + T.f[f].plane_base + c] * PLANE_BYTES;
+      dst = T.f[f].dst + (dst_k0 + k) * T.f[f].row_bytes + (int64_t)c * PLANE_BYTES;
       return;
     }
     const int64_t off = (int64_t)c * CHUNK;

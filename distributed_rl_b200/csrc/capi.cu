@@ -25,6 +25,7 @@ extern "C" int b2rl_version(void) { return 100; }
 extern "C" int64_t b2rl_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 
 static void free_all(b2rl_replay* h) {
+  dedup_free(h);
   for (int f = 0; f < B2RL_MAX_FIELDS; ++f)
     if (h->field[f]) cudaFree(h->field[f]);
   if (h->tree.leaf) cudaFree(h->tree.leaf);

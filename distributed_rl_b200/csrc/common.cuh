@@ -139,6 +139,14 @@ struct b2rl_replay;
 namespace b2rl {
 // Stream-ordered publication of the host-side `size` to n_valid_dev (tree.cu).
 int publish_size(b2rl_replay* h, cudaStream_t st);
+// Record i of fields_src -> ring slot (start + i) % capacity; a NULL field is skipped (gather.cu).
+int copy_ring_range(b2rl_replay* h, const void* const* fields_src, int64_t start, int64_t n, cudaStream_t st);
+// The n records at head become sampleable with the device priorities prios_dev; head moves past them (gather.cu).
+int publish(b2rl_replay* h, const float* prios_dev, int64_t n, cudaStream_t st);
+struct DedupState;                        // the frame pool of a deduplicated Ape-X replay (dedup.cu)
+void dedup_free(b2rl_replay* h);
+int dedup_planes_field(const b2rl_replay* h);
+const uint8_t* dedup_pool(const b2rl_replay* h);
 }  // namespace b2rl
 
 // The opaque handle.
@@ -167,4 +175,5 @@ struct b2rl_replay {
   float* pipe_prios = nullptr;
   int64_t pipe_cap = 0;   // floats allocated at pipe_prios
   int64_t pipe_n = 0;     // records of the batch whose copy is in flight (0: none)
+  b2rl::DedupState* dedup = nullptr;   // b2rl_dedup_attach: frame pool, key table, insertion marks
 };

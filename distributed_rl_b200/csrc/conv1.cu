@@ -25,7 +25,7 @@
 //                thread = (tile row, channel pair)
 //   warp 16      TMA loader: weights once, then one 28 224-byte frame stack per item, from base + row * row_stride
 //                (a stride of 7 056 reads the overlapping 4-frame windows of a frame strip: channel c of row r is
-//                frame r + c)
+//                frame r + c), or as four 7 056-byte frames of a frame pool named by a plane table
 #include "common.cuh"
 #include "hopper.cuh"
 
@@ -121,8 +121,31 @@ struct TableParams : Params {
   const uint8_t* const* table;   // one entry: the field base
 };
 
+// The plane-table variant (b2rl_conv1_fused_planes): `frames` is a frame pool, and channel c of row r is pool frame
+// planes[8 r + plane_base + c].
+struct PlaneParams : Params {
+  const int32_t* planes;
+  int32_t plane_base;
+};
+
 __device__ __forceinline__ const uint8_t* frame_base(const Params& P) { return P.frames; }
 __device__ __forceinline__ const uint8_t* frame_base(const TableParams& P) { return *P.table; }
+
+// Row `row` -> `dst` in SMEM, completing FRAME_BYTES of transactions on `bar`: one bulk copy of a frame stack, or
+// four of a plane table's frames.
+__device__ __forceinline__ void load_row(const Params& P, const uint8_t* frames, int64_t row, uint8_t* dst,
+                                         uint64_t* bar) {
+  mbar_expect_tx(bar, FRAME_BYTES);
+  bulk_g2s(dst, frames + row * P.row_stride, FRAME_BYTES, bar);
+}
+__device__ __forceinline__ void load_row(const PlaneParams& P, const uint8_t* frames, int64_t row, uint8_t* dst,
+                                         uint64_t* bar) {
+  constexpr int PLANE = HW * HW;
+  mbar_expect_tx(bar, FRAME_BYTES);
+#pragma unroll
+  for (int c = 0; c < C_IN; ++c)
+    bulk_g2s(dst + c * PLANE, frames + (int64_t)P.planes[row * 8 + P.plane_base + c] * PLANE, PLANE, bar);
+}
 
 template <int N> struct Acc;
 template <> struct Acc<128> {
@@ -177,8 +200,7 @@ k_conv1_fused(const __grid_constant__ PARAMS P) {
         mbar_wait(&raw_empty[s], ((it >> 1) & 1) ^ 1);
         int64_t row = P.idx ? P.idx[k] : k;
         row = row < 0 ? 0 : (row >= P.capacity ? P.capacity - 1 : row);
-        mbar_expect_tx(&raw_full[s], FRAME_BYTES);
-        bulk_g2s(sRaw + s * RAW_STRIDE, frames + row * P.row_stride, FRAME_BYTES, &raw_full[s]);
+        load_row(P, frames, row, sRaw + s * RAW_STRIDE, &raw_full[s]);
       }
     }
   } else if (warp >= CONSUMERS / 32) {
@@ -382,6 +404,22 @@ extern "C" int b2rl_conv1_fused_strided(const uint8_t* frames_dev, const uint8_t
   }
   conv1::TableParams P{};
   P.idx = idx_dev, P.n = n, P.capacity = rows, P.row_stride = row_stride, P.relu = relu, P.table = frame_table_dev;
+  return conv1_fused_run(P, bq_dev, scale_dev, n_nets, c_out, out_dev, stream);
+}
+
+extern "C" int b2rl_conv1_fused_planes(const uint8_t* pool_dev, const int32_t* planes_dev, int32_t plane_base,
+                                       int64_t rows, const int64_t* idx_dev, int64_t n, const int8_t* bq_dev,
+                                       const float* scale_dev, int32_t n_nets, int32_t c_out, float* out_dev,
+                                       int32_t relu, void* stream) {
+  B2RL_REQUIRE(n >= 0, "negative n");
+  B2RL_REQUIRE(pool_dev != nullptr && planes_dev != nullptr, "null frame pool or plane table");
+  B2RL_REQUIRE((uintptr_t)pool_dev % 16 == 0 && (uintptr_t)planes_dev % 4 == 0,
+               "the frame pool must be 16-byte aligned, the plane table 4-byte aligned");
+  B2RL_REQUIRE(plane_base == 0 || plane_base == 4, "plane_base must be 0 or 4");
+  if (n == 0) return B2RL_OK;
+  conv1::PlaneParams P{};
+  P.frames = pool_dev, P.idx = idx_dev, P.n = n, P.capacity = rows, P.row_stride = conv1::FRAME_BYTES, P.relu = relu;
+  P.planes = planes_dev, P.plane_base = plane_base;
   return conv1_fused_run(P, bq_dev, scale_dev, n_nets, c_out, out_dev, stream);
 }
 

@@ -68,8 +68,30 @@ struct TableParams : Params {
   int64_t frame_off;         // rows of the earlier launches of a split n (idx == nullptr), in bytes
 };
 
+// The plane-table variant (b2rl_conv1_wgrad_planes): `frames` is a frame pool, and channel c of row r is pool frame
+// planes[8 r + plane_base + c].
+struct PlaneParams : Params {
+  const int32_t* planes;
+  int32_t plane_base;
+};
+
 __device__ __forceinline__ const uint8_t* frame_base(const Params& P) { return P.frames; }
 __device__ __forceinline__ const uint8_t* frame_base(const TableParams& P) { return *P.table + P.frame_off; }
+
+// Row `row` -> `dst` in SMEM, completing FRAME_BYTES of transactions on `bar` (as in conv1.cu).
+__device__ __forceinline__ void load_row(const Params& P, const uint8_t* frames, int64_t row, uint8_t* dst,
+                                         uint64_t* bar) {
+  mbar_expect_tx(bar, FRAME_BYTES);
+  bulk_g2s(dst, frames + row * P.row_stride, FRAME_BYTES, bar);
+}
+__device__ __forceinline__ void load_row(const PlaneParams& P, const uint8_t* frames, int64_t row, uint8_t* dst,
+                                         uint64_t* bar) {
+  constexpr int PLANE = FRAME_BYTES / 4;
+  mbar_expect_tx(bar, FRAME_BYTES);
+#pragma unroll
+  for (int c = 0; c < 4; ++c)
+    bulk_g2s(dst + c * PLANE, frames + (int64_t)P.planes[row * 8 + P.plane_base + c] * PLANE, PLANE, bar);
+}
 
 template <int N> struct Acc;
 template <> struct Acc<128> {
@@ -120,8 +142,7 @@ k_conv1_wgrad(const __grid_constant__ PARAMS P) {
     if (k >= P.n) return;
     int64_t row = P.idx ? P.idx[k] : k;
     row = row < 0 ? 0 : (row >= P.capacity ? P.capacity - 1 : row);
-    mbar_expect_tx(&raw_full[it & 1], FRAME_BYTES);
-    bulk_g2s(sRaw + (it & 1) * RAW_STRIDE, frames + row * P.row_stride, FRAME_BYTES, &raw_full[it & 1]);
+    load_row(P, frames, row, sRaw + (it & 1) * RAW_STRIDE, &raw_full[it & 1]);
   };
   if (threadIdx.x == 0) load_frame(0);
 
@@ -365,10 +386,12 @@ extern "C" int64_t b2rl_conv1_wgrad_workspace_floats(int32_t c_out) {
 }
 
 // The launches of every conv_1 weight-gradient entry point.  `frames_dev` null: the frame base is the table entry
-// (read on the device, where the offset of each launch of a split n is added).
+// (read on the device, where the offset of each launch of a split n is added).  `planes_dev` non-null: frames_dev is
+// a frame pool read through that plane table (whose rows each launch of a split n advances).
 static int wgrad_run(const uint8_t* frames_dev, const uint8_t* const* table_dev, int64_t row_stride, int64_t capacity,
                      const int64_t* idx_dev, int64_t n, const float* gy_dev, const float* y_relu_dev, int32_t c_out,
-                     float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream) {
+                     float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream,
+                     const int32_t* planes_dev = nullptr, int32_t plane_base = 0) {
   B2RL_REQUIRE(gy_dev && workspace_dev && gw_dev, "null argument");
   B2RL_REQUIRE(c_out == 16 || c_out == 32, "c_out must be 16 or 32");
   B2RL_REQUIRE(capacity >= 1, "capacity must be positive");
@@ -389,7 +412,12 @@ static int wgrad_run(const uint8_t* frames_dev, const uint8_t* const* table_dev,
     const int64_t frame_off = idx_dev ? 0 : off * row_stride;
     if (!idx_dev) P.capacity = capacity - off;
     const unsigned grid = (unsigned)((m < sms) ? m : sms);
-    if (frames_dev) {
+    if (planes_dev) {
+      conv1w::PlaneParams Q{};
+      static_cast<conv1w::Params&>(Q) = P;
+      Q.frames = frames_dev, Q.planes = planes_dev + (idx_dev ? 0 : off * 8), Q.plane_base = plane_base;
+      B2RL_CUDA(c_out == 32 ? wgrad_launch<32>(Q, grid, st) : wgrad_launch<16>(Q, grid, st));
+    } else if (frames_dev) {
       P.frames = frames_dev + frame_off;
       B2RL_CUDA(c_out == 32 ? wgrad_launch<32>(P, grid, st) : wgrad_launch<16>(P, grid, st));
     } else {
@@ -435,4 +463,17 @@ extern "C" int b2rl_conv1_wgrad_table(const uint8_t* const* frame_table_dev, int
   B2RL_REQUIRE(frame_table_dev != nullptr, "null frame table");
   return b2rl_conv1_wgrad_strided(nullptr, frame_table_dev, conv1w::FRAME_BYTES, capacity, idx_dev, n, gy_dev,
                                   y_relu_dev, c_out, workspace_dev, gw_dev, accumulate, stream);
+}
+
+extern "C" int b2rl_conv1_wgrad_planes(const uint8_t* pool_dev, const int32_t* planes_dev, int32_t plane_base,
+                                       int64_t rows, const int64_t* idx_dev, int64_t n, const float* gy_dev,
+                                       const float* y_relu_dev, int32_t c_out, float* workspace_dev, float* gw_dev,
+                                       int32_t accumulate, void* stream) {
+  B2RL_REQUIRE(n >= 1, "n must be positive");
+  B2RL_REQUIRE(pool_dev != nullptr && planes_dev != nullptr, "null frame pool or plane table");
+  B2RL_REQUIRE((uintptr_t)pool_dev % 16 == 0 && (uintptr_t)planes_dev % 4 == 0,
+               "the frame pool must be 16-byte aligned, the plane table 4-byte aligned");
+  B2RL_REQUIRE(plane_base == 0 || plane_base == 4, "plane_base must be 0 or 4");
+  return wgrad_run(pool_dev, nullptr, conv1w::FRAME_BYTES, rows, idx_dev, n, gy_dev, y_relu_dev, c_out, workspace_dev,
+                   gw_dev, accumulate, stream, planes_dev, plane_base);
 }

@@ -1,0 +1,422 @@
+// Frame-deduplicated Ape-X store: ingest (hash -> resolve -> assign + copy) into a frame pool, and the bookkeeping of
+// its eviction rule (include/b2rl.h b2rl_dedup_*, DESIGN.md §4.16).
+//
+// A pushed batch of n records is 8n frames; frame j is plane j % 8 of record j / 8 (planes 0-3 of s, then of s').
+//   1. k_dedup_hash   one warp per frame: 64-bit content key, inserted into a batch table keyed by it that keeps the
+//                     lowest position holding each key
+//   2. k_dedup_resolve one warp per frame: a frame equal (all 7 056 bytes) to the lowest position with its key reuses
+//                     it; any other frame probes the key table, whose entry for a key is the newest stored frame with
+//                     that key, and reuses that frame when it lies inside the window and all its bytes are equal
+//   3. k_dedup_scan   the remaining frames (misses) get seq = head, head + 1, ... in batch order (one CTA)
+//   4. the host reads the miss count (one synchronisation), zeroes the priorities of the slots the eviction rule
+//      kills, then k_dedup_copy writes the 8 pool ids of every record, copies the misses into the pool and enters them
+//      in the key table; the other fields and the priorities follow as for b2rl_replay_push.
+// Everything a frame's id depends on is a function of the record stream (keys, positions, the window), so the ids
+// can be checked against a CPU model (tests/dedup_model.py).
+#include "common.cuh"
+
+#include <new>
+#include <vector>
+
+int b2rl_tree_update_impl(b2rl_replay* h, const int64_t* idx_dev, int64_t ring_start, const float* vals_dev,
+                          float const_val, int64_t n, cudaStream_t st, bool publish_size_too);
+
+namespace b2rl {
+
+constexpr int DD_FRAME = 84 * 84;                 // 7 056 bytes per frame
+constexpr int DD_STACK = 4 * DD_FRAME;            // 28 224 bytes per stack
+constexpr int DD_WORDS = DD_FRAME / 8;            // 882
+constexpr int DD_VEC = DD_FRAME / 16;             // 441
+constexpr unsigned long long DD_EMPTY = ~0ULL;    // key of an unused table entry (keys are below 2^63)
+constexpr unsigned long long DD_KEY_BITS = 0x7FFFFFFFFFFFFFFFULL;
+constexpr int64_t DD_MAX_BATCH = 8192;            // records per push
+constexpr int DD_THREADS = 256;                   // 8 frames per CTA
+
+struct DedupState {
+  int32_t planes_field = -1;
+  int64_t F = 0, W = 0, T = 0;                    // pool frames, window, key-table entries (a power of two)
+  unsigned long long mask = 0;
+  uint8_t* pool = nullptr;                        // [F][7056]
+  unsigned long long* pool_key = nullptr;         // [F] key of the frame in each pool slot, for table rebuilds
+  unsigned long long* tkey = nullptr;             // [T]
+  unsigned long long* tseq = nullptr;             // [T] 1 + seq of the newest frame stored under tkey (0: none)
+  int64_t used = 0;                               // table entries claimed since the last rebuild, at most
+  int64_t head = 0;                               // frames stored so far
+  int64_t max_batch = 0;
+  int64_t BT = 0;                                 // batch-table entries (a power of two >= 16 * max_batch)
+  unsigned long long* key = nullptr;              // [8 max_batch] per batch frame
+  int32_t* rep = nullptr;                         // [8 max_batch] position whose frame it reuses (itself if none)
+  int64_t* fseq = nullptr;                        // [8 max_batch] seq (-1 before the scan: a miss)
+  unsigned long long* bkey = nullptr;             // [BT]
+  int32_t* bpos = nullptr;                        // [BT] lowest batch position holding bkey
+  int64_t* misses_dev = nullptr;
+  int64_t* misses_host = nullptr;                 // pinned
+  cudaEvent_t done = nullptr;                     // recorded behind each push: the next one waits for it, so pushes
+                                                  // on different streams never share the scratch or the key table
+  std::vector<int64_t> ins;                       // per slot: head at the start of the batch that inserted it
+};
+
+__host__ __device__ __forceinline__ uint64_t mix64(uint64_t z) {   // splitmix64's finaliser
+  z ^= z >> 30; z *= 0xBF58476D1CE4E5B9ULL;
+  z ^= z >> 27; z *= 0x94D049BB133111EBULL;
+  return z ^ (z >> 31);
+}
+
+// Frame j of the batch: plane j % 8 of record j / 8.
+__device__ __forceinline__ const uint8_t* batch_frame(const uint8_t* s, const uint8_t* ns, int64_t j) {
+  const int64_t r = j >> 3;
+  const int c = (int)(j & 7);
+  return (c < 4 ? s : ns) + r * DD_STACK + (c & 3) * DD_FRAME;
+}
+
+__device__ __forceinline__ bool warp_equal(const uint8_t* a, const uint8_t* b, int lane) {
+  const uint4* x = reinterpret_cast<const uint4*>(a);
+  const uint4* y = reinterpret_cast<const uint4*>(b);
+  bool eq = true;
+  for (int i = lane; i < DD_VEC; i += 32) {
+    const uint4 u = x[i], v = y[i];
+    eq = eq && u.x == v.x && u.y == v.y && u.z == v.z && u.w == v.w;
+  }
+  return __all_sync(0xffffffffu, eq);
+}
+
+// Entry of `key` in an open-addressing table of `size` entries (claimed if absent).  The table never fills: the host
+// keeps at most half of its entries claimed.
+__device__ __forceinline__ int64_t claim(unsigned long long* keys, int64_t size, unsigned long long key) {
+  int64_t i = (int64_t)(key & (unsigned long long)(size - 1));
+  while (true) {
+    const unsigned long long old = atomicCAS(keys + i, DD_EMPTY, key);
+    if (old == DD_EMPTY || old == key) return i;
+    i = (i + 1) & (size - 1);
+  }
+}
+
+// Entry of `key`, or -1.
+__device__ __forceinline__ int64_t find(const unsigned long long* keys, int64_t size, unsigned long long key) {
+  int64_t i = (int64_t)(key & (unsigned long long)(size - 1));
+  while (true) {
+    const unsigned long long k = keys[i];
+    if (k == key) return i;
+    if (k == DD_EMPTY) return -1;
+    i = (i + 1) & (size - 1);
+  }
+}
+
+// key = mix64(sum over the frame's 8-byte words w_i of mix64(w_i ^ i * golden)) & mask, without its top bit.  The sum
+// is order-free, so the lanes' partial sums combine in any order.
+__global__ void __launch_bounds__(DD_THREADS)
+k_dedup_hash(const uint8_t* __restrict__ s, const uint8_t* __restrict__ ns, int64_t frames, unsigned long long mask,
+             unsigned long long* __restrict__ key, unsigned long long* __restrict__ bkey, int32_t* __restrict__ bpos,
+             int64_t BT) {
+  const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (j >= frames) return;
+  const uint64_t* w = reinterpret_cast<const uint64_t*>(batch_frame(s, ns, j));
+  uint64_t h = 0;
+  for (int i = lane; i < DD_WORDS; i += 32) h += mix64(w[i] ^ ((uint64_t)i * 0x9E3779B97F4A7C15ULL));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) h += __shfl_xor_sync(0xffffffffu, h, o);
+  if (lane == 0) {
+    const unsigned long long k = mix64(h) & mask & DD_KEY_BITS;
+    key[j] = k;
+    atomicMin(bpos + claim(bkey, BT, k), (int32_t)j);
+  }
+}
+
+struct ResolveArgs {
+  const uint8_t* s;
+  const uint8_t* ns;
+  int64_t frames;
+  const unsigned long long* key;
+  const unsigned long long* bkey;
+  const int32_t* bpos;
+  int64_t BT;
+  const unsigned long long* tkey;
+  const unsigned long long* tseq;
+  int64_t T;
+  const uint8_t* pool;
+  int64_t F;
+  int64_t oldest;           // head - W: the oldest seq a hit may reuse
+  int32_t* rep;
+  int64_t* fseq;
+};
+
+__global__ void __launch_bounds__(DD_THREADS)
+k_dedup_resolve(const __grid_constant__ ResolveArgs A) {
+  const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (j >= A.frames) return;
+  const unsigned long long k = A.key[j];
+  const uint8_t* me = batch_frame(A.s, A.ns, j);
+  const int32_t first = A.bpos[find(A.bkey, A.BT, k)];
+  if (first < j && warp_equal(batch_frame(A.s, A.ns, first), me, lane)) {
+    if (lane == 0) { A.rep[j] = first; A.fseq[j] = -2; }
+    return;
+  }
+  int64_t cand = -1;
+  if (lane == 0) {
+    const int64_t e = find(A.tkey, A.T, k);
+    if (e >= 0) {
+      const unsigned long long s1 = A.tseq[e];
+      if (s1 > 0 && (int64_t)(s1 - 1) >= A.oldest) cand = (int64_t)(s1 - 1);
+    }
+  }
+  cand = __shfl_sync(0xffffffffu, cand, 0);
+  const bool hit = cand >= 0 && warp_equal(A.pool + (cand % A.F) * DD_FRAME, me, lane);
+  if (lane == 0) { A.rep[j] = (int32_t)j; A.fseq[j] = hit ? cand : -1; }
+}
+
+// Misses (fseq == -1) get seq head, head + 1, ... in batch order; *misses = their count.  One CTA of 1024 threads.
+__global__ void __launch_bounds__(1024)
+k_dedup_scan(int64_t* __restrict__ fseq, int64_t frames, int64_t head, int64_t* __restrict__ misses) {
+  __shared__ int32_t s_warp[32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int64_t running = 0;
+  for (int64_t base = 0; base < frames; base += 1024) {
+    const int64_t j = base + threadIdx.x;
+    const int32_t flag = (j < frames && fseq[j] == -1) ? 1 : 0;
+    int32_t incl = flag;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int32_t v = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += v;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    if (warp == 0) {
+      int32_t w = s_warp[lane], wi = w;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int32_t v = __shfl_up_sync(0xffffffffu, wi, o);
+        if (lane >= o) wi += v;
+      }
+      s_warp[lane] = wi - w;          // exclusive prefix of the warp totals
+    }
+    __syncthreads();
+    if (flag) fseq[j] = head + running + s_warp[warp] + incl - 1;
+    const int32_t total = __shfl_sync(0xffffffffu, incl, 31);   // warp 31's inclusive total
+    __syncthreads();
+    if (warp == 31) s_warp[0] = s_warp[31] + total;
+    __syncthreads();
+    running += s_warp[0];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *misses = running;
+}
+
+struct CopyArgs {
+  const uint8_t* s;
+  const uint8_t* ns;
+  int64_t frames;
+  const unsigned long long* key;
+  const int32_t* rep;
+  const int64_t* fseq;
+  int64_t head;             // first seq of this batch's misses
+  uint8_t* pool;
+  unsigned long long* pool_key;
+  int64_t F;
+  unsigned long long* tkey;
+  unsigned long long* tseq;
+  int64_t T;
+  int32_t* planes;          // the replay's planes field
+  int64_t slot0, capacity;  // record r goes to slot (slot0 + r) % capacity
+};
+
+__global__ void __launch_bounds__(DD_THREADS)
+k_dedup_copy(const __grid_constant__ CopyArgs A) {
+  const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (j >= A.frames) return;
+  const int32_t r = A.rep[j];
+  const int64_t sq = A.fseq[r];
+  const int64_t ps = sq % A.F;
+  if (lane == 0) {
+    int64_t slot = A.slot0 + (j >> 3);
+    if (slot >= A.capacity) slot -= A.capacity;
+    A.planes[slot * 8 + (j & 7)] = (int32_t)ps;
+  }
+  if (r != j || sq < A.head) return;        // a batch duplicate or a hit: nothing to store
+  const uint4* src = reinterpret_cast<const uint4*>(batch_frame(A.s, A.ns, j));
+  uint4* dst = reinterpret_cast<uint4*>(A.pool + ps * DD_FRAME);
+  for (int i = lane; i < DD_VEC; i += 32) dst[i] = src[i];
+  if (lane == 0) {
+    const unsigned long long k = A.key[j];
+    A.pool_key[ps] = k;
+    atomicMax(A.tseq + claim(A.tkey, A.T, k), (unsigned long long)(sq + 1));
+  }
+}
+
+// The key table from scratch: the frames with seq in [lo, hi), newest per key.
+__global__ void __launch_bounds__(256)
+k_dedup_rebuild(const unsigned long long* __restrict__ pool_key, int64_t F, int64_t lo, int64_t hi,
+                unsigned long long* __restrict__ tkey, unsigned long long* __restrict__ tseq, int64_t T) {
+  const int64_t q = lo + (int64_t)blockIdx.x * 256 + threadIdx.x;
+  if (q >= hi) return;
+  atomicMax(tseq + claim(tkey, T, pool_key[q % F]), (unsigned long long)(q + 1));
+}
+
+void dedup_free(b2rl_replay* h) {
+  DedupState* d = h->dedup;
+  if (d == nullptr) return;
+  for (void* p : {(void*)d->pool, (void*)d->pool_key, (void*)d->tkey, (void*)d->tseq, (void*)d->key, (void*)d->rep,
+                  (void*)d->fseq, (void*)d->bkey, (void*)d->bpos, (void*)d->misses_dev})
+    if (p) cudaFree(p);
+  if (d->misses_host) cudaFreeHost(d->misses_host);
+  if (d->done) cudaEventDestroy(d->done);
+  delete d;
+  h->dedup = nullptr;
+}
+
+int dedup_planes_field(const b2rl_replay* h) { return h->dedup->planes_field; }
+const uint8_t* dedup_pool(const b2rl_replay* h) { return h->dedup->pool; }
+
+}  // namespace b2rl
+
+using namespace b2rl;
+
+static int64_t pow2_at_least(int64_t x) {
+  int64_t p = 1024;
+  while (p < x) p <<= 1;
+  return p;
+}
+
+extern "C" int b2rl_dedup_attach(b2rl_replay* h, int32_t planes_field, int64_t pool_frames, int64_t window,
+                                 uint64_t hash_mask) {
+  B2RL_REQUIRE(h != nullptr, "null handle");
+  B2RL_REQUIRE(h->dedup == nullptr, "the replay already has a frame pool");
+  B2RL_REQUIRE(h->size == 0 && h->head == 0 && h->reserved == 0 && h->pipe_n == 0, "the replay must be empty");
+  B2RL_REQUIRE(planes_field >= 0 && planes_field < h->n_fields && h->field_bytes[planes_field] == 32,
+               "the planes field must hold 8 int32 per slot");
+  B2RL_REQUIRE(window >= 0 && pool_frames - window > 8, "need window >= 0 and pool_frames - window > 8");
+  B2RL_REQUIRE(pool_frames < (1LL << 31), "pool_frames must be below 2^31");
+  DeviceGuard g(h->device);
+  DedupState* d = new (std::nothrow) DedupState();
+  if (!d) { set_error("out of host memory"); return B2RL_ERR_NOMEM; }
+  h->dedup = d;
+  d->planes_field = planes_field;
+  d->F = pool_frames;
+  d->W = window;
+  d->mask = (unsigned long long)hash_mask;
+  d->max_batch = (pool_frames - window - 1) / 8;
+  if (d->max_batch > DD_MAX_BATCH) d->max_batch = DD_MAX_BATCH;
+  if (d->max_batch > h->capacity) d->max_batch = h->capacity;
+  d->T = pow2_at_least(2 * (window + 8 * d->max_batch));   // at most half claimed: window + one batch
+  d->BT = pow2_at_least(16 * d->max_batch);
+  const int64_t nf = 8 * d->max_batch;
+  cudaError_t e = cudaSuccess;
+  auto alloc = [&](void** p, size_t bytes) {
+    if (e == cudaSuccess) e = cudaMalloc(p, bytes);
+  };
+  alloc((void**)&d->pool, (size_t)d->F * DD_FRAME);
+  alloc((void**)&d->pool_key, sizeof(unsigned long long) * (size_t)d->F);
+  alloc((void**)&d->tkey, sizeof(unsigned long long) * (size_t)d->T);
+  alloc((void**)&d->tseq, sizeof(unsigned long long) * (size_t)d->T);
+  alloc((void**)&d->key, sizeof(unsigned long long) * (size_t)nf);
+  alloc((void**)&d->rep, sizeof(int32_t) * (size_t)nf);
+  alloc((void**)&d->fseq, sizeof(int64_t) * (size_t)nf);
+  alloc((void**)&d->bkey, sizeof(unsigned long long) * (size_t)d->BT);
+  alloc((void**)&d->bpos, sizeof(int32_t) * (size_t)d->BT);
+  alloc((void**)&d->misses_dev, sizeof(int64_t));
+  if (e == cudaSuccess) e = cudaMallocHost((void**)&d->misses_host, sizeof(int64_t));
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&d->done, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaMemset(d->tkey, 0xFF, sizeof(unsigned long long) * (size_t)d->T);
+  if (e == cudaSuccess) e = cudaMemset(d->tseq, 0, sizeof(unsigned long long) * (size_t)d->T);
+  if (e == cudaSuccess) e = cudaMemset(h->field[planes_field], 0, (size_t)h->capacity * 32);
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {
+    set_error("allocating a %lld-frame pool failed: %s", (long long)pool_frames, cudaGetErrorString(e));
+    dedup_free(h);
+    cudaGetLastError();
+    return B2RL_ERR_NOMEM;
+  }
+  try {
+    d->ins.assign((size_t)h->capacity, 0);
+  } catch (...) {
+    dedup_free(h);
+    set_error("out of host memory");
+    return B2RL_ERR_NOMEM;
+  }
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_dedup_info(const b2rl_replay* h, void** pool_dev, int64_t* head_seq, int64_t* max_batch) {
+  B2RL_REQUIRE(h != nullptr, "null handle");
+  B2RL_REQUIRE(h->dedup != nullptr, "not a frame-deduplicated replay (b2rl_dedup_attach)");
+  if (pool_dev) *pool_dev = h->dedup->pool;
+  if (head_seq) *head_seq = h->dedup->head;
+  if (max_batch) *max_batch = h->dedup->max_batch;
+  return B2RL_OK;
+}
+
+static unsigned warps_grid(int64_t frames) { return (unsigned)((frames * 32 + DD_THREADS - 1) / DD_THREADS); }
+
+extern "C" int b2rl_dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8_t* ns_dev,
+                               const void* const* fields_src, const float* prios, int64_t n, void* stream) {
+  B2RL_REQUIRE(h != nullptr, "null handle");
+  DedupState* d = h->dedup;
+  B2RL_REQUIRE(d != nullptr, "not a frame-deduplicated replay (b2rl_dedup_attach)");
+  B2RL_REQUIRE(n >= 0 && n <= d->max_batch, "n out of range (0..max_batch of b2rl_dedup_info)");
+  if (n == 0) return B2RL_OK;
+  B2RL_REQUIRE(s_dev != nullptr && ns_dev != nullptr && prios != nullptr && fields_src != nullptr, "null argument");
+  B2RL_REQUIRE((uintptr_t)s_dev % 16 == 0 && (uintptr_t)ns_dev % 16 == 0, "frame stacks must be 16-byte aligned");
+  B2RL_REQUIRE(fields_src[d->planes_field] == nullptr, "the planes field is written by the push itself");
+  B2RL_REQUIRE(h->reserved == 0, "a reservation is pending");
+  DeviceGuard g(h->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t frames = 8 * n;
+  const int64_t head = d->head;
+  B2RL_CUDA(cudaStreamWaitEvent(st, d->done, 0));     // the previous push (on any stream) is done with the scratch
+  // 1. the key table: rebuilt from the window when this batch could take it past half full
+  if (d->used + frames > d->T / 2) {
+    const int64_t lo = head > d->W ? head - d->W : 0;
+    B2RL_CUDA(cudaMemsetAsync(d->tkey, 0xFF, sizeof(unsigned long long) * (size_t)d->T, st));
+    B2RL_CUDA(cudaMemsetAsync(d->tseq, 0, sizeof(unsigned long long) * (size_t)d->T, st));
+    if (head > lo) {
+      k_dedup_rebuild<<<(unsigned)((head - lo + 255) / 256), 256, 0, st>>>(d->pool_key, d->F, lo, head, d->tkey,
+                                                                           d->tseq, d->T);
+      count_launch();
+    }
+    d->used = head - lo;
+  }
+  // 2. keys, batch duplicates, hits, and the misses' seqs
+  B2RL_CUDA(cudaMemsetAsync(d->bkey, 0xFF, sizeof(unsigned long long) * (size_t)d->BT, st));
+  B2RL_CUDA(cudaMemsetAsync(d->bpos, 0x7F, sizeof(int32_t) * (size_t)d->BT, st));
+  k_dedup_hash<<<warps_grid(frames), DD_THREADS, 0, st>>>(s_dev, ns_dev, frames, d->mask, d->key, d->bkey, d->bpos,
+                                                          d->BT);
+  ResolveArgs A{s_dev, ns_dev, frames, d->key, d->bkey, d->bpos, d->BT, d->tkey, d->tseq, d->T, d->pool, d->F,
+                head - d->W, d->rep, d->fseq};
+  k_dedup_resolve<<<warps_grid(frames), DD_THREADS, 0, st>>>(A);
+  k_dedup_scan<<<1, 1024, 0, st>>>(d->fseq, frames, head, d->misses_dev);
+  count_launch(3);
+  B2RL_CHECK_LAUNCH();
+  B2RL_CUDA(cudaMemcpyAsync(d->misses_host, d->misses_dev, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  B2RL_CUDA(cudaStreamSynchronize(st));
+  const int64_t head_new = head + *d->misses_host;
+  // 3. the eviction rule: the oldest slots with F - W or more frames stored since their batch began lose their
+  //    priority, in stream order before their frames can be overwritten
+  int64_t tail = h->head - h->size;
+  if (tail < 0) tail += h->capacity;
+  int64_t dead = 0;
+  while (dead < h->size && head_new - d->ins[(size_t)((tail + dead) % h->capacity)] >= d->F - d->W) ++dead;
+  if (dead > 0) {
+    h->size -= dead;
+    int rc = b2rl_tree_update_impl(h, nullptr, tail, nullptr, 0.0f, dead, st, true);
+    if (rc != B2RL_OK) return rc;
+  }
+  // 4. pool ids, new frames, key table; then the other fields and the priorities as b2rl_replay_push does
+  CopyArgs C{s_dev, ns_dev, frames, d->key, d->rep, d->fseq, head, d->pool, d->pool_key, d->F, d->tkey, d->tseq, d->T,
+             (int32_t*)h->field[d->planes_field], h->head, h->capacity};
+  k_dedup_copy<<<warps_grid(frames), DD_THREADS, 0, st>>>(C);
+  count_launch();
+  B2RL_CHECK_LAUNCH();
+  int rc = copy_ring_range(h, fields_src, h->head, n, st);
+  if (rc != B2RL_OK) return rc;
+  B2RL_CUDA(cudaMemcpyAsync(h->scratch_val, prios, (size_t)n * sizeof(float), cudaMemcpyDefault, st));
+  for (int64_t i = 0; i < n; ++i) d->ins[(size_t)((h->head + i) % h->capacity)] = head;
+  rc = publish(h, h->scratch_val, n, st);
+  if (rc != B2RL_OK) return rc;
+  B2RL_CUDA(cudaEventRecord(d->done, st));
+  d->head = head_new;
+  d->used += head_new - head;
+  return B2RL_OK;
+}

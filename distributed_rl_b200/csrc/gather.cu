@@ -129,21 +129,23 @@ static int gather_mode() {
   return mode;
 }
 
-extern "C" int b2rl_replay_gather(b2rl_replay* h, const int64_t* idx_dev, int64_t n,
-                                  void* const* out_fields_dev, void* stream) {
-  B2RL_REQUIRE(h != nullptr, "null handle");
-  B2RL_REQUIRE(n >= 0, "negative n");
-  if (n == 0) return B2RL_OK;
-  B2RL_REQUIRE(idx_dev != nullptr && out_fields_dev != nullptr, "null argument");
-  DeviceGuard g(h->device);
-  cudaStream_t st = (cudaStream_t)stream;
-
+// b2rl_replay_gather, and for a dedup replay b2rl_replay_gather_planes: stacks_out (2 entries, or nullptr) receives
+// the frame stacks of planes 0-3 / 4-7, copied as plane rows by the same launch.
+static int gather_run(b2rl_replay* h, const int64_t* idx_dev, int64_t n, void* const* stacks_out,
+                      void* const* out_fields_dev, cudaStream_t st) {
   GatherParams P{};
   P.n = n;
   P.capacity = h->capacity;
+  if (stacks_out != nullptr) {
+    const int32_t* planes = (const int32_t*)h->field[dedup_planes_field(h)];
+    for (int i = 0; i < 2; ++i) {
+      B2RL_REQUIRE((uintptr_t)stacks_out[i] % 16 == 0, "frame stack outputs must be 16-byte aligned");
+      if (stacks_out[i] != nullptr) P.bulk.add_planes(dedup_pool(h), planes, 4 * i, (uint8_t*)stacks_out[i]);
+    }
+  }
   for (int f = 0; f < h->n_fields; ++f) {
-    uint8_t* out = (uint8_t*)out_fields_dev[f];
-    if (out == nullptr) continue;
+    uint8_t* out = out_fields_dev ? (uint8_t*)out_fields_dev[f] : nullptr;
+    if (out == nullptr || (stacks_out != nullptr && f == dedup_planes_field(h))) continue;
     const int64_t rb = h->field_bytes[f];
     const bool big = rb >= 1024;
     const bool bulk = is_bulk_row(rb) && ((uintptr_t)out % 16 == 0) && ((uintptr_t)h->field[f] % 16 == 0);
@@ -183,9 +185,31 @@ extern "C" int b2rl_replay_gather(b2rl_replay* h, const int64_t* idx_dev, int64_
   return B2RL_OK;
 }
 
+extern "C" int b2rl_replay_gather(b2rl_replay* h, const int64_t* idx_dev, int64_t n,
+                                  void* const* out_fields_dev, void* stream) {
+  B2RL_REQUIRE(h != nullptr, "null handle");
+  B2RL_REQUIRE(n >= 0, "negative n");
+  if (n == 0) return B2RL_OK;
+  B2RL_REQUIRE(idx_dev != nullptr && out_fields_dev != nullptr, "null argument");
+  DeviceGuard g(h->device);
+  return gather_run(h, idx_dev, n, nullptr, out_fields_dev, (cudaStream_t)stream);
+}
+
+extern "C" int b2rl_replay_gather_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, void* const* stacks_out_dev,
+                                         void* const* out_fields_dev, void* stream) {
+  B2RL_REQUIRE(h != nullptr, "null handle");
+  B2RL_REQUIRE(h->dedup != nullptr, "not a frame-deduplicated replay (b2rl_dedup_attach)");
+  B2RL_REQUIRE(n >= 0, "negative n");
+  if (n == 0) return B2RL_OK;
+  B2RL_REQUIRE(idx_dev != nullptr && stacks_out_dev != nullptr, "null argument");
+  DeviceGuard g(h->device);
+  return gather_run(h, idx_dev, n, stacks_out_dev, out_fields_dev, (cudaStream_t)stream);
+}
+
 extern "C" int b2rl_replay_fill_hash(b2rl_replay* h, int64_t n, uint32_t seed, void* stream) {
   B2RL_REQUIRE(h != nullptr, "null handle");
   B2RL_REQUIRE(n >= 0 && n <= h->capacity, "n out of range");
+  B2RL_REQUIRE(h->dedup == nullptr, "a frame-deduplicated replay holds pool ids, not hashable payload");
   DeviceGuard g(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   for (int f = 0; f < h->n_fields; ++f) {
@@ -203,9 +227,7 @@ extern "C" int b2rl_replay_fill_hash(b2rl_replay* h, int64_t n, uint32_t seed, v
   return publish_size(h, st);
 }
 
-// Record i of fields_src -> ring slot (start + i) % capacity, i < n; a NULL field is skipped.
-static int copy_ring_range(b2rl_replay* h, const void* const* fields_src, int64_t start, int64_t n,
-                           cudaStream_t st) {
+int b2rl::copy_ring_range(b2rl_replay* h, const void* const* fields_src, int64_t start, int64_t n, cudaStream_t st) {
   const int64_t first = (start + n <= h->capacity) ? n : (h->capacity - start);  // before the wrap
   for (int f = 0; f < h->n_fields; ++f) {
     const uint8_t* src = (const uint8_t*)fields_src[f];
@@ -218,8 +240,7 @@ static int copy_ring_range(b2rl_replay* h, const void* const* fields_src, int64_
   return B2RL_OK;
 }
 
-// The n records at head become sampleable with the device priorities prios_dev; head moves past them.
-static int publish(b2rl_replay* h, const float* prios_dev, int64_t n, cudaStream_t st) {
+int b2rl::publish(b2rl_replay* h, const float* prios_dev, int64_t n, cudaStream_t st) {
   h->size = (h->size + n > h->capacity) ? h->capacity : h->size + n;   // published by the update kernel itself
   int rc = b2rl_tree_update_impl(h, nullptr, h->head, prios_dev, 0.0f, n, st, true);
   if (rc != B2RL_OK) return rc;
@@ -241,6 +262,7 @@ extern "C" int b2rl_replay_push(b2rl_replay* h, const void* const* fields_src, c
   if (n == 0) return B2RL_OK;
   B2RL_REQUIRE(prios != nullptr, "null priorities");
   B2RL_REQUIRE(h->n_fields == 0 || fields_src != nullptr, "null fields");
+  B2RL_REQUIRE(h->dedup == nullptr, "a frame-deduplicated replay takes its records through b2rl_dedup_push");
   DeviceGuard g(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   int rc = copy_ring_range(h, fields_src, h->head, n, st);
@@ -253,6 +275,7 @@ extern "C" int b2rl_replay_reserve(b2rl_replay* h, int64_t n, int64_t* start_slo
   B2RL_REQUIRE(h != nullptr, "null handle");
   B2RL_REQUIRE(n >= 1 && n <= h->capacity, "n out of range (1..capacity)");
   B2RL_REQUIRE(h->reserved == 0, "a reservation is already pending (call b2rl_replay_commit first)");
+  B2RL_REQUIRE(h->dedup == nullptr, "a frame-deduplicated replay takes its records through b2rl_dedup_push");
   DeviceGuard g(h->device);
   int rc = retire(h, n, (cudaStream_t)stream);
   if (rc != B2RL_OK) return rc;
@@ -291,6 +314,7 @@ extern "C" int b2rl_replay_ingest_pipelined(b2rl_replay* h, const void* const* f
                                             int64_t n, void* stream) {
   B2RL_REQUIRE(h != nullptr, "null handle");
   B2RL_REQUIRE(fields_src == nullptr || (n >= 1 && n <= h->capacity && prios_src != nullptr), "bad batch");
+  B2RL_REQUIRE(h->dedup == nullptr, "a frame-deduplicated replay takes its records through b2rl_dedup_push");
   DeviceGuard g(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   if (h->ingest_stream == nullptr) {

@@ -218,10 +218,27 @@ extern "C" int b2rl_serve_layout_init(int64_t batch, int32_t slots, int32_t n_fi
   return B2RL_OK;
 }
 
+// The fields a ring slot carries for replay h: its own fields, except that a frame-deduplicated replay's planes field
+// becomes two frame stacks (planes 0-3, then 4-7), so the slot holds the stack store's record layout.  -> count.
+static int served_fields(const b2rl_replay* h, int64_t* bytes) {
+  int n = 0;
+  for (int f = 0; f < h->n_fields; ++f) {
+    if (h->dedup != nullptr && f == dedup_planes_field(h)) {
+      bytes[n++] = 4 * PLANE_BYTES;
+      bytes[n++] = 4 * PLANE_BYTES;
+    } else {
+      bytes[n++] = h->field_bytes[f];
+    }
+  }
+  return n;
+}
+
 extern "C" int b2rl_serve_ring_create(b2rl_replay* h, int64_t batch, int32_t slots, b2rl_serve_ring** out) {
   B2RL_REQUIRE(h != nullptr && out != nullptr, "null argument");
+  B2RL_REQUIRE(h->dedup == nullptr || h->n_fields < B2RL_MAX_FIELDS, "too many fields to serve");
   b2rl_serve_layout L;
-  int rc = b2rl_serve_layout_init(batch, slots, h->n_fields, h->field_bytes, &L);
+  int64_t bytes[B2RL_MAX_FIELDS];
+  int rc = b2rl_serve_layout_init(batch, slots, served_fields(h, bytes), bytes, &L);
   if (rc != B2RL_OK) return rc;
   DeviceGuard g(h->device);
   b2rl_serve_ring* r = new (std::nothrow) b2rl_serve_ring();
@@ -336,9 +353,12 @@ static int fill_slot_ptrs(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, void
   B2RL_REQUIRE(h != nullptr && r != nullptr, "null argument");
   B2RL_REQUIRE(r->owned && r->device == h->device, "fill needs the ring created for this replay, on its device");
   B2RL_REQUIRE(slot >= 0 && slot < r->L.slots, "slot out of range");
-  B2RL_REQUIRE(r->L.n_fields == h->n_fields, "ring and replay have different fields");
-  for (int f = 0; f < h->n_fields; ++f)
-    B2RL_REQUIRE(h->field_bytes[f] == r->L.field_bytes[f], "ring and replay have different fields");
+  B2RL_REQUIRE(h->dedup == nullptr || h->n_fields < B2RL_MAX_FIELDS, "too many fields to serve");
+  int64_t bytes[B2RL_MAX_FIELDS];
+  const int n = served_fields(h, bytes);
+  B2RL_REQUIRE(r->L.n_fields == n, "ring and replay have different fields");
+  for (int f = 0; f < n; ++f)
+    B2RL_REQUIRE(bytes[f] == r->L.field_bytes[f], "ring and replay have different fields");
   B2RL_REQUIRE(h->size > 0, "sampling from an empty replay");
   return b2rl_serve_slot_ptrs(r, slot, ptrs, nullptr);
 }
@@ -362,17 +382,21 @@ extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot,
   BulkRows P{};
   SmallFields small{};
   SmallRows rows{};
-  for (int f = 0; f < h->n_fields; ++f) {
+  for (int f = 0, o = 3; f < h->n_fields; ++f, ++o) {
     const int64_t b = h->field_bytes[f];
-    if (is_bulk_row(b)) {
-      P.add(h->field[f], (uint8_t*)ptrs[3 + f], b, 14336);   // the CHUNK of k_serve_fill's copy_rows
+    if (h->dedup != nullptr && f == dedup_planes_field(h)) {   // s and s' stacks assembled from the frame pool
+      const int32_t* planes = (const int32_t*)h->field[f];
+      P.add_planes(dedup_pool(h), planes, 0, (uint8_t*)ptrs[o]);
+      P.add_planes(dedup_pool(h), planes, 4, (uint8_t*)ptrs[++o]);
+    } else if (is_bulk_row(b)) {
+      P.add(h->field[f], (uint8_t*)ptrs[o], b, 14336);   // the CHUNK of k_serve_fill's copy_rows
     } else if (b == 1 || b == 2 || b == 4 || b == 8) {
       small.src[small.n] = h->field[f];
-      small.dst[small.n] = (uint8_t*)ptrs[3 + f];
+      small.dst[small.n] = (uint8_t*)ptrs[o];
       small.bytes[small.n] = (int)b;
       small.n++;
     } else {
-      rows.f[rows.n++] = SmallField{h->field[f], (uint8_t*)ptrs[3 + f], b};
+      rows.f[rows.n++] = SmallField{h->field[f], (uint8_t*)ptrs[o], b};
     }
   }
   DeviceGuard g(h->device);
@@ -397,6 +421,7 @@ extern "C" int b2rl_serve_fill_uniform(b2rl_replay* h, b2rl_serve_ring* r, int32
   int rc = fill_slot_ptrs(h, r, slot, ptrs);
   if (rc != B2RL_OK) return rc;
   B2RL_REQUIRE(steps >= 1, "steps must be >= 1");
+  B2RL_REQUIRE(h->dedup == nullptr, "a frame-deduplicated replay holds Ape-X transitions, not rollouts");
   const int64_t n = r->L.batch, size = h->size, cap = h->capacity;
   B2RL_REQUIRE(n <= size, "sample larger than population: the batch exceeds the stored records");
   B2RL_REQUIRE(size <= (1LL << 32), "a uniform fill draws from at most 2^32 records");

@@ -560,6 +560,7 @@ extern "C" int b2rl_tree_build(b2rl_replay* h, const float* prios_dev, int64_t n
   B2RL_REQUIRE(h != nullptr, "null handle");
   B2RL_REQUIRE(n >= 0 && n <= h->capacity, "n out of range");
   B2RL_REQUIRE(n == 0 || prios_dev != nullptr, "null priorities");
+  B2RL_REQUIRE(h->dedup == nullptr, "a frame-deduplicated replay's slots are made live by b2rl_dedup_push");
   DeviceGuard g(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   const TreeView& t = h->tree;

@@ -45,6 +45,12 @@ APEX_FIELDS = (  # [s, a, R_n, s', done, prio]  APE_X/Player.py:252-261
 )
 
 
+# The frame-deduplicated Ape-X store (ApexConfig.FRAME_DEDUP, DESIGN.md §4.16): per slot 8 int32 pool ids, planes 0-3
+# of s then planes 0-3 of s', into a library-owned ring of 84x84 frames; the scalar fields are APEX_FIELDS' own.
+APEX_DEDUP_FIELDS = (Field("planes", torch.int32, (8,)),) + APEX_FIELDS[2:]
+DEDUP_HASH_MASK = (1 << 63) - 1     # every key bit; a test passes 0 to make every frame collide
+
+
 def r2d2_fields(T: int = 80, hidden: int = 512, strip: bool = False):
     """[(h0,h1), (s,a,r) x T, done, prio]  R2D2/ReplayMemory.py:70-88.  `strip`: `state` holds the sequence's T + 3
     distinct frames (T + 3, 84, 84) instead of its T stacks (T, 4, 84, 84); stack t is frames t .. t + 3."""
@@ -433,6 +439,10 @@ class DeviceReplay:
         check(self.lib.b2rl_replay_gather(self._h, idx.data_ptr(), n, ptrs, self._st()))
         return out
 
+    def frame_source(self, name: str):
+        """What conv1_fused / conv1_wgrad read frame field `name` from: its zero-copy view."""
+        return self.field_view(name)
+
     def uniform_fetch(self, n: int, steps: int, out: dict) -> dict:
         """n distinct rollouts of `steps` steps drawn uniformly WITHOUT replacement from the valid region
         [head - size, head) (random.sample, baseline/utils.py:310-315) on the device-resident Philox stream, with
@@ -455,6 +465,90 @@ class DeviceReplay:
         check(self.lib.b2rl_uniform_fetch(self._h, int(n), int(steps), idx.data_ptr(), ptrs,
                                           None if rows is None else rows.data_ptr(), self._st()))
         return out
+
+
+class DedupReplay(DeviceReplay):
+    """An Ape-X replay that stores every distinct frame once (b2rl_dedup_attach): slots hold APEX_DEDUP_FIELDS, the
+    frames live in a pool of `pool_frames` frames, and a pushed frame reuses a stored one with the same content among
+    the last `window` frames stored.  push / gather / sample / update / evict take and return what a DeviceReplay of
+    APEX_FIELDS does, bit for bit; a slot also stops being live once pool_frames - window frames have been stored
+    since its batch began (len() counts live slots).  The pipelined ingest forms are refused."""
+
+    def __init__(self, capacity: int, pool_frames: int, window: int, device="cuda:0",
+                 hash_mask: int = DEDUP_HASH_MASK):
+        super().__init__(capacity, APEX_DEDUP_FIELDS, device)
+        check(self.lib.b2rl_dedup_attach(self._h, 0, int(pool_frames), int(window), int(hash_mask)))
+        self.pool_frames, self.window = int(pool_frames), int(window)
+        p, mb = C.c_void_p(), C.c_int64()
+        check(self.lib.b2rl_dedup_info(self._h, C.byref(p), None, C.byref(mb)))
+        self.max_batch = mb.value
+        with torch.cuda.device(self.device):
+            self.pool = torch.as_tensor(_CudaView(p.value, (self.pool_frames, 84, 84), "|u1", self), device=self.device)
+
+    @property
+    def head_seq(self) -> int:
+        """Frames stored so far: the next new frame's sequence number (it goes to pool slot head_seq % pool_frames)."""
+        h = C.c_int64()
+        check(self.lib.b2rl_dedup_info(self._h, None, C.byref(h), None))
+        return h.value
+
+    def push(self, fields: Sequence, priorities) -> None:
+        """fields: [state, next_state, action, reward, done] as for a DeviceReplay of APEX_FIELDS (host, pinned
+        preferred, or device).  The stacks are staged on the device (the same host->device bytes as a stack store),
+        then pushed in chunks of at most max_batch records; each chunk synchronizes the current stream once."""
+        s, ns, rest = fields[0], fields[1], list(fields[2:])
+        pr = torch.as_tensor(priorities).to(torch.float32).contiguous()
+        n = pr.numel()
+        small = []
+        for f, x in zip(APEX_FIELDS[2:], rest):
+            t = torch.as_tensor(x)
+            t = (t if t.dtype == f.dtype else t.to(f.dtype)).contiguous()
+            assert t.numel() * t.element_size() == n * f.nbytes, f"bad shape for {f.name}"
+            small.append(t)
+        stacks = []
+        for x in (s, ns):
+            t = torch.as_tensor(x)
+            assert t.dtype == torch.uint8 and t.numel() == n * FRAME_STACK_BYTES, "frame stacks must be uint8 (n, 4, 84, 84)"
+            stacks.append(t.reshape(n, FRAME_STACK_BYTES).to(self.device, non_blocking=True).contiguous())
+        ptrs = (C.c_void_p * _lib.MAX_FIELDS)()
+        for a in range(0, n, self.max_batch):
+            b = min(n, a + self.max_batch)
+            ptrs[0] = None
+            for i, t in enumerate(small):
+                ptrs[1 + i] = t[a:b].data_ptr()
+            check(self.lib.b2rl_dedup_push(self._h, stacks[0][a:b].data_ptr(), stacks[1][a:b].data_ptr(), ptrs,
+                                           pr[a:b].data_ptr(), b - a, self._st()))
+        self._inflight = stacks + small + [pr]
+
+    def push_begin(self, fields, n):
+        raise ValueError("a frame-deduplicated replay (FRAME_DEDUP) has no pipelined ingest: use push")
+
+    def ingest_pipelined(self, fields, priorities=None):
+        raise ValueError("a frame-deduplicated replay (FRAME_DEDUP) has no pipelined ingest: use push")
+
+    def fill_hash(self, n: int, seed: int = 0xB200):
+        raise ValueError("a frame-deduplicated replay (FRAME_DEDUP) holds pool ids, not hashable payload")
+
+    def alloc_batch(self, n: int, names: Sequence[str] | None = None):
+        return alloc_rows(APEX_FIELDS, n, self.device, names)
+
+    def gather(self, idx: torch.Tensor, out: dict | None = None) -> dict:
+        """The sampled slots' fields as a DeviceReplay of APEX_FIELDS returns them: state and next_state are (n, 4,
+        84, 84) stacks assembled from the pool (b2rl_replay_gather_planes)."""
+        n = idx.numel()
+        if out is None:
+            out = self.alloc_batch(n)
+        stacks = (C.c_void_p * 2)(*[out[k].data_ptr() if out.get(k) is not None else None
+                                    for k in ("state", "next_state")])
+        ptrs = (C.c_void_p * _lib.MAX_FIELDS)()
+        for i, f in enumerate(self.fields):
+            t = out.get(f.name) if i > 0 else None
+            ptrs[i] = t.data_ptr() if t is not None else None
+        check(self.lib.b2rl_replay_gather_planes(self._h, idx.data_ptr(), n, stacks, ptrs, self._st()))
+        return out
+
+    def frame_source(self, name: str) -> "PlaneFrames":
+        return PlaneFrames(self.pool, self.field_view("planes"), {"state": 0, "next_state": 4}[name])
 
 
 # ---- stateless target kernels -------------------------------------------------
@@ -569,6 +663,20 @@ class BoundFrames:
         return self.table.data_ptr() + 8 * self.entry
 
 
+@dataclass(frozen=True)
+class PlaneFrames:
+    """Frame stacks held as a plane table over a frame pool (DedupReplay): row r is the stack whose channel c is
+    pool frame planes[r, base + c].  `pool`: uint8 (F, 84, 84); `planes`: int32 (rows, 8); `base`: 0 for `state`, 4
+    for `next_state`.  conv1_fused / conv1_wgrad read the four frames of each row in place."""
+    pool: torch.Tensor
+    planes: torch.Tensor
+    base: int
+
+    @property
+    def device(self) -> torch.device:
+        return self.pool.device
+
+
 def _frame_source(frames):
     """-> (rows, row stride in bytes, the frames' pointer or None, the table entry's pointer or None).  A tensor's rows
     are its first dimension, each a contiguous FRAME_STACK_BYTES; stride(0) is the row stride (the library checks
@@ -582,9 +690,18 @@ def _frame_source(frames):
 
 def conv1_fused(frames, idx, pack: Conv1Pack, relu: bool = False, out=None):
     """frames: uint8 (rows, 4, 84, 84) with its inner three dimensions contiguous: frame stacks (e.g.
-    DeviceReplay.field_view("state")), the windows of frame strips (strip_windows), or a BoundFrames;
+    DeviceReplay.field_view("state")), the windows of frame strips (strip_windows), a BoundFrames or a PlaneFrames;
     idx: int64[n] rows to take (None: all rows in order).
     -> list of n_nets tensors (n, c_out, 20, 20) fp32 in channels_last memory format."""
+    if isinstance(frames, PlaneFrames):
+        n = frames.planes.shape[0] if idx is None else idx.numel()
+        if out is None:
+            out = torch.empty((pack.n_nets, n, 20, 20, pack.c_out), dtype=torch.float32, device=frames.device)
+        check(_lib.load().b2rl_conv1_fused_planes(
+            frames.pool.data_ptr(), frames.planes.data_ptr(), frames.base, frames.planes.shape[0],
+            None if idx is None else idx.data_ptr(), n, pack.bq.data_ptr(), pack.scale.data_ptr(), pack.n_nets,
+            pack.c_out, out.data_ptr(), int(bool(relu)), _stream_ptr(frames.device)))
+        return [out[i].permute(0, 3, 1, 2) for i in range(pack.n_nets)]
     rows, row_stride, ptr, entry = _frame_source(frames)
     n = rows if idx is None else idx.numel()
     dev = frames.device
@@ -605,7 +722,8 @@ def conv1_wgrad(frames, idx, gy: torch.Tensor, out: torch.Tensor | None = None,
     frames: as for conv1_fused; idx: int64[n] or None; gy: (n, c_out, 20, 20) fp32
     (made channels_last if it is not) -> (c_out, 4, 8, 8) fp32.  relu_y: the post-ReLU output of
     conv1_fused(relu=True) for the same rows; gy is then dL/d(relu output) and is masked by (y > 0) in the kernel."""
-    rows, row_stride, ptr, entry = _frame_source(frames)
+    planes = isinstance(frames, PlaneFrames)
+    rows, row_stride, ptr, entry = (frames.planes.shape[0], 0, None, None) if planes else _frame_source(frames)
     n = rows if idx is None else idx.numel()
     c_out = gy.shape[1]
     assert gy.shape == (n, c_out, 20, 20) and gy.dtype == torch.float32
@@ -622,6 +740,12 @@ def conv1_wgrad(frames, idx, gy: torch.Tensor, out: torch.Tensor | None = None,
         out = torch.empty((c_out, 4, 8, 8), dtype=torch.float32, device=dev)
         accumulate = False
     assert out.is_contiguous() and out.numel() == c_out * 256
+    if planes:
+        check(_lib.load().b2rl_conv1_wgrad_planes(
+            frames.pool.data_ptr(), frames.planes.data_ptr(), frames.base, rows, None if idx is None else idx.data_ptr(),
+            n, gy.data_ptr(), None if relu_y is None else relu_y.data_ptr(), c_out, _wgrad_ws[key].data_ptr(),
+            out.data_ptr(), int(bool(accumulate)), _stream_ptr(dev)))
+        return out
     check(_lib.load().b2rl_conv1_wgrad_strided(
         ptr, entry, row_stride, rows, None if idx is None else idx.data_ptr(), n, gy.data_ptr(),
         None if relu_y is None else relu_y.data_ptr(), c_out, _wgrad_ws[key].data_ptr(), out.data_ptr(),

@@ -16,6 +16,10 @@ ALG = DATA["ALG"]
 BASE_PATH = f"./log/{ALG}"
 if ALG == "APE_X":
     USE_REWARD_CLIP = DATA.get("USE_REWARD_CLIP", True)
+    FRAME_DEDUP = bool(DATA.get("FRAME_DEDUP", False))   # not a reference key: store every distinct frame once
+    for _k in ("FRAMES_PER_TRANSITION", "DEDUP_WINDOW"):
+        if _k in DATA:
+            globals()[_k] = DATA[_k]
 elif ALG == "R2D2":
     FIXED_TRAJECTORY = DATA["FIXED_TRAJECTORY"]
     MEM = DATA["MEM"]

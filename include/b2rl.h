@@ -190,6 +190,40 @@ int b2rl_tree_leaves(b2rl_replay* h, int64_t start, int64_t n, float* out_dev, v
 int b2rl_replay_gather(b2rl_replay* h, const int64_t* idx_dev, int64_t n,
                        void* const* out_fields_dev, void* stream);
 
+/* Frame-deduplicated Ape-X store.  An Ape-X record (APE_X/Player.py:252-261) carries two frame stacks, s and s', and
+ * most of their frames repeat: LocalBuffer.get_traj (APE_X/Player.py:33-57) makes record k's s' record k + 1's s,
+ * stacks UNROLL_STEP steps apart share frames, and an episode starts with one frame four times (:203-209).
+ *
+ * b2rl_dedup_attach turns the replay into one whose field `planes_field` (32 bytes per slot) holds 8 int32 pool ids
+ * (planes 0-3 of s, then of s') into a library-owned ring of `pool_frames` 84x84 frames; frame sequence number seq
+ * lives in pool slot seq mod pool_frames.  A frame of a pushed batch reuses a stored frame only when that frame has
+ * seq >= head - window (head: frames stored before the batch), its key (64-bit content hash & hash_mask) matches and
+ * all 7 056 bytes compare equal.  A slot is live while the slot ring has not overwritten it and fewer than
+ * pool_frames - window frames have been stored since the batch that inserted it began; slots that stop being live
+ * get priority 0 before the pool is overwritten.  hash_mask is for tests (0 makes every frame collide);
+ * normal use passes ~0.  Requires window >= 0 and pool_frames - window > 8 (one record) and pool_frames < 2^31.
+ *
+ * b2rl_dedup_push: PER.push (baseline/PER.py:69-75) of n records on a dedup replay.  s_dev / ns_dev: device (n, 4,
+ * 84, 84) uint8 stacks; fields_src: the other fields as for b2rl_replay_push (the planes entry must be NULL).  The
+ * call synchronizes `stream` once, to learn how many frames the batch adds.  n <= *max_batch of b2rl_dedup_info.
+ * Pushes may come from different streams: each one waits for the previous one's work before it starts.  The host
+ * calls themselves must not overlap (one thread at a time, as for every entry point on a handle).
+ * b2rl_replay_push, _reserve, _ingest_pipelined, _fill_hash, b2rl_tree_build and b2rl_serve_fill_uniform refuse a
+ * dedup replay.  b2rl_serve_ring_create / b2rl_serve_fill serve it with the stack store's record layout: the planes
+ * field becomes two (B, 4, 84, 84) frame-stack fields (s, then s') in the ring slot, assembled from the pool.
+ *
+ * b2rl_dedup_info: *pool_dev (the frame pool), *head_seq (frames stored so far), *max_batch (records per push).
+ *
+ * b2rl_replay_gather_planes: b2rl_replay_gather for a dedup replay, plus the sampled slots' s and s' stacks
+ * (Replay.buffer, APE_X/ReplayMemory.py:61-116): stacks_out_dev[0] / [1] (either may be NULL) receive (n, 4, 84,
+ * 84) uint8 assembled from planes 0-3 / 4-7 by TMA bulk copies.  out_fields_dev[planes_field] is ignored. */
+int b2rl_dedup_attach(b2rl_replay* h, int32_t planes_field, int64_t pool_frames, int64_t window, uint64_t hash_mask);
+int b2rl_dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8_t* ns_dev, const void* const* fields_src,
+                    const float* prios, int64_t n, void* stream);
+int b2rl_dedup_info(const b2rl_replay* h, void** pool_dev, int64_t* head_seq, int64_t* max_batch);
+int b2rl_replay_gather_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, void* const* stacks_out_dev,
+                              void* const* out_fields_dev, void* stream);
+
 /* IMPALA's minibatch for a captured learner step (IMPALA/ReplayMemory.py:30-54, drawn as random.sample draws,
  * baseline/utils.py:310-315) in ONE launch: n rollouts drawn uniformly WITHOUT replacement from the ring's valid
  * region [head - size, head) with exactly the permutation of b2rl_serve_fill_uniform (same slots from the same
@@ -308,6 +342,19 @@ int b2rl_conv1_wgrad_strided(const uint8_t* frames_dev, const uint8_t* const* fr
                              int64_t rows, const int64_t* idx_dev, int64_t n, const float* gy_dev,
                              const float* y_relu_dev, int32_t c_out, float* workspace_dev, float* gw_dev,
                              int32_t accumulate, void* stream);
+
+/* conv_1 forward and weight gradient over frame stacks held as plane tables (the frame-deduplicated Ape-X store,
+ * b2rl_dedup_attach): row r is the stack whose channel c is the 7 056-byte frame pool_dev + planes_dev[8 r +
+ * plane_base + c] * 7 056 (plane_base 0: `state`, 4: `next_state` of the transition APE_X/Player.py:252-261 sends).
+ * Same arithmetic, outputs and arguments otherwise as b2rl_conv1_fused_strided / _wgrad_strided; `rows` is the
+ * number of plane-table rows indices are clamped to.  An error, and no launch, for a null or misaligned pool or
+ * table, or a plane_base other than 0 or 4. */
+int b2rl_conv1_fused_planes(const uint8_t* pool_dev, const int32_t* planes_dev, int32_t plane_base, int64_t rows,
+                            const int64_t* idx_dev, int64_t n, const int8_t* bq_dev, const float* scale_dev,
+                            int32_t n_nets, int32_t c_out, float* out_dev, int32_t relu, void* stream);
+int b2rl_conv1_wgrad_planes(const uint8_t* pool_dev, const int32_t* planes_dev, int32_t plane_base, int64_t rows,
+                            const int64_t* idx_dev, int64_t n, const float* gy_dev, const float* y_relu_dev,
+                            int32_t c_out, float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream);
 
 /* Learner.step (APE_X/Learner.py:123-138; IMPALA/Learner.py:258-266 without the clipping) with
  * torch.optim.RMSprop's update (baseline/utils.py getOptim :124-130; centered for Ape-X,
