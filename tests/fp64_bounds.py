@@ -1,0 +1,322 @@
+"""fp64 references and per-element error bounds of the library's hand-written kernels, shared by the GPU tests that hold
+conv_1 (forward and weight gradient), the 3xTF32 dense layers, the dueling tail and the fused RMSprop to fp64 at the
+learners' step shapes (test_gpu_22_step_shapes, test_gpu_25_apex_step_shapes).
+
+Every output element is held to its own bound, computed by the same fp64 reference applied to absolute values
+(`mag`), so the bound grows with the length of the sum behind that element; u = 2^-24.  The bound of each kernel is
+written in its checker's docstring.  The fp64 references run on the device, a chunk of frame stacks at a time; the
+frames are drawn on the device from seeded generators.  Importing this module needs torch, not a GPU."""
+import math
+
+import torch
+
+F = torch.nn.functional
+
+U = 2.0 ** -24
+CHUNK = 512                     # frame stacks per fp64 reference chunk (im2col of 512 stacks in fp64: 420 MB)
+
+
+def _gen(seed):
+    return torch.Generator(device="cuda").manual_seed(seed)
+
+
+def _frames(n, seed):
+    return torch.randint(0, 256, (n, 4, 84, 84), dtype=torch.uint8, device="cuda", generator=_gen(seed))
+
+
+class _Worst:
+    """Largest |got - ref| / tol over the chunks of one check, and where it occurs."""
+
+    def __init__(self, what):
+        self.what, self.ratio, self.where = what, 0.0, None
+
+    def add(self, got, ref, tol, at=""):
+        err = (got.double() - ref).abs()
+        r = torch.where(err == 0, torch.zeros_like(err), err / tol).nan_to_num(nan=math.inf)
+        k = int(r.argmax())
+        v = r.reshape(-1)[k].item()
+        if v > self.ratio or self.where is None:
+            pos = []
+            for s in reversed(r.shape):
+                pos.append(k % s)
+                k //= s
+            pos = tuple(reversed(pos))
+            self.ratio = max(v, self.ratio)
+            self.where = (at, pos, got.double()[pos].item(), ref[pos].item(), tol[pos].item())
+
+    def check(self):
+        print(f"[err/tol] {self.what}: {self.ratio:.3g}")
+        assert self.ratio <= 1.0, (f"{self.what}: largest |got - ref| / tol = {self.ratio:.3g} at (chunk, index, got, "
+                                   f"ref, tol) = {self.where}")
+        return self.ratio
+
+
+# --------------------------------------------------------------------------- #
+# conv_1                                                                        #
+# --------------------------------------------------------------------------- #
+def check_conv1(what, frames, idx, weights, outs, relu):
+    """conv1_fused output `outs[i]` (n, C, 20, 20) of net i against F.conv2d(x / 255, W_i) in fp64, per element
+        |got - ref| <= 2^-22 s_c sum_e x_e / 255 + 4u |ref|,      s_c = max|W_c| / 127,
+    the first term the four 7-bit digits' truncation |W - s sum_j q_j 2^-7j| <= s 2^-22 times the patch sum, the second
+    the fp32 roundings after the exact integer sums (two conversions, one FMA, the scale).  |ref| is the value before
+    the ReLU, which can only shrink the difference."""
+    n = outs[0].shape[0]
+    ones = torch.ones(1, 4, 8, 8, dtype=torch.float64, device="cuda")
+    worst = [_Worst(f"{what} net {i}") for i in range(len(weights))]
+    wd = [w.double() for w in weights]
+    sc = [(w.abs().amax(dim=(1, 2, 3)).float() / 127.0).double().view(1, -1, 1, 1) for w in weights]
+    for a in range(0, n, CHUNK):
+        b = min(n, a + CHUNK)
+        x = (frames[a:b] if idx is None else frames[idx[a:b]]).double() / 255.0
+        sx = F.conv2d(x, ones, stride=4)
+        for i, o in enumerate(outs):
+            ref = F.conv2d(x, wd[i], stride=4)
+            tol = 2.0 ** -22 * sc[i] * sx + 4 * U * ref.abs()
+            worst[i].add(o[a:b], ref.clamp_min(0) if relu else ref, tol, at=a)
+        del x, sx
+    return [w.check() for w in worst]
+
+
+def wgrad_ref(frames, idx, gy, relu_y=None):
+    """-> (dW, mag = sum |gy| x, S_e = sum_{k,p} x_e, G_c = max |gy_c|) in fp64, gy masked by relu_y > 0 when given."""
+    n, c = gy.shape[:2]
+    ref = torch.zeros(c, 256, dtype=torch.float64, device="cuda")
+    mag, S = torch.zeros_like(ref), torch.zeros(256, dtype=torch.float64, device="cuda")
+    G = torch.zeros(c, dtype=torch.float64, device="cuda")
+    for a in range(0, n, CHUNK):
+        b = min(n, a + CHUNK)
+        x = (frames[a:b] if idx is None else frames[idx[a:b]]).double() / 255.0
+        cols = F.unfold(x, 8, stride=4).transpose(1, 2).reshape(-1, 256)          # [(k, p)][e]
+        del x
+        g = gy[a:b].double()
+        if relu_y is not None:
+            g = g * (relu_y[a:b] > 0)
+        g = g.reshape(b - a, c, 400).transpose(0, 1).reshape(c, -1)               # [c][(k, p)]
+        ref += g @ cols
+        mag += g.abs() @ cols
+        S += cols.sum(0)
+        G = torch.maximum(G, g.abs().amax(1))
+        del cols, g
+    return ref, mag, S, G
+
+
+def check_wgrad(what, frames, idx, gy, got, base=None, relu_y=None):
+    """conv1_wgrad result `got` (C, 4, 8, 8) against base + the fp64 weight gradient, per element
+        |got - ref| <= (2 G_c / 127) 2^-25 S_e + 6u mag + 2u |base|,
+    G_c = max |gy_c| over all items bounds each CTA's power-of-two digit scale s < 2 G_c / 127, and s 2^-25 is the
+    rounding of gy to four base-256 digits; S_e = sum_{k,p} x/255 at patch element e, mag = sum |gy| x/255.  6u: the
+    digit recombination (two conversions, one FMA, the scale), the fp32 store of the reduction and the second store
+    of a split launch; 2u |base|: the two additions into an existing gradient."""
+    ref, mag, S, G = wgrad_ref(frames, idx, gy, relu_y)
+    c = ref.shape[0]
+    tol = (2.0 * G / 127.0).view(c, 1) * 2.0 ** -25 * S.view(1, 256) + 6 * U * mag
+    if base is not None:
+        b = base.double().reshape(c, 256)
+        ref, tol = ref + b, tol + 2 * U * b.abs()
+    w = _Worst(what)
+    w.add(got.reshape(c, 256), ref, tol)
+    return w.check()
+
+
+# --------------------------------------------------------------------------- #
+# 3xTF32 GEMM                                                                   #
+# --------------------------------------------------------------------------- #
+def gemm_splits(M, N, K):
+    """The K splits b2rl_gemm_tf32x3 uses for C[M][N] = A[M][K] B[N][K]^T (from its workspace size)."""
+    from distributed_rl_b200 import _lib
+    ldc = (N + 3) // 4 * 4
+    n_ws = _lib.load().b2rl_gemm_workspace_floats(M, N, K, ldc)
+    return n_ws // (M * ldc) if n_ws else 1
+
+
+def _rel(c, ref):
+    return ((c.double() - ref).abs().max() / ref.abs().max()).item()
+
+
+def gemm_tol(M, N, K, mag):
+    """check_gemm's per-element bound (5 2^-22 + d 2^-23) mag of a [M][K] x [N][K]^T product, `mag` = |a| @ |b|^T in
+    fp64."""
+    sp = gemm_splits(M, N, K)
+    d = 12 * math.ceil(math.ceil(K / 32) / sp) + sp
+    return (5 * 2.0 ** -22 + d * 2.0 ** -23) * mag
+
+
+def check_gemm(what, a, b, got, vs_cublas=4):
+    """3xTF32 result `got` = a @ b.T ([M][K] x [N][K]) against fp64, two ways.
+    Worst case, per element: |got - ref| <= (5 2^-22 + d 2^-23) mag with mag = |a| @ |b|^T and
+    d = 12 ceil(ceil(K/32) / splits) + splits: lo = x - rn_tf32(x) is read by the tensor core truncated to TF32
+    (2^-21 relative to x, once per operand) and lo*lo (2^-22) is dropped; each 32-wide K chunk is 3 MMAs x 4 k8 steps
+    of fp32 accumulation, then the splits are summed.  That bound would not notice a dropped lo term, so also, as in
+    test_gpu_03_gemm: max|err| / max|ref| below `vs_cublas` (4) x cuBLAS fp32's on the same inputs + 5e-7, and below
+    plain TF32's / 20."""
+    M, K = a.shape
+    N = b.shape[0]
+    sp = gemm_splits(M, N, K)
+    ad, bd = a.double(), b.double()
+    ref = ad @ bd.T
+    tol = gemm_tol(M, N, K, ad.abs() @ bd.abs().T)
+    del ad, bd
+    w = _Worst(f"{what} [{M}x{K}]·[{N}x{K}]^T, {sp} split(s)")
+    w.add(got, ref, tol)
+    del tol
+    e3, e32 = _rel(got, ref), _rel(a @ b.T, ref)
+    old = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = True
+    try:
+        e_tf32 = _rel(a @ b.T, ref)
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = old
+    print(f"[gemm] {what}: 3xTF32 {e3:.3g}, cuBLAS fp32 {e32:.3g}, TF32 {e_tf32:.3g} (of max|ref|)")
+    w.check()
+    assert e3 < vs_cublas * e32 + 5e-7, (what, e3, e32, e_tf32)
+    if K >= 512 and M > 1:
+        assert e3 < e_tf32 / 20, (what, e3, e32, e_tf32)
+    return e3, e32, e_tf32
+
+
+# --------------------------------------------------------------------------- #
+# dueling tail                                                                  #
+# --------------------------------------------------------------------------- #
+def _dueling_nodes(h, wa, wv):
+    r = torch.relu(h)
+    H = wa.shape[1]
+    adv, val = r[:, :H] @ wa.T, r[:, H:] @ wv.T
+    return (adv + val) - adv.mean(dim=-1, keepdim=True)
+
+
+def dueling_forward_tol(h, wa, wv):
+    """check_dueling_forward's per-element bound (d + 2) u mag, in fp64 (see there)."""
+    A, H = wa.shape
+    r = torch.relu(h.double())
+    ma = r[:, :H] @ wa.double().abs().T
+    mag = ma + r[:, H:] @ wv.double().abs().T + ma.mean(dim=-1, keepdim=True)
+    d = H // 32 + 5 + (A - 1) + 2
+    return (d + 2) * U * mag
+
+
+def check_dueling_forward(what, h, wa, wv, q):
+    """Dueling forward q against the unfused node sequence in fp64, per element |got - ref| <= (d + 2) u mag, mag the
+    node sequence on |wa|, |wv| (relu(h) >= 0 already), d = H/32 + 5 + (A - 1) + 2: one lane's FMA chain, the 5-step
+    warp reduction, the sum of the A advantages, the mean's division and the final add and subtract."""
+    A, H = wa.shape
+    ref = _dueling_nodes(h.double(), wa.double(), wv.double())
+    w = _Worst(f"{what} forward, M={h.shape[0]} H={H} A={A}")
+    w.add(q, ref, dueling_forward_tol(h, wa, wv))
+    return w.check()
+
+
+def check_dueling_backward(what, h, wa, wv, gq, gh, gwa, gwv):
+    """Dueling backward against fp64 autograd of the node sequence, per element |got - ref| <= (d + 2) u mag, mag the
+    same backward on absolute values (g_adv -> |gq| + mean |gq|, g_val -> sum |gq|):
+    dL/dh: d = A + 5 + 2 (the A-long FMA chain over the advantages, the 5-step warp sum of gq, the mean's division and
+    subtraction); dL/dWa, dL/dWv: d = ceil(M/32) + 2 + 8 + 7 (one thread's rows, two shuffles, eight warp partials,
+    and the row table's own 7 roundings).  A None gradient is not checked."""
+    M, A, H = h.shape[0], wa.shape[0], wa.shape[1]
+    hd, wad, wvd = (t.detach().double().requires_grad_() for t in (h, wa, wv))
+    _dueling_nodes(hd, wad, wvd).backward(gq.double())
+    g = gq.double().abs()
+    g_adv = g + g.mean(dim=-1, keepdim=True)
+    g_val = g.sum(dim=-1, keepdim=True)
+    r = torch.relu(hd.detach())
+    on = (hd.detach() > 0).double()
+    m_gh = torch.cat([(g_adv @ wad.detach().abs()) * on[:, :H], (g_val @ wvd.detach().abs()) * on[:, H:]], 1)
+    m_wa, m_wv = g_adv.T @ r[:, :H], g_val.T @ r[:, H:]
+    out = []
+    for name, got, ref, mag, d in (("dL/dh", gh, hd.grad, m_gh, A + 5 + 2),
+                                   ("dL/dWa", gwa, wad.grad, m_wa, math.ceil(M / 32) + 2 + 8 + 7),
+                                   ("dL/dWv", gwv, wvd.grad, m_wv, math.ceil(M / 32) + 2 + 8 + 7)):
+        if got is None:
+            continue
+        w = _Worst(f"{what} {name}, M={M} H={H} A={A}")
+        w.add(got, ref, (d + 2) * U * mag)
+        out.append(w.check())
+    return out
+
+
+# --------------------------------------------------------------------------- #
+# the Ape-X heads: ReLU + NCHW flatten + 3xTF32 GEMM + dueling tail             #
+# --------------------------------------------------------------------------- #
+def relu_flat(y):
+    """flatten_NCHW(relu(y)) of a (B, C, H, W) tensor in any memory format, in fp64: the heads' A operand in the
+    weights' feature order c * H * W + p."""
+    return torch.relu(y.double()).reshape(y.shape[0], -1)
+
+
+def check_heads_dueling_forward(what, y, ws, wa, wv, q):
+    """q of linear.relu_flat_heads_dueling against dueling(h) in fp64, h = flatten_NCHW(relu(y)) @ cat(ws)^T, per element
+        |got - ref| <= tol_duel(h) + tol_h[:, :H] @ |Wa|^T + tol_h[:, H:] @ |Wv|^T + mean_a(tol_h[:, :H] @ |Wa|^T),
+    tol_duel the dueling-forward bound of check_dueling_forward evaluated on the fp64 h, tol_h = gemm_tol(M, 2H, K,
+    flatten_NCHW(relu(y)) @ |cat(ws)|^T) the 3xTF32 GEMM's bound on each element of the h the kernel sums from the
+    split partials.  ReLU is 1-Lipschitz, so an error e in h moves adv by at most e[:, :H] @ |Wa|^T, val by
+    e[:, H:] @ |Wv|^T and the advantages' mean by the mean of the first: to first order the three propagated terms."""
+    a = relu_flat(y)
+    w = torch.cat([t.double() for t in ws], 0)
+    M, K = a.shape
+    N, (A, H) = w.shape[0], wa.shape
+    h = a @ w.T
+    tol_h = gemm_tol(M, N, K, a @ w.abs().T)
+    del a, w
+    e_adv = tol_h[:, :H] @ wa.double().abs().T
+    tol = (dueling_forward_tol(h, wa, wv) + e_adv + tol_h[:, H:] @ wv.double().abs().T
+           + e_adv.mean(dim=-1, keepdim=True))
+    worst = _Worst(f"{what} q, M={M} K={K} N={N} H={H} A={A}")
+    worst.add(q, _dueling_nodes(h, wa.double(), wv.double()), tol)
+    return worst.check()
+
+
+def check_relu_flat_dgrad(what, y, ws, gh, gy):
+    """dL/dy of h = flatten_NCHW(relu(y)) @ cat(ws)^T (y (M, C, H, W), pre-ReLU) against fp64: unflatten_NCHW(gh @ cat(ws))
+    where y > 0 and exactly 0 elsewhere, per element gemm_tol(M, K, N, |gh| @ |cat(ws)|) masked alike.  The dL/dx GEMM
+    contracts over N = 2H and b2rl_unflatten_relu_mask sums its split partials in split order, as the GEMM's own
+    reduction does, so check_gemm's bound holds as it stands."""
+    M = y.shape[0]
+    w = torch.cat([t.double() for t in ws], 0)
+    N, K = w.shape
+    g = gh.double()
+    mask = (y.double() > 0).reshape(M, -1)
+    ref = (g @ w) * mask
+    tol = gemm_tol(M, K, N, g.abs() @ w.abs()) * mask
+    worst = _Worst(f"{what} dL/dy [{M}x{N}]·[{N}x{K}], {gemm_splits(M, K, N)} split(s)")
+    worst.add(gy.reshape(M, -1), ref, tol)
+    return worst.check()
+
+
+# --------------------------------------------------------------------------- #
+# the fused centered RMSprop                                                    #
+# --------------------------------------------------------------------------- #
+def check_rmsprop_centered(what, pre, post, lr, alpha, eps):
+    """One centered RMSprop update of the fused optimizer (csrc/optim.cu rmsprop_elem) against fp64, per element, from
+    the tensors the launch read (`pre`: p, g, sq, ga) and wrote (`post`: p, sq, ga, g).  The hyper-parameters are the
+    fp32 values the kernel receives (a = alpha, b = 1 - alpha formed in double, lr, eps); the reference is
+        S = a sq + b g^2,   G = ga + b (g - ga),   D = S - G^2,   P = p - s,   s = lr g / (sqrt(D) + eps).
+    The kernel rounds each operation once (u = 2^-24; -fmad=false, its FMAs are explicit):
+      sq' = fma(fl(b g), g, fl(sq a)): two non-negative products rounded once each, then their sum:
+            |sq' - S| <= ((1 + u)^2 - 1) S <= 3u S =: t_s;
+      ga' = fma(b, fl(g - ga), ga):  |ga' - G| <= u b |g - ga| (1 + u) + u |G| <= u (2 b |g - ga| + |G|) =: t_g;
+      D'  = fma(-ga', ga', sq'):     |D' - D| <= t_s + 2 |G| t_g + t_g^2 + u |D'|: relative r_D = (t_s + 2 |G| t_g +
+            t_g^2) / D + 2u, the cancellation term, of order u (S + G^2) / D;
+      avg = sqrt(D'): r_D / 2 + u;  avg + eps: r_D / 2 + 2u (eps exact, both terms non-negative);  g / ., lr * .:
+            r_D / 2 + 4u on the step s;
+      p'  = fl(p - s'):              |p' - P| <= |s| (r_D / 2 + 5u) + u |P|,
+    one u of slack on the step for the second-order terms (r_D stays near 1e-6 here).  Where the averages and g are all
+    zero, D = 0 and s = 0: p' must equal p.  The gradient must read zero after the launch."""
+    import numpy as np
+    a, b = float(np.float32(alpha)), float(np.float32(1.0 - alpha))
+    lr, eps = float(np.float32(lr)), float(np.float32(eps))
+    p, g, sq, ga = (pre[k].double() for k in ("p", "g", "sq", "ga"))
+    S = a * sq + b * g * g
+    G = ga + b * (g - ga)
+    D = S - G * G
+    s = lr * g / (D.clamp_min(0).sqrt() + eps)
+    P = p - s
+    t_s = 3 * U * S
+    t_g = U * (2 * b * (g - ga).abs() + G.abs())
+    r_D = torch.where(D > 0, (t_s + 2 * G.abs() * t_g + t_g * t_g) / D.where(D > 0, torch.ones_like(D)), 0.0) + 2 * U
+    out = []
+    for name, got, ref, tol in (("square_avg", post["sq"], S, t_s), ("grad_avg", post["ga"], G, t_g),
+                                ("param", post["p"], P, s.abs() * (r_D / 2 + 5 * U) + U * P.abs())):
+        w = _Worst(f"{what} {name}")
+        w.add(got, ref, tol)
+        out.append(w.check())
+    assert not post["g"].any(), f"{what}: the gradient is not zero after the update"
+    return out
