@@ -28,6 +28,12 @@ class ServeLayout(C.Structure):
                 ("total_bytes", c_i64)]
 
 
+class Frames(C.Structure):
+    """b2rl_frames: where conv_1 reads frame row r (include/b2rl.h); exactly one of base, table and pool + planes."""
+    _fields_ = [("base", c_vp), ("table", c_vp), ("pool", c_vp), ("planes", c_vp), ("row_stride", c_i64),
+                ("rows", c_i64), ("plane_base", c_i32), ("reserved", c_i32)]
+
+
 # name -> (restype, argtypes); must list every symbol include/b2rl.h declares.
 SIGNATURES = {
     "b2rl_last_error": (C.c_char_p, []),
@@ -61,19 +67,9 @@ SIGNATURES = {
     "b2rl_conv1_pack": (C.c_int, [c_vp, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp]),
     "b2rl_conv1_pack_jobs": (C.c_int, [C.POINTER(c_vp), C.POINTER(c_i32), C.POINTER(c_i32), C.POINTER(c_vp),
                                        C.POINTER(c_vp), c_i32, c_i32, c_vp]),
-    "b2rl_conv1_fused": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp]),
+    "b2rl_conv1_fused": (C.c_int, [C.POINTER(Frames), c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp]),
     "b2rl_conv1_wgrad_workspace_floats": (c_i64, [c_i32]),
-    "b2rl_conv1_wgrad": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp]),
-    "b2rl_conv1_fused_table": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp]),
-    "b2rl_conv1_wgrad_table": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp]),
-    "b2rl_conv1_fused_strided": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_vp,
-                                           c_i32, c_vp]),
-    "b2rl_conv1_wgrad_strided": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp,
-                                           c_i32, c_vp]),
-    "b2rl_conv1_fused_planes": (C.c_int, [c_vp, c_vp, c_i32, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_vp,
-                                          c_i32, c_vp]),
-    "b2rl_conv1_wgrad_planes": (C.c_int, [c_vp, c_vp, c_i32, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp,
-                                          c_i32, c_vp]),
+    "b2rl_conv1_wgrad": (C.c_int, [C.POINTER(Frames), c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp]),
     "b2rl_dedup_attach": (C.c_int, [c_vp, c_i32, c_i64, c_i64, c_u64]),
     "b2rl_dedup_push": (C.c_int, [c_vp, c_vp, c_vp, C.POINTER(c_vp), c_vp, c_i64, c_vp]),
     "b2rl_dedup_info": (C.c_int, [c_vp, C.POINTER(c_vp), C.POINTER(c_i64), C.POINTER(c_i64)]),

@@ -10,6 +10,7 @@
 // and refills the stage of item t - LAG once all but the newest LAG store groups have finished reading SMEM.
 #pragma once
 #include "common.cuh"
+#include "frames.cuh"
 #include "hopper.cuh"
 
 namespace b2rl {
@@ -33,8 +34,6 @@ struct BulkField {
   const int32_t* planes;   // plane rows only: 8 pool ids per replay row; chunk c of a row is pool frame planes[8 row +
   int32_t plane_base;      // plane_base + c] (src is the frame pool), so a frame stack is four PLANE_BYTES copies
 };
-
-constexpr int PLANE_BYTES = 84 * 84;   // one frame of the deduplicated Ape-X store's pool
 
 struct BulkRows {
   BulkField f[B2RL_MAX_FIELDS];
@@ -94,7 +93,7 @@ struct ItemCursor {
     }
     if (T.f[f].planes != nullptr) {
       bytes = PLANE_BYTES;
-      src = T.f[f].src + (int64_t)T.f[f].planes[row * 8 + T.f[f].plane_base + c] * PLANE_BYTES;
+      src = plane_ptr(T.f[f].src, T.f[f].planes, row, T.f[f].plane_base, c);
       dst = T.f[f].dst + (dst_k0 + k) * T.f[f].row_bytes + (int64_t)c * PLANE_BYTES;
       return;
     }

@@ -23,10 +23,12 @@
 //                NHWC stores straight from the accumulator fragment
 //   warps 8-15   im2col producers: SMEM frame -> 128B-swizzled K-major A tile (uint8);
 //                thread = (tile row, channel pair)
-//   warp 16      TMA loader: weights once, then one 28 224-byte frame stack per item, from base + row * row_stride
-//                (a stride of 7 056 reads the overlapping 4-frame windows of a frame strip: channel c of row r is
-//                frame r + c), or as four 7 056-byte frames of a frame pool named by a plane table
+//   warp 16      TMA loader: weights once, then one 28 224-byte frame stack per item, from the frame source of
+//                frames.cuh: base + row * row_stride (a stride of 7 056 reads the overlapping 4-frame windows of a
+//                frame strip: channel c of row r is frame r + c), or four 7 056-byte frames of a frame pool named by
+//                a plane table
 #include "common.cuh"
+#include "frames.cuh"
 #include "hopper.cuh"
 
 namespace b2rl {
@@ -37,7 +39,6 @@ using namespace sm90;
 constexpr int C_IN = 4, HW = 84, KS = 8, STRIDE = 4, OHW = 20;
 constexpr int C_OUT_MAX = 32;                      // output channels: 32 (Ape-X / R2D2) or 16 (IMPALA), a template parameter
 constexpr int K_TOTAL = C_IN * KS * KS;            // 256
-constexpr int FRAME_BYTES = C_IN * HW * HW;        // 28 224
 constexpr int POS = OHW * OHW;                     // 400 output positions per frame stack
 constexpr int TILE_M = 128;
 constexpr int TILES = (POS + TILE_M - 1) / TILE_M; // 4 (the last one has 16 valid rows)
@@ -45,7 +46,7 @@ constexpr int NSPLIT = 4;
 constexpr int A_STAGES = 2;
 constexpr int A_TILE_BYTES = TILE_M * K_TOTAL;     // 32 768: 2 K-chunks x 128 rows x 128 B
 constexpr int A_CHUNK_BYTES = TILE_M * 128;        // 16 384
-constexpr int RAW_STRIDE = 28288;                  // FRAME_BYTES rounded up to 128
+constexpr int RAW_STRIDE = 28288;                  // STACK_BYTES rounded up to 128
 constexpr int CONSUMERS = 256, PRODUCERS = 256;
 constexpr int THREADS = CONSUMERS + PRODUCERS + 32;
 
@@ -104,48 +105,14 @@ k_conv1_pack_jobs(const __grid_constant__ PackJobs J, int c_out) {
 }
 
 struct Params {
-  const uint8_t* frames;     // field base: row r is the FRAME_BYTES starting at frames + r * row_stride
+  FrameSource src;           // where row r is read from (frames.cuh)
   const int64_t* idx;        // sampled rows, or nullptr for rows 0..n-1
   int64_t n;                 // frame stacks to process
-  int64_t capacity;          // rows in `frames` (indices are clamped)
-  int64_t row_stride;        // bytes between rows: FRAME_BYTES (stacks) or 7 056 (overlapping windows of a frame strip)
   const int8_t* bq;          // packed weights (n_nets * 128 rows, SW128 layout), n_nets*128*256 bytes
   const float* scale;        // [n_nets][32] = s_c / 255
   float* out;                // [n_nets][n][400][32] fp32 (NHWC)
   int relu;
 };
-
-// The table variant: the frame base is read from device memory when the kernel starts (`frames` is unused), so a
-// captured launch follows whatever b2rl_serve_bind last wrote into the entry (the ring slot of this step).
-struct TableParams : Params {
-  const uint8_t* const* table;   // one entry: the field base
-};
-
-// The plane-table variant (b2rl_conv1_fused_planes): `frames` is a frame pool, and channel c of row r is pool frame
-// planes[8 r + plane_base + c].
-struct PlaneParams : Params {
-  const int32_t* planes;
-  int32_t plane_base;
-};
-
-__device__ __forceinline__ const uint8_t* frame_base(const Params& P) { return P.frames; }
-__device__ __forceinline__ const uint8_t* frame_base(const TableParams& P) { return *P.table; }
-
-// Row `row` -> `dst` in SMEM, completing FRAME_BYTES of transactions on `bar`: one bulk copy of a frame stack, or
-// four of a plane table's frames.
-__device__ __forceinline__ void load_row(const Params& P, const uint8_t* frames, int64_t row, uint8_t* dst,
-                                         uint64_t* bar) {
-  mbar_expect_tx(bar, FRAME_BYTES);
-  bulk_g2s(dst, frames + row * P.row_stride, FRAME_BYTES, bar);
-}
-__device__ __forceinline__ void load_row(const PlaneParams& P, const uint8_t* frames, int64_t row, uint8_t* dst,
-                                         uint64_t* bar) {
-  constexpr int PLANE = HW * HW;
-  mbar_expect_tx(bar, FRAME_BYTES);
-#pragma unroll
-  for (int c = 0; c < C_IN; ++c)
-    bulk_g2s(dst + c * PLANE, frames + (int64_t)P.planes[row * 8 + P.plane_base + c] * PLANE, PLANE, bar);
-}
 
 template <int N> struct Acc;
 template <> struct Acc<128> {
@@ -157,9 +124,9 @@ template <> struct Acc<64> {
   __device__ __forceinline__ void mma(uint64_t a, uint64_t b, uint32_t acc) { mma_u8s8_n64(d, a, b, acc); }
 };
 
-template <int N_NETS, int C_OUT, class PARAMS = Params>
+template <int N_NETS, int C_OUT, FrameKind KIND>
 __global__ void __launch_bounds__(THREADS, 1)
-k_conv1_fused(const __grid_constant__ PARAMS P) {
+k_conv1_fused(const __grid_constant__ Params P) {
   constexpr int N_PER_NET = NSPLIT * C_OUT;            // MMA columns per network: 128 (64 for 16 channels)
   constexpr int N_TOTAL = N_NETS * N_PER_NET;          // rows of the packed weights: 64 .. 256
   constexpr int B_BYTES = N_TOTAL * K_TOTAL;           // 16 .. 64 KiB
@@ -190,7 +157,7 @@ k_conv1_fused(const __grid_constant__ PARAMS P) {
   if (warp == (CONSUMERS + PRODUCERS) / 32) {
     // ------------------------------ TMA loader ------------------------------
     if (lane == 0) {
-      const uint8_t* frames = frame_base(P);
+      const uint8_t* frames = frame_base<KIND>(P.src);
       mbar_expect_tx(&b_full, B_BYTES);
       constexpr int LOAD_CHUNK = (B_BYTES < 32768) ? B_BYTES : 32768;
       for (int off = 0; off < B_BYTES; off += LOAD_CHUNK) bulk_g2s(sB + off, P.bq + off, LOAD_CHUNK, &b_full);
@@ -199,8 +166,8 @@ k_conv1_fused(const __grid_constant__ PARAMS P) {
         const int s = it & 1;
         mbar_wait(&raw_empty[s], ((it >> 1) & 1) ^ 1);
         int64_t row = P.idx ? P.idx[k] : k;
-        row = row < 0 ? 0 : (row >= P.capacity ? P.capacity - 1 : row);
-        load_row(P, frames, row, sRaw + s * RAW_STRIDE, &raw_full[s]);
+        row = row < 0 ? 0 : (row >= P.src.rows ? P.src.rows - 1 : row);
+        load_row<KIND>(P.src, frames, row, sRaw + s * RAW_STRIDE, &raw_full[s]);
       }
     }
   } else if (warp >= CONSUMERS / 32) {
@@ -350,93 +317,45 @@ extern "C" int b2rl_conv1_pack_jobs(const float* const* w_dev, const int32_t* ne
   return B2RL_OK;
 }
 
-template <int N_NETS, int C_OUT, class PARAMS>
-static cudaError_t conv1_launch(const PARAMS& P, unsigned grid, cudaStream_t st) {
+template <int N_NETS, int C_OUT, FrameKind KIND>
+static cudaError_t conv1_launch(const conv1::Params& P, unsigned grid, cudaStream_t st) {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e == cudaSuccess)
-    e = set_max_dynamic_smem<conv1::k_conv1_fused<N_NETS, C_OUT, PARAMS>>(dev, conv1::smem_bytes<N_NETS, C_OUT>());
+    e = set_max_dynamic_smem<conv1::k_conv1_fused<N_NETS, C_OUT, KIND>>(dev, conv1::smem_bytes<N_NETS, C_OUT>());
   if (e != cudaSuccess) return e;
-  conv1::k_conv1_fused<N_NETS, C_OUT, PARAMS><<<grid, conv1::THREADS, conv1::smem_bytes<N_NETS, C_OUT>(), st>>>(P);
+  conv1::k_conv1_fused<N_NETS, C_OUT, KIND><<<grid, conv1::THREADS, conv1::smem_bytes<N_NETS, C_OUT>(), st>>>(P);
   return cudaSuccess;
 }
 
-// What the direct and the table frame source share once the source is checked.
-template <class PARAMS>
-static int conv1_fused_run(PARAMS& P, const int8_t* bq_dev, const float* scale_dev, int32_t n_nets, int32_t c_out,
-                           float* out_dev, void* stream) {
+extern "C" int b2rl_conv1_fused(const b2rl_frames* frames, const int64_t* idx_dev, int64_t n, const int8_t* bq_dev,
+                                const float* scale_dev, int32_t n_nets, int32_t c_out, float* out_dev, int32_t relu,
+                                void* stream) {
+  B2RL_REQUIRE(n >= 0, "negative n");
+  conv1::Params P{};
+  FrameKind kind;
+  if (const int rc = check_frames(frames, P.src, kind)) return rc;
+  if (n == 0) return B2RL_OK;
   B2RL_REQUIRE(bq_dev && scale_dev && out_dev, "null argument");
   B2RL_REQUIRE(n_nets == 1 || n_nets == 2, "n_nets must be 1 or 2");
   B2RL_REQUIRE(c_out == 16 || c_out == 32, "c_out must be 16 or 32");
-  B2RL_REQUIRE(P.capacity >= 1, "capacity must be positive");
   B2RL_REQUIRE(((uintptr_t)bq_dev % 16 == 0) && ((uintptr_t)out_dev % 16 == 0),
-               "frames, packed weights and output must be 16-byte aligned");
+               "packed weights and output must be 16-byte aligned");
   int dev = 0;
   B2RL_CUDA(cudaGetDevice(&dev));
   int sms = 0;
   B2RL_CUDA(sm_count(dev, &sms));
-  P.bq = bq_dev, P.scale = scale_dev, P.out = out_dev;
-  const int64_t units = P.n * conv1::TILES;
+  P.idx = idx_dev, P.n = n, P.bq = bq_dev, P.scale = scale_dev, P.out = out_dev, P.relu = relu;
+  const int64_t units = n * conv1::TILES;
   const unsigned grid = (unsigned)((units < sms) ? units : sms);
   cudaStream_t st = (cudaStream_t)stream;
-  cudaError_t e;
-  if (c_out == 32) e = (n_nets == 1) ? conv1_launch<1, 32>(P, grid, st) : conv1_launch<2, 32>(P, grid, st);
-  else             e = (n_nets == 1) ? conv1_launch<1, 16>(P, grid, st) : conv1_launch<2, 16>(P, grid, st);
+  const cudaError_t e = with_frame_kind(kind, [&](auto K) {
+    constexpr FrameKind KIND = decltype(K)::value;
+    if (c_out == 32) return n_nets == 1 ? conv1_launch<1, 32, KIND>(P, grid, st) : conv1_launch<2, 32, KIND>(P, grid, st);
+    return n_nets == 1 ? conv1_launch<1, 16, KIND>(P, grid, st) : conv1_launch<2, 16, KIND>(P, grid, st);
+  });
   B2RL_CUDA(e);
   count_launch();
   B2RL_CHECK_LAUNCH();
   return B2RL_OK;
-}
-
-extern "C" int b2rl_conv1_fused_strided(const uint8_t* frames_dev, const uint8_t* const* frame_table_dev,
-                                        int64_t row_stride, int64_t rows, const int64_t* idx_dev, int64_t n,
-                                        const int8_t* bq_dev, const float* scale_dev, int32_t n_nets, int32_t c_out,
-                                        float* out_dev, int32_t relu, void* stream) {
-  B2RL_REQUIRE(n >= 0, "negative n");
-  B2RL_REQUIRE((frames_dev != nullptr) != (frame_table_dev != nullptr), "exactly one of frames and frame table");
-  B2RL_REQUIRE(row_stride > 0 && row_stride % 16 == 0, "the row stride must be a positive multiple of 16 bytes");
-  B2RL_REQUIRE(frames_dev ? (uintptr_t)frames_dev % 16 == 0 : (uintptr_t)frame_table_dev % 8 == 0,
-               "frames must be 16-byte aligned, a frame table entry 8-byte aligned");
-  if (n == 0) return B2RL_OK;
-  if (frames_dev) {
-    conv1::Params P{frames_dev, idx_dev, n, rows, row_stride, nullptr, nullptr, nullptr, relu};
-    return conv1_fused_run(P, bq_dev, scale_dev, n_nets, c_out, out_dev, stream);
-  }
-  conv1::TableParams P{};
-  P.idx = idx_dev, P.n = n, P.capacity = rows, P.row_stride = row_stride, P.relu = relu, P.table = frame_table_dev;
-  return conv1_fused_run(P, bq_dev, scale_dev, n_nets, c_out, out_dev, stream);
-}
-
-extern "C" int b2rl_conv1_fused_planes(const uint8_t* pool_dev, const int32_t* planes_dev, int32_t plane_base,
-                                       int64_t rows, const int64_t* idx_dev, int64_t n, const int8_t* bq_dev,
-                                       const float* scale_dev, int32_t n_nets, int32_t c_out, float* out_dev,
-                                       int32_t relu, void* stream) {
-  B2RL_REQUIRE(n >= 0, "negative n");
-  B2RL_REQUIRE(pool_dev != nullptr && planes_dev != nullptr, "null frame pool or plane table");
-  B2RL_REQUIRE((uintptr_t)pool_dev % 16 == 0 && (uintptr_t)planes_dev % 4 == 0,
-               "the frame pool must be 16-byte aligned, the plane table 4-byte aligned");
-  B2RL_REQUIRE(plane_base == 0 || plane_base == 4, "plane_base must be 0 or 4");
-  if (n == 0) return B2RL_OK;
-  conv1::PlaneParams P{};
-  P.frames = pool_dev, P.idx = idx_dev, P.n = n, P.capacity = rows, P.row_stride = conv1::FRAME_BYTES, P.relu = relu;
-  P.planes = planes_dev, P.plane_base = plane_base;
-  return conv1_fused_run(P, bq_dev, scale_dev, n_nets, c_out, out_dev, stream);
-}
-
-extern "C" int b2rl_conv1_fused(const uint8_t* frames_dev, int64_t capacity, const int64_t* idx_dev, int64_t n,
-                                const int8_t* bq_dev, const float* scale_dev, int32_t n_nets, int32_t c_out,
-                                float* out_dev, int32_t relu, void* stream) {
-  B2RL_REQUIRE(n >= 0, "negative n");
-  if (n == 0) return B2RL_OK;
-  B2RL_REQUIRE(frames_dev, "null argument");
-  return b2rl_conv1_fused_strided(frames_dev, nullptr, conv1::FRAME_BYTES, capacity, idx_dev, n, bq_dev, scale_dev,
-                                  n_nets, c_out, out_dev, relu, stream);
-}
-
-extern "C" int b2rl_conv1_fused_table(const uint8_t* const* frame_table_dev, int64_t capacity, const int64_t* idx_dev,
-                                      int64_t n, const int8_t* bq_dev, const float* scale_dev, int32_t n_nets,
-                                      int32_t c_out, float* out_dev, int32_t relu, void* stream) {
-  B2RL_REQUIRE(frame_table_dev != nullptr, "null frame table");
-  return b2rl_conv1_fused_strided(nullptr, frame_table_dev, conv1::FRAME_BYTES, capacity, idx_dev, n, bq_dev,
-                                  scale_dev, n_nets, c_out, out_dev, relu, stream);
 }

@@ -27,6 +27,7 @@
 //   thread 0 also issues the TMA bulk copy of the next frame stack when it starts on a stack's first chunk: the
 //   buffer it overwrites was last read two stacks before, by chunks that every producer has finished
 #include "common.cuh"
+#include "frames.cuh"
 #include "hopper.cuh"
 
 namespace b2rl {
@@ -36,7 +37,6 @@ using namespace sm90;
 
 constexpr int C_IN = 4, HW = 84, KS = 8, STRIDE = 4, OHW = 20;
 constexpr int E_TOTAL = C_IN * KS * KS;            // 256 patch elements = GEMM M (four warpgroups of 64)
-constexpr int FRAME_BYTES = C_IN * HW * HW;        // 28 224
 constexpr int RAW_STRIDE = 28288;
 constexpr int POS = OHW * OHW;                     // 400 output positions per frame stack
 constexpr int NSPLIT = 4;
@@ -52,46 +52,13 @@ constexpr int MAX_ITEMS_PER_CTA = 160;             // int32 accumulators: 128*25
 __device__ __forceinline__ int sw_row(int row) { return (row >> 3) * 1024 + (row & 7) * 128; }
 
 struct Params {
-  const uint8_t* frames;     // field base: row r is the FRAME_BYTES starting at frames + r * row_stride
+  FrameSource src;           // where row r is read from (frames.cuh)
   const int64_t* idx;        // sampled rows, or nullptr for rows 0..n-1
-  int64_t n, capacity;
-  int64_t row_stride;        // bytes between rows: FRAME_BYTES (stacks) or 7 056 (overlapping windows of a frame strip)
+  int64_t n;
   const float* gy;           // [n][400][C_OUT] fp32 (NHWC)
   const float* y;            // optional conv_1 output after ReLU, same layout: dL/dy is taken as gy * (y > 0); else nullptr
   float* partial;            // [gridDim.x][C_OUT][256]
 };
-
-// The table variant (b2rl_conv1_wgrad_table): the frame base is read from device memory when the kernel starts and
-// advanced by frame_off bytes there (`frames` is unused), so a captured launch follows the entry b2rl_serve_bind wrote.
-struct TableParams : Params {
-  const uint8_t* const* table;
-  int64_t frame_off;         // rows of the earlier launches of a split n (idx == nullptr), in bytes
-};
-
-// The plane-table variant (b2rl_conv1_wgrad_planes): `frames` is a frame pool, and channel c of row r is pool frame
-// planes[8 r + plane_base + c].
-struct PlaneParams : Params {
-  const int32_t* planes;
-  int32_t plane_base;
-};
-
-__device__ __forceinline__ const uint8_t* frame_base(const Params& P) { return P.frames; }
-__device__ __forceinline__ const uint8_t* frame_base(const TableParams& P) { return *P.table + P.frame_off; }
-
-// Row `row` -> `dst` in SMEM, completing FRAME_BYTES of transactions on `bar` (as in conv1.cu).
-__device__ __forceinline__ void load_row(const Params& P, const uint8_t* frames, int64_t row, uint8_t* dst,
-                                         uint64_t* bar) {
-  mbar_expect_tx(bar, FRAME_BYTES);
-  bulk_g2s(dst, frames + row * P.row_stride, FRAME_BYTES, bar);
-}
-__device__ __forceinline__ void load_row(const PlaneParams& P, const uint8_t* frames, int64_t row, uint8_t* dst,
-                                         uint64_t* bar) {
-  constexpr int PLANE = FRAME_BYTES / 4;
-  mbar_expect_tx(bar, FRAME_BYTES);
-#pragma unroll
-  for (int c = 0; c < 4; ++c)
-    bulk_g2s(dst + c * PLANE, frames + (int64_t)P.planes[row * 8 + P.plane_base + c] * PLANE, PLANE, bar);
-}
 
 template <int N> struct Acc;
 template <> struct Acc<128> {
@@ -110,9 +77,9 @@ __device__ __forceinline__ int digit_exponent(uint32_t absmax_bits) {
   return e < 27 ? 27 : (e > 227 ? 227 : e);
 }
 
-template <int C_OUT, class PARAMS = Params>
+template <int C_OUT, FrameKind KIND>
 __global__ void __launch_bounds__(THREADS, 1)
-k_conv1_wgrad(const __grid_constant__ PARAMS P) {
+k_conv1_wgrad(const __grid_constant__ Params P) {
   constexpr int N_TOTAL = NSPLIT * C_OUT;              // 128 (64 for 16 channels)
   constexpr int B_BYTES = N_TOTAL * KCHUNK;
   constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
@@ -134,15 +101,15 @@ k_conv1_wgrad(const __grid_constant__ PARAMS P) {
   }
   __syncthreads();
   const int64_t first = blockIdx.x, stride = gridDim.x;
-  const uint8_t* frames = frame_base(P);
+  const uint8_t* frames = frame_base<KIND>(P.src);
 
   // frame stack `it` of this CTA -> raw buffer it & 1
   auto load_frame = [&](int64_t it) {
     const int64_t k = first + it * stride;
     if (k >= P.n) return;
     int64_t row = P.idx ? P.idx[k] : k;
-    row = row < 0 ? 0 : (row >= P.capacity ? P.capacity - 1 : row);
-    load_row(P, frames, row, sRaw + (it & 1) * RAW_STRIDE, &raw_full[it & 1]);
+    row = row < 0 ? 0 : (row >= P.src.rows ? P.src.rows - 1 : row);
+    load_row<KIND>(P.src, frames, row, sRaw + (it & 1) * RAW_STRIDE, &raw_full[it & 1]);
   };
   if (threadIdx.x == 0) load_frame(0);
 
@@ -367,14 +334,14 @@ constexpr size_t smem_bytes() {
 
 using namespace b2rl;
 
-template <int C_OUT, class PARAMS>
-static cudaError_t wgrad_launch(const PARAMS& P, unsigned grid, cudaStream_t st) {
+template <int C_OUT, FrameKind KIND>
+static cudaError_t wgrad_launch(const conv1w::Params& P, unsigned grid, cudaStream_t st) {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e == cudaSuccess)
-    e = set_max_dynamic_smem<conv1w::k_conv1_wgrad<C_OUT, PARAMS>>(dev, conv1w::smem_bytes<C_OUT>());
+    e = set_max_dynamic_smem<conv1w::k_conv1_wgrad<C_OUT, KIND>>(dev, conv1w::smem_bytes<C_OUT>());
   if (e != cudaSuccess) return e;
-  conv1w::k_conv1_wgrad<C_OUT, PARAMS><<<grid, conv1w::THREADS, conv1w::smem_bytes<C_OUT>(), st>>>(P);
+  conv1w::k_conv1_wgrad<C_OUT, KIND><<<grid, conv1w::THREADS, conv1w::smem_bytes<C_OUT>(), st>>>(P);
   return cudaSuccess;
 }
 
@@ -385,18 +352,16 @@ extern "C" int64_t b2rl_conv1_wgrad_workspace_floats(int32_t c_out) {
   return (int64_t)sms * c_out * conv1w::E_TOTAL;
 }
 
-// The launches of every conv_1 weight-gradient entry point.  `frames_dev` null: the frame base is the table entry
-// (read on the device, where the offset of each launch of a split n is added).  `planes_dev` non-null: frames_dev is
-// a frame pool read through that plane table (whose rows each launch of a split n advances).
-static int wgrad_run(const uint8_t* frames_dev, const uint8_t* const* table_dev, int64_t row_stride, int64_t capacity,
-                     const int64_t* idx_dev, int64_t n, const float* gy_dev, const float* y_relu_dev, int32_t c_out,
-                     float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream,
-                     const int32_t* planes_dev = nullptr, int32_t plane_base = 0) {
+extern "C" int b2rl_conv1_wgrad(const b2rl_frames* frames, const int64_t* idx_dev, int64_t n, const float* gy_dev,
+                                const float* y_relu_dev, int32_t c_out, float* workspace_dev, float* gw_dev,
+                                int32_t accumulate, void* stream) {
+  B2RL_REQUIRE(n >= 1, "n must be positive");
+  FrameSource src;
+  FrameKind kind;
+  if (const int rc = check_frames(frames, src, kind)) return rc;
   B2RL_REQUIRE(gy_dev && workspace_dev && gw_dev, "null argument");
   B2RL_REQUIRE(c_out == 16 || c_out == 32, "c_out must be 16 or 32");
-  B2RL_REQUIRE(capacity >= 1, "capacity must be positive");
-  B2RL_REQUIRE(((uintptr_t)gy_dev % 16 == 0) && ((uintptr_t)y_relu_dev % 16 == 0),
-               "frames, gy and y must be 16-byte aligned");
+  B2RL_REQUIRE(((uintptr_t)gy_dev % 16 == 0) && ((uintptr_t)y_relu_dev % 16 == 0), "gy and y must be 16-byte aligned");
   int dev = 0;
   B2RL_CUDA(cudaGetDevice(&dev));
   int sms = 0;
@@ -406,26 +371,16 @@ static int wgrad_run(const uint8_t* frames_dev, const uint8_t* const* table_dev,
   const int64_t per_launch = (int64_t)sms * conv1w::MAX_ITEMS_PER_CTA;   // int32 accumulator bound
   for (int64_t off = 0; off < n; off += per_launch) {
     const int64_t m = (n - off < per_launch) ? n - off : per_launch;
-    conv1w::Params P{frames_dev, idx_dev ? idx_dev + off : nullptr, m, capacity, row_stride,
-                     gy_dev + off * (int64_t)(conv1w::POS * c_out),
-                     y_relu_dev ? y_relu_dev + off * (int64_t)(conv1w::POS * c_out) : nullptr, workspace_dev};
-    const int64_t frame_off = idx_dev ? 0 : off * row_stride;
-    if (!idx_dev) P.capacity = capacity - off;
+    // without idx, launch j reads rows [off, off + m) of the source: its rows 0..m-1 once advanced by off
+    const conv1w::Params P{idx_dev ? src : advance(src, kind, off), idx_dev ? idx_dev + off : nullptr, m,
+                           gy_dev + off * (int64_t)(conv1w::POS * c_out),
+                           y_relu_dev ? y_relu_dev + off * (int64_t)(conv1w::POS * c_out) : nullptr, workspace_dev};
     const unsigned grid = (unsigned)((m < sms) ? m : sms);
-    if (planes_dev) {
-      conv1w::PlaneParams Q{};
-      static_cast<conv1w::Params&>(Q) = P;
-      Q.frames = frames_dev, Q.planes = planes_dev + (idx_dev ? 0 : off * 8), Q.plane_base = plane_base;
-      B2RL_CUDA(c_out == 32 ? wgrad_launch<32>(Q, grid, st) : wgrad_launch<16>(Q, grid, st));
-    } else if (frames_dev) {
-      P.frames = frames_dev + frame_off;
-      B2RL_CUDA(c_out == 32 ? wgrad_launch<32>(P, grid, st) : wgrad_launch<16>(P, grid, st));
-    } else {
-      conv1w::TableParams T{};
-      static_cast<conv1w::Params&>(T) = P;
-      T.frames = nullptr, T.table = table_dev, T.frame_off = frame_off;
-      B2RL_CUDA(c_out == 32 ? wgrad_launch<32>(T, grid, st) : wgrad_launch<16>(T, grid, st));
-    }
+    const cudaError_t e = with_frame_kind(kind, [&](auto K) {
+      constexpr FrameKind KIND = decltype(K)::value;
+      return c_out == 32 ? wgrad_launch<32, KIND>(P, grid, st) : wgrad_launch<16, KIND>(P, grid, st);
+    });
+    B2RL_CUDA(e);
     count_launch();
     B2RL_CHECK_LAUNCH();
     conv1w::k_conv1_wgrad_reduce<<<(numel + 31) / 32, dim3(32, conv1w::RED_SLICES), 0, st>>>(
@@ -434,46 +389,4 @@ static int wgrad_run(const uint8_t* frames_dev, const uint8_t* const* table_dev,
     B2RL_CHECK_LAUNCH();
   }
   return B2RL_OK;
-}
-
-extern "C" int b2rl_conv1_wgrad_strided(const uint8_t* frames_dev, const uint8_t* const* frame_table_dev,
-                                        int64_t row_stride, int64_t rows, const int64_t* idx_dev, int64_t n,
-                                        const float* gy_dev, const float* y_relu_dev, int32_t c_out,
-                                        float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream) {
-  B2RL_REQUIRE(n >= 1, "n must be positive");
-  B2RL_REQUIRE((frames_dev != nullptr) != (frame_table_dev != nullptr), "exactly one of frames and frame table");
-  B2RL_REQUIRE(row_stride > 0 && row_stride % 16 == 0, "the row stride must be a positive multiple of 16 bytes");
-  B2RL_REQUIRE(frames_dev ? (uintptr_t)frames_dev % 16 == 0 : (uintptr_t)frame_table_dev % 8 == 0,
-               "frames must be 16-byte aligned, a frame table entry 8-byte aligned");
-  return wgrad_run(frames_dev, frame_table_dev, row_stride, rows, idx_dev, n, gy_dev, y_relu_dev, c_out,
-                   workspace_dev, gw_dev, accumulate, stream);
-}
-
-extern "C" int b2rl_conv1_wgrad(const uint8_t* frames_dev, int64_t capacity, const int64_t* idx_dev, int64_t n,
-                                const float* gy_dev, const float* y_relu_dev, int32_t c_out, float* workspace_dev,
-                                float* gw_dev, int32_t accumulate, void* stream) {
-  B2RL_REQUIRE(frames_dev, "null argument");
-  return b2rl_conv1_wgrad_strided(frames_dev, nullptr, conv1w::FRAME_BYTES, capacity, idx_dev, n, gy_dev, y_relu_dev,
-                                  c_out, workspace_dev, gw_dev, accumulate, stream);
-}
-
-extern "C" int b2rl_conv1_wgrad_table(const uint8_t* const* frame_table_dev, int64_t capacity, const int64_t* idx_dev,
-                                      int64_t n, const float* gy_dev, const float* y_relu_dev, int32_t c_out,
-                                      float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream) {
-  B2RL_REQUIRE(frame_table_dev != nullptr, "null frame table");
-  return b2rl_conv1_wgrad_strided(nullptr, frame_table_dev, conv1w::FRAME_BYTES, capacity, idx_dev, n, gy_dev,
-                                  y_relu_dev, c_out, workspace_dev, gw_dev, accumulate, stream);
-}
-
-extern "C" int b2rl_conv1_wgrad_planes(const uint8_t* pool_dev, const int32_t* planes_dev, int32_t plane_base,
-                                       int64_t rows, const int64_t* idx_dev, int64_t n, const float* gy_dev,
-                                       const float* y_relu_dev, int32_t c_out, float* workspace_dev, float* gw_dev,
-                                       int32_t accumulate, void* stream) {
-  B2RL_REQUIRE(n >= 1, "n must be positive");
-  B2RL_REQUIRE(pool_dev != nullptr && planes_dev != nullptr, "null frame pool or plane table");
-  B2RL_REQUIRE((uintptr_t)pool_dev % 16 == 0 && (uintptr_t)planes_dev % 4 == 0,
-               "the frame pool must be 16-byte aligned, the plane table 4-byte aligned");
-  B2RL_REQUIRE(plane_base == 0 || plane_base == 4, "plane_base must be 0 or 4");
-  return wgrad_run(pool_dev, nullptr, conv1w::FRAME_BYTES, rows, idx_dev, n, gy_dev, y_relu_dev, c_out, workspace_dev,
-                   gw_dev, accumulate, stream, planes_dev, plane_base);
 }

@@ -1,0 +1,108 @@
+// Where a frame row lives: the frame source of conv_1's forward (conv1.cu) and weight-gradient (conv1_wgrad.cu)
+// kernels, and the plane address of the frame-deduplicated store's row copies (bulk_rows.cuh).
+//
+// A row is one 28 224-byte frame stack (four 84x84 uint8 frames).  The host turns a b2rl_frames descriptor
+// (include/b2rl.h) into a FrameSource and its FrameKind once; the kernels take the kind as a template parameter, so
+// each kind is its own instantiation with only its own address arithmetic.
+#pragma once
+#include <type_traits>
+
+#include "common.cuh"
+#include "hopper.cuh"
+
+namespace b2rl {
+
+constexpr int PLANE_BYTES = 84 * 84;          // one frame: a channel of a stack, or one frame of a frame pool
+constexpr int STACK_BYTES = 4 * PLANE_BYTES;  // one row
+
+enum class FrameKind {
+  Direct,   // row r at base + r * row_stride
+  Table,    // the same, with the base read from a device-resident entry when the kernel starts
+  Planes,   // channel c of row r is pool frame planes[8 r + plane_base + c]
+};
+
+struct FrameSource {
+  const uint8_t* base;           // Direct: the first row; Planes: the frame pool
+  const uint8_t* const* table;   // Table: the entry that holds the first row's address
+  const int32_t* planes;         // Planes: 8 pool ids per row
+  int64_t row_stride;            // Direct, Table: bytes between rows
+  int64_t table_off;             // Table: bytes added to the entry's address (the rows of earlier split launches)
+  int64_t rows;                  // indices are clamped to [0, rows)
+  int32_t plane_base;            // Planes: 0 or 4
+};
+
+// Frame c of plane-table row `row`.
+__device__ __forceinline__ const uint8_t* plane_ptr(const uint8_t* pool, const int32_t* planes, int64_t row,
+                                                    int32_t plane_base, int c) {
+  return pool + (int64_t)planes[row * 8 + plane_base + c] * PLANE_BYTES;
+}
+
+// The address rows are read from: the base (the pool for Planes), or the table entry's as the kernel starts.
+template <FrameKind KIND>
+__device__ __forceinline__ const uint8_t* frame_base(const FrameSource& S) {
+  if constexpr (KIND == FrameKind::Table) return *S.table + S.table_off;
+  return S.base;
+}
+
+// Row `row` -> `dst` in SMEM, completing STACK_BYTES of transactions on `bar`: one bulk copy of a frame stack, or
+// four of a plane table's frames.  `frames` is frame_base<KIND>(S).
+template <FrameKind KIND>
+__device__ __forceinline__ void load_row(const FrameSource& S, const uint8_t* frames, int64_t row, uint8_t* dst,
+                                         uint64_t* bar) {
+  sm90::mbar_expect_tx(bar, STACK_BYTES);
+  if constexpr (KIND == FrameKind::Planes) {
+#pragma unroll
+    for (int c = 0; c < 4; ++c)
+      sm90::bulk_g2s(dst + c * PLANE_BYTES, plane_ptr(frames, S.planes, row, S.plane_base, c), PLANE_BYTES, bar);
+  } else {
+    sm90::bulk_g2s(dst, frames + row * S.row_stride, STACK_BYTES, bar);
+  }
+}
+
+// Host: refuse a descriptor that does not name exactly one well-formed source, else fill `src` and `kind`.
+inline int check_frames(const b2rl_frames* f, FrameSource& src, FrameKind& kind) {
+  B2RL_REQUIRE(f != nullptr, "null b2rl_frames");
+  const bool pooled = f->pool != nullptr || f->planes != nullptr;
+  const int sources = (f->base != nullptr) + (f->table != nullptr) + pooled;
+  B2RL_REQUIRE(sources > 0, "null frame source: set exactly one of frames, frame table and frame pool");
+  B2RL_REQUIRE(sources == 1, "exactly one of frames, frame table and frame pool may be set");
+  B2RL_REQUIRE(f->rows >= 1, "rows must be positive");
+  src = FrameSource{};
+  src.rows = f->rows;
+  if (pooled) {
+    B2RL_REQUIRE(f->pool != nullptr && f->planes != nullptr, "null frame pool or plane table");
+    B2RL_REQUIRE((uintptr_t)f->pool % 16 == 0 && (uintptr_t)f->planes % 4 == 0,
+                 "the frame pool must be 16-byte aligned, the plane table 4-byte aligned");
+    B2RL_REQUIRE(f->plane_base == 0 || f->plane_base == 4, "plane_base must be 0 or 4");
+    kind = FrameKind::Planes;
+    src.base = f->pool, src.planes = f->planes, src.plane_base = f->plane_base;
+    return B2RL_OK;
+  }
+  B2RL_REQUIRE(f->row_stride > 0 && f->row_stride % 16 == 0, "the row stride must be a positive multiple of 16 bytes");
+  B2RL_REQUIRE(f->base ? (uintptr_t)f->base % 16 == 0 : (uintptr_t)f->table % 8 == 0,
+               "frames must be 16-byte aligned, a frame table entry 8-byte aligned");
+  kind = f->base ? FrameKind::Direct : FrameKind::Table;
+  src.base = f->base, src.table = f->table, src.row_stride = f->row_stride;
+  return B2RL_OK;
+}
+
+// Host: the rows [off, rows) of `S` as rows [0, rows - off), for the launches a weight gradient splits n into.
+inline FrameSource advance(FrameSource S, FrameKind kind, int64_t off) {
+  if (kind == FrameKind::Direct) S.base += off * S.row_stride;
+  else if (kind == FrameKind::Table) S.table_off += off * S.row_stride;
+  else S.planes += 8 * off;
+  S.rows -= off;
+  return S;
+}
+
+// Host: f(std::integral_constant<FrameKind, kind>{}), so that a launch site names each kernel's kind once.
+template <class F>
+inline cudaError_t with_frame_kind(FrameKind kind, F&& f) {
+  switch (kind) {
+    case FrameKind::Table: return f(std::integral_constant<FrameKind, FrameKind::Table>{});
+    case FrameKind::Planes: return f(std::integral_constant<FrameKind, FrameKind::Planes>{});
+    default: return f(std::integral_constant<FrameKind, FrameKind::Direct>{});
+  }
+}
+
+}  // namespace b2rl

@@ -677,15 +677,18 @@ class PlaneFrames:
         return self.pool.device
 
 
-def _frame_source(frames):
-    """-> (rows, row stride in bytes, the frames' pointer or None, the table entry's pointer or None).  A tensor's rows
-    are its first dimension, each a contiguous FRAME_STACK_BYTES; stride(0) is the row stride (the library checks
-    that it is a positive multiple of 16)."""
+def _frame_source(frames) -> _lib.Frames:
+    """The b2rl_frames descriptor of a frame tensor, a BoundFrames or a PlaneFrames.  A tensor's rows are its first
+    dimension, each a contiguous FRAME_STACK_BYTES; stride(0) is the row stride (the library checks that it is a
+    positive multiple of 16)."""
+    if isinstance(frames, PlaneFrames):
+        return _lib.Frames(pool=frames.pool.data_ptr(), planes=frames.planes.data_ptr(), plane_base=frames.base,
+                           rows=frames.planes.shape[0])
     if isinstance(frames, BoundFrames):
-        return frames.rows, frames.row_stride, None, frames.entry_ptr()
+        return _lib.Frames(table=frames.entry_ptr(), row_stride=frames.row_stride, rows=frames.rows)
     assert frames.dtype == torch.uint8 and frames[0].is_contiguous() and frames[0].numel() == FRAME_STACK_BYTES
     stride = frames.stride(0) if frames.shape[0] > 1 else FRAME_STACK_BYTES   # a size-1 dimension's stride is arbitrary
-    return frames.shape[0], stride * frames.element_size(), frames.data_ptr(), None
+    return _lib.Frames(base=frames.data_ptr(), row_stride=stride * frames.element_size(), rows=frames.shape[0])
 
 
 def conv1_fused(frames, idx, pack: Conv1Pack, relu: bool = False, out=None):
@@ -693,23 +696,14 @@ def conv1_fused(frames, idx, pack: Conv1Pack, relu: bool = False, out=None):
     DeviceReplay.field_view("state")), the windows of frame strips (strip_windows), a BoundFrames or a PlaneFrames;
     idx: int64[n] rows to take (None: all rows in order).
     -> list of n_nets tensors (n, c_out, 20, 20) fp32 in channels_last memory format."""
-    if isinstance(frames, PlaneFrames):
-        n = frames.planes.shape[0] if idx is None else idx.numel()
-        if out is None:
-            out = torch.empty((pack.n_nets, n, 20, 20, pack.c_out), dtype=torch.float32, device=frames.device)
-        check(_lib.load().b2rl_conv1_fused_planes(
-            frames.pool.data_ptr(), frames.planes.data_ptr(), frames.base, frames.planes.shape[0],
-            None if idx is None else idx.data_ptr(), n, pack.bq.data_ptr(), pack.scale.data_ptr(), pack.n_nets,
-            pack.c_out, out.data_ptr(), int(bool(relu)), _stream_ptr(frames.device)))
-        return [out[i].permute(0, 3, 1, 2) for i in range(pack.n_nets)]
-    rows, row_stride, ptr, entry = _frame_source(frames)
-    n = rows if idx is None else idx.numel()
+    src = _frame_source(frames)
+    n = src.rows if idx is None else idx.numel()
     dev = frames.device
     if out is None:
         out = torch.empty((pack.n_nets, n, 20, 20, pack.c_out), dtype=torch.float32, device=dev)
-    check(_lib.load().b2rl_conv1_fused_strided(
-        ptr, entry, row_stride, rows, None if idx is None else idx.data_ptr(), n, pack.bq.data_ptr(),
-        pack.scale.data_ptr(), pack.n_nets, pack.c_out, out.data_ptr(), int(bool(relu)), _stream_ptr(dev)))
+    check(_lib.load().b2rl_conv1_fused(
+        src, None if idx is None else idx.data_ptr(), n, pack.bq.data_ptr(), pack.scale.data_ptr(), pack.n_nets,
+        pack.c_out, out.data_ptr(), int(bool(relu)), _stream_ptr(dev)))
     return [out[i].permute(0, 3, 1, 2) for i in range(pack.n_nets)]   # logical NCHW, physical NHWC
 
 
@@ -722,9 +716,8 @@ def conv1_wgrad(frames, idx, gy: torch.Tensor, out: torch.Tensor | None = None,
     frames: as for conv1_fused; idx: int64[n] or None; gy: (n, c_out, 20, 20) fp32
     (made channels_last if it is not) -> (c_out, 4, 8, 8) fp32.  relu_y: the post-ReLU output of
     conv1_fused(relu=True) for the same rows; gy is then dL/d(relu output) and is masked by (y > 0) in the kernel."""
-    planes = isinstance(frames, PlaneFrames)
-    rows, row_stride, ptr, entry = (frames.planes.shape[0], 0, None, None) if planes else _frame_source(frames)
-    n = rows if idx is None else idx.numel()
+    src = _frame_source(frames)
+    n = src.rows if idx is None else idx.numel()
     c_out = gy.shape[1]
     assert gy.shape == (n, c_out, 20, 20) and gy.dtype == torch.float32
     gy = gy.contiguous(memory_format=torch.channels_last)
@@ -740,14 +733,7 @@ def conv1_wgrad(frames, idx, gy: torch.Tensor, out: torch.Tensor | None = None,
         out = torch.empty((c_out, 4, 8, 8), dtype=torch.float32, device=dev)
         accumulate = False
     assert out.is_contiguous() and out.numel() == c_out * 256
-    if planes:
-        check(_lib.load().b2rl_conv1_wgrad_planes(
-            frames.pool.data_ptr(), frames.planes.data_ptr(), frames.base, rows, None if idx is None else idx.data_ptr(),
-            n, gy.data_ptr(), None if relu_y is None else relu_y.data_ptr(), c_out, _wgrad_ws[key].data_ptr(),
-            out.data_ptr(), int(bool(accumulate)), _stream_ptr(dev)))
-        return out
-    check(_lib.load().b2rl_conv1_wgrad_strided(
-        ptr, entry, row_stride, rows, None if idx is None else idx.data_ptr(), n, gy.data_ptr(),
-        None if relu_y is None else relu_y.data_ptr(), c_out, _wgrad_ws[key].data_ptr(), out.data_ptr(),
-        int(bool(accumulate)), _stream_ptr(dev)))
+    check(_lib.load().b2rl_conv1_wgrad(
+        src, None if idx is None else idx.data_ptr(), n, gy.data_ptr(), None if relu_y is None else relu_y.data_ptr(),
+        c_out, _wgrad_ws[key].data_ptr(), out.data_ptr(), int(bool(accumulate)), _stream_ptr(dev)))
     return out

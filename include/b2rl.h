@@ -274,6 +274,34 @@ int b2rl_vtrace(const float* pi_a_dev, const float* mu_a_dev, const float* value
                 float gamma, float c_lambda, float c_bar, float p_bar, float* vtarget_out_dev,
                 float* advantage_out_dev, void* stream);
 
+/* Where conv_1 (b2rl_conv1_fused, b2rl_conv1_wgrad) reads frame row r: a 28 224-byte stack of four 84x84 uint8
+ * frames.  Exactly one of three sources is set, the other pointers NULL:
+ *   base    row r is at base + r * row_stride (16-byte aligned).  A stride of 28 224 reads whole frame stacks, e.g.
+ *           b2rl_replay_field_ptr of the state field.  A stride of 7 056 reads the overlapping 4-frame windows of an
+ *           R2D2 frame strip: a sequence of T observations stored as its T + 3 distinct frames, where stack t is
+ *           frames t .. t + 3 (R2D2/Player.py:38-63 stacks the last four frames of one episode, and
+ *           R2D2/ReplayMemory.py:70-88 stores T such stacks per sequence).
+ *   table   ONE device-resident entry (const uint8_t*, 8-byte aligned) that holds `base`, read when the kernels
+ *           start, e.g. written by b2rl_serve_bind: a launch captured in a CUDA graph reads whichever served
+ *           minibatch slot (Replay_Server.sample, APE_X/ReplayMemory.py:251-257) was bound before the replay.  The
+ *           base it holds must be 16-byte aligned.  When b2rl_conv1_wgrad splits a large n over several launches
+ *           (idx_dev NULL), each launch adds its row offset to the loaded base on the device.
+ *   pool + planes (+ plane_base)   the frame-deduplicated Ape-X store (b2rl_dedup_attach): channel c of row r is
+ *           the 7 056-byte frame pool + planes[8 r + plane_base + c] * 7 056 (pool 16-byte aligned, planes 4-byte
+ *           aligned; plane_base 0: `state`, 4: `next_state` of the transition APE_X/Player.py:252-261 sends).
+ * row_stride (base and table) must be a positive multiple of 16.  Row indices are clamped to [0, rows), rows >= 1:
+ * the caller guarantees that row rows - 1 ends inside the allocation. */
+typedef struct {
+  const uint8_t* base;
+  const uint8_t* const* table;
+  const uint8_t* pool;
+  const int32_t* planes;
+  int64_t row_stride;
+  int64_t rows;
+  int32_t plane_base;
+  int32_t reserved;
+} b2rl_frames;
+
 /* Fused gather + first convolution (north-star "TMA staging of sampled transition slices
  * into shared memory for the Q-network's first GEMM"): conv_1 of cfg/ape_x.json / cfg/r2d2.json
  * (8x8, stride 4, 4 -> 32 channels, no bias; baseline/baseNetwork.py:165-172) applied to
@@ -282,9 +310,9 @@ int b2rl_vtrace(const float* pi_a_dev, const float* mu_a_dev, const float* value
  * c_out = 32 (cfg/ape_x.json, cfg/r2d2.json) or 16 (cfg/impala.json:25-37).
  *   b2rl_conv1_pack   w_dev fp32 [c_out][4][8][8] of network `net` -> packed int8 digits
  *                     (bq_out: n_nets*4*c_out*256 bytes) and per-channel scale (scale_out: n_nets*c_out fp32)
- *   b2rl_conv1_fused  frames_dev: rows of 28 224 bytes (e.g. b2rl_replay_field_ptr of the state
- *                     field), idx_dev int64[n] or NULL (rows 0..n-1), out_dev fp32
- *                     [n_nets][n][20][20][c_out] (NHWC), relu != 0 applies ReLU. */
+ *   b2rl_conv1_fused  frames: the rows' source (host struct), idx_dev int64[n] or NULL (rows 0..n-1), out_dev fp32
+ *                     [n_nets][n][20][20][c_out] (NHWC), relu != 0 applies ReLU.  An error, and no launch, for a
+ *                     source b2rl_frames does not allow. */
 int b2rl_conv1_pack(const float* w_dev, int32_t net, int32_t n_nets, int32_t c_out, int8_t* bq_out_dev,
                     float* scale_out_dev, void* stream);
 /* Up to 4 such packs in ONE launch (host arrays of `jobs` entries): the learner step packs the online conv_1 weights
@@ -293,68 +321,22 @@ int b2rl_conv1_pack(const float* w_dev, int32_t net, int32_t n_nets, int32_t c_o
 int b2rl_conv1_pack_jobs(const float* const* w_dev, const int32_t* net, const int32_t* n_nets,
                          int8_t* const* bq_out_dev, float* const* scale_out_dev, int32_t jobs, int32_t c_out,
                          void* stream);
-int b2rl_conv1_fused(const uint8_t* frames_dev, int64_t capacity, const int64_t* idx_dev, int64_t n,
-                     const int8_t* bq_dev, const float* scale_dev, int32_t n_nets, int32_t c_out,
-                     float* out_dev, int32_t relu, void* stream);
+int b2rl_conv1_fused(const b2rl_frames* frames, const int64_t* idx_dev, int64_t n, const int8_t* bq_dev,
+                     const float* scale_dev, int32_t n_nets, int32_t c_out, float* out_dev, int32_t relu,
+                     void* stream);
 
 /* Weight gradient of conv_1 fused with the gather (the backward half of b2rl_conv1_fused;
  * loss.backward() in APE_X/Learner.py:123-138 for baseline/baseNetwork.py:165-172's first layer):
  *   gw[co][c][ky][kx] (+)= (1/255) * sum_{k,oy,ox} gy[k][oy][ox][co] * frames[idx[k]][c][4oy+ky][4ox+kx]
- * gy_dev: [n][20][20][c_out] fp32 (NHWC); y_relu_dev: NULL, or the post-ReLU output of b2rl_conv1_fused(relu = 1)
- * for the same rows — gy is then the gradient w.r.t. that output and is masked by (y > 0) on the fly (the
- * ReLU's backward); gw_dev: [c_out][4][8][8] fp32; workspace_dev:
+ * frames: as for b2rl_conv1_fused; gy_dev: [n][20][20][c_out] fp32 (NHWC); y_relu_dev: NULL, or the post-ReLU output
+ * of b2rl_conv1_fused(relu = 1) for the same rows — gy is then the gradient w.r.t. that output and is masked by
+ * (y > 0) on the fly (the ReLU's backward); gw_dev: [c_out][4][8][8] fp32; workspace_dev:
  * b2rl_conv1_wgrad_workspace_floats(c_out) floats of scratch (per-SM partial sums, summed in fp64 in a
  * fixed order: the result is deterministic).  idx_dev may be NULL (rows 0..n-1). */
 int64_t b2rl_conv1_wgrad_workspace_floats(int32_t c_out);
-int b2rl_conv1_wgrad(const uint8_t* frames_dev, int64_t capacity, const int64_t* idx_dev, int64_t n,
-                     const float* gy_dev, const float* y_relu_dev, int32_t c_out, float* workspace_dev,
-                     float* gw_dev, int32_t accumulate, void* stream);
-
-/* conv_1 forward and weight gradient of a learner step on a minibatch served by the stand-alone replay server
- * (Replay_Server.sample, APE_X/ReplayMemory.py:251-257, feeding Learner.train, APE_X/Learner.py:55-121): the same
- * kernels and results as b2rl_conv1_fused / b2rl_conv1_wgrad, but the frame base is not an argument.
- * frame_table_dev points to ONE device-resident entry (const uint8_t*) that the kernels read when they start, e.g.
- * written by b2rl_serve_bind, so a launch captured in a CUDA graph reads whichever slot was bound before the replay.
- * The base it holds must be 16-byte aligned; when b2rl_conv1_wgrad_table splits a large n over several launches
- * (idx_dev NULL) each launch adds its row offset to the loaded base on the device.  An error, and no launch, for a
- * null or misaligned entry. */
-int b2rl_conv1_fused_table(const uint8_t* const* frame_table_dev, int64_t capacity, const int64_t* idx_dev, int64_t n,
-                           const int8_t* bq_dev, const float* scale_dev, int32_t n_nets, int32_t c_out,
-                           float* out_dev, int32_t relu, void* stream);
-int b2rl_conv1_wgrad_table(const uint8_t* const* frame_table_dev, int64_t capacity, const int64_t* idx_dev,
-                           int64_t n, const float* gy_dev, const float* y_relu_dev, int32_t c_out,
-                           float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream);
-
-/* conv_1 forward and weight gradient over frame rows `row_stride` bytes apart: row r is the 28 224 bytes that start
- * at base + r * row_stride.  A stride of 28 224 reads whole frame stacks, exactly as b2rl_conv1_fused / _wgrad (and
- * their _table forms, which call these with that stride).  A stride of 7 056 reads the overlapping 4-frame windows
- * of an R2D2 frame strip: a sequence of T observations stored as its T + 3 distinct 84x84 frames, where stack t is
- * frames t .. t + 3 (R2D2/Player.py:38-63 stacks the last four frames of one episode, and R2D2/ReplayMemory.py:70-88
- * stores T such stacks per sequence).  Exactly one of frames_dev (the base, 16-byte aligned) and frame_table_dev
- * (one device-resident entry holding the base, 8-byte aligned, as for the _table forms) is non-null.  `rows` is the
- * number of rows indices are clamped to: the caller guarantees that row rows - 1 ends inside the allocation.  An
- * error, and no launch, for a stride that is not a positive multiple of 16 or a null or misaligned source. */
-int b2rl_conv1_fused_strided(const uint8_t* frames_dev, const uint8_t* const* frame_table_dev, int64_t row_stride,
-                             int64_t rows, const int64_t* idx_dev, int64_t n, const int8_t* bq_dev,
-                             const float* scale_dev, int32_t n_nets, int32_t c_out, float* out_dev, int32_t relu,
-                             void* stream);
-int b2rl_conv1_wgrad_strided(const uint8_t* frames_dev, const uint8_t* const* frame_table_dev, int64_t row_stride,
-                             int64_t rows, const int64_t* idx_dev, int64_t n, const float* gy_dev,
-                             const float* y_relu_dev, int32_t c_out, float* workspace_dev, float* gw_dev,
-                             int32_t accumulate, void* stream);
-
-/* conv_1 forward and weight gradient over frame stacks held as plane tables (the frame-deduplicated Ape-X store,
- * b2rl_dedup_attach): row r is the stack whose channel c is the 7 056-byte frame pool_dev + planes_dev[8 r +
- * plane_base + c] * 7 056 (plane_base 0: `state`, 4: `next_state` of the transition APE_X/Player.py:252-261 sends).
- * Same arithmetic, outputs and arguments otherwise as b2rl_conv1_fused_strided / _wgrad_strided; `rows` is the
- * number of plane-table rows indices are clamped to.  An error, and no launch, for a null or misaligned pool or
- * table, or a plane_base other than 0 or 4. */
-int b2rl_conv1_fused_planes(const uint8_t* pool_dev, const int32_t* planes_dev, int32_t plane_base, int64_t rows,
-                            const int64_t* idx_dev, int64_t n, const int8_t* bq_dev, const float* scale_dev,
-                            int32_t n_nets, int32_t c_out, float* out_dev, int32_t relu, void* stream);
-int b2rl_conv1_wgrad_planes(const uint8_t* pool_dev, const int32_t* planes_dev, int32_t plane_base, int64_t rows,
-                            const int64_t* idx_dev, int64_t n, const float* gy_dev, const float* y_relu_dev,
-                            int32_t c_out, float* workspace_dev, float* gw_dev, int32_t accumulate, void* stream);
+int b2rl_conv1_wgrad(const b2rl_frames* frames, const int64_t* idx_dev, int64_t n, const float* gy_dev,
+                     const float* y_relu_dev, int32_t c_out, float* workspace_dev, float* gw_dev, int32_t accumulate,
+                     void* stream);
 
 /* Learner.step (APE_X/Learner.py:123-138; IMPALA/Learner.py:258-266 without the clipping) with
  * torch.optim.RMSprop's update (baseline/utils.py getOptim :124-130; centered for Ape-X,
@@ -517,7 +499,7 @@ int b2rl_serve_take(const b2rl_serve_ring* r, int32_t slot, void* dst_dev, void*
  * with b2rl_serve_take), laid out by `layout`, is bound to the step's fixed buffers.  The header {seq, n}, idx and
  * w are copied to header_out_dev (16 B), idx_out_dev (int64[n]) and w_out_dev (fp32[n]).  For each field f:
  * fields_out_dev[f] != NULL receives a copy of its n rows; table_out_dev[f] != NULL (an 8-byte aligned device
- * entry, for b2rl_conv1_fused_table / b2rl_conv1_wgrad_table) receives the device address of its rows instead, so
+ * entry, the `table` of a b2rl_frames source) receives the device address of its rows instead, so
  * the frames are read in the slot.  Either host array may be NULL.  An error, and no launch, for a null slot, a slot
  * base that is not 16-byte aligned or a layout whose batch is not n.  The slot must stay unreleased until the last
  * kernel that reads a table entry has run. */

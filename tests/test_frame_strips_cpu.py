@@ -326,16 +326,22 @@ def test_the_reference_actor_sends_sequences_that_slide(golden):
     np.testing.assert_array_equal(cols[0], strips)
 
 
-def test_strided_entry_points_refuse_bad_sources_before_any_launch(rs):
+def test_conv1_refuses_bad_frame_sources_before_any_launch(rs):
+    """conv_1's forward and weight gradient refuse a bad frame source, strided or plane table, before any launch."""
     from distributed_rl_b200 import _lib
     lib = _lib.load()
     A = 0x10000                                                     # 16-byte aligned, never dereferenced
-    fwd = lambda f, t, stride: lib.b2rl_conv1_fused_strided(f, t, stride, 8, None, 8, A, A, 1, 32, A, 0, None)
-    bwd = lambda f, t, stride: lib.b2rl_conv1_wgrad_strided(f, t, stride, 8, None, 8, A, None, 32, A, A, 0, None)
+    fwd = lambda src: lib.b2rl_conv1_fused(src, None, 8, A, A, 1, 32, A, 0, None)
+    bwd = lambda src: lib.b2rl_conv1_wgrad(src, None, 8, A, None, 32, A, A, 0, None)
+    strided = [(dict(base=f, table=t, row_stride=stride), msg)
+               for f, t, stride, msg in ((A, None, 0, b"row stride"), (A, None, -7056, b"row stride"),
+                                         (A, None, 7000, b"row stride"), (A + 8, None, 7056, b"aligned"),
+                                         (None, A + 4, 7056, b"aligned"), (None, None, 7056, b"exactly one"),
+                                         (A, A, 7056, b"exactly one"))]
+    planes = [(dict(pool=A, planes=A, plane_base=2), b"plane_base"), (dict(pool=A + 8, planes=A), b"16-byte aligned"),
+              (dict(pool=A, planes=A + 2, plane_base=4), b"4-byte aligned"), (dict(pool=A), b"plane table"),
+              (dict(pool=A, planes=A, base=A), b"exactly one"), (dict(pool=A, planes=A, rows=0), b"rows")]
     for call in (fwd, bwd):
-        for f, t, stride, msg in ((A, None, 0, b"row stride"), (A, None, -7056, b"row stride"),
-                                  (A, None, 7000, b"row stride"), (A + 8, None, 7056, b"aligned"),
-                                  (None, A + 4, 7056, b"aligned"), (None, None, 7056, b"exactly one"),
-                                  (A, A, 7056, b"exactly one")):
-            assert call(f, t, stride) < 0, (f, t, stride)
+        for kw, msg in strided + planes:
+            assert call(_lib.Frames(**{"rows": 8, **kw})) < 0, kw
             assert msg in lib.b2rl_last_error(), lib.b2rl_last_error()

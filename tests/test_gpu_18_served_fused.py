@@ -1,7 +1,7 @@
 """GPU tests of the captured Ape-X step on served minibatches (ApexConfig.SERVED_FUSED_STEP).
 
-Kernels: conv_1 forward and weight gradient through a device-resident frame-table entry (b2rl_conv1_fused_table,
-b2rl_conv1_wgrad_table) against the direct kernels, bit for bit, including an n that the weight gradient splits
+Kernels: conv_1 forward and weight gradient through a device-resident frame-table entry (the `table` source of
+b2rl_frames) against the direct kernels, bit for bit, including an n that the weight gradient splits
 over several launches, and a captured graph rebound to other frames.  Bind: b2rl_serve_bind against the slot it
 binds.  Learner: a two-process run (the pattern of test_gpu_14_serve.py) whose every bound step is replayed by an
 in-process learner, which must end with the same weights, and whose write-backs must all land in the server's
@@ -69,7 +69,7 @@ def test_table_variants_equal_the_direct_kernels(relu, n_nets):
 
 
 def test_table_weight_gradient_split_over_several_launches():
-    """n above SMs x 160 frame stacks: b2rl_conv1_wgrad_table adds each launch's row offset on the device."""
+    """n above SMs x 160 frame stacks: b2rl_conv1_wgrad adds each launch's row offset to the table entry on the device."""
     from distributed_rl_b200 import replay as R
     per_launch = torch.cuda.get_device_properties(0).multi_processor_count * 160
     n = per_launch + 257

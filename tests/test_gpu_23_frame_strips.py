@@ -3,10 +3,8 @@
 Kernels: conv_1 forward and weight gradient over the windows of frame strips (rows 7 056 bytes apart) against the
 same kernels over the materialised stacks, for direct and table sources, time-major rows with repeated slots, ReLU
 on and off, one and two networks, 32 and 16 channels, the last window of the allocation and a weight gradient split
-over two launches; and every existing conv_1 entry point against its `_strided` twin at 28 224 bytes.  Learner:
-train(), the captured in-process fused_step and the captured served step on strips against stacks, a two-process run,
-the reference-format ingest, and a 100 000-sequence strip replay on an 80 GB card."""
-import ctypes
+over two launches.  Learner: train(), the captured in-process fused_step and the captured served step on strips
+against stacks, a two-process run, the reference-format ingest, and a 100 000-sequence strip replay on an 80 GB card."""
 import multiprocessing as mp
 import pickle
 import time
@@ -111,39 +109,6 @@ def test_weight_gradient_over_windows_split_over_two_launches(accumulate):
     assert not torch.equal(R.conv1_wgrad(win, None, gy, relu_y=y), part)      # the second launch's rows count
     del win, stacks, bound, gy, y
     torch.cuda.empty_cache()
-
-
-def test_existing_entry_points_equal_their_strided_twins():
-    from distributed_rl_b200 import _lib, replay as R
-    lib = _lib.load()
-    n_rows, n = 300, 200
-    X = _strips(1, n_rows * 4 - 3, 9).view(n_rows, 4, 84, 84)
-    table = torch.tensor([X.data_ptr()], dtype=torch.int64, device="cuda")
-    tp = ctypes.c_void_p(table.data_ptr())
-    idx = torch.randint(0, n_rows, (n,), device="cuda", generator=torch.Generator(device="cuda").manual_seed(1))
-    pack = _pack(2, 32, 3)
-    st = torch.cuda.current_stream().cuda_stream
-    for rows_ptr, m in ((idx.data_ptr(), n), (None, n_rows)):
-        outs = [torch.empty((2, m, 20, 20, 32), device="cuda") for _ in range(4)]
-        args = (m, pack.bq.data_ptr(), pack.scale.data_ptr(), 2, 32)
-        _lib.check(lib.b2rl_conv1_fused(X.data_ptr(), n_rows, rows_ptr, *args, outs[0].data_ptr(), 1, st))
-        _lib.check(lib.b2rl_conv1_fused_strided(X.data_ptr(), None, R.FRAME_STACK_BYTES, n_rows, rows_ptr, *args,
-                                                outs[1].data_ptr(), 1, st))
-        _lib.check(lib.b2rl_conv1_fused_table(tp, n_rows, rows_ptr, *args, outs[2].data_ptr(), 1, st))
-        _lib.check(lib.b2rl_conv1_fused_strided(None, tp, R.FRAME_STACK_BYTES, n_rows, rows_ptr, *args,
-                                                outs[3].data_ptr(), 1, st))
-        assert all(torch.equal(outs[0], o) for o in outs[1:])
-        gy = _gy(m, 32, 4)
-        ws = torch.empty(lib.b2rl_conv1_wgrad_workspace_floats(32), device="cuda")
-        gws = [torch.full((32, 4, 8, 8), 0.5, device="cuda") for _ in range(4)]
-        wargs = (m, gy.data_ptr(), outs[0][0].data_ptr(), 32, ws.data_ptr())
-        _lib.check(lib.b2rl_conv1_wgrad(X.data_ptr(), n_rows, rows_ptr, *wargs, gws[0].data_ptr(), 1, st))
-        _lib.check(lib.b2rl_conv1_wgrad_strided(X.data_ptr(), None, R.FRAME_STACK_BYTES, n_rows, rows_ptr, *wargs,
-                                                gws[1].data_ptr(), 1, st))
-        _lib.check(lib.b2rl_conv1_wgrad_table(tp, n_rows, rows_ptr, *wargs, gws[2].data_ptr(), 1, st))
-        _lib.check(lib.b2rl_conv1_wgrad_strided(None, tp, R.FRAME_STACK_BYTES, n_rows, rows_ptr, *wargs,
-                                                gws[3].data_ptr(), 1, st))
-        assert all(torch.equal(gws[0], g) for g in gws[1:])
 
 
 # ---- the learner ----------------------------------------------------------------------------------------------------

@@ -1,6 +1,7 @@
 """GPU tests of the frame-deduplicated Ape-X store (R.DedupReplay, ApexConfig.FRAME_DEDUP): pool ids against the CPU
 model after several wraps of both rings, byte-exact stacks for every live slot, zero priority for dead ones, with
-exact and with forced-collision keys; conv_1 over plane tables; the captured learner step against a stack store."""
+exact and with forced-collision keys; conv_1 over plane tables, and a weight gradient over them split over two
+launches; the captured learner step against a stack store."""
 import os
 import pickle
 import sys
@@ -114,6 +115,29 @@ def test_conv1_on_plane_tables_equals_rows(R, n_nets, c_out, relu):
     full = st.gather(all_rows)
     y_all = R.conv1_fused(st.frame_source("state"), None, pack, relu=relu)[0]
     assert torch.equal(y_all, R.conv1_fused(full["state"], None, pack, relu=relu)[0])
+
+
+@pytest.mark.parametrize("accumulate", [False, True])
+def test_plane_weight_gradient_split_over_two_launches(R, accumulate):
+    """n = SMs * 160 + 257 plane-table rows without idx: the second launch starts 8 * off pool ids into the table."""
+    per_launch = torch.cuda.get_device_properties(0).multi_processor_count * 160
+    n = per_launch + 257
+    g = torch.Generator(device="cuda"); g.manual_seed(9)
+    pool = torch.randint(0, 256, (1024, 84, 84), dtype=torch.uint8, device="cuda", generator=g)
+    planes = torch.randint(0, 1024, (n, 8), dtype=torch.int32, device="cuda", generator=g)
+    src = R.PlaneFrames(pool, planes, 4)
+    stacks = pool[planes[:, 4:8].long()]                          # the same rows gathered: (n, 4, 84, 84)
+    gy = torch.randn(n, 32, 20, 20, device="cuda", generator=g)
+    y = torch.relu(torch.randn(n, 32, 20, 20, device="cuda", generator=g))
+    outs = []
+    for frames in (stacks, src):
+        out = torch.full((32, 4, 8, 8), 0.25, device="cuda")
+        outs.append(R.conv1_wgrad(frames, None, gy, out=out, accumulate=accumulate, relu_y=y))
+    assert torch.equal(outs[0], outs[1])
+    part = R.conv1_wgrad(stacks[:per_launch], None, gy[:per_launch], relu_y=y[:per_launch])
+    assert not torch.equal(R.conv1_wgrad(src, None, gy, relu_y=y), part)   # the second launch's rows count
+    del stacks, gy, y
+    torch.cuda.empty_cache()
 
 
 def _learner(apex, dedup, B, N):

@@ -167,7 +167,7 @@ def test_served_fused_step_refusals(rs):
         L.enable_data_parallel()
 
 
-def test_new_entry_points_reject_bad_arguments_before_any_launch(rs):
+def test_serve_bind_and_table_sources_reject_bad_arguments_before_any_launch(rs):
     from distributed_rl_b200 import _lib, replay as R
     lib = _lib.load()
     L = rs.serve_layout(8, 2, [f.nbytes for f in R.APEX_FIELDS])
@@ -182,9 +182,10 @@ def test_new_entry_points_reject_bad_arguments_before_any_launch(rs):
     both = (ctypes.c_void_p * _lib.MAX_FIELDS)(0x20000)
     assert lib.b2rl_serve_bind(0x100000, ctypes.byref(L), 8, *bufs, both, both, None) < 0
     assert b"not both" in lib.b2rl_last_error()
-    assert lib.b2rl_conv1_fused_table(None, 8, None, 8, 0x1000, 0x1000, 1, 32, 0x1000, 1, None) < 0
-    assert b"null frame table" in lib.b2rl_last_error()
-    assert lib.b2rl_conv1_fused_table(0x1004, 8, None, 8, 0x1000, 0x1000, 1, 32, 0x1000, 1, None) < 0
+    table = lambda entry: _lib.Frames(table=entry, row_stride=R.FRAME_STACK_BYTES, rows=8)
+    assert lib.b2rl_conv1_fused(table(None), None, 8, 0x1000, 0x1000, 1, 32, 0x1000, 1, None) < 0
+    assert b"null frame source" in lib.b2rl_last_error()
+    assert lib.b2rl_conv1_fused(table(0x1004), None, 8, 0x1000, 0x1000, 1, 32, 0x1000, 1, None) < 0
     assert b"8-byte" in lib.b2rl_last_error()
-    assert lib.b2rl_conv1_wgrad_table(None, 8, None, 8, 0x1000, None, 32, 0x1000, 0x1000, 0, None) < 0
-    assert b"null frame table" in lib.b2rl_last_error()
+    assert lib.b2rl_conv1_wgrad(table(None), None, 8, 0x1000, None, 32, 0x1000, 0x1000, 0, None) < 0
+    assert b"null frame source" in lib.b2rl_last_error()
