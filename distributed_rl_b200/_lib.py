@@ -40,6 +40,8 @@ SIGNATURES = {
     "b2rl_version": (C.c_int, []),
     "b2rl_replay_create": (C.c_int, [C.POINTER(ReplayDesc), C.POINTER(c_vp)]),
     "b2rl_replay_destroy": (C.c_int, [c_vp]),
+    "b2rl_replay_create_placed": (C.c_int, [C.POINTER(ReplayDesc), C.POINTER(c_i32), C.POINTER(c_vp)]),
+    "b2rl_replay_field_placement": (C.c_int, [c_vp, c_i32, C.POINTER(c_i32)]),
     "b2rl_replay_size": (C.c_int, [c_vp, C.POINTER(c_i64), C.POINTER(c_i64), C.POINTER(c_i64)]),
     "b2rl_replay_field_ptr": (C.c_int, [c_vp, c_i32, C.POINTER(c_vp)]),
     "b2rl_replay_push": (C.c_int, [c_vp, C.POINTER(c_vp), c_vp, c_i64, c_vp]),

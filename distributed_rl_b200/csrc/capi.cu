@@ -26,8 +26,10 @@ extern "C" int64_t b2rl_launch_count(void) { return g_launches.load(std::memory_
 
 static void free_all(b2rl_replay* h) {
   dedup_free(h);
-  for (int f = 0; f < B2RL_MAX_FIELDS; ++f)
-    if (h->field[f]) cudaFree(h->field[f]);
+  for (int f = 0; f < B2RL_MAX_FIELDS; ++f) {
+    if (h->host_field[f]) cudaFreeHost(h->host_field[f]);
+    else if (h->field[f]) cudaFree(h->field[f]);
+  }
   if (h->tree.leaf) cudaFree(h->tree.leaf);
   if (h->tree.sum) cudaFree(h->tree.sum);
   if (h->tree.minv) cudaFree(h->tree.minv);
@@ -43,10 +45,17 @@ static void free_all(b2rl_replay* h) {
 }
 
 extern "C" int b2rl_replay_create(const b2rl_replay_desc* d, b2rl_replay** out) {
+  return b2rl_replay_create_placed(d, nullptr, out);
+}
+
+extern "C" int b2rl_replay_create_placed(const b2rl_replay_desc* d, const int32_t* on_host, b2rl_replay** out) {
   B2RL_REQUIRE(d != nullptr && out != nullptr, "null argument");
   B2RL_REQUIRE(d->capacity >= 1 && d->capacity <= (1LL << 31), "capacity must be in [1, 2^31]");
   B2RL_REQUIRE(d->n_fields >= 0 && d->n_fields <= B2RL_MAX_FIELDS, "n_fields out of range");
   for (int f = 0; f < d->n_fields; ++f) B2RL_REQUIRE(d->field_bytes[f] >= 1, "field_bytes must be >= 1");
+  for (int f = 0; on_host != nullptr && f < d->n_fields; ++f)
+    B2RL_REQUIRE(!on_host[f] || d->field_bytes[f] % 16 == 0,
+                 "a field placed on the host must have rows of a whole number of 16-byte units");
   int ndev = 0;
   B2RL_CUDA(cudaGetDeviceCount(&ndev));
   B2RL_REQUIRE(d->device >= 0 && d->device < ndev, "no such CUDA device");
@@ -77,7 +86,24 @@ extern "C" int b2rl_replay_create(const b2rl_replay_desc* d, b2rl_replay** out) 
   for (int f = 0; f < d->n_fields; ++f) {
     h->field_bytes[f] = d->field_bytes[f];
     // +16 B so a 16-byte bulk/vector access on the last row never leaves the allocation
-    alloc((void**)&h->field[f], (size_t)d->capacity * (size_t)d->field_bytes[f] + 16);
+    const size_t bytes = (size_t)d->capacity * (size_t)d->field_bytes[f] + 16;
+    if (on_host == nullptr || !on_host[f]) {
+      alloc((void**)&h->field[f], bytes);
+      continue;
+    }
+    if (e != cudaSuccess) continue;
+    h->on_host[f] = h->any_on_host = true;
+    const cudaError_t eh = cudaHostAlloc((void**)&h->host_field[f], bytes, cudaHostAllocMapped | cudaHostAllocPortable);
+    if (eh != cudaSuccess) {
+      h->host_field[f] = nullptr;
+      set_error("cudaHostAlloc of %.3f GB (%zu bytes) of pinned host memory for field %d failed: %s", bytes * 1e-9,
+                bytes, f, cudaGetErrorString(eh));
+      free_all(h);
+      delete h;
+      cudaGetLastError();
+      return B2RL_ERR_NOMEM;
+    }
+    e = cudaHostGetDevicePointer((void**)&h->field[f], h->host_field[f], 0);
   }
   alloc((void**)&t.leaf, sizeof(float) * (size_t)h->cap2);
   alloc((void**)&t.sum, sizeof(double) * (size_t)total);
@@ -131,6 +157,13 @@ extern "C" int b2rl_replay_size(const b2rl_replay* h, int64_t* size, int64_t* ca
 extern "C" int b2rl_replay_field_ptr(const b2rl_replay* h, int32_t field, void** ptr_dev) {
   B2RL_REQUIRE(h != nullptr && ptr_dev != nullptr, "null argument");
   B2RL_REQUIRE(field >= 0 && field < h->n_fields, "no such field");
-  *ptr_dev = h->field[field];
+  *ptr_dev = h->on_host[field] ? h->host_field[field] : h->field[field];
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_replay_field_placement(const b2rl_replay* h, int32_t field, int32_t* on_host) {
+  B2RL_REQUIRE(h != nullptr && on_host != nullptr, "null argument");
+  B2RL_REQUIRE(field >= 0 && field < h->n_fields, "no such field");
+  *on_host = h->on_host[field] ? 1 : 0;
   return B2RL_OK;
 }

@@ -139,11 +139,19 @@ struct b2rl_replay;
 namespace b2rl {
 // Stream-ordered publication of the host-side `size` to n_valid_dev (tree.cu).
 int publish_size(b2rl_replay* h, cudaStream_t st);
-// Record i of fields_src -> ring slot (start + i) % capacity; a NULL field is skipped (gather.cu).
+// Record i of fields_src -> ring slot (start + i) % capacity; a NULL field is skipped (gather.cu).  Call
+// check_host_sources first: a host field's source must be device or pinned host memory.
+int check_host_sources(const b2rl_replay* h, const void* const* fields_src);
 int copy_ring_range(b2rl_replay* h, const void* const* fields_src, int64_t start, int64_t n, cudaStream_t st);
 // The n records at head become sampleable with the device priorities prios_dev; head moves past them (gather.cu).
 int publish(b2rl_replay* h, const float* prios_dev, int64_t n, cudaStream_t st);
-struct DedupState;                        // the frame pool of a deduplicated Ape-X replay (dedup.cu)
+// Rows clamp_row(idx_dev[k]) of host field f -> dst_dev + k * field_bytes[f], k < n, through 16-byte loads of the
+// mapped rows (hostrows.cu).  dst_dev 16-byte aligned.
+int gather_host_rows(b2rl_replay* h, int f, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, cudaStream_t st);
+// `bytes` from src (device or pinned host memory) into host field f from ring slot `slot` on, in stream order
+// (hostrows.cu).
+int copy_into_host_field(b2rl_replay* h, int f, int64_t slot, const uint8_t* src, int64_t bytes, cudaStream_t st);
+struct DedupState;                       // the frame pool of a deduplicated Ape-X replay (dedup.cu)
 void dedup_free(b2rl_replay* h);
 int dedup_planes_field(const b2rl_replay* h);
 const uint8_t* dedup_pool(const b2rl_replay* h);
@@ -157,7 +165,11 @@ struct b2rl_replay {
   int levels = 0;
   int n_fields = 0;
   int64_t field_bytes[B2RL_MAX_FIELDS] = {0};
-  uint8_t* field[B2RL_MAX_FIELDS] = {nullptr};
+  uint8_t* field[B2RL_MAX_FIELDS] = {nullptr};      // the address kernels use: device memory, or the device alias of
+                                                    // a host field's pinned rows
+  uint8_t* host_field[B2RL_MAX_FIELDS] = {nullptr}; // b2rl_replay_create_placed: the host address of a host field
+  bool on_host[B2RL_MAX_FIELDS] = {false};
+  bool any_on_host = false;
   TreeView tree = {};         // leaves + sparse fp64 levels (owned: tree.leaf, tree.sum, tree.minv)
   uint32_t* tag = nullptr;    // [cap2]   last-writer tags of the large scattered update, self-cleaning
   int64_t* scratch_idx = nullptr;  // [capacity] ring indices for push/evict

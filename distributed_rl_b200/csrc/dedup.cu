@@ -284,6 +284,7 @@ extern "C" int b2rl_dedup_attach(b2rl_replay* h, int32_t planes_field, int64_t p
                                  uint64_t hash_mask) {
   B2RL_REQUIRE(h != nullptr, "null handle");
   B2RL_REQUIRE(h->dedup == nullptr, "the replay already has a frame pool");
+  B2RL_REQUIRE(!h->any_on_host, "a replay with fields placed on the host cannot take a frame pool");
   B2RL_REQUIRE(h->size == 0 && h->head == 0 && h->reserved == 0 && h->pipe_n == 0, "the replay must be empty");
   B2RL_REQUIRE(planes_field >= 0 && planes_field < h->n_fields && h->field_bytes[planes_field] == 32,
                "the planes field must hold 8 int32 per slot");

@@ -146,6 +146,11 @@ static int gather_run(b2rl_replay* h, const int64_t* idx_dev, int64_t n, void* c
   for (int f = 0; f < h->n_fields; ++f) {
     uint8_t* out = out_fields_dev ? (uint8_t*)out_fields_dev[f] : nullptr;
     if (out == nullptr || (stacks_out != nullptr && f == dedup_planes_field(h))) continue;
+    if (h->on_host[f]) {                  // never the TMA row copy: the 16-byte load gather of hostrows.cu
+      const int rc = gather_host_rows(h, f, idx_dev, n, out, st);
+      if (rc != B2RL_OK) return rc;
+      continue;
+    }
     const int64_t rb = h->field_bytes[f];
     const bool big = rb >= 1024;
     const bool bulk = is_bulk_row(rb) && ((uintptr_t)out % 16 == 0) && ((uintptr_t)h->field[f] % 16 == 0);
@@ -233,6 +238,12 @@ int b2rl::copy_ring_range(b2rl_replay* h, const void* const* fields_src, int64_t
     const uint8_t* src = (const uint8_t*)fields_src[f];
     if (src == nullptr) continue;
     const int64_t rb = h->field_bytes[f];
+    if (h->on_host[f]) {
+      int rc = copy_into_host_field(h, f, start, src, first * rb, st);
+      if (rc == B2RL_OK && first < n) rc = copy_into_host_field(h, f, 0, src + first * rb, (n - first) * rb, st);
+      if (rc != B2RL_OK) return rc;
+      continue;
+    }
     B2RL_CUDA(cudaMemcpyAsync(h->field[f] + start * rb, src, (size_t)(first * rb), cudaMemcpyDefault, st));
     if (first < n)
       B2RL_CUDA(cudaMemcpyAsync(h->field[f], src + first * rb, (size_t)((n - first) * rb), cudaMemcpyDefault, st));
@@ -265,7 +276,9 @@ extern "C" int b2rl_replay_push(b2rl_replay* h, const void* const* fields_src, c
   B2RL_REQUIRE(h->dedup == nullptr, "a frame-deduplicated replay takes its records through b2rl_dedup_push");
   DeviceGuard g(h->device);
   cudaStream_t st = (cudaStream_t)stream;
-  int rc = copy_ring_range(h, fields_src, h->head, n, st);
+  int rc = check_host_sources(h, fields_src);
+  if (rc != B2RL_OK) return rc;
+  rc = copy_ring_range(h, fields_src, h->head, n, st);
   if (rc != B2RL_OK) return rc;
   B2RL_CUDA(cudaMemcpyAsync(h->scratch_val, prios, (size_t)n * sizeof(float), cudaMemcpyDefault, st));
   return publish(h, h->scratch_val, n, st);
@@ -289,6 +302,8 @@ extern "C" int b2rl_replay_copy_payload(b2rl_replay* h, const void* const* field
   B2RL_REQUIRE(h != nullptr && fields_src != nullptr, "null argument");
   B2RL_REQUIRE(n >= 1 && n <= h->capacity && start_slot >= 0 && start_slot < h->capacity, "range out of bounds");
   DeviceGuard g(h->device);
+  const int rc = check_host_sources(h, fields_src);
+  if (rc != B2RL_OK) return rc;
   return copy_ring_range(h, fields_src, start_slot, n, (cudaStream_t)stream);
 }
 
@@ -317,6 +332,10 @@ extern "C" int b2rl_replay_ingest_pipelined(b2rl_replay* h, const void* const* f
   B2RL_REQUIRE(h->dedup == nullptr, "a frame-deduplicated replay takes its records through b2rl_dedup_push");
   DeviceGuard g(h->device);
   cudaStream_t st = (cudaStream_t)stream;
+  {
+    const int rc = check_host_sources(h, fields_src);
+    if (rc != B2RL_OK) return rc;
+  }
   if (h->ingest_stream == nullptr) {
     B2RL_CUDA(cudaStreamCreateWithFlags(&h->ingest_stream, cudaStreamNonBlocking));
     B2RL_CUDA(cudaEventCreateWithFlags(&h->ev_reserved, cudaEventDisableTiming));

@@ -382,9 +382,13 @@ extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot,
   BulkRows P{};
   SmallFields small{};
   SmallRows rows{};
+  int host_f[B2RL_MAX_FIELDS], host_o[B2RL_MAX_FIELDS], n_host = 0;
   for (int f = 0, o = 3; f < h->n_fields; ++f, ++o) {
     const int64_t b = h->field_bytes[f];
-    if (h->dedup != nullptr && f == dedup_planes_field(h)) {   // s and s' stacks assembled from the frame pool
+    if (h->on_host[f]) {         // copied after the draw, from the slot's idx, by the host-row gather (hostrows.cu)
+      host_f[n_host] = f;
+      host_o[n_host++] = o;
+    } else if (h->dedup != nullptr && f == dedup_planes_field(h)) {   // s and s' stacks assembled from the frame pool
       const int32_t* planes = (const int32_t*)h->field[f];
       P.add_planes(dedup_pool(h), planes, 0, (uint8_t*)ptrs[o]);
       P.add_planes(dedup_pool(h), planes, 4, (uint8_t*)ptrs[++o]);
@@ -412,6 +416,10 @@ extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot,
       (float*)ptrs[2], (uint64_t*)ptrs[0], seq, r->done_ticket);
   count_launch();
   B2RL_CHECK_LAUNCH();
+  for (int i = 0; i < n_host; ++i) {
+    rc = gather_host_rows(h, host_f[i], (const int64_t*)ptrs[1], n, (uint8_t*)ptrs[host_o[i]], (cudaStream_t)stream);
+    if (rc != B2RL_OK) return rc;
+  }
   return B2RL_OK;
 }
 
@@ -422,6 +430,7 @@ extern "C" int b2rl_serve_fill_uniform(b2rl_replay* h, b2rl_serve_ring* r, int32
   if (rc != B2RL_OK) return rc;
   B2RL_REQUIRE(steps >= 1, "steps must be >= 1");
   B2RL_REQUIRE(h->dedup == nullptr, "a frame-deduplicated replay holds Ape-X transitions, not rollouts");
+  B2RL_REQUIRE(!h->any_on_host, "a replay with fields placed on the host serves prioritized minibatches only");
   const int64_t n = r->L.batch, size = h->size, cap = h->capacity;
   B2RL_REQUIRE(n <= size, "sample larger than population: the batch exceeds the stored records");
   B2RL_REQUIRE(size <= (1LL << 32), "a uniform fill draws from at most 2^32 records");

@@ -69,6 +69,15 @@ class R2D2Config:
     FRAME_STRIP: bool = False    # store each sequence's T + 3 distinct frames instead of its T stacks (3.83x fewer
                                  # bytes per sequence at T = 80); conv_1 reads stack t as frames t .. t + 3 in place.
                                  # Only records whose stacks slide (every one R2D2/Player.py sends) can be stored.
+    HOST_FRAMES: bool = False    # keep the replay's `state` field (the frames: 99.2 % of a strip sequence's bytes) in
+                                 # pinned host memory; the small fields and the sum-tree stay in HBM.  Each step copies
+                                 # the sampled sequences' frames over PCIe into a device staging buffer (DESIGN §4.17).
+                                 # Replaces PAYLOAD_POOL as the way to a replay larger than HBM, with real ingest.
+
+    def __post_init__(self):
+        if self.HOST_FRAMES and self.PAYLOAD_POOL:
+            raise ValueError("HOST_FRAMES stores every sequence's frames in host memory and replaces the PAYLOAD_POOL "
+                             "benchmark stand-in: set PAYLOAD_POOL = 0 with HOST_FRAMES")
 
     @staticmethod
     def from_configuration():
@@ -77,7 +86,7 @@ class R2D2Config:
                  "USE_RESCALING", "REPLAY_MEMORY_LEN", "BUFFER_SIZE", "TARGET_FREQUENCY", "LEARNER_DEVICE",
                  "REDIS_SERVER", "OPTIM_INFO", "MODEL")
         return R2D2Config(LOG_W=getattr(C, "LOG_W", None), FRAME_STRIP=bool(getattr(C, "FRAME_STRIP", False)),
-                          **{k: getattr(C, k) for k in names})
+                          HOST_FRAMES=bool(getattr(C, "HOST_FRAMES", False)), **{k: getattr(C, k) for k in names})
 
 
 class Replay(ReplayThread):
@@ -91,7 +100,8 @@ class Replay(ReplayThread):
             self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, (), self.device)          # priorities only
             self.pool = R.DeviceReplay(self.cfg.PAYLOAD_POOL, fields, self.device)           # the stored sequences
         else:
-            self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, fields, self.device)
+            self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, fields, self.device,
+                                        host_fields=("state",) if self.cfg.HOST_FRAMES else ())
             self.pool = self.store
         self.memory = MemoryView(self.store, self.cfg.BETA)
 
@@ -260,7 +270,10 @@ class Learner(TargetNetLearner):
         backward, clip + Adam, priority write-back.  No host round trip (R2D2/Learner.py:235-274 in one call).
         `use_graph`: the first call runs three eager warm-ups and captures the step as a CUDA graph (under the
         replay's lock, so that no ingest work lands in the capture); every later call replays it.  The draw reads
-        the tree's device-resident size and Philox counter, so each replay draws a new minibatch."""
+        the tree's device-resident size and Philox counter, so each replay draws a new minibatch.
+        With HOST_FRAMES the frames are not in HBM: the same gather launch sequence also copies the sampled sequences'
+        `state` rows from host memory into a fixed device staging buffer, and conv_1 reads that buffer with the rows
+        train() uses on a staged batch (row = b * pitch + t)."""
         if self._graph is not None:
             self._graph.replay()
             return self._static
@@ -272,7 +285,12 @@ class Learner(TargetNetLearner):
         st, pool = mem.store, mem.pool
         if not hasattr(self, "_small"):
             self._small = pool.alloc_batch(B, ("action", "reward", "h0", "h1", "notdone"))
-            if c.FRAME_STRIP:
+            if c.HOST_FRAMES:
+                self._small.update(pool.alloc_batch(B, ("state",)))    # the staging buffer: B sequences' frames
+                staged = self._small["state"]
+                self._frames = R.strip_windows(staged) if c.FRAME_STRIP else staged.view(-1, 4, 84, 84)
+                self._pitch = T + 3 if c.FRAME_STRIP else T
+            elif c.FRAME_STRIP:
                 self._frames, self._pitch = R.strip_windows(pool.field_view("state")), T + 3
             else:
                 self._frames, self._pitch = pool.field_view("state").view(-1, 4, 84, 84), T
@@ -284,7 +302,9 @@ class Learner(TargetNetLearner):
             h0, h1 = b["h0"].unsqueeze(0), b["h1"].unsqueeze(0)
             self.model.setCellState((h0, h1))
             self.target_model.setCellState((h0, h1))
-            q, q_target = self._forward_fused(self._frames, self._time_major_rows(rows, T, B, self._pitch), T, MEM, B, A)
+            seq_rows = None if c.HOST_FRAMES else rows          # staged: sequence b's frames start at row b * pitch
+            q, q_target = self._forward_fused(self._frames, self._time_major_rows(seq_rows, T, B, self._pitch), T, MEM,
+                                              B, A)
             out, info = self._learn(q, q_target, b["action"], b["reward"], b["notdone"], w)
             st.update(idx, out["prio"])
             return {"scalars": out["scalars"], "p_norm": info["p_norm"], "prio": out["prio"], "idx": idx}

@@ -14,7 +14,7 @@ from typing import Sequence
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, hostmem
 from ._lib import ReplayDesc, check
 
 FRAME_STACK_BYTES = 4 * 84 * 84  # one (4,84,84) uint8 observation, 28 224 B
@@ -169,6 +169,14 @@ class _CudaView:
         self._owner = owner
 
 
+class _HostView:
+    """Expose library-owned pinned host memory to numpy (and so to a CPU torch tensor) via __array_interface__."""
+
+    def __init__(self, ptr: int, shape, typestr: str, owner):
+        self.__array_interface__ = {"shape": tuple(shape), "typestr": typestr, "data": (ptr, False), "version": 3}
+        self._owner = owner
+
+
 _TYPESTR = {torch.uint8: "|u1", torch.int32: "<i4", torch.int64: "<i8", torch.float32: "<f4",
             torch.float64: "<f8", torch.int8: "|i1", torch.int16: "<i2", torch.float16: "<f2"}
 
@@ -181,7 +189,14 @@ def alloc_rows(fields: Sequence[Field], n: int, device, names: Sequence[str] | N
 
 
 class DeviceReplay:
-    def __init__(self, capacity: int, fields: Sequence[Field] = APEX_FIELDS, device="cuda:0"):
+    """`host_fields`: names of fields whose rows live in pinned, mapped host memory owned by the library
+    (b2rl_replay_create_placed) instead of HBM: R2D2's `state`, which a step reads only for its sampled sequences.
+    Their rows must be a multiple of 16 bytes.  gather() copies the sampled rows into device memory over PCIe,
+    field_view() of such a field is a CPU tensor over the pinned rows, and conv1_fused / conv1_wgrad do not read them
+    in place."""
+
+    def __init__(self, capacity: int, fields: Sequence[Field] = APEX_FIELDS, device="cuda:0",
+                 host_fields: Sequence[str] = ()):
         self.lib = _lib.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -198,11 +213,21 @@ class DeviceReplay:
         d.device = self.device.index
         for i, f in enumerate(self.fields):
             d.field_bytes[i] = f.nbytes
+        names = [f.name for f in self.fields]
+        unknown = set(host_fields) - set(names)
+        if unknown:
+            raise ValueError(f"host_fields names fields this replay does not have: {sorted(unknown)}")
+        self.host_fields = frozenset(host_fields)
+        on_host = (C.c_int32 * _lib.MAX_FIELDS)(*[int(n in self.host_fields) for n in names])
         torch.cuda.init()
         with torch.cuda.device(self.device):
             torch.zeros(1, device=self.device)  # make sure the primary context exists
         h = C.c_void_p()
-        check(self.lib.b2rl_replay_create(C.byref(d), C.byref(h)))
+        if self.host_fields:
+            with hostmem.on_gpu_node(self.device):   # pinned pages on the GPU's NUMA node (first touch: the library)
+                check(self.lib.b2rl_replay_create_placed(C.byref(d), on_host, C.byref(h)))
+        else:
+            check(self.lib.b2rl_replay_create(C.byref(d), C.byref(h)))
         self._h = h
 
     # -- bookkeeping -----------------------------------------------------------
@@ -233,11 +258,15 @@ class DeviceReplay:
         return _stream_ptr(self.device)
 
     def field_view(self, name_or_idx) -> torch.Tensor:
-        """Zero-copy torch view (capacity, *shape) of a library-owned payload field."""
+        """Zero-copy torch view (capacity, *shape) of a library-owned payload field: a CUDA tensor, or for a host
+        field a CPU tensor over its pinned rows (torch never treats host memory as device memory)."""
         i = name_or_idx if isinstance(name_or_idx, int) else [f.name for f in self.fields].index(name_or_idx)
         f = self.fields[i]
         p = C.c_void_p()
         check(self.lib.b2rl_replay_field_ptr(self._h, i, C.byref(p)))
+        if f.name in self.host_fields:
+            return torch.from_numpy(np.asarray(_HostView(p.value, (self.capacity,) + tuple(f.shape),
+                                                         _TYPESTR[f.dtype], self)))
         view = _CudaView(p.value, (self.capacity,) + tuple(f.shape), _TYPESTR[f.dtype], self)
         with torch.cuda.device(self.device):
             return torch.as_tensor(view, device=self.device)
@@ -256,6 +285,10 @@ class DeviceReplay:
             if t.dtype != f.dtype:
                 t = t.to(f.dtype)
             t = t.contiguous()
+            if f.name in self.host_fields and not t.is_cuda and not t.is_pinned():
+                # A host field is written in stream order (a host-to-host copy would not be): pageable rows are
+                # staged in device memory on this stream, whose allocator reuses the staging in stream order.
+                t = t.to(self.device)
             if n is None:
                 n = t.shape[0]
             assert t.shape[0] == n and t.numel() * t.element_size() == n * f.nbytes, f"bad shape for {f.name}"
@@ -686,6 +719,9 @@ def _frame_source(frames) -> _lib.Frames:
                            rows=frames.planes.shape[0])
     if isinstance(frames, BoundFrames):
         return _lib.Frames(table=frames.entry_ptr(), row_stride=frames.row_stride, rows=frames.rows)
+    if frames.device.type != "cuda":
+        raise ValueError("conv_1 reads its frame rows in place on the GPU: a frame source in host memory (a host "
+                         "field's view) must be gathered into device memory first")
     assert frames.dtype == torch.uint8 and frames[0].is_contiguous() and frames[0].numel() == FRAME_STACK_BYTES
     stride = frames.stride(0) if frames.shape[0] > 1 else FRAME_STACK_BYTES   # a size-1 dimension's stride is arbitrary
     return _lib.Frames(base=frames.data_ptr(), row_stride=stride * frames.element_size(), rows=frames.shape[0])

@@ -25,6 +25,7 @@ elif ALG == "R2D2":
     MEM = DATA["MEM"]
     USE_RESCALING = DATA["USE_RESCALING"]
     FRAME_STRIP = bool(DATA.get("FRAME_STRIP", False))   # not a reference key: store sequences as frame strips
+    HOST_FRAMES = bool(DATA.get("HOST_FRAMES", False))   # not a reference key: keep the frames in pinned host memory
 elif ALG == "IMPALA":
     C_LAMBDA = DATA["C_LAMBDA"]
     C_VALUE = DATA["C_VALUE"]

@@ -59,12 +59,30 @@ int b2rl_version(void);
 int b2rl_replay_create(const b2rl_replay_desc* desc, b2rl_replay** out);
 int b2rl_replay_destroy(b2rl_replay* h);
 
+/* PER.__init__ (baseline/PER.py:49-66) with each field placed where it is read from: on_host[f] != 0 puts field f in
+ * pinned, mapped host memory owned by the handle (cudaHostAlloc with cudaHostAllocMapped | cudaHostAllocPortable;
+ * the kernels address it through cudaHostGetDevicePointer), every other field and the sum-tree in device memory.
+ * Meant for the frames of R2D2 sequences (R2D2/ReplayMemory.py:70-88), which a step reads only for the sampled
+ * sequences.  A host field's row must be a whole number of 16-byte units.  B2RL_ERR_NOMEM, with the size in the
+ * message, when the pinned allocation fails.  on_host == NULL is b2rl_replay_create.
+ * Host fields are never read by bulk async (TMA) copies: b2rl_replay_gather and b2rl_serve_fill copy their sampled rows
+ * with 16-byte loads through the mapped pointer, from a few CTAs (B2RL_HOST_GATHER_CTAS, default 8).  Every write
+ * into a host field is stream-ordered on the call's stream: push, copy_payload and ingest_pipelined take a host
+ * field's rows from device memory (cudaMemcpyAsync) or from pinned host memory (a copy kernel), and refuse pageable
+ * host memory before any work; fill_hash writes them with its kernel.  b2rl_dedup_attach and b2rl_serve_fill_uniform
+ * refuse a handle with host fields. */
+int b2rl_replay_create_placed(const b2rl_replay_desc* desc, const int32_t* on_host, b2rl_replay** out);
+/* Where field f of PER.memory (baseline/PER.py:7-28) lives: *on_host = 1 for pinned host memory, 0 for device. */
+int b2rl_replay_field_placement(const b2rl_replay* h, int32_t field, int32_t* on_host);
+
 /* PER.__len__ (baseline/PER.py:80-81): number of valid slots, capacity, and
  * the ring head (next slot to be written). Host-side, no sync. */
 int b2rl_replay_size(const b2rl_replay* h, int64_t* size, int64_t* capacity, int64_t* head);
 
 /* Device base pointer of payload field f (capacity x field_bytes[f] bytes): the storage behind
- * PER.memory / Tree.data (baseline/PER.py:7-28), exposed so that consumers (b2rl_conv1_fused) read rows in place. */
+ * PER.memory / Tree.data (baseline/PER.py:7-28), exposed so that consumers (b2rl_conv1_fused) read rows in place.
+ * For a field placed on the host (b2rl_replay_create_placed) it is the HOST address of the pinned rows: never pass
+ * it to b2rl_conv1_fused or b2rl_conv1_wgrad. */
 int b2rl_replay_field_ptr(const b2rl_replay* h, int32_t field, void** ptr_dev);
 
 /* PER.push (baseline/PER.py:69-75) / PrioritizedMemory.push
