@@ -29,9 +29,10 @@ class ServeLayout(C.Structure):
 
 
 class Frames(C.Structure):
-    """b2rl_frames: where conv_1 reads frame row r (include/b2rl.h); exactly one of base, table and pool + planes."""
+    """b2rl_frames: where conv_1 reads frame row r (include/b2rl.h); exactly one of base, table and pool + planes.
+    plane_stride 0 means 8 (the Ape-X plane table)."""
     _fields_ = [("base", c_vp), ("table", c_vp), ("pool", c_vp), ("planes", c_vp), ("row_stride", c_i64),
-                ("rows", c_i64), ("plane_base", c_i32), ("reserved", c_i32)]
+                ("rows", c_i64), ("plane_base", c_i32), ("plane_stride", c_i32)]
 
 
 # name -> (restype, argtypes); must list every symbol include/b2rl.h declares.
@@ -74,6 +75,8 @@ SIGNATURES = {
     "b2rl_conv1_wgrad": (C.c_int, [C.POINTER(Frames), c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp]),
     "b2rl_dedup_attach": (C.c_int, [c_vp, c_i32, c_i64, c_i64, c_u64]),
     "b2rl_dedup_push": (C.c_int, [c_vp, c_vp, c_vp, C.POINTER(c_vp), c_vp, c_i64, c_vp]),
+    "b2rl_dedup_attach_strips": (C.c_int, [c_vp, c_i32, c_i32, c_i64, c_i64, c_u64]),
+    "b2rl_dedup_push_strips": (C.c_int, [c_vp, c_vp, C.POINTER(c_vp), c_vp, c_i64, c_vp]),
     "b2rl_dedup_info": (C.c_int, [c_vp, C.POINTER(c_vp), C.POINTER(c_i64), C.POINTER(c_i64)]),
     "b2rl_replay_gather_planes": (C.c_int, [c_vp, c_vp, c_i64, C.POINTER(c_vp), C.POINTER(c_vp), c_vp]),
     "b2rl_rmsprop_step": (C.c_int, [C.POINTER(c_vp), C.POINTER(c_vp), C.POINTER(c_vp), C.POINTER(c_vp),

@@ -31,8 +31,9 @@ struct BulkField {
   int64_t row_bytes;    // is_bulk_row
   int32_t chunks;       // ceil(row_bytes / CHUNK); time-major: steps * ceil(step_bytes / CHUNK)
   int32_t step_bytes;   // time-major destination only: bytes of one time step of the row (a multiple of 16)
-  const int32_t* planes;   // plane rows only: 8 pool ids per replay row; chunk c of a row is pool frame planes[8 row +
-  int32_t plane_base;      // plane_base + c] (src is the frame pool), so a frame stack is four PLANE_BYTES copies
+  const int32_t* planes;   // plane rows only: chunk c of replay row `row` is pool frame planes[plane_stride row +
+  int32_t plane_base;      // plane_base + c] (src is the frame pool), so a row of k frames is k PLANE_BYTES copies
+  int32_t plane_stride;
 };
 
 struct BulkRows {
@@ -42,22 +43,26 @@ struct BulkRows {
   int32_t pad;
 
   void add(const uint8_t* src, uint8_t* dst, int64_t row_bytes, int chunk) {
-    f[n] = BulkField{src, dst, row_bytes, (int32_t)((row_bytes + chunk - 1) / chunk), 0, nullptr, 0};
+    f[n] = BulkField{src, dst, row_bytes, (int32_t)((row_bytes + chunk - 1) / chunk), 0, nullptr, 0, 0};
     items_per_row += f[n].chunks;
     ++n;
   }
-  // Frame stacks assembled from a frame pool: output row k is planes plane_base .. plane_base + 3 of replay row
-  // row_of(k), one chunk per plane (the copy loop's CHUNK must be at least PLANE_BYTES).
-  void add_planes(const uint8_t* pool, const int32_t* planes, int32_t plane_base, uint8_t* dst) {
-    f[n] = BulkField{pool, dst, 4 * PLANE_BYTES, 4, 0, planes, plane_base};
-    items_per_row += 4;
+  // Rows of k frames assembled from a frame pool: output row k' is the frames of pool ids plane_base .. plane_base +
+  // k - 1 of replay row row_of(k'), whose ids start at planes + stride * row_of(k'); one chunk per frame (the copy
+  // loop's CHUNK must be at least PLANE_BYTES).  Ape-X: k = 4 at stride 8 (s: base 0, s': base 4); R2D2 strip
+  // records: k = stride = T + 3, base 0.
+  void add_planes(const uint8_t* pool, const int32_t* planes, int32_t stride, int32_t plane_base, int32_t k,
+                  uint8_t* dst) {
+    f[n] = BulkField{pool, dst, (int64_t)k * PLANE_BYTES, k, 0, planes, plane_base, stride};
+    items_per_row += k;
     ++n;
   }
   // A row of `steps` time steps whose step t of draw k goes to output row t * batch + k: chunked per step, so no
   // chunk straddles two steps and each one is a single bulk copy with a contiguous destination.
   void add_time_major(const uint8_t* src, uint8_t* dst, int64_t row_bytes, int64_t steps, int chunk) {
     const int64_t step = row_bytes / steps;
-    f[n] = BulkField{src, dst, row_bytes, (int32_t)(steps * ((step + chunk - 1) / chunk)), (int32_t)step, nullptr, 0};
+    f[n] = BulkField{src, dst, row_bytes, (int32_t)(steps * ((step + chunk - 1) / chunk)), (int32_t)step, nullptr, 0,
+                     0};
     items_per_row += f[n].chunks;
     ++n;
   }
@@ -93,7 +98,7 @@ struct ItemCursor {
     }
     if (T.f[f].planes != nullptr) {
       bytes = PLANE_BYTES;
-      src = plane_ptr(T.f[f].src, T.f[f].planes, row, T.f[f].plane_base, c);
+      src = plane_ptr(T.f[f].src, T.f[f].planes, row, T.f[f].plane_stride, T.f[f].plane_base, c);
       dst = T.f[f].dst + (dst_k0 + k) * T.f[f].row_bytes + (int64_t)c * PLANE_BYTES;
       return;
     }

@@ -151,10 +151,11 @@ int gather_host_rows(b2rl_replay* h, int f, const int64_t* idx_dev, int64_t n, u
 // `bytes` from src (device or pinned host memory) into host field f from ring slot `slot` on, in stream order
 // (hostrows.cu).
 int copy_into_host_field(b2rl_replay* h, int f, int64_t slot, const uint8_t* src, int64_t bytes, cudaStream_t st);
-struct DedupState;                       // the frame pool of a deduplicated Ape-X replay (dedup.cu)
+struct DedupState;                       // the frame pool of a deduplicated replay (dedup.cu)
 void dedup_free(b2rl_replay* h);
 int dedup_planes_field(const b2rl_replay* h);
 const uint8_t* dedup_pool(const b2rl_replay* h);
+int dedup_strip_frames(const b2rl_replay* h);     // R of a strip handle (b2rl_dedup_attach_strips), else 0
 }  // namespace b2rl
 
 // The opaque handle.

@@ -1,7 +1,10 @@
-// Frame-deduplicated Ape-X store: ingest (hash -> resolve -> assign + copy) into a frame pool, and the bookkeeping of
-// its eviction rule (include/b2rl.h b2rl_dedup_*, DESIGN.md §4.16).
+// Frame-deduplicated stores: ingest (hash -> resolve -> assign + copy) into a frame pool, and the bookkeeping of
+// its eviction rule (include/b2rl.h b2rl_dedup_*, DESIGN.md §4.16, §4.18).
 //
-// A pushed batch of n records is 8n frames; frame j is plane j % 8 of record j / 8 (planes 0-3 of s, then of s').
+// A pushed batch of n records is R n frames, R frames per record, laid out as the batch's Layout says:
+//   Pairs   Ape-X transitions, R = 8: frame j is plane j % 8 of record j / 8 (planes 0-3 of s, then of s')
+//   Strips  R2D2 frame strips, R = T + 3: frame j is the contiguous strips' frame j, of record j / R
+// and frame j % R of record r gets its pool id in planes[R slot(r) + j % R].
 //   1. k_dedup_hash   one warp per frame: 64-bit content key, inserted into a batch table keyed by it that keeps the
 //                     lowest position holding each key
 //   2. k_dedup_resolve one warp per frame: a frame equal (all 7 056 bytes) to the lowest position with its key reuses
@@ -9,7 +12,7 @@
 //                     that key, and reuses that frame when it lies inside the window and all its bytes are equal
 //   3. k_dedup_scan   the remaining frames (misses) get seq = head, head + 1, ... in batch order (one CTA)
 //   4. the host reads the miss count (one synchronisation), zeroes the priorities of the slots the eviction rule
-//      kills, then k_dedup_copy writes the 8 pool ids of every record, copies the misses into the pool and enters them
+//      kills, then k_dedup_copy writes the R pool ids of every record, copies the misses into the pool and enters them
 //      in the key table; the other fields and the priorities follow as for b2rl_replay_push.
 // Everything a frame's id depends on is a function of the record stream (keys, positions, the window), so the ids
 // can be checked against a CPU model (tests/dedup_model.py).
@@ -29,11 +32,15 @@ constexpr int DD_WORDS = DD_FRAME / 8;            // 882
 constexpr int DD_VEC = DD_FRAME / 16;             // 441
 constexpr unsigned long long DD_EMPTY = ~0ULL;    // key of an unused table entry (keys are below 2^63)
 constexpr unsigned long long DD_KEY_BITS = 0x7FFFFFFFFFFFFFFFULL;
-constexpr int64_t DD_MAX_BATCH = 8192;            // records per push
+constexpr int64_t DD_MAX_FRAMES = 65536;          // frames per push: the batch scratch (8192 Ape-X records)
 constexpr int DD_THREADS = 256;                   // 8 frames per CTA
+
+enum class Layout { Pairs, Strips };
 
 struct DedupState {
   int32_t planes_field = -1;
+  int32_t R = 8;                                  // frames per record
+  Layout layout = Layout::Pairs;
   int64_t F = 0, W = 0, T = 0;                    // pool frames, window, key-table entries (a power of two)
   unsigned long long mask = 0;
   uint8_t* pool = nullptr;                        // [F][7056]
@@ -43,10 +50,10 @@ struct DedupState {
   int64_t used = 0;                               // table entries claimed since the last rebuild, at most
   int64_t head = 0;                               // frames stored so far
   int64_t max_batch = 0;
-  int64_t BT = 0;                                 // batch-table entries (a power of two >= 16 * max_batch)
-  unsigned long long* key = nullptr;              // [8 max_batch] per batch frame
-  int32_t* rep = nullptr;                         // [8 max_batch] position whose frame it reuses (itself if none)
-  int64_t* fseq = nullptr;                        // [8 max_batch] seq (-1 before the scan: a miss)
+  int64_t BT = 0;                                 // batch-table entries (a power of two >= 2 R max_batch)
+  unsigned long long* key = nullptr;              // [R max_batch] per batch frame
+  int32_t* rep = nullptr;                         // [R max_batch] position whose frame it reuses (itself if none)
+  int64_t* fseq = nullptr;                        // [R max_batch] seq (-1 before the scan: a miss)
   unsigned long long* bkey = nullptr;             // [BT]
   int32_t* bpos = nullptr;                        // [BT] lowest batch position holding bkey
   int64_t* misses_dev = nullptr;
@@ -62,8 +69,10 @@ __host__ __device__ __forceinline__ uint64_t mix64(uint64_t z) {   // splitmix64
   return z ^ (z >> 31);
 }
 
-// Frame j of the batch: plane j % 8 of record j / 8.
+// Frame j of the batch.  Pairs: plane j % 8 of record j / 8, from s and ns.  Strips: frame j of the strips s.
+template <Layout L>
 __device__ __forceinline__ const uint8_t* batch_frame(const uint8_t* s, const uint8_t* ns, int64_t j) {
+  if constexpr (L == Layout::Strips) return s + j * DD_FRAME;
   const int64_t r = j >> 3;
   const int c = (int)(j & 7);
   return (c < 4 ? s : ns) + r * DD_STACK + (c & 3) * DD_FRAME;
@@ -104,6 +113,7 @@ __device__ __forceinline__ int64_t find(const unsigned long long* keys, int64_t 
 
 // key = mix64(sum over the frame's 8-byte words w_i of mix64(w_i ^ i * golden)) & mask, without its top bit.  The sum
 // is order-free, so the lanes' partial sums combine in any order.
+template <Layout L>
 __global__ void __launch_bounds__(DD_THREADS)
 k_dedup_hash(const uint8_t* __restrict__ s, const uint8_t* __restrict__ ns, int64_t frames, unsigned long long mask,
              unsigned long long* __restrict__ key, unsigned long long* __restrict__ bkey, int32_t* __restrict__ bpos,
@@ -111,7 +121,7 @@ k_dedup_hash(const uint8_t* __restrict__ s, const uint8_t* __restrict__ ns, int6
   const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (j >= frames) return;
-  const uint64_t* w = reinterpret_cast<const uint64_t*>(batch_frame(s, ns, j));
+  const uint64_t* w = reinterpret_cast<const uint64_t*>(batch_frame<L>(s, ns, j));
   uint64_t h = 0;
   for (int i = lane; i < DD_WORDS; i += 32) h += mix64(w[i] ^ ((uint64_t)i * 0x9E3779B97F4A7C15ULL));
 #pragma unroll
@@ -141,15 +151,16 @@ struct ResolveArgs {
   int64_t* fseq;
 };
 
+template <Layout L>
 __global__ void __launch_bounds__(DD_THREADS)
 k_dedup_resolve(const __grid_constant__ ResolveArgs A) {
   const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (j >= A.frames) return;
   const unsigned long long k = A.key[j];
-  const uint8_t* me = batch_frame(A.s, A.ns, j);
+  const uint8_t* me = batch_frame<L>(A.s, A.ns, j);
   const int32_t first = A.bpos[find(A.bkey, A.BT, k)];
-  if (first < j && warp_equal(batch_frame(A.s, A.ns, first), me, lane)) {
+  if (first < j && warp_equal(batch_frame<L>(A.s, A.ns, first), me, lane)) {
     if (lane == 0) { A.rep[j] = first; A.fseq[j] = -2; }
     return;
   }
@@ -220,8 +231,10 @@ struct CopyArgs {
   int64_t T;
   int32_t* planes;          // the replay's planes field
   int64_t slot0, capacity;  // record r goes to slot (slot0 + r) % capacity
+  int32_t R;                // Strips: frames per record (Pairs: 8)
 };
 
+template <Layout L>
 __global__ void __launch_bounds__(DD_THREADS)
 k_dedup_copy(const __grid_constant__ CopyArgs A) {
   const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
@@ -231,12 +244,14 @@ k_dedup_copy(const __grid_constant__ CopyArgs A) {
   const int64_t sq = A.fseq[r];
   const int64_t ps = sq % A.F;
   if (lane == 0) {
-    int64_t slot = A.slot0 + (j >> 3);
+    const int64_t R = L == Layout::Pairs ? 8 : A.R;
+    const int64_t rec = L == Layout::Pairs ? j >> 3 : j / R;
+    int64_t slot = A.slot0 + rec;
     if (slot >= A.capacity) slot -= A.capacity;
-    A.planes[slot * 8 + (j & 7)] = (int32_t)ps;
+    A.planes[slot * R + (j - rec * R)] = (int32_t)ps;
   }
   if (r != j || sq < A.head) return;        // a batch duplicate or a hit: nothing to store
-  const uint4* src = reinterpret_cast<const uint4*>(batch_frame(A.s, A.ns, j));
+  const uint4* src = reinterpret_cast<const uint4*>(batch_frame<L>(A.s, A.ns, j));
   uint4* dst = reinterpret_cast<uint4*>(A.pool + ps * DD_FRAME);
   for (int i = lane; i < DD_VEC; i += 32) dst[i] = src[i];
   if (lane == 0) {
@@ -269,6 +284,7 @@ void dedup_free(b2rl_replay* h) {
 
 int dedup_planes_field(const b2rl_replay* h) { return h->dedup->planes_field; }
 const uint8_t* dedup_pool(const b2rl_replay* h) { return h->dedup->pool; }
+int dedup_strip_frames(const b2rl_replay* h) { return h->dedup->layout == Layout::Strips ? h->dedup->R : 0; }
 
 }  // namespace b2rl
 
@@ -280,30 +296,37 @@ static int64_t pow2_at_least(int64_t x) {
   return p;
 }
 
-extern "C" int b2rl_dedup_attach(b2rl_replay* h, int32_t planes_field, int64_t pool_frames, int64_t window,
-                                 uint64_t hash_mask) {
+// b2rl_dedup_attach (Pairs, R = 8) and b2rl_dedup_attach_strips (Strips, R = frames_per_record).
+static int dedup_attach(b2rl_replay* h, int32_t planes_field, Layout layout, int32_t R, int64_t pool_frames,
+                        int64_t window, uint64_t hash_mask) {
   B2RL_REQUIRE(h != nullptr, "null handle");
   B2RL_REQUIRE(h->dedup == nullptr, "the replay already has a frame pool");
   B2RL_REQUIRE(!h->any_on_host, "a replay with fields placed on the host cannot take a frame pool");
   B2RL_REQUIRE(h->size == 0 && h->head == 0 && h->reserved == 0 && h->pipe_n == 0, "the replay must be empty");
-  B2RL_REQUIRE(planes_field >= 0 && planes_field < h->n_fields && h->field_bytes[planes_field] == 32,
-               "the planes field must hold 8 int32 per slot");
-  B2RL_REQUIRE(window >= 0 && pool_frames - window > 8, "need window >= 0 and pool_frames - window > 8");
+  B2RL_REQUIRE(R >= 4 && R <= DD_MAX_FRAMES, "frames_per_record must be in [4, 65536]");
+  B2RL_REQUIRE(planes_field >= 0 && planes_field < h->n_fields && h->field_bytes[planes_field] == 4 * (int64_t)R,
+               layout == Layout::Pairs ? "the planes field must hold 8 int32 per slot"
+                                       : "the planes field must hold frames_per_record int32 per slot");
+  B2RL_REQUIRE(window >= 0 && pool_frames - window > R,
+               layout == Layout::Pairs ? "need window >= 0 and pool_frames - window > 8"
+                                       : "need window >= 0 and pool_frames - window > frames_per_record");
   B2RL_REQUIRE(pool_frames < (1LL << 31), "pool_frames must be below 2^31");
   DeviceGuard g(h->device);
   DedupState* d = new (std::nothrow) DedupState();
   if (!d) { set_error("out of host memory"); return B2RL_ERR_NOMEM; }
   h->dedup = d;
   d->planes_field = planes_field;
+  d->R = R;
+  d->layout = layout;
   d->F = pool_frames;
   d->W = window;
   d->mask = (unsigned long long)hash_mask;
-  d->max_batch = (pool_frames - window - 1) / 8;
-  if (d->max_batch > DD_MAX_BATCH) d->max_batch = DD_MAX_BATCH;
+  d->max_batch = (pool_frames - window - 1) / R;
+  if (d->max_batch > DD_MAX_FRAMES / R) d->max_batch = DD_MAX_FRAMES / R;
   if (d->max_batch > h->capacity) d->max_batch = h->capacity;
-  d->T = pow2_at_least(2 * (window + 8 * d->max_batch));   // at most half claimed: window + one batch
-  d->BT = pow2_at_least(16 * d->max_batch);
-  const int64_t nf = 8 * d->max_batch;
+  const int64_t nf = R * d->max_batch;
+  d->T = pow2_at_least(2 * (window + nf));   // at most half claimed: window + one batch
+  d->BT = pow2_at_least(2 * nf);
   cudaError_t e = cudaSuccess;
   auto alloc = [&](void** p, size_t bytes) {
     if (e == cudaSuccess) e = cudaMalloc(p, bytes);
@@ -322,7 +345,7 @@ extern "C" int b2rl_dedup_attach(b2rl_replay* h, int32_t planes_field, int64_t p
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&d->done, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaMemset(d->tkey, 0xFF, sizeof(unsigned long long) * (size_t)d->T);
   if (e == cudaSuccess) e = cudaMemset(d->tseq, 0, sizeof(unsigned long long) * (size_t)d->T);
-  if (e == cudaSuccess) e = cudaMemset(h->field[planes_field], 0, (size_t)h->capacity * 32);
+  if (e == cudaSuccess) e = cudaMemset(h->field[planes_field], 0, (size_t)h->capacity * 4 * R);
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
     set_error("allocating a %lld-frame pool failed: %s", (long long)pool_frames, cudaGetErrorString(e));
@@ -340,6 +363,16 @@ extern "C" int b2rl_dedup_attach(b2rl_replay* h, int32_t planes_field, int64_t p
   return B2RL_OK;
 }
 
+extern "C" int b2rl_dedup_attach(b2rl_replay* h, int32_t planes_field, int64_t pool_frames, int64_t window,
+                                 uint64_t hash_mask) {
+  return dedup_attach(h, planes_field, Layout::Pairs, 8, pool_frames, window, hash_mask);
+}
+
+extern "C" int b2rl_dedup_attach_strips(b2rl_replay* h, int32_t planes_field, int32_t frames_per_record,
+                                        int64_t pool_frames, int64_t window, uint64_t hash_mask) {
+  return dedup_attach(h, planes_field, Layout::Strips, frames_per_record, pool_frames, window, hash_mask);
+}
+
 extern "C" int b2rl_dedup_info(const b2rl_replay* h, void** pool_dev, int64_t* head_seq, int64_t* max_batch) {
   B2RL_REQUIRE(h != nullptr, "null handle");
   B2RL_REQUIRE(h->dedup != nullptr, "not a frame-deduplicated replay (b2rl_dedup_attach)");
@@ -351,20 +384,16 @@ extern "C" int b2rl_dedup_info(const b2rl_replay* h, void** pool_dev, int64_t* h
 
 static unsigned warps_grid(int64_t frames) { return (unsigned)((frames * 32 + DD_THREADS - 1) / DD_THREADS); }
 
-extern "C" int b2rl_dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8_t* ns_dev,
-                               const void* const* fields_src, const float* prios, int64_t n, void* stream) {
-  B2RL_REQUIRE(h != nullptr, "null handle");
+// The push of n records whose frames the layout L places (the caller has checked the frame pointers).
+template <Layout L>
+static int dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8_t* ns_dev, const void* const* fields_src,
+                      const float* prios, int64_t n, cudaStream_t st) {
   DedupState* d = h->dedup;
-  B2RL_REQUIRE(d != nullptr, "not a frame-deduplicated replay (b2rl_dedup_attach)");
-  B2RL_REQUIRE(n >= 0 && n <= d->max_batch, "n out of range (0..max_batch of b2rl_dedup_info)");
-  if (n == 0) return B2RL_OK;
-  B2RL_REQUIRE(s_dev != nullptr && ns_dev != nullptr && prios != nullptr && fields_src != nullptr, "null argument");
-  B2RL_REQUIRE((uintptr_t)s_dev % 16 == 0 && (uintptr_t)ns_dev % 16 == 0, "frame stacks must be 16-byte aligned");
+  B2RL_REQUIRE(prios != nullptr && fields_src != nullptr, "null argument");
   B2RL_REQUIRE(fields_src[d->planes_field] == nullptr, "the planes field is written by the push itself");
   B2RL_REQUIRE(h->reserved == 0, "a reservation is pending");
   DeviceGuard g(h->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t frames = 8 * n;
+  const int64_t frames = d->R * n;
   const int64_t head = d->head;
   B2RL_CUDA(cudaStreamWaitEvent(st, d->done, 0));     // the previous push (on any stream) is done with the scratch
   // 1. the key table: rebuilt from the window when this batch could take it past half full
@@ -382,11 +411,11 @@ extern "C" int b2rl_dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8
   // 2. keys, batch duplicates, hits, and the misses' seqs
   B2RL_CUDA(cudaMemsetAsync(d->bkey, 0xFF, sizeof(unsigned long long) * (size_t)d->BT, st));
   B2RL_CUDA(cudaMemsetAsync(d->bpos, 0x7F, sizeof(int32_t) * (size_t)d->BT, st));
-  k_dedup_hash<<<warps_grid(frames), DD_THREADS, 0, st>>>(s_dev, ns_dev, frames, d->mask, d->key, d->bkey, d->bpos,
+  k_dedup_hash<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(s_dev, ns_dev, frames, d->mask, d->key, d->bkey, d->bpos,
                                                           d->BT);
   ResolveArgs A{s_dev, ns_dev, frames, d->key, d->bkey, d->bpos, d->BT, d->tkey, d->tseq, d->T, d->pool, d->F,
                 head - d->W, d->rep, d->fseq};
-  k_dedup_resolve<<<warps_grid(frames), DD_THREADS, 0, st>>>(A);
+  k_dedup_resolve<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(A);
   k_dedup_scan<<<1, 1024, 0, st>>>(d->fseq, frames, head, d->misses_dev);
   count_launch(3);
   B2RL_CHECK_LAUNCH();
@@ -406,8 +435,8 @@ extern "C" int b2rl_dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8
   }
   // 4. pool ids, new frames, key table; then the other fields and the priorities as b2rl_replay_push does
   CopyArgs C{s_dev, ns_dev, frames, d->key, d->rep, d->fseq, head, d->pool, d->pool_key, d->F, d->tkey, d->tseq, d->T,
-             (int32_t*)h->field[d->planes_field], h->head, h->capacity};
-  k_dedup_copy<<<warps_grid(frames), DD_THREADS, 0, st>>>(C);
+             (int32_t*)h->field[d->planes_field], h->head, h->capacity, d->R};
+  k_dedup_copy<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(C);
   count_launch();
   B2RL_CHECK_LAUNCH();
   int rc = copy_ring_range(h, fields_src, h->head, n, st);
@@ -420,4 +449,30 @@ extern "C" int b2rl_dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8
   d->head = head_new;
   d->used += head_new - head;
   return B2RL_OK;
+}
+
+extern "C" int b2rl_dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8_t* ns_dev,
+                               const void* const* fields_src, const float* prios, int64_t n, void* stream) {
+  B2RL_REQUIRE(h != nullptr, "null handle");
+  DedupState* d = h->dedup;
+  B2RL_REQUIRE(d != nullptr, "not a frame-deduplicated replay (b2rl_dedup_attach)");
+  B2RL_REQUIRE(d->layout == Layout::Pairs, "a strip handle (b2rl_dedup_attach_strips) takes b2rl_dedup_push_strips");
+  B2RL_REQUIRE(n >= 0 && n <= d->max_batch, "n out of range (0..max_batch of b2rl_dedup_info)");
+  if (n == 0) return B2RL_OK;
+  B2RL_REQUIRE(s_dev != nullptr && ns_dev != nullptr, "null argument");
+  B2RL_REQUIRE((uintptr_t)s_dev % 16 == 0 && (uintptr_t)ns_dev % 16 == 0, "frame stacks must be 16-byte aligned");
+  return dedup_push<Layout::Pairs>(h, s_dev, ns_dev, fields_src, prios, n, (cudaStream_t)stream);
+}
+
+extern "C" int b2rl_dedup_push_strips(b2rl_replay* h, const uint8_t* strips_dev, const void* const* fields_src,
+                                      const float* prios, int64_t n, void* stream) {
+  B2RL_REQUIRE(h != nullptr, "null handle");
+  DedupState* d = h->dedup;
+  B2RL_REQUIRE(d != nullptr, "not a frame-deduplicated replay (b2rl_dedup_attach_strips)");
+  B2RL_REQUIRE(d->layout == Layout::Strips, "an Ape-X handle (b2rl_dedup_attach) takes b2rl_dedup_push");
+  B2RL_REQUIRE(n >= 0 && n <= d->max_batch, "n out of range (0..max_batch of b2rl_dedup_info)");
+  if (n == 0) return B2RL_OK;
+  B2RL_REQUIRE(strips_dev != nullptr, "null argument");
+  B2RL_REQUIRE((uintptr_t)strips_dev % 16 == 0, "frame strips must be 16-byte aligned");
+  return dedup_push<Layout::Strips>(h, strips_dev, nullptr, fields_src, prios, n, (cudaStream_t)stream);
 }

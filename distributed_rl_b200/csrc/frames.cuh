@@ -18,23 +18,24 @@ constexpr int STACK_BYTES = 4 * PLANE_BYTES;  // one row
 enum class FrameKind {
   Direct,   // row r at base + r * row_stride
   Table,    // the same, with the base read from a device-resident entry when the kernel starts
-  Planes,   // channel c of row r is pool frame planes[8 r + plane_base + c]
+  Planes,   // channel c of row r is pool frame planes[plane_stride r + plane_base + c]
 };
 
 struct FrameSource {
   const uint8_t* base;           // Direct: the first row; Planes: the frame pool
   const uint8_t* const* table;   // Table: the entry that holds the first row's address
-  const int32_t* planes;         // Planes: 8 pool ids per row
+  const int32_t* planes;         // Planes: pool ids, plane_stride per row
   int64_t row_stride;            // Direct, Table: bytes between rows
   int64_t table_off;             // Table: bytes added to the entry's address (the rows of earlier split launches)
   int64_t rows;                  // indices are clamped to [0, rows)
-  int32_t plane_base;            // Planes: 0 or 4
+  int32_t plane_base;            // Planes: 0 or 4 at stride 8, 0 at stride 1
+  int32_t plane_stride;          // Planes: 8 (Ape-X s / s') or 1 (the windows of R2D2 strip records)
 };
 
-// Frame c of plane-table row `row`.
+// Frame c of plane-table row `row`: pool ids are `stride` apart from row to row.
 __device__ __forceinline__ const uint8_t* plane_ptr(const uint8_t* pool, const int32_t* planes, int64_t row,
-                                                    int32_t plane_base, int c) {
-  return pool + (int64_t)planes[row * 8 + plane_base + c] * PLANE_BYTES;
+                                                    int32_t stride, int32_t plane_base, int c) {
+  return pool + (int64_t)planes[row * stride + plane_base + c] * PLANE_BYTES;
 }
 
 // The address rows are read from: the base (the pool for Planes), or the table entry's as the kernel starts.
@@ -53,7 +54,7 @@ __device__ __forceinline__ void load_row(const FrameSource& S, const uint8_t* fr
   if constexpr (KIND == FrameKind::Planes) {
 #pragma unroll
     for (int c = 0; c < 4; ++c)
-      sm90::bulk_g2s(dst + c * PLANE_BYTES, plane_ptr(frames, S.planes, row, S.plane_base, c), PLANE_BYTES, bar);
+      sm90::bulk_g2s(dst + c * PLANE_BYTES, plane_ptr(frames, S.planes, row, S.plane_stride, S.plane_base, c), PLANE_BYTES, bar);
   } else {
     sm90::bulk_g2s(dst, frames + row * S.row_stride, STACK_BYTES, bar);
   }
@@ -73,9 +74,12 @@ inline int check_frames(const b2rl_frames* f, FrameSource& src, FrameKind& kind)
     B2RL_REQUIRE(f->pool != nullptr && f->planes != nullptr, "null frame pool or plane table");
     B2RL_REQUIRE((uintptr_t)f->pool % 16 == 0 && (uintptr_t)f->planes % 4 == 0,
                  "the frame pool must be 16-byte aligned, the plane table 4-byte aligned");
-    B2RL_REQUIRE(f->plane_base == 0 || f->plane_base == 4, "plane_base must be 0 or 4");
+    const int32_t stride = f->plane_stride == 0 ? 8 : f->plane_stride;
+    B2RL_REQUIRE(stride == 8 || stride == 1, "plane_stride must be 0 or 8 (Ape-X s / s') or 1 (strip windows)");
+    if (stride == 8) B2RL_REQUIRE(f->plane_base == 0 || f->plane_base == 4, "plane_base must be 0 or 4");
+    else B2RL_REQUIRE(f->plane_base == 0, "plane_base must be 0 at plane_stride 1");
     kind = FrameKind::Planes;
-    src.base = f->pool, src.planes = f->planes, src.plane_base = f->plane_base;
+    src.base = f->pool, src.planes = f->planes, src.plane_base = f->plane_base, src.plane_stride = stride;
     return B2RL_OK;
   }
   B2RL_REQUIRE(f->row_stride > 0 && f->row_stride % 16 == 0, "the row stride must be a positive multiple of 16 bytes");
@@ -90,7 +94,7 @@ inline int check_frames(const b2rl_frames* f, FrameSource& src, FrameKind& kind)
 inline FrameSource advance(FrameSource S, FrameKind kind, int64_t off) {
   if (kind == FrameKind::Direct) S.base += off * S.row_stride;
   else if (kind == FrameKind::Table) S.table_off += off * S.row_stride;
-  else S.planes += 8 * off;
+  else S.planes += S.plane_stride * off;
   S.rows -= off;
   return S;
 }

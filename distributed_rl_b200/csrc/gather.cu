@@ -130,7 +130,8 @@ static int gather_mode() {
 }
 
 // b2rl_replay_gather, and for a dedup replay b2rl_replay_gather_planes: stacks_out (2 entries, or nullptr) receives
-// the frame stacks of planes 0-3 / 4-7, copied as plane rows by the same launch.
+// the frame stacks of planes 0-3 / 4-7 (Ape-X), or in its first entry the R-frame strips of a strip handle, copied
+// as plane rows by the same launch.
 static int gather_run(b2rl_replay* h, const int64_t* idx_dev, int64_t n, void* const* stacks_out,
                       void* const* out_fields_dev, cudaStream_t st) {
   GatherParams P{};
@@ -138,9 +139,16 @@ static int gather_run(b2rl_replay* h, const int64_t* idx_dev, int64_t n, void* c
   P.capacity = h->capacity;
   if (stacks_out != nullptr) {
     const int32_t* planes = (const int32_t*)h->field[dedup_planes_field(h)];
-    for (int i = 0; i < 2; ++i) {
-      B2RL_REQUIRE((uintptr_t)stacks_out[i] % 16 == 0, "frame stack outputs must be 16-byte aligned");
-      if (stacks_out[i] != nullptr) P.bulk.add_planes(dedup_pool(h), planes, 4 * i, (uint8_t*)stacks_out[i]);
+    const int R = dedup_strip_frames(h);
+    if (R > 0) {
+      B2RL_REQUIRE(stacks_out[1] == nullptr, "a strip handle has one frame output: stacks_out_dev[1] must be NULL");
+      B2RL_REQUIRE((uintptr_t)stacks_out[0] % 16 == 0, "frame strip outputs must be 16-byte aligned");
+      if (stacks_out[0] != nullptr) P.bulk.add_planes(dedup_pool(h), planes, R, 0, R, (uint8_t*)stacks_out[0]);
+    } else {
+      for (int i = 0; i < 2; ++i) {
+        B2RL_REQUIRE((uintptr_t)stacks_out[i] % 16 == 0, "frame stack outputs must be 16-byte aligned");
+        if (stacks_out[i] != nullptr) P.bulk.add_planes(dedup_pool(h), planes, 8, 4 * i, 4, (uint8_t*)stacks_out[i]);
+      }
     }
   }
   for (int f = 0; f < h->n_fields; ++f) {

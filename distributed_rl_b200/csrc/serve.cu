@@ -219,11 +219,14 @@ extern "C" int b2rl_serve_layout_init(int64_t batch, int32_t slots, int32_t n_fi
 }
 
 // The fields a ring slot carries for replay h: its own fields, except that a frame-deduplicated replay's planes field
-// becomes two frame stacks (planes 0-3, then 4-7), so the slot holds the stack store's record layout.  -> count.
+// becomes two frame stacks (planes 0-3, then 4-7), so the slot holds the stack store's record layout; a strip
+// handle's becomes the R-frame strip field, so the slot holds the strip store's.  -> count.
 static int served_fields(const b2rl_replay* h, int64_t* bytes) {
   int n = 0;
   for (int f = 0; f < h->n_fields; ++f) {
-    if (h->dedup != nullptr && f == dedup_planes_field(h)) {
+    if (h->dedup != nullptr && f == dedup_planes_field(h) && dedup_strip_frames(h) > 0) {
+      bytes[n++] = (int64_t)dedup_strip_frames(h) * PLANE_BYTES;
+    } else if (h->dedup != nullptr && f == dedup_planes_field(h)) {
       bytes[n++] = 4 * PLANE_BYTES;
       bytes[n++] = 4 * PLANE_BYTES;
     } else {
@@ -388,10 +391,15 @@ extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot,
     if (h->on_host[f]) {         // copied after the draw, from the slot's idx, by the host-row gather (hostrows.cu)
       host_f[n_host] = f;
       host_o[n_host++] = o;
-    } else if (h->dedup != nullptr && f == dedup_planes_field(h)) {   // s and s' stacks assembled from the frame pool
+    } else if (h->dedup != nullptr && f == dedup_planes_field(h)) {   // frames assembled from the frame pool
       const int32_t* planes = (const int32_t*)h->field[f];
-      P.add_planes(dedup_pool(h), planes, 0, (uint8_t*)ptrs[o]);
-      P.add_planes(dedup_pool(h), planes, 4, (uint8_t*)ptrs[++o]);
+      const int R = dedup_strip_frames(h);
+      if (R > 0) {                                                     // the strips
+        P.add_planes(dedup_pool(h), planes, R, 0, R, (uint8_t*)ptrs[o]);
+      } else {                                                         // the s and s' stacks
+        P.add_planes(dedup_pool(h), planes, 8, 0, 4, (uint8_t*)ptrs[o]);
+        P.add_planes(dedup_pool(h), planes, 8, 4, 4, (uint8_t*)ptrs[++o]);
+      }
     } else if (is_bulk_row(b)) {
       P.add(h->field[f], (uint8_t*)ptrs[o], b, 14336);   // the CHUNK of k_serve_fill's copy_rows
     } else if (b == 1 || b == 2 || b == 4 || b == 8) {
@@ -429,7 +437,7 @@ extern "C" int b2rl_serve_fill_uniform(b2rl_replay* h, b2rl_serve_ring* r, int32
   int rc = fill_slot_ptrs(h, r, slot, ptrs);
   if (rc != B2RL_OK) return rc;
   B2RL_REQUIRE(steps >= 1, "steps must be >= 1");
-  B2RL_REQUIRE(h->dedup == nullptr, "a frame-deduplicated replay holds Ape-X transitions, not rollouts");
+  B2RL_REQUIRE(h->dedup == nullptr, "a frame-deduplicated replay serves prioritized minibatches, not rollouts");
   B2RL_REQUIRE(!h->any_on_host, "a replay with fields placed on the host serves prioritized minibatches only");
   const int64_t n = r->L.batch, size = h->size, cap = h->capacity;
   B2RL_REQUIRE(n <= size, "sample larger than population: the batch exceeds the stored records");

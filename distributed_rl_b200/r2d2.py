@@ -73,11 +73,23 @@ class R2D2Config:
                                  # pinned host memory; the small fields and the sum-tree stay in HBM.  Each step copies
                                  # the sampled sequences' frames over PCIe into a device staging buffer (DESIGN §4.17).
                                  # Replaces PAYLOAD_POOL as the way to a replay larger than HBM, with real ingest.
+    FRAME_DEDUP: bool = False    # store every distinct frame once, in a pool of FRAMES_PER_SEQUENCE frames per slot
+                                 # (R.StripDedupReplay, DESIGN §4.18): the half-overlapping sequences an actor sends
+                                 # share their frames.  Records are frame strips (FRAME_STRIP is set with it), and the
+                                 # samples are a strip store's.
+    FRAMES_PER_SEQUENCE: float = 48.0
+    DEDUP_WINDOW: int = 1 << 14  # a frame is reused only from the last DEDUP_WINDOW frames stored (at most 1/8 of the
+                                 # pool, see dedup_geometry)
 
     def __post_init__(self):
         if self.HOST_FRAMES and self.PAYLOAD_POOL:
             raise ValueError("HOST_FRAMES stores every sequence's frames in host memory and replaces the PAYLOAD_POOL "
                              "benchmark stand-in: set PAYLOAD_POOL = 0 with HOST_FRAMES")
+        if self.FRAME_DEDUP and (self.HOST_FRAMES or self.PAYLOAD_POOL):
+            raise ValueError("FRAME_DEDUP keeps its frame pool in HBM and stores every pushed sequence: it takes "
+                             "neither HOST_FRAMES nor PAYLOAD_POOL")
+        if self.FRAME_DEDUP:
+            self.FRAME_STRIP = True
 
     @staticmethod
     def from_configuration():
@@ -85,8 +97,28 @@ class R2D2Config:
         names = ("BATCHSIZE", "ACTION_SIZE", "ALPHA", "BETA", "GAMMA", "UNROLL_STEP", "FIXED_TRAJECTORY", "MEM",
                  "USE_RESCALING", "REPLAY_MEMORY_LEN", "BUFFER_SIZE", "TARGET_FREQUENCY", "LEARNER_DEVICE",
                  "REDIS_SERVER", "OPTIM_INFO", "MODEL")
+        kw = {k: getattr(C, k) for k in names}
+        for k in ("FRAME_DEDUP", "FRAMES_PER_SEQUENCE", "DEDUP_WINDOW"):     # optional keys of cfg/r2d2.json
+            if hasattr(C, k):
+                kw[k] = getattr(C, k)
         return R2D2Config(LOG_W=getattr(C, "LOG_W", None), FRAME_STRIP=bool(getattr(C, "FRAME_STRIP", False)),
-                          HOST_FRAMES=bool(getattr(C, "HOST_FRAMES", False)), **{k: getattr(C, k) for k in names})
+                          HOST_FRAMES=bool(getattr(C, "HOST_FRAMES", False)), **kw)
+
+
+def dedup_geometry(cfg: R2D2Config) -> tuple:
+    """(pool frames, window) of a FRAME_DEDUP replay: ceil(FRAMES_PER_SEQUENCE * REPLAY_MEMORY_LEN) frames, and
+    DEDUP_WINDOW capped at an eighth of them (as apex.dedup_geometry).  A slot stays live until pool - window frames
+    have been stored after it: at the default 48 frames per slot, 42 REPLAY_MEMORY_LEN frames or more, above the
+    ~40 new frames per sequence the reference actors send (T / 2 in mid-episode), so the slot ring wraps first.  The
+    window only has to reach back to the same actor's previous sequence."""
+    import math
+    import warnings
+    F = int(math.ceil(cfg.FRAMES_PER_SEQUENCE * cfg.REPLAY_MEMORY_LEN))
+    W = min(int(cfg.DEDUP_WINDOW), F // 8)
+    if W < cfg.DEDUP_WINDOW:
+        warnings.warn(f"DEDUP_WINDOW = {cfg.DEDUP_WINDOW} frames is more than an eighth of the {F}-frame pool: the "
+                      f"frame-deduplicated replay uses a window of {W} frames", stacklevel=2)
+    return F, W
 
 
 class Replay(ReplayThread):
@@ -99,6 +131,9 @@ class Replay(ReplayThread):
         if self.cfg.PAYLOAD_POOL:
             self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, (), self.device)          # priorities only
             self.pool = R.DeviceReplay(self.cfg.PAYLOAD_POOL, fields, self.device)           # the stored sequences
+        elif self.cfg.FRAME_DEDUP:
+            self.store = self.pool = R.StripDedupReplay(self.cfg.REPLAY_MEMORY_LEN, *dedup_geometry(self.cfg),
+                                                        T=self.cfg.FIXED_TRAJECTORY, device=self.device)
         else:
             self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, fields, self.device,
                                         host_fields=("state",) if self.cfg.HOST_FRAMES else ())
@@ -106,9 +141,9 @@ class Replay(ReplayThread):
         self.memory = MemoryView(self.store, self.cfg.BETA)
 
     def push_arrays(self, s, a, r, h0, h1, notdone, p):
-        """`s`: (n, T, 4, 84, 84) stacks or, with FRAME_STRIP, (n, T + 3, 84, 84) strips.  With FRAME_STRIP, stacks are
-        encoded into strips first (R.encode_strips): a record whose stacks do not slide raises ValueError naming it,
-        and nothing of the batch is pushed."""
+        """`s`: (n, T, 4, 84, 84) stacks or, with FRAME_STRIP (and so FRAME_DEDUP), (n, T + 3, 84, 84) strips.  With
+        FRAME_STRIP, stacks are encoded into strips first (R.encode_strips): a record whose stacks do not slide raises
+        ValueError naming it, and nothing of the batch is pushed."""
         if self.cfg.FRAME_STRIP and tuple(s.shape[1:]) != (self.cfg.FIXED_TRAJECTORY + 3, 84, 84):
             s = R.encode_strips(s)
         with self._lock:
@@ -271,7 +306,8 @@ class Learner(TargetNetLearner):
         `use_graph`: the first call runs three eager warm-ups and captures the step as a CUDA graph (under the
         replay's lock, so that no ingest work lands in the capture); every later call replays it.  The draw reads
         the tree's device-resident size and Philox counter, so each replay draws a new minibatch.
-        With HOST_FRAMES the frames are not in HBM: the same gather launch sequence also copies the sampled sequences'
+        With FRAME_DEDUP conv_1 reads each stack's four frames from the frame pool through the slots' plane table
+        (R.StripDedupReplay.frame_source), with the rows of a strip store.  With HOST_FRAMES the frames are not in HBM: the same gather launch sequence also copies the sampled sequences'
         `state` rows from host memory into a fixed device staging buffer, and conv_1 reads that buffer with the rows
         train() uses on a staged batch (row = b * pitch + t)."""
         if self._graph is not None:
@@ -290,6 +326,8 @@ class Learner(TargetNetLearner):
                 staged = self._small["state"]
                 self._frames = R.strip_windows(staged) if c.FRAME_STRIP else staged.view(-1, 4, 84, 84)
                 self._pitch = T + 3 if c.FRAME_STRIP else T
+            elif c.FRAME_DEDUP:                                         # the windows through the plane table
+                self._frames, self._pitch = pool.frame_source("state"), T + 3
             elif c.FRAME_STRIP:
                 self._frames, self._pitch = R.strip_windows(pool.field_view("state")), T + 3
             else:

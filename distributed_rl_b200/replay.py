@@ -69,6 +69,13 @@ def r2d2_config_fields(cfg):
     return r2d2_fields(cfg.FIXED_TRAJECTORY, strip=bool(getattr(cfg, "FRAME_STRIP", False)))
 
 
+def R2D2_DEDUP_FIELDS(T: int = 80, hidden: int = 512):
+    """The slot of the frame-deduplicated R2D2 store (R2D2Config.FRAME_DEDUP, DESIGN.md §4.18): `planes`, the T + 3
+    int32 pool ids of the sequence's frame strip (frame j of the strip is pool frame planes[j]), then the small fields
+    of r2d2_fields."""
+    return (Field("planes", torch.int32, (T + 3,)),) + r2d2_fields(T, hidden, strip=True)[1:]
+
+
 # ---- R2D2 frame strips: a sequence of T stacks stored as its T + 3 distinct frames ----------------------------------
 # Every R2D2 record slides: R2D2/Player.py:38-63 stacks the last four frames of one episode, so stack t + 1 is stack t
 # shifted by one frame (s[t+1][:3] == s[t][1:]).  Frames t .. t + 3 of a strip are stack t, and stack t is the
@@ -507,10 +514,15 @@ class DedupReplay(DeviceReplay):
     APEX_FIELDS does, bit for bit; a slot also stops being live once pool_frames - window frames have been stored
     since its batch began (len() counts live slots).  The pipelined ingest forms are refused."""
 
+    RECORD_FIELDS = APEX_FIELDS      # what push takes and gather returns
+
     def __init__(self, capacity: int, pool_frames: int, window: int, device="cuda:0",
                  hash_mask: int = DEDUP_HASH_MASK):
         super().__init__(capacity, APEX_DEDUP_FIELDS, device)
         check(self.lib.b2rl_dedup_attach(self._h, 0, int(pool_frames), int(window), int(hash_mask)))
+        self._attached(pool_frames, window)
+
+    def _attached(self, pool_frames: int, window: int) -> None:
         self.pool_frames, self.window = int(pool_frames), int(window)
         p, mb = C.c_void_p(), C.c_int64()
         check(self.lib.b2rl_dedup_info(self._h, C.byref(p), None, C.byref(mb)))
@@ -529,15 +541,10 @@ class DedupReplay(DeviceReplay):
         """fields: [state, next_state, action, reward, done] as for a DeviceReplay of APEX_FIELDS (host, pinned
         preferred, or device).  The stacks are staged on the device (the same host->device bytes as a stack store),
         then pushed in chunks of at most max_batch records; each chunk synchronizes the current stream once."""
-        s, ns, rest = fields[0], fields[1], list(fields[2:])
+        s, ns = fields[0], fields[1]
         pr = torch.as_tensor(priorities).to(torch.float32).contiguous()
         n = pr.numel()
-        small = []
-        for f, x in zip(APEX_FIELDS[2:], rest):
-            t = torch.as_tensor(x)
-            t = (t if t.dtype == f.dtype else t.to(f.dtype)).contiguous()
-            assert t.numel() * t.element_size() == n * f.nbytes, f"bad shape for {f.name}"
-            small.append(t)
+        small = _small_rows(APEX_FIELDS[2:], fields[2:], n)
         stacks = []
         for x in (s, ns):
             t = torch.as_tensor(x)
@@ -563,7 +570,7 @@ class DedupReplay(DeviceReplay):
         raise ValueError("a frame-deduplicated replay (FRAME_DEDUP) holds pool ids, not hashable payload")
 
     def alloc_batch(self, n: int, names: Sequence[str] | None = None):
-        return alloc_rows(APEX_FIELDS, n, self.device, names)
+        return alloc_rows(self.RECORD_FIELDS, n, self.device, names)
 
     def gather(self, idx: torch.Tensor, out: dict | None = None) -> dict:
         """The sampled slots' fields as a DeviceReplay of APEX_FIELDS returns them: state and next_state are (n, 4,
@@ -582,6 +589,78 @@ class DedupReplay(DeviceReplay):
 
     def frame_source(self, name: str) -> "PlaneFrames":
         return PlaneFrames(self.pool, self.field_view("planes"), {"state": 0, "next_state": 4}[name])
+
+
+def _small_rows(fields: Sequence[Field], xs: Sequence, n: int) -> list:
+    """The non-frame fields of a dedup push as contiguous tensors of their fields' dtypes, n rows each."""
+    out = []
+    for f, x in zip(fields, xs):
+        t = torch.as_tensor(x)
+        t = (t if t.dtype == f.dtype else t.to(f.dtype)).contiguous()
+        assert t.numel() * t.element_size() == n * f.nbytes, f"bad shape for {f.name}"
+        out.append(t)
+    return out
+
+
+class StripDedupReplay(DedupReplay):
+    """The strip form of DedupReplay (b2rl_dedup_attach_strips, R2D2Config.FRAME_DEDUP, DESIGN.md §4.18): an R2D2
+    replay whose slots hold R2D2_DEDUP_FIELDS(T), the T + 3 frames of each sequence's strip living in the frame pool.
+    Sequences an actor cuts with half overlap (R2D2/Player.py:37-62) share about half of their frames, which are
+    stored once.  push / gather / sample / update take and return what a DeviceReplay of r2d2_fields(T, strip=True)
+    does, bit for bit, while every slot is live; the liveness rule and the refusals are DedupReplay's."""
+
+    def __init__(self, capacity: int, pool_frames: int, window: int, T: int = 80, device="cuda:0",
+                 hash_mask: int = DEDUP_HASH_MASK, hidden: int = 512):
+        DeviceReplay.__init__(self, capacity, R2D2_DEDUP_FIELDS(T, hidden), device)
+        self.T = int(T)
+        self.RECORD_FIELDS = r2d2_fields(self.T, hidden, strip=True)
+        check(self.lib.b2rl_dedup_attach_strips(self._h, 0, self.T + 3, int(pool_frames), int(window),
+                                                int(hash_mask)))
+        self._attached(pool_frames, window)
+
+    def push(self, fields: Sequence, priorities) -> None:
+        """fields: [state, action, reward, h0, h1, notdone] as for a DeviceReplay of r2d2_fields(T, strip=True),
+        `state` (n, T + 3, 84, 84) uint8 strips (host, pinned preferred, or device).  The strips are staged on the
+        device, then pushed in chunks of at most max_batch sequences; each chunk synchronizes the current stream
+        once."""
+        pr = torch.as_tensor(priorities).to(torch.float32).contiguous()
+        n = pr.numel()
+        small = _small_rows(self.RECORD_FIELDS[1:], fields[1:], n)
+        t = torch.as_tensor(fields[0])
+        row = (self.T + 3) * FRAME_BYTES
+        assert t.dtype == torch.uint8 and t.numel() == n * row, "frame strips must be uint8 (n, T + 3, 84, 84)"
+        strips = t.reshape(n, row).to(self.device, non_blocking=True).contiguous()
+        ptrs = (C.c_void_p * _lib.MAX_FIELDS)()
+        for a in range(0, n, self.max_batch):
+            b = min(n, a + self.max_batch)
+            ptrs[0] = None
+            for i, x in enumerate(small):
+                ptrs[1 + i] = x[a:b].data_ptr()
+            check(self.lib.b2rl_dedup_push_strips(self._h, strips[a:b].data_ptr(), ptrs, pr[a:b].data_ptr(), b - a,
+                                                  self._st()))
+        self._inflight = [strips] + small + [pr]
+
+    def gather(self, idx: torch.Tensor, out: dict | None = None) -> dict:
+        """The sampled slots' fields as a DeviceReplay of r2d2_fields(T, strip=True) returns them: `state` is the
+        (n, T + 3, 84, 84) strips assembled from the pool (b2rl_replay_gather_planes)."""
+        n = idx.numel()
+        if out is None:
+            out = self.alloc_batch(n)
+        st = out.get("state")
+        frames = (C.c_void_p * 2)(None if st is None else st.data_ptr(), None)
+        ptrs = (C.c_void_p * _lib.MAX_FIELDS)()
+        for i, f in enumerate(self.fields):
+            t = out.get(f.name) if i > 0 else None
+            ptrs[i] = t.data_ptr() if t is not None else None
+        check(self.lib.b2rl_replay_gather_planes(self._h, idx.data_ptr(), n, frames, ptrs, self._st()))
+        return out
+
+    def frame_source(self, name: str) -> "PlaneFrames":
+        """conv_1's rows of `state`: the windows of every slot's strip, row slot * (T + 3) + t being stack t of the
+        slot (the row numbering of strip_windows over a strip store's state field)."""
+        if name != "state":
+            raise KeyError(name)
+        return PlaneFrames(self.pool, self.field_view("planes"), 0, 1)
 
 
 # ---- stateless target kernels -------------------------------------------------
@@ -698,16 +777,25 @@ class BoundFrames:
 
 @dataclass(frozen=True)
 class PlaneFrames:
-    """Frame stacks held as a plane table over a frame pool (DedupReplay): row r is the stack whose channel c is
-    pool frame planes[r, base + c].  `pool`: uint8 (F, 84, 84); `planes`: int32 (rows, 8); `base`: 0 for `state`, 4
-    for `next_state`.  conv1_fused / conv1_wgrad read the four frames of each row in place."""
+    """Frame stacks held as a plane table over a frame pool: row r is the stack whose channel c is pool frame
+    planes.flatten()[plane_stride * r + base + c].  `pool`: uint8 (F, 84, 84).  DedupReplay: `planes` int32 (slots,
+    8), plane_stride 8, `base` 0 for `state` and 4 for `next_state`.  StripDedupReplay: `planes` int32 (slots, T + 3),
+    plane_stride 1, base 0, so row slot * (T + 3) + t is stack t of the slot's strip.  conv1_fused / conv1_wgrad read
+    the four frames of each row in place."""
     pool: torch.Tensor
     planes: torch.Tensor
     base: int
+    plane_stride: int = 8
 
     @property
     def device(self) -> torch.device:
         return self.pool.device
+
+    @property
+    def rows(self) -> int:
+        """The rows whose four pool ids lie inside `planes`: every slot at stride 8; at stride 1 every window but the
+        last three, which would run past the table's end."""
+        return (self.planes.numel() - self.base - 4) // self.plane_stride + 1
 
 
 def _frame_source(frames) -> _lib.Frames:
@@ -716,7 +804,7 @@ def _frame_source(frames) -> _lib.Frames:
     positive multiple of 16)."""
     if isinstance(frames, PlaneFrames):
         return _lib.Frames(pool=frames.pool.data_ptr(), planes=frames.planes.data_ptr(), plane_base=frames.base,
-                           rows=frames.planes.shape[0])
+                           plane_stride=frames.plane_stride, rows=frames.rows)
     if isinstance(frames, BoundFrames):
         return _lib.Frames(table=frames.entry_ptr(), row_stride=frames.row_stride, rows=frames.rows)
     if frames.device.type != "cuda":
@@ -729,7 +817,8 @@ def _frame_source(frames) -> _lib.Frames:
 
 def conv1_fused(frames, idx, pack: Conv1Pack, relu: bool = False, out=None):
     """frames: uint8 (rows, 4, 84, 84) with its inner three dimensions contiguous: frame stacks (e.g.
-    DeviceReplay.field_view("state")), the windows of frame strips (strip_windows), a BoundFrames or a PlaneFrames;
+    DeviceReplay.field_view("state")), the windows of frame strips (strip_windows), a BoundFrames or a PlaneFrames
+    (DedupReplay.frame_source, StripDedupReplay.frame_source);
     idx: int64[n] rows to take (None: all rows in order).
     -> list of n_nets tensors (n, c_out, 20, 20) fp32 in channels_last memory format."""
     src = _frame_source(frames)

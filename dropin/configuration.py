@@ -26,6 +26,10 @@ elif ALG == "R2D2":
     USE_RESCALING = DATA["USE_RESCALING"]
     FRAME_STRIP = bool(DATA.get("FRAME_STRIP", False))   # not a reference key: store sequences as frame strips
     HOST_FRAMES = bool(DATA.get("HOST_FRAMES", False))   # not a reference key: keep the frames in pinned host memory
+    FRAME_DEDUP = bool(DATA.get("FRAME_DEDUP", False))   # not a reference key: store every distinct frame once
+    for _k in ("FRAMES_PER_SEQUENCE", "DEDUP_WINDOW"):
+        if _k in DATA:
+            globals()[_k] = DATA[_k]
 elif ALG == "IMPALA":
     C_LAMBDA = DATA["C_LAMBDA"]
     C_VALUE = DATA["C_VALUE"]

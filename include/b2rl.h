@@ -234,10 +234,25 @@ int b2rl_replay_gather(b2rl_replay* h, const int64_t* idx_dev, int64_t n,
  *
  * b2rl_replay_gather_planes: b2rl_replay_gather for a dedup replay, plus the sampled slots' s and s' stacks
  * (Replay.buffer, APE_X/ReplayMemory.py:61-116): stacks_out_dev[0] / [1] (either may be NULL) receive (n, 4, 84,
- * 84) uint8 assembled from planes 0-3 / 4-7 by TMA bulk copies.  out_fields_dev[planes_field] is ignored. */
+ * 84) uint8 assembled from planes 0-3 / 4-7 by TMA bulk copies.  out_fields_dev[planes_field] is ignored.
+ *
+ * The same pool for R2D2 frame strips.  R2D2/Player.py:37-62 (LocalBuffer.get_traj) cuts an episode's sequences with
+ * half overlap, so a strip record (b2rl_frames: T + 3 frames, stack t = frames t .. t + 3) shares about half of its
+ * frames with the record before it.  b2rl_dedup_attach_strips is b2rl_dedup_attach for records of R =
+ * frames_per_record frames each: the planes field holds R int32 pool ids per slot (4 R bytes), frame j of a record
+ * having id planes[R slot + j].  Requires pool_frames - window > R; a push takes at most min(capacity, (pool_frames -
+ * window - 1) / R, 65536 / R) records.  b2rl_dedup_push_strips is b2rl_dedup_push for it: strips_dev is device
+ * (n, R, 84, 84) uint8.  Each push refuses the other kind of handle; b2rl_dedup_info serves both, and so do the
+ * refusals above.  b2rl_replay_gather_planes on a strip handle: stacks_out_dev[0] receives the (n, R, 84, 84)
+ * strips assembled from the pool and stacks_out_dev[1] must be NULL.  b2rl_serve_ring_create / b2rl_serve_fill
+ * serve it with the strip store's record layout: the planes field becomes the (B, R, 84, 84) strip field. */
 int b2rl_dedup_attach(b2rl_replay* h, int32_t planes_field, int64_t pool_frames, int64_t window, uint64_t hash_mask);
 int b2rl_dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8_t* ns_dev, const void* const* fields_src,
                     const float* prios, int64_t n, void* stream);
+int b2rl_dedup_attach_strips(b2rl_replay* h, int32_t planes_field, int32_t frames_per_record, int64_t pool_frames,
+                             int64_t window, uint64_t hash_mask);
+int b2rl_dedup_push_strips(b2rl_replay* h, const uint8_t* strips_dev, const void* const* fields_src,
+                           const float* prios, int64_t n, void* stream);
 int b2rl_dedup_info(const b2rl_replay* h, void** pool_dev, int64_t* head_seq, int64_t* max_batch);
 int b2rl_replay_gather_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, void* const* stacks_out_dev,
                               void* const* out_fields_dev, void* stream);
@@ -304,9 +319,12 @@ int b2rl_vtrace(const float* pi_a_dev, const float* mu_a_dev, const float* value
  *           minibatch slot (Replay_Server.sample, APE_X/ReplayMemory.py:251-257) was bound before the replay.  The
  *           base it holds must be 16-byte aligned.  When b2rl_conv1_wgrad splits a large n over several launches
  *           (idx_dev NULL), each launch adds its row offset to the loaded base on the device.
- *   pool + planes (+ plane_base)   the frame-deduplicated Ape-X store (b2rl_dedup_attach): channel c of row r is
- *           the 7 056-byte frame pool + planes[8 r + plane_base + c] * 7 056 (pool 16-byte aligned, planes 4-byte
- *           aligned; plane_base 0: `state`, 4: `next_state` of the transition APE_X/Player.py:252-261 sends).
+ *   pool + planes (+ plane_base, plane_stride)   a frame-deduplicated store (b2rl_dedup_attach,
+ *           b2rl_dedup_attach_strips): channel c of row r is the 7 056-byte frame pool +
+ *           planes[plane_stride r + plane_base + c] * 7 056 (pool 16-byte aligned, planes 4-byte aligned).
+ *           plane_stride 0 means 8, the Ape-X layout: plane_base 0 reads `state`, 4 `next_state` of the transition
+ *           APE_X/Player.py:252-261 sends.  plane_stride 1 (plane_base 0) reads the overlapping windows of R2D2 strip
+ *           records, whose T + 3 pool ids per slot are consecutive: row slot * (T + 3) + t is stack t of the slot.
  * row_stride (base and table) must be a positive multiple of 16.  Row indices are clamped to [0, rows), rows >= 1:
  * the caller guarantees that row rows - 1 ends inside the allocation. */
 typedef struct {
@@ -317,7 +335,7 @@ typedef struct {
   int64_t row_stride;
   int64_t rows;
   int32_t plane_base;
-  int32_t reserved;
+  int32_t plane_stride;
 } b2rl_frames;
 
 /* Fused gather + first convolution (north-star "TMA staging of sampled transition slices
