@@ -16,6 +16,10 @@
 //      in the key table; the other fields and the priorities follow as for b2rl_replay_push.
 // Everything a frame's id depends on is a function of the record stream (keys, positions, the window), so the ids
 // can be checked against a CPU model (tests/dedup_model.py).
+// A strip handle's pool may live in pinned, mapped host memory (b2rl_dedup_attach_strips_placed, DESIGN.md §4.19).
+// The kernels are the same: k_dedup_resolve compares a hit's frame and k_dedup_copy stores the misses through the
+// pool's device alias with plain 16-byte loads and stores, over PCIe, in order on the push's stream.  The key
+// tables, pool_key and the batch scratch stay in HBM.
 #include "common.cuh"
 
 #include <new>
@@ -43,7 +47,9 @@ struct DedupState {
   Layout layout = Layout::Pairs;
   int64_t F = 0, W = 0, T = 0;                    // pool frames, window, key-table entries (a power of two)
   unsigned long long mask = 0;
-  uint8_t* pool = nullptr;                        // [F][7056]
+  uint8_t* pool = nullptr;                        // [F][7056] the address kernels use: device memory, or the device
+                                                  // alias of a host pool's pinned frames
+  uint8_t* pool_host = nullptr;                   // b2rl_dedup_attach_strips_placed: the host address of a host pool
   unsigned long long* pool_key = nullptr;         // [F] key of the frame in each pool slot, for table rebuilds
   unsigned long long* tkey = nullptr;             // [T]
   unsigned long long* tseq = nullptr;             // [T] 1 + seq of the newest frame stored under tkey (0: none)
@@ -273,7 +279,9 @@ k_dedup_rebuild(const unsigned long long* __restrict__ pool_key, int64_t F, int6
 void dedup_free(b2rl_replay* h) {
   DedupState* d = h->dedup;
   if (d == nullptr) return;
-  for (void* p : {(void*)d->pool, (void*)d->pool_key, (void*)d->tkey, (void*)d->tseq, (void*)d->key, (void*)d->rep,
+  if (d->pool_host) cudaFreeHost(d->pool_host);
+  else if (d->pool) cudaFree(d->pool);
+  for (void* p : {(void*)d->pool_key, (void*)d->tkey, (void*)d->tseq, (void*)d->key, (void*)d->rep,
                   (void*)d->fseq, (void*)d->bkey, (void*)d->bpos, (void*)d->misses_dev})
     if (p) cudaFree(p);
   if (d->misses_host) cudaFreeHost(d->misses_host);
@@ -284,6 +292,8 @@ void dedup_free(b2rl_replay* h) {
 
 int dedup_planes_field(const b2rl_replay* h) { return h->dedup->planes_field; }
 const uint8_t* dedup_pool(const b2rl_replay* h) { return h->dedup->pool; }
+int64_t dedup_pool_frames(const b2rl_replay* h) { return h->dedup->F; }
+bool dedup_pool_on_host(const b2rl_replay* h) { return h->dedup->pool_host != nullptr; }
 int dedup_strip_frames(const b2rl_replay* h) { return h->dedup->layout == Layout::Strips ? h->dedup->R : 0; }
 
 }  // namespace b2rl
@@ -296,21 +306,24 @@ static int64_t pow2_at_least(int64_t x) {
   return p;
 }
 
-// b2rl_dedup_attach (Pairs, R = 8) and b2rl_dedup_attach_strips (Strips, R = frames_per_record).
+// b2rl_dedup_attach (Pairs, R = 8), b2rl_dedup_attach_strips and b2rl_dedup_attach_strips_placed (Strips, R =
+// frames_per_record).  The arguments are checked before the handle, so every refusal comes before any CUDA work.
 static int dedup_attach(b2rl_replay* h, int32_t planes_field, Layout layout, int32_t R, int64_t pool_frames,
-                        int64_t window, uint64_t hash_mask) {
-  B2RL_REQUIRE(h != nullptr, "null handle");
-  B2RL_REQUIRE(h->dedup == nullptr, "the replay already has a frame pool");
-  B2RL_REQUIRE(!h->any_on_host, "a replay with fields placed on the host cannot take a frame pool");
-  B2RL_REQUIRE(h->size == 0 && h->head == 0 && h->reserved == 0 && h->pipe_n == 0, "the replay must be empty");
+                        int64_t window, uint64_t hash_mask, bool pool_on_host) {
+  B2RL_REQUIRE(!pool_on_host || layout == Layout::Strips,
+               "an Ape-X (Pairs) frame pool stays in HBM: only a strip handle's pool can be placed on the host");
   B2RL_REQUIRE(R >= 4 && R <= DD_MAX_FRAMES, "frames_per_record must be in [4, 65536]");
-  B2RL_REQUIRE(planes_field >= 0 && planes_field < h->n_fields && h->field_bytes[planes_field] == 4 * (int64_t)R,
-               layout == Layout::Pairs ? "the planes field must hold 8 int32 per slot"
-                                       : "the planes field must hold frames_per_record int32 per slot");
   B2RL_REQUIRE(window >= 0 && pool_frames - window > R,
                layout == Layout::Pairs ? "need window >= 0 and pool_frames - window > 8"
                                        : "need window >= 0 and pool_frames - window > frames_per_record");
   B2RL_REQUIRE(pool_frames < (1LL << 31), "pool_frames must be below 2^31");
+  B2RL_REQUIRE(h != nullptr, "null handle");
+  B2RL_REQUIRE(h->dedup == nullptr, "the replay already has a frame pool");
+  B2RL_REQUIRE(!h->any_on_host, "a replay with fields placed on the host cannot take a frame pool");
+  B2RL_REQUIRE(h->size == 0 && h->head == 0 && h->reserved == 0 && h->pipe_n == 0, "the replay must be empty");
+  B2RL_REQUIRE(planes_field >= 0 && planes_field < h->n_fields && h->field_bytes[planes_field] == 4 * (int64_t)R,
+               layout == Layout::Pairs ? "the planes field must hold 8 int32 per slot"
+                                       : "the planes field must hold frames_per_record int32 per slot");
   DeviceGuard g(h->device);
   DedupState* d = new (std::nothrow) DedupState();
   if (!d) { set_error("out of host memory"); return B2RL_ERR_NOMEM; }
@@ -331,7 +344,21 @@ static int dedup_attach(b2rl_replay* h, int32_t planes_field, Layout layout, int
   auto alloc = [&](void** p, size_t bytes) {
     if (e == cudaSuccess) e = cudaMalloc(p, bytes);
   };
-  alloc((void**)&d->pool, (size_t)d->F * DD_FRAME);
+  if (pool_on_host) {   // pinned, mapped frames: the kernels read and write them through the device alias
+    const size_t bytes = (size_t)d->F * DD_FRAME;
+    const cudaError_t eh = cudaHostAlloc((void**)&d->pool_host, bytes, cudaHostAllocMapped | cudaHostAllocPortable);
+    if (eh != cudaSuccess) {
+      d->pool_host = nullptr;
+      set_error("cudaHostAlloc of %.3f GB (%zu bytes) of pinned host memory for a %lld-frame pool failed: %s",
+                bytes * 1e-9, bytes, (long long)pool_frames, cudaGetErrorString(eh));
+      dedup_free(h);
+      cudaGetLastError();
+      return B2RL_ERR_NOMEM;
+    }
+    e = cudaHostGetDevicePointer((void**)&d->pool, d->pool_host, 0);
+  } else {
+    alloc((void**)&d->pool, (size_t)d->F * DD_FRAME);
+  }
   alloc((void**)&d->pool_key, sizeof(unsigned long long) * (size_t)d->F);
   alloc((void**)&d->tkey, sizeof(unsigned long long) * (size_t)d->T);
   alloc((void**)&d->tseq, sizeof(unsigned long long) * (size_t)d->T);
@@ -365,12 +392,20 @@ static int dedup_attach(b2rl_replay* h, int32_t planes_field, Layout layout, int
 
 extern "C" int b2rl_dedup_attach(b2rl_replay* h, int32_t planes_field, int64_t pool_frames, int64_t window,
                                  uint64_t hash_mask) {
-  return dedup_attach(h, planes_field, Layout::Pairs, 8, pool_frames, window, hash_mask);
+  return dedup_attach(h, planes_field, Layout::Pairs, 8, pool_frames, window, hash_mask, false);
 }
 
 extern "C" int b2rl_dedup_attach_strips(b2rl_replay* h, int32_t planes_field, int32_t frames_per_record,
                                         int64_t pool_frames, int64_t window, uint64_t hash_mask) {
-  return dedup_attach(h, planes_field, Layout::Strips, frames_per_record, pool_frames, window, hash_mask);
+  return dedup_attach(h, planes_field, Layout::Strips, frames_per_record, pool_frames, window, hash_mask, false);
+}
+
+extern "C" int b2rl_dedup_attach_strips_placed(b2rl_replay* h, int32_t planes_field, int32_t frames_per_record,
+                                               int64_t pool_frames, int64_t window, uint64_t hash_mask,
+                                               int32_t pool_on_host) {
+  B2RL_REQUIRE(pool_on_host == 0 || pool_on_host == 1, "pool_on_host must be 0 or 1");
+  return dedup_attach(h, planes_field, Layout::Strips, frames_per_record, pool_frames, window, hash_mask,
+                      pool_on_host != 0);
 }
 
 extern "C" int b2rl_dedup_info(const b2rl_replay* h, void** pool_dev, int64_t* head_seq, int64_t* max_batch) {
@@ -379,6 +414,14 @@ extern "C" int b2rl_dedup_info(const b2rl_replay* h, void** pool_dev, int64_t* h
   if (pool_dev) *pool_dev = h->dedup->pool;
   if (head_seq) *head_seq = h->dedup->head;
   if (max_batch) *max_batch = h->dedup->max_batch;
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_dedup_pool_placement(const b2rl_replay* h, int32_t* on_host, void** pool) {
+  B2RL_REQUIRE(h != nullptr && on_host != nullptr, "null argument");
+  B2RL_REQUIRE(h->dedup != nullptr, "not a frame-deduplicated replay (b2rl_dedup_attach)");
+  *on_host = h->dedup->pool_host != nullptr ? 1 : 0;
+  if (pool) *pool = *on_host ? h->dedup->pool_host : h->dedup->pool;
   return B2RL_OK;
 }
 

@@ -143,7 +143,12 @@ static int gather_run(b2rl_replay* h, const int64_t* idx_dev, int64_t n, void* c
     if (R > 0) {
       B2RL_REQUIRE(stacks_out[1] == nullptr, "a strip handle has one frame output: stacks_out_dev[1] must be NULL");
       B2RL_REQUIRE((uintptr_t)stacks_out[0] % 16 == 0, "frame strip outputs must be 16-byte aligned");
-      if (stacks_out[0] != nullptr) P.bulk.add_planes(dedup_pool(h), planes, R, 0, R, (uint8_t*)stacks_out[0]);
+      if (stacks_out[0] != nullptr && dedup_pool_on_host(h)) {   // never the TMA row copy: hostrows.cu's gather
+        const int rc = gather_host_planes(h, idx_dev, n, (uint8_t*)stacks_out[0], st);
+        if (rc != B2RL_OK) return rc;
+      } else if (stacks_out[0] != nullptr) {
+        P.bulk.add_planes(dedup_pool(h), planes, R, 0, R, (uint8_t*)stacks_out[0]);
+      }
     } else {
       for (int i = 0; i < 2; ++i) {
         B2RL_REQUIRE((uintptr_t)stacks_out[i] % 16 == 0, "frame stack outputs must be 16-byte aligned");

@@ -1,5 +1,6 @@
 // Replay fields placed in pinned, mapped host memory (b2rl_replay_create_placed): the sampled-row gather over PCIe
-// and the stream-ordered ingest into host rows.
+// and the stream-ordered ingest into host rows.  The same gather for the frames of a strip handle whose frame pool is
+// on the host (b2rl_dedup_attach_strips_placed): each sampled slot's R pool frames, scattered over the pool.
 //
 // A host field is never read by the TMA row copy of bulk_rows.cuh: whether bulk async copies read mapped host memory
 // has not been established, so the rows travel through plain 16-byte loads of the mapped pointer.  PCIe latency is
@@ -31,6 +32,35 @@ k_gather_host_rows(const int4* __restrict__ src, int4* __restrict__ dst, int64_t
       if (v < total) {
         const int64_t k = v / row_vecs;
         r[u] = __ldcg(src + clamp_row(idx[k], capacity) * row_vecs + (v - k * row_vecs));
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < HOST_ROWS_UNROLL; ++u) {
+      const int64_t v = v0 + u * stride;
+      if (v < total) dst[v] = r[u];
+    }
+  }
+}
+
+// The frame-pool form of k_gather_host_rows, for a strip handle whose pool is on the host: dst row k (R frames of
+// PLANE_BYTES) = the frames of slot clamp_row(idx[k]), frame j being pool frame planes[R slot + j] % F.  The n R frames'
+// 16-byte units are dealt out grid-stride the same way, so a warp reads consecutive units of one frame.
+__global__ void __launch_bounds__(HOST_ROWS_THREADS)
+k_gather_host_planes(const int4* __restrict__ pool, int4* __restrict__ dst, const int32_t* __restrict__ planes,
+                     int32_t R, int64_t F, const int64_t* __restrict__ idx, int64_t n, int64_t capacity) {
+  constexpr int64_t FRAME_VECS = PLANE_BYTES / 16;   // 441
+  const int64_t total = n * R * FRAME_VECS;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t v0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v0 < total; v0 += stride * HOST_ROWS_UNROLL) {
+    int4 r[HOST_ROWS_UNROLL];
+#pragma unroll
+    for (int u = 0; u < HOST_ROWS_UNROLL; ++u) {
+      const int64_t v = v0 + u * stride;
+      if (v < total) {
+        const int64_t fr = v / FRAME_VECS;   // frame fr - k R of draw k
+        const int64_t k = fr / R;
+        const int64_t id = planes[R * clamp_row(idx[k], capacity) + (fr - k * R)];
+        r[u] = __ldcg(pool + (id % F) * FRAME_VECS + (v - fr * FRAME_VECS));
       }
     }
 #pragma unroll
@@ -84,6 +114,18 @@ int gather_host_rows(b2rl_replay* h, int f, const int64_t* idx_dev, int64_t n, u
   k_gather_host_rows<<<host_ctas(h->device, n * row_vecs), HOST_ROWS_THREADS, 0, st>>>(
       reinterpret_cast<const int4*>(h->field[f]), reinterpret_cast<int4*>(dst_dev), row_vecs, idx_dev, n,
       h->capacity);
+  count_launch();
+  B2RL_CHECK_LAUNCH();
+  return B2RL_OK;
+}
+
+int gather_host_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, cudaStream_t st) {
+  B2RL_REQUIRE((uintptr_t)dst_dev % 16 == 0, "frame strip outputs must be 16-byte aligned");
+  if (n == 0) return B2RL_OK;
+  const int R = dedup_strip_frames(h);
+  k_gather_host_planes<<<host_ctas(h->device, n * R * (PLANE_BYTES / 16)), HOST_ROWS_THREADS, 0, st>>>(
+      reinterpret_cast<const int4*>(dedup_pool(h)), reinterpret_cast<int4*>(dst_dev),
+      (const int32_t*)h->field[dedup_planes_field(h)], R, dedup_pool_frames(h), idx_dev, n, h->capacity);
   count_launch();
   B2RL_CHECK_LAUNCH();
   return B2RL_OK;

@@ -80,14 +80,20 @@ class R2D2Config:
     FRAMES_PER_SEQUENCE: float = 48.0
     DEDUP_WINDOW: int = 1 << 14  # a frame is reused only from the last DEDUP_WINDOW frames stored (at most 1/8 of the
                                  # pool, see dedup_geometry)
+    HOST_POOL: bool = False      # keep a FRAME_DEDUP store's frame pool in pinned, mapped host memory; the plane table,
+                                 # the keys and the sum-tree stay in HBM.  Each step copies the sampled sequences' frames
+                                 # over PCIe into a device staging buffer, as HOST_FRAMES does (DESIGN §4.19).
 
     def __post_init__(self):
         if self.HOST_FRAMES and self.PAYLOAD_POOL:
             raise ValueError("HOST_FRAMES stores every sequence's frames in host memory and replaces the PAYLOAD_POOL "
                              "benchmark stand-in: set PAYLOAD_POOL = 0 with HOST_FRAMES")
+        if self.HOST_POOL and not self.FRAME_DEDUP:
+            raise ValueError("HOST_POOL places the frame pool of a FRAME_DEDUP store: set FRAME_DEDUP with it "
+                             "(HOST_FRAMES places a strip or stack store's frames)")
         if self.FRAME_DEDUP and (self.HOST_FRAMES or self.PAYLOAD_POOL):
-            raise ValueError("FRAME_DEDUP keeps its frame pool in HBM and stores every pushed sequence: it takes "
-                             "neither HOST_FRAMES nor PAYLOAD_POOL")
+            raise ValueError("FRAME_DEDUP keeps its frames in a frame pool (in host memory with HOST_POOL) and stores "
+                             "every pushed sequence: it takes neither HOST_FRAMES nor PAYLOAD_POOL")
         if self.FRAME_DEDUP:
             self.FRAME_STRIP = True
 
@@ -98,7 +104,7 @@ class R2D2Config:
                  "USE_RESCALING", "REPLAY_MEMORY_LEN", "BUFFER_SIZE", "TARGET_FREQUENCY", "LEARNER_DEVICE",
                  "REDIS_SERVER", "OPTIM_INFO", "MODEL")
         kw = {k: getattr(C, k) for k in names}
-        for k in ("FRAME_DEDUP", "FRAMES_PER_SEQUENCE", "DEDUP_WINDOW"):     # optional keys of cfg/r2d2.json
+        for k in ("FRAME_DEDUP", "FRAMES_PER_SEQUENCE", "DEDUP_WINDOW", "HOST_POOL"):   # optional keys of cfg/r2d2.json
             if hasattr(C, k):
                 kw[k] = getattr(C, k)
         return R2D2Config(LOG_W=getattr(C, "LOG_W", None), FRAME_STRIP=bool(getattr(C, "FRAME_STRIP", False)),
@@ -133,7 +139,8 @@ class Replay(ReplayThread):
             self.pool = R.DeviceReplay(self.cfg.PAYLOAD_POOL, fields, self.device)           # the stored sequences
         elif self.cfg.FRAME_DEDUP:
             self.store = self.pool = R.StripDedupReplay(self.cfg.REPLAY_MEMORY_LEN, *dedup_geometry(self.cfg),
-                                                        T=self.cfg.FIXED_TRAJECTORY, device=self.device)
+                                                        T=self.cfg.FIXED_TRAJECTORY, device=self.device,
+                                                        host_pool=self.cfg.HOST_POOL)
         else:
             self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, fields, self.device,
                                         host_fields=("state",) if self.cfg.HOST_FRAMES else ())
@@ -307,9 +314,10 @@ class Learner(TargetNetLearner):
         replay's lock, so that no ingest work lands in the capture); every later call replays it.  The draw reads
         the tree's device-resident size and Philox counter, so each replay draws a new minibatch.
         With FRAME_DEDUP conv_1 reads each stack's four frames from the frame pool through the slots' plane table
-        (R.StripDedupReplay.frame_source), with the rows of a strip store.  With HOST_FRAMES the frames are not in HBM: the same gather launch sequence also copies the sampled sequences'
-        `state` rows from host memory into a fixed device staging buffer, and conv_1 reads that buffer with the rows
-        train() uses on a staged batch (row = b * pitch + t)."""
+        (R.StripDedupReplay.frame_source), with the rows of a strip store.  With HOST_FRAMES or HOST_POOL the frames
+        are not in HBM: the same gather launch sequence also copies the sampled sequences' `state` rows (with
+        HOST_POOL their strips, assembled from the host pool) from host memory into a fixed device staging buffer,
+        and conv_1 reads that buffer with the rows train() uses on a staged batch (row = b * pitch + t)."""
         if self._graph is not None:
             self._graph.replay()
             return self._static
@@ -319,12 +327,13 @@ class Learner(TargetNetLearner):
         T, MEM, B, A = c.FIXED_TRAJECTORY, c.MEM, c.BATCHSIZE, c.ACTION_SIZE
         mem = self.memory
         st, pool = mem.store, mem.pool
+        staged = c.HOST_FRAMES or c.HOST_POOL                   # the frames are in host memory
         if not hasattr(self, "_small"):
             self._small = pool.alloc_batch(B, ("action", "reward", "h0", "h1", "notdone"))
-            if c.HOST_FRAMES:
+            if staged:
                 self._small.update(pool.alloc_batch(B, ("state",)))    # the staging buffer: B sequences' frames
-                staged = self._small["state"]
-                self._frames = R.strip_windows(staged) if c.FRAME_STRIP else staged.view(-1, 4, 84, 84)
+                buf = self._small["state"]
+                self._frames = R.strip_windows(buf) if c.FRAME_STRIP else buf.view(-1, 4, 84, 84)
                 self._pitch = T + 3 if c.FRAME_STRIP else T
             elif c.FRAME_DEDUP:                                         # the windows through the plane table
                 self._frames, self._pitch = pool.frame_source("state"), T + 3
@@ -340,7 +349,7 @@ class Learner(TargetNetLearner):
             h0, h1 = b["h0"].unsqueeze(0), b["h1"].unsqueeze(0)
             self.model.setCellState((h0, h1))
             self.target_model.setCellState((h0, h1))
-            seq_rows = None if c.HOST_FRAMES else rows          # staged: sequence b's frames start at row b * pitch
+            seq_rows = None if staged else rows                 # staged: sequence b's frames start at row b * pitch
             q, q_target = self._forward_fused(self._frames, self._time_major_rows(seq_rows, T, B, self._pitch), T, MEM,
                                               B, A)
             out, info = self._learn(q, q_target, b["action"], b["reward"], b["notdone"], w)

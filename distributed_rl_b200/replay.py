@@ -524,9 +524,13 @@ class DedupReplay(DeviceReplay):
 
     def _attached(self, pool_frames: int, window: int) -> None:
         self.pool_frames, self.window = int(pool_frames), int(window)
-        p, mb = C.c_void_p(), C.c_int64()
-        check(self.lib.b2rl_dedup_info(self._h, C.byref(p), None, C.byref(mb)))
+        p, mb, on_host = C.c_void_p(), C.c_int64(), C.c_int32()
+        check(self.lib.b2rl_dedup_info(self._h, None, None, C.byref(mb)))
+        check(self.lib.b2rl_dedup_pool_placement(self._h, C.byref(on_host), C.byref(p)))
         self.max_batch = mb.value
+        if on_host.value:       # a CPU tensor over the pinned frames, as field_view of a host field
+            self.pool = torch.from_numpy(np.asarray(_HostView(p.value, (self.pool_frames, 84, 84), "|u1", self)))
+            return
         with torch.cuda.device(self.device):
             self.pool = torch.as_tensor(_CudaView(p.value, (self.pool_frames, 84, 84), "|u1", self), device=self.device)
 
@@ -607,15 +611,24 @@ class StripDedupReplay(DedupReplay):
     replay whose slots hold R2D2_DEDUP_FIELDS(T), the T + 3 frames of each sequence's strip living in the frame pool.
     Sequences an actor cuts with half overlap (R2D2/Player.py:37-62) share about half of their frames, which are
     stored once.  push / gather / sample / update take and return what a DeviceReplay of r2d2_fields(T, strip=True)
-    does, bit for bit, while every slot is live; the liveness rule and the refusals are DedupReplay's."""
+    does, bit for bit, while every slot is live; the liveness rule and the refusals are DedupReplay's.
+    `host_pool` (R2D2Config.HOST_POOL, DESIGN.md §4.19): the frame pool lives in pinned, mapped host memory owned by
+    the library (b2rl_dedup_attach_strips_placed), allocated from a thread bound to the GPU's NUMA node; the planes,
+    keys and sum-tree stay in HBM.  `pool` is then a CPU tensor, gather() copies the sampled strips over PCIe, and
+    frame_source() is refused: conv_1 reads a gathered (staged) batch instead."""
 
     def __init__(self, capacity: int, pool_frames: int, window: int, T: int = 80, device="cuda:0",
-                 hash_mask: int = DEDUP_HASH_MASK, hidden: int = 512):
+                 hash_mask: int = DEDUP_HASH_MASK, hidden: int = 512, host_pool: bool = False):
         DeviceReplay.__init__(self, capacity, R2D2_DEDUP_FIELDS(T, hidden), device)
         self.T = int(T)
         self.RECORD_FIELDS = r2d2_fields(self.T, hidden, strip=True)
-        check(self.lib.b2rl_dedup_attach_strips(self._h, 0, self.T + 3, int(pool_frames), int(window),
-                                                int(hash_mask)))
+        self.host_pool = bool(host_pool)
+        args = (self._h, 0, self.T + 3, int(pool_frames), int(window), int(hash_mask))
+        if self.host_pool:
+            with hostmem.on_gpu_node(self.device):   # pinned pages on the GPU's NUMA node (first touch: the library)
+                check(self.lib.b2rl_dedup_attach_strips_placed(*args, 1))
+        else:
+            check(self.lib.b2rl_dedup_attach_strips(*args))
         self._attached(pool_frames, window)
 
     def push(self, fields: Sequence, priorities) -> None:
@@ -660,6 +673,9 @@ class StripDedupReplay(DedupReplay):
         slot (the row numbering of strip_windows over a strip store's state field)."""
         if name != "state":
             raise KeyError(name)
+        if self.host_pool:
+            raise ValueError("conv_1 reads its frame rows in place on the GPU: a frame pool in host memory (host_pool) "
+                             "has no frame source; gather the sampled strips into device memory first")
         return PlaneFrames(self.pool, self.field_view("planes"), 0, 1)
 
 
@@ -803,6 +819,9 @@ def _frame_source(frames) -> _lib.Frames:
     dimension, each a contiguous FRAME_STACK_BYTES; stride(0) is the row stride (the library checks that it is a
     positive multiple of 16)."""
     if isinstance(frames, PlaneFrames):
+        if frames.pool.device.type != "cuda":
+            raise ValueError("conv_1 reads its frame rows in place on the GPU: a frame pool in host memory must be "
+                             "gathered into device memory first")
         return _lib.Frames(pool=frames.pool.data_ptr(), planes=frames.planes.data_ptr(), plane_base=frames.base,
                            plane_stride=frames.plane_stride, rows=frames.rows)
     if isinstance(frames, BoundFrames):

@@ -27,6 +27,7 @@ elif ALG == "R2D2":
     FRAME_STRIP = bool(DATA.get("FRAME_STRIP", False))   # not a reference key: store sequences as frame strips
     HOST_FRAMES = bool(DATA.get("HOST_FRAMES", False))   # not a reference key: keep the frames in pinned host memory
     FRAME_DEDUP = bool(DATA.get("FRAME_DEDUP", False))   # not a reference key: store every distinct frame once
+    HOST_POOL = bool(DATA.get("HOST_POOL", False))       # not a reference key: keep that frame pool in host memory
     for _k in ("FRAMES_PER_SEQUENCE", "DEDUP_WINDOW"):
         if _k in DATA:
             globals()[_k] = DATA[_k]

@@ -254,6 +254,22 @@ int b2rl_dedup_attach_strips(b2rl_replay* h, int32_t planes_field, int32_t frame
 int b2rl_dedup_push_strips(b2rl_replay* h, const uint8_t* strips_dev, const void* const* fields_src,
                            const float* prios, int64_t n, void* stream);
 int b2rl_dedup_info(const b2rl_replay* h, void** pool_dev, int64_t* head_seq, int64_t* max_batch);
+
+/* The strip store of R2D2/ReplayMemory.py:70-88 behind PER.__init__ (baseline/PER.py:49-66), with the frame pool
+ * placed where it is read from: b2rl_dedup_attach_strips when pool_on_host is 0; with 1 the pool lives in pinned,
+ * mapped host memory owned by the handle (cudaHostAlloc with cudaHostAllocMapped | cudaHostAllocPortable; the kernels
+ * address it through cudaHostGetDevicePointer).  The planes field, pool keys, key table, batch scratch and sum-tree
+ * stay in device memory.  B2RL_ERR_NOMEM, with the size in the message, when the pinned allocation fails.  A push
+ * compares hits and stores misses through the mapped pointer, in order on its stream.  A host pool is never read by
+ * bulk async (TMA) copies: b2rl_replay_gather_planes and b2rl_serve_fill copy the sampled slots' strips with 16-byte
+ * loads through the mapped pointer, from a few CTAs (B2RL_HOST_GATHER_CTAS, default 8).  b2rl_dedup_info's *pool_dev
+ * is then the device alias: never pass it to b2rl_conv1_fused or b2rl_conv1_wgrad.  Ape-X's b2rl_dedup_attach has no
+ * placed form.  Arguments are checked before the handle is read. */
+int b2rl_dedup_attach_strips_placed(b2rl_replay* h, int32_t planes_field, int32_t frames_per_record,
+                                    int64_t pool_frames, int64_t window, uint64_t hash_mask, int32_t pool_on_host);
+/* Where the frame pool (the frames of PER.memory, baseline/PER.py:7-28) of a dedup replay lives: *on_host = 1 for
+ * pinned host memory, 0 for device; *pool (may be NULL) its host address, or its device address for a device pool. */
+int b2rl_dedup_pool_placement(const b2rl_replay* h, int32_t* on_host, void** pool);
 int b2rl_replay_gather_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, void* const* stacks_out_dev,
                               void* const* out_fields_dev, void* stream);
 
