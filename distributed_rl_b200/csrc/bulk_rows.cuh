@@ -57,6 +57,14 @@ struct BulkRows {
     items_per_row += k;
     ++n;
   }
+  // The time-major form of add_planes for rows of `steps` frame stacks (IMPALA rollout records, stride = 4 steps):
+  // stack t of draw k, pool ids planes[stride row_of(k) + 4t .. 4t + 3], goes to output row t * batch + k; one chunk
+  // per frame.  Only for a TIME_MAJOR copy.
+  void add_planes_time_major(const uint8_t* pool, const int32_t* planes, int32_t stride, int64_t steps, uint8_t* dst) {
+    f[n] = BulkField{pool, dst, steps * STACK_BYTES, (int32_t)(4 * steps), STACK_BYTES, planes, 0, stride};
+    items_per_row += f[n].chunks;
+    ++n;
+  }
   // A row of `steps` time steps whose step t of draw k goes to output row t * batch + k: chunked per step, so no
   // chunk straddles two steps and each one is a single bulk copy with a contiguous destination.
   void add_time_major(const uint8_t* src, uint8_t* dst, int64_t row_bytes, int64_t steps, int chunk) {
@@ -85,6 +93,12 @@ struct ItemCursor {
   }
   __device__ __forceinline__ void get(const BulkRows& T, int64_t dst_k0, const uint8_t*& src, uint8_t*& dst,
                                       uint32_t& bytes, int64_t batch = 0) const {
+    if (TIME_MAJOR && T.f[f].planes != nullptr) {   // frame c of the row is frame c % 4 of stack c / 4
+      bytes = PLANE_BYTES;
+      src = plane_ptr(T.f[f].src, T.f[f].planes, row, T.f[f].plane_stride, T.f[f].plane_base, c);
+      dst = T.f[f].dst + ((int64_t)(c >> 2) * batch + dst_k0 + k) * STACK_BYTES + (int64_t)(c & 3) * PLANE_BYTES;
+      return;
+    }
     if (TIME_MAJOR) {
       const int32_t step = T.f[f].step_bytes;
       const int32_t cps = (step + CHUNK - 1) / CHUNK;   // chunks per step

@@ -158,6 +158,7 @@ const uint8_t* dedup_pool(const b2rl_replay* h);  // the address kernels use (a 
 int64_t dedup_pool_frames(const b2rl_replay* h);
 bool dedup_pool_on_host(const b2rl_replay* h);     // b2rl_dedup_attach_strips_placed with pool_on_host
 int dedup_strip_frames(const b2rl_replay* h);     // R of a strip handle (b2rl_dedup_attach_strips), else 0
+int dedup_rollout_stacks(const b2rl_replay* h);   // T + 1 of a rollout handle (b2rl_dedup_attach_rollouts), else 0
 // The (n, R, 84, 84) strips of the sampled slots clamp_row(idx_dev[k]) of a strip handle whose pool is on the host,
 // assembled from the pool through 16-byte loads of its mapped frames (hostrows.cu).  dst_dev 16-byte aligned.
 int gather_host_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, cudaStream_t st);

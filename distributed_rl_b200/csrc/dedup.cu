@@ -3,7 +3,9 @@
 //
 // A pushed batch of n records is R n frames, R frames per record, laid out as the batch's Layout says:
 //   Pairs   Ape-X transitions, R = 8: frame j is plane j % 8 of record j / 8 (planes 0-3 of s, then of s')
-//   Strips  R2D2 frame strips, R = T + 3: frame j is the contiguous strips' frame j, of record j / R
+//   Strips  R2D2 frame strips, R = T + 3: frame j is the contiguous strips' frame j, of record j / R; and IMPALA
+//           rollouts (b2rl_dedup_attach_rollouts), R = 4 (T + 1): a rollout's `state` row is its T + 1 frame stacks
+//           back to back, so it is a strip of R frames whose stack t is frames 4t .. 4t + 3 (DESIGN.md §4.20)
 // and frame j % R of record r gets its pool id in planes[R slot(r) + j % R].
 //   1. k_dedup_hash   one warp per frame: 64-bit content key, inserted into a batch table keyed by it that keeps the
 //                     lowest position holding each key
@@ -45,6 +47,7 @@ struct DedupState {
   int32_t planes_field = -1;
   int32_t R = 8;                                  // frames per record
   Layout layout = Layout::Pairs;
+  int32_t stacks = 0;                             // b2rl_dedup_attach_rollouts: frame stacks per rollout (T + 1)
   int64_t F = 0, W = 0, T = 0;                    // pool frames, window, key-table entries (a power of two)
   unsigned long long mask = 0;
   uint8_t* pool = nullptr;                        // [F][7056] the address kernels use: device memory, or the device
@@ -295,6 +298,7 @@ const uint8_t* dedup_pool(const b2rl_replay* h) { return h->dedup->pool; }
 int64_t dedup_pool_frames(const b2rl_replay* h) { return h->dedup->F; }
 bool dedup_pool_on_host(const b2rl_replay* h) { return h->dedup->pool_host != nullptr; }
 int dedup_strip_frames(const b2rl_replay* h) { return h->dedup->layout == Layout::Strips ? h->dedup->R : 0; }
+int dedup_rollout_stacks(const b2rl_replay* h) { return h->dedup->stacks; }
 
 }  // namespace b2rl
 
@@ -408,6 +412,16 @@ extern "C" int b2rl_dedup_attach_strips_placed(b2rl_replay* h, int32_t planes_fi
                       pool_on_host != 0);
 }
 
+extern "C" int b2rl_dedup_attach_rollouts(b2rl_replay* h, int32_t planes_field, int32_t stacks_per_record,
+                                          int64_t pool_frames, int64_t window, uint64_t hash_mask) {
+  B2RL_REQUIRE(stacks_per_record >= 1 && stacks_per_record <= DD_MAX_FRAMES / 4,
+               "stacks_per_record must be in [1, 16384]");
+  const int rc = dedup_attach(h, planes_field, Layout::Strips, 4 * stacks_per_record, pool_frames, window, hash_mask,
+                              false);
+  if (rc == B2RL_OK) h->dedup->stacks = stacks_per_record;
+  return rc;
+}
+
 extern "C" int b2rl_dedup_info(const b2rl_replay* h, void** pool_dev, int64_t* head_seq, int64_t* max_batch) {
   B2RL_REQUIRE(h != nullptr, "null handle");
   B2RL_REQUIRE(h->dedup != nullptr, "not a frame-deduplicated replay (b2rl_dedup_attach)");
@@ -499,7 +513,7 @@ extern "C" int b2rl_dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8
   B2RL_REQUIRE(h != nullptr, "null handle");
   DedupState* d = h->dedup;
   B2RL_REQUIRE(d != nullptr, "not a frame-deduplicated replay (b2rl_dedup_attach)");
-  B2RL_REQUIRE(d->layout == Layout::Pairs, "a strip handle (b2rl_dedup_attach_strips) takes b2rl_dedup_push_strips");
+  B2RL_REQUIRE(d->layout == Layout::Pairs, "a strip or rollout handle (b2rl_dedup_attach_strips, _rollouts) takes b2rl_dedup_push_strips");
   B2RL_REQUIRE(n >= 0 && n <= d->max_batch, "n out of range (0..max_batch of b2rl_dedup_info)");
   if (n == 0) return B2RL_OK;
   B2RL_REQUIRE(s_dev != nullptr && ns_dev != nullptr, "null argument");

@@ -28,8 +28,9 @@ struct FrameSource {
   int64_t row_stride;            // Direct, Table: bytes between rows
   int64_t table_off;             // Table: bytes added to the entry's address (the rows of earlier split launches)
   int64_t rows;                  // indices are clamped to [0, rows)
-  int32_t plane_base;            // Planes: 0 or 4 at stride 8, 0 at stride 1
-  int32_t plane_stride;          // Planes: 8 (Ape-X s / s') or 1 (the windows of R2D2 strip records)
+  int32_t plane_base;            // Planes: 0 or 4 at stride 8, 0 at strides 1 and 4
+  int32_t plane_stride;          // Planes: 8 (Ape-X s / s'), 1 (the windows of R2D2 strip records) or 4 (the stacks
+                                 // of IMPALA rollout records)
 };
 
 // Frame c of plane-table row `row`: pool ids are `stride` apart from row to row.
@@ -75,9 +76,10 @@ inline int check_frames(const b2rl_frames* f, FrameSource& src, FrameKind& kind)
     B2RL_REQUIRE((uintptr_t)f->pool % 16 == 0 && (uintptr_t)f->planes % 4 == 0,
                  "the frame pool must be 16-byte aligned, the plane table 4-byte aligned");
     const int32_t stride = f->plane_stride == 0 ? 8 : f->plane_stride;
-    B2RL_REQUIRE(stride == 8 || stride == 1, "plane_stride must be 0 or 8 (Ape-X s / s') or 1 (strip windows)");
+    B2RL_REQUIRE(stride == 8 || stride == 1 || stride == 4,
+                 "plane_stride must be 0 or 8 (Ape-X s / s'), 1 (strip windows) or 4 (rollout stacks)");
     if (stride == 8) B2RL_REQUIRE(f->plane_base == 0 || f->plane_base == 4, "plane_base must be 0 or 4");
-    else B2RL_REQUIRE(f->plane_base == 0, "plane_base must be 0 at plane_stride 1");
+    else B2RL_REQUIRE(f->plane_base == 0, "plane_base must be 0 at plane_stride 1 or 4");
     kind = FrameKind::Planes;
     src.base = f->pool, src.planes = f->planes, src.plane_base = f->plane_base, src.plane_stride = stride;
     return B2RL_OK;

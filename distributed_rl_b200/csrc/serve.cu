@@ -442,7 +442,10 @@ extern "C" int b2rl_serve_fill_uniform(b2rl_replay* h, b2rl_serve_ring* r, int32
   int rc = fill_slot_ptrs(h, r, slot, ptrs);
   if (rc != B2RL_OK) return rc;
   B2RL_REQUIRE(steps >= 1, "steps must be >= 1");
-  B2RL_REQUIRE(h->dedup == nullptr, "a frame-deduplicated replay serves prioritized minibatches, not rollouts");
+  B2RL_REQUIRE(h->dedup == nullptr || dedup_rollout_stacks(h) > 0,
+               "a frame-deduplicated replay serves prioritized minibatches, not rollouts");
+  B2RL_REQUIRE(h->dedup == nullptr || dedup_rollout_stacks(h) == steps + 1,
+               "the rollout frame pool holds steps + 1 frame stacks per rollout: steps does not match it");
   B2RL_REQUIRE(!h->any_on_host, "a replay with fields placed on the host serves prioritized minibatches only");
   const int64_t n = r->L.batch, size = h->size, cap = h->capacity;
   B2RL_REQUIRE(n <= size, "sample larger than population: the batch exceeds the stored records");
@@ -453,6 +456,11 @@ extern "C" int b2rl_serve_fill_uniform(b2rl_replay* h, b2rl_serve_ring* r, int32
   SmallRows rows{};
   for (int f = 0; f < h->n_fields; ++f) {
     const int64_t b = h->field_bytes[f];
+    if (h->dedup != nullptr && f == dedup_planes_field(h)) {   // the stacks assembled from the frame pool
+      P.add_planes_time_major(dedup_pool(h), (const int32_t*)h->field[f], dedup_strip_frames(h), steps + 1,
+                              (uint8_t*)ptrs[3 + f]);
+      continue;
+    }
     RolloutField kind;
     const char* bad = rollout_field(b, steps, kind);
     B2RL_REQUIRE(bad == nullptr, bad);

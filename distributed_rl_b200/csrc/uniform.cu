@@ -1,7 +1,9 @@
 // b2rl_uniform_fetch: the minibatch of IMPALA's captured in-process learner step (impala.Learner.fused_step with
 // use_graph) in ONE launch.  The draw of b2rl_serve_fill_uniform (uniform.cuh) over the ring's valid region, written
 // into the step's fixed buffers instead of a ring slot: idx, action / mu / reward time-major, done, and conv_1's
-// time-major frame rows.  The frames themselves are not copied: conv_1 reads them in place in the replay payload.
+// time-major frame rows.  The frames themselves are not copied: conv_1 reads them in place in the replay payload, or
+// for a frame-deduplicated rollout store (b2rl_dedup_attach_rollouts) through its plane table at stride 4, whose row
+// numbering is the same.
 //
 // Replaces Replay.draw (torch.randperm on a torch generator) + DeviceReplay.gather of the small fields + the
 // transposes and time_major_rows of impala.Learner.fused_step, whose host-side arguments a CUDA graph would bake in.
@@ -61,14 +63,22 @@ extern "C" int b2rl_uniform_fetch(b2rl_replay* h, int64_t n, int32_t steps, int6
   const int64_t size = h->size;
   B2RL_REQUIRE(n <= size, "sample larger than population: n exceeds the stored records");
   B2RL_REQUIRE(size <= (1LL << 32), "a uniform draw is from at most 2^32 records");
+  B2RL_REQUIRE(h->dedup == nullptr || dedup_rollout_stacks(h) == steps + 1,
+               h->dedup == nullptr || dedup_rollout_stacks(h) == 0
+                   ? "a frame-deduplicated replay of transitions or sequences holds no rollouts"
+                   : "the rollout frame pool holds steps + 1 frame stacks per rollout: steps does not match it");
   SmallFields small{};
   SmallRows rows{};
   for (int f = 0; f < h->n_fields; ++f) {
     const int64_t b = h->field_bytes[f];
+    uint8_t* out = fields_out_dev ? (uint8_t*)fields_out_dev[f] : nullptr;
+    if (h->dedup != nullptr && f == dedup_planes_field(h)) {   // the rollout's stacks, read through its pool ids
+      B2RL_REQUIRE(out == nullptr, "frames are read in place: a frame field takes frame rows, not a buffer");
+      continue;
+    }
     RolloutField kind;
     const char* bad = rollout_field(b, steps, kind);
     B2RL_REQUIRE(bad == nullptr, bad);
-    uint8_t* out = fields_out_dev ? (uint8_t*)fields_out_dev[f] : nullptr;
     if (kind == RolloutField::FRAMES) {
       B2RL_REQUIRE(out == nullptr, "frames are read in place: a frame field takes frame rows, not a buffer");
     } else if (out == nullptr) {

@@ -49,13 +49,47 @@ class ImpalaConfig:
     DENSE_3XTF32: bool = True    # the 2592 -> 256 layer as a 3xTF32 wgmma GEMM (csrc/gemm.cu) instead of an fp32 SIMT sgemm
     SERVED_FUSED_STEP: bool = False  # on a served replay (DeviceReplayClient), run() steps a captured step on the
                                      # bound ring slot instead of sample() -> train()
+    FRAME_DEDUP: bool = False    # store every distinct frame once, in a pool of FRAMES_PER_ROLLOUT frames per slot
+                                 # (R.RolloutDedupReplay, DESIGN §4.20): overlapping stacks, the bootstrap stack and
+                                 # the padding of short rollouts share their frames.  Draws and samples are a stack
+                                 # store's.
+    FRAMES_PER_ROLLOUT: float = 24.0
+    DEDUP_WINDOW: int = 1 << 14  # a frame is reused only from the last DEDUP_WINDOW frames stored (at most 1/8 of the
+                                 # pool, see dedup_geometry)
 
     @staticmethod
     def from_configuration():
         import configuration as C
         names = ("BATCHSIZE", "ACTION_SIZE", "GAMMA", "C_LAMBDA", "C_VALUE", "P_VALUE", "ENTROPY_R", "UNROLL_STEP",
                  "REPLAY_MEMORY_LEN", "BUFFER_SIZE", "LEARNER_DEVICE", "REDIS_SERVER", "OPTIM_INFO", "MODEL")
-        return ImpalaConfig(LOG_W=getattr(C, "LOG_W", None), **{k: getattr(C, k) for k in names})
+        kw = {k: getattr(C, k) for k in names}
+        for k in ("FRAME_DEDUP", "FRAMES_PER_ROLLOUT", "DEDUP_WINDOW"):      # optional keys of cfg/impala.json
+            if hasattr(C, k):
+                kw[k] = getattr(C, k)
+        return ImpalaConfig(LOG_W=getattr(C, "LOG_W", None), **kw)
+
+
+def dedup_geometry(cfg: ImpalaConfig) -> tuple:
+    """(pool frames, window) of a FRAME_DEDUP replay: ceil(FRAMES_PER_ROLLOUT * REPLAY_MEMORY_LEN) frames, and
+    DEDUP_WINDOW capped at an eighth of them (as apex.dedup_geometry and r2d2.dedup_geometry).  A slot stays live until
+    pool - window frames have been stored after it: at the default 24 frames per slot, 21 REPLAY_MEMORY_LEN frames or
+    more, above the ~T = 20 new frames per rollout the reference actors send, so the slot ring wraps first.  The window
+    only has to reach back two rollouts of the same actor (the bootstrap stack and checkLength's padding)."""
+    import math
+    import warnings
+    F = int(math.ceil(cfg.FRAMES_PER_ROLLOUT * cfg.REPLAY_MEMORY_LEN))
+    W = min(int(cfg.DEDUP_WINDOW), F // 8)
+    if W < cfg.DEDUP_WINDOW:
+        warnings.warn(f"DEDUP_WINDOW = {cfg.DEDUP_WINDOW} frames is more than an eighth of the {F}-frame pool: the "
+                      f"frame-deduplicated replay uses a window of {W} frames", stacklevel=2)
+    return F, W
+
+
+def rollout_frames(store):
+    """conv_1's frame rows over a rollout store's `state`, row slot * (T + 1) + t being stack t of the slot: the
+    field viewed as one stack per row, or a RolloutDedupReplay's plane table."""
+    src = store.frame_source("state")
+    return src if isinstance(src, R.PlaneFrames) else src.view(-1, 4, 84, 84)
 
 
 class Replay(ReplayThread):
@@ -66,7 +100,11 @@ class Replay(ReplayThread):
 
     def __init__(self, cfg: ImpalaConfig | None = None, connect=None):
         super().__init__(cfg or ImpalaConfig.from_configuration(), connect)
-        self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, R.impala_fields(self.cfg.UNROLL_STEP), self.device)
+        if self.cfg.FRAME_DEDUP:
+            self.store = R.RolloutDedupReplay(self.cfg.REPLAY_MEMORY_LEN, *dedup_geometry(self.cfg),
+                                              T=self.cfg.UNROLL_STEP, device=self.device)
+        else:
+            self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, R.impala_fields(self.cfg.UNROLL_STEP), self.device)
         self._rng = torch.Generator(device=self.device)        # uniform sampling stream (random.sample in the reference)
         self._rng.manual_seed(0x1A9A1A)
 
@@ -167,7 +205,8 @@ class Learner(CapturedStep):
         """One learner step with everything resident: draw B rollouts uniformly without replacement
         (random.sample, baseline/utils.py:310-315), gather only a / mu / r / done (244 B of the 593 KB rollout),
         run conv_1 over the rollouts' (T+1) frames IN PLACE in the replay payload (row = slot * (T+1) + t,
-        time-major), V-trace kernel, loss, backward, clip + RMSprop.
+        time-major; with FRAME_DEDUP through the store's plane table, rollout_frames), V-trace kernel, loss, backward,
+        clip + RMSprop.
         `use_graph`: the step as a CUDA graph (_captured_step), its draw one launch of DeviceReplay.uniform_fetch
         before each replay.  -> `last` (for the graph: its static buffers, plus `idx`)."""
         if use_graph:
@@ -178,7 +217,7 @@ class Learner(CapturedStep):
         st = mem.store
         if not hasattr(self, "_small"):
             self._small = st.alloc_batch(B, ("action", "mu", "reward", "done"))
-            self._frames = st.field_view("state").view(-1, 4, 84, 84)
+            self._frames = rollout_frames(st)
             self._t_idx = torch.arange(T + 1, device=self.device).view(T + 1, 1)
         idx = mem.draw(B)
         b = st.gather(idx, self._small)
@@ -383,7 +422,8 @@ class _DrawnRollouts:
     """The fixed buffers of the captured in-process step (fused_step(use_graph=True)), built once before its first
     warm-up, and the stream it is warmed up and captured on.  DeviceReplay.uniform_fetch draws into `cur`: idx (B,),
     action / mu / reward (T, B), done (B,) and `rows`, the (T+1) * B time-major rows of the drawn rollouts' frames in
-    `frames`, the replay's `state` field with one frame stack per row (row = slot * (T+1) + t)."""
+    `frames`, the replay's `state` field with one frame stack per row (row = slot * (T+1) + t), or with FRAME_DEDUP
+    the store's plane table with the same rows (rollout_frames)."""
 
     def __init__(self, L: "Learner"):
         c, dev = L.cfg, L.device
@@ -394,7 +434,7 @@ class _DrawnRollouts:
         self.stream = torch.cuda.Stream(dev)
         self.cur = _rollout_buffers(T, B, dev)
         self.cur["rows"] = torch.empty((T + 1) * B, dtype=torch.int64, device=dev)
-        self.frames = L._memory.store.field_view("state").view(-1, 4, 84, 84)
+        self.frames = rollout_frames(L._memory.store)
 
 
 def _rollout_buffers(T: int, B: int, dev) -> dict:

@@ -163,6 +163,13 @@ def impala_fields(T: int = 20):
     )
 
 
+def IMPALA_DEDUP_FIELDS(T: int = 20):
+    """The slot of the frame-deduplicated IMPALA store (ImpalaConfig.FRAME_DEDUP, DESIGN.md §4.20): `planes`, the
+    4 (T + 1) int32 pool ids of the rollout's T + 1 frame stacks (frame c of stack t is pool frame planes[4 t + c]),
+    then the small fields of impala_fields."""
+    return (Field("planes", torch.int32, (4 * (T + 1),)),) + impala_fields(T)[1:]
+
+
 def _stream_ptr(device: torch.device) -> int:
     return torch.cuda.current_stream(device).cuda_stream
 
@@ -640,8 +647,9 @@ class StripDedupReplay(DedupReplay):
         n = pr.numel()
         small = _small_rows(self.RECORD_FIELDS[1:], fields[1:], n)
         t = torch.as_tensor(fields[0])
-        row = (self.T + 3) * FRAME_BYTES
-        assert t.dtype == torch.uint8 and t.numel() == n * row, "frame strips must be uint8 (n, T + 3, 84, 84)"
+        row = self.RECORD_FIELDS[0].nbytes
+        assert t.dtype == torch.uint8 and t.numel() == n * row, \
+            f"frames must be uint8 ({n}, {', '.join(map(str, self.RECORD_FIELDS[0].shape))})"
         strips = t.reshape(n, row).to(self.device, non_blocking=True).contiguous()
         ptrs = (C.c_void_p * _lib.MAX_FIELDS)()
         for a in range(0, n, self.max_batch):
@@ -677,6 +685,33 @@ class StripDedupReplay(DedupReplay):
             raise ValueError("conv_1 reads its frame rows in place on the GPU: a frame pool in host memory (host_pool) "
                              "has no frame source; gather the sampled strips into device memory first")
         return PlaneFrames(self.pool, self.field_view("planes"), 0, 1)
+
+
+class RolloutDedupReplay(StripDedupReplay):
+    """The rollout form of StripDedupReplay (b2rl_dedup_attach_rollouts, ImpalaConfig.FRAME_DEDUP, DESIGN.md §4.20): an
+    IMPALA replay whose slots hold IMPALA_DEDUP_FIELDS(T), the 4 (T + 1) frames of each rollout's T + 1 stacks living
+    in the frame pool.  A stack repeats three frames of the one before it, a rollout's bootstrap stack is the first
+    stack of the same actor's next rollout, and a rollout cut short at an episode end is padded with the previous
+    rollout's stacks (IMPALA/Player.py:88-203), so about T of the 4 (T + 1) frames are new.  push / gather /
+    uniform_fetch take and return what a DeviceReplay of impala_fields(T) does, bit for bit, while every slot is live;
+    the liveness rule and the refusals are DedupReplay's, and the frame pool stays in HBM."""
+
+    def __init__(self, capacity: int, pool_frames: int, window: int, T: int = 20, device="cuda:0",
+                 hash_mask: int = DEDUP_HASH_MASK):
+        DeviceReplay.__init__(self, capacity, IMPALA_DEDUP_FIELDS(T), device)
+        self.T = int(T)
+        self.RECORD_FIELDS = impala_fields(self.T)
+        self.host_pool = False
+        check(self.lib.b2rl_dedup_attach_rollouts(self._h, 0, self.T + 1, int(pool_frames), int(window),
+                                                  int(hash_mask)))
+        self._attached(pool_frames, window)
+
+    def frame_source(self, name: str) -> "PlaneFrames":
+        """conv_1's rows of `state`: every slot's stacks, row slot * (T + 1) + t being stack t of the slot (the row
+        numbering of a stack store's state field viewed as (capacity * (T + 1), 4, 84, 84))."""
+        if name != "state":
+            raise KeyError(name)
+        return PlaneFrames(self.pool, self.field_view("planes"), 0, 4)
 
 
 # ---- stateless target kernels -------------------------------------------------
@@ -796,8 +831,9 @@ class PlaneFrames:
     """Frame stacks held as a plane table over a frame pool: row r is the stack whose channel c is pool frame
     planes.flatten()[plane_stride * r + base + c].  `pool`: uint8 (F, 84, 84).  DedupReplay: `planes` int32 (slots,
     8), plane_stride 8, `base` 0 for `state` and 4 for `next_state`.  StripDedupReplay: `planes` int32 (slots, T + 3),
-    plane_stride 1, base 0, so row slot * (T + 3) + t is stack t of the slot's strip.  conv1_fused / conv1_wgrad read
-    the four frames of each row in place."""
+    plane_stride 1, base 0, so row slot * (T + 3) + t is stack t of the slot's strip.  RolloutDedupReplay: `planes`
+    int32 (slots, 4 (T + 1)), plane_stride 4, base 0, so row slot * (T + 1) + t is stack t of the slot's rollout.
+    conv1_fused / conv1_wgrad read the four frames of each row in place."""
     pool: torch.Tensor
     planes: torch.Tensor
     base: int
@@ -809,8 +845,8 @@ class PlaneFrames:
 
     @property
     def rows(self) -> int:
-        """The rows whose four pool ids lie inside `planes`: every slot at stride 8; at stride 1 every window but the
-        last three, which would run past the table's end."""
+        """The rows whose four pool ids lie inside `planes`: every slot at stride 8, every stack at stride 4; at
+        stride 1 every window but the last three, which would run past the table's end."""
         return (self.planes.numel() - self.base - 4) // self.plane_stride + 1
 
 
@@ -837,7 +873,7 @@ def _frame_source(frames) -> _lib.Frames:
 def conv1_fused(frames, idx, pack: Conv1Pack, relu: bool = False, out=None):
     """frames: uint8 (rows, 4, 84, 84) with its inner three dimensions contiguous: frame stacks (e.g.
     DeviceReplay.field_view("state")), the windows of frame strips (strip_windows), a BoundFrames or a PlaneFrames
-    (DedupReplay.frame_source, StripDedupReplay.frame_source);
+    (DedupReplay.frame_source, StripDedupReplay.frame_source, RolloutDedupReplay.frame_source);
     idx: int64[n] rows to take (None: all rows in order).
     -> list of n_nets tensors (n, c_out, 20, 20) fp32 in channels_last memory format."""
     src = _frame_source(frames)

@@ -36,6 +36,10 @@ elif ALG == "IMPALA":
     C_VALUE = DATA["C_VALUE"]
     P_VALUE = DATA["P_VALUE"]
     ENTROPY_R = DATA["ENTROPY_R"]
+    FRAME_DEDUP = bool(DATA.get("FRAME_DEDUP", False))   # not a reference key: store every distinct frame once
+    for _k in ("FRAMES_PER_ROLLOUT", "DEDUP_WINDOW"):
+        if _k in DATA:
+            globals()[_k] = DATA[_k]
 
 use_per = ALG != "IMPALA"
 if use_per:

@@ -227,7 +227,7 @@ int b2rl_replay_gather(b2rl_replay* h, const int64_t* idx_dev, int64_t n,
  * Pushes may come from different streams: each one waits for the previous one's work before it starts.  The host
  * calls themselves must not overlap (one thread at a time, as for every entry point on a handle).
  * b2rl_replay_push, _reserve, _ingest_pipelined, _fill_hash, b2rl_tree_build and b2rl_serve_fill_uniform refuse a
- * dedup replay.  b2rl_serve_ring_create / b2rl_serve_fill serve it with the stack store's record layout: the planes
+ * dedup replay (b2rl_serve_fill_uniform serves a rollout handle, b2rl_dedup_attach_rollouts below).  b2rl_serve_ring_create / b2rl_serve_fill serve it with the stack store's record layout: the planes
  * field becomes two (B, 4, 84, 84) frame-stack fields (s, then s') in the ring slot, assembled from the pool.
  *
  * b2rl_dedup_info: *pool_dev (the frame pool), *head_seq (frames stored so far), *max_batch (records per push).
@@ -245,7 +245,19 @@ int b2rl_replay_gather(b2rl_replay* h, const int64_t* idx_dev, int64_t n,
  * (n, R, 84, 84) uint8.  Each push refuses the other kind of handle; b2rl_dedup_info serves both, and so do the
  * refusals above.  b2rl_replay_gather_planes on a strip handle: stacks_out_dev[0] receives the (n, R, 84, 84)
  * strips assembled from the pool and stacks_out_dev[1] must be NULL.  b2rl_serve_ring_create / b2rl_serve_fill
- * serve it with the strip store's record layout: the planes field becomes the (B, R, 84, 84) strip field. */
+ * serve it with the strip store's record layout: the planes field becomes the (B, R, 84, 84) strip field.
+ *
+ * The same pool for IMPALA rollouts.  IMPALA/Player.py:88-95 stacks the last four frames, so stack t + 1 repeats three
+ * frames of stack t; a rollout's bootstrap stack is the first stack of the same actor's next rollout (:181-203); and
+ * checkLength (:116-125) pads a short rollout with the previous rollout's stacks.  A rollout's `state` row (T + 1
+ * stacks of 28 224 bytes, IMPALA/ReplayMemory.py:34-43) is R = 4 (T + 1) frames back to back, stack t being frames
+ * 4t .. 4t + 3.  b2rl_dedup_attach_rollouts is b2rl_dedup_attach_strips with R = 4 stacks_per_record (T + 1) that
+ * also marks the handle as holding rollouts; it takes b2rl_dedup_push_strips with strips_dev the device (n, T + 1,
+ * 28 224) uint8 rows, and b2rl_replay_gather_planes / b2rl_serve_fill as for a strip handle (the slot's row is the
+ * stack store's `state` row).  Unlike every other dedup replay it is also drawn by b2rl_uniform_fetch (its planes
+ * field takes no buffer; the frame rows are those of a stack store, read through plane_stride 4 of b2rl_frames) and
+ * b2rl_serve_fill_uniform (the slot's `state` field holds the time-major stacks assembled from the pool, byte for
+ * byte the stack store's slot); both require steps + 1 == stacks_per_record.  It has no host-pool form. */
 int b2rl_dedup_attach(b2rl_replay* h, int32_t planes_field, int64_t pool_frames, int64_t window, uint64_t hash_mask);
 int b2rl_dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8_t* ns_dev, const void* const* fields_src,
                     const float* prios, int64_t n, void* stream);
@@ -253,6 +265,8 @@ int b2rl_dedup_attach_strips(b2rl_replay* h, int32_t planes_field, int32_t frame
                              int64_t window, uint64_t hash_mask);
 int b2rl_dedup_push_strips(b2rl_replay* h, const uint8_t* strips_dev, const void* const* fields_src,
                            const float* prios, int64_t n, void* stream);
+int b2rl_dedup_attach_rollouts(b2rl_replay* h, int32_t planes_field, int32_t stacks_per_record, int64_t pool_frames,
+                               int64_t window, uint64_t hash_mask);
 int b2rl_dedup_info(const b2rl_replay* h, void** pool_dev, int64_t* head_seq, int64_t* max_batch);
 
 /* The strip store of R2D2/ReplayMemory.py:70-88 behind PER.__init__ (baseline/PER.py:49-66), with the frame pool
@@ -341,6 +355,8 @@ int b2rl_vtrace(const float* pi_a_dev, const float* mu_a_dev, const float* value
  *           plane_stride 0 means 8, the Ape-X layout: plane_base 0 reads `state`, 4 `next_state` of the transition
  *           APE_X/Player.py:252-261 sends.  plane_stride 1 (plane_base 0) reads the overlapping windows of R2D2 strip
  *           records, whose T + 3 pool ids per slot are consecutive: row slot * (T + 3) + t is stack t of the slot.
+ *           plane_stride 4 (plane_base 0) reads the stacks of IMPALA rollout records (b2rl_dedup_attach_rollouts),
+ *           4 (T + 1) pool ids per slot: row slot * (T + 1) + t is stack t of the slot, as in a stack store.
  * row_stride (base and table) must be a positive multiple of 16.  Row indices are clamped to [0, rows), rows >= 1:
  * the caller guarantees that row rows - 1 ends inside the allocation. */
 typedef struct {
@@ -540,7 +556,9 @@ int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, uint64_t s
  * layout, with steps = T: a bulk row of (T + 1) equal steps -> step t of draw k at row t * B + k; a row of T 4-byte
  * words -> word t of draw k at t * B + k; a 1/2/4/8-byte scalar -> row k.  idx is written, w is not (uniform replay
  * has no IS weights), the header {seq, B} last.  Same slot layout and ring as b2rl_serve_fill.  An error, and no
- * launch, when B > size or the ring was not created for h. */
+ * launch, when B > size or the ring was not created for h.  Of the frame-deduplicated replays it serves the rollout
+ * handle (b2rl_dedup_attach_rollouts) only, assembling each drawn rollout's T + 1 stacks from the frame pool in the
+ * same launch. */
 int b2rl_serve_fill_uniform(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, uint64_t seq, int32_t steps,
                             void* stream);
 /* Replay_Server.sample (APE_X/ReplayMemory.py:251-257) without the unpickle: copy minibatch slot k (slot_bytes,
