@@ -61,6 +61,8 @@ SIGNATURES = {
     "b2rl_tree_update": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_vp]),
     "b2rl_tree_stats": (C.c_int, [c_vp, c_f32, c_vp, c_vp, c_vp]),
     "b2rl_tree_leaves": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_vp]),
+    "b2rl_tree_level": (C.c_int, [c_vp, c_i32, C.POINTER(c_i64), C.POINTER(c_i32), C.POINTER(c_i32), c_vp, c_vp,
+                                  c_vp]),
     "b2rl_replay_gather": (C.c_int, [c_vp, c_vp, c_i64, C.POINTER(c_vp), c_vp]),
     "b2rl_uniform_fetch": (C.c_int, [c_vp, c_i64, c_i32, c_vp, C.POINTER(c_vp), c_vp, c_vp]),
     "b2rl_apex_target": (C.c_int, [c_vp] * 7 + [c_i32, c_i32, c_f32, c_f32] + [c_vp] * 6),

@@ -706,3 +706,23 @@ extern "C" int b2rl_tree_leaves(b2rl_replay* h, int64_t start, int64_t n, float*
   B2RL_CHECK_LAUNCH();
   return B2RL_OK;
 }
+
+extern "C" int b2rl_tree_level(const b2rl_replay* h, int32_t k, int64_t* n_nodes, int32_t* levels, int32_t* top_bits,
+                               double* sums_out_dev, float* mins_out_dev, void* stream) {
+  B2RL_REQUIRE(h != nullptr, "null handle");
+  B2RL_REQUIRE(n_nodes != nullptr, "null n_nodes");
+  const TreeView& t = h->tree;
+  B2RL_REQUIRE(k >= 0 && k <= t.G, "no such stored level (0..G)");
+  if (levels) *levels = t.G;
+  if (top_bits) *top_bits = t.top_bits;
+  if (k == 0) { *n_nodes = t.cap2; return B2RL_OK; }
+  const int64_t nk = (k == t.G) ? 1 : (t.cap2 >> (4 * k));
+  *n_nodes = nk;
+  DeviceGuard g(h->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (sums_out_dev)
+    B2RL_CUDA(cudaMemcpyAsync(sums_out_dev, t.sum + t.off[k], sizeof(double) * (size_t)nk, cudaMemcpyDeviceToDevice, st));
+  if (mins_out_dev)
+    B2RL_CUDA(cudaMemcpyAsync(mins_out_dev, t.minv + t.off[k], sizeof(float) * (size_t)nk, cudaMemcpyDeviceToDevice, st));
+  return B2RL_OK;
+}

@@ -471,6 +471,25 @@ class DeviceReplay:
         check(self.lib.b2rl_tree_leaves(self._h, start, n, out.data_ptr(), self._st()))
         return out
 
+    def tree_shape(self) -> tuple:
+        """-> (cap2, G, top_bits): the tree's leaves (a power of two >= capacity), its stored internal levels and the
+        binary levels its top group spans (b2rl_tree_level)."""
+        n, g, tb = C.c_int64(), C.c_int32(), C.c_int32()
+        check(self.lib.b2rl_tree_level(self._h, 0, C.byref(n), C.byref(g), C.byref(tb), None, None, None))
+        return n.value, g.value, tb.value
+
+    def tree_level(self, k: int) -> tuple:
+        """Stored level k in 1..G of the sum-tree -> (sums fp64[n], mins fp32[n]) device tensors, n = cap2 >> 4k
+        (1 at k = G: the root).  Level k holds the binary tree's nodes at height 4k; level 0, the leaves, is
+        priorities()."""
+        n = C.c_int64()
+        check(self.lib.b2rl_tree_level(self._h, int(k), C.byref(n), None, None, None, None, None))
+        sums = torch.empty(n.value, dtype=torch.float64, device=self.device)
+        mins = torch.empty(n.value, dtype=torch.float32, device=self.device)
+        check(self.lib.b2rl_tree_level(self._h, int(k), C.byref(n), None, None, sums.data_ptr(), mins.data_ptr(),
+                                       self._st()))
+        return sums, mins
+
     # -- gather ----------------------------------------------------------------
     def alloc_batch(self, n: int, names: Sequence[str] | None = None):
         return alloc_rows(self.fields, n, self.device, names)

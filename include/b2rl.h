@@ -200,6 +200,14 @@ int b2rl_tree_stats(b2rl_replay* h, float beta, double* stats_out_dev, float* ma
  * [start, start+n) as fp32. */
 int b2rl_tree_leaves(b2rl_replay* h, int64_t start, int64_t n, float* out_dev, void* stream);
 
+/* Stored level k of the sum-tree, for tests and diagnostics: the internal node values (Node._reduce,
+ * baseline/sumtree.py:21-27) that every draw descends through.  k = 0 fills the shape only: *n_nodes = cap2 (the
+ * leaves), *levels = G (stored internal levels), *top_bits = binary levels spanned by the top group.  For k in
+ * 1..G, *n_nodes = cap2 >> 4k (1 at k = G, the root), and the nodes' fp64 sums and fp32 minima are copied on
+ * `stream` into sums_out_dev / mins_out_dev when those are not null.  levels / top_bits may be NULL.  No kernel. */
+int b2rl_tree_level(const b2rl_replay* h, int32_t k, int64_t* n_nodes, int32_t* levels, int32_t* top_bits,
+                    double* sums_out_dev, float* mins_out_dev, void* stream);
+
 /* Minibatch assembly of Replay.buffer (APE_X/ReplayMemory.py:61-116,
  * R2D2/ReplayMemory.py:53-122, IMPALA/ReplayMemory.py:30-54): for every
  * field f with out_fields[f] != NULL copy row idx[k] to out_fields[f] + k *

@@ -53,6 +53,14 @@ def test_invalid_arguments_are_reported_not_crashed(lib):
     h = ctypes.c_void_p()
     assert lib.b2rl_replay_create(ctypes.byref(d), ctypes.byref(h)) < 0
     assert lib.b2rl_apex_target(*([None] * 7), 0, 0, 0.0, 0.0, *([None] * 6)) < 0
+    # the stored-level read-back refuses a null handle or a null n_nodes before it looks at the tree (a level
+    # outside 0..G is refused on a live handle: tests/test_gpu_30_tree_at_scale.py)
+    n, g, tb = ctypes.c_int64(-1), ctypes.c_int32(-1), ctypes.c_int32(-1)
+    for k in (0, 1, -1, 99):
+        assert lib.b2rl_tree_level(None, k, ctypes.byref(n), ctypes.byref(g), ctypes.byref(tb), None, None, None) < 0
+        assert b"null handle" in lib.b2rl_last_error()
+        assert lib.b2rl_tree_level(None, k, None, None, None, None, None, None) < 0
+    assert (n.value, g.value, tb.value) == (-1, -1, -1)      # nothing written on a refusal
 
 
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):
