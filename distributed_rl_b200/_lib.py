@@ -83,6 +83,10 @@ SIGNATURES = {
     "b2rl_dedup_attach_strips_placed": (C.c_int, [c_vp, c_i32, c_i32, c_i64, c_i64, c_u64, c_i32]),
     "b2rl_dedup_attach_rollouts": (C.c_int, [c_vp, c_i32, c_i32, c_i64, c_i64, c_u64]),
     "b2rl_dedup_pool_placement": (C.c_int, [c_vp, C.POINTER(c_i32), C.POINTER(c_vp)]),
+    "b2rl_dedup_attach_strips_coded": (C.c_int, [c_vp, c_i32, c_i32, c_i64, c_i64, c_u64, c_i64]),
+    "b2rl_dedup_codec_stats": (C.c_int, [c_vp, C.POINTER(c_i64), C.POINTER(c_i64), C.POINTER(c_i64)]),
+    "b2rl_frame_encode": (C.c_int, [c_vp, c_i64, c_vp, c_vp, c_vp]),
+    "b2rl_frame_decode": (C.c_int, [c_vp, c_i64, c_vp, c_vp]),
     "b2rl_replay_gather_planes": (C.c_int, [c_vp, c_vp, c_i64, C.POINTER(c_vp), C.POINTER(c_vp), c_vp]),
     "b2rl_rmsprop_step": (C.c_int, [C.POINTER(c_vp), C.POINTER(c_vp), C.POINTER(c_vp), C.POINTER(c_vp),
                                     C.POINTER(c_i64), c_i32, c_f64, c_f64, c_f64, c_i32, C.POINTER(c_i64), c_vp, c_vp,

@@ -22,7 +22,13 @@
 // The kernels are the same: k_dedup_resolve compares a hit's frame and k_dedup_copy stores the misses through the
 // pool's device alias with plain 16-byte loads and stores, over PCIe, in order on the push's stream.  The key
 // tables, pool_key and the batch scratch stay in HBM.
+// A strip handle's pool may instead be a ring of P 16-byte units holding each frame losslessly encoded
+// (b2rl_dedup_attach_strips_coded, frame_codec.cuh, DESIGN.md §4.21).  Frame seq's entry seq % F is then a descriptor
+// (absolute unit offset, length) and the same ids name it.  k_coded_resolve compares a hit's encoding with the frame
+// by decoding it, and sizes the misses; k_coded_offsets lays them out in the unit ring (a frame never straddles its
+// end); k_coded_copy encodes them in place.  The readers decode each sampled slot's frames (k_decode_planes).
 #include "common.cuh"
+#include "frame_codec.cuh"
 
 #include <new>
 #include <vector>
@@ -70,6 +76,14 @@ struct DedupState {
   cudaEvent_t done = nullptr;                     // recorded behind each push: the next one waits for it, so pushes
                                                   // on different streams never share the scratch or the key table
   std::vector<int64_t> ins;                       // per slot: head at the start of the batch that inserted it
+  // b2rl_dedup_attach_strips_coded: pool is a ring of P 16-byte units of encoded frames, then FC_RAW_BYTES of zeros
+  int64_t P = 0;                                  // 0: frames stored raw, frame seq at pool + (seq % F) 7056
+  int64_t units = 0;                              // units written so far, wrap padding included
+  int64_t* foff = nullptr;                        // [F] absolute unit offset of the frame in each entry
+  int32_t* flen = nullptr;                        // [F] its length in units
+  int32_t* usz = nullptr;                         // [R max_batch] units of each miss's encoding
+  int64_t* uoff = nullptr;                        // [R max_batch] absolute unit offset of each miss
+  std::vector<int64_t> uins;                      // per slot: units at the start of the batch that inserted it
 };
 
 __host__ __device__ __forceinline__ uint64_t mix64(uint64_t z) {   // splitmix64's finaliser
@@ -279,13 +293,194 @@ k_dedup_rebuild(const unsigned long long* __restrict__ pool_key, int64_t F, int6
   atomicMax(tseq + claim(tkey, T, pool_key[q % F]), (unsigned long long)(q + 1));
 }
 
+// ---- the coded pool (b2rl_dedup_attach_strips_coded): frames as frame_codec.cuh encodings in a ring of P units ----
+
+// k_dedup_resolve for a coded pool (strips): a hit's stored encoding is decoded and compared with the frame, and
+// every miss gets the length of its encoding in usz.
+struct CodedResolveArgs {
+  const uint8_t* s;
+  int64_t frames;
+  const unsigned long long* key;
+  const unsigned long long* bkey;
+  const int32_t* bpos;
+  int64_t BT;
+  const unsigned long long* tkey;
+  const unsigned long long* tseq;
+  int64_t T;
+  const uint8_t* pool;
+  int64_t P;
+  const int64_t* foff;
+  int64_t F;
+  int64_t oldest;           // head - W: the oldest seq a hit may reuse
+  int32_t* rep;
+  int64_t* fseq;
+  int32_t* usz;
+};
+
+__global__ void __launch_bounds__(DD_THREADS)
+k_coded_resolve(const __grid_constant__ CodedResolveArgs A) {
+  __shared__ FcRows s_rows[DD_THREADS / 32];
+  const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (j >= A.frames) return;
+  const unsigned long long k = A.key[j];
+  const uint8_t* me = A.s + j * DD_FRAME;
+  const int32_t first = A.bpos[find(A.bkey, A.BT, k)];
+  if (first < j && warp_equal(A.s + (int64_t)first * DD_FRAME, me, lane)) {
+    if (lane == 0) { A.rep[j] = first; A.fseq[j] = -2; }
+    return;
+  }
+  int64_t cand = -1;
+  if (lane == 0) {
+    const int64_t e = find(A.tkey, A.T, k);
+    if (e >= 0) {
+      const unsigned long long s1 = A.tseq[e];
+      if (s1 > 0 && (int64_t)(s1 - 1) >= A.oldest) cand = (int64_t)(s1 - 1);
+    }
+  }
+  cand = __shfl_sync(0xffffffffu, cand, 0);
+  const bool hit = cand >= 0 && fc_equal(A.pool + (A.foff[cand % A.F] % A.P) * 16, me, s_rows[threadIdx.x >> 5], lane);
+  const int units = hit ? 0 : fc_encode(me, nullptr, lane);
+  if (lane == 0) { A.rep[j] = (int32_t)j; A.fseq[j] = hit ? cand : -1; A.usz[j] = units; }
+}
+
+// After k_dedup_scan: the misses (fseq >= head) get absolute unit offsets in batch order from U0 on, and out[1] = the
+// units written once they are stored.  A miss that would straddle the ring's end starts at the next multiple of P
+// instead, and the skipped units count as written.  The attach bounds a batch's units plus that padding by P, so at
+// most one miss of a batch straddles.  One CTA of 1024 threads.
+__global__ void __launch_bounds__(1024)
+k_coded_offsets(const int64_t* __restrict__ fseq, const int32_t* __restrict__ usz, int64_t frames, int64_t head,
+                int64_t U0, int64_t P, int64_t* __restrict__ uoff, int64_t* __restrict__ out) {
+  __shared__ int32_t s_warp[32];
+  __shared__ int32_t s_total, s_jstar;
+  __shared__ int64_t s_pad;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int64_t running = U0;
+  for (int64_t base = 0; base < frames; base += 1024) {
+    const int64_t j = base + threadIdx.x;
+    const int32_t u = (j < frames && fseq[j] >= head) ? usz[j] : 0;
+    int32_t incl = u;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int32_t v = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += v;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    if (warp == 0) {
+      const int32_t w = s_warp[lane];
+      int32_t wi = w;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int32_t v = __shfl_up_sync(0xffffffffu, wi, o);
+        if (lane >= o) wi += v;
+      }
+      s_warp[lane] = wi - w;          // exclusive prefix of the warp totals
+      if (lane == 31) { s_total = wi; s_pad = 0; s_jstar = 1 << 30; }
+    }
+    __syncthreads();
+    int64_t a = running + s_warp[warp] + incl - u;
+    if (u > 0 && a % P + u > P) { s_pad = P - a % P; s_jstar = threadIdx.x; }
+    __syncthreads();
+    if (u > 0) uoff[j] = a + ((int)threadIdx.x >= s_jstar ? s_pad : 0);
+    running += s_total + s_pad;
+  }
+  if (threadIdx.x == 0) out[1] = running;
+}
+
+struct CodedCopyArgs {
+  const uint8_t* s;
+  int64_t frames;
+  const unsigned long long* key;
+  const int32_t* rep;
+  const int64_t* fseq;
+  int64_t head;             // first seq of this batch's misses
+  const int64_t* uoff;
+  const int32_t* usz;
+  uint8_t* pool;
+  int64_t P;
+  int64_t* foff;
+  int32_t* flen;
+  unsigned long long* pool_key;
+  int64_t F;
+  unsigned long long* tkey;
+  unsigned long long* tseq;
+  int64_t T;
+  int32_t* planes;          // the replay's planes field
+  int64_t slot0, capacity;  // record r goes to slot (slot0 + r) % capacity
+  int32_t R;
+};
+
+// k_dedup_copy for a coded pool: each miss is encoded in place at its unit offset, and its entry gets the descriptor.
+__global__ void __launch_bounds__(DD_THREADS)
+k_coded_copy(const __grid_constant__ CodedCopyArgs A) {
+  const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (j >= A.frames) return;
+  const int32_t r = A.rep[j];
+  const int64_t sq = A.fseq[r];
+  const int64_t ps = sq % A.F;
+  if (lane == 0) {
+    const int64_t rec = j / A.R;
+    int64_t slot = A.slot0 + rec;
+    if (slot >= A.capacity) slot -= A.capacity;
+    A.planes[slot * A.R + (j - rec * A.R)] = (int32_t)ps;
+  }
+  if (r != j || sq < A.head) return;        // a batch duplicate or a hit: nothing to store
+  const int64_t off = A.uoff[j];
+  fc_encode(A.s + j * DD_FRAME, A.pool + (off % A.P) * 16, lane);
+  if (lane == 0) {
+    const unsigned long long k = A.key[j];
+    A.foff[ps] = off;
+    A.flen[ps] = A.usz[j];
+    A.pool_key[ps] = k;
+    atomicMax(A.tseq + claim(A.tkey, A.T, k), (unsigned long long)(sq + 1));
+  }
+}
+
+// dst frame j of draw k = j / R: slot clamp_row(idx[k])'s frame j % R, decoded from the pool.  One warp per frame.
+__global__ void __launch_bounds__(DD_THREADS)
+k_decode_planes(const uint8_t* __restrict__ pool, int64_t P, const int64_t* __restrict__ foff, int64_t F,
+                const int32_t* __restrict__ planes, int32_t R, const int64_t* __restrict__ idx, int64_t n,
+                int64_t capacity, uint8_t* __restrict__ dst) {
+  __shared__ FcRows s_rows[DD_THREADS / 32];
+  const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (j >= n * R) return;
+  const int64_t k = j / R;
+  int64_t slot = idx[k];
+  slot = slot < 0 ? 0 : (slot >= capacity ? capacity - 1 : slot);
+  const int64_t id = (uint32_t)planes[R * slot + (j - k * R)] % (uint64_t)F;   // any int32 names an entry
+  fc_decode(pool + (foff[id] % P) * 16, dst + j * DD_FRAME, s_rows[threadIdx.x >> 5], lane);
+}
+
+// b2rl_frame_encode / b2rl_frame_decode: frame j <-> the encoding at enc + j * FC_RAW_BYTES.  One warp per frame.
+__global__ void __launch_bounds__(DD_THREADS)
+k_frame_encode(const uint8_t* __restrict__ frames, int64_t n, uint8_t* __restrict__ enc, int32_t* __restrict__ units) {
+  const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (j >= n) return;
+  const int u = fc_encode(frames + j * DD_FRAME, enc + j * FC_RAW_BYTES, lane);
+  if (lane == 0 && units != nullptr) units[j] = u;
+}
+
+__global__ void __launch_bounds__(DD_THREADS)
+k_frame_decode(const uint8_t* __restrict__ enc, int64_t n, uint8_t* __restrict__ frames) {
+  __shared__ FcRows s_rows[DD_THREADS / 32];
+  const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (j >= n) return;
+  fc_decode(enc + j * FC_RAW_BYTES, frames + j * DD_FRAME, s_rows[threadIdx.x >> 5], lane);
+}
+
 void dedup_free(b2rl_replay* h) {
   DedupState* d = h->dedup;
   if (d == nullptr) return;
   if (d->pool_host) cudaFreeHost(d->pool_host);
   else if (d->pool) cudaFree(d->pool);
   for (void* p : {(void*)d->pool_key, (void*)d->tkey, (void*)d->tseq, (void*)d->key, (void*)d->rep,
-                  (void*)d->fseq, (void*)d->bkey, (void*)d->bpos, (void*)d->misses_dev})
+                  (void*)d->fseq, (void*)d->bkey, (void*)d->bpos, (void*)d->misses_dev, (void*)d->foff,
+                  (void*)d->flen, (void*)d->usz, (void*)d->uoff})
     if (p) cudaFree(p);
   if (d->misses_host) cudaFreeHost(d->misses_host);
   if (d->done) cudaEventDestroy(d->done);
@@ -299,6 +494,21 @@ int64_t dedup_pool_frames(const b2rl_replay* h) { return h->dedup->F; }
 bool dedup_pool_on_host(const b2rl_replay* h) { return h->dedup->pool_host != nullptr; }
 int dedup_strip_frames(const b2rl_replay* h) { return h->dedup->layout == Layout::Strips ? h->dedup->R : 0; }
 int dedup_rollout_stacks(const b2rl_replay* h) { return h->dedup->stacks; }
+bool dedup_pool_coded(const b2rl_replay* h) { return h->dedup->P > 0; }
+
+static unsigned warps_grid(int64_t frames) { return (unsigned)((frames * 32 + DD_THREADS - 1) / DD_THREADS); }
+
+int gather_coded_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, cudaStream_t st) {
+  B2RL_REQUIRE((uintptr_t)dst_dev % 16 == 0, "frame strip outputs must be 16-byte aligned");
+  if (n == 0) return B2RL_OK;
+  const DedupState* d = h->dedup;
+  k_decode_planes<<<warps_grid(n * d->R), DD_THREADS, 0, st>>>(d->pool, d->P, d->foff, d->F,
+                                                               (const int32_t*)h->field[d->planes_field], d->R,
+                                                               idx_dev, n, h->capacity, dst_dev);
+  count_launch();
+  B2RL_CHECK_LAUNCH();
+  return B2RL_OK;
+}
 
 }  // namespace b2rl
 
@@ -310,17 +520,23 @@ static int64_t pow2_at_least(int64_t x) {
   return p;
 }
 
-// b2rl_dedup_attach (Pairs, R = 8), b2rl_dedup_attach_strips and b2rl_dedup_attach_strips_placed (Strips, R =
-// frames_per_record).  The arguments are checked before the handle, so every refusal comes before any CUDA work.
+// b2rl_dedup_attach (Pairs, R = 8), b2rl_dedup_attach_strips, _placed and _coded (Strips, R = frames_per_record).
+// pool_bytes > 0: a coded pool of pool_bytes / 16 units.  The arguments are checked before the handle, so every
+// refusal comes before any CUDA work.
 static int dedup_attach(b2rl_replay* h, int32_t planes_field, Layout layout, int32_t R, int64_t pool_frames,
-                        int64_t window, uint64_t hash_mask, bool pool_on_host) {
+                        int64_t window, uint64_t hash_mask, bool pool_on_host, int64_t pool_bytes = 0) {
   B2RL_REQUIRE(!pool_on_host || layout == Layout::Strips,
                "an Ape-X (Pairs) frame pool stays in HBM: only a strip handle's pool can be placed on the host");
+  B2RL_REQUIRE(pool_bytes == 0 || (layout == Layout::Strips && !pool_on_host),
+               "only a strip handle's pool in HBM can be coded");
   B2RL_REQUIRE(R >= 4 && R <= DD_MAX_FRAMES, "frames_per_record must be in [4, 65536]");
   B2RL_REQUIRE(window >= 0 && pool_frames - window > R,
                layout == Layout::Pairs ? "need window >= 0 and pool_frames - window > 8"
                                        : "need window >= 0 and pool_frames - window > frames_per_record");
   B2RL_REQUIRE(pool_frames < (1LL << 31), "pool_frames must be below 2^31");
+  B2RL_REQUIRE(pool_bytes >= 0 && pool_bytes % 16 == 0, "pool_bytes must be a non-negative multiple of 16");
+  B2RL_REQUIRE(pool_bytes == 0 || pool_bytes / 16 - (window + 2) * FC_RAW_UNITS >= (int64_t)R * FC_RAW_UNITS,
+               "need pool_bytes >= 7072 (window + 2 + frames_per_record): one record beyond the window");
   B2RL_REQUIRE(h != nullptr, "null handle");
   B2RL_REQUIRE(h->dedup == nullptr, "the replay already has a frame pool");
   B2RL_REQUIRE(!h->any_on_host, "a replay with fields placed on the host cannot take a frame pool");
@@ -341,6 +557,9 @@ static int dedup_attach(b2rl_replay* h, int32_t planes_field, Layout layout, int
   d->max_batch = (pool_frames - window - 1) / R;
   if (d->max_batch > DD_MAX_FRAMES / R) d->max_batch = DD_MAX_FRAMES / R;
   if (d->max_batch > h->capacity) d->max_batch = h->capacity;
+  d->P = pool_bytes / 16;
+  if (d->P > 0 && d->max_batch > (d->P - (window + 2) * FC_RAW_UNITS) / (R * (int64_t)FC_RAW_UNITS))
+    d->max_batch = (d->P - (window + 2) * FC_RAW_UNITS) / (R * (int64_t)FC_RAW_UNITS);   // DESIGN.md §4.21
   const int64_t nf = R * d->max_batch;
   d->T = pow2_at_least(2 * (window + nf));   // at most half claimed: window + one batch
   d->BT = pow2_at_least(2 * nf);
@@ -360,6 +579,18 @@ static int dedup_attach(b2rl_replay* h, int32_t planes_field, Layout layout, int
       return B2RL_ERR_NOMEM;
     }
     e = cudaHostGetDevicePointer((void**)&d->pool, d->pool_host, 0);
+  } else if (d->P > 0) {
+    // FC_RAW_BYTES of slack past the ring: a decode reads at most that many bytes from a frame's start, whatever the
+    // bytes there (fc_prepare), so a descriptor near the end of the ring never reads past the allocation.  Zeroed, so
+    // an entry no frame has been written to decodes as an all-zero raw frame.
+    alloc((void**)&d->pool, (size_t)d->P * 16 + FC_RAW_BYTES);
+    if (e == cudaSuccess) e = cudaMemset(d->pool, 0, (size_t)d->P * 16 + FC_RAW_BYTES);
+    alloc((void**)&d->foff, sizeof(int64_t) * (size_t)d->F);
+    alloc((void**)&d->flen, sizeof(int32_t) * (size_t)d->F);
+    alloc((void**)&d->usz, sizeof(int32_t) * (size_t)nf);
+    alloc((void**)&d->uoff, sizeof(int64_t) * (size_t)nf);
+    if (e == cudaSuccess) e = cudaMemset(d->foff, 0, sizeof(int64_t) * (size_t)d->F);
+    if (e == cudaSuccess) e = cudaMemset(d->flen, 0, sizeof(int32_t) * (size_t)d->F);
   } else {
     alloc((void**)&d->pool, (size_t)d->F * DD_FRAME);
   }
@@ -371,21 +602,26 @@ static int dedup_attach(b2rl_replay* h, int32_t planes_field, Layout layout, int
   alloc((void**)&d->fseq, sizeof(int64_t) * (size_t)nf);
   alloc((void**)&d->bkey, sizeof(unsigned long long) * (size_t)d->BT);
   alloc((void**)&d->bpos, sizeof(int32_t) * (size_t)d->BT);
-  alloc((void**)&d->misses_dev, sizeof(int64_t));
-  if (e == cudaSuccess) e = cudaMallocHost((void**)&d->misses_host, sizeof(int64_t));
+  alloc((void**)&d->misses_dev, 2 * sizeof(int64_t));        // misses, and units written (a coded pool)
+  if (e == cudaSuccess) e = cudaMallocHost((void**)&d->misses_host, 2 * sizeof(int64_t));
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&d->done, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaMemset(d->tkey, 0xFF, sizeof(unsigned long long) * (size_t)d->T);
   if (e == cudaSuccess) e = cudaMemset(d->tseq, 0, sizeof(unsigned long long) * (size_t)d->T);
   if (e == cudaSuccess) e = cudaMemset(h->field[planes_field], 0, (size_t)h->capacity * 4 * R);
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
-    set_error("allocating a %lld-frame pool failed: %s", (long long)pool_frames, cudaGetErrorString(e));
+    if (d->P > 0)
+      set_error("allocating a %lld-frame coded pool of %.3f GB failed: %s", (long long)pool_frames,
+                pool_bytes * 1e-9, cudaGetErrorString(e));
+    else
+      set_error("allocating a %lld-frame pool failed: %s", (long long)pool_frames, cudaGetErrorString(e));
     dedup_free(h);
     cudaGetLastError();
     return B2RL_ERR_NOMEM;
   }
   try {
     d->ins.assign((size_t)h->capacity, 0);
+    if (d->P > 0) d->uins.assign((size_t)h->capacity, 0);
   } catch (...) {
     dedup_free(h);
     set_error("out of host memory");
@@ -412,6 +648,14 @@ extern "C" int b2rl_dedup_attach_strips_placed(b2rl_replay* h, int32_t planes_fi
                       pool_on_host != 0);
 }
 
+extern "C" int b2rl_dedup_attach_strips_coded(b2rl_replay* h, int32_t planes_field, int32_t frames_per_record,
+                                              int64_t pool_frames, int64_t window, uint64_t hash_mask,
+                                              int64_t pool_bytes) {
+  B2RL_REQUIRE(pool_bytes > 0, "pool_bytes must be positive");
+  return dedup_attach(h, planes_field, Layout::Strips, frames_per_record, pool_frames, window, hash_mask, false,
+                      pool_bytes);
+}
+
 extern "C" int b2rl_dedup_attach_rollouts(b2rl_replay* h, int32_t planes_field, int32_t stacks_per_record,
                                           int64_t pool_frames, int64_t window, uint64_t hash_mask) {
   B2RL_REQUIRE(stacks_per_record >= 1 && stacks_per_record <= DD_MAX_FRAMES / 4,
@@ -431,6 +675,39 @@ extern "C" int b2rl_dedup_info(const b2rl_replay* h, void** pool_dev, int64_t* h
   return B2RL_OK;
 }
 
+extern "C" int b2rl_dedup_codec_stats(const b2rl_replay* h, int64_t* units_written, int64_t* pool_units,
+                                      int64_t* frames_stored) {
+  B2RL_REQUIRE(h != nullptr, "null handle");
+  B2RL_REQUIRE(h->dedup != nullptr && h->dedup->P > 0, "not a coded frame pool (b2rl_dedup_attach_strips_coded)");
+  if (units_written) *units_written = h->dedup->units;
+  if (pool_units) *pool_units = h->dedup->P;
+  if (frames_stored) *frames_stored = h->dedup->head;
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_frame_encode(const uint8_t* frames_dev, int64_t n, uint8_t* enc_dev, int32_t* units_dev,
+                                 void* stream) {
+  B2RL_REQUIRE(n >= 0, "n must be >= 0");
+  if (n == 0) return B2RL_OK;
+  B2RL_REQUIRE(frames_dev != nullptr && enc_dev != nullptr, "null argument");
+  B2RL_REQUIRE((uintptr_t)frames_dev % 16 == 0 && (uintptr_t)enc_dev % 16 == 0, "buffers must be 16-byte aligned");
+  k_frame_encode<<<warps_grid(n), DD_THREADS, 0, (cudaStream_t)stream>>>(frames_dev, n, enc_dev, units_dev);
+  count_launch();
+  B2RL_CHECK_LAUNCH();
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_frame_decode(const uint8_t* enc_dev, int64_t n, uint8_t* frames_dev, void* stream) {
+  B2RL_REQUIRE(n >= 0, "n must be >= 0");
+  if (n == 0) return B2RL_OK;
+  B2RL_REQUIRE(frames_dev != nullptr && enc_dev != nullptr, "null argument");
+  B2RL_REQUIRE((uintptr_t)frames_dev % 16 == 0 && (uintptr_t)enc_dev % 16 == 0, "buffers must be 16-byte aligned");
+  k_frame_decode<<<warps_grid(n), DD_THREADS, 0, (cudaStream_t)stream>>>(enc_dev, n, frames_dev);
+  count_launch();
+  B2RL_CHECK_LAUNCH();
+  return B2RL_OK;
+}
+
 extern "C" int b2rl_dedup_pool_placement(const b2rl_replay* h, int32_t* on_host, void** pool) {
   B2RL_REQUIRE(h != nullptr && on_host != nullptr, "null argument");
   B2RL_REQUIRE(h->dedup != nullptr, "not a frame-deduplicated replay (b2rl_dedup_attach)");
@@ -438,8 +715,6 @@ extern "C" int b2rl_dedup_pool_placement(const b2rl_replay* h, int32_t* on_host,
   if (pool) *pool = *on_host ? h->dedup->pool_host : h->dedup->pool;
   return B2RL_OK;
 }
-
-static unsigned warps_grid(int64_t frames) { return (unsigned)((frames * 32 + DD_THREADS - 1) / DD_THREADS); }
 
 // The push of n records whose frames the layout L places (the caller has checked the frame pointers).
 template <Layout L>
@@ -470,41 +745,69 @@ static int dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8_t* ns_de
   B2RL_CUDA(cudaMemsetAsync(d->bpos, 0x7F, sizeof(int32_t) * (size_t)d->BT, st));
   k_dedup_hash<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(s_dev, ns_dev, frames, d->mask, d->key, d->bkey, d->bpos,
                                                           d->BT);
-  ResolveArgs A{s_dev, ns_dev, frames, d->key, d->bkey, d->bpos, d->BT, d->tkey, d->tseq, d->T, d->pool, d->F,
-                head - d->W, d->rep, d->fseq};
-  k_dedup_resolve<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(A);
+  const bool coded = L == Layout::Strips && d->P > 0;
+  if (coded) {
+    CodedResolveArgs A{s_dev, frames, d->key, d->bkey, d->bpos, d->BT, d->tkey, d->tseq, d->T, d->pool, d->P,
+                       d->foff, d->F, head - d->W, d->rep, d->fseq, d->usz};
+    k_coded_resolve<<<warps_grid(frames), DD_THREADS, 0, st>>>(A);
+  } else {
+    ResolveArgs A{s_dev, ns_dev, frames, d->key, d->bkey, d->bpos, d->BT, d->tkey, d->tseq, d->T, d->pool, d->F,
+                  head - d->W, d->rep, d->fseq};
+    k_dedup_resolve<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(A);
+  }
   k_dedup_scan<<<1, 1024, 0, st>>>(d->fseq, frames, head, d->misses_dev);
   count_launch(3);
+  if (coded) {
+    k_coded_offsets<<<1, 1024, 0, st>>>(d->fseq, d->usz, frames, head, d->units, d->P, d->uoff, d->misses_dev);
+    count_launch();
+  }
   B2RL_CHECK_LAUNCH();
-  B2RL_CUDA(cudaMemcpyAsync(d->misses_host, d->misses_dev, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  B2RL_CUDA(cudaMemcpyAsync(d->misses_host, d->misses_dev, (coded ? 2 : 1) * sizeof(int64_t), cudaMemcpyDeviceToHost,
+                            st));
   B2RL_CUDA(cudaStreamSynchronize(st));
-  const int64_t head_new = head + *d->misses_host;
+  const int64_t head_new = head + d->misses_host[0];
+  const int64_t units_new = coded ? d->misses_host[1] : 0;
   // 3. the eviction rule: the oldest slots with F - W or more frames stored since their batch began lose their
-  //    priority, in stream order before their frames can be overwritten
+  //    priority, in stream order before their frames can be overwritten; with a coded pool also those with
+  //    P - (W + 1) 442 or more units written since (DESIGN.md §4.21)
   int64_t tail = h->head - h->size;
   if (tail < 0) tail += h->capacity;
   int64_t dead = 0;
-  while (dead < h->size && head_new - d->ins[(size_t)((tail + dead) % h->capacity)] >= d->F - d->W) ++dead;
+  auto dies = [&](int64_t slot) {
+    return head_new - d->ins[(size_t)slot] >= d->F - d->W ||
+           (coded && units_new - d->uins[(size_t)slot] >= d->P - (d->W + 1) * FC_RAW_UNITS);
+  };
+  while (dead < h->size && dies((tail + dead) % h->capacity)) ++dead;
   if (dead > 0) {
     h->size -= dead;
     int rc = b2rl_tree_update_impl(h, nullptr, tail, nullptr, 0.0f, dead, st, true);
     if (rc != B2RL_OK) return rc;
   }
   // 4. pool ids, new frames, key table; then the other fields and the priorities as b2rl_replay_push does
-  CopyArgs C{s_dev, ns_dev, frames, d->key, d->rep, d->fseq, head, d->pool, d->pool_key, d->F, d->tkey, d->tseq, d->T,
-             (int32_t*)h->field[d->planes_field], h->head, h->capacity, d->R};
-  k_dedup_copy<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(C);
+  if (coded) {
+    CodedCopyArgs C{s_dev, frames, d->key, d->rep, d->fseq, head, d->uoff, d->usz, d->pool, d->P, d->foff, d->flen,
+                    d->pool_key, d->F, d->tkey, d->tseq, d->T, (int32_t*)h->field[d->planes_field], h->head,
+                    h->capacity, d->R};
+    k_coded_copy<<<warps_grid(frames), DD_THREADS, 0, st>>>(C);
+  } else {
+    CopyArgs C{s_dev, ns_dev, frames, d->key, d->rep, d->fseq, head, d->pool, d->pool_key, d->F, d->tkey, d->tseq,
+               d->T, (int32_t*)h->field[d->planes_field], h->head, h->capacity, d->R};
+    k_dedup_copy<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(C);
+  }
   count_launch();
   B2RL_CHECK_LAUNCH();
   int rc = copy_ring_range(h, fields_src, h->head, n, st);
   if (rc != B2RL_OK) return rc;
   B2RL_CUDA(cudaMemcpyAsync(h->scratch_val, prios, (size_t)n * sizeof(float), cudaMemcpyDefault, st));
   for (int64_t i = 0; i < n; ++i) d->ins[(size_t)((h->head + i) % h->capacity)] = head;
+  if (coded)
+    for (int64_t i = 0; i < n; ++i) d->uins[(size_t)((h->head + i) % h->capacity)] = d->units;
   rc = publish(h, h->scratch_val, n, st);
   if (rc != B2RL_OK) return rc;
   B2RL_CUDA(cudaEventRecord(d->done, st));
   d->head = head_new;
   d->used += head_new - head;
+  if (coded) d->units = units_new;
   return B2RL_OK;
 }
 

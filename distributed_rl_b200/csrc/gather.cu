@@ -146,6 +146,9 @@ static int gather_run(b2rl_replay* h, const int64_t* idx_dev, int64_t n, void* c
       if (stacks_out[0] != nullptr && dedup_pool_on_host(h)) {   // never the TMA row copy: hostrows.cu's gather
         const int rc = gather_host_planes(h, idx_dev, n, (uint8_t*)stacks_out[0], st);
         if (rc != B2RL_OK) return rc;
+      } else if (stacks_out[0] != nullptr && dedup_pool_coded(h)) {   // decoded from the unit ring (dedup.cu)
+        const int rc = gather_coded_planes(h, idx_dev, n, (uint8_t*)stacks_out[0], st);
+        if (rc != B2RL_OK) return rc;
       } else if (stacks_out[0] != nullptr) {
         P.bulk.add_planes(dedup_pool(h), planes, R, 0, R, (uint8_t*)stacks_out[0]);
       }

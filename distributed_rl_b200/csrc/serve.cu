@@ -386,7 +386,7 @@ extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot,
   SmallFields small{};
   SmallRows rows{};
   int host_f[B2RL_MAX_FIELDS], host_o[B2RL_MAX_FIELDS], n_host = 0;
-  int host_planes_o = -1;
+  int host_planes_o = -1, coded_planes_o = -1;
   for (int f = 0, o = 3; f < h->n_fields; ++f, ++o) {
     const int64_t b = h->field_bytes[f];
     if (h->on_host[f]) {         // copied after the draw, from the slot's idx, by the host-row gather (hostrows.cu)
@@ -394,6 +394,8 @@ extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot,
       host_o[n_host++] = o;
     } else if (h->dedup != nullptr && f == dedup_planes_field(h) && dedup_pool_on_host(h)) {
       host_planes_o = o;         // the strips of a host pool: likewise, by the host-plane gather (hostrows.cu)
+    } else if (h->dedup != nullptr && f == dedup_planes_field(h) && dedup_pool_coded(h)) {
+      coded_planes_o = o;        // the strips of a coded pool: decoded after the draw, from the slot's idx (dedup.cu)
     } else if (h->dedup != nullptr && f == dedup_planes_field(h)) {   // frames assembled from the frame pool
       const int32_t* planes = (const int32_t*)h->field[f];
       const int R = dedup_strip_frames(h);
@@ -433,6 +435,8 @@ extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot,
   }
   if (host_planes_o >= 0)
     return gather_host_planes(h, (const int64_t*)ptrs[1], n, (uint8_t*)ptrs[host_planes_o], (cudaStream_t)stream);
+  if (coded_planes_o >= 0)
+    return gather_coded_planes(h, (const int64_t*)ptrs[1], n, (uint8_t*)ptrs[coded_planes_o], (cudaStream_t)stream);
   return B2RL_OK;
 }
 

@@ -83,6 +83,11 @@ class R2D2Config:
     HOST_POOL: bool = False      # keep a FRAME_DEDUP store's frame pool in pinned, mapped host memory; the plane table,
                                  # the keys and the sum-tree stay in HBM.  Each step copies the sampled sequences' frames
                                  # over PCIe into a device staging buffer, as HOST_FRAMES does (DESIGN §4.19).
+    POOL_CODEC: bool = False     # store a FRAME_DEDUP store's frames losslessly encoded in a ring of bytes in HBM
+                                 # (DESIGN §4.21); each step decodes the sampled sequences' frames into a device
+                                 # staging buffer, as HOST_POOL copies them.
+    POOL_BYTES_PER_SEQUENCE: float | None = None   # POOL_CODEC's ring: this many bytes per slot (see pool_bytes);
+                                                   # size it from StripDedupReplay.codec_stats()
 
     def __post_init__(self):
         if self.HOST_FRAMES and self.PAYLOAD_POOL:
@@ -94,6 +99,14 @@ class R2D2Config:
         if self.FRAME_DEDUP and (self.HOST_FRAMES or self.PAYLOAD_POOL):
             raise ValueError("FRAME_DEDUP keeps its frames in a frame pool (in host memory with HOST_POOL) and stores "
                              "every pushed sequence: it takes neither HOST_FRAMES nor PAYLOAD_POOL")
+        if self.POOL_CODEC and not self.FRAME_DEDUP:
+            raise ValueError("POOL_CODEC encodes the frame pool of a FRAME_DEDUP store: set FRAME_DEDUP with it")
+        if self.POOL_CODEC and self.HOST_POOL:
+            raise ValueError("POOL_CODEC keeps its coded frame pool in HBM: it does not take HOST_POOL")
+        if self.POOL_BYTES_PER_SEQUENCE is not None and not self.POOL_CODEC:
+            raise ValueError("POOL_BYTES_PER_SEQUENCE sizes the coded frame pool: set POOL_CODEC with it")
+        if self.POOL_BYTES_PER_SEQUENCE is not None and not self.POOL_BYTES_PER_SEQUENCE > 0:
+            raise ValueError(f"POOL_BYTES_PER_SEQUENCE must be positive, not {self.POOL_BYTES_PER_SEQUENCE}")
         if self.FRAME_DEDUP:
             self.FRAME_STRIP = True
 
@@ -104,11 +117,18 @@ class R2D2Config:
                  "USE_RESCALING", "REPLAY_MEMORY_LEN", "BUFFER_SIZE", "TARGET_FREQUENCY", "LEARNER_DEVICE",
                  "REDIS_SERVER", "OPTIM_INFO", "MODEL")
         kw = {k: getattr(C, k) for k in names}
-        for k in ("FRAME_DEDUP", "FRAMES_PER_SEQUENCE", "DEDUP_WINDOW", "HOST_POOL"):   # optional keys of cfg/r2d2.json
+        for k in ("FRAME_DEDUP", "FRAMES_PER_SEQUENCE", "DEDUP_WINDOW", "HOST_POOL", "POOL_CODEC",
+                  "POOL_BYTES_PER_SEQUENCE"):                                    # optional keys of cfg/r2d2.json
             if hasattr(C, k):
                 kw[k] = getattr(C, k)
         return R2D2Config(LOG_W=getattr(C, "LOG_W", None), FRAME_STRIP=bool(getattr(C, "FRAME_STRIP", False)),
                           HOST_FRAMES=bool(getattr(C, "HOST_FRAMES", False)), **kw)
+
+
+def _pool_frames(cfg: R2D2Config) -> int:
+    """F of a FRAME_DEDUP replay: ceil(FRAMES_PER_SEQUENCE * REPLAY_MEMORY_LEN) frames (dedup_geometry, pool_bytes)."""
+    import math
+    return int(math.ceil(cfg.FRAMES_PER_SEQUENCE * cfg.REPLAY_MEMORY_LEN))
 
 
 def dedup_geometry(cfg: R2D2Config) -> tuple:
@@ -117,14 +137,26 @@ def dedup_geometry(cfg: R2D2Config) -> tuple:
     have been stored after it: at the default 48 frames per slot, 42 REPLAY_MEMORY_LEN frames or more, above the
     ~40 new frames per sequence the reference actors send (T / 2 in mid-episode), so the slot ring wraps first.  The
     window only has to reach back to the same actor's previous sequence."""
-    import math
     import warnings
-    F = int(math.ceil(cfg.FRAMES_PER_SEQUENCE * cfg.REPLAY_MEMORY_LEN))
+    F = _pool_frames(cfg)
     W = min(int(cfg.DEDUP_WINDOW), F // 8)
     if W < cfg.DEDUP_WINDOW:
         warnings.warn(f"DEDUP_WINDOW = {cfg.DEDUP_WINDOW} frames is more than an eighth of the {F}-frame pool: the "
                       f"frame-deduplicated replay uses a window of {W} frames", stacklevel=2)
     return F, W
+
+
+def pool_bytes(cfg: R2D2Config) -> int | None:
+    """Bytes of a POOL_CODEC store's frame ring (None without POOL_CODEC): POOL_BYTES_PER_SEQUENCE x REPLAY_MEMORY_LEN,
+    rounded down to 16 bytes.  The default is the raw size plus one frame, (F + 1) x 7 072 for dedup_geometry's F
+    frames: a slot then dies by the byte rule no earlier than by the frame rule (DESIGN §4.21), so the ring holds
+    whatever the frame pool would.  A smaller ring trades that for memory, at the mean stored bytes per frame that
+    codec_stats() reports."""
+    if not cfg.POOL_CODEC:
+        return None
+    if cfg.POOL_BYTES_PER_SEQUENCE is None:
+        return (_pool_frames(cfg) + 1) * 7072
+    return int(cfg.POOL_BYTES_PER_SEQUENCE * cfg.REPLAY_MEMORY_LEN) // 16 * 16
 
 
 class Replay(ReplayThread):
@@ -140,7 +172,7 @@ class Replay(ReplayThread):
         elif self.cfg.FRAME_DEDUP:
             self.store = self.pool = R.StripDedupReplay(self.cfg.REPLAY_MEMORY_LEN, *dedup_geometry(self.cfg),
                                                         T=self.cfg.FIXED_TRAJECTORY, device=self.device,
-                                                        host_pool=self.cfg.HOST_POOL)
+                                                        host_pool=self.cfg.HOST_POOL, pool_bytes=pool_bytes(self.cfg))
         else:
             self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, fields, self.device,
                                         host_fields=("state",) if self.cfg.HOST_FRAMES else ())
@@ -317,7 +349,8 @@ class Learner(TargetNetLearner):
         (R.StripDedupReplay.frame_source), with the rows of a strip store.  With HOST_FRAMES or HOST_POOL the frames
         are not in HBM: the same gather launch sequence also copies the sampled sequences' `state` rows (with
         HOST_POOL their strips, assembled from the host pool) from host memory into a fixed device staging buffer,
-        and conv_1 reads that buffer with the rows train() uses on a staged batch (row = b * pitch + t)."""
+        and conv_1 reads that buffer with the rows train() uses on a staged batch (row = b * pitch + t).  With
+        POOL_CODEC the frames are encoded: the same gather decodes the sampled strips into that staging buffer."""
         if self._graph is not None:
             self._graph.replay()
             return self._static
@@ -327,7 +360,7 @@ class Learner(TargetNetLearner):
         T, MEM, B, A = c.FIXED_TRAJECTORY, c.MEM, c.BATCHSIZE, c.ACTION_SIZE
         mem = self.memory
         st, pool = mem.store, mem.pool
-        staged = c.HOST_FRAMES or c.HOST_POOL                   # the frames are in host memory
+        staged = c.HOST_FRAMES or c.HOST_POOL or c.POOL_CODEC   # the frames are in host memory, or encoded
         if not hasattr(self, "_small"):
             self._small = pool.alloc_batch(B, ("action", "reward", "h0", "h1", "notdone"))
             if staged:

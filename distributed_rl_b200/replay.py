@@ -632,6 +632,39 @@ def _small_rows(fields: Sequence[Field], xs: Sequence, n: int) -> list:
     return out
 
 
+CODED_FRAME_BYTES = 7072      # the largest encoding of a frame: 16 header bytes and the 7 056 raw pixels
+
+
+def _check_device_bytes(t, row: int, what: str) -> None:
+    """The codec kernels read device uint8 rows of `row` bytes: refuse anything else before a launch."""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.uint8 or t.numel() % row != 0:
+        desc = f"{t.dtype} {t.device} tensor of {t.numel()} elements" if isinstance(t, torch.Tensor) else type(t)
+        raise ValueError(f"{what} must be a CUDA uint8 tensor of whole {row}-byte rows, not a {desc}")
+
+
+def encode_frames(frames: torch.Tensor, stream=None) -> tuple:
+    """The coded pool's encoding of each frame of a device uint8 (n, 84, 84) tensor (b2rl_frame_encode) -> (enc uint8
+    (n, 7072), units int32 (n,)): frame j's encoding is enc[j, :16 units[j]]; the rest of the row is zero."""
+    _check_device_bytes(frames, FRAME_BYTES, "frames")
+    frames = frames.contiguous().view(-1, FRAME_BYTES)
+    n = frames.shape[0]
+    enc = torch.zeros(n, CODED_FRAME_BYTES, dtype=torch.uint8, device=frames.device)
+    units = torch.empty(n, dtype=torch.int32, device=frames.device)
+    st = torch.cuda.current_stream(frames.device).cuda_stream if stream is None else stream
+    check(_lib.load().b2rl_frame_encode(frames.data_ptr(), n, enc.data_ptr(), units.data_ptr(), st))
+    return enc, units
+
+
+def decode_frames(enc: torch.Tensor, stream=None) -> torch.Tensor:
+    """The inverse of encode_frames: a device uint8 (n, 7072) tensor of encodings -> (n, 84, 84) frames."""
+    _check_device_bytes(enc, CODED_FRAME_BYTES, "encodings")
+    enc = enc.contiguous().view(-1, CODED_FRAME_BYTES)
+    out = torch.empty(enc.shape[0], 84, 84, dtype=torch.uint8, device=enc.device)
+    st = torch.cuda.current_stream(enc.device).cuda_stream if stream is None else stream
+    check(_lib.load().b2rl_frame_decode(enc.data_ptr(), enc.shape[0], out.data_ptr(), st))
+    return out
+
+
 class StripDedupReplay(DedupReplay):
     """The strip form of DedupReplay (b2rl_dedup_attach_strips, R2D2Config.FRAME_DEDUP, DESIGN.md §4.18): an R2D2
     replay whose slots hold R2D2_DEDUP_FIELDS(T), the T + 3 frames of each sequence's strip living in the frame pool.
@@ -641,21 +674,48 @@ class StripDedupReplay(DedupReplay):
     `host_pool` (R2D2Config.HOST_POOL, DESIGN.md §4.19): the frame pool lives in pinned, mapped host memory owned by
     the library (b2rl_dedup_attach_strips_placed), allocated from a thread bound to the GPU's NUMA node; the planes,
     keys and sum-tree stay in HBM.  `pool` is then a CPU tensor, gather() copies the sampled strips over PCIe, and
-    frame_source() is refused: conv_1 reads a gathered (staged) batch instead."""
+    frame_source() is refused: conv_1 reads a gathered (staged) batch instead.
+    `pool_bytes` (R2D2Config.POOL_CODEC, DESIGN.md §4.21): the frames are stored losslessly encoded in a device ring of
+    pool_bytes (b2rl_dedup_attach_strips_coded), and a slot also dies once pool_bytes - 7072 (window + 1) bytes have
+    been written since its batch began.  `pool` is then that flat uint8 ring, gather() decodes the sampled strips,
+    codec_stats() reports the bytes stored per frame, and frame_source() is refused as for a host pool."""
 
     def __init__(self, capacity: int, pool_frames: int, window: int, T: int = 80, device="cuda:0",
-                 hash_mask: int = DEDUP_HASH_MASK, hidden: int = 512, host_pool: bool = False):
+                 hash_mask: int = DEDUP_HASH_MASK, hidden: int = 512, host_pool: bool = False,
+                 pool_bytes: int | None = None):
+        if host_pool and pool_bytes is not None:
+            raise ValueError("a coded frame pool (pool_bytes) lives in HBM: it takes no host_pool")
         DeviceReplay.__init__(self, capacity, R2D2_DEDUP_FIELDS(T, hidden), device)
         self.T = int(T)
         self.RECORD_FIELDS = r2d2_fields(self.T, hidden, strip=True)
         self.host_pool = bool(host_pool)
+        self.coded = pool_bytes is not None
         args = (self._h, 0, self.T + 3, int(pool_frames), int(window), int(hash_mask))
         if self.host_pool:
             with hostmem.on_gpu_node(self.device):   # pinned pages on the GPU's NUMA node (first touch: the library)
                 check(self.lib.b2rl_dedup_attach_strips_placed(*args, 1))
+        elif self.coded:
+            check(self.lib.b2rl_dedup_attach_strips_coded(*args, int(pool_bytes)))
         else:
             check(self.lib.b2rl_dedup_attach_strips(*args))
         self._attached(pool_frames, window)
+        if self.coded:          # the encoded frames: a flat ring of 16-byte units, not (F, 84, 84) frames
+            p = C.c_void_p()
+            check(self.lib.b2rl_dedup_info(self._h, C.byref(p), None, None))
+            self.pool_bytes = 16 * self.codec_stats()["pool_units"]
+            with torch.cuda.device(self.device):
+                self.pool = torch.as_tensor(_CudaView(p.value, (self.pool_bytes,), "|u1", self), device=self.device)
+
+    def codec_stats(self) -> dict:
+        """A coded pool's counters (b2rl_dedup_codec_stats): units_written (16-byte units, the wrap's skipped units
+        included), pool_units, frames_stored, and bytes_per_frame = 16 units_written / frames_stored, the mean
+        stored size of a frame (7 072 at most: raw)."""
+        if not self.coded:
+            raise ValueError("codec_stats() reports a coded frame pool (pool_bytes)")
+        u, p, f = C.c_int64(), C.c_int64(), C.c_int64()
+        check(self.lib.b2rl_dedup_codec_stats(self._h, C.byref(u), C.byref(p), C.byref(f)))
+        return {"units_written": u.value, "pool_units": p.value, "frames_stored": f.value,
+                "bytes_per_frame": 16.0 * u.value / f.value if f.value else 0.0}
 
     def push(self, fields: Sequence, priorities) -> None:
         """fields: [state, action, reward, h0, h1, notdone] as for a DeviceReplay of r2d2_fields(T, strip=True),
@@ -703,6 +763,9 @@ class StripDedupReplay(DedupReplay):
         if self.host_pool:
             raise ValueError("conv_1 reads its frame rows in place on the GPU: a frame pool in host memory (host_pool) "
                              "has no frame source; gather the sampled strips into device memory first")
+        if self.coded:
+            raise ValueError("conv_1 reads raw frame rows: a coded frame pool (pool_bytes) holds encoded frames and "
+                             "has no frame source; gather (decode) the sampled strips into device memory first")
         return PlaneFrames(self.pool, self.field_view("planes"), 0, 1)
 
 
@@ -720,7 +783,7 @@ class RolloutDedupReplay(StripDedupReplay):
         DeviceReplay.__init__(self, capacity, IMPALA_DEDUP_FIELDS(T), device)
         self.T = int(T)
         self.RECORD_FIELDS = impala_fields(self.T)
-        self.host_pool = False
+        self.host_pool = self.coded = False
         check(self.lib.b2rl_dedup_attach_rollouts(self._h, 0, self.T + 1, int(pool_frames), int(window),
                                                   int(hash_mask)))
         self._attached(pool_frames, window)
@@ -874,6 +937,9 @@ def _frame_source(frames) -> _lib.Frames:
     dimension, each a contiguous FRAME_STACK_BYTES; stride(0) is the row stride (the library checks that it is a
     positive multiple of 16)."""
     if isinstance(frames, PlaneFrames):
+        if frames.pool.dim() != 3:
+            raise ValueError("conv_1 reads raw (F, 84, 84) pool frames: a coded frame pool holds encoded frames; "
+                             "gather (decode) the sampled strips into device memory first")
         if frames.pool.device.type != "cuda":
             raise ValueError("conv_1 reads its frame rows in place on the GPU: a frame pool in host memory must be "
                              "gathered into device memory first")

@@ -28,7 +28,8 @@ elif ALG == "R2D2":
     HOST_FRAMES = bool(DATA.get("HOST_FRAMES", False))   # not a reference key: keep the frames in pinned host memory
     FRAME_DEDUP = bool(DATA.get("FRAME_DEDUP", False))   # not a reference key: store every distinct frame once
     HOST_POOL = bool(DATA.get("HOST_POOL", False))       # not a reference key: keep that frame pool in host memory
-    for _k in ("FRAMES_PER_SEQUENCE", "DEDUP_WINDOW"):
+    POOL_CODEC = bool(DATA.get("POOL_CODEC", False))     # not a reference key: store that frame pool encoded
+    for _k in ("FRAMES_PER_SEQUENCE", "DEDUP_WINDOW", "POOL_BYTES_PER_SEQUENCE"):
         if _k in DATA:
             globals()[_k] = DATA[_k]
 elif ALG == "IMPALA":

@@ -292,6 +292,30 @@ int b2rl_dedup_attach_strips_placed(b2rl_replay* h, int32_t planes_field, int32_
 /* Where the frame pool (the frames of PER.memory, baseline/PER.py:7-28) of a dedup replay lives: *on_host = 1 for
  * pinned host memory, 0 for device; *pool (may be NULL) its host address, or its device address for a device pool. */
 int b2rl_dedup_pool_placement(const b2rl_replay* h, int32_t* on_host, void** pool);
+
+/* The strip store with its frames stored encoded, as CompressedDeque.append / __getitem__ (baseline/utils.py:277-296)
+ * stores the reference's replay entries, here with a lossless per-frame codec (csrc/frame_codec.cuh, DESIGN.md §4.21):
+ * b2rl_dedup_attach_strips whose pool is a ring of P = pool_bytes / 16 units in device memory.  Frame seq's entry
+ * seq % pool_frames holds its absolute unit offset and length, so ids, the window and the frame rule are the strip
+ * handle's.  A frame takes 1..442 units and never straddles the ring's end (the units skipped count as written).  A hit
+ * still needs all 7 056 bytes equal to the stored frame.  A slot also stops being live once P - (window + 1) * 442
+ * units or more have been written since its batch began; a push takes at most (P - (window + 2) * 442) / (442 R)
+ * records too.  Requires pool_bytes a positive multiple of 16 with P >= 442 (window + 2 + R).  b2rl_replay_gather_planes
+ * and b2rl_serve_fill decode the sampled slots' strips (k_decode_planes), byte for byte the strip handle's while the
+ * slots are live; a dead or never-written slot decodes to unspecified frames, read inside the pool's allocation (P
+ * units plus 7 072 zeroed bytes).  The pool (*pool_dev of b2rl_dedup_info) is never a conv_1 frame source.  Arguments are checked before the handle is read. */
+int b2rl_dedup_attach_strips_coded(b2rl_replay* h, int32_t planes_field, int32_t frames_per_record,
+                                   int64_t pool_frames, int64_t window, uint64_t hash_mask, int64_t pool_bytes);
+/* A coded pool's counters, the sizes CompressedDeque (baseline/utils.py:277-296) leaves to pickle (each may be NULL):
+ * units written so far (wrap padding included), P, and frames stored. */
+int b2rl_dedup_codec_stats(const b2rl_replay* h, int64_t* units_written, int64_t* pool_units, int64_t* frames_stored);
+/* The pool's codec on device buffers, as CompressedDeque.append / __getitem__ (baseline/utils.py:277-296) on one
+ * frame: b2rl_frame_encode writes frame j (n frames of 7 056 bytes) to enc_dev + 7 072 j and its length in units to
+ * units_dev[j] (units_dev may be NULL); the bytes after the encoding in its 7 072 are left as they were.
+ * b2rl_frame_decode is its inverse for encodings at the same stride; any other bytes decode to unspecified frames,
+ * each read from its own 7 072 bytes only.  Buffers 16-byte aligned. */
+int b2rl_frame_encode(const uint8_t* frames_dev, int64_t n, uint8_t* enc_dev, int32_t* units_dev, void* stream);
+int b2rl_frame_decode(const uint8_t* enc_dev, int64_t n, uint8_t* frames_dev, void* stream);
 int b2rl_replay_gather_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, void* const* stacks_out_dev,
                               void* const* out_fields_dev, void* stream);
 
