@@ -30,9 +30,11 @@ class ServeLayout(C.Structure):
 
 class Frames(C.Structure):
     """b2rl_frames: where conv_1 reads frame row r (include/b2rl.h); exactly one of base, table and pool + planes.
-    plane_stride 0 means 8 (the Ape-X plane table)."""
+    plane_stride 0 means 8 (the Ape-X plane table).  offsets (with pool_units, pool_frames) makes the pool a coded
+    one, whose frames conv_1 decodes on chip."""
     _fields_ = [("base", c_vp), ("table", c_vp), ("pool", c_vp), ("planes", c_vp), ("row_stride", c_i64),
-                ("rows", c_i64), ("plane_base", c_i32), ("plane_stride", c_i32)]
+                ("rows", c_i64), ("plane_base", c_i32), ("plane_stride", c_i32), ("offsets", c_vp),
+                ("pool_units", c_i64), ("pool_frames", c_i64)]
 
 
 # name -> (restype, argtypes); must list every symbol include/b2rl.h declares.
@@ -84,6 +86,8 @@ SIGNATURES = {
     "b2rl_dedup_attach_rollouts": (C.c_int, [c_vp, c_i32, c_i32, c_i64, c_i64, c_u64]),
     "b2rl_dedup_pool_placement": (C.c_int, [c_vp, C.POINTER(c_i32), C.POINTER(c_vp)]),
     "b2rl_dedup_attach_strips_coded": (C.c_int, [c_vp, c_i32, c_i32, c_i64, c_i64, c_u64, c_i64]),
+    "b2rl_dedup_attach_coded": (C.c_int, [c_vp, c_i32, c_i64, c_i64, c_u64, c_i64]),
+    "b2rl_dedup_coded_offsets": (C.c_int, [c_vp, C.POINTER(c_vp)]),
     "b2rl_dedup_codec_stats": (C.c_int, [c_vp, C.POINTER(c_i64), C.POINTER(c_i64), C.POINTER(c_i64)]),
     "b2rl_frame_encode": (C.c_int, [c_vp, c_i64, c_vp, c_vp, c_vp]),
     "b2rl_frame_decode": (C.c_int, [c_vp, c_i64, c_vp, c_vp]),

@@ -67,6 +67,20 @@ class ApexConfig:
     FRAMES_PER_TRANSITION: float = 4.0
     DEDUP_WINDOW: int = 1 << 20      # a frame is reused only from the last DEDUP_WINDOW frames stored (at most 1/8 of
                                      # the pool, see dedup_geometry)
+    FRAME_CODEC: bool = False        # store a FRAME_DEDUP store's frames losslessly encoded in a ring of bytes in HBM
+                                     # (R.CodedDedupReplay, DESIGN.md §4.22).  Unlike R2D2's POOL_CODEC, which decodes
+                                     # into a staged minibatch, the step still reads the pool in place: conv_1 decodes
+                                     # the sampled frames on chip
+    POOL_BYTES_PER_TRANSITION: float | None = None   # FRAME_CODEC's ring: this many bytes per slot (see pool_bytes);
+                                                     # size it from CodedDedupReplay.codec_stats()
+
+    def __post_init__(self):
+        if self.FRAME_CODEC and not self.FRAME_DEDUP:
+            raise ValueError("FRAME_CODEC encodes the frame pool of a FRAME_DEDUP store: set FRAME_DEDUP with it")
+        if self.POOL_BYTES_PER_TRANSITION is not None and not self.FRAME_CODEC:
+            raise ValueError("POOL_BYTES_PER_TRANSITION sizes the coded frame pool: set FRAME_CODEC with it")
+        if self.POOL_BYTES_PER_TRANSITION is not None and not self.POOL_BYTES_PER_TRANSITION > 0:
+            raise ValueError(f"POOL_BYTES_PER_TRANSITION must be positive, not {self.POOL_BYTES_PER_TRANSITION}")
 
     @staticmethod
     def from_configuration():
@@ -75,7 +89,8 @@ class ApexConfig:
                                          "REPLAY_MEMORY_LEN", "BUFFER_SIZE", "TARGET_FREQUENCY",
                                          "LEARNER_DEVICE", "REDIS_SERVER", "OPTIM_INFO", "MODEL")}
         kw["LOG_W"] = getattr(C, "LOG_W", None)
-        for k in ("FRAME_DEDUP", "FRAMES_PER_TRANSITION", "DEDUP_WINDOW"):     # optional keys of cfg/ape_x.json
+        for k in ("FRAME_DEDUP", "FRAMES_PER_TRANSITION", "DEDUP_WINDOW", "FRAME_CODEC",
+                  "POOL_BYTES_PER_TRANSITION"):                                # optional keys of cfg/ape_x.json
             if hasattr(C, k):
                 kw[k] = getattr(C, k)
         return ApexConfig(**kw)
@@ -94,6 +109,20 @@ def dedup_geometry(cfg: ApexConfig) -> tuple:
         warnings.warn(f"DEDUP_WINDOW = {cfg.DEDUP_WINDOW} frames is more than an eighth of the {F}-frame pool: the "
                       f"frame-deduplicated replay uses a window of {W} frames", stacklevel=2)
     return F, W
+
+
+def pool_bytes(cfg: ApexConfig) -> int | None:
+    """Bytes of a FRAME_CODEC store's frame ring (None without FRAME_CODEC): POOL_BYTES_PER_TRANSITION x
+    REPLAY_MEMORY_LEN, rounded down to 16 bytes.  The default is the raw size plus one frame, (F + 1) x 7 072 for
+    dedup_geometry's F frames, as r2d2.pool_bytes: a slot then dies by the byte rule no earlier than by the frame rule
+    (DESIGN.md §4.21).  A smaller ring trades that for memory, at the mean stored bytes per frame codec_stats()
+    reports; it must hold 7 072 (W + 10) bytes whatever the frames (§4.22)."""
+    import math
+    if not cfg.FRAME_CODEC:
+        return None
+    if cfg.POOL_BYTES_PER_TRANSITION is None:
+        return (int(math.ceil(cfg.FRAMES_PER_TRANSITION * cfg.REPLAY_MEMORY_LEN)) + 1) * 7072
+    return int(cfg.POOL_BYTES_PER_TRANSITION * cfg.REPLAY_MEMORY_LEN) // 16 * 16
 
 
 def default_apex_model() -> dict:
@@ -118,7 +147,10 @@ class Replay(ReplayThread):
 
     def __init__(self, cfg: ApexConfig | None = None, connect=None):
         super().__init__(cfg or ApexConfig.from_configuration(), connect)
-        if self.cfg.FRAME_DEDUP:
+        if self.cfg.FRAME_CODEC:
+            self.store = R.CodedDedupReplay(self.cfg.REPLAY_MEMORY_LEN, *dedup_geometry(self.cfg), pool_bytes(self.cfg),
+                                            device=self.device)
+        elif self.cfg.FRAME_DEDUP:
             self.store = R.DedupReplay(self.cfg.REPLAY_MEMORY_LEN, *dedup_geometry(self.cfg), device=self.device)
         else:
             self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, R.APEX_FIELDS, self.device)

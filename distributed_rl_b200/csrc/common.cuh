@@ -162,10 +162,12 @@ int dedup_rollout_stacks(const b2rl_replay* h);   // T + 1 of a rollout handle (
 // The (n, R, 84, 84) strips of the sampled slots clamp_row(idx_dev[k]) of a strip handle whose pool is on the host,
 // assembled from the pool through 16-byte loads of its mapped frames (hostrows.cu).  dst_dev 16-byte aligned.
 int gather_host_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, cudaStream_t st);
-bool dedup_pool_coded(const b2rl_replay* h);      // b2rl_dedup_attach_strips_coded: frames encoded in a unit ring
-// The (n, R, 84, 84) strips of the sampled slots clamp_row(idx_dev[k]) of a strip handle whose pool is coded, decoded
-// from the pool (dedup.cu).  dst_dev 16-byte aligned.
-int gather_coded_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, cudaStream_t st);
+bool dedup_pool_coded(const b2rl_replay* h);      // b2rl_dedup_attach_strips_coded, _coded: frames encoded in a unit ring
+// The frames of the sampled slots clamp_row(idx_dev[k]) of a handle whose pool is coded, decoded from the pool
+// (dedup.cu): a strip handle's (n, R, 84, 84) strips into dst_dev (dst2_dev NULL), an Ape-X handle's s and s' stacks
+// into dst_dev and dst2_dev (either may be NULL).  Outputs 16-byte aligned.
+int gather_coded_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, uint8_t* dst2_dev,
+                        cudaStream_t st);
 }  // namespace b2rl
 
 // The opaque handle.

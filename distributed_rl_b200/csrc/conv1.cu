@@ -27,6 +27,13 @@
 //                frames.cuh: base + row * row_stride (a stride of 7 056 reads the overlapping 4-frame windows of a
 //                frame strip: channel c of row r is frame r + c), or four 7 056-byte frames of a frame pool named by
 //                a plane table
+//
+// A coded frame pool (FrameKind::CodedPlanes, b2rl_dedup_attach_coded) keeps the rule that the sampled frames never
+// pass through HBM: the im2col producers decode them (frame_codec.cuh) straight into the raw buffers.  The encodings
+// are read from global memory (a few hundred bytes per frame, L1/L2-resident once the row tables are prepared), and
+// the loader warp loads only the weights.  The producers decode one frame of the next stack after each tile of the
+// current one, and the rest after its last tile, so the consumers' MMAs on the staged A tiles overlap the decoding;
+// raw buffer s is then handed over by a named barrier of the producers instead of raw_full / raw_empty.
 #include "common.cuh"
 #include "frames.cuh"
 #include "hopper.cuh"
@@ -136,6 +143,7 @@ k_conv1_fused(const __grid_constant__ Params P) {
   uint8_t* sB = smem;
   uint8_t* sA = smem + B_BYTES;
   uint8_t* sRaw = sA + A_STAGES * A_TILE_BYTES;
+  FcRows* sRows = reinterpret_cast<FcRows*>(sRaw + 2 * RAW_STRIDE);   // CodedPlanes: the decoders' row tables
   __shared__ __align__(8) uint64_t b_full, raw_full[2], raw_empty[2], a_full[A_STAGES], a_empty[A_STAGES];
   __shared__ float s_scale[2 * C_OUT_MAX];
   if (threadIdx.x < N_NETS * C_OUT) s_scale[threadIdx.x] = P.scale[threadIdx.x] * (1.0f / 128.0f);   // exact
@@ -161,13 +169,15 @@ k_conv1_fused(const __grid_constant__ Params P) {
       mbar_expect_tx(&b_full, B_BYTES);
       constexpr int LOAD_CHUNK = (B_BYTES < 32768) ? B_BYTES : 32768;
       for (int off = 0; off < B_BYTES; off += LOAD_CHUNK) bulk_g2s(sB + off, P.bq + off, LOAD_CHUNK, &b_full);
-      int it = 0;
-      for (int64_t k = k_first; k < k_end; ++k, ++it) {
-        const int s = it & 1;
-        mbar_wait(&raw_empty[s], ((it >> 1) & 1) ^ 1);
-        int64_t row = P.idx ? P.idx[k] : k;
-        row = row < 0 ? 0 : (row >= P.src.rows ? P.src.rows - 1 : row);
-        load_row<KIND>(P.src, frames, row, sRaw + s * RAW_STRIDE, &raw_full[s]);
+      if constexpr (KIND != FrameKind::CodedPlanes) {
+        int it = 0;
+        for (int64_t k = k_first; k < k_end; ++k, ++it) {
+          const int s = it & 1;
+          mbar_wait(&raw_empty[s], ((it >> 1) & 1) ^ 1);
+          int64_t row = P.idx ? P.idx[k] : k;
+          row = row < 0 ? 0 : (row >= P.src.rows ? P.src.rows - 1 : row);
+          load_row<KIND>(P.src, frames, row, sRaw + s * RAW_STRIDE, &raw_full[s]);
+        }
       }
     }
   } else if (warp >= CONSUMERS / 32) {
@@ -175,11 +185,28 @@ k_conv1_fused(const __grid_constant__ Params P) {
     const int pt = threadIdx.x - CONSUMERS;      // 0..255
     const int r_local = pt & (TILE_M - 1);       // A-tile row
     const int chalf = pt >> 7;                   // this thread converts channels 2*chalf, 2*chalf+1 (one K chunk)
+    // CodedPlanes: frame c of stack k -> raw buffer `raw`, decoded by the eight producer warps together
+    const int pw = pt >> 5;
+    auto decode = [&](int64_t k, int c, uint8_t* raw) {
+      int64_t row = P.idx ? P.idx[k] : k;
+      row = row < 0 ? 0 : (row >= P.src.rows ? P.src.rows - 1 : row);
+      decode_frame<PRODUCERS / 32>(coded_frame(P.src, row, c), raw + c * PLANE_BYTES, sRows, c & 1, 1, pw, lane);
+    };
+    if constexpr (KIND == FrameKind::CodedPlanes) {
+      if (k_first < k_end) {
+#pragma unroll 1
+        for (int c = 0; c < C_IN; ++c) decode(k_first, c, sRaw);
+        named_sync(1, PRODUCERS);
+      }
+    }
     int at = 0, it = 0;
     for (int64_t k = k_first; k < k_end; ++k, ++it) {
       const int s = it & 1;
-      mbar_wait(&raw_full[s], (it >> 1) & 1);
+      if constexpr (KIND != FrameKind::CodedPlanes) mbar_wait(&raw_full[s], (it >> 1) & 1);
       const uint8_t* raw = sRaw + s * RAW_STRIDE;
+      // CodedPlanes: buffer s ^ 1 was last read for stack k - 1, before the barrier that ended it
+      uint8_t* raw_next = sRaw + (s ^ 1) * RAW_STRIDE;
+      int c_next = k + 1 < k_end ? 0 : C_IN;     // frames of stack k + 1 decoded so far
       const int t_lo = (int)max((int64_t)0, u0 - k * TILES), t_hi = (int)min((int64_t)TILES, u1 - k * TILES);
       for (int t = t_lo; t < t_hi; ++t, ++at) {
         const int stage = at % A_STAGES;
@@ -206,8 +233,16 @@ k_conv1_fused(const __grid_constant__ Params P) {
         }
         fence_async_smem();            // generic-proxy writes -> visible to the tensor core (async proxy)
         mbar_arrive(&a_full[stage]);
+        if constexpr (KIND == FrameKind::CodedPlanes)
+          if (c_next < C_IN) decode(k + 1, c_next++, raw_next);
       }
-      mbar_arrive(&raw_empty[s]);      // this thread is done reading the raw frame
+      if constexpr (KIND == FrameKind::CodedPlanes) {
+#pragma unroll 1
+        for (; c_next < C_IN; ++c_next) decode(k + 1, c_next, raw_next);
+        named_sync(1, PRODUCERS);      // stack k + 1 is in raw_next, and every producer is done reading raw
+      } else {
+        mbar_arrive(&raw_empty[s]);    // this thread is done reading the raw frame
+      }
     }
   } else {
     // ------------------------- consumers: wgmma + epilogue -------------------------
@@ -276,9 +311,10 @@ k_conv1_fused(const __grid_constant__ Params P) {
   }
 }
 
-template <int N_NETS, int C_OUT>
+template <int N_NETS, int C_OUT, FrameKind KIND>
 constexpr size_t smem_bytes() {
-  return (size_t)N_NETS * NSPLIT * C_OUT * K_TOTAL + (size_t)A_STAGES * A_TILE_BYTES + 2 * (size_t)RAW_STRIDE + 1024;
+  return (size_t)N_NETS * NSPLIT * C_OUT * K_TOTAL + (size_t)A_STAGES * A_TILE_BYTES + 2 * (size_t)RAW_STRIDE + 1024 +
+         (KIND == FrameKind::CodedPlanes ? DECODE_TABLES * sizeof(FcRows) : 0);
 }
 
 }  // namespace conv1
@@ -322,9 +358,9 @@ static cudaError_t conv1_launch(const conv1::Params& P, unsigned grid, cudaStrea
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e == cudaSuccess)
-    e = set_max_dynamic_smem<conv1::k_conv1_fused<N_NETS, C_OUT, KIND>>(dev, conv1::smem_bytes<N_NETS, C_OUT>());
+    e = set_max_dynamic_smem<conv1::k_conv1_fused<N_NETS, C_OUT, KIND>>(dev, conv1::smem_bytes<N_NETS, C_OUT, KIND>());
   if (e != cudaSuccess) return e;
-  conv1::k_conv1_fused<N_NETS, C_OUT, KIND><<<grid, conv1::THREADS, conv1::smem_bytes<N_NETS, C_OUT>(), st>>>(P);
+  conv1::k_conv1_fused<N_NETS, C_OUT, KIND><<<grid, conv1::THREADS, conv1::smem_bytes<N_NETS, C_OUT, KIND>(), st>>>(P);
   return cudaSuccess;
 }
 

@@ -26,6 +26,11 @@
 //                 (warp = 8 channels x half of a chunk's 16-position units)
 //   thread 0 also issues the TMA bulk copy of the next frame stack when it starts on a stack's first chunk: the
 //   buffer it overwrites was last read two stacks before, by chunks that every producer has finished
+//
+// A coded frame pool (FrameKind::CodedPlanes, b2rl_dedup_attach_coded): no TMA copy.  The A producers decode the
+// frames (frame_codec.cuh) from global memory straight into the raw buffer, frame j of stack it + 1 after building
+// chunk j of stack it, so the decoding fills the time the A producers would spend waiting for the B producers.  The
+// per-chunk barrier that publishes a chunk also publishes the decoded frames; stack 0 is decoded before the loop.
 #include "common.cuh"
 #include "frames.cuh"
 #include "hopper.cuh"
@@ -88,6 +93,7 @@ k_conv1_wgrad(const __grid_constant__ Params P) {
   uint8_t* sStage = smem;
   uint8_t* sZero = smem + STAGES * STAGE_BYTES;        // a B operand of zeros: the K steps past position 415
   uint8_t* sRaw = sZero + B_BYTES;
+  FcRows* sRows = reinterpret_cast<FcRows*>(sRaw + 2 * RAW_STRIDE);   // CodedPlanes: the decoders' row tables
   __shared__ __align__(8) uint64_t raw_full[2];
   __shared__ uint32_t s_absmax[32];                    // per channel: bits of max |gy| over this CTA's items
 
@@ -111,9 +117,26 @@ k_conv1_wgrad(const __grid_constant__ Params P) {
     row = row < 0 ? 0 : (row >= P.src.rows ? P.src.rows - 1 : row);
     load_row<KIND>(P.src, frames, row, sRaw + (it & 1) * RAW_STRIDE, &raw_full[it & 1]);
   };
-  if (threadIdx.x == 0) load_frame(0);
+  // CodedPlanes: frame c of the CTA's stack `it` -> raw buffer it & 1, decoded by the eight A producer warps together
+  auto decode = [&](int64_t it, int c) {
+    const int64_t k = first + it * stride;
+    if (k >= P.n) return;
+    int64_t row = P.idx ? P.idx[k] : k;
+    row = row < 0 ? 0 : (row >= P.src.rows ? P.src.rows - 1 : row);
+    decode_frame<A_PRODUCERS / 32>(coded_frame(P.src, row, c), sRaw + (it & 1) * RAW_STRIDE + c * PLANE_BYTES,
+                                   sRows, c & 1, 3, warp, lane);
+  };
+  if constexpr (KIND != FrameKind::CodedPlanes) {
+    if (threadIdx.x == 0) load_frame(0);
+  }
 
   const bool is_a = warp < A_PRODUCERS / 32;
+  if constexpr (KIND == FrameKind::CodedPlanes) {
+    if (is_a) {
+      for (int c = 0; c < C_IN; ++c) decode(0, c);
+      named_sync(3, A_PRODUCERS);
+    }
+  }
   // -------- the B producers first find max |gy| per channel over this CTA's items (the digit scale);
   //          the A producers need no scale and build the first chunk meanwhile --------
   if (!is_a) {
@@ -189,9 +212,11 @@ k_conv1_wgrad(const __grid_constant__ Params P) {
     if (is_a) {
       // ------------------- A: transposed im2col, uint8 -------------------
       const int it = at >> 2, s = it & 1;
-      if (j == 0) {
-        if (threadIdx.x == 0) load_frame(it + 1);
-        mbar_wait(&raw_full[s], (it >> 1) & 1);
+      if constexpr (KIND != FrameKind::CodedPlanes) {
+        if (j == 0) {
+          if (threadIdx.x == 0) load_frame(it + 1);
+          mbar_wait(&raw_full[s], (it >> 1) & 1);
+        }
       }
       const uint8_t* raw = sRaw + s * RAW_STRIDE;
       const int p0 = j * KCHUNK + 4 * lane;          // this lane's 4 consecutive positions (same oy: 20 % 4 == 0)
@@ -268,6 +293,15 @@ k_conv1_wgrad(const __grid_constant__ Params P) {
       acc.mma(make_desc(a_base + ks * 32), make_desc((ks == 0 ? b_base : b_tail) + ks * 32), (at | ks) ? 1u : 0u);
     wg_commit();
     wg_wait<1>();
+    if constexpr (KIND == FrameKind::CodedPlanes) {
+      // frame j of the next stack, while this chunk's MMAs run; buffer (it + 1) & 1 was last read for stack it - 1,
+      // before the barrier of this stack's chunk 0, and the barrier after the last frame publishes the stack
+      if (is_a) {
+        const int64_t it = at >> 2;
+        decode(it + 1, j);
+        if (j == CHUNKS - 1) named_sync(3, A_PRODUCERS);
+      }
+    }
   }
   wg_wait<0>();
   wg_fence_regs(acc.d);
@@ -324,9 +358,10 @@ k_conv1_wgrad_reduce(const float* __restrict__ partial, int n_parts, int numel, 
   }
 }
 
-template <int C_OUT>
+template <int C_OUT, FrameKind KIND>
 constexpr size_t smem_bytes() {
-  return (size_t)STAGES * (A_BYTES + NSPLIT * C_OUT * KCHUNK) + 2 * (size_t)RAW_STRIDE + NSPLIT * C_OUT * KCHUNK + 1024;
+  return (size_t)STAGES * (A_BYTES + NSPLIT * C_OUT * KCHUNK) + 2 * (size_t)RAW_STRIDE + NSPLIT * C_OUT * KCHUNK + 1024 +
+         (KIND == FrameKind::CodedPlanes ? DECODE_TABLES * sizeof(FcRows) : 0);
 }
 
 }  // namespace conv1w
@@ -339,9 +374,9 @@ static cudaError_t wgrad_launch(const conv1w::Params& P, unsigned grid, cudaStre
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e == cudaSuccess)
-    e = set_max_dynamic_smem<conv1w::k_conv1_wgrad<C_OUT, KIND>>(dev, conv1w::smem_bytes<C_OUT>());
+    e = set_max_dynamic_smem<conv1w::k_conv1_wgrad<C_OUT, KIND>>(dev, conv1w::smem_bytes<C_OUT, KIND>());
   if (e != cudaSuccess) return e;
-  conv1w::k_conv1_wgrad<C_OUT, KIND><<<grid, conv1w::THREADS, conv1w::smem_bytes<C_OUT>(), st>>>(P);
+  conv1w::k_conv1_wgrad<C_OUT, KIND><<<grid, conv1w::THREADS, conv1w::smem_bytes<C_OUT, KIND>(), st>>>(P);
   return cudaSuccess;
 }
 

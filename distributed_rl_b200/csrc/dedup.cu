@@ -22,11 +22,12 @@
 // The kernels are the same: k_dedup_resolve compares a hit's frame and k_dedup_copy stores the misses through the
 // pool's device alias with plain 16-byte loads and stores, over PCIe, in order on the push's stream.  The key
 // tables, pool_key and the batch scratch stay in HBM.
-// A strip handle's pool may instead be a ring of P 16-byte units holding each frame losslessly encoded
-// (b2rl_dedup_attach_strips_coded, frame_codec.cuh, DESIGN.md §4.21).  Frame seq's entry seq % F is then a descriptor
+// A strip or Ape-X handle's pool may instead be a ring of P 16-byte units holding each frame losslessly encoded
+// (b2rl_dedup_attach_strips_coded, b2rl_dedup_attach_coded, frame_codec.cuh, DESIGN.md §4.21, §4.22).  Frame seq's entry seq % F is then a descriptor
 // (absolute unit offset, length) and the same ids name it.  k_coded_resolve compares a hit's encoding with the frame
 // by decoding it, and sizes the misses; k_coded_offsets lays them out in the unit ring (a frame never straddles its
-// end); k_coded_copy encodes them in place.  The readers decode each sampled slot's frames (k_decode_planes).
+// end); k_coded_copy encodes them in place.  The readers decode each sampled slot's frames (k_decode_planes), and conv_1
+// decodes an Ape-X pool's frames on chip (frames.cuh, FrameKind::CodedPlanes).
 #include "common.cuh"
 #include "frame_codec.cuh"
 
@@ -76,7 +77,8 @@ struct DedupState {
   cudaEvent_t done = nullptr;                     // recorded behind each push: the next one waits for it, so pushes
                                                   // on different streams never share the scratch or the key table
   std::vector<int64_t> ins;                       // per slot: head at the start of the batch that inserted it
-  // b2rl_dedup_attach_strips_coded: pool is a ring of P 16-byte units of encoded frames, then FC_RAW_BYTES of zeros
+  // b2rl_dedup_attach_strips_coded, _coded: pool is a ring of P 16-byte units of encoded frames, then FC_RAW_BYTES of
+  // zeros
   int64_t P = 0;                                  // 0: frames stored raw, frame seq at pool + (seq % F) 7056
   int64_t units = 0;                              // units written so far, wrap padding included
   int64_t* foff = nullptr;                        // [F] absolute unit offset of the frame in each entry
@@ -293,10 +295,11 @@ k_dedup_rebuild(const unsigned long long* __restrict__ pool_key, int64_t F, int6
   atomicMax(tseq + claim(tkey, T, pool_key[q % F]), (unsigned long long)(q + 1));
 }
 
-// ---- the coded pool (b2rl_dedup_attach_strips_coded): frames as frame_codec.cuh encodings in a ring of P units ----
+// ---- the coded pool (b2rl_dedup_attach_strips_coded, _coded): frames as frame_codec.cuh encodings in a ring of P
+// units ----
 
-// k_dedup_resolve for a coded pool (strips): a hit's stored encoding is decoded and compared with the frame, and
-// every miss gets the length of its encoding in usz.
+// k_dedup_resolve for a coded pool: a hit's stored encoding is decoded and compared with the frame, and every miss
+// gets the length of its encoding in usz.
 struct CodedResolveArgs {
   const uint8_t* s;
   int64_t frames;
@@ -315,8 +318,10 @@ struct CodedResolveArgs {
   int32_t* rep;
   int64_t* fseq;
   int32_t* usz;
+  const uint8_t* ns;        // Pairs: the s' stacks
 };
 
+template <Layout L>
 __global__ void __launch_bounds__(DD_THREADS)
 k_coded_resolve(const __grid_constant__ CodedResolveArgs A) {
   __shared__ FcRows s_rows[DD_THREADS / 32];
@@ -324,9 +329,9 @@ k_coded_resolve(const __grid_constant__ CodedResolveArgs A) {
   const int lane = threadIdx.x & 31;
   if (j >= A.frames) return;
   const unsigned long long k = A.key[j];
-  const uint8_t* me = A.s + j * DD_FRAME;
+  const uint8_t* me = batch_frame<L>(A.s, A.ns, j);
   const int32_t first = A.bpos[find(A.bkey, A.BT, k)];
-  if (first < j && warp_equal(A.s + (int64_t)first * DD_FRAME, me, lane)) {
+  if (first < j && warp_equal(batch_frame<L>(A.s, A.ns, first), me, lane)) {
     if (lane == 0) { A.rep[j] = first; A.fseq[j] = -2; }
     return;
   }
@@ -409,9 +414,11 @@ struct CodedCopyArgs {
   int32_t* planes;          // the replay's planes field
   int64_t slot0, capacity;  // record r goes to slot (slot0 + r) % capacity
   int32_t R;
+  const uint8_t* ns;        // Pairs: the s' stacks
 };
 
 // k_dedup_copy for a coded pool: each miss is encoded in place at its unit offset, and its entry gets the descriptor.
+template <Layout L>
 __global__ void __launch_bounds__(DD_THREADS)
 k_coded_copy(const __grid_constant__ CodedCopyArgs A) {
   const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
@@ -428,7 +435,7 @@ k_coded_copy(const __grid_constant__ CodedCopyArgs A) {
   }
   if (r != j || sq < A.head) return;        // a batch duplicate or a hit: nothing to store
   const int64_t off = A.uoff[j];
-  fc_encode(A.s + j * DD_FRAME, A.pool + (off % A.P) * 16, lane);
+  fc_encode(batch_frame<L>(A.s, A.ns, j), A.pool + (off % A.P) * 16, lane);
   if (lane == 0) {
     const unsigned long long k = A.key[j];
     A.foff[ps] = off;
@@ -438,20 +445,30 @@ k_coded_copy(const __grid_constant__ CodedCopyArgs A) {
   }
 }
 
-// dst frame j of draw k = j / R: slot clamp_row(idx[k])'s frame j % R, decoded from the pool.  One warp per frame.
+// Frame j of draw k = j / R: slot clamp_row(idx[k])'s frame j % R, decoded from the pool.  One warp per frame.
+// Strips: into dst + j * 7 056, the (n, R, 84, 84) strips.  Pairs (R = 8): planes 0-3 into the (n, 4, 84, 84) s stacks
+// at dst, planes 4-7 into the s' stacks at dst2; a NULL output's frames are skipped.
+template <Layout L>
 __global__ void __launch_bounds__(DD_THREADS)
 k_decode_planes(const uint8_t* __restrict__ pool, int64_t P, const int64_t* __restrict__ foff, int64_t F,
                 const int32_t* __restrict__ planes, int32_t R, const int64_t* __restrict__ idx, int64_t n,
-                int64_t capacity, uint8_t* __restrict__ dst) {
+                int64_t capacity, uint8_t* __restrict__ dst, uint8_t* __restrict__ dst2) {
   __shared__ FcRows s_rows[DD_THREADS / 32];
   const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (j >= n * R) return;
   const int64_t k = j / R;
+  uint8_t* out = dst + j * DD_FRAME;
+  if constexpr (L == Layout::Pairs) {
+    const int c = (int)(j - k * R);
+    out = (c < 4 ? dst : dst2);
+    if (out == nullptr) return;
+    out += (4 * k + (c & 3)) * DD_FRAME;
+  }
   int64_t slot = idx[k];
   slot = slot < 0 ? 0 : (slot >= capacity ? capacity - 1 : slot);
   const int64_t id = (uint32_t)planes[R * slot + (j - k * R)] % (uint64_t)F;   // any int32 names an entry
-  fc_decode(pool + (foff[id] % P) * 16, dst + j * DD_FRAME, s_rows[threadIdx.x >> 5], lane);
+  fc_decode(pool + (foff[id] % P) * 16, out, s_rows[threadIdx.x >> 5], lane);
 }
 
 // b2rl_frame_encode / b2rl_frame_decode: frame j <-> the encoding at enc + j * FC_RAW_BYTES.  One warp per frame.
@@ -498,13 +515,18 @@ bool dedup_pool_coded(const b2rl_replay* h) { return h->dedup->P > 0; }
 
 static unsigned warps_grid(int64_t frames) { return (unsigned)((frames * 32 + DD_THREADS - 1) / DD_THREADS); }
 
-int gather_coded_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, cudaStream_t st) {
-  B2RL_REQUIRE((uintptr_t)dst_dev % 16 == 0, "frame strip outputs must be 16-byte aligned");
-  if (n == 0) return B2RL_OK;
+int gather_coded_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, uint8_t* dst2_dev,
+                        cudaStream_t st) {
   const DedupState* d = h->dedup;
-  k_decode_planes<<<warps_grid(n * d->R), DD_THREADS, 0, st>>>(d->pool, d->P, d->foff, d->F,
-                                                               (const int32_t*)h->field[d->planes_field], d->R,
-                                                               idx_dev, n, h->capacity, dst_dev);
+  const bool pairs = d->layout == Layout::Pairs;
+  B2RL_REQUIRE((uintptr_t)dst_dev % 16 == 0 && (uintptr_t)dst2_dev % 16 == 0,
+               pairs ? "frame stack outputs must be 16-byte aligned" : "frame strip outputs must be 16-byte aligned");
+  B2RL_REQUIRE(pairs || dst2_dev == nullptr, "a strip handle has one frame output");
+  if (n == 0 || (dst_dev == nullptr && dst2_dev == nullptr)) return B2RL_OK;
+  auto kernel = pairs ? k_decode_planes<Layout::Pairs> : k_decode_planes<Layout::Strips>;
+  kernel<<<warps_grid(n * d->R), DD_THREADS, 0, st>>>(d->pool, d->P, d->foff, d->F,
+                                                      (const int32_t*)h->field[d->planes_field], d->R, idx_dev, n,
+                                                      h->capacity, dst_dev, dst2_dev);
   count_launch();
   B2RL_CHECK_LAUNCH();
   return B2RL_OK;
@@ -520,15 +542,15 @@ static int64_t pow2_at_least(int64_t x) {
   return p;
 }
 
-// b2rl_dedup_attach (Pairs, R = 8), b2rl_dedup_attach_strips, _placed and _coded (Strips, R = frames_per_record).
+// b2rl_dedup_attach and _coded (Pairs, R = 8), b2rl_dedup_attach_strips, _placed and _strips_coded (Strips, R =
+// frames_per_record).
 // pool_bytes > 0: a coded pool of pool_bytes / 16 units.  The arguments are checked before the handle, so every
 // refusal comes before any CUDA work.
 static int dedup_attach(b2rl_replay* h, int32_t planes_field, Layout layout, int32_t R, int64_t pool_frames,
                         int64_t window, uint64_t hash_mask, bool pool_on_host, int64_t pool_bytes = 0) {
   B2RL_REQUIRE(!pool_on_host || layout == Layout::Strips,
                "an Ape-X (Pairs) frame pool stays in HBM: only a strip handle's pool can be placed on the host");
-  B2RL_REQUIRE(pool_bytes == 0 || (layout == Layout::Strips && !pool_on_host),
-               "only a strip handle's pool in HBM can be coded");
+  B2RL_REQUIRE(pool_bytes == 0 || !pool_on_host, "a coded frame pool stays in HBM: it cannot be placed on the host");
   B2RL_REQUIRE(R >= 4 && R <= DD_MAX_FRAMES, "frames_per_record must be in [4, 65536]");
   B2RL_REQUIRE(window >= 0 && pool_frames - window > R,
                layout == Layout::Pairs ? "need window >= 0 and pool_frames - window > 8"
@@ -536,7 +558,8 @@ static int dedup_attach(b2rl_replay* h, int32_t planes_field, Layout layout, int
   B2RL_REQUIRE(pool_frames < (1LL << 31), "pool_frames must be below 2^31");
   B2RL_REQUIRE(pool_bytes >= 0 && pool_bytes % 16 == 0, "pool_bytes must be a non-negative multiple of 16");
   B2RL_REQUIRE(pool_bytes == 0 || pool_bytes / 16 - (window + 2) * FC_RAW_UNITS >= (int64_t)R * FC_RAW_UNITS,
-               "need pool_bytes >= 7072 (window + 2 + frames_per_record): one record beyond the window");
+               layout == Layout::Pairs ? "need pool_bytes >= 7072 (window + 10): one record beyond the window"
+                                       : "need pool_bytes >= 7072 (window + 2 + frames_per_record): one record beyond the window");
   B2RL_REQUIRE(h != nullptr, "null handle");
   B2RL_REQUIRE(h->dedup == nullptr, "the replay already has a frame pool");
   B2RL_REQUIRE(!h->any_on_host, "a replay with fields placed on the host cannot take a frame pool");
@@ -656,6 +679,12 @@ extern "C" int b2rl_dedup_attach_strips_coded(b2rl_replay* h, int32_t planes_fie
                       pool_bytes);
 }
 
+extern "C" int b2rl_dedup_attach_coded(b2rl_replay* h, int32_t planes_field, int64_t pool_frames, int64_t window,
+                                       uint64_t hash_mask, int64_t pool_bytes) {
+  B2RL_REQUIRE(pool_bytes > 0, "pool_bytes must be positive");
+  return dedup_attach(h, planes_field, Layout::Pairs, 8, pool_frames, window, hash_mask, false, pool_bytes);
+}
+
 extern "C" int b2rl_dedup_attach_rollouts(b2rl_replay* h, int32_t planes_field, int32_t stacks_per_record,
                                           int64_t pool_frames, int64_t window, uint64_t hash_mask) {
   B2RL_REQUIRE(stacks_per_record >= 1 && stacks_per_record <= DD_MAX_FRAMES / 4,
@@ -678,10 +707,19 @@ extern "C" int b2rl_dedup_info(const b2rl_replay* h, void** pool_dev, int64_t* h
 extern "C" int b2rl_dedup_codec_stats(const b2rl_replay* h, int64_t* units_written, int64_t* pool_units,
                                       int64_t* frames_stored) {
   B2RL_REQUIRE(h != nullptr, "null handle");
-  B2RL_REQUIRE(h->dedup != nullptr && h->dedup->P > 0, "not a coded frame pool (b2rl_dedup_attach_strips_coded)");
+  B2RL_REQUIRE(h->dedup != nullptr && h->dedup->P > 0,
+               "not a coded frame pool (b2rl_dedup_attach_strips_coded, b2rl_dedup_attach_coded)");
   if (units_written) *units_written = h->dedup->units;
   if (pool_units) *pool_units = h->dedup->P;
   if (frames_stored) *frames_stored = h->dedup->head;
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_dedup_coded_offsets(const b2rl_replay* h, void** offsets_dev) {
+  B2RL_REQUIRE(h != nullptr && offsets_dev != nullptr, "null argument");
+  B2RL_REQUIRE(h->dedup != nullptr && h->dedup->P > 0,
+               "not a coded frame pool (b2rl_dedup_attach_strips_coded, b2rl_dedup_attach_coded)");
+  *offsets_dev = h->dedup->foff;
   return B2RL_OK;
 }
 
@@ -745,11 +783,11 @@ static int dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8_t* ns_de
   B2RL_CUDA(cudaMemsetAsync(d->bpos, 0x7F, sizeof(int32_t) * (size_t)d->BT, st));
   k_dedup_hash<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(s_dev, ns_dev, frames, d->mask, d->key, d->bkey, d->bpos,
                                                           d->BT);
-  const bool coded = L == Layout::Strips && d->P > 0;
+  const bool coded = d->P > 0;
   if (coded) {
     CodedResolveArgs A{s_dev, frames, d->key, d->bkey, d->bpos, d->BT, d->tkey, d->tseq, d->T, d->pool, d->P,
-                       d->foff, d->F, head - d->W, d->rep, d->fseq, d->usz};
-    k_coded_resolve<<<warps_grid(frames), DD_THREADS, 0, st>>>(A);
+                       d->foff, d->F, head - d->W, d->rep, d->fseq, d->usz, ns_dev};
+    k_coded_resolve<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(A);
   } else {
     ResolveArgs A{s_dev, ns_dev, frames, d->key, d->bkey, d->bpos, d->BT, d->tkey, d->tseq, d->T, d->pool, d->F,
                   head - d->W, d->rep, d->fseq};
@@ -787,8 +825,8 @@ static int dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8_t* ns_de
   if (coded) {
     CodedCopyArgs C{s_dev, frames, d->key, d->rep, d->fseq, head, d->uoff, d->usz, d->pool, d->P, d->foff, d->flen,
                     d->pool_key, d->F, d->tkey, d->tseq, d->T, (int32_t*)h->field[d->planes_field], h->head,
-                    h->capacity, d->R};
-    k_coded_copy<<<warps_grid(frames), DD_THREADS, 0, st>>>(C);
+                    h->capacity, d->R, ns_dev};
+    k_coded_copy<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(C);
   } else {
     CopyArgs C{s_dev, ns_dev, frames, d->key, d->rep, d->fseq, head, d->pool, d->pool_key, d->F, d->tkey, d->tseq,
                d->T, (int32_t*)h->field[d->planes_field], h->head, h->capacity, d->R};

@@ -147,11 +147,14 @@ static int gather_run(b2rl_replay* h, const int64_t* idx_dev, int64_t n, void* c
         const int rc = gather_host_planes(h, idx_dev, n, (uint8_t*)stacks_out[0], st);
         if (rc != B2RL_OK) return rc;
       } else if (stacks_out[0] != nullptr && dedup_pool_coded(h)) {   // decoded from the unit ring (dedup.cu)
-        const int rc = gather_coded_planes(h, idx_dev, n, (uint8_t*)stacks_out[0], st);
+        const int rc = gather_coded_planes(h, idx_dev, n, (uint8_t*)stacks_out[0], nullptr, st);
         if (rc != B2RL_OK) return rc;
       } else if (stacks_out[0] != nullptr) {
         P.bulk.add_planes(dedup_pool(h), planes, R, 0, R, (uint8_t*)stacks_out[0]);
       }
+    } else if (dedup_pool_coded(h)) {   // s and s' decoded from the unit ring (dedup.cu)
+      const int rc = gather_coded_planes(h, idx_dev, n, (uint8_t*)stacks_out[0], (uint8_t*)stacks_out[1], st);
+      if (rc != B2RL_OK) return rc;
     } else {
       for (int i = 0; i < 2; ++i) {
         B2RL_REQUIRE((uintptr_t)stacks_out[i] % 16 == 0, "frame stack outputs must be 16-byte aligned");

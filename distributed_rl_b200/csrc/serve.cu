@@ -395,7 +395,8 @@ extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot,
     } else if (h->dedup != nullptr && f == dedup_planes_field(h) && dedup_pool_on_host(h)) {
       host_planes_o = o;         // the strips of a host pool: likewise, by the host-plane gather (hostrows.cu)
     } else if (h->dedup != nullptr && f == dedup_planes_field(h) && dedup_pool_coded(h)) {
-      coded_planes_o = o;        // the strips of a coded pool: decoded after the draw, from the slot's idx (dedup.cu)
+      coded_planes_o = o;        // the strips, or s and s', of a coded pool: decoded after the draw, from the slot's
+      if (dedup_strip_frames(h) == 0) ++o;   // idx (dedup.cu)
     } else if (h->dedup != nullptr && f == dedup_planes_field(h)) {   // frames assembled from the frame pool
       const int32_t* planes = (const int32_t*)h->field[f];
       const int R = dedup_strip_frames(h);
@@ -436,7 +437,9 @@ extern "C" int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot,
   if (host_planes_o >= 0)
     return gather_host_planes(h, (const int64_t*)ptrs[1], n, (uint8_t*)ptrs[host_planes_o], (cudaStream_t)stream);
   if (coded_planes_o >= 0)
-    return gather_coded_planes(h, (const int64_t*)ptrs[1], n, (uint8_t*)ptrs[coded_planes_o], (cudaStream_t)stream);
+    return gather_coded_planes(h, (const int64_t*)ptrs[1], n, (uint8_t*)ptrs[coded_planes_o],
+                               dedup_strip_frames(h) == 0 ? (uint8_t*)ptrs[coded_planes_o + 1] : nullptr,
+                               (cudaStream_t)stream);
   return B2RL_OK;
 }
 

@@ -196,7 +196,7 @@ class Conv1Gathered(torch.autograd.Function):
                 return (None,) * len(ctx.needs_input_grad)
             gw = R.conv1_wgrad(ctx.frames, idx if ctx.has_idx else None, gy, relu_y=y)
             return (gw,) + (None,) * (len(ctx.needs_input_grad) - 1)
-        if isinstance(ctx.frames, (R.BoundFrames, R.PlaneFrames)):
+        if isinstance(ctx.frames, (R.BoundFrames, R.PlaneFrames, R.CodedPlaneFrames)):
             raise RuntimeError("conv_1 over a bound ring slot or a frame pool has no cuDNN weight gradient: set "
                                "Conv1Gathered.fused_wgrad")
         if y is not None:

@@ -541,6 +541,7 @@ class DedupReplay(DeviceReplay):
     since its batch began (len() counts live slots).  The pipelined ingest forms are refused."""
 
     RECORD_FIELDS = APEX_FIELDS      # what push takes and gather returns
+    coded = False                    # frames stored encoded (CodedDedupReplay, StripDedupReplay(pool_bytes=...))
 
     def __init__(self, capacity: int, pool_frames: int, window: int, device="cuda:0",
                  hash_mask: int = DEDUP_HASH_MASK):
@@ -559,6 +560,25 @@ class DedupReplay(DeviceReplay):
             return
         with torch.cuda.device(self.device):
             self.pool = torch.as_tensor(_CudaView(p.value, (self.pool_frames, 84, 84), "|u1", self), device=self.device)
+
+    def _coded_pool(self) -> None:
+        """`pool` of a coded store: the flat uint8 ring of 16-byte units the encodings live in, not (F, 84, 84)."""
+        p = C.c_void_p()
+        check(self.lib.b2rl_dedup_info(self._h, C.byref(p), None, None))
+        self.pool_bytes = 16 * self.codec_stats()["pool_units"]
+        with torch.cuda.device(self.device):
+            self.pool = torch.as_tensor(_CudaView(p.value, (self.pool_bytes,), "|u1", self), device=self.device)
+
+    def codec_stats(self) -> dict:
+        """A coded pool's counters (b2rl_dedup_codec_stats): units_written (16-byte units, the wrap's skipped units
+        included), pool_units, frames_stored, and bytes_per_frame = 16 units_written / frames_stored, the mean
+        stored size of a frame (7 072 at most: raw)."""
+        if not self.coded:
+            raise ValueError("codec_stats() reports a coded frame pool (pool_bytes)")
+        u, p, f = C.c_int64(), C.c_int64(), C.c_int64()
+        check(self.lib.b2rl_dedup_codec_stats(self._h, C.byref(u), C.byref(p), C.byref(f)))
+        return {"units_written": u.value, "pool_units": p.value, "frames_stored": f.value,
+                "bytes_per_frame": 16.0 * u.value / f.value if f.value else 0.0}
 
     @property
     def head_seq(self) -> int:
@@ -665,6 +685,32 @@ def decode_frames(enc: torch.Tensor, stream=None) -> torch.Tensor:
     return out
 
 
+class CodedDedupReplay(DedupReplay):
+    """DedupReplay with its frames stored losslessly encoded (b2rl_dedup_attach_coded, ApexConfig.FRAME_CODEC, DESIGN.md
+    §4.22): the pool is a device ring of pool_bytes holding each distinct frame's encoding (frame_codec.cuh), and a
+    slot also dies once pool_bytes - 7072 (window + 1) bytes have been written since its batch began.  push / gather /
+    sample / update take and return what a DedupReplay does, bit for bit, while every slot is live; gather() decodes
+    the sampled s and s' stacks.  `pool` is the flat uint8 ring, and frame_source() is a CodedPlaneFrames: conv_1
+    decodes each row's four frames on chip, so the sampled frames never pass through HBM decoded."""
+
+    def __init__(self, capacity: int, pool_frames: int, window: int, pool_bytes: int, device="cuda:0",
+                 hash_mask: int = DEDUP_HASH_MASK):
+        DeviceReplay.__init__(self, capacity, APEX_DEDUP_FIELDS, device)
+        self.coded = True
+        check(self.lib.b2rl_dedup_attach_coded(self._h, 0, int(pool_frames), int(window), int(hash_mask),
+                                               int(pool_bytes)))
+        self._attached(pool_frames, window)
+        self._coded_pool()
+        p = C.c_void_p()
+        check(self.lib.b2rl_dedup_coded_offsets(self._h, C.byref(p)))
+        with torch.cuda.device(self.device):     # the descriptor table: absolute unit offset of each pool entry
+            self.offsets = torch.as_tensor(_CudaView(p.value, (self.pool_frames,), "<i8", self), device=self.device)
+
+    def frame_source(self, name: str) -> "CodedPlaneFrames":
+        return CodedPlaneFrames(self.pool, self.field_view("planes"), self.offsets, self.pool_frames,
+                                {"state": 0, "next_state": 4}[name])
+
+
 class StripDedupReplay(DedupReplay):
     """The strip form of DedupReplay (b2rl_dedup_attach_strips, R2D2Config.FRAME_DEDUP, DESIGN.md §4.18): an R2D2
     replay whose slots hold R2D2_DEDUP_FIELDS(T), the T + 3 frames of each sequence's strip living in the frame pool.
@@ -700,22 +746,7 @@ class StripDedupReplay(DedupReplay):
             check(self.lib.b2rl_dedup_attach_strips(*args))
         self._attached(pool_frames, window)
         if self.coded:          # the encoded frames: a flat ring of 16-byte units, not (F, 84, 84) frames
-            p = C.c_void_p()
-            check(self.lib.b2rl_dedup_info(self._h, C.byref(p), None, None))
-            self.pool_bytes = 16 * self.codec_stats()["pool_units"]
-            with torch.cuda.device(self.device):
-                self.pool = torch.as_tensor(_CudaView(p.value, (self.pool_bytes,), "|u1", self), device=self.device)
-
-    def codec_stats(self) -> dict:
-        """A coded pool's counters (b2rl_dedup_codec_stats): units_written (16-byte units, the wrap's skipped units
-        included), pool_units, frames_stored, and bytes_per_frame = 16 units_written / frames_stored, the mean
-        stored size of a frame (7 072 at most: raw)."""
-        if not self.coded:
-            raise ValueError("codec_stats() reports a coded frame pool (pool_bytes)")
-        u, p, f = C.c_int64(), C.c_int64(), C.c_int64()
-        check(self.lib.b2rl_dedup_codec_stats(self._h, C.byref(u), C.byref(p), C.byref(f)))
-        return {"units_written": u.value, "pool_units": p.value, "frames_stored": f.value,
-                "bytes_per_frame": 16.0 * u.value / f.value if f.value else 0.0}
+            self._coded_pool()
 
     def push(self, fields: Sequence, priorities) -> None:
         """fields: [state, action, reward, h0, h1, notdone] as for a DeviceReplay of r2d2_fields(T, strip=True),
@@ -932,10 +963,42 @@ class PlaneFrames:
         return (self.planes.numel() - self.base - 4) // self.plane_stride + 1
 
 
+@dataclass(frozen=True)
+class CodedPlaneFrames:
+    """The Ape-X plane table over a coded frame pool (CodedDedupReplay.frame_source): row r is the stack whose channel
+    c is the frame encoded at pool[16 (offsets[id % pool_frames] % (pool.numel() / 16)):], id = planes.flatten()[8 r +
+    base + c].  `pool`: the flat uint8 ring; `offsets`: int64 (pool_frames,) descriptor table; `base` 0 for `state`,
+    4 for `next_state`.  conv1_fused / conv1_wgrad decode each row's four frames in shared memory."""
+    pool: torch.Tensor
+    planes: torch.Tensor
+    offsets: torch.Tensor
+    pool_frames: int
+    base: int
+
+    @property
+    def device(self) -> torch.device:
+        return self.pool.device
+
+    @property
+    def rows(self) -> int:
+        return (self.planes.numel() - self.base - 4) // 8 + 1
+
+
 def _frame_source(frames) -> _lib.Frames:
-    """The b2rl_frames descriptor of a frame tensor, a BoundFrames or a PlaneFrames.  A tensor's rows are its first
-    dimension, each a contiguous FRAME_STACK_BYTES; stride(0) is the row stride (the library checks that it is a
-    positive multiple of 16)."""
+    """The b2rl_frames descriptor of a frame tensor, a BoundFrames, a PlaneFrames or a CodedPlaneFrames.  A tensor's
+    rows are its first dimension, each a contiguous FRAME_STACK_BYTES; stride(0) is the row stride (the library checks
+    that it is a positive multiple of 16)."""
+    if isinstance(frames, CodedPlaneFrames):
+        if frames.pool.dim() != 1 or frames.pool.dtype != torch.uint8 or frames.pool.numel() % 16 != 0:
+            raise ValueError("a coded frame pool is a flat uint8 ring of 16-byte units")
+        if frames.pool.device.type != "cuda" or frames.offsets.device.type != "cuda":
+            raise ValueError("conv_1 decodes a coded frame pool in place on the GPU: pool and offsets must be device "
+                             "tensors")
+        if frames.offsets.dtype != torch.int64 or frames.offsets.numel() != frames.pool_frames:
+            raise ValueError("the descriptor table must be int64 (pool_frames,)")
+        return _lib.Frames(pool=frames.pool.data_ptr(), planes=frames.planes.data_ptr(), plane_base=frames.base,
+                           plane_stride=8, rows=frames.rows, offsets=frames.offsets.data_ptr(),
+                           pool_units=frames.pool.numel() // 16, pool_frames=frames.pool_frames)
     if isinstance(frames, PlaneFrames):
         if frames.pool.dim() != 3:
             raise ValueError("conv_1 reads raw (F, 84, 84) pool frames: a coded frame pool holds encoded frames; "
@@ -957,8 +1020,9 @@ def _frame_source(frames) -> _lib.Frames:
 
 def conv1_fused(frames, idx, pack: Conv1Pack, relu: bool = False, out=None):
     """frames: uint8 (rows, 4, 84, 84) with its inner three dimensions contiguous: frame stacks (e.g.
-    DeviceReplay.field_view("state")), the windows of frame strips (strip_windows), a BoundFrames or a PlaneFrames
-    (DedupReplay.frame_source, StripDedupReplay.frame_source, RolloutDedupReplay.frame_source);
+    DeviceReplay.field_view("state")), the windows of frame strips (strip_windows), a BoundFrames, a PlaneFrames
+    (DedupReplay.frame_source, StripDedupReplay.frame_source, RolloutDedupReplay.frame_source) or a CodedPlaneFrames
+    (CodedDedupReplay.frame_source);
     idx: int64[n] rows to take (None: all rows in order).
     -> list of n_nets tensors (n, c_out, 20, 20) fp32 in channels_last memory format."""
     src = _frame_source(frames)

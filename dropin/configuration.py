@@ -17,7 +17,8 @@ BASE_PATH = f"./log/{ALG}"
 if ALG == "APE_X":
     USE_REWARD_CLIP = DATA.get("USE_REWARD_CLIP", True)
     FRAME_DEDUP = bool(DATA.get("FRAME_DEDUP", False))   # not a reference key: store every distinct frame once
-    for _k in ("FRAMES_PER_TRANSITION", "DEDUP_WINDOW"):
+    FRAME_CODEC = bool(DATA.get("FRAME_CODEC", False))   # not a reference key: store that frame pool encoded
+    for _k in ("FRAMES_PER_TRANSITION", "DEDUP_WINDOW", "POOL_BYTES_PER_TRANSITION"):
         if _k in DATA:
             globals()[_k] = DATA[_k]
 elif ALG == "R2D2":

@@ -303,11 +303,24 @@ int b2rl_dedup_pool_placement(const b2rl_replay* h, int32_t* on_host, void** poo
  * records too.  Requires pool_bytes a positive multiple of 16 with P >= 442 (window + 2 + R).  b2rl_replay_gather_planes
  * and b2rl_serve_fill decode the sampled slots' strips (k_decode_planes), byte for byte the strip handle's while the
  * slots are live; a dead or never-written slot decodes to unspecified frames, read inside the pool's allocation (P
- * units plus 7 072 zeroed bytes).  The pool (*pool_dev of b2rl_dedup_info) is never a conv_1 frame source.  Arguments are checked before the handle is read. */
+ * units plus 7 072 zeroed bytes).  A strip handle's coded pool is never a conv_1 frame source.  Arguments are checked before the handle is read. */
 int b2rl_dedup_attach_strips_coded(b2rl_replay* h, int32_t planes_field, int32_t frames_per_record,
                                    int64_t pool_frames, int64_t window, uint64_t hash_mask, int64_t pool_bytes);
+/* The Ape-X store (b2rl_dedup_attach, APE_X/ReplayMemory.py:61-116) with its frames stored encoded, the Pairs twin of
+ * b2rl_dedup_attach_strips_coded: R = 8, planes 0-3 of s and 4-7 of s'.  Ids, the window, the frame rule, the byte
+ * rule and the push bound are those above with R = 8; requires P >= 442 (window + 10).  b2rl_dedup_push stores into
+ * it.  b2rl_replay_gather_planes and b2rl_serve_fill decode the sampled slots' s and s' stacks, byte for byte the raw
+ * handle's while the slots are live.  Unlike the strip form, conv_1 reads its frames in place: a b2rl_frames source
+ * with `offsets` (b2rl_dedup_coded_offsets) decodes each row's four frames on chip.  Arguments are checked before the
+ * handle is read. */
+int b2rl_dedup_attach_coded(b2rl_replay* h, int32_t planes_field, int64_t pool_frames, int64_t window,
+                            uint64_t hash_mask, int64_t pool_bytes);
+/* A coded pool's descriptor table, what CompressedDeque (baseline/utils.py:277-296) keeps as its list of pickles:
+ * *offsets_dev receives the device int64[pool_frames] absolute unit offsets of the entries (frame id i is encoded at
+ * pool + (offsets[i] % P) * 16), the `offsets` of a coded b2rl_frames source. */
+int b2rl_dedup_coded_offsets(const b2rl_replay* h, void** offsets_dev);
 /* A coded pool's counters, the sizes CompressedDeque (baseline/utils.py:277-296) leaves to pickle (each may be NULL):
- * units written so far (wrap padding included), P, and frames stored. */
+ * units written so far (wrap padding included), P, and frames stored.  Strip and Ape-X coded handles alike. */
 int b2rl_dedup_codec_stats(const b2rl_replay* h, int64_t* units_written, int64_t* pool_units, int64_t* frames_stored);
 /* The pool's codec on device buffers, as CompressedDeque.append / __getitem__ (baseline/utils.py:277-296) on one
  * frame: b2rl_frame_encode writes frame j (n frames of 7 056 bytes) to enc_dev + 7 072 j and its length in units to
@@ -389,8 +402,15 @@ int b2rl_vtrace(const float* pi_a_dev, const float* mu_a_dev, const float* value
  *           records, whose T + 3 pool ids per slot are consecutive: row slot * (T + 3) + t is stack t of the slot.
  *           plane_stride 4 (plane_base 0) reads the stacks of IMPALA rollout records (b2rl_dedup_attach_rollouts),
  *           4 (T + 1) pool ids per slot: row slot * (T + 1) + t is stack t of the slot, as in a stack store.
+ *   pool + planes + offsets (+ plane_base, pool_units, pool_frames)   an Ape-X store whose pool is coded
+ *           (b2rl_dedup_attach_coded): channel c of row r is the frame encoded at pool + (offsets[id % pool_frames] %
+ *           pool_units) * 16, id = planes[8 r + plane_base + c] read as unsigned, decoded on chip into the row's
+ *           shared-memory buffer (as CompressedDeque.__getitem__, baseline/utils.py:277-296, decodes an entry before
+ *           the learner reads it).  plane_stride must be 0 or 8, pool_units and pool_frames positive, offsets 8-byte
+ *           aligned; the pool must have 7 072 readable bytes past its last unit, as a coded handle's has.
  * row_stride (base and table) must be a positive multiple of 16.  Row indices are clamped to [0, rows), rows >= 1:
- * the caller guarantees that row rows - 1 ends inside the allocation. */
+ * the caller guarantees that row rows - 1 ends inside the allocation.  Zeroed trailing fields (offsets NULL) keep a
+ * descriptor's meaning from before they were added. */
 typedef struct {
   const uint8_t* base;
   const uint8_t* const* table;
@@ -400,6 +420,9 @@ typedef struct {
   int64_t rows;
   int32_t plane_base;
   int32_t plane_stride;
+  const int64_t* offsets;
+  int64_t pool_units;
+  int64_t pool_frames;
 } b2rl_frames;
 
 /* Fused gather + first convolution (north-star "TMA staging of sampled transition slices
