@@ -88,6 +88,8 @@ SIGNATURES = {
     "b2rl_dedup_attach_strips_coded": (C.c_int, [c_vp, c_i32, c_i32, c_i64, c_i64, c_u64, c_i64]),
     "b2rl_dedup_attach_coded": (C.c_int, [c_vp, c_i32, c_i64, c_i64, c_u64, c_i64]),
     "b2rl_dedup_coded_offsets": (C.c_int, [c_vp, C.POINTER(c_vp)]),
+    "b2rl_dedup_attach_rollouts_coded": (C.c_int, [c_vp, c_i32, c_i32, c_i64, c_i64, c_u64, c_i64]),
+    "b2rl_dedup_stage_rollouts": (C.c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_vp]),
     "b2rl_dedup_codec_stats": (C.c_int, [c_vp, C.POINTER(c_i64), C.POINTER(c_i64), C.POINTER(c_i64)]),
     "b2rl_frame_encode": (C.c_int, [c_vp, c_i64, c_vp, c_vp, c_vp]),
     "b2rl_frame_decode": (C.c_int, [c_vp, c_i64, c_vp, c_vp]),

@@ -168,6 +168,10 @@ bool dedup_pool_coded(const b2rl_replay* h);      // b2rl_dedup_attach_strips_co
 // into dst_dev and dst2_dev (either may be NULL).  Outputs 16-byte aligned.
 int gather_coded_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, uint8_t* dst2_dev,
                         cudaStream_t st);
+// The T + 1 stacks of the sampled slots clamp_row(idx_dev[k]) of a coded rollout handle, decoded time-major: stack t
+// of draw k into row t * n + k of dst_dev, as b2rl_serve_fill_uniform lays out a slot's `state` (dedup.cu).  dst_dev
+// 16-byte aligned.
+int decode_rollouts_time_major(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, cudaStream_t st);
 }  // namespace b2rl
 
 // The opaque handle.

@@ -27,7 +27,10 @@
 // (absolute unit offset, length) and the same ids name it.  k_coded_resolve compares a hit's encoding with the frame
 // by decoding it, and sizes the misses; k_coded_offsets lays them out in the unit ring (a frame never straddles its
 // end); k_coded_copy encodes them in place.  The readers decode each sampled slot's frames (k_decode_planes), and conv_1
-// decodes an Ape-X pool's frames on chip (frames.cuh, FrameKind::CodedPlanes).
+// decodes an Ape-X pool's frames on chip (frames.cuh, FrameKind::CodedPlanes).  A rollout handle's pool is coded too
+// (b2rl_dedup_attach_rollouts_coded, DESIGN.md §4.23): its learner step decodes each drawn rollout's distinct frames
+// into a staged pool (k_stage_rollouts) that conv_1 reads as a raw one, and its served slots decode time-major
+// (k_decode_time_major).
 #include "common.cuh"
 #include "frame_codec.cuh"
 
@@ -471,6 +474,58 @@ k_decode_planes(const uint8_t* __restrict__ pool, int64_t P, const int64_t* __re
   fc_decode(pool + (foff[id] % P) * 16, out, s_rows[threadIdx.x >> 5], lane);
 }
 
+// b2rl_serve_fill_uniform on a coded rollout handle (R = 4 (T + 1)): k_decode_planes<Strips> with the time-major
+// destination of add_planes_time_major, frame c = j % R of draw k = j / R to frame c % 4 of row (c / 4) n + k of the
+// (T + 1) n stacks at dst.  One warp per frame.
+__global__ void __launch_bounds__(DD_THREADS)
+k_decode_time_major(const uint8_t* __restrict__ pool, int64_t P, const int64_t* __restrict__ foff, int64_t F,
+                    const int32_t* __restrict__ planes, int32_t R, const int64_t* __restrict__ idx, int64_t n,
+                    int64_t capacity, uint8_t* __restrict__ dst) {
+  __shared__ FcRows s_rows[DD_THREADS / 32];
+  const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (j >= n * R) return;
+  const int64_t k = j / R;
+  const int64_t c = j - k * R;
+  int64_t slot = idx[k];
+  slot = slot < 0 ? 0 : (slot >= capacity ? capacity - 1 : slot);
+  const int64_t id = (uint32_t)planes[R * slot + c] % (uint64_t)F;
+  fc_decode(pool + (foff[id] % P) * 16, dst + (((c >> 2) * n + k) * 4 + (c & 3)) * DD_FRAME,
+            s_rows[threadIdx.x >> 5], lane);
+}
+
+// b2rl_dedup_stage_rollouts: frame c = j % R of draw k = j / R is pool id planes[R slot + c] % F of slot
+// clamp_row(idx[k]).  staged_planes[j] = k R + i, i the first of the draw's R positions holding the same id, and only
+// the warp of that first position decodes the frame, into staged_pool + (k R + c) 7 056.  The other staged frames are
+// left as they were.  One warp per frame; the lanes compare 32 earlier positions at a time.
+__global__ void __launch_bounds__(DD_THREADS)
+k_stage_rollouts(const uint8_t* __restrict__ pool, int64_t P, const int64_t* __restrict__ foff, int64_t F,
+                 const int32_t* __restrict__ planes, int32_t R, const int64_t* __restrict__ idx, int64_t n,
+                 int64_t capacity, uint8_t* __restrict__ staged_pool, int32_t* __restrict__ staged_planes) {
+  __shared__ FcRows s_rows[DD_THREADS / 32];
+  const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (j >= n * R) return;
+  const int64_t k = j / R;
+  const int32_t c = (int32_t)(j - k * R);
+  int64_t slot = idx[k];
+  slot = slot < 0 ? 0 : (slot >= capacity ? capacity - 1 : slot);
+  const int32_t* ids = planes + R * slot;
+  const int64_t id = (uint32_t)ids[c] % (uint64_t)F;   // any int32 names an entry
+  int32_t first = c;
+  for (int32_t i0 = 0; i0 < c; i0 += 32) {              // c is the warp's: every lane takes the same exit
+    const int32_t i = i0 + lane;
+    const unsigned m = __ballot_sync(0xffffffffu, i < c && (int64_t)((uint32_t)ids[i] % (uint64_t)F) == id);
+    if (m != 0u) {
+      first = i0 + __ffs((int)m) - 1;
+      break;
+    }
+  }
+  if (lane == 0) staged_planes[j] = (int32_t)(k * R + first);
+  if (first != c) return;
+  fc_decode(pool + (foff[id] % P) * 16, staged_pool + j * DD_FRAME, s_rows[threadIdx.x >> 5], lane);
+}
+
 // b2rl_frame_encode / b2rl_frame_decode: frame j <-> the encoding at enc + j * FC_RAW_BYTES.  One warp per frame.
 __global__ void __launch_bounds__(DD_THREADS)
 k_frame_encode(const uint8_t* __restrict__ frames, int64_t n, uint8_t* __restrict__ enc, int32_t* __restrict__ units) {
@@ -527,6 +582,16 @@ int gather_coded_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8
   kernel<<<warps_grid(n * d->R), DD_THREADS, 0, st>>>(d->pool, d->P, d->foff, d->F,
                                                       (const int32_t*)h->field[d->planes_field], d->R, idx_dev, n,
                                                       h->capacity, dst_dev, dst2_dev);
+  count_launch();
+  B2RL_CHECK_LAUNCH();
+  return B2RL_OK;
+}
+
+int decode_rollouts_time_major(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, cudaStream_t st) {
+  const DedupState* d = h->dedup;
+  k_decode_time_major<<<warps_grid(n * d->R), DD_THREADS, 0, st>>>(d->pool, d->P, d->foff, d->F,
+                                                                    (const int32_t*)h->field[d->planes_field], d->R,
+                                                                    idx_dev, n, h->capacity, dst_dev);
   count_launch();
   B2RL_CHECK_LAUNCH();
   return B2RL_OK;
@@ -685,14 +750,49 @@ extern "C" int b2rl_dedup_attach_coded(b2rl_replay* h, int32_t planes_field, int
   return dedup_attach(h, planes_field, Layout::Pairs, 8, pool_frames, window, hash_mask, false, pool_bytes);
 }
 
-extern "C" int b2rl_dedup_attach_rollouts(b2rl_replay* h, int32_t planes_field, int32_t stacks_per_record,
-                                          int64_t pool_frames, int64_t window, uint64_t hash_mask) {
+// b2rl_dedup_attach_rollouts and _rollouts_coded: the strip attach with R = 4 stacks_per_record that marks the handle
+// as holding rollouts.
+static int rollout_attach(b2rl_replay* h, int32_t planes_field, int32_t stacks_per_record, int64_t pool_frames,
+                          int64_t window, uint64_t hash_mask, int64_t pool_bytes) {
   B2RL_REQUIRE(stacks_per_record >= 1 && stacks_per_record <= DD_MAX_FRAMES / 4,
                "stacks_per_record must be in [1, 16384]");
   const int rc = dedup_attach(h, planes_field, Layout::Strips, 4 * stacks_per_record, pool_frames, window, hash_mask,
-                              false);
+                              false, pool_bytes);
   if (rc == B2RL_OK) h->dedup->stacks = stacks_per_record;
   return rc;
+}
+
+extern "C" int b2rl_dedup_attach_rollouts(b2rl_replay* h, int32_t planes_field, int32_t stacks_per_record,
+                                          int64_t pool_frames, int64_t window, uint64_t hash_mask) {
+  return rollout_attach(h, planes_field, stacks_per_record, pool_frames, window, hash_mask, 0);
+}
+
+extern "C" int b2rl_dedup_attach_rollouts_coded(b2rl_replay* h, int32_t planes_field, int32_t stacks_per_record,
+                                                int64_t pool_frames, int64_t window, uint64_t hash_mask,
+                                                int64_t pool_bytes) {
+  B2RL_REQUIRE(pool_bytes > 0, "pool_bytes must be positive");
+  return rollout_attach(h, planes_field, stacks_per_record, pool_frames, window, hash_mask, pool_bytes);
+}
+
+extern "C" int b2rl_dedup_stage_rollouts(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* staged_pool_dev,
+                                         int32_t* staged_planes_dev, void* stream) {
+  B2RL_REQUIRE(h != nullptr, "null handle");
+  const DedupState* d = h->dedup;
+  B2RL_REQUIRE(d != nullptr && d->stacks > 0 && d->P > 0,
+               "not a coded rollout frame pool (b2rl_dedup_attach_rollouts_coded)");
+  B2RL_REQUIRE(n >= 0, "n must be >= 0");
+  if (n == 0) return B2RL_OK;
+  B2RL_REQUIRE(idx_dev != nullptr && staged_pool_dev != nullptr && staged_planes_dev != nullptr, "null argument");
+  B2RL_REQUIRE((uintptr_t)staged_pool_dev % 16 == 0 && (uintptr_t)staged_planes_dev % 4 == 0,
+               "the staged pool must be 16-byte aligned and the staged planes 4-byte aligned");
+  B2RL_REQUIRE(n <= ((1LL << 31) - 1) / d->R, "n out of range: n * 4 (T + 1) staged frames must stay below 2^31");
+  DeviceGuard g(h->device);
+  k_stage_rollouts<<<warps_grid(n * d->R), DD_THREADS, 0, (cudaStream_t)stream>>>(
+      d->pool, d->P, d->foff, d->F, (const int32_t*)h->field[d->planes_field], d->R, idx_dev, n, h->capacity,
+      staged_pool_dev, staged_planes_dev);
+  count_launch();
+  B2RL_CHECK_LAUNCH();
+  return B2RL_OK;
 }
 
 extern "C" int b2rl_dedup_info(const b2rl_replay* h, void** pool_dev, int64_t* head_seq, int64_t* max_batch) {
@@ -708,7 +808,7 @@ extern "C" int b2rl_dedup_codec_stats(const b2rl_replay* h, int64_t* units_writt
                                       int64_t* frames_stored) {
   B2RL_REQUIRE(h != nullptr, "null handle");
   B2RL_REQUIRE(h->dedup != nullptr && h->dedup->P > 0,
-               "not a coded frame pool (b2rl_dedup_attach_strips_coded, b2rl_dedup_attach_coded)");
+               "not a coded frame pool (b2rl_dedup_attach_strips_coded, _coded, _rollouts_coded)");
   if (units_written) *units_written = h->dedup->units;
   if (pool_units) *pool_units = h->dedup->P;
   if (frames_stored) *frames_stored = h->dedup->head;

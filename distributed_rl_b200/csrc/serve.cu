@@ -461,8 +461,13 @@ extern "C" int b2rl_serve_fill_uniform(b2rl_replay* h, b2rl_serve_ring* r, int32
   BulkRows P{};
   SmallFields small{};
   SmallRows rows{};
+  uint8_t* coded_stacks = nullptr;
   for (int f = 0; f < h->n_fields; ++f) {
     const int64_t b = h->field_bytes[f];
+    if (h->dedup != nullptr && f == dedup_planes_field(h) && dedup_pool_coded(h)) {
+      coded_stacks = (uint8_t*)ptrs[3 + f];   // decoded after the draw, from the slot's idx (dedup.cu)
+      continue;
+    }
     if (h->dedup != nullptr && f == dedup_planes_field(h)) {   // the stacks assembled from the frame pool
       P.add_planes_time_major(dedup_pool(h), (const int32_t*)h->field[f], dedup_strip_frames(h), steps + 1,
                               (uint8_t*)ptrs[3 + f]);
@@ -493,6 +498,8 @@ extern "C" int b2rl_serve_fill_uniform(b2rl_replay* h, b2rl_serve_ring* r, int32
       P, small, rows, h->rng_dev, n, u, (int64_t*)ptrs[1], (uint64_t*)ptrs[0], seq, r->done_ticket);
   count_launch();
   B2RL_CHECK_LAUNCH();
+  if (coded_stacks != nullptr)
+    return decode_rollouts_time_major(h, (const int64_t*)ptrs[1], n, coded_stacks, (cudaStream_t)stream);
   return B2RL_OK;
 }
 

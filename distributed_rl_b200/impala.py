@@ -56,6 +56,20 @@ class ImpalaConfig:
     FRAMES_PER_ROLLOUT: float = 24.0
     DEDUP_WINDOW: int = 1 << 14  # a frame is reused only from the last DEDUP_WINDOW frames stored (at most 1/8 of the
                                  # pool, see dedup_geometry)
+    STAGED_POOL_CODEC: bool = False  # store a FRAME_DEDUP store's frames losslessly encoded in a ring of bytes in HBM
+                                     # (DESIGN §4.23); each step decodes the drawn rollouts' distinct frames into a
+                                     # staged frame pool that conv_1 reads, as R2D2's POOL_CODEC decodes into a staged
+                                     # batch.  Not named POOL_CODEC: IMPALA's staged pool is a plane table, not a batch.
+    POOL_BYTES_PER_ROLLOUT: float | None = None    # STAGED_POOL_CODEC's ring: this many bytes per slot (pool_bytes);
+                                                   # size it from RolloutDedupReplay.codec_stats()
+
+    def __post_init__(self):
+        if self.STAGED_POOL_CODEC and not self.FRAME_DEDUP:
+            raise ValueError("STAGED_POOL_CODEC encodes the frame pool of a FRAME_DEDUP store: set FRAME_DEDUP with it")
+        if self.POOL_BYTES_PER_ROLLOUT is not None and not self.STAGED_POOL_CODEC:
+            raise ValueError("POOL_BYTES_PER_ROLLOUT sizes the coded frame pool: set STAGED_POOL_CODEC with it")
+        if self.POOL_BYTES_PER_ROLLOUT is not None and not self.POOL_BYTES_PER_ROLLOUT > 0:
+            raise ValueError(f"POOL_BYTES_PER_ROLLOUT must be positive, not {self.POOL_BYTES_PER_ROLLOUT}")
 
     @staticmethod
     def from_configuration():
@@ -63,7 +77,8 @@ class ImpalaConfig:
         names = ("BATCHSIZE", "ACTION_SIZE", "GAMMA", "C_LAMBDA", "C_VALUE", "P_VALUE", "ENTROPY_R", "UNROLL_STEP",
                  "REPLAY_MEMORY_LEN", "BUFFER_SIZE", "LEARNER_DEVICE", "REDIS_SERVER", "OPTIM_INFO", "MODEL")
         kw = {k: getattr(C, k) for k in names}
-        for k in ("FRAME_DEDUP", "FRAMES_PER_ROLLOUT", "DEDUP_WINDOW"):      # optional keys of cfg/impala.json
+        for k in ("FRAME_DEDUP", "FRAMES_PER_ROLLOUT", "DEDUP_WINDOW", "STAGED_POOL_CODEC",
+                  "POOL_BYTES_PER_ROLLOUT"):                                    # optional keys of cfg/impala.json
             if hasattr(C, k):
                 kw[k] = getattr(C, k)
         return ImpalaConfig(LOG_W=getattr(C, "LOG_W", None), **kw)
@@ -85,6 +100,20 @@ def dedup_geometry(cfg: ImpalaConfig) -> tuple:
     return F, W
 
 
+def pool_bytes(cfg: ImpalaConfig) -> int | None:
+    """Bytes of a STAGED_POOL_CODEC store's frame ring (None without STAGED_POOL_CODEC): POOL_BYTES_PER_ROLLOUT x
+    REPLAY_MEMORY_LEN, rounded down to 16 bytes.  The default is the raw size plus one frame, (F + 1) x 7 072 for
+    dedup_geometry's F frames, as r2d2.pool_bytes and apex.pool_bytes: a slot then dies by the byte rule no earlier than
+    by the frame rule (DESIGN §4.21).  A smaller ring trades that for memory, at the mean stored bytes per frame
+    codec_stats() reports; it must hold 7 072 (W + 2 + 4 (T + 1)) bytes whatever the frames (§4.23)."""
+    import math
+    if not cfg.STAGED_POOL_CODEC:
+        return None
+    if cfg.POOL_BYTES_PER_ROLLOUT is None:
+        return (int(math.ceil(cfg.FRAMES_PER_ROLLOUT * cfg.REPLAY_MEMORY_LEN)) + 1) * 7072
+    return int(cfg.POOL_BYTES_PER_ROLLOUT * cfg.REPLAY_MEMORY_LEN) // 16 * 16
+
+
 def rollout_frames(store):
     """conv_1's frame rows over a rollout store's `state`, row slot * (T + 1) + t being stack t of the slot: the
     field viewed as one stack per row, or a RolloutDedupReplay's plane table."""
@@ -102,7 +131,8 @@ class Replay(ReplayThread):
         super().__init__(cfg or ImpalaConfig.from_configuration(), connect)
         if self.cfg.FRAME_DEDUP:
             self.store = R.RolloutDedupReplay(self.cfg.REPLAY_MEMORY_LEN, *dedup_geometry(self.cfg),
-                                              T=self.cfg.UNROLL_STEP, device=self.device)
+                                              T=self.cfg.UNROLL_STEP, device=self.device,
+                                              pool_bytes=pool_bytes(self.cfg))
         else:
             self.store = R.DeviceReplay(self.cfg.REPLAY_MEMORY_LEN, R.impala_fields(self.cfg.UNROLL_STEP), self.device)
         self._rng = torch.Generator(device=self.device)        # uniform sampling stream (random.sample in the reference)
@@ -205,8 +235,9 @@ class Learner(CapturedStep):
         """One learner step with everything resident: draw B rollouts uniformly without replacement
         (random.sample, baseline/utils.py:310-315), gather only a / mu / r / done (244 B of the 593 KB rollout),
         run conv_1 over the rollouts' (T+1) frames IN PLACE in the replay payload (row = slot * (T+1) + t,
-        time-major; with FRAME_DEDUP through the store's plane table, rollout_frames), V-trace kernel, loss, backward,
-        clip + RMSprop.
+        time-major; with FRAME_DEDUP through the store's plane table, rollout_frames; with STAGED_POOL_CODEC through
+        the staged pool the draw's distinct frames are decoded into, _StagedRollouts), V-trace kernel, loss,
+        backward, clip + RMSprop.
         `use_graph`: the step as a CUDA graph (_captured_step), its draw one launch of DeviceReplay.uniform_fetch
         before each replay.  -> `last` (for the graph: its static buffers, plus `idx`)."""
         if use_graph:
@@ -217,14 +248,26 @@ class Learner(CapturedStep):
         st = mem.store
         if not hasattr(self, "_small"):
             self._small = st.alloc_batch(B, ("action", "mu", "reward", "done"))
-            self._frames = rollout_frames(st)
             self._t_idx = torch.arange(T + 1, device=self.device).view(T + 1, 1)
+            self._frames = None if self._staged_pool() is not None else rollout_frames(st)
         idx = mem.draw(B)
         b = st.gather(idx, self._small)
-        rows = time_major_rows(idx, self._t_idx)
-        self._train_core(self._frames, rows, b["action"].t().contiguous(), b["mu"].t().contiguous(),
+        staged = self._staged_pool()
+        if staged is not None:
+            frames, rows = staged.stage(idx), staged.rows
+        else:
+            frames, rows = self._frames, time_major_rows(idx, self._t_idx)
+        self._train_core(frames, rows, b["action"].t().contiguous(), b["mu"].t().contiguous(),
                          b["reward"].t().contiguous(), b["done"], step)
         return self.last
+
+    def _staged_pool(self) -> "_StagedRollouts | None":
+        """The staged frame pool of a STAGED_POOL_CODEC store, built once per learner and shared by the eager and
+        captured steps (None for a store conv_1 reads in place)."""
+        if not hasattr(self, "_staged"):
+            st = self._memory.store
+            self._staged = _StagedRollouts(st, self.cfg.BATCHSIZE) if getattr(st, "coded", False) else None
+        return self._staged
 
     def _drawn_state(self) -> "_DrawnRollouts":
         if self._drawn is None:
@@ -250,7 +293,11 @@ class Learner(CapturedStep):
             mem.store.uniform_fetch(B, T, cur)
 
         def body():
-            self._train_core(s.frames, cur["rows"], cur["action"], cur["mu"], cur["reward"], cur["done"], 0)
+            if s.staged is not None:
+                frames, rows = s.staged.stage(cur["idx"]), s.staged.rows
+            else:
+                frames, rows = s.frames, cur["rows"]
+            self._train_core(frames, rows, cur["action"], cur["mu"], cur["reward"], cur["done"], 0)
             self.last["idx"] = cur["idx"]
             return self.last
 
@@ -423,7 +470,8 @@ class _DrawnRollouts:
     warm-up, and the stream it is warmed up and captured on.  DeviceReplay.uniform_fetch draws into `cur`: idx (B,),
     action / mu / reward (T, B), done (B,) and `rows`, the (T+1) * B time-major rows of the drawn rollouts' frames in
     `frames`, the replay's `state` field with one frame stack per row (row = slot * (T+1) + t), or with FRAME_DEDUP
-    the store's plane table with the same rows (rollout_frames)."""
+    the store's plane table with the same rows (rollout_frames).  With STAGED_POOL_CODEC the step stages the drawn
+    rollouts' frames instead (`staged`), and reads them through the staged pool's fixed rows."""
 
     def __init__(self, L: "Learner"):
         c, dev = L.cfg, L.device
@@ -433,8 +481,27 @@ class _DrawnRollouts:
                              "the model's first node must be the Atari conv_1")
         self.stream = torch.cuda.Stream(dev)
         self.cur = _rollout_buffers(T, B, dev)
-        self.cur["rows"] = torch.empty((T + 1) * B, dtype=torch.int64, device=dev)
-        self.frames = rollout_frames(L._memory.store)
+        self.staged = L._staged_pool()
+        if self.staged is None:
+            self.cur["rows"] = torch.empty((T + 1) * B, dtype=torch.int64, device=dev)
+            self.frames = rollout_frames(L._memory.store)
+
+
+class _StagedRollouts:
+    """The staged frame pool of a STAGED_POOL_CODEC store (R.RolloutDedupReplay.stage_frames, DESIGN.md §4.23),
+    allocated once per learner: B 4 (T + 1) frames and their plane table.  stage(idx) decodes the distinct frames of the
+    drawn rollouts into it (one launch, captured with the step) and returns conv_1's frame source; `rows` are its fixed
+    time-major rows, row t * B + k = k (T + 1) + t being stack t of draw k."""
+
+    def __init__(self, store, B: int):
+        T = store.T
+        self.store = store
+        self.buffers = store.alloc_staged(B)
+        self.rows = time_major_rows(torch.arange(B, device=store.device),
+                                    torch.arange(T + 1, device=store.device).view(T + 1, 1))
+
+    def stage(self, idx: torch.Tensor):
+        return self.store.stage_frames(idx, self.buffers)
 
 
 def _rollout_buffers(T: int, B: int, dev) -> dict:

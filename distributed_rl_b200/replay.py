@@ -807,24 +807,67 @@ class RolloutDedupReplay(StripDedupReplay):
     stack of the same actor's next rollout, and a rollout cut short at an episode end is padded with the previous
     rollout's stacks (IMPALA/Player.py:88-203), so about T of the 4 (T + 1) frames are new.  push / gather /
     uniform_fetch take and return what a DeviceReplay of impala_fields(T) does, bit for bit, while every slot is live;
-    the liveness rule and the refusals are DedupReplay's, and the frame pool stays in HBM."""
+    the liveness rule and the refusals are DedupReplay's, and the frame pool stays in HBM.
+    `pool_bytes` (ImpalaConfig.STAGED_POOL_CODEC, DESIGN.md §4.23): the frames are stored losslessly encoded in a
+    device ring of pool_bytes (b2rl_dedup_attach_rollouts_coded), and a slot also dies once pool_bytes - 7072 (window +
+    1) bytes have been written since its batch began.  `pool` is then that flat uint8 ring, gather() and the served
+    fill decode the sampled rollouts, codec_stats() reports the bytes stored per frame, frame_source() is refused, and
+    stage_frames() decodes the distinct frames of drawn rollouts into a staged pool that conv_1 reads instead."""
 
     def __init__(self, capacity: int, pool_frames: int, window: int, T: int = 20, device="cuda:0",
-                 hash_mask: int = DEDUP_HASH_MASK):
+                 hash_mask: int = DEDUP_HASH_MASK, pool_bytes: int | None = None):
         DeviceReplay.__init__(self, capacity, IMPALA_DEDUP_FIELDS(T), device)
         self.T = int(T)
         self.RECORD_FIELDS = impala_fields(self.T)
-        self.host_pool = self.coded = False
-        check(self.lib.b2rl_dedup_attach_rollouts(self._h, 0, self.T + 1, int(pool_frames), int(window),
-                                                  int(hash_mask)))
+        self.host_pool = False
+        self.coded = pool_bytes is not None
+        args = (self._h, 0, self.T + 1, int(pool_frames), int(window), int(hash_mask))
+        if self.coded:
+            check(self.lib.b2rl_dedup_attach_rollouts_coded(*args, int(pool_bytes)))
+        else:
+            check(self.lib.b2rl_dedup_attach_rollouts(*args))
         self._attached(pool_frames, window)
+        if self.coded:          # the encoded frames: a flat ring of 16-byte units, not (F, 84, 84) frames
+            self._coded_pool()
 
     def frame_source(self, name: str) -> "PlaneFrames":
         """conv_1's rows of `state`: every slot's stacks, row slot * (T + 1) + t being stack t of the slot (the row
         numbering of a stack store's state field viewed as (capacity * (T + 1), 4, 84, 84))."""
         if name != "state":
             raise KeyError(name)
+        if self.coded:
+            raise ValueError("conv_1 reads raw frame rows: a coded frame pool (pool_bytes) holds encoded frames and "
+                             "has no frame source; stage the drawn rollouts (stage_frames) into device memory first")
         return PlaneFrames(self.pool, self.field_view("planes"), 0, 4)
+
+    def alloc_staged(self, n: int) -> dict:
+        """stage_frames' buffers for n drawn rollouts, allocated once per learner: `pool` uint8 (n 4 (T + 1), 84, 84)
+        and `planes` int32 (n, 4 (T + 1))."""
+        R = 4 * (self.T + 1)
+        return {"pool": torch.empty(n * R, 84, 84, dtype=torch.uint8, device=self.device),
+                "planes": torch.empty(n, R, dtype=torch.int32, device=self.device)}
+
+    def stage_frames(self, idx: torch.Tensor, staged: dict) -> "PlaneFrames":
+        """The frames of the drawn slots idx (device int64 (n,), as uniform_fetch writes them) for conv_1, in one
+        launch that a CUDA graph can capture (b2rl_dedup_stage_rollouts): each distinct frame of a rollout is decoded
+        once into staged["pool"], and staged["planes"] names, for each of the rollout's 4 (T + 1) frames, the staged
+        frame it equals.  -> the stride-4 PlaneFrames over them: row k (T + 1) + t is stack t of draw k, bit for bit
+        what frame_source() of a raw store reads at row idx[k] (T + 1) + t."""
+        if not self.coded:
+            raise ValueError("stage_frames() decodes a coded frame pool (pool_bytes): read a raw pool through "
+                             "frame_source()")
+        n = idx.numel()
+        pool, planes = staged["pool"], staged["planes"]
+        if not (idx.is_cuda and idx.dtype == torch.int64 and idx.is_contiguous()):
+            raise ValueError("idx must be a contiguous CUDA int64 tensor")
+        R = 4 * (self.T + 1)
+        if pool.dtype != torch.uint8 or not pool.is_contiguous() or pool.numel() != n * R * FRAME_BYTES or \
+                planes.dtype != torch.int32 or not planes.is_contiguous() or planes.numel() != n * R:
+            raise ValueError(f"staged buffers must be alloc_staged({n})'s: uint8 ({n * R}, 84, 84) and int32 "
+                             f"({n}, {R})")
+        check(self.lib.b2rl_dedup_stage_rollouts(self._h, idx.data_ptr(), n, pool.data_ptr(), planes.data_ptr(),
+                                                 self._st()))
+        return PlaneFrames(pool.view(n * R, 84, 84), planes.view(n, R), 0, 4)
 
 
 # ---- stateless target kernels -------------------------------------------------

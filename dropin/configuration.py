@@ -39,7 +39,8 @@ elif ALG == "IMPALA":
     P_VALUE = DATA["P_VALUE"]
     ENTROPY_R = DATA["ENTROPY_R"]
     FRAME_DEDUP = bool(DATA.get("FRAME_DEDUP", False))   # not a reference key: store every distinct frame once
-    for _k in ("FRAMES_PER_ROLLOUT", "DEDUP_WINDOW"):
+    STAGED_POOL_CODEC = bool(DATA.get("STAGED_POOL_CODEC", False))   # not a reference key: store that pool encoded
+    for _k in ("FRAMES_PER_ROLLOUT", "DEDUP_WINDOW", "POOL_BYTES_PER_ROLLOUT"):
         if _k in DATA:
             globals()[_k] = DATA[_k]
 

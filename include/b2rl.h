@@ -319,8 +319,32 @@ int b2rl_dedup_attach_coded(b2rl_replay* h, int32_t planes_field, int64_t pool_f
  * *offsets_dev receives the device int64[pool_frames] absolute unit offsets of the entries (frame id i is encoded at
  * pool + (offsets[i] % P) * 16), the `offsets` of a coded b2rl_frames source. */
 int b2rl_dedup_coded_offsets(const b2rl_replay* h, void** offsets_dev);
+/* The IMPALA rollout store (b2rl_dedup_attach_rollouts, IMPALA/ReplayMemory.py:14-85) with its frames stored encoded,
+ * the rollout twin of b2rl_dedup_attach_strips_coded (DESIGN.md §4.23): R = 4 stacks_per_record, and the handle is
+ * marked as holding rollouts.  Ids, the window, the frame rule, the byte rule and the push bound are the strip form's
+ * at that R; requires P >= 442 (window + 2 + R).  b2rl_dedup_push_strips stores into it; b2rl_uniform_fetch draws it
+ * as the raw rollout store; b2rl_replay_gather_planes decodes the sampled slots' (n, T + 1, 28 224) rows; and
+ * b2rl_serve_fill_uniform serves it, decoding the drawn rollouts' stacks time-major after the fill's launch from the
+ * slot's idx (a second launch on the same stream), byte for byte the raw rollout store's slot while the slots are
+ * live.  Its pool is never a conv_1 frame source: b2rl_dedup_stage_rollouts decodes what a step reads.  Whatever
+ * b2rl_dedup_attach_rollouts refuses it refuses with the same message; arguments are checked before the handle. */
+int b2rl_dedup_attach_rollouts_coded(b2rl_replay* h, int32_t planes_field, int32_t stacks_per_record,
+                                     int64_t pool_frames, int64_t window, uint64_t hash_mask, int64_t pool_bytes);
+/* The frames a learner step reads of n drawn rollouts (IMPALA/ReplayMemory.py:30-54, drawn as random.sample draws,
+ * baseline/utils.py:310-315) of a coded rollout handle, staged as a small raw frame pool: with R = 4 (T + 1) and
+ * idx_dev the device int64[n] slots (b2rl_uniform_fetch's idx, clamped into [0, capacity)), frame c of draw k has pool
+ * id planes[R slot + c] % pool_frames; staged_planes_dev[k R + c] (int32[n R]) receives k R + i, i the first of the
+ * draw's R positions holding that id, and only those first positions are decoded, into staged_pool_dev + (k R + i)
+ * 7 056 (n R frames of 7 056 bytes; the others are left as they were).  conv_1 then reads row k (T + 1) + t of the
+ * staged pool through plane_stride 4 of b2rl_frames (pool = staged_pool_dev, planes = staged_planes_dev): stack t of
+ * draw k, byte for byte the raw rollout store's while the slot is live.  A dead or never-written slot stages
+ * unspecified frames, each read inside the pool's allocation.  One launch, no host synchronisation: capturable in a
+ * CUDA graph.  An error, and no launch, unless h is a coded rollout handle, the buffers are non-NULL, staged_pool_dev
+ * 16-byte and staged_planes_dev 4-byte aligned, and n R < 2^31. */
+int b2rl_dedup_stage_rollouts(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* staged_pool_dev,
+                              int32_t* staged_planes_dev, void* stream);
 /* A coded pool's counters, the sizes CompressedDeque (baseline/utils.py:277-296) leaves to pickle (each may be NULL):
- * units written so far (wrap padding included), P, and frames stored.  Strip and Ape-X coded handles alike. */
+ * units written so far (wrap padding included), P, and frames stored.  Strip, Ape-X and rollout coded handles alike. */
 int b2rl_dedup_codec_stats(const b2rl_replay* h, int64_t* units_written, int64_t* pool_units, int64_t* frames_stored);
 /* The pool's codec on device buffers, as CompressedDeque.append / __getitem__ (baseline/utils.py:277-296) on one
  * frame: b2rl_frame_encode writes frame j (n frames of 7 056 bytes) to enc_dev + 7 072 j and its length in units to
@@ -613,7 +637,7 @@ int b2rl_serve_fill(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, uint64_t s
  * has no IS weights), the header {seq, B} last.  Same slot layout and ring as b2rl_serve_fill.  An error, and no
  * launch, when B > size or the ring was not created for h.  Of the frame-deduplicated replays it serves the rollout
  * handle (b2rl_dedup_attach_rollouts) only, assembling each drawn rollout's T + 1 stacks from the frame pool in the
- * same launch. */
+ * same launch; a coded rollout handle's stacks are decoded by a second launch (b2rl_dedup_attach_rollouts_coded). */
 int b2rl_serve_fill_uniform(b2rl_replay* h, b2rl_serve_ring* r, int32_t slot, uint64_t seq, int32_t steps,
                             void* stream);
 /* Replay_Server.sample (APE_X/ReplayMemory.py:251-257) without the unpickle: copy minibatch slot k (slot_bytes,
