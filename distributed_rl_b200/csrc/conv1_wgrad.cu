@@ -23,7 +23,8 @@
 //                 chunk while they run; the accumulators stay in registers over all of the CTA's frame stacks
 //     warps 0-7   A: SMEM frame -> [256 patch elements][128 positions] uint8, K-major SW128
 //     warps 8-15  B: gy (NHWC fp32, global) -> digits -> [4*C_OUT][128 positions] int8
-//                 (warp = 8 channels x half of a chunk's 16-position units)
+//                 (warp = 8 channels x half of a chunk's 16-position units); the ReLU mask of the CTA's first
+//                 MASK_ITEMS items comes from shared memory, written by the pre-scan that finds the digit scale
 //   thread 0 also issues the TMA bulk copy of the next frame stack when it starts on a stack's first chunk: the
 //   buffer it overwrites was last read two stacks before, by chunks that every producer has finished
 //
@@ -52,6 +53,9 @@ constexpr int STAGES = 3;                          // a stage is rebuilt two chu
 constexpr int A_PRODUCERS = 256, B_PRODUCERS = 256;
 constexpr int THREADS = A_PRODUCERS + B_PRODUCERS;
 constexpr int MAX_ITEMS_PER_CTA = 160;             // int32 accumulators: 128*255*400*T < 2^31
+// ReLU masks of a CTA's first MASK_ITEMS items kept on chip from the pre-scan (one word of channel bits per position),
+// so the digit build does not read y again; 4 covers a batch of 512 on 132 SMs
+constexpr int MASK_ITEMS = 4;
 
 // byte offset of (row, 16-byte unit) in a one-chunk K-major SW128 operand
 __device__ __forceinline__ int sw_row(int row) { return (row >> 3) * 1024 + (row & 7) * 128; }
@@ -93,13 +97,15 @@ k_conv1_wgrad(const __grid_constant__ Params P) {
   uint8_t* sStage = smem;
   uint8_t* sZero = smem + STAGES * STAGE_BYTES;        // a B operand of zeros: the K steps past position 415
   uint8_t* sRaw = sZero + B_BYTES;
-  FcRows* sRows = reinterpret_cast<FcRows*>(sRaw + 2 * RAW_STRIDE);   // CodedPlanes: the decoders' row tables
+  uint32_t* sMask = reinterpret_cast<uint32_t*>(sRaw + 2 * RAW_STRIDE);   // [MASK_ITEMS][POS]: bit co is y > 0
+  FcRows* sRows = reinterpret_cast<FcRows*>(sMask + MASK_ITEMS * POS);   // CodedPlanes: the decoders' row tables
   __shared__ __align__(8) uint64_t raw_full[2];
   __shared__ uint32_t s_absmax[32];                    // per channel: bits of max |gy| over this CTA's items
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x < 32) s_absmax[threadIdx.x] = 0u;
   for (int i = threadIdx.x; i < B_BYTES / 16; i += THREADS) reinterpret_cast<uint4*>(sZero)[i] = make_uint4(0u, 0u, 0u, 0u);
+  for (int i = threadIdx.x; i < MASK_ITEMS * POS; i += THREADS) sMask[i] = 0u;
   fence_async_smem();
   if (threadIdx.x == 0) {
     for (int i = 0; i < 2; ++i) mbar_init(&raw_full[i], 1);
@@ -143,9 +149,13 @@ k_conv1_wgrad(const __grid_constant__ Params P) {
     const int pt = threadIdx.x - A_PRODUCERS;         // 0..255
     const int c4 = (pt * 4) % C_OUT;                  // this thread always sees channels c4..c4+3 (1024 % C_OUT == 0)
     uint4 m = make_uint4(0u, 0u, 0u, 0u);
-    for (int64_t k = first; k < P.n; k += stride) {
+    // last item first: the items the main loop starts with are then the ones most recently read, still in L2
+    const int64_t last = first + (P.n - 1 - first) / stride * stride;
+    for (int64_t k = last; k >= first; k -= stride) {
       const uint4* g = reinterpret_cast<const uint4*>(P.gy + k * (int64_t)(POS * C_OUT));
       const float4* yk = P.y ? reinterpret_cast<const float4*>(P.y + k * (int64_t)(POS * C_OUT)) : nullptr;
+      const int64_t it = (k - first) / stride;
+      uint32_t* mk = it < MASK_ITEMS ? sMask + it * POS : nullptr;
 #pragma unroll
       for (int i = 0; i < (POS * C_OUT / 4 + 255) / 256; ++i) {
         const int e = pt + 256 * i;
@@ -155,6 +165,9 @@ k_conv1_wgrad(const __grid_constant__ Params P) {
             const float4 yv = yk[e];
             v.x = yv.x > 0.0f ? v.x : 0u; v.y = yv.y > 0.0f ? v.y : 0u;
             v.z = yv.z > 0.0f ? v.z : 0u; v.w = yv.w > 0.0f ? v.w : 0u;
+            const uint32_t bits = (yv.x > 0.0f ? 1u : 0u) | (yv.y > 0.0f ? 2u : 0u) | (yv.z > 0.0f ? 4u : 0u) |
+                                  (yv.w > 0.0f ? 8u : 0u);
+            if (mk && bits) atomicOr(&mk[4 * e / C_OUT], bits << c4);   // element 4e is position 4e / C_OUT
           }
           m.x = max(m.x, v.x & 0x7FFFFFFFu); m.y = max(m.y, v.y & 0x7FFFFFFFu);
           m.z = max(m.z, v.z & 0x7FFFFFFFu); m.w = max(m.w, v.w & 0x7FFFFFFFu);
@@ -190,7 +203,16 @@ k_conv1_wgrad(const __grid_constant__ Params P) {
 #pragma unroll
       for (int i = 0; i < 4; ++i) v[uu][i] = (uu < nu && p < POS) ? g[(int64_t)(p + i) * C_OUT] : 0.0f;
     }
-    if (P.y) {                                       // ReLU mask of the fused forward
+    if (P.y && (at >> 2) < MASK_ITEMS) {             // ReLU mask of the fused forward, kept by the pre-scan
+      const uint32_t* mk = sMask + (at >> 2) * POS;
+#pragma unroll
+      for (int uu = 0; uu < 4; ++uu) {
+        const int p = j * KCHUNK + (u0 + uu) * 16 + 4 * pq;
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          if (uu < nu && p < POS && !((mk[p + i] >> co) & 1u)) v[uu][i] = 0.0f;
+      }
+    } else if (P.y) {                                // later items: read y again
       const float* yk = P.y + base;
 #pragma unroll
       for (int uu = 0; uu < 4; ++uu) {
@@ -361,8 +383,10 @@ k_conv1_wgrad_reduce(const float* __restrict__ partial, int n_parts, int numel, 
 template <int C_OUT, FrameKind KIND>
 constexpr size_t smem_bytes() {
   return (size_t)STAGES * (A_BYTES + NSPLIT * C_OUT * KCHUNK) + 2 * (size_t)RAW_STRIDE + NSPLIT * C_OUT * KCHUNK + 1024 +
-         (KIND == FrameKind::CodedPlanes ? DECODE_TABLES * sizeof(FcRows) : 0);
+         (size_t)MASK_ITEMS * POS * sizeof(uint32_t) + (KIND == FrameKind::CodedPlanes ? DECODE_TABLES * sizeof(FcRows) : 0);
 }
+// the largest instance and the kernel's 1 KiB of static shared memory within the 227 KiB a CTA can have
+static_assert(smem_bytes<32, FrameKind::CodedPlanes>() + 1024 <= 227 * 1024, "conv_1 wgrad shared memory");
 
 }  // namespace conv1w
 }  // namespace b2rl
