@@ -1,11 +1,13 @@
 """fp64 references and per-element error bounds of the library's hand-written kernels, shared by the GPU tests that hold
-conv_1 (forward and weight gradient), the 3xTF32 dense layers, the dueling tail and the fused RMSprop to fp64 at the
-learners' step shapes (test_gpu_22_step_shapes, test_gpu_25_apex_step_shapes).
+conv_1 (forward and weight gradient), the 3xTF32 dense layers, the dueling tail, V-trace and the fused RMSprop to fp64
+at the learners' step shapes (test_gpu_22_step_shapes, test_gpu_25_apex_step_shapes,
+test_gpu_35_secondary_steps_fp64), and the whole-step comparison against an fp64 restatement (check_vs_reference).
 
 Every output element is held to its own bound, computed by the same fp64 reference applied to absolute values
 (`mag`), so the bound grows with the length of the sum behind that element; u = 2^-24.  The bound of each kernel is
 written in its checker's docstring.  The fp64 references run on the device, a chunk of frame stacks at a time; the
-frames are drawn on the device from seeded generators.  Importing this module needs torch, not a GPU."""
+frames are drawn on the device from seeded generators.  Importing this module needs torch, not a GPU;
+check_vtrace and check_vs_reference run on tensors of any device."""
 import math
 
 import torch
@@ -320,3 +322,119 @@ def check_rmsprop_centered(what, pre, post, lr, alpha, eps):
         out.append(w.check())
     assert not post["g"].any(), f"{what}: the gradient is not zero after the update"
     return out
+
+
+# --------------------------------------------------------------------------- #
+# V-trace                                                                       #
+# --------------------------------------------------------------------------- #
+def _f32(x):
+    import numpy as np
+    return float(np.float32(x))
+
+
+def vtrace_inputs(T, B, seed):
+    """fp32 (pi, mu, value, boot, reward) numpy arrays for V-trace at its edges: pi from 1e-30 to 1 (half of it in
+    [0.05, 1], a tenth equal to mu, pi[0, 0] = 1), mu in [1e-3, 0.9], so that pi / mu lies far above and below any
+    clip; 30 % of the bootstraps zero."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    f32 = np.float32
+    pi = (10.0 ** rng.uniform(-30, 0, size=(T, B))).astype(f32)
+    mid = rng.random((T, B)) < 0.5
+    pi[mid] = rng.uniform(0.05, 1.0, size=int(mid.sum())).astype(f32)
+    mu = (10.0 ** rng.uniform(-3, np.log10(0.9), size=(T, B))).astype(f32)
+    same = rng.random((T, B)) < 0.1
+    pi[same] = mu[same]
+    pi[0, 0] = 1.0
+    v = rng.standard_normal((T, B)).astype(f32)
+    boot = (rng.standard_normal(B) * (rng.random(B) > 0.3)).astype(f32)
+    r = rng.standard_normal((T, B)).astype(f32)
+    return pi, mu, v, boot, r
+
+
+def vtrace_ref(pi, mu, value, boot, reward, gamma, lam, cbar, pbar):
+    """-> (vt, adv, tol_vt, tol_adv) in fp64: V-trace as csrc/targets.cu k_vtrace and oracle.vtrace compute it (the
+    last step not rho-clipped, c_bar both the delta weight and the trace), and check_vtrace's per-element bounds."""
+    g, lam, cbar, pbar = (_f32(x) for x in (gamma, lam, cbar, pbar))
+    pi, mu, v, r, bs = (t.double() for t in (pi, mu, value, reward, boot))
+    T = v.shape[0]
+    lp, lm = pi.log(), mu.log()
+    ratio = (lp - lm).exp()
+    rho = 9 * U * (lp.abs() + lm.abs()) + 7 * U
+    cr, pt = ratio.clamp(max=cbar), ratio.clamp(max=pbar)
+    e_c, e_p = rho * cr, rho * pt
+    vt, adv, t_vt, t_adv = (torch.empty_like(v) for _ in range(4))
+    zero = torch.zeros_like(bs)
+    vmt_n, e_vmt_n, vt_n, e_vt_n, v_n = zero, zero, bs, zero, zero
+    for i in reversed(range(T)):
+        nxt = bs if i == T - 1 else v_n
+        td = r[i] + g * nxt - v[i]
+        e_td = 3 * U * (r[i].abs() + g * nxt.abs() + v[i].abs())
+        if i == T - 1:
+            vmt, e_vmt = td, e_td
+        else:
+            t1, t2 = td * cr[i], g * lam * cr[i] * vmt_n
+            vmt = t1 + t2
+            e_vmt = (td.abs() * e_c[i] + cr[i] * e_td + U * t1.abs()
+                     + g * lam * (cr[i] * e_vmt_n + vmt_n.abs() * (e_c[i] + 3 * U * cr[i]))
+                     + U * (t1.abs() + t2.abs()))
+        vt[i] = v[i] + vmt
+        e_vt = e_vmt + U * (v[i].abs() + vmt.abs())
+        at = r[i] + g * vt_n
+        d = at - v[i]
+        e_d = g * e_vt_n + U * (g * vt_n.abs() + at.abs() + d.abs())
+        adv[i] = d * pt[i]
+        t_vt[i], t_adv[i] = e_vt, pt[i] * e_d + d.abs() * e_p[i] + U * adv[i].abs()
+        vmt_n, e_vmt_n, vt_n, e_vt_n, v_n = vmt, e_vmt, vt[i], e_vt, v[i]
+    return vt, adv, t_vt, t_adv
+
+
+def check_vtrace(what, pi, mu, value, boot, reward, gamma, lam, cbar, pbar, vt, adv):
+    """V-trace targets `vt` and advantages `adv` (T, B) of fp32 inputs against fp64, per element.  The parameters are
+    the fp32 values the kernel receives; every operation of the kernel is rounded once (u = 2^-24).
+    The ratio expf(logf(pi) - logf(mu)): logf within 4 ulp (2^-23 |ln x| each), the subtraction within u, so the
+    exponent errs by 8u (|ln pi| + |ln mu|) + u |ln pi - ln mu|; expf within 3 ulp.  Relative to pi / mu:
+        rho = 9u (|ln pi| + |ln mu|) + 7u
+    (4 and 3 ulp cover numpy's float32 log and exp as well as CUDA's logf and expf, 1 and 2 ulp).  The clips
+    min(c, ratio) and min(p, ratio) are 1-Lipschitz: e_c = rho min(ratio, c), e_p = rho min(ratio, p).
+    td = r + g v' - v errs by 3u (|r| + g |v'| + |v|) =: e_td (v' the next value, the bootstrap at T - 1).  The
+    recursion vmt = td cr + (g (lam cr)) vmt' carries its error by the same recursion on absolute values with factor
+    g lam cr:
+        e_vmt = |td| e_c + cr e_td + u |td cr| + g lam (cr e_vmt' + |vmt'| (e_c + 3u cr)) + u (|td cr| + |g lam cr vmt'|),
+    e_vmt = e_td at T - 1 (no ratio there).  vt = v + vmt: e_vt = e_vmt + u (|v| + |vmt|).  adv = ((r + g vt') - v) pt
+    with vt' the next target (the bootstrap, exact, at T - 1), at = r + g vt' and d = at - v: three roundings,
+    e_d = g e_vt' + u (g |vt'| + |at| + |d|), and e_adv = pt e_d + |d| e_p + u |adv|.  First order in u; the bounds keep 1u of slack per ratio for the rest."""
+    ref_vt, ref_adv, t_vt, t_adv = vtrace_ref(pi, mu, value, boot, reward, gamma, lam, cbar, pbar)
+    T, B = ref_vt.shape
+    out = []
+    for name, got, ref, tol in (("vtarget", vt, ref_vt, t_vt), ("advantage", adv, ref_adv, t_adv)):
+        w = _Worst(f"{what} {name}, T={T} B={B}")
+        w.add(got, ref, tol)
+        out.append(w.check())
+    return out
+
+
+# --------------------------------------------------------------------------- #
+# a whole step against the fp64, fp32 and TF32 restatements                    #
+# --------------------------------------------------------------------------- #
+def rel_err(x, ref64):
+    """max |x - ref64| / max |ref64| (the absolute error where ref64 is all zero)."""
+    err = (x.double() - ref64).abs().max().item()
+    den = ref64.abs().max().item()
+    return err / den if den > 0 else err
+
+
+def check_vs_reference(what, got, ref64, ref32, reftf32, k=16, floor=1e-6, sharp=True):
+    """A learner step's tensor `got` against the same tensor of an fp64 restatement of the step (`ref64`), with
+    e(x) = max |x - ref64| / max |ref64|:
+        e(got) <= k e(ref32) + floor      no less accurate than the reference's own fp32 arithmetic, within k;
+        e(got) <= e(reftf32) / 20         the comparison is sharp enough to see a TF32-class fault.
+    `ref32`, `reftf32`: the restatement in fp32 and with TF32 convolutions and matmuls.  sharp=False drops the second
+    test, for a quantity TF32's roundings average out in (the caller says why).  -> (e(got), e(ref32), e(reftf32))."""
+    ref64 = ref64.double()
+    e, e32, etf = rel_err(got, ref64), rel_err(ref32, ref64), rel_err(reftf32, ref64)
+    ratio = e / e32 if e32 > 0 else (0.0 if e == 0 else math.inf)
+    print(f"[err/ref] {what}: {e:.3g} of max|ref64|, fp32 {e32:.3g} ({ratio:.3g}x), TF32 {etf:.3g}")
+    assert e <= k * e32 + floor, f"{what}: {e:.3g} of max|ref64| exceeds {k} x fp32's {e32:.3g} + {floor:g}"
+    assert e <= etf / 20 or not sharp, f"{what}: {e:.3g} of max|ref64| is not below TF32's {etf:.3g} / 20"
+    return e, e32, etf

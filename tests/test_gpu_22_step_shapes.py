@@ -312,25 +312,53 @@ class _Spies:
             check_dueling_forward(f"{what} dueling_tail", c["h"], c["wa"], c["wv"], c["q"])
 
 
+def r2d2_learner(N=256, payload_pool=0):
+    """bench.py's R2D2 learner (B = 64, T = 80, MEM = 20) with N sum-tree slots, filled the way bench.py fills it:
+    hashed frames, seeded small fields and priorities.  payload_pool > 0: bench.py's row map, N slots over that many
+    stored sequences (slot s reads row s % payload_pool)."""
+    from distributed_rl_b200 import r2d2
+    B, T = 64, 80
+    P = payload_pool or N
+    cfg = r2d2.R2D2Config(BATCHSIZE=B, REPLAY_MEMORY_LEN=N, BUFFER_SIZE=0, PAYLOAD_POOL=payload_pool,
+                          FIXED_TRAJECTORY=T, MEM=20, LEARNER_DEVICE="cuda:0")
+    torch.manual_seed(0)
+    lrn = r2d2.Learner(cfg, start_replay=False)
+    st, pool = lrn.memory.store, lrn.memory.pool
+    g = _gen(0xB207)
+    pool.fill_hash(P, seed=0xB203)
+    pool.field_view("action").copy_(torch.randint(0, 6, (P, T), device="cuda", generator=g, dtype=torch.int32))
+    pool.field_view("reward").copy_(torch.randn(P, T, device="cuda", generator=g))
+    pool.field_view("h0").copy_(torch.randn(P, 512, device="cuda", generator=g) * 0.1)
+    pool.field_view("h1").copy_(torch.randn(P, 512, device="cuda", generator=g) * 0.1)
+    pool.field_view("notdone").copy_((torch.rand(P, device="cuda", generator=g) > 0.02).float())
+    st.build((torch.randn(N, device="cuda", generator=g).abs().clamp(max=1) + 1e-7) ** cfg.ALPHA)
+    st.seed(1234, 0)
+    return lrn
+
+
+def impala_learner():
+    """bench.py's IMPALA learner (B = 1024, T = 20) on 2 048 rollouts filled the way bench.py fills them."""
+    from distributed_rl_b200 import impala
+    B, T, N = 1024, 20, 2048
+    cfg = impala.ImpalaConfig(BATCHSIZE=B, REPLAY_MEMORY_LEN=N, BUFFER_SIZE=0, UNROLL_STEP=T, LEARNER_DEVICE="cuda:0")
+    torch.manual_seed(0)
+    lrn = impala.Learner(cfg, start_replay=False)
+    st = lrn._memory.store
+    g = _gen(0xB208)
+    st.fill_hash(N, seed=0xB204)
+    st.field_view("action").copy_(torch.randint(0, 6, (N, T), device="cuda", generator=g, dtype=torch.int32))
+    st.field_view("mu").copy_(torch.rand(N, T, device="cuda", generator=g) * 0.85 + 0.05)
+    st.field_view("reward").copy_(torch.randn(N, T, device="cuda", generator=g))
+    st.field_view("done").copy_((torch.rand(N, device="cuda", generator=g) > 0.05).float())
+    st.build(torch.ones(N, device="cuda"))
+    return lrn
+
+
 def test_one_r2d2_step_at_the_bench_shapes(R, L, monkeypatch):
     """bench.py's R2D2 line (B = 64, T = 80, MEM = 20) on a 256-sequence replay filled the way bench.py fills it: every
     conv_1, conv_1 weight gradient, heads GEMM and dueling tail of one eager fused step against fp64."""
-    from distributed_rl_b200 import r2d2
-    B, T, N = 64, 80, 256
-    cfg = r2d2.R2D2Config(BATCHSIZE=B, REPLAY_MEMORY_LEN=N, BUFFER_SIZE=0, FIXED_TRAJECTORY=T, MEM=20,
-                          LEARNER_DEVICE="cuda:0")
-    torch.manual_seed(0)
-    lrn = r2d2.Learner(cfg, start_replay=False)
+    lrn = r2d2_learner()
     st = lrn.memory.store
-    g = _gen(0xB207)
-    st.fill_hash(N, seed=0xB203)
-    st.field_view("action").copy_(torch.randint(0, 6, (N, T), device="cuda", generator=g, dtype=torch.int32))
-    st.field_view("reward").copy_(torch.randn(N, T, device="cuda", generator=g))
-    st.field_view("h0").copy_(torch.randn(N, 512, device="cuda", generator=g) * 0.1)
-    st.field_view("h1").copy_(torch.randn(N, 512, device="cuda", generator=g) * 0.1)
-    st.field_view("notdone").copy_((torch.rand(N, device="cuda", generator=g) > 0.02).float())
-    st.build((torch.randn(N, device="cuda", generator=g).abs().clamp(max=1) + 1e-7) ** cfg.ALPHA)
-    st.seed(1234, 0)
     spies = _Spies(monkeypatch, R, L)
     lrn.fused_step(use_graph=False)
     torch.cuda.synchronize()
@@ -345,19 +373,8 @@ def test_one_impala_step_at_the_bench_shapes(R, L, monkeypatch):
     """bench.py's IMPALA line (B = 1024, T = 20) on 2 048 rollouts filled the way bench.py fills them: conv_1 of all
     21 504 frame stacks, its weight gradient over the 20 480 sequence rows and the 2592 -> 256 layer's forward passes
     (1 024 bootstrap rows, 20 480 sequence rows) of one eager fused step against fp64."""
-    from distributed_rl_b200 import impala
-    B, T, N = 1024, 20, 2048
-    cfg = impala.ImpalaConfig(BATCHSIZE=B, REPLAY_MEMORY_LEN=N, BUFFER_SIZE=0, UNROLL_STEP=T, LEARNER_DEVICE="cuda:0")
-    torch.manual_seed(0)
-    lrn = impala.Learner(cfg, start_replay=False)
+    lrn = impala_learner()
     st = lrn._memory.store
-    g = _gen(0xB208)
-    st.fill_hash(N, seed=0xB204)
-    st.field_view("action").copy_(torch.randint(0, 6, (N, T), device="cuda", generator=g, dtype=torch.int32))
-    st.field_view("mu").copy_(torch.rand(N, T, device="cuda", generator=g) * 0.85 + 0.05)
-    st.field_view("reward").copy_(torch.randn(N, T, device="cuda", generator=g))
-    st.field_view("done").copy_((torch.rand(N, device="cuda", generator=g) > 0.05).float())
-    st.build(torch.ones(N, device="cuda"))
     spies = _Spies(monkeypatch, R, L)
     lrn.fused_step(use_graph=False)
     torch.cuda.synchronize()
