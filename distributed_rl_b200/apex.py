@@ -75,12 +75,7 @@ class ApexConfig:
                                                      # size it from CodedDedupReplay.codec_stats()
 
     def __post_init__(self):
-        if self.FRAME_CODEC and not self.FRAME_DEDUP:
-            raise ValueError("FRAME_CODEC encodes the frame pool of a FRAME_DEDUP store: set FRAME_DEDUP with it")
-        if self.POOL_BYTES_PER_TRANSITION is not None and not self.FRAME_CODEC:
-            raise ValueError("POOL_BYTES_PER_TRANSITION sizes the coded frame pool: set FRAME_CODEC with it")
-        if self.POOL_BYTES_PER_TRANSITION is not None and not self.POOL_BYTES_PER_TRANSITION > 0:
-            raise ValueError(f"POOL_BYTES_PER_TRANSITION must be positive, not {self.POOL_BYTES_PER_TRANSITION}")
+        R.check_codec_keys(self, "FRAME_CODEC", "POOL_BYTES_PER_TRANSITION")
 
     @staticmethod
     def from_configuration():
@@ -101,28 +96,16 @@ def dedup_geometry(cfg: ApexConfig) -> tuple:
     DEDUP_WINDOW capped at an eighth of them.  A slot stays live until pool - window frames have been stored after it,
     so the cap keeps that at least 7/8 of the pool: ~2.3 REPLAY_MEMORY_LEN records at the ~3 new frames per record
     the reference actor sends, more than the slot ring holds."""
-    import math
-    import warnings
-    F = int(math.ceil(cfg.FRAMES_PER_TRANSITION * cfg.REPLAY_MEMORY_LEN))
-    W = min(int(cfg.DEDUP_WINDOW), F // 8)
-    if W < cfg.DEDUP_WINDOW:
-        warnings.warn(f"DEDUP_WINDOW = {cfg.DEDUP_WINDOW} frames is more than an eighth of the {F}-frame pool: the "
-                      f"frame-deduplicated replay uses a window of {W} frames", stacklevel=2)
-    return F, W
+    return R.dedup_pool_geometry(cfg.FRAMES_PER_TRANSITION, cfg.REPLAY_MEMORY_LEN, cfg.DEDUP_WINDOW)
 
 
 def pool_bytes(cfg: ApexConfig) -> int | None:
-    """Bytes of a FRAME_CODEC store's frame ring (None without FRAME_CODEC): POOL_BYTES_PER_TRANSITION x
-    REPLAY_MEMORY_LEN, rounded down to 16 bytes.  The default is the raw size plus one frame, (F + 1) x 7 072 for
-    dedup_geometry's F frames, as r2d2.pool_bytes: a slot then dies by the byte rule no earlier than by the frame rule
-    (DESIGN.md §4.21).  A smaller ring trades that for memory, at the mean stored bytes per frame codec_stats()
-    reports; it must hold 7 072 (W + 10) bytes whatever the frames (§4.22)."""
-    import math
+    """Bytes of a FRAME_CODEC store's frame ring (None without FRAME_CODEC): R.coded_pool_bytes at
+    POOL_BYTES_PER_TRANSITION bytes per slot, by default (F + 1) x 7 072 for dedup_geometry's F frames.  It must hold
+    7 072 (W + 10) bytes whatever the frames (DESIGN.md §4.22)."""
     if not cfg.FRAME_CODEC:
         return None
-    if cfg.POOL_BYTES_PER_TRANSITION is None:
-        return (int(math.ceil(cfg.FRAMES_PER_TRANSITION * cfg.REPLAY_MEMORY_LEN)) + 1) * 7072
-    return int(cfg.POOL_BYTES_PER_TRANSITION * cfg.REPLAY_MEMORY_LEN) // 16 * 16
+    return R.coded_pool_bytes(cfg.FRAMES_PER_TRANSITION, cfg.REPLAY_MEMORY_LEN, cfg.POOL_BYTES_PER_TRANSITION)
 
 
 def default_apex_model() -> dict:

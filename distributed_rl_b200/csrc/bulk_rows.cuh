@@ -21,10 +21,6 @@ constexpr int BULK_RING_BYTES = 229376;   // 224 KiB of dynamic shared memory pe
 // granularity of a bulk copy); smaller rows cost more in descriptors than they move.
 inline bool is_bulk_row(int64_t row_bytes) { return row_bytes >= 1024 && row_bytes % 16 == 0; }
 
-__host__ __device__ __forceinline__ int64_t clamp_row(int64_t r, int64_t capacity) {
-  return r < 0 ? 0 : (r >= capacity ? capacity - 1 : r);
-}
-
 struct BulkField {
   const uint8_t* src;   // replay field base
   uint8_t* dst;         // output base

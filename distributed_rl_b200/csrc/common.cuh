@@ -117,6 +117,11 @@ __host__ __device__ __forceinline__ double philox_u01(uint64_t seed, uint64_t ct
   return (double)(x & ((1ULL << 53) - 1)) * (1.0 / 9007199254740992.0);
 }
 
+// The slot a sampled index reads: indices outside [0, capacity) are clamped to the nearest slot.
+__host__ __device__ __forceinline__ int64_t clamp_row(int64_t r, int64_t capacity) {
+  return r < 0 ? 0 : (r >= capacity ? capacity - 1 : r);
+}
+
 }  // namespace b2rl
 
 // The sum-tree as the kernels see it (tree.cu): a binary tree of depth `levels` stored sparsely — every 4th

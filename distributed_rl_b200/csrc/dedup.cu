@@ -24,13 +24,14 @@
 // tables, pool_key and the batch scratch stay in HBM.
 // A strip or Ape-X handle's pool may instead be a ring of P 16-byte units holding each frame losslessly encoded
 // (b2rl_dedup_attach_strips_coded, b2rl_dedup_attach_coded, frame_codec.cuh, DESIGN.md §4.21, §4.22).  Frame seq's entry seq % F is then a descriptor
-// (absolute unit offset, length) and the same ids name it.  k_coded_resolve compares a hit's encoding with the frame
-// by decoding it, and sizes the misses; k_coded_offsets lays them out in the unit ring (a frame never straddles its
-// end); k_coded_copy encodes them in place.  The readers decode each sampled slot's frames (k_decode_planes), and conv_1
-// decodes an Ape-X pool's frames on chip (frames.cuh, FrameKind::CodedPlanes).  A rollout handle's pool is coded too
-// (b2rl_dedup_attach_rollouts_coded, DESIGN.md §4.23): its learner step decodes each drawn rollout's distinct frames
-// into a staged pool (k_stage_rollouts) that conv_1 reads as a raw one, and its served slots decode time-major
-// (k_decode_time_major).
+// (absolute unit offset, length) and the same ids name it.  The same kernels run with CODED set: k_dedup_resolve
+// compares a hit's encoding with the frame by decoding it, and sizes the misses; k_coded_offsets lays them out in the
+// unit ring (a frame never straddles its end); k_dedup_copy encodes them in place.  The readers decode each sampled
+// slot's frames (k_decode_planes), and conv_1 decodes an Ape-X pool's frames on chip (frames.cuh,
+// FrameKind::CodedPlanes); every one of them finds an id's encoding through fc_entry (frame_codec.cuh).  A rollout
+// handle's pool is coded too (b2rl_dedup_attach_rollouts_coded, DESIGN.md §4.23): its learner step decodes each drawn
+// rollout's distinct frames into a staged pool (k_stage_rollouts) that conv_1 reads as a raw one, and its served slots
+// decode time-major (k_decode_planes with TIME_MAJOR).
 #include "common.cuh"
 #include "frame_codec.cuh"
 
@@ -177,9 +178,14 @@ struct ResolveArgs {
   int64_t oldest;           // head - W: the oldest seq a hit may reuse
   int32_t* rep;
   int64_t* fseq;
+  int64_t P;                // a coded pool: units in the ring (a raw pool: 0, and the pointers below null)
+  const int64_t* foff;
+  int32_t* usz;             // a coded pool: units of each miss's encoding
 };
 
-template <Layout L>
+// CODED: a hit's stored encoding is decoded and compared with the frame, and every miss gets the length of its
+// encoding in usz.
+template <Layout L, bool CODED>
 __global__ void __launch_bounds__(DD_THREADS)
 k_dedup_resolve(const __grid_constant__ ResolveArgs A) {
   const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
@@ -201,8 +207,21 @@ k_dedup_resolve(const __grid_constant__ ResolveArgs A) {
     }
   }
   cand = __shfl_sync(0xffffffffu, cand, 0);
-  const bool hit = cand >= 0 && warp_equal(A.pool + (cand % A.F) * DD_FRAME, me, lane);
-  if (lane == 0) { A.rep[j] = (int32_t)j; A.fseq[j] = hit ? cand : -1; }
+  bool hit;
+  int units = 0;
+  if constexpr (CODED) {
+    __shared__ FcRows s_rows[DD_THREADS / 32];
+    hit = cand >= 0 && fc_equal(fc_entry(A.pool, A.P, A.foff, A.F, (int32_t)(cand % A.F)), me, s_rows[threadIdx.x >> 5],
+                                lane);
+    units = hit ? 0 : fc_encode(me, nullptr, lane);
+  } else {
+    hit = cand >= 0 && warp_equal(A.pool + (cand % A.F) * DD_FRAME, me, lane);
+  }
+  if (lane == 0) {
+    A.rep[j] = (int32_t)j;
+    A.fseq[j] = hit ? cand : -1;
+    if constexpr (CODED) A.usz[j] = units;
+  }
 }
 
 // Misses (fseq == -1) get seq head, head + 1, ... in batch order; *misses = their count.  One CTA of 1024 threads.
@@ -260,9 +279,15 @@ struct CopyArgs {
   int32_t* planes;          // the replay's planes field
   int64_t slot0, capacity;  // record r goes to slot (slot0 + r) % capacity
   int32_t R;                // Strips: frames per record (Pairs: 8)
+  int64_t P;                // a coded pool: units in the ring (a raw pool: 0, and the pointers below null)
+  const int64_t* uoff;      // a coded pool: absolute unit offset and units of each miss (k_coded_offsets, resolve)
+  const int32_t* usz;
+  int64_t* foff;            // a coded pool: the descriptor of each entry
+  int32_t* flen;
 };
 
-template <Layout L>
+// CODED: each miss is encoded in place at its unit offset, and its entry gets the descriptor.
+template <Layout L, bool CODED>
 __global__ void __launch_bounds__(DD_THREADS)
 k_dedup_copy(const __grid_constant__ CopyArgs A) {
   const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
@@ -279,9 +304,18 @@ k_dedup_copy(const __grid_constant__ CopyArgs A) {
     A.planes[slot * R + (j - rec * R)] = (int32_t)ps;
   }
   if (r != j || sq < A.head) return;        // a batch duplicate or a hit: nothing to store
-  const uint4* src = reinterpret_cast<const uint4*>(batch_frame<L>(A.s, A.ns, j));
-  uint4* dst = reinterpret_cast<uint4*>(A.pool + ps * DD_FRAME);
-  for (int i = lane; i < DD_VEC; i += 32) dst[i] = src[i];
+  if constexpr (CODED) {
+    const int64_t off = A.uoff[j];
+    fc_encode(batch_frame<L>(A.s, A.ns, j), A.pool + (off % A.P) * 16, lane);
+    if (lane == 0) {
+      A.foff[ps] = off;
+      A.flen[ps] = A.usz[j];
+    }
+  } else {
+    const uint4* src = reinterpret_cast<const uint4*>(batch_frame<L>(A.s, A.ns, j));
+    uint4* dst = reinterpret_cast<uint4*>(A.pool + ps * DD_FRAME);
+    for (int i = lane; i < DD_VEC; i += 32) dst[i] = src[i];
+  }
   if (lane == 0) {
     const unsigned long long k = A.key[j];
     A.pool_key[ps] = k;
@@ -296,60 +330,6 @@ k_dedup_rebuild(const unsigned long long* __restrict__ pool_key, int64_t F, int6
   const int64_t q = lo + (int64_t)blockIdx.x * 256 + threadIdx.x;
   if (q >= hi) return;
   atomicMax(tseq + claim(tkey, T, pool_key[q % F]), (unsigned long long)(q + 1));
-}
-
-// ---- the coded pool (b2rl_dedup_attach_strips_coded, _coded): frames as frame_codec.cuh encodings in a ring of P
-// units ----
-
-// k_dedup_resolve for a coded pool: a hit's stored encoding is decoded and compared with the frame, and every miss
-// gets the length of its encoding in usz.
-struct CodedResolveArgs {
-  const uint8_t* s;
-  int64_t frames;
-  const unsigned long long* key;
-  const unsigned long long* bkey;
-  const int32_t* bpos;
-  int64_t BT;
-  const unsigned long long* tkey;
-  const unsigned long long* tseq;
-  int64_t T;
-  const uint8_t* pool;
-  int64_t P;
-  const int64_t* foff;
-  int64_t F;
-  int64_t oldest;           // head - W: the oldest seq a hit may reuse
-  int32_t* rep;
-  int64_t* fseq;
-  int32_t* usz;
-  const uint8_t* ns;        // Pairs: the s' stacks
-};
-
-template <Layout L>
-__global__ void __launch_bounds__(DD_THREADS)
-k_coded_resolve(const __grid_constant__ CodedResolveArgs A) {
-  __shared__ FcRows s_rows[DD_THREADS / 32];
-  const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (j >= A.frames) return;
-  const unsigned long long k = A.key[j];
-  const uint8_t* me = batch_frame<L>(A.s, A.ns, j);
-  const int32_t first = A.bpos[find(A.bkey, A.BT, k)];
-  if (first < j && warp_equal(batch_frame<L>(A.s, A.ns, first), me, lane)) {
-    if (lane == 0) { A.rep[j] = first; A.fseq[j] = -2; }
-    return;
-  }
-  int64_t cand = -1;
-  if (lane == 0) {
-    const int64_t e = find(A.tkey, A.T, k);
-    if (e >= 0) {
-      const unsigned long long s1 = A.tseq[e];
-      if (s1 > 0 && (int64_t)(s1 - 1) >= A.oldest) cand = (int64_t)(s1 - 1);
-    }
-  }
-  cand = __shfl_sync(0xffffffffu, cand, 0);
-  const bool hit = cand >= 0 && fc_equal(A.pool + (A.foff[cand % A.F] % A.P) * 16, me, s_rows[threadIdx.x >> 5], lane);
-  const int units = hit ? 0 : fc_encode(me, nullptr, lane);
-  if (lane == 0) { A.rep[j] = (int32_t)j; A.fseq[j] = hit ? cand : -1; A.usz[j] = units; }
 }
 
 // After k_dedup_scan: the misses (fseq >= head) get absolute unit offsets in batch order from U0 on, and out[1] = the
@@ -396,62 +376,12 @@ k_coded_offsets(const int64_t* __restrict__ fseq, const int32_t* __restrict__ us
   if (threadIdx.x == 0) out[1] = running;
 }
 
-struct CodedCopyArgs {
-  const uint8_t* s;
-  int64_t frames;
-  const unsigned long long* key;
-  const int32_t* rep;
-  const int64_t* fseq;
-  int64_t head;             // first seq of this batch's misses
-  const int64_t* uoff;
-  const int32_t* usz;
-  uint8_t* pool;
-  int64_t P;
-  int64_t* foff;
-  int32_t* flen;
-  unsigned long long* pool_key;
-  int64_t F;
-  unsigned long long* tkey;
-  unsigned long long* tseq;
-  int64_t T;
-  int32_t* planes;          // the replay's planes field
-  int64_t slot0, capacity;  // record r goes to slot (slot0 + r) % capacity
-  int32_t R;
-  const uint8_t* ns;        // Pairs: the s' stacks
-};
-
-// k_dedup_copy for a coded pool: each miss is encoded in place at its unit offset, and its entry gets the descriptor.
-template <Layout L>
-__global__ void __launch_bounds__(DD_THREADS)
-k_coded_copy(const __grid_constant__ CodedCopyArgs A) {
-  const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (j >= A.frames) return;
-  const int32_t r = A.rep[j];
-  const int64_t sq = A.fseq[r];
-  const int64_t ps = sq % A.F;
-  if (lane == 0) {
-    const int64_t rec = j / A.R;
-    int64_t slot = A.slot0 + rec;
-    if (slot >= A.capacity) slot -= A.capacity;
-    A.planes[slot * A.R + (j - rec * A.R)] = (int32_t)ps;
-  }
-  if (r != j || sq < A.head) return;        // a batch duplicate or a hit: nothing to store
-  const int64_t off = A.uoff[j];
-  fc_encode(batch_frame<L>(A.s, A.ns, j), A.pool + (off % A.P) * 16, lane);
-  if (lane == 0) {
-    const unsigned long long k = A.key[j];
-    A.foff[ps] = off;
-    A.flen[ps] = A.usz[j];
-    A.pool_key[ps] = k;
-    atomicMax(A.tseq + claim(A.tkey, A.T, k), (unsigned long long)(sq + 1));
-  }
-}
-
-// Frame j of draw k = j / R: slot clamp_row(idx[k])'s frame j % R, decoded from the pool.  One warp per frame.
+// Frame c = j % R of draw k = j / R: slot clamp_row(idx[k])'s frame c, decoded from the pool.  One warp per frame.
 // Strips: into dst + j * 7 056, the (n, R, 84, 84) strips.  Pairs (R = 8): planes 0-3 into the (n, 4, 84, 84) s stacks
-// at dst, planes 4-7 into the s' stacks at dst2; a NULL output's frames are skipped.
-template <Layout L>
+// at dst, planes 4-7 into the s' stacks at dst2; a NULL output's frames are skipped.  TIME_MAJOR (b2rl_serve_fill_uniform
+// on a coded rollout handle, Strips with R = 4 (T + 1)): the destination of add_planes_time_major, frame c % 4 of row
+// (c / 4) n + k of the (T + 1) n stacks at dst.
+template <Layout L, bool TIME_MAJOR>
 __global__ void __launch_bounds__(DD_THREADS)
 k_decode_planes(const uint8_t* __restrict__ pool, int64_t P, const int64_t* __restrict__ foff, int64_t F,
                 const int32_t* __restrict__ planes, int32_t R, const int64_t* __restrict__ idx, int64_t n,
@@ -461,37 +391,16 @@ k_decode_planes(const uint8_t* __restrict__ pool, int64_t P, const int64_t* __re
   const int lane = threadIdx.x & 31;
   if (j >= n * R) return;
   const int64_t k = j / R;
+  const int64_t c = j - k * R;
   uint8_t* out = dst + j * DD_FRAME;
+  if constexpr (TIME_MAJOR) out = dst + (((c >> 2) * n + k) * 4 + (c & 3)) * DD_FRAME;
   if constexpr (L == Layout::Pairs) {
-    const int c = (int)(j - k * R);
     out = (c < 4 ? dst : dst2);
     if (out == nullptr) return;
     out += (4 * k + (c & 3)) * DD_FRAME;
   }
-  int64_t slot = idx[k];
-  slot = slot < 0 ? 0 : (slot >= capacity ? capacity - 1 : slot);
-  const int64_t id = (uint32_t)planes[R * slot + (j - k * R)] % (uint64_t)F;   // any int32 names an entry
-  fc_decode(pool + (foff[id] % P) * 16, out, s_rows[threadIdx.x >> 5], lane);
-}
-
-// b2rl_serve_fill_uniform on a coded rollout handle (R = 4 (T + 1)): k_decode_planes<Strips> with the time-major
-// destination of add_planes_time_major, frame c = j % R of draw k = j / R to frame c % 4 of row (c / 4) n + k of the
-// (T + 1) n stacks at dst.  One warp per frame.
-__global__ void __launch_bounds__(DD_THREADS)
-k_decode_time_major(const uint8_t* __restrict__ pool, int64_t P, const int64_t* __restrict__ foff, int64_t F,
-                    const int32_t* __restrict__ planes, int32_t R, const int64_t* __restrict__ idx, int64_t n,
-                    int64_t capacity, uint8_t* __restrict__ dst) {
-  __shared__ FcRows s_rows[DD_THREADS / 32];
-  const int64_t j = ((int64_t)blockIdx.x * DD_THREADS + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (j >= n * R) return;
-  const int64_t k = j / R;
-  const int64_t c = j - k * R;
-  int64_t slot = idx[k];
-  slot = slot < 0 ? 0 : (slot >= capacity ? capacity - 1 : slot);
-  const int64_t id = (uint32_t)planes[R * slot + c] % (uint64_t)F;
-  fc_decode(pool + (foff[id] % P) * 16, dst + (((c >> 2) * n + k) * 4 + (c & 3)) * DD_FRAME,
-            s_rows[threadIdx.x >> 5], lane);
+  fc_decode(fc_entry(pool, P, foff, F, planes[R * clamp_row(idx[k], capacity) + c]), out, s_rows[threadIdx.x >> 5],
+            lane);
 }
 
 // b2rl_dedup_stage_rollouts: frame c = j % R of draw k = j / R is pool id planes[R slot + c] % F of slot
@@ -508,14 +417,12 @@ k_stage_rollouts(const uint8_t* __restrict__ pool, int64_t P, const int64_t* __r
   if (j >= n * R) return;
   const int64_t k = j / R;
   const int32_t c = (int32_t)(j - k * R);
-  int64_t slot = idx[k];
-  slot = slot < 0 ? 0 : (slot >= capacity ? capacity - 1 : slot);
-  const int32_t* ids = planes + R * slot;
-  const int64_t id = (uint32_t)ids[c] % (uint64_t)F;   // any int32 names an entry
+  const int32_t* ids = planes + R * clamp_row(idx[k], capacity);
+  const uint32_t id = (uint32_t)ids[c] % (uint32_t)F;   // fc_entry's entry
   int32_t first = c;
   for (int32_t i0 = 0; i0 < c; i0 += 32) {              // c is the warp's: every lane takes the same exit
     const int32_t i = i0 + lane;
-    const unsigned m = __ballot_sync(0xffffffffu, i < c && (int64_t)((uint32_t)ids[i] % (uint64_t)F) == id);
+    const unsigned m = __ballot_sync(0xffffffffu, i < c && (uint32_t)ids[i] % (uint32_t)F == id);
     if (m != 0u) {
       first = i0 + __ffs((int)m) - 1;
       break;
@@ -523,7 +430,7 @@ k_stage_rollouts(const uint8_t* __restrict__ pool, int64_t P, const int64_t* __r
   }
   if (lane == 0) staged_planes[j] = (int32_t)(k * R + first);
   if (first != c) return;
-  fc_decode(pool + (foff[id] % P) * 16, staged_pool + j * DD_FRAME, s_rows[threadIdx.x >> 5], lane);
+  fc_decode(fc_entry(pool, P, foff, F, ids[c]), staged_pool + j * DD_FRAME, s_rows[threadIdx.x >> 5], lane);
 }
 
 // b2rl_frame_encode / b2rl_frame_decode: frame j <-> the encoding at enc + j * FC_RAW_BYTES.  One warp per frame.
@@ -570,15 +477,11 @@ bool dedup_pool_coded(const b2rl_replay* h) { return h->dedup->P > 0; }
 
 static unsigned warps_grid(int64_t frames) { return (unsigned)((frames * 32 + DD_THREADS - 1) / DD_THREADS); }
 
-int gather_coded_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, uint8_t* dst2_dev,
-                        cudaStream_t st) {
+// n draws' frames through k_decode_planes (one of its instantiations), one warp per frame.
+template <class Kernel>
+static int decode_planes(Kernel kernel, b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev,
+                         uint8_t* dst2_dev, cudaStream_t st) {
   const DedupState* d = h->dedup;
-  const bool pairs = d->layout == Layout::Pairs;
-  B2RL_REQUIRE((uintptr_t)dst_dev % 16 == 0 && (uintptr_t)dst2_dev % 16 == 0,
-               pairs ? "frame stack outputs must be 16-byte aligned" : "frame strip outputs must be 16-byte aligned");
-  B2RL_REQUIRE(pairs || dst2_dev == nullptr, "a strip handle has one frame output");
-  if (n == 0 || (dst_dev == nullptr && dst2_dev == nullptr)) return B2RL_OK;
-  auto kernel = pairs ? k_decode_planes<Layout::Pairs> : k_decode_planes<Layout::Strips>;
   kernel<<<warps_grid(n * d->R), DD_THREADS, 0, st>>>(d->pool, d->P, d->foff, d->F,
                                                       (const int32_t*)h->field[d->planes_field], d->R, idx_dev, n,
                                                       h->capacity, dst_dev, dst2_dev);
@@ -587,14 +490,19 @@ int gather_coded_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8
   return B2RL_OK;
 }
 
+int gather_coded_planes(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, uint8_t* dst2_dev,
+                        cudaStream_t st) {
+  const bool pairs = h->dedup->layout == Layout::Pairs;
+  B2RL_REQUIRE((uintptr_t)dst_dev % 16 == 0 && (uintptr_t)dst2_dev % 16 == 0,
+               pairs ? "frame stack outputs must be 16-byte aligned" : "frame strip outputs must be 16-byte aligned");
+  B2RL_REQUIRE(pairs || dst2_dev == nullptr, "a strip handle has one frame output");
+  if (n == 0 || (dst_dev == nullptr && dst2_dev == nullptr)) return B2RL_OK;
+  return decode_planes(pairs ? k_decode_planes<Layout::Pairs, false> : k_decode_planes<Layout::Strips, false>, h,
+                       idx_dev, n, dst_dev, dst2_dev, st);
+}
+
 int decode_rollouts_time_major(b2rl_replay* h, const int64_t* idx_dev, int64_t n, uint8_t* dst_dev, cudaStream_t st) {
-  const DedupState* d = h->dedup;
-  k_decode_time_major<<<warps_grid(n * d->R), DD_THREADS, 0, st>>>(d->pool, d->P, d->foff, d->F,
-                                                                    (const int32_t*)h->field[d->planes_field], d->R,
-                                                                    idx_dev, n, h->capacity, dst_dev);
-  count_launch();
-  B2RL_CHECK_LAUNCH();
-  return B2RL_OK;
+  return decode_planes(k_decode_planes<Layout::Strips, true>, h, idx_dev, n, dst_dev, nullptr, st);
 }
 
 }  // namespace b2rl
@@ -884,15 +792,10 @@ static int dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8_t* ns_de
   k_dedup_hash<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(s_dev, ns_dev, frames, d->mask, d->key, d->bkey, d->bpos,
                                                           d->BT);
   const bool coded = d->P > 0;
-  if (coded) {
-    CodedResolveArgs A{s_dev, frames, d->key, d->bkey, d->bpos, d->BT, d->tkey, d->tseq, d->T, d->pool, d->P,
-                       d->foff, d->F, head - d->W, d->rep, d->fseq, d->usz, ns_dev};
-    k_coded_resolve<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(A);
-  } else {
-    ResolveArgs A{s_dev, ns_dev, frames, d->key, d->bkey, d->bpos, d->BT, d->tkey, d->tseq, d->T, d->pool, d->F,
-                  head - d->W, d->rep, d->fseq};
-    k_dedup_resolve<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(A);
-  }
+  const ResolveArgs A{s_dev, ns_dev, frames, d->key, d->bkey, d->bpos, d->BT, d->tkey, d->tseq, d->T, d->pool, d->F,
+                      head - d->W, d->rep, d->fseq, d->P, d->foff, d->usz};
+  auto resolve = coded ? k_dedup_resolve<L, true> : k_dedup_resolve<L, false>;
+  resolve<<<warps_grid(frames), DD_THREADS, 0, st>>>(A);
   k_dedup_scan<<<1, 1024, 0, st>>>(d->fseq, frames, head, d->misses_dev);
   count_launch(3);
   if (coded) {
@@ -922,30 +825,27 @@ static int dedup_push(b2rl_replay* h, const uint8_t* s_dev, const uint8_t* ns_de
     if (rc != B2RL_OK) return rc;
   }
   // 4. pool ids, new frames, key table; then the other fields and the priorities as b2rl_replay_push does
-  if (coded) {
-    CodedCopyArgs C{s_dev, frames, d->key, d->rep, d->fseq, head, d->uoff, d->usz, d->pool, d->P, d->foff, d->flen,
-                    d->pool_key, d->F, d->tkey, d->tseq, d->T, (int32_t*)h->field[d->planes_field], h->head,
-                    h->capacity, d->R, ns_dev};
-    k_coded_copy<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(C);
-  } else {
-    CopyArgs C{s_dev, ns_dev, frames, d->key, d->rep, d->fseq, head, d->pool, d->pool_key, d->F, d->tkey, d->tseq,
-               d->T, (int32_t*)h->field[d->planes_field], h->head, h->capacity, d->R};
-    k_dedup_copy<L><<<warps_grid(frames), DD_THREADS, 0, st>>>(C);
-  }
+  const CopyArgs C{s_dev, ns_dev, frames, d->key, d->rep, d->fseq, head, d->pool, d->pool_key, d->F, d->tkey, d->tseq,
+                   d->T, (int32_t*)h->field[d->planes_field], h->head, h->capacity, d->R, d->P, d->uoff, d->usz,
+                   d->foff, d->flen};
+  auto copy = coded ? k_dedup_copy<L, true> : k_dedup_copy<L, false>;
+  copy<<<warps_grid(frames), DD_THREADS, 0, st>>>(C);
   count_launch();
   B2RL_CHECK_LAUNCH();
   int rc = copy_ring_range(h, fields_src, h->head, n, st);
   if (rc != B2RL_OK) return rc;
   B2RL_CUDA(cudaMemcpyAsync(h->scratch_val, prios, (size_t)n * sizeof(float), cudaMemcpyDefault, st));
-  for (int64_t i = 0; i < n; ++i) d->ins[(size_t)((h->head + i) % h->capacity)] = head;
-  if (coded)
-    for (int64_t i = 0; i < n; ++i) d->uins[(size_t)((h->head + i) % h->capacity)] = d->units;
+  for (int64_t i = 0; i < n; ++i) {
+    const size_t slot = (size_t)((h->head + i) % h->capacity);
+    d->ins[slot] = head;
+    if (coded) d->uins[slot] = d->units;
+  }
   rc = publish(h, h->scratch_val, n, st);
   if (rc != B2RL_OK) return rc;
   B2RL_CUDA(cudaEventRecord(d->done, st));
   d->head = head_new;
   d->used += head_new - head;
-  if (coded) d->units = units_new;
+  d->units = units_new;
   return B2RL_OK;
 }
 

@@ -204,6 +204,16 @@ __device__ __forceinline__ void fc_decode(const uint8_t* __restrict__ e, uint8_t
   __syncwarp();     // S is free for the warp's next frame
 }
 
+// The encoding of pool id `id` in a coded pool: a ring `pool` of P 16-byte units whose entry e starts at unit
+// foff[e] % P.  Any int32 names an entry (read as unsigned, % F; the attach keeps F below 2^31) and any offset a unit
+// of the ring, so whatever a plane table holds the decode reads inside the pool's allocation (P units plus
+// FC_RAW_BYTES: fc_prepare).  Every reader of a coded pool takes its address from here (dedup.cu's ingest and
+// decoders, conv_1's coded_frame in frames.cuh), so all of them read the same bytes for the same id.
+__device__ __forceinline__ const uint8_t* fc_entry(const uint8_t* pool, int64_t P, const int64_t* foff, int64_t F,
+                                                   int32_t id) {
+  return pool + (foff[(uint32_t)id % (uint32_t)F] % P) * 16;
+}
+
 // One warp: whether the encoding e decodes to the frame f (16-byte aligned); the same answer in every lane.
 __device__ __forceinline__ bool fc_equal(const uint8_t* __restrict__ e, const uint8_t* __restrict__ f, FcRows& S,
                                          int lane) {

@@ -66,12 +66,9 @@ __device__ __forceinline__ void load_row(const FrameSource& S, const uint8_t* fr
   }
 }
 
-// CodedPlanes: the encoding of frame c of row `row`.  Any int32 id names an entry (read as unsigned, % F), and any
-// offset a unit of the ring, so whatever the table holds the decode reads inside the pool's allocation (P units plus
-// FC_RAW_BYTES: fc_prepare).  The arithmetic is k_decode_planes' (dedup.cu), so both decode the same bytes.
+// CodedPlanes: the encoding of frame c of row `row`, at fc_entry's address for its id.
 __device__ __forceinline__ const uint8_t* coded_frame(const FrameSource& S, int64_t row, int c) {
-  const uint32_t id = (uint32_t)S.planes[row * S.plane_stride + S.plane_base + c] % (uint32_t)S.entries;   // F < 2^31
-  return S.base + (S.foff[id] % S.units) * 16;
+  return fc_entry(S.base, S.units, S.foff, S.entries, S.planes[row * S.plane_stride + S.plane_base + c]);
 }
 
 // NWARPS warps decode the encoding e into the frame dst (16-byte aligned, shared memory) together, as barrier `bar`;

@@ -64,12 +64,7 @@ class ImpalaConfig:
                                                    # size it from RolloutDedupReplay.codec_stats()
 
     def __post_init__(self):
-        if self.STAGED_POOL_CODEC and not self.FRAME_DEDUP:
-            raise ValueError("STAGED_POOL_CODEC encodes the frame pool of a FRAME_DEDUP store: set FRAME_DEDUP with it")
-        if self.POOL_BYTES_PER_ROLLOUT is not None and not self.STAGED_POOL_CODEC:
-            raise ValueError("POOL_BYTES_PER_ROLLOUT sizes the coded frame pool: set STAGED_POOL_CODEC with it")
-        if self.POOL_BYTES_PER_ROLLOUT is not None and not self.POOL_BYTES_PER_ROLLOUT > 0:
-            raise ValueError(f"POOL_BYTES_PER_ROLLOUT must be positive, not {self.POOL_BYTES_PER_ROLLOUT}")
+        R.check_codec_keys(self, "STAGED_POOL_CODEC", "POOL_BYTES_PER_ROLLOUT")
 
     @staticmethod
     def from_configuration():
@@ -90,28 +85,16 @@ def dedup_geometry(cfg: ImpalaConfig) -> tuple:
     pool - window frames have been stored after it: at the default 24 frames per slot, 21 REPLAY_MEMORY_LEN frames or
     more, above the ~T = 20 new frames per rollout the reference actors send, so the slot ring wraps first.  The window
     only has to reach back two rollouts of the same actor (the bootstrap stack and checkLength's padding)."""
-    import math
-    import warnings
-    F = int(math.ceil(cfg.FRAMES_PER_ROLLOUT * cfg.REPLAY_MEMORY_LEN))
-    W = min(int(cfg.DEDUP_WINDOW), F // 8)
-    if W < cfg.DEDUP_WINDOW:
-        warnings.warn(f"DEDUP_WINDOW = {cfg.DEDUP_WINDOW} frames is more than an eighth of the {F}-frame pool: the "
-                      f"frame-deduplicated replay uses a window of {W} frames", stacklevel=2)
-    return F, W
+    return R.dedup_pool_geometry(cfg.FRAMES_PER_ROLLOUT, cfg.REPLAY_MEMORY_LEN, cfg.DEDUP_WINDOW)
 
 
 def pool_bytes(cfg: ImpalaConfig) -> int | None:
-    """Bytes of a STAGED_POOL_CODEC store's frame ring (None without STAGED_POOL_CODEC): POOL_BYTES_PER_ROLLOUT x
-    REPLAY_MEMORY_LEN, rounded down to 16 bytes.  The default is the raw size plus one frame, (F + 1) x 7 072 for
-    dedup_geometry's F frames, as r2d2.pool_bytes and apex.pool_bytes: a slot then dies by the byte rule no earlier than
-    by the frame rule (DESIGN §4.21).  A smaller ring trades that for memory, at the mean stored bytes per frame
-    codec_stats() reports; it must hold 7 072 (W + 2 + 4 (T + 1)) bytes whatever the frames (§4.23)."""
-    import math
+    """Bytes of a STAGED_POOL_CODEC store's frame ring (None without STAGED_POOL_CODEC): R.coded_pool_bytes at
+    POOL_BYTES_PER_ROLLOUT bytes per slot, by default (F + 1) x 7 072 for dedup_geometry's F frames.  It must hold
+    7 072 (W + 2 + 4 (T + 1)) bytes whatever the frames (DESIGN.md §4.23)."""
     if not cfg.STAGED_POOL_CODEC:
         return None
-    if cfg.POOL_BYTES_PER_ROLLOUT is None:
-        return (int(math.ceil(cfg.FRAMES_PER_ROLLOUT * cfg.REPLAY_MEMORY_LEN)) + 1) * 7072
-    return int(cfg.POOL_BYTES_PER_ROLLOUT * cfg.REPLAY_MEMORY_LEN) // 16 * 16
+    return R.coded_pool_bytes(cfg.FRAMES_PER_ROLLOUT, cfg.REPLAY_MEMORY_LEN, cfg.POOL_BYTES_PER_ROLLOUT)
 
 
 def rollout_frames(store):

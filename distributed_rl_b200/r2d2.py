@@ -99,14 +99,9 @@ class R2D2Config:
         if self.FRAME_DEDUP and (self.HOST_FRAMES or self.PAYLOAD_POOL):
             raise ValueError("FRAME_DEDUP keeps its frames in a frame pool (in host memory with HOST_POOL) and stores "
                              "every pushed sequence: it takes neither HOST_FRAMES nor PAYLOAD_POOL")
-        if self.POOL_CODEC and not self.FRAME_DEDUP:
-            raise ValueError("POOL_CODEC encodes the frame pool of a FRAME_DEDUP store: set FRAME_DEDUP with it")
         if self.POOL_CODEC and self.HOST_POOL:
             raise ValueError("POOL_CODEC keeps its coded frame pool in HBM: it does not take HOST_POOL")
-        if self.POOL_BYTES_PER_SEQUENCE is not None and not self.POOL_CODEC:
-            raise ValueError("POOL_BYTES_PER_SEQUENCE sizes the coded frame pool: set POOL_CODEC with it")
-        if self.POOL_BYTES_PER_SEQUENCE is not None and not self.POOL_BYTES_PER_SEQUENCE > 0:
-            raise ValueError(f"POOL_BYTES_PER_SEQUENCE must be positive, not {self.POOL_BYTES_PER_SEQUENCE}")
+        R.check_codec_keys(self, "POOL_CODEC", "POOL_BYTES_PER_SEQUENCE")
         if self.FRAME_DEDUP:
             self.FRAME_STRIP = True
 
@@ -125,38 +120,21 @@ class R2D2Config:
                           HOST_FRAMES=bool(getattr(C, "HOST_FRAMES", False)), **kw)
 
 
-def _pool_frames(cfg: R2D2Config) -> int:
-    """F of a FRAME_DEDUP replay: ceil(FRAMES_PER_SEQUENCE * REPLAY_MEMORY_LEN) frames (dedup_geometry, pool_bytes)."""
-    import math
-    return int(math.ceil(cfg.FRAMES_PER_SEQUENCE * cfg.REPLAY_MEMORY_LEN))
-
-
 def dedup_geometry(cfg: R2D2Config) -> tuple:
     """(pool frames, window) of a FRAME_DEDUP replay: ceil(FRAMES_PER_SEQUENCE * REPLAY_MEMORY_LEN) frames, and
     DEDUP_WINDOW capped at an eighth of them (as apex.dedup_geometry).  A slot stays live until pool - window frames
     have been stored after it: at the default 48 frames per slot, 42 REPLAY_MEMORY_LEN frames or more, above the
     ~40 new frames per sequence the reference actors send (T / 2 in mid-episode), so the slot ring wraps first.  The
     window only has to reach back to the same actor's previous sequence."""
-    import warnings
-    F = _pool_frames(cfg)
-    W = min(int(cfg.DEDUP_WINDOW), F // 8)
-    if W < cfg.DEDUP_WINDOW:
-        warnings.warn(f"DEDUP_WINDOW = {cfg.DEDUP_WINDOW} frames is more than an eighth of the {F}-frame pool: the "
-                      f"frame-deduplicated replay uses a window of {W} frames", stacklevel=2)
-    return F, W
+    return R.dedup_pool_geometry(cfg.FRAMES_PER_SEQUENCE, cfg.REPLAY_MEMORY_LEN, cfg.DEDUP_WINDOW)
 
 
 def pool_bytes(cfg: R2D2Config) -> int | None:
-    """Bytes of a POOL_CODEC store's frame ring (None without POOL_CODEC): POOL_BYTES_PER_SEQUENCE x REPLAY_MEMORY_LEN,
-    rounded down to 16 bytes.  The default is the raw size plus one frame, (F + 1) x 7 072 for dedup_geometry's F
-    frames: a slot then dies by the byte rule no earlier than by the frame rule (DESIGN §4.21), so the ring holds
-    whatever the frame pool would.  A smaller ring trades that for memory, at the mean stored bytes per frame that
-    codec_stats() reports."""
+    """Bytes of a POOL_CODEC store's frame ring (None without POOL_CODEC): R.coded_pool_bytes at
+    POOL_BYTES_PER_SEQUENCE bytes per slot, by default (F + 1) x 7 072 for dedup_geometry's F frames."""
     if not cfg.POOL_CODEC:
         return None
-    if cfg.POOL_BYTES_PER_SEQUENCE is None:
-        return (_pool_frames(cfg) + 1) * 7072
-    return int(cfg.POOL_BYTES_PER_SEQUENCE * cfg.REPLAY_MEMORY_LEN) // 16 * 16
+    return R.coded_pool_bytes(cfg.FRAMES_PER_SEQUENCE, cfg.REPLAY_MEMORY_LEN, cfg.POOL_BYTES_PER_SEQUENCE)
 
 
 class Replay(ReplayThread):

@@ -8,6 +8,8 @@ facing mirrors (per.py: PER / PrioritizedMemory, apex.py: Replay) are built on.
 from __future__ import annotations
 
 import ctypes as C
+import math
+import warnings
 from dataclasses import dataclass
 from typing import Sequence
 
@@ -533,6 +535,40 @@ class DeviceReplay:
         return out
 
 
+def dedup_pool_geometry(frames_per_slot: float, slots: int, window: int) -> tuple:
+    """(pool frames F, window W) of a frame-deduplicated store: ceil(frames_per_slot * slots) frames, and `window`
+    capped at an eighth of them, with a UserWarning when the cap applies.  A slot stays live until F - W frames have
+    been stored after it, so the cap keeps that at least 7/8 of the pool (apex, r2d2 and impala.dedup_geometry)."""
+    F = int(math.ceil(frames_per_slot * slots))
+    W = min(int(window), F // 8)
+    if W < window:
+        warnings.warn(f"DEDUP_WINDOW = {window} frames is more than an eighth of the {F}-frame pool: the "
+                      f"frame-deduplicated replay uses a window of {W} frames", stacklevel=3)
+    return F, W
+
+
+def coded_pool_bytes(frames_per_slot: float, slots: int, bytes_per_slot: float | None) -> int:
+    """Bytes of a coded frame pool's ring: bytes_per_slot * slots rounded down to 16 bytes, or by default the raw size
+    plus one frame, (F + 1) * 7 072 for dedup_pool_geometry's F, at which a slot dies by the byte rule no earlier than
+    by the frame rule (DESIGN.md §4.21).  A smaller ring trades that for memory, at the mean stored bytes per frame
+    codec_stats() reports (apex, r2d2 and impala.pool_bytes)."""
+    if bytes_per_slot is None:
+        return (int(math.ceil(frames_per_slot * slots)) + 1) * CODED_FRAME_BYTES
+    return int(bytes_per_slot * slots) // 16 * 16
+
+
+def check_codec_keys(cfg, codec: str, bytes_per_slot: str) -> None:
+    """Refuse a learner config whose codec key `codec` is set without FRAME_DEDUP, or whose ring size key
+    `bytes_per_slot` is set without `codec` or is not positive."""
+    per = getattr(cfg, bytes_per_slot)
+    if getattr(cfg, codec) and not cfg.FRAME_DEDUP:
+        raise ValueError(f"{codec} encodes the frame pool of a FRAME_DEDUP store: set FRAME_DEDUP with it")
+    if per is not None and not getattr(cfg, codec):
+        raise ValueError(f"{bytes_per_slot} sizes the coded frame pool: set {codec} with it")
+    if per is not None and not per > 0:
+        raise ValueError(f"{bytes_per_slot} must be positive, not {per}")
+
+
 class DedupReplay(DeviceReplay):
     """An Ape-X replay that stores every distinct frame once (b2rl_dedup_attach): slots hold APEX_DEDUP_FIELDS, the
     frames live in a pool of `pool_frames` frames, and a pushed frame reuses a stored one with the same content among
@@ -542,32 +578,47 @@ class DedupReplay(DeviceReplay):
 
     RECORD_FIELDS = APEX_FIELDS      # what push takes and gather returns
     coded = False                    # frames stored encoded (CodedDedupReplay, StripDedupReplay(pool_bytes=...))
+    host_pool = False                # frames in pinned host memory (StripDedupReplay(host_pool=True))
 
     def __init__(self, capacity: int, pool_frames: int, window: int, device="cuda:0",
                  hash_mask: int = DEDUP_HASH_MASK):
-        super().__init__(capacity, APEX_DEDUP_FIELDS, device)
-        check(self.lib.b2rl_dedup_attach(self._h, 0, int(pool_frames), int(window), int(hash_mask)))
-        self._attached(pool_frames, window)
+        self._attach(capacity, APEX_DEDUP_FIELDS, device, "b2rl_dedup_attach", (), pool_frames, window, hash_mask)
 
-    def _attached(self, pool_frames: int, window: int) -> None:
+    def _attach(self, capacity: int, fields, device, entry: str, lead: tuple, pool_frames: int, window: int,
+                hash_mask: int, pool_bytes: int | None = None, host_pool: bool = False) -> None:
+        """Every deduplicated store's constructor: the slot ring of `fields`, then the frame pool attached by the
+        entry point `entry` (its _placed form with host_pool, its _coded form with pool_bytes) with the arguments
+        `lead` between the planes field and pool_frames.  `pool` is the (F, 84, 84) frames on the device, a CPU
+        tensor over them with host_pool, or the flat uint8 ring of 16-byte units of a coded pool, whose `offsets`
+        are each entry's absolute unit offset."""
+        DeviceReplay.__init__(self, capacity, fields, device)
         self.pool_frames, self.window = int(pool_frames), int(window)
-        p, mb, on_host = C.c_void_p(), C.c_int64(), C.c_int32()
-        check(self.lib.b2rl_dedup_info(self._h, None, None, C.byref(mb)))
-        check(self.lib.b2rl_dedup_pool_placement(self._h, C.byref(on_host), C.byref(p)))
+        self.coded, self.host_pool = pool_bytes is not None, bool(host_pool)
+        args = (self._h, 0, *lead, self.pool_frames, self.window, int(hash_mask))
+        if self.host_pool:
+            with hostmem.on_gpu_node(self.device):   # pinned pages on the GPU's NUMA node (first touch: the library)
+                check(getattr(self.lib, entry + "_placed")(*args, 1))
+        elif self.coded:
+            check(getattr(self.lib, entry + "_coded")(*args, int(pool_bytes)))
+        else:
+            check(getattr(self.lib, entry)(*args))
+        p, mb = C.c_void_p(), C.c_int64()
+        check(self.lib.b2rl_dedup_info(self._h, C.byref(p), None, C.byref(mb)))
         self.max_batch = mb.value
-        if on_host.value:       # a CPU tensor over the pinned frames, as field_view of a host field
+        if self.host_pool:      # a CPU tensor over the pinned frames, as field_view of a host field
+            on_host = C.c_int32()
+            check(self.lib.b2rl_dedup_pool_placement(self._h, C.byref(on_host), C.byref(p)))
             self.pool = torch.from_numpy(np.asarray(_HostView(p.value, (self.pool_frames, 84, 84), "|u1", self)))
             return
         with torch.cuda.device(self.device):
-            self.pool = torch.as_tensor(_CudaView(p.value, (self.pool_frames, 84, 84), "|u1", self), device=self.device)
-
-    def _coded_pool(self) -> None:
-        """`pool` of a coded store: the flat uint8 ring of 16-byte units the encodings live in, not (F, 84, 84)."""
-        p = C.c_void_p()
-        check(self.lib.b2rl_dedup_info(self._h, C.byref(p), None, None))
-        self.pool_bytes = 16 * self.codec_stats()["pool_units"]
-        with torch.cuda.device(self.device):
+            if not self.coded:
+                self.pool = torch.as_tensor(_CudaView(p.value, (self.pool_frames, 84, 84), "|u1", self),
+                                            device=self.device)
+                return
+            self.pool_bytes = int(pool_bytes)
             self.pool = torch.as_tensor(_CudaView(p.value, (self.pool_bytes,), "|u1", self), device=self.device)
+            check(self.lib.b2rl_dedup_coded_offsets(self._h, C.byref(p)))
+            self.offsets = torch.as_tensor(_CudaView(p.value, (self.pool_frames,), "<i8", self), device=self.device)
 
     def codec_stats(self) -> dict:
         """A coded pool's counters (b2rl_dedup_codec_stats): units_written (16-byte units, the wrap's skipped units
@@ -588,27 +639,35 @@ class DedupReplay(DeviceReplay):
         return h.value
 
     def push(self, fields: Sequence, priorities) -> None:
-        """fields: [state, next_state, action, reward, done] as for a DeviceReplay of APEX_FIELDS (host, pinned
-        preferred, or device).  The stacks are staged on the device (the same host->device bytes as a stack store),
-        then pushed in chunks of at most max_batch records; each chunk synchronizes the current stream once."""
-        s, ns = fields[0], fields[1]
+        """fields: rows of RECORD_FIELDS, as for a DeviceReplay of them (host, pinned preferred, or device): Ape-X's
+        [state, next_state, action, reward, done], R2D2's [state, ...] with `state` (n, T + 3, 84, 84) uint8 strips,
+        IMPALA's [state, ...].  The frames are staged on the device (the same host->device bytes as a store without a
+        frame pool), then pushed in chunks of at most max_batch records (b2rl_dedup_push, b2rl_dedup_push_strips);
+        each chunk synchronizes the current stream once."""
         pr = torch.as_tensor(priorities).to(torch.float32).contiguous()
         n = pr.numel()
-        small = _small_rows(APEX_FIELDS[2:], fields[2:], n)
-        stacks = []
-        for x in (s, ns):
+        framed = self._frame_fields
+        small = _small_rows(self.RECORD_FIELDS[len(framed):], fields[len(framed):], n)
+        frames = []
+        for f, x in zip(framed, fields):
             t = torch.as_tensor(x)
-            assert t.dtype == torch.uint8 and t.numel() == n * FRAME_STACK_BYTES, "frame stacks must be uint8 (n, 4, 84, 84)"
-            stacks.append(t.reshape(n, FRAME_STACK_BYTES).to(self.device, non_blocking=True).contiguous())
+            assert t.dtype == torch.uint8 and t.numel() == n * f.nbytes, \
+                f"{f.name} must be uint8 ({n}, {', '.join(map(str, f.shape))})"
+            frames.append(t.reshape(n, f.nbytes).to(self.device, non_blocking=True).contiguous())
+        push = self.lib.b2rl_dedup_push if len(frames) == 2 else self.lib.b2rl_dedup_push_strips
         ptrs = (C.c_void_p * _lib.MAX_FIELDS)()
         for a in range(0, n, self.max_batch):
             b = min(n, a + self.max_batch)
             ptrs[0] = None
             for i, t in enumerate(small):
                 ptrs[1 + i] = t[a:b].data_ptr()
-            check(self.lib.b2rl_dedup_push(self._h, stacks[0][a:b].data_ptr(), stacks[1][a:b].data_ptr(), ptrs,
-                                           pr[a:b].data_ptr(), b - a, self._st()))
-        self._inflight = stacks + small + [pr]
+            check(push(self._h, *[t[a:b].data_ptr() for t in frames], ptrs, pr[a:b].data_ptr(), b - a, self._st()))
+        self._inflight = frames + small + [pr]
+
+    @property
+    def _frame_fields(self) -> tuple:
+        """The leading RECORD_FIELDS, whose frames live in the pool: the slot holds `planes` in their place."""
+        return self.RECORD_FIELDS[:len(self.RECORD_FIELDS) + 1 - len(self.fields)]
 
     def push_begin(self, fields, n):
         raise ValueError("a frame-deduplicated replay (FRAME_DEDUP) has no pipelined ingest: use push")
@@ -623,18 +682,18 @@ class DedupReplay(DeviceReplay):
         return alloc_rows(self.RECORD_FIELDS, n, self.device, names)
 
     def gather(self, idx: torch.Tensor, out: dict | None = None) -> dict:
-        """The sampled slots' fields as a DeviceReplay of APEX_FIELDS returns them: state and next_state are (n, 4,
-        84, 84) stacks assembled from the pool (b2rl_replay_gather_planes)."""
+        """The sampled slots' fields as a DeviceReplay of RECORD_FIELDS returns them, the frame fields assembled from
+        the pool (b2rl_replay_gather_planes): Ape-X's (n, 4, 84, 84) state and next_state stacks, R2D2's (n, T + 3,
+        84, 84) strips, IMPALA's (n, T + 1, 28 224) stacks; a coded pool's frames decoded."""
         n = idx.numel()
         if out is None:
             out = self.alloc_batch(n)
-        stacks = (C.c_void_p * 2)(*[out[k].data_ptr() if out.get(k) is not None else None
-                                    for k in ("state", "next_state")])
+        frames = (C.c_void_p * 2)(*[_p(out.get(f.name)) for f in self._frame_fields])
         ptrs = (C.c_void_p * _lib.MAX_FIELDS)()
         for i, f in enumerate(self.fields):
             t = out.get(f.name) if i > 0 else None
             ptrs[i] = t.data_ptr() if t is not None else None
-        check(self.lib.b2rl_replay_gather_planes(self._h, idx.data_ptr(), n, stacks, ptrs, self._st()))
+        check(self.lib.b2rl_replay_gather_planes(self._h, idx.data_ptr(), n, frames, ptrs, self._st()))
         return out
 
     def frame_source(self, name: str) -> "PlaneFrames":
@@ -695,16 +754,8 @@ class CodedDedupReplay(DedupReplay):
 
     def __init__(self, capacity: int, pool_frames: int, window: int, pool_bytes: int, device="cuda:0",
                  hash_mask: int = DEDUP_HASH_MASK):
-        DeviceReplay.__init__(self, capacity, APEX_DEDUP_FIELDS, device)
-        self.coded = True
-        check(self.lib.b2rl_dedup_attach_coded(self._h, 0, int(pool_frames), int(window), int(hash_mask),
-                                               int(pool_bytes)))
-        self._attached(pool_frames, window)
-        self._coded_pool()
-        p = C.c_void_p()
-        check(self.lib.b2rl_dedup_coded_offsets(self._h, C.byref(p)))
-        with torch.cuda.device(self.device):     # the descriptor table: absolute unit offset of each pool entry
-            self.offsets = torch.as_tensor(_CudaView(p.value, (self.pool_frames,), "<i8", self), device=self.device)
+        self._attach(capacity, APEX_DEDUP_FIELDS, device, "b2rl_dedup_attach", (), pool_frames, window, hash_mask,
+                     pool_bytes=pool_bytes)
 
     def frame_source(self, name: str) -> "CodedPlaneFrames":
         return CodedPlaneFrames(self.pool, self.field_view("planes"), self.offsets, self.pool_frames,
@@ -731,73 +782,29 @@ class StripDedupReplay(DedupReplay):
                  pool_bytes: int | None = None):
         if host_pool and pool_bytes is not None:
             raise ValueError("a coded frame pool (pool_bytes) lives in HBM: it takes no host_pool")
-        DeviceReplay.__init__(self, capacity, R2D2_DEDUP_FIELDS(T, hidden), device)
         self.T = int(T)
         self.RECORD_FIELDS = r2d2_fields(self.T, hidden, strip=True)
-        self.host_pool = bool(host_pool)
-        self.coded = pool_bytes is not None
-        args = (self._h, 0, self.T + 3, int(pool_frames), int(window), int(hash_mask))
-        if self.host_pool:
-            with hostmem.on_gpu_node(self.device):   # pinned pages on the GPU's NUMA node (first touch: the library)
-                check(self.lib.b2rl_dedup_attach_strips_placed(*args, 1))
-        elif self.coded:
-            check(self.lib.b2rl_dedup_attach_strips_coded(*args, int(pool_bytes)))
-        else:
-            check(self.lib.b2rl_dedup_attach_strips(*args))
-        self._attached(pool_frames, window)
-        if self.coded:          # the encoded frames: a flat ring of 16-byte units, not (F, 84, 84) frames
-            self._coded_pool()
-
-    def push(self, fields: Sequence, priorities) -> None:
-        """fields: [state, action, reward, h0, h1, notdone] as for a DeviceReplay of r2d2_fields(T, strip=True),
-        `state` (n, T + 3, 84, 84) uint8 strips (host, pinned preferred, or device).  The strips are staged on the
-        device, then pushed in chunks of at most max_batch sequences; each chunk synchronizes the current stream
-        once."""
-        pr = torch.as_tensor(priorities).to(torch.float32).contiguous()
-        n = pr.numel()
-        small = _small_rows(self.RECORD_FIELDS[1:], fields[1:], n)
-        t = torch.as_tensor(fields[0])
-        row = self.RECORD_FIELDS[0].nbytes
-        assert t.dtype == torch.uint8 and t.numel() == n * row, \
-            f"frames must be uint8 ({n}, {', '.join(map(str, self.RECORD_FIELDS[0].shape))})"
-        strips = t.reshape(n, row).to(self.device, non_blocking=True).contiguous()
-        ptrs = (C.c_void_p * _lib.MAX_FIELDS)()
-        for a in range(0, n, self.max_batch):
-            b = min(n, a + self.max_batch)
-            ptrs[0] = None
-            for i, x in enumerate(small):
-                ptrs[1 + i] = x[a:b].data_ptr()
-            check(self.lib.b2rl_dedup_push_strips(self._h, strips[a:b].data_ptr(), ptrs, pr[a:b].data_ptr(), b - a,
-                                                  self._st()))
-        self._inflight = [strips] + small + [pr]
-
-    def gather(self, idx: torch.Tensor, out: dict | None = None) -> dict:
-        """The sampled slots' fields as a DeviceReplay of r2d2_fields(T, strip=True) returns them: `state` is the
-        (n, T + 3, 84, 84) strips assembled from the pool (b2rl_replay_gather_planes)."""
-        n = idx.numel()
-        if out is None:
-            out = self.alloc_batch(n)
-        st = out.get("state")
-        frames = (C.c_void_p * 2)(None if st is None else st.data_ptr(), None)
-        ptrs = (C.c_void_p * _lib.MAX_FIELDS)()
-        for i, f in enumerate(self.fields):
-            t = out.get(f.name) if i > 0 else None
-            ptrs[i] = t.data_ptr() if t is not None else None
-        check(self.lib.b2rl_replay_gather_planes(self._h, idx.data_ptr(), n, frames, ptrs, self._st()))
-        return out
+        self._attach(capacity, R2D2_DEDUP_FIELDS(T, hidden), device, "b2rl_dedup_attach_strips", (self.T + 3,),
+                     pool_frames, window, hash_mask, pool_bytes, host_pool)
 
     def frame_source(self, name: str) -> "PlaneFrames":
         """conv_1's rows of `state`: the windows of every slot's strip, row slot * (T + 3) + t being stack t of the
         slot (the row numbering of strip_windows over a strip store's state field)."""
-        if name != "state":
-            raise KeyError(name)
-        if self.host_pool:
-            raise ValueError("conv_1 reads its frame rows in place on the GPU: a frame pool in host memory (host_pool) "
-                             "has no frame source; gather the sampled strips into device memory first")
-        if self.coded:
-            raise ValueError("conv_1 reads raw frame rows: a coded frame pool (pool_bytes) holds encoded frames and "
-                             "has no frame source; gather (decode) the sampled strips into device memory first")
-        return PlaneFrames(self.pool, self.field_view("planes"), 0, 1)
+        return _pool_rows(self, name, 1, "gather (decode) the sampled strips")
+
+
+def _pool_rows(store, name: str, stride: int, read_first: str) -> "PlaneFrames":
+    """conv_1's rows of a strip or rollout store's `state`: its plane table at `stride` over the pool.  Refused for a
+    pool conv_1 cannot read in place, whose frames `read_first` brings into device memory instead."""
+    if name != "state":
+        raise KeyError(name)
+    if store.coded:
+        raise ValueError("conv_1 reads raw frame rows: a coded frame pool (pool_bytes) holds encoded frames and "
+                         f"has no frame source; {read_first} into device memory first")
+    if store.host_pool:
+        raise ValueError("conv_1 reads its frame rows in place on the GPU: a frame pool in host memory (host_pool) "
+                         "has no frame source; gather the sampled strips into device memory first")
+    return PlaneFrames(store.pool, store.field_view("planes"), 0, stride)
 
 
 class RolloutDedupReplay(StripDedupReplay):
@@ -816,29 +823,15 @@ class RolloutDedupReplay(StripDedupReplay):
 
     def __init__(self, capacity: int, pool_frames: int, window: int, T: int = 20, device="cuda:0",
                  hash_mask: int = DEDUP_HASH_MASK, pool_bytes: int | None = None):
-        DeviceReplay.__init__(self, capacity, IMPALA_DEDUP_FIELDS(T), device)
         self.T = int(T)
         self.RECORD_FIELDS = impala_fields(self.T)
-        self.host_pool = False
-        self.coded = pool_bytes is not None
-        args = (self._h, 0, self.T + 1, int(pool_frames), int(window), int(hash_mask))
-        if self.coded:
-            check(self.lib.b2rl_dedup_attach_rollouts_coded(*args, int(pool_bytes)))
-        else:
-            check(self.lib.b2rl_dedup_attach_rollouts(*args))
-        self._attached(pool_frames, window)
-        if self.coded:          # the encoded frames: a flat ring of 16-byte units, not (F, 84, 84) frames
-            self._coded_pool()
+        self._attach(capacity, IMPALA_DEDUP_FIELDS(T), device, "b2rl_dedup_attach_rollouts", (self.T + 1,),
+                     pool_frames, window, hash_mask, pool_bytes)
 
     def frame_source(self, name: str) -> "PlaneFrames":
         """conv_1's rows of `state`: every slot's stacks, row slot * (T + 1) + t being stack t of the slot (the row
         numbering of a stack store's state field viewed as (capacity * (T + 1), 4, 84, 84))."""
-        if name != "state":
-            raise KeyError(name)
-        if self.coded:
-            raise ValueError("conv_1 reads raw frame rows: a coded frame pool (pool_bytes) holds encoded frames and "
-                             "has no frame source; stage the drawn rollouts (stage_frames) into device memory first")
-        return PlaneFrames(self.pool, self.field_view("planes"), 0, 4)
+        return _pool_rows(self, name, 4, "stage the drawn rollouts (stage_frames)")
 
     def alloc_staged(self, n: int) -> dict:
         """stage_frames' buffers for n drawn rollouts, allocated once per learner: `pool` uint8 (n 4 (T + 1), 84, 84)
