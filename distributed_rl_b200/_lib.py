@@ -113,6 +113,9 @@ SIGNATURES = {
     "b2rl_dueling_backward": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b2rl_dueling_backward_w": (C.c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp]),
     "b2rl_launch_count": (c_i64, []),
+    "b2rl_wire_decode": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i32, c_vp, c_i32, c_vp, c_i32, c_vp,
+                                   C.POINTER(c_vp), C.POINTER(c_i64), c_i32, c_vp, c_i64, c_vp]),
+    "b2rl_wire_gather": (C.c_int, [C.POINTER(C.c_char_p), C.POINTER(c_i64), c_i64, c_vp, c_i64, c_vp]),
     "b2rl_serve_layout_init": (C.c_int, [c_i64, c_i32, c_i32, C.POINTER(c_i64), C.POINTER(ServeLayout)]),
     "b2rl_serve_ring_create": (C.c_int, [c_vp, c_i64, c_i32, C.POINTER(c_vp)]),
     "b2rl_serve_ring_layout": (C.c_int, [c_vp, C.POINTER(ServeLayout)]),

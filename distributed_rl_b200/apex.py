@@ -142,9 +142,16 @@ class Replay(ReplayThread):
     # -- ingest: records are [s, a, R_n, s', done, prio] pickled by the actors ----
     def push_records(self, blobs) -> None:
         """PER.push (baseline/PER.py:69-75) for a list of pickled actor records
-        (APE_X/Player.py:252-261): decoded once on the host, then one batched
-        H2D copy + fused leaf write / path refresh."""
+        (APE_X/Player.py:252-261): the raw blobs copied to the device once and decoded
+        there (wire.WireIngest), or decoded on the host when the batch must take that
+        path whole; then the store's push (leaf write / path refresh)."""
         if not blobs:
+            return
+        batch = self._wire_decode(blobs)
+        if batch is not None:        # decoded on the device (wire.WireIngest)
+            with self._lock:
+                self.store.push([batch[k] for k in ("s", "ns", "a", "r", "d")], batch["p"])
+            self.total_frame += len(blobs)
             return
         from .wire import decode_apex
         recs = [pickle.loads(b) for b in blobs]
@@ -155,6 +162,10 @@ class Replay(ReplayThread):
             self.store.push([st[k][:n] for k in ("s", "ns", "a", "r", "d")], st["p"][:n])
             st["event"].record(torch.cuda.current_stream(self.device))
         self.total_frame += n
+
+    def _wire_ingest(self):
+        from .wire import WireIngest
+        return WireIngest("apex", self.device)
 
     def _staging(self, n: int) -> dict:
         """One of two pinned staging sets (alternating), grown on demand; reused only after the copy that

@@ -131,9 +131,17 @@ class Replay(ReplayThread):
         (IMPALA/Player.py:183-190): FIFO ring, oldest rollouts overwritten beyond REPLAY_MEMORY_LEN."""
         if not blobs:
             return
+        batch = self._wire_decode(blobs)
+        if batch is not None:        # decoded on the device (wire.WireIngest)
+            self.push_arrays(*[batch[k] for k in ("state", "action", "mu", "reward", "done")])
+            return
         import pickle
         from .wire import decode_impala
         self.push_arrays(*decode_impala([pickle.loads(b) for b in blobs], self.cfg.UNROLL_STEP))
+
+    def _wire_ingest(self):
+        from .wire import WireIngest
+        return WireIngest("impala", self.device, T=self.cfg.UNROLL_STEP)
 
     def bufferSave(self, m: int = 1):
         """IMPALA/ReplayMemory.py:30-54 with random.sample's no-replacement semantics."""

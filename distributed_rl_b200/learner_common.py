@@ -97,6 +97,15 @@ class ReplayThread(Stoppable, threading.Thread):
             if not data:
                 time.sleep(0.002)
 
+    def _wire_decode(self, blobs):
+        """push_records' device path: the pickled records decoded on the GPU by the subclass's wire.WireIngest (made on
+        first use), or None for the host path: a replay not on a GPU, or a batch the device path hands back whole."""
+        if torch.device(self.cfg.LEARNER_DEVICE).type != "cuda":
+            return None
+        if self.__dict__.get("_wire") is None:
+            self._wire = self._wire_ingest()
+        return self._wire.decode(blobs)
+
     def _evict_on_request(self) -> None:
         """The `lock` handshake (APE_X/ReplayMemory.py:151-160, APE_X/Learner.py:189-197): once the memory is full,
         drop queued minibatches and trim to REPLAY_MEMORY_LEN (PER.remove_to_fit, baseline/PER.py:118-127).  The

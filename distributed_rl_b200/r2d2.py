@@ -168,14 +168,23 @@ class Replay(ReplayThread):
         self.total_frame += int(torch.as_tensor(p).numel())
 
     def push_records(self, blobs) -> None:
-        """PER.push for the actors' pickled sequences (R2D2/Player.py:312-319): decoded once on the host with
-        the indexing of R2D2/ReplayMemory.py:70-88, one batched H2D copy + leaf writes."""
+        """PER.push for the actors' pickled sequences (R2D2/Player.py:312-319) with the indexing of
+        R2D2/ReplayMemory.py:70-88: decoded on the device (wire.WireIngest), or on the host when the batch must take
+        that path whole (a sequence that does not slide into a strip raises ValueError naming it, nothing pushed)."""
         if not blobs:
+            return
+        batch = self._wire_decode(blobs)
+        if batch is not None:        # decoded on the device (wire.WireIngest), strips already encoded
+            self.push_arrays(*[batch[k] for k in ("state", "action", "reward", "h0", "h1", "notdone", "p")])
             return
         import pickle
         from .wire import decode_r2d2
         cols, p = decode_r2d2([pickle.loads(b) for b in blobs], self.cfg.FIXED_TRAJECTORY, strip=self.cfg.FRAME_STRIP)
         self.push_arrays(*cols, p)
+
+    def _wire_ingest(self):
+        from .wire import WireIngest
+        return WireIngest("r2d2", self.device, T=self.cfg.FIXED_TRAJECTORY, strip=self.cfg.FRAME_STRIP)
 
     def buffer(self, m: int = 1):
         B = self.cfg.BATCHSIZE

@@ -660,6 +660,27 @@ int b2rl_serve_bind(const void* slot_dev, const b2rl_serve_layout* layout, int64
 int b2rl_serve_put_update(b2rl_serve_ring* r, int32_t slot, uint64_t seq, const int64_t* idx_dev,
                           const float* prio_dev, int64_t n, void* stream);
 
+/* The actors' pickled records decoded on the device (DESIGN.md §4.24), in place of the learner's pickle.loads of each
+ * record (APE_X/ReplayMemory.py:74, R2D2/ReplayMemory.py:63) and the host decoders after it.  n records of one template are staged at
+ * `stride` bytes apart in blobs_dev (16-byte aligned; stride a multiple of 16 and at least tmpl_len + 16, the last
+ * 16 bytes readable), record r being lengths_dev[r] bytes long.  The template: its tmpl_len bytes at tmpl_dev and
+ * n_runs runs of 8 int32 at runs_dev ([op, src, len, field, dst, count, aux, kinds], wire.py), dealt to CTAs by the
+ * n_tasks [begin, end) run ranges at tasks_dev.  Record r compares its skeleton runs with the template's bytes and
+ * writes its values into row rows_dev[r] (r when rows_dev is NULL) of each field: fields_dev[f] (a host array of
+ * n_fields device pointers) with row_bytes[f] bytes per row.  status_dev (int32[n_rows], zeroed by the caller, so that
+ * several templates can decode into one batch) has ORed into the record's row 1 (skeleton mismatch, the length
+ * included), 2 (a value out of range of its field) or 4 (an R2D2 stack that is not the previous one shifted by one
+ * frame): it stays 0 for a record decoded.  A row whose status is not 0 holds undefined values.  One launch on
+ * `stream`; arguments are checked before it. */
+int b2rl_wire_decode(const uint8_t* blobs_dev, int64_t stride, const int32_t* lengths_dev, int64_t n,
+                     const uint8_t* tmpl_dev, int32_t tmpl_len, const int32_t* runs_dev, int32_t n_runs,
+                     const int32_t* tasks_dev, int32_t n_tasks, const int32_t* rows_dev, void* const* fields_dev,
+                     const int64_t* row_bytes, int32_t n_fields, int32_t* status_dev, int64_t n_rows, void* stream);
+/* Host side of the same ingest (APE_X/ReplayMemory.py:74, R2D2/ReplayMemory.py:63): blob i (src[i], lengths[i] <= stride bytes) -> dst + i * stride, and its length ->
+ * lengths_out[i] (int32).  A plain memcpy loop, so a caller through ctypes holds no interpreter lock meanwhile. */
+int b2rl_wire_gather(const void* const* src, const int64_t* lengths, int64_t n, uint8_t* dst, int64_t stride,
+                     int32_t* lengths_out);
+
 /* Number of kernels this library has launched in this process (bench.py's
  * `gpu_launches`). */
 int64_t b2rl_launch_count(void);
