@@ -27,7 +27,8 @@ __device__ __forceinline__ uint64_t load_le(const uint8_t* p, int n) {
 }
 
 // double -> float32 as the host's cast does: round to nearest even, and a NaN keeps its sign and the top of its
-// payload, quieted (cvt.rn.f32.f64 would return the canonical NaN).
+// payload, quieted.  The NaN case is spelled out rather than left to cvt.rn.f32.f64, although on an H100 that
+// instruction returned the same bits for 2^20 random NaN payloads (so __double2float_rn alone decodes the same there).
 __device__ __forceinline__ uint32_t f64_to_f32_bits(uint64_t b) {
   const double d = __longlong_as_double((long long)b);
   if (isnan(d)) return (uint32_t)(b >> 32 & 0x80000000u) | 0x7fc00000u | (uint32_t)(b >> 29 & 0x003fffffu);
@@ -70,7 +71,8 @@ __device__ __forceinline__ int convert(const uint8_t* p, int sk, uint8_t* q, int
       break;
     case D_F32:
     case D_F32_DIRECT:
-      if (sk == S_F32) out = (uint32_t)f;
+      // float(x) widens a float32 to double, which quiets a signalling NaN; numpy's float32 array cast keeps its bits
+      if (sk == S_F32) out = (uint32_t)f | (dk == D_F32 && (f & 0x7fffffffu) > 0x7f800000u ? 0x00400000u : 0u);
       else if (is_float) out = f64_to_f32_bits(f);
       else if (dk == D_F32) out = __float_as_uint(__double2float_rn(__ll2double_rn(i)));   // float(int), then float32
       else out = __float_as_uint(__ll2float_rn(i));                                        // numpy's int -> float32

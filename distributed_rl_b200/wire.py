@@ -150,8 +150,9 @@ S_U8, S_U16, S_I32, S_I64, S_F32, S_F64, S_F64BE, S_BOOLOP, S_B1 = range(9)
 SRC_BYTES = (1, 2, 4, 8, 4, 8, 8, 1, 1)
 SRC_FLOAT = (S_F32, S_F64, S_F64BE)
 D_I32, D_F32, D_F32_DIRECT, D_U8_BOOL, D_F32_NOT = range(5)
-# D_F32: float(x) then the float32 store (an int rounds to double first, as Python's float() does); D_F32_DIRECT: numpy's
-# int -> float32 array cast, one rounding.  D_U8_BOOL: bool(x).  D_F32_NOT: float(not x).
+# D_F32: float(x) then the float32 store (an int rounds to double first, as Python's float() does, and a float32 NaN is
+# quieted by the widening); D_F32_DIRECT: numpy's array cast to float32 (an int rounds once, a float32 keeps its bits).
+# D_U8_BOOL: bool(x).  D_F32_NOT: float(not x).
 STATUS_OK, STATUS_SKELETON, STATUS_RANGE, STATUS_NO_SLIDE = 0, 1, 2, 4
 TASK_BYTES = 32 << 10            # record bytes per CTA (runs are whole; a frame stack is never split)
 FRAME_BYTES, STACK_BYTES = 84 * 84, 4 * 84 * 84
@@ -366,8 +367,8 @@ class _Builder:
         kind = _DTYPE_KIND[dt]
         if to == D_I32:
             _need(kind not in SRC_FLOAT and kind != S_B1)
-        elif kind not in SRC_FLOAT:
-            to = D_F32_DIRECT
+        else:
+            to = D_F32_DIRECT            # np.asarray(x, np.float32) / astype: a float32 NaN keeps its bits
         self.run(RUN_CONVERT, data.off, data.n, field, 0, numel, 0, kind | to << 8)
 
     def frames(self, node, numel) -> int:
@@ -431,7 +432,7 @@ class _Builder:
         self.run(RUN_SAME, base + again_at, len(key), aux=base + key_at)
         at = keys[-1][2]
         _need(int.from_bytes(raw[at:at + 8], "little") == numel and len(raw) == at + 8 + 4 * numel)
-        self.run(RUN_CONVERT, base + at + 8, 4 * numel, field, 0, numel, 0, S_F32 | D_F32 << 8)
+        self.run(RUN_CONVERT, base + at + 8, 4 * numel, field, 0, numel, 0, S_F32 | D_F32_DIRECT << 8)
 
 
 class Template:

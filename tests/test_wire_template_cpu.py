@@ -20,7 +20,7 @@ def _apex(rng, i):
     return [s, a, r, ns, d, p]
 
 
-def _r2d2(rng, i, numpy_hidden=False, slide=True):
+def _r2d2(rng, i, numpy_hidden=False, slide=True, T=T):
     frames = rng.integers(0, 256, (T + 3, 84, 84), dtype=np.uint8)
     stacks = [frames[t:t + 4].copy() if slide else rng.integers(0, 256, (4, 84, 84), dtype=np.uint8) for t in range(T)]
     h = [rng.standard_normal((1, 1, 512)).astype(np.float32) for _ in range(2)]
@@ -35,7 +35,7 @@ def _r2d2(rng, i, numpy_hidden=False, slide=True):
     return np.append(arr, float(rng.random()) + 0.1)           # R2D2/Player.py:312-314
 
 
-def _impala(rng, i):
+def _impala(rng, i, T=T):
     return [rng.integers(0, 256, (T + 1, 28224), dtype=np.uint8), rng.integers(0, 6, (T, 1)),
             rng.uniform(0.05, 0.9, (T, 1)).astype(np.float32 if i % 2 else np.float64), rng.standard_normal(T),
             i % 2]
@@ -44,7 +44,7 @@ def _impala(rng, i):
 MAKE = {"apex": _apex, "r2d2": _r2d2, "impala": _impala}
 
 
-def _host(kind, blobs, strip=False):
+def _host(kind, blobs, strip=False, T=T):
     recs = [pickle.loads(b) for b in blobs]
     if kind == "apex":
         out = {name: np.zeros((len(recs),) + shape, dt) for name, dt, shape in W.record_fields("apex")}
@@ -80,8 +80,11 @@ def _convert(b: np.ndarray, sk: int, dk: int):
             return None, W.STATUS_RANGE
         return np.int32(int(v)).tobytes(), 0
     if dk in (W.D_F32, W.D_F32_DIRECT):
-        if sk == W.S_F32:
-            return b.tobytes(), 0
+        if sk == W.S_F32:                       # float() quiets a float32 NaN, numpy's array cast keeps its bits
+            bits = int(np.frombuffer(b.tobytes(), "<u4")[0])
+            if dk == W.D_F32 and np.isnan(v):
+                bits |= 0x400000
+            return np.uint32(bits).tobytes(), 0
         if is_float:
             return np.float64(v).astype(np.float32).tobytes(), 0
         if dk == W.D_F32:
@@ -189,8 +192,43 @@ def test_the_kernel_model_equals_the_host_decoders(kind, strip):
             np.testing.assert_array_equal(got[name].view(np.uint8), want[name][pos].view(np.uint8), err_msg=name)
 
 
+SNAN32 = np.array([0x7F800001, 0xFFA00000], np.uint32).view(np.float32)     # signalling NaNs, low / high payload
+
+
+def test_float32_nans_decode_like_the_host():
+    """Signalling float32 NaNs in scalar fields (float(x): quieted) and in arrays and LSTM states (the array cast: bits
+    kept), through the templates derive_template builds."""
+    rng = np.random.default_rng(8)
+    apex = _apex(rng, 1)
+    apex[2], apex[5] = SNAN32[0], SNAN32[1]
+    r2d2 = _r2d2(rng, 0)
+    h = rng.standard_normal((2, 1, 1, 512)).astype(np.float32)
+    h[:, 0, 0, 5:7] = SNAN32
+    r2d2[0] = (torch.from_numpy(h[0]), h[1])
+    r2d2[3], r2d2[-1] = SNAN32[1], SNAN32[0]
+    imp = _impala(rng, 1)
+    imp[2][1:3, 0] = SNAN32
+    imp[3] = imp[3].astype(np.float32)
+    imp[3][0], imp[4] = SNAN32[0], SNAN32[1]
+    for kind, rec in (("apex", apex), ("r2d2", r2d2), ("impala", imp)):
+        blob = pickle.dumps(rec, protocol=4)
+        got, status = model_decode(_template(kind, blob), [blob])
+        want = _host(kind, [blob])
+        assert status.tolist() == [0]
+        for name in want:
+            np.testing.assert_array_equal(got[name].view(np.uint8), want[name].view(np.uint8), err_msg=f"{kind} {name}")
+
+
 def test_float_conversions_round_like_numpy():
-    """fp64 -> fp32 rounds to nearest even, overflows to inf and keeps a NaN's payload top, as the host cast does."""
+    """fp64 -> fp32 rounds to nearest even, overflows to inf and keeps a NaN's payload top, as the host cast does; a
+    float32 scalar's signalling NaN is quieted, as float() quiets it, while a float32 array element keeps its bits."""
+    for bits in (0x7F800001, 0xFF800001, 0x7FA00000, 0xFFBFFFFF, 0x7FC00001, 0x00000001, 0x7F7FFFFF, 0xFF800000):
+        x = np.array([bits], np.uint32).view(np.float32)
+        src = np.frombuffer(x.tobytes(), np.uint8)
+        host = np.zeros(1, np.float32)
+        host[0] = float(x[0])                                       # decode_apex / decode_r2d2 / decode_impala scalars
+        assert _convert(src, W.S_F32, W.D_F32)[0] == host.tobytes(), hex(bits)
+        assert _convert(src, W.S_F32, W.D_F32_DIRECT)[0] == np.asarray(x, np.float32).tobytes(), hex(bits)
     vals = np.array([1 + 2 ** -24, 1 + 3 * 2 ** -24, 3.4e38, 1e300, -1e-50, np.nan, -np.inf, 16777217.0])
     vals = np.concatenate([vals, np.frombuffer(np.array([0x7FF0000000000123, 0xFFF8000012345678], np.uint64), np.float64)])
     for v in vals:
