@@ -8,11 +8,12 @@
 // registers); the dropped lo*lo term is 2^-22 relative.  SURVEY.md §8f rank 2 ("TF32x3 policy").
 //
 //   k_split_pack   fp32 matrix (optionally transposed) -> {hi, lo} operand images in exactly the
-//                  128B-swizzled, K-major tile layout the MMA reads, so the GEMM's loader is a
+//                  64B-swizzled, K-major tile layout the MMA reads, so the GEMM's loader is a
 //                  plain cp.async.bulk per tile (no tensor map, no SM-side staging)
-//   k_gemm_tf32x3  one CTA per (m-tile 128, n-tile 256, K-split): a TMA loader warp and two consumer
-//                  warpgroups (64 rows each, 12 x wgmma m64n256k8 per 32-float K chunk) that store the tile
-//                  (or, when K is split, this split's partial tile) straight from their accumulators
+//   k_gemm_tf32x3  one CTA per (m-tile 128, n-tile 256, K-split): a TMA loader warp that keeps four 16-float
+//                  half-chunk stages in flight, and two consumer warpgroups (64 rows each, 6 x wgmma m64n256k8
+//                  per half-chunk) that store the tile (or, when K is split, this split's partial tile) straight
+//                  from their accumulators
 //   k_splitk_reduce sums the K-split partials in split order: the result is deterministic (no atomics).
 //                  b2rl_gemm_tf32x3_partials leaves the partials in memory instead, for a consumer that sums them
 //                  in the same order while it reads its input (k_dueling_forward, k_unflatten_relu_mask)
@@ -25,16 +26,21 @@ namespace gemm {
 
 using namespace sm90;
 
-constexpr int TM = 128, TN = 256, KC = image::KC;   // tile rows of A / of B, floats per K chunk (128 B)
-constexpr int A_TILE = TM * 128, B_TILE = TN * 128;  // bytes of one {term, k-chunk} tile: 16 KiB / 32 KiB
-constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;       // hi+lo of both operands: 96 KiB
-constexpr int STAGES = 2;
+constexpr int TM = 128, TN = 256;                   // tile rows of A / of B
+constexpr int KC = image::KC, KH = image::KH;        // floats per K chunk (the split unit) / per staged half-chunk
+constexpr int A_TILE = TM * KH * 4, B_TILE = TN * KH * 4;   // bytes of one {term, k_half} tile: 8 KiB / 16 KiB
+constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;       // hi+lo of both operands: 48 KiB
+constexpr int STAGES = 4;                            // the loader runs up to three half-chunks ahead of the MMAs
+// wgmma groups (one per half-chunk) a warpgroup leaves in flight before it releases a stage: the stage of
+// half-chunk i - WG_DEPTH is refilled once half-chunk i's MMAs are issued
+constexpr int WG_DEPTH = 1;
+static_assert(WG_DEPTH >= 0 && WG_DEPTH < STAGES, "a released stage must not be one the MMAs still read");
 constexpr int CONSUMERS = 256;                       // warpgroups 0-1: MMA + epilogue
 constexpr int THREADS = CONSUMERS + 32;              // warp 8: TMA loader
 
 // ---- operand packing ---------------------------------------------------------
 // Image layout: operand_image.cuh.  One CTA per (32 operand rows, one K chunk); thread = (row r = tid / 8, 16-byte unit = tid % 8), so
-// both the source row segment and the image row are one contiguous 128 B per 8 threads.
+// the source row segment is one contiguous 128 B per 8 threads, and each image row half one contiguous 64 B per 4.
 // TRANSPOSE: the operand's rows are the source's columns; the 32x32 block goes through SMEM so that
 // the source is still read along its contiguous dimension.
 template <bool TRANSPOSE>
@@ -70,7 +76,8 @@ k_split_pack(const float* __restrict__ src, int src_rows, int src_cols, int64_t 
   }
   const int irow = row_off + row, ikc = kc_off + kc;
   if (irow >= rows_pad) return;
-  image::store_unit(out, image::offset(irow, ikc, unit, tile_rows, rows_pad), image::term_stride(k_chunks, rows_pad), v);
+  image::store_unit(out, image::offset(irow, ikc * KC + unit * 4, tile_rows, rows_pad), image::term_stride(k_chunks, rows_pad),
+                    v);
 }
 
 // ---- activation-side packs that fold act_3 (ReLU) + nn.Flatten into the heads' operand images ----------------
@@ -116,7 +123,7 @@ k_pack_act_nhwc(const float* __restrict__ y, int B, int HW, int C, int relu, flo
         v[e] = (b < B && f0 + e < K) ? s_act[hw * ld + c] : 0.0f;
         if (++hw == HW) { hw = 0; ++c; }
       }
-      image::store_unit(out, image::offset(b, kc, unit, TM, rows_pad), ts, v);
+      image::store_unit(out, image::offset(b, f0, TM, rows_pad), ts, v);
     }
   } else {
     // one CTA per (chunk of 32 b's, hw): s[b][c], row stride C + 1; image rows f = c*HW + hw, contraction = b
@@ -135,7 +142,7 @@ k_pack_act_nhwc(const float* __restrict__ y, int B, int HW, int C, int relu, flo
       float v[4];
 #pragma unroll
       for (int e = 0; e < 4; ++e) v[e] = s_act[(unit * 4 + e) * ld + c];
-      image::store_unit(out, image::offset(c * HW + hw, kc, unit, TN, rows_pad), ts, v);
+      image::store_unit(out, image::offset(c * HW + hw, kc * KC + unit * 4, TN, rows_pad), ts, v);
     }
   }
 }
@@ -151,7 +158,7 @@ k_pack_zero_rows(float* __restrict__ out, int row0, int rows_pad, int k_chunks, 
     const int unit = (int)(w & 7);
     const int64_t q = w >> 3;
     const int kc = (int)(q / n_rows), f = row0 + (int)(q - (int64_t)kc * n_rows);
-    image::store_unit(out, image::offset(f, kc, unit, tile_rows, rows_pad), ts, zero);
+    image::store_unit(out, image::offset(f, kc * KC + unit * 4, tile_rows, rows_pad), ts, zero);
   }
 }
 
@@ -193,11 +200,11 @@ k_gemm_tf32x3(const __grid_constant__ Params P) {
   __shared__ __align__(8) uint64_t full[STAGES], empty[STAGES];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t mt = blockIdx.x, nt = blockIdx.y;
-  // K range of this split
+  // K range of this split, in 32-float chunks; staged and multiplied as 2 (k1 - k0) half-chunks from 2 k0 on
   const int64_t per = (P.k_chunks + P.splits - 1) / P.splits;
   const int64_t k0 = (int64_t)blockIdx.z * per;
   const int64_t k1 = (k0 + per < P.k_chunks) ? k0 + per : P.k_chunks;
-  const int64_t nk = k1 - k0;   // > 0: the host never launches an empty trailing split (gemm_splits)
+  const int64_t nk = 2 * (k1 - k0);   // > 0: the host never launches an empty trailing split (gemm_splits)
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], CONSUMERS); }
@@ -209,14 +216,14 @@ k_gemm_tf32x3(const __grid_constant__ Params P) {
   if (warp == CONSUMERS / 32) {
     // ------------------------------ TMA loader ------------------------------
     if (lane == 0) {
-      const int64_t a_term = P.k_chunks * P.m_tiles * (TM * 32);   // floats between the hi and lo images
-      const int64_t b_term = P.k_chunks * P.n_tiles * (TN * 32);
+      const int64_t a_term = P.k_chunks * P.m_tiles * (TM * KC);   // floats between the hi and lo images
+      const int64_t b_term = P.k_chunks * P.n_tiles * (TN * KC);
       for (int64_t i = 0; i < nk; ++i) {
         const int s = (int)(i % STAGES);
         mbar_wait(&empty[s], ((i / STAGES) & 1) ^ 1);
-        const int64_t kc = k0 + i;
-        const float* a_hi = P.a + (kc * P.m_tiles + mt) * (TM * 32);
-        const float* b_hi = P.b + (kc * P.n_tiles + nt) * (TN * 32);
+        const int64_t kh = 2 * k0 + i;
+        const float* a_hi = P.a + (kh * P.m_tiles + mt) * (TM * KH);
+        const float* b_hi = P.b + (kh * P.n_tiles + nt) * (TN * KH);
         uint8_t* st = smem + (size_t)s * STAGE;
         mbar_expect_tx(&full[s], STAGE);
         bulk_g2s(st, a_hi, A_TILE, &full[s]);
@@ -231,23 +238,24 @@ k_gemm_tf32x3(const __grid_constant__ Params P) {
   // ------------------------- consumers: wgmma + epilogue -------------------------
   const int wg = warp >> 2;                            // rows [64 wg, 64 wg + 64) of the tile
   float acc[128];
+#pragma unroll 1       // unrolled, the remainder path makes ptxas serialize the wgmmas (C7520)
   for (int64_t i = 0; i < nk; ++i) {
     const int s = (int)(i % STAGES);
     mbar_wait(&full[s], (i / STAGES) & 1);
     const uint32_t base = sptr(smem + (size_t)s * STAGE);
-    const uint32_t a_hi = base + wg * (64 * 128), a_lo = a_hi + A_TILE, b_hi = base + 2 * A_TILE, b_lo = b_hi + B_TILE;
+    const uint32_t a_hi = base + wg * (64 * KH * 4), a_lo = a_hi + A_TILE, b_hi = base + 2 * A_TILE, b_lo = b_hi + B_TILE;
     wg_fence();
 #pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
+    for (int ks = 0; ks < KH / 8; ++ks) {
       const uint32_t o = ks * 32;
-      mma_tf32_n256(acc, make_desc(a_lo + o), make_desc(b_hi + o), (i | ks) ? 1u : 0u);   // small terms first
-      mma_tf32_n256(acc, make_desc(a_hi + o), make_desc(b_lo + o), 1u);
-      mma_tf32_n256(acc, make_desc(a_hi + o), make_desc(b_hi + o), 1u);
+      mma_tf32_n256(acc, make_desc_sw64(a_lo + o), make_desc_sw64(b_hi + o), (i | ks) ? 1u : 0u);   // small terms first
+      mma_tf32_n256(acc, make_desc_sw64(a_hi + o), make_desc_sw64(b_lo + o), 1u);
+      mma_tf32_n256(acc, make_desc_sw64(a_hi + o), make_desc_sw64(b_hi + o), 1u);
     }
     wg_commit();
-    wg_wait<1>();                                      // the MMAs of chunk i - 1 are done: its stage may be refilled
+    wg_wait<WG_DEPTH>();                               // the MMAs of half-chunk i - WG_DEPTH are done: refill its stage
     wg_fence_regs(acc);
-    if (i > 0) mbar_arrive(&empty[(i - 1) % STAGES]);
+    if (i >= WG_DEPTH) mbar_arrive(&empty[(i - WG_DEPTH) % STAGES]);
   }
   wg_wait<0>();
   wg_fence_regs(acc);

@@ -58,6 +58,12 @@ __device__ __forceinline__ void named_sync(int id, int threads) {
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
   return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
+// The same for SWIZZLE_64B (layout 2): 8-row x 64-byte atoms, 512-byte aligned, 512 B between 8-row groups, the
+// 16-byte units of row r XOR-ed by ((r >> 1) & 3) (the PTX ISA's canonical K-major 64B-swizzle layout); a K step
+// inside the 64-byte row advances the start address by its byte width.
+__device__ __forceinline__ uint64_t make_desc_sw64(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (2ull << 62);
+}
 
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

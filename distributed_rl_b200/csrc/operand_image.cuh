@@ -2,15 +2,19 @@
 // image (the packs in gemm.cu, the fused optimizer in optim.cu that keeps the dense heads' weight images current)
 // must produce bit for bit.
 //
-// Layout: [term 0=hi,1=lo][k_chunk][row_tile][row_in_tile][128 B, 16-byte units XOR (row & 7)]
-// tile_rows is 128 for the A (M) side and 256 for the B (N) side; a k_chunk is 32 floats of the contraction.
+// Layout: [term 0=hi,1=lo][k_half][row_tile][row_in_tile][64 B, 16-byte units XOR ((row >> 1) & 3)]
+// tile_rows is 128 for the A (M) side and 256 for the B (N) side; a k_half is 16 floats of the contraction, so one
+// {term, k_half, row_tile} tile is a whole SWIZZLE_64B K-major operand (8-row x 64-byte atoms, 512 B apart) and the
+// GEMM's loader stages it with one bulk copy.  The contraction is padded to a multiple of KC = 32 floats (two
+// halves), which is the unit the GEMM splits K by.
 #pragma once
 #include <cstdint>
 
 namespace b2rl {
 namespace image {
 
-constexpr int KC = 32;                          // floats per K chunk (128 B)
+constexpr int KC = 32;                          // contraction padding and K-split unit (floats)
+constexpr int KH = 16;                          // floats of one k_half (64 B rows)
 
 // x = hi + lo, hi = rn_tf32(x), lo = x - hi (exact in fp32)
 __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
@@ -27,10 +31,11 @@ __host__ __device__ __forceinline__ int64_t term_stride(int k_chunks, int rows_p
   return (int64_t)k_chunks * rows_pad * KC;
 }
 
-// float offset of 16-byte unit `unit` (contraction elements 4 unit .. 4 unit + 3 of chunk kc) of image row `row`
-__device__ __forceinline__ int64_t offset(int row, int kc, int unit, int tile_rows, int rows_pad) {
+// float offset of the 16-byte unit holding contraction elements k .. k + 3 (k a multiple of 4) of image row `row`
+__device__ __forceinline__ int64_t offset(int row, int k, int tile_rows, int rows_pad) {
   const int rt = row / tile_rows, rr = row - rt * tile_rows;
-  return (((int64_t)kc * (rows_pad / tile_rows) + rt) * tile_rows + rr) * KC + ((unit ^ (rr & 7)) << 2);
+  const int kh = k / KH, unit = (k / 4) & 3;
+  return (((int64_t)kh * (rows_pad / tile_rows) + rt) * tile_rows + rr) * KH + ((unit ^ ((rr >> 1) & 3)) << 2);
 }
 
 // split v[0..3] and store the {hi, lo} units at `off` of an image with term stride `ts`

@@ -88,12 +88,12 @@ k_rmsprop(const __grid_constant__ OptTable T, float lr, float alpha, float one_m
     *reinterpret_cast<float4*>(SQ + i0) = sq4;
     if (centered) *reinterpret_cast<float4*>(GA + i0) = ga4;
     *reinterpret_cast<float4*>(G + i0) = make_float4(0.f, 0.f, 0.f, 0.f);               // zero_grad
-    if (T.img_fwd[t]) {          // image row = the weight's row n_off + rt*32 + r, chunk kc (k_split_pack<false>)
+    if (T.img_fwd[t]) {          // image row = the weight's row n_off + rt*32 + r, contraction = its columns (k_split_pack<false>)
       const int rows_pad = T.fwd_rows_pad[t];
-      image::store_unit(T.img_fwd[t], image::offset(T.n_off[t] + rt * 32 + r, kc, unit, 256, rows_pad),
+      image::store_unit(T.img_fwd[t], image::offset(T.n_off[t] + rt * 32 + r, kc * image::KC + unit * 4, 256, rows_pad),
                         image::term_stride(T.fwd_kc[t], rows_pad), pv);
     }
-    if (T.img_wt[t]) {           // transposed through SMEM: image row = column kc*32 + r (k_split_pack<true>)
+    if (T.img_wt[t]) {           // transposed through SMEM: image row = column kc*32 + r, contraction = stack rows (k_split_pack<true>)
 #pragma unroll
       for (int e = 0; e < 4; ++e) tile[r][unit * 4 + e] = pv[e];
       __syncthreads();
@@ -101,7 +101,7 @@ k_rmsprop(const __grid_constant__ OptTable T, float lr, float alpha, float one_m
 #pragma unroll
       for (int e = 0; e < 4; ++e) v[e] = tile[unit * 4 + e][r];
       const int rows_pad = T.wt_rows_pad[t];
-      image::store_unit(T.img_wt[t], image::offset(kc * image::KC + r, T.n_off[t] / image::KC + rt, unit, 256, rows_pad),
+      image::store_unit(T.img_wt[t], image::offset(kc * image::KC + r, T.n_off[t] + rt * 32 + unit * 4, 256, rows_pad),
                         image::term_stride(T.wt_kc[t], rows_pad), v);
     }
   } else {
