@@ -218,7 +218,10 @@ def split_pack(x: torch.Tensor, transpose: bool, b_role: bool) -> torch.Tensor:
     rows, k = (x.shape[1], x.shape[0]) if transpose else (x.shape[0], x.shape[1])
     n = _lib.load().b2rl_gemm_packed_floats(rows, k, int(b_role))
     out = torch.empty(n, dtype=torch.float32, device=x.device)
-    _lib.check(_lib.load().b2rl_gemm_split_pack(x.data_ptr(), x.shape[0], x.shape[1], x.stride(0), int(transpose),
+    # a one-row matrix may carry any row stride (the transpose of an [n][1] column has stride 1): its rows are never
+    # stepped, so give the pack the row length as the leading dimension
+    ld = x.stride(0) if x.shape[0] > 1 else x.shape[1]
+    _lib.check(_lib.load().b2rl_gemm_split_pack(x.data_ptr(), x.shape[0], x.shape[1], ld, int(transpose),
                                                int(b_role), out.data_ptr(), _stream()))
     return out
 
