@@ -15,7 +15,7 @@ namespace b2rl {
 
 constexpr int HOST_ROWS_THREADS = 256;
 constexpr int HOST_ROWS_UNROLL = 8;       // 16-byte loads in flight per thread
-constexpr int HOST_GATHER_CTAS = 8;       // the fewest at the plateau of tools/bench_host_frames.py's sweep (§4.17)
+constexpr int HOST_GATHER_CTAS = 8;       // the fewest at the plateau of the B2RL_HOST_GATHER_CTAS sweep (§4.17)
 
 // dst[k] = src row clamp_row(idx[k]) for k < n, rows of row_vecs 16-byte units; the n * row_vecs units are dealt out
 // grid-stride, so consecutive threads read consecutive units of a row.
