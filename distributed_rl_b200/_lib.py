@@ -77,6 +77,10 @@ SIGNATURES = {
     "b2rl_conv1_fused": (C.c_int, [C.POINTER(Frames), c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_vp, c_i32, c_vp]),
     "b2rl_conv1_wgrad_workspace_floats": (c_i64, [c_i32]),
     "b2rl_conv1_wgrad": (C.c_int, [C.POINTER(Frames), c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp]),
+    "b2rl_stem_pack": (C.c_int, [c_vp, c_vp, c_vp, c_vp]),
+    "b2rl_stem_fused": (C.c_int, [C.POINTER(Frames), c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b2rl_stem_wgrad_workspace_doubles": (c_i64, []),
+    "b2rl_stem_wgrad": (C.c_int, [C.POINTER(Frames), c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp]),
     "b2rl_dedup_attach": (C.c_int, [c_vp, c_i32, c_i64, c_i64, c_u64]),
     "b2rl_dedup_push": (C.c_int, [c_vp, c_vp, c_vp, C.POINTER(c_vp), c_vp, c_i64, c_vp]),
     "b2rl_dedup_attach_strips": (C.c_int, [c_vp, c_i32, c_i32, c_i64, c_i64, c_u64]),

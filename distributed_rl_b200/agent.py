@@ -9,7 +9,8 @@ much smaller interpreter for the node types the three shipped configs use
 
     CNN2D  MLP  LSTMNET  ViewV2  Add  Mean  Substract
 
-with the same call surface the learners rely on: forward([inputs]) -> tuple,
+and RESCNN2D, the IMPALA paper's residual network (impala.resnet_small_model; no shipped config uses it), with the
+same call surface the learners rely on: forward([inputs]) -> tuple,
 getParameters, updateParameter(other, tau), setCellState / detachCellState /
 zeroCellState, calculateNorm, clippingNorm, and state_dict() key names
 (`module00.conv_1.weight`, `module02.MLP_1.weight`, `module02.rnn.weight_ih_l0`,
@@ -132,6 +133,59 @@ class ConvStack(nn.Sequential):
                 and isinstance(layers[-1], nn.Flatten))
 
 
+class ResidualBlock(nn.Module):
+    """x + conv_2(relu(conv_1(relu(x)))), both convs 3x3 / stride 1 / pad 1, bias-free."""
+
+    def __init__(self, ch):
+        super().__init__()
+        self.act_1 = nn.ReLU()
+        self.conv_1 = nn.Conv2d(ch, ch, 3, stride=1, padding=1, bias=False)
+        self.act_2 = nn.ReLU()
+        self.conv_2 = nn.Conv2d(ch, ch, 3, stride=1, padding=1, bias=False)
+
+    def forward(self, x):
+        return x + self.conv_2(self.act_2(self.conv_1(self.act_1(x))))
+
+
+class ResidualStack(nn.Sequential):
+    """netCat RESCNN2D: the IMPALA paper's "large" network without its LSTM (Espeholt et al. 2018, Fig. 3).  Section
+    i = 1..len(nUnit) is conv_i (3x3, stride 1, pad 1), pool_i (3x3 max-pool, stride 2, pad 1) and blockNum residual
+    blocks block_i_j; then a ReLU and, with `linear`, a Flatten.  Every conv is bias-free.  84x84 frames give 42, 21
+    and 11: 32 * 11 * 11 = 3 872 features at nUnit [16, 32, 32].  The first conv and pool are the stem libb2rl runs
+    fused with the frame gather (csrc/stem.cu)."""
+
+    def __init__(self, d):
+        super().__init__()
+        ch = d["iSize"]
+        for i, c in enumerate(d["nUnit"], 1):
+            self.add_module(f"conv_{i}", nn.Conv2d(ch, c, 3, stride=1, padding=1, bias=False))
+            self.add_module(f"pool_{i}", nn.MaxPool2d(3, stride=2, padding=1))
+            for j in range(1, d["blockNum"] + 1):
+                self.add_module(f"block_{i}_{j}", ResidualBlock(c))
+            ch = c
+        self.add_module("act", nn.ReLU())
+        if d.get("linear", True):
+            self.add_module("Flatten", nn.Flatten())
+
+    def forward(self, xs):
+        x = xs[0] if isinstance(xs, (tuple, list)) else xs
+        for layer in self:
+            x = layer(x)
+        return x
+
+    def is_fused_stem(self) -> bool:
+        """True if the stem is the 3x3 / stride-1 / pad-1, 4 -> 16 channel conv that libb2rl's stem kernels run."""
+        c = self.conv_1
+        return (c.in_channels, c.out_channels, c.kernel_size, c.stride, c.padding) == (4, 16, (3, 3), (1, 1), (1, 1))
+
+    def forward_tail(self, p):
+        """Continue after the stem: `p` is pool_1's output."""
+        x = p
+        for layer in list(self.children())[2:]:
+            x = layer(x)
+        return x
+
+
 class DenseStack(nn.Sequential):
     """netCat MLP: Linear layers (bias off unless cfg says so) with activations."""
 
@@ -241,7 +295,7 @@ def _refresh_after_load(module, incompatible_keys):
     module.refresh_resident_heads()
 
 
-_NODE = {"CNN2D": ConvStack, "MLP": DenseStack, "LSTMNET": Recurrent,
+_NODE = {"CNN2D": ConvStack, "RESCNN2D": ResidualStack, "MLP": DenseStack, "LSTMNET": Recurrent,
          "ViewV2": lambda d: ViewAs(), "Add": lambda d: _Add(), "Substract": lambda d: _Sub(),
          "Mean": lambda d: _Mean()}
 
@@ -472,6 +526,20 @@ class GraphAgent(nn.Module):
             if isinstance(m, ConvStack) and self._ext[name] == [0] and not self._prev[name]:
                 return name if m.is_atari_conv1() else None
         return None
+
+    def first_stem_node(self):
+        """Name of the RESCNN2D node fed by external input 0, if its stem is the one libb2rl's stem kernels run
+        (the parallel of first_conv_node for the residual network)."""
+        for name in self._order:
+            m = getattr(self, name)
+            if isinstance(m, ResidualStack) and self._ext[name] == [0] and not self._prev[name]:
+                return name if m.is_fused_stem() else None
+        return None
+
+    def forward_from_stem(self, p, extra_inputs=()):
+        """Forward pass given the stem's pooled output of the first RESCNN2D node (fused gather + stem kernel)."""
+        name = self.first_stem_node()
+        return self.forward([None, *extra_inputs], preset={name: getattr(self, name).forward_tail(p)})
 
     def forward_from_conv1(self, y, relu_applied: bool, extra_inputs=()):
         """Forward pass given conv_1's output of the first CNN2D node (fused gather+conv1 kernel)."""

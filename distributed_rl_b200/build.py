@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb2rl.so")
 STAMP = LIB + ".stamp"     # the nvcc flags the library was built with: a change of target or flags forces a rebuild
 SOURCES = ["capi.cu", "tree.cu", "gather.cu", "targets.cu", "conv1.cu", "conv1_wgrad.cu", "optim.cu", "gemm.cu", "dueling.cu", "peer.cu", "serve.cu",
-           "uniform.cu", "dedup.cu", "hostrows.cu", "wire.cu"]
+           "uniform.cu", "dedup.cu", "hostrows.cu", "wire.cu", "stem.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

@@ -12,8 +12,8 @@ import torch
 
 from . import replay as R
 from .agent import GraphAgent
-from .learner_common import (CapturedStep, Conv1Gathered, ReplayThread, _attach_replay, check_served_fused,
-                             conv1_packs, make_optimizer, publishers, time_major_rows)
+from .learner_common import (CapturedStep, Conv1Gathered, ReplayThread, StemGathered, _attach_replay,
+                             check_served_fused, conv1_packs, make_optimizer, publishers, time_major_rows)
 from .publish import ParamPublisher
 
 
@@ -24,6 +24,19 @@ def default_impala_model() -> dict:
                      "padding": [0, 0], "stride": [4, 2], "act": ["relu", "relu"], "BN": [False] * 3,
                      "linear": True, "input": [0], "prior": 0},
         "module01": {"netCat": "MLP", "iSize": 2592, "nLayer": 2, "fSize": [256, 7], "act": ["relu", "linear"],
+                     "BN": [False, False], "prior": 1, "prevNodeNames": ["module00"], "output": True},
+    }
+
+
+def resnet_small_model() -> dict:
+    """The IMPALA paper's residual network (Espeholt et al. 2018, Fig. 3, without the LSTM) in the same graph form:
+    a RESCNN2D node (three sections of conv, max-pool and two residual blocks at 16, 32, 32 channels; 84 -> 42 -> 21
+    -> 11) and the MLP head 3 872 -> 256 (ReLU) -> 7.  1 090 368 parameters.  ImpalaConfig(MODEL=resnet_small_model())
+    trains it; with FUSED_CONV1 its stem (first conv + max-pool) reads the frames in place (csrc/stem.cu)."""
+    return {
+        "module00": {"netCat": "RESCNN2D", "iSize": 4, "nUnit": [16, 32, 32], "blockNum": 2, "linear": True,
+                     "input": [0], "prior": 0},
+        "module01": {"netCat": "MLP", "iSize": 3872, "nLayer": 2, "fSize": [256, 7], "act": ["relu", "linear"],
                      "BN": [False, False], "prior": 1, "prevNodeNames": ["module00"], "output": True},
     }
 
@@ -45,8 +58,10 @@ class ImpalaConfig:
     LOG_W: str | None = None
     OPTIM_INFO: dict = field(default_factory=lambda: {"name": "rmsprop", "lr": 6e-4, "decay": 0})
     MODEL: dict = field(default_factory=default_impala_model)
-    FUSED_CONV1: bool = True     # conv_1 (4 -> 16 channels) of every frame through libb2rl's wgmma kernel
-    DENSE_3XTF32: bool = True    # the 2592 -> 256 layer as a 3xTF32 wgmma GEMM (csrc/gemm.cu) instead of an fp32 SIMT sgemm
+    FUSED_CONV1: bool = True     # conv_1 (4 -> 16 channels) of every frame through libb2rl's wgmma kernel; with a
+                                 # RESCNN2D model (resnet_small_model), its stem through libb2rl's stem kernels
+    DENSE_3XTF32: bool = True    # the head's first layer (2592 -> 256; 3872 -> 256 for resnet_small_model) as a 3xTF32
+                                 # wgmma GEMM (csrc/gemm.cu) instead of an fp32 SIMT sgemm
     SERVED_FUSED_STEP: bool = False  # on a served replay (DeviceReplayClient), run() steps a captured step on the
                                      # bound ring slot instead of sample() -> train()
     FRAME_DEDUP: bool = False    # store every distinct frame once, in a pool of FRAMES_PER_ROLLOUT frames per slot
@@ -215,7 +230,7 @@ class Learner(CapturedStep):
         T, B = c.UNROLL_STEP, c.BATCHSIZE
         dev = self.device
         state, action, mu, reward, done = [torch.as_tensor(x).to(dev) for x in transition]
-        fused = c.FUSED_CONV1 and state.dtype == torch.uint8 and self.model.first_conv_node() is not None
+        fused = c.FUSED_CONV1 and state.dtype == torch.uint8 and _fused_first_layer(self.model)
         if fused:   # the staged batch is the frame table: rows already are time-major
             frames = state.contiguous().view((T + 1) * B, 4, 84, 84)
             self._train_core(frames, None, action, mu, reward, done, step)
@@ -333,15 +348,27 @@ class Learner(CapturedStep):
 
     def _train_core(self, frames, rows, action, mu, reward, done, step, seq_frames=None):
         """IMPALA/Learner.py:121-235 on a uint8 frame table read in place (`rows`: time-major frame rows, None =
-        all rows in order) or, with rows == "staged", on a staged (T+1, B, 28224) batch through PyTorch's conv_1.
+        all rows in order) or, with rows == "staged", on a staged (T+1, B, 28224) batch through PyTorch's first layer.
+        The model's first layer is conv_1 or, for a RESCNN2D model, the residual network's stem (R.stem_fused).
         `seq_frames`: with rows None and `frames` a bound ring slot (R.BoundFrames), the same slot's first T * B
         rows, which the grad pass reads (a BoundFrames cannot be sliced)."""
         c = self.cfg
         T, B, A = c.UNROLL_STEP, c.BATCHSIZE, c.ACTION_SIZE
         dev = self.device
         fused = not isinstance(rows, str)
+        stem = fused and self.model.first_stem_node() is not None
         with torch.no_grad():
-            if fused:
+            if stem:
+                # one launch: the residual network's stem (conv + max-pool) of all (T+1)*B frame stacks
+                if not hasattr(self, "_stem_pack"):
+                    self._stem_pack = R.StemPack(dev)
+                w1 = getattr(self.model, self.model.first_stem_node()).conv_1.weight
+                self._stem_pack.pack(w1)
+                p_all, a_all = R.stem_fused(frames, rows, self._stem_pack)
+                p_seq, a_seq = p_all[:T * B], a_all[:T * B]
+                out_last = self.model.forward_from_stem(p_all[T * B:])[0]
+                out_seq = self.model.forward_from_stem(p_seq)[0]
+            elif fused:
                 # one launch: conv_1 of all (T+1)*B frame stacks, uint8 -> /255 folded in, no fp32 staging
                 if not hasattr(self, "_pack1"):
                     self._conv_name, self._pack1 = conv1_packs(self.model, dev, 1)
@@ -363,11 +390,15 @@ class Learner(CapturedStep):
             vt, adv = R.vtrace(pi_a.view(T, B).contiguous(), mu.float().view(T, B).contiguous(),
                                value.view(T, B).contiguous(), boot, reward.float().view(T, B).contiguous(),
                                c.GAMMA, c.C_LAMBDA, c.C_VALUE, c.P_VALUE)       # :151-215 in one launch
-        # calLoss (:95-119): second forward with grad (conv_1's output is reused: same weights, same frames)
+        # calLoss (:95-119): second forward with grad (conv_1's or the stem's output is reused: same weights, same frames)
         if fused:
             if seq_frames is None:
                 seq_frames = frames[:T * B] if rows is None else frames
             seq_rows = None if rows is None else rows[:T * B]
+        if stem:
+            pooled = StemGathered.apply(w1, seq_frames, seq_rows, p_seq, a_seq)
+            out = self.model.forward_from_stem(pooled)[0]
+        elif fused:
             y = Conv1Gathered.apply(w1, seq_frames, seq_rows, self._pack1, torch.contiguous_format, None, y_seq)
             out = self.model.forward_from_conv1(y, False)[0]
         else:
@@ -444,9 +475,9 @@ class _BoundRollouts:
     def __init__(self, L: "Learner"):
         c, dev = L.cfg, L.device
         T, B = c.UNROLL_STEP, c.BATCHSIZE
-        if L.model.first_conv_node() is None:
-            raise ValueError("SERVED_FUSED_STEP reads the ring slot's frames with the fused conv_1 kernels: the "
-                             "model's first node must be the Atari conv_1")
+        if not _fused_first_layer(L.model):
+            raise ValueError("SERVED_FUSED_STEP reads the ring slot's frames with the fused conv_1 or stem kernels: "
+                             "the model's first node must be the Atari conv_1 or a RESCNN2D stem")
         self.stream = torch.cuda.Stream(dev)
         self.cur = _rollout_buffers(T, B, dev)
         self.cur.update(w=torch.empty(B, dtype=torch.float32, device=dev),
@@ -467,9 +498,9 @@ class _DrawnRollouts:
     def __init__(self, L: "Learner"):
         c, dev = L.cfg, L.device
         T, B = c.UNROLL_STEP, c.BATCHSIZE
-        if L.model.first_conv_node() is None:
-            raise ValueError("fused_step(use_graph=True) reads the replay's frames with the fused conv_1 kernels: "
-                             "the model's first node must be the Atari conv_1")
+        if not _fused_first_layer(L.model):
+            raise ValueError("fused_step(use_graph=True) reads the replay's frames with the fused conv_1 or stem "
+                             "kernels: the model's first node must be the Atari conv_1 or a RESCNN2D stem")
         self.stream = torch.cuda.Stream(dev)
         self.cur = _rollout_buffers(T, B, dev)
         self.staged = L._staged_pool()
@@ -493,6 +524,12 @@ class _StagedRollouts:
 
     def stage(self, idx: torch.Tensor):
         return self.store.stage_frames(idx, self.buffers)
+
+
+def _fused_first_layer(model) -> bool:
+    """True if the model's first layer reads frames on libb2rl's kernels: the Atari conv_1, or the stem of a RESCNN2D
+    node."""
+    return model.first_conv_node() is not None or model.first_stem_node() is not None
 
 
 def _rollout_buffers(T: int, B: int, dev) -> dict:

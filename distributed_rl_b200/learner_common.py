@@ -222,6 +222,31 @@ class Conv1Gathered(torch.autograd.Function):
         return (gw,) + (None,) * (len(ctx.needs_input_grad) - 1)
 
 
+class StemGathered(torch.autograd.Function):
+    """The residual network's stem (3x3 conv + max-pool, R.stem_fused) over rows `idx` of a uint8 frame table, as
+    Conv1Gathered is conv_1: forward returns the pooled output the fused kernel already computed (`pooled`, with its
+    `argmax`); backward computes only dL/dW (the input is data) with the fused weight-gradient kernel, the max-pool's
+    backward folded into its loader through `argmax`, from the same rows read in place."""
+
+    @staticmethod
+    def forward(ctx, weight, frames, idx, pooled, argmax):
+        ctx.frames, ctx.weight_param, ctx.has_idx = frames, weight, idx is not None
+        idx_t = idx if idx is not None else torch.empty(0, dtype=torch.int64, device=frames.device)
+        ctx.save_for_backward(idx_t, argmax)
+        return pooled.view_as(pooled)
+
+    @staticmethod
+    def backward(ctx, gp):
+        idx, argmax = ctx.saved_tensors
+        idx = idx if ctx.has_idx else None
+        w = ctx.weight_param
+        from . import linear as _lin
+        if _lin._SINK is not None and w.grad is not None and w.grad.is_contiguous():
+            R.stem_wgrad(ctx.frames, idx, gp, argmax, out=w.grad, accumulate=True)
+            return (None,) * len(ctx.needs_input_grad)
+        return (R.stem_wgrad(ctx.frames, idx, gp, argmax),) + (None,) * (len(ctx.needs_input_grad) - 1)
+
+
 def conv1_packs(model, device, *n_nets):
     """-> (name of `model`'s first conv node, one Conv1Pack per entry of `n_nets`): each pack holds the conv_1
     weights of that many networks (1: online; 2: online + target, run as one launch)."""

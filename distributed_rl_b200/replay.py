@@ -1072,6 +1072,68 @@ def conv1_fused(frames, idx, pack: Conv1Pack, relu: bool = False, out=None):
     return [out[i].permute(0, 3, 1, 2) for i in range(pack.n_nets)]   # logical NCHW, physical NHWC
 
 
+STEM_OUT, STEM_HW = 16, 42      # the stem's channels and pooled size (84 -> 42)
+
+
+class StemPack:
+    """Packed stem weights (the RESCNN2D node's first conv, 16 x 4 x 3 x 3) for b2rl_stem_fused: four signed 7-bit
+    digits per weight and a per-channel scale, re-packed after every optimizer step (one tiny launch)."""
+
+    def __init__(self, device):
+        self.device = torch.device(device)
+        self.bq = torch.empty(STEM_OUT * 4 * 48, dtype=torch.int8, device=self.device)
+        self.scale = torch.empty(STEM_OUT, dtype=torch.float32, device=self.device)
+
+    def pack(self, weight: torch.Tensor) -> None:
+        w = weight.detach().to(torch.float32).contiguous(memory_format=torch.contiguous_format)
+        assert w.shape == (STEM_OUT, 4, 3, 3)
+        check(_lib.load().b2rl_stem_pack(w.data_ptr(), self.bq.data_ptr(), self.scale.data_ptr(),
+                                         _stream_ptr(self.device)))
+
+
+def stem_fused(frames, idx, pack: StemPack, out=None):
+    """The residual network's stem (3x3 conv of frames / 255, then a 3x3 / stride-2 max-pool) over rows `idx` of
+    `frames` (any source conv1_fused takes, except a CodedPlaneFrames and an Ape-X plane table) -> (pooled fp32
+    (n, 16, 42, 42), argmax uint8 (n, 16, 42, 42)): 3i + j of the first maximum of each window, row-major.
+    `out`: a (pooled, argmax) pair to write into."""
+    src = _frame_source(frames)
+    n = src.rows if idx is None else idx.numel()
+    dev = frames.device
+    if out is None:
+        out = (torch.empty((n, STEM_OUT, STEM_HW, STEM_HW), dtype=torch.float32, device=dev),
+               torch.empty((n, STEM_OUT, STEM_HW, STEM_HW), dtype=torch.uint8, device=dev))
+    pooled, amax = out
+    assert pooled.is_contiguous() and amax.is_contiguous() and pooled.shape[0] == n and amax.shape[0] == n
+    check(_lib.load().b2rl_stem_fused(src, None if idx is None else idx.data_ptr(), n, pack.bq.data_ptr(),
+                                      pack.scale.data_ptr(), pooled.data_ptr(), amax.data_ptr(), _stream_ptr(dev)))
+    return pooled, amax
+
+
+_stem_ws = {}
+
+
+def stem_wgrad(frames, idx, gpooled: torch.Tensor, argmax: torch.Tensor, out: torch.Tensor | None = None,
+               accumulate: bool = False) -> torch.Tensor:
+    """dL/dW of the stem's conv from the same rows, dL/d(pooled) (n, 16, 42, 42) and stem_fused's argmax: the
+    max-pool's backward folded into the kernel's loader (b2rl_stem_wgrad) -> (16, 4, 3, 3) fp32."""
+    src = _frame_source(frames)
+    n = src.rows if idx is None else idx.numel()
+    shape = (n, STEM_OUT, STEM_HW, STEM_HW)
+    assert gpooled.shape == shape and argmax.shape == shape and gpooled.dtype == torch.float32
+    gpooled, argmax = gpooled.contiguous(), argmax.contiguous()
+    dev = frames.device
+    if dev not in _stem_ws:
+        _stem_ws[dev] = torch.empty(_lib.load().b2rl_stem_wgrad_workspace_doubles(), dtype=torch.float64, device=dev)
+    if out is None:
+        out = torch.empty((STEM_OUT, 4, 3, 3), dtype=torch.float32, device=dev)
+        accumulate = False
+    assert out.is_contiguous() and out.numel() == STEM_OUT * 36
+    check(_lib.load().b2rl_stem_wgrad(src, None if idx is None else idx.data_ptr(), n, gpooled.data_ptr(),
+                                      argmax.data_ptr(), _stem_ws[dev].data_ptr(), out.data_ptr(),
+                                      int(bool(accumulate)), _stream_ptr(dev)))
+    return out
+
+
 _wgrad_ws = {}
 
 

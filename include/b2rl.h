@@ -485,6 +485,27 @@ int b2rl_conv1_wgrad(const b2rl_frames* frames, const int64_t* idx_dev, int64_t 
                      const float* y_relu_dev, int32_t c_out, float* workspace_dev, float* gw_dev, int32_t accumulate,
                      void* stream);
 
+/* The stem of the IMPALA residual network (netCat RESCNN2D, Espeholt et al. 2018 Fig. 3): a 3x3 / stride-1 / pad-1,
+ * 4 -> 16 channel bias-free conv of frames[idx[k]] / 255 followed by a 3x3 / stride-2 / pad-1 max-pool, fused with
+ * the gather (the RESCONV2D node of baseline/baseNetwork.py:796-820 cannot be built, and describes a different
+ * block; the convs are bias-free as its conv2D helper's, baseline/baseNetwork.py:742-760); the frames are read as
+ * conv_1 reads them, from any b2rl_frames source except a coded pool and
+ * plane_stride 0 / 8 (Ape-X's transition pairs).  Deterministic: no atomics, fixed summation orders.
+ *   b2rl_stem_pack   w_dev fp32 [16][4][3][3] -> packed int8 digits (bq_out: 3 072 bytes, 16-byte aligned) and
+ *                    per-channel scale (scale_out: 16 fp32)
+ *   b2rl_stem_fused  pooled_out_dev fp32 [n][16][42][42] (NCHW), argmax_out_dev uint8 [n][16][42][42]: 3i + j of
+ *                    the window position (row 2py - 1 + i, column 2px - 1 + j) that holds the first maximum in
+ *                    row-major window order, padded positions never chosen (torch's max_pool2d picks the same one)
+ *   b2rl_stem_wgrad  gw[co][c][ky][kx] (+)= dL/dW from the same rows, the pooled gradient gpooled_dev fp32
+ *                    [n][16][42][42] and the forward's argmax (16-byte aligned); workspace_dev:
+ *                    b2rl_stem_wgrad_workspace_doubles() doubles of per-SM partial sums. */
+int b2rl_stem_pack(const float* w_dev, int8_t* bq_out_dev, float* scale_out_dev, void* stream);
+int b2rl_stem_fused(const b2rl_frames* frames, const int64_t* idx_dev, int64_t n, const int8_t* bq_dev,
+                    const float* scale_dev, float* pooled_out_dev, uint8_t* argmax_out_dev, void* stream);
+int64_t b2rl_stem_wgrad_workspace_doubles(void);
+int b2rl_stem_wgrad(const b2rl_frames* frames, const int64_t* idx_dev, int64_t n, const float* gpooled_dev,
+                    const uint8_t* argmax_dev, double* workspace_dev, float* gw_dev, int32_t accumulate, void* stream);
+
 /* Learner.step (APE_X/Learner.py:123-138; IMPALA/Learner.py:258-266 without the clipping) with
  * torch.optim.RMSprop's update (baseline/utils.py getOptim :124-130; centered for Ape-X,
  * cfg/ape_x.json:27-35) in ONE pass: square_avg / grad_avg / param update, gradient zeroed, and
