@@ -1,16 +1,19 @@
 """fp64 references and per-element error bounds of the library's hand-written kernels, shared by the GPU tests that hold
-conv_1 (forward and weight gradient), the 3xTF32 dense layers, the dueling tail, V-trace and the fused RMSprop to fp64
-at the learners' step shapes (test_gpu_22_step_shapes, test_gpu_25_apex_step_shapes,
-test_gpu_35_secondary_steps_fp64), and the whole-step comparison against an fp64 restatement (check_vs_reference).
+conv_1 (forward and weight gradient), the residual network's stem (forward and weight gradient), the 3xTF32 dense
+layers, the dueling tail, V-trace and the fused RMSprop to fp64 at the learners' step shapes (test_gpu_22_step_shapes,
+test_gpu_25_apex_step_shapes, test_gpu_35_secondary_steps_fp64, test_gpu_40_impala_resnet,
+test_gpu_41_impala_resnet_step_fp64), and the whole-step comparison against an fp64 restatement (check_vs_reference).
 
 Every output element is held to its own bound, computed by the same fp64 reference applied to absolute values
 (`mag`), so the bound grows with the length of the sum behind that element; u = 2^-24.  The bound of each kernel is
 written in its checker's docstring.  The fp64 references run on the device, a chunk of frame stacks at a time; the
 frames are drawn on the device from seeded generators.  Importing this module needs torch, not a GPU;
-check_vtrace and check_vs_reference run on tensors of any device."""
+check_stem, check_stem_wgrad, check_vtrace and check_vs_reference run on tensors of any device."""
 import math
 
 import torch
+
+from stem_model import digit_exponent_t, pow2
 
 F = torch.nn.functional
 
@@ -117,6 +120,106 @@ def check_wgrad(what, frames, idx, gy, got, base=None, relu_y=None):
         ref, tol = ref + b, tol + 2 * U * b.abs()
     w = _Worst(what)
     w.add(got.reshape(c, 256), ref, tol)
+    return w.check()
+
+
+# --------------------------------------------------------------------------- #
+# the residual network's stem (csrc/stem.cu)                                    #
+# --------------------------------------------------------------------------- #
+def _stem_rows(frames, idx, a, b, dev):
+    return (frames[a:b] if idx is None else frames[idx[a:b]]).to(dev)
+
+
+def _stem_unpool(gp, argmax, H, W):
+    """The max-pool's backward through `argmax` in fp64 (n, C, H, W): each pooled gradient added at its window's
+    chosen position."""
+    n, C, PH, PW = gp.shape
+    a = argmax.long()
+    py = torch.arange(PH, device=gp.device).view(PH, 1)
+    px = torch.arange(PW, device=gp.device).view(1, PW)
+    pos = ((2 * py - 1 + a // 3) * W + (2 * px - 1 + a % 3)).view(n, C, -1)
+    gy = torch.zeros(n, C, H * W, dtype=torch.float64, device=gp.device)
+    return gy.scatter_add_(2, pos, gp.double().reshape(n, C, -1)).view(n, C, H, W)
+
+
+def check_stem(what, frames, idx, weight, pooled, argmax):
+    """stem_fused's pooled output and argmax (n, 16, PH, PW) of rows `idx` of uint8 `frames` against the fp64 conv
+    ref = F.conv2d(x / 255, W, padding=1), per conv position
+        tol = 2^-22 (1 + 2^-8) s_c sum_e x_e / 255 + 6u |ref|,      s_c = max|W_c| / 127,
+    sum_e over the zero-padded 3x3 patch.  The first term is the four 7-bit digits' truncation
+    |W - s sum_j q_j 2^-7j| <= s 2^-22 times the patch sum; its 2^-8 covers ft's fp32 conversion, which is inexact only
+    when |ft| >= 2^24 and then errs by at most 2^-38 |ft| <= 2^-24 sum_e x_e of the digit sums' unit s / (255 * 128),
+    below 2^-9 of the first term.  6u |ref|: the fp32 roundings after the exact sums (fu's conversion, inexact only when
+    |fu| >= 2^24 >> |ft 2^-14| so within u of |ref|; the FMA; the stored s / 255; the product), plus 1u for the second
+    order terms.  The pooled value is the kernel's conv value at its own argmax a, so
+        |pooled - ref[a]| <= tol[a],   and   ref[a] + tol[a] >= max_j (ref[j] - tol[j]) over every window's positions j:
+    the kernel's maximum is at least each of its window's kernel values.  Every argmax is 3i + j <= 8 and names a
+    position inside the frame, never the padding.  -> (pooled value ratio, window ratio)."""
+    n = pooled.shape[0]
+    dev = pooled.device
+    wd = weight.detach().to(dev, torch.float64)
+    sc = (weight.detach().abs().amax(dim=(1, 2, 3)).float() / 127.0).to(dev, torch.float64).view(1, -1, 1, 1)
+    ones = torch.ones(1, 4, 3, 3, dtype=torch.float64, device=dev)
+    held_w, win_w = _Worst(f"{what} pooled value at its argmax"), _Worst(f"{what} window maximum")
+    PH, PW = pooled.shape[-2:]
+    py = torch.arange(PH, device=dev).view(PH, 1)
+    px = torch.arange(PW, device=dev).view(1, PW)
+    for a in range(0, n, CHUNK):
+        b = min(n, a + CHUNK)
+        x = _stem_rows(frames, idx, a, b, dev).double() / 255.0
+        ref = F.conv2d(x, wd, padding=1)
+        tol = 2.0 ** -22 * (1 + 2.0 ** -8) * sc * F.conv2d(x, ones, padding=1) + 6 * U * ref.abs()
+        del x
+        H, W = ref.shape[-2:]
+        am = argmax[a:b].long()
+        assert am.max().item() <= 8, f"{what}: an argmax above 8"
+        yy, xx = 2 * py - 1 + am // 3, 2 * px - 1 + am % 3
+        assert ((yy >= 0) & (xx >= 0) & (yy < H) & (xx < W)).all(), f"{what}: an argmax names a padded position"
+        pos = (yy * W + xx).flatten(2)
+        held = ref.flatten(2).gather(2, pos).view_as(am)
+        t_held = tol.flatten(2).gather(2, pos).view_as(am)
+        del pos, yy, xx, am
+        held_w.add(pooled[a:b], held, t_held, at=a)
+        lower = F.max_pool2d(ref - tol, 3, 2, 1)                    # max_j (ref[j] - tol[j]), padding skipped
+        del ref, tol
+        win_w.add(torch.maximum(lower, held), held, t_held, at=a)  # error: how far the window's floor lies above
+        del lower, held, t_held
+    return held_w.check(), win_w.check()
+
+
+def check_stem_wgrad(what, frames, idx, gp, argmax, got, base=None):
+    """stem_wgrad's result `got` (16, 4, 3, 3) against base + the fp64 weight gradient of the same rows, routed through
+    the kernel's `argmax`: ref[c, e] = sum_{n,p} gy[n, c, p] x_e[n, p] / 255 with gy the pool's backward, per element
+        tol = 2^-25 sum_n s_{n,c} S_{n,e} + 5u mag + 2u |base|.
+    s_{n,c} = 2^(e-127) is the kernel's power-of-two digit scale of stack n, channel c (digit_exponent(4 max|gp|),
+    clamped to [27, 227]); rounding gy 2^24 / s to an integer errs by at most 1/2, s 2^-25 in gy, times
+    S_{n,e} = sum_p x_e[n, p] / 255, the stack's patch sum of element e over its positions.  mag = the same fp64 weight
+    gradient of the fold of |gp|: 3u for the fp32 fold (at most four terms, three roundings), 1u for the fp32 store,
+    1u for the fp64 sums over stacks, warps and CTAs (n 2^-53 << u) and the second order terms.  2u |base|: the
+    addition into an existing gradient.  The digit sums themselves and their scaling by s 2^-24 are exact."""
+    n, C = gp.shape[:2]
+    dev = gp.device
+    ref = torch.zeros(C, 36, dtype=torch.float64, device=dev)
+    mag, D = torch.zeros_like(ref), torch.zeros_like(ref)
+    for a in range(0, n, CHUNK):
+        b = min(n, a + CHUNK)
+        x = _stem_rows(frames, idx, a, b, dev).double() / 255.0
+        H, W = x.shape[-2:]
+        g, am = gp[a:b], argmax[a:b]
+        shape = (C,) + x.shape[1:2] + (3, 3)
+        ref += torch.nn.grad.conv2d_weight(x, shape, _stem_unpool(g, am, H, W), padding=1).view(C, 36)
+        mag += torch.nn.grad.conv2d_weight(x, shape, _stem_unpool(g.abs(), am, H, W), padding=1).view(C, 36)
+        p = F.pad(x, (1, 1, 1, 1))
+        S = torch.stack([p[:, :, ky:ky + H, kx:kx + W].sum(dim=(2, 3)) for ky in range(3) for kx in range(3)], 2)
+        s = pow2(digit_exponent_t(4 * g.abs().amax(dim=(2, 3))) - 127)                 # (n, C)
+        D += 2.0 ** -25 * (s.T @ S.reshape(b - a, 36))
+        del x, p
+    tol = D + 5 * U * mag
+    if base is not None:
+        bd = base.double().reshape(C, 36)
+        ref, tol = ref + bd, tol + 2 * U * bd.abs()
+    w = _Worst(what)
+    w.add(got.reshape(C, 36), ref, tol)
     return w.check()
 
 

@@ -1,10 +1,11 @@
 """GPU tests of the IMPALA residual network's fused stem (csrc/stem.cu: R.stem_fused, R.stem_wgrad) and of the IMPALA
 learner on impala.resnet_small_model().
 
-The stem forward against the numpy restatement of its arithmetic (tests/stem_model.py) bit for bit, pooled values and
-argmax, on random, constant and flat-block stacks (exact ties), borders included; against an fp64 conv + max-pool
-within conv_1's bound, each argmax holding a value within that bound of its window's fp64 maximum.  The weight
-gradient within 2e-6 of the largest |dW| of an fp64 one routed through the kernel's argmax.  Both bit-identical across
+The stem forward against the restatement of its arithmetic (tests/stem_model.py) bit for bit, pooled values and
+argmax, on random, constant and flat-block stacks (exact ties), borders included, at one stack per CTA and at three
+or four per CTA through a permuting, repeating idx; against fp64 within check_stem's per-element bounds (each pooled
+value within its own position's bound, each argmax within that bound of its window's maximum).  The weight gradient
+within one fp32 ulp of the restatement and within check_stem_wgrad's per-element bound.  Both bit-identical across
 runs and across frame sources holding the same frames.  The learner: fused_step against train() on the PyTorch stem;
 the captured step against the eager one; the served captured step against the in-process one; dedup and coded stores
 against a stack store."""
@@ -17,6 +18,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import stem_model as M                                          # noqa: E402
+from fp64_bounds import check_stem, check_stem_wgrad            # noqa: E402
 from impala_atari_rollouts import atari_rollouts                # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -57,49 +59,68 @@ def _weights(seed, scale=0.1):
     return torch.randn(16, 4, 3, 3, generator=g) * scale
 
 
-def test_stem_forward_equals_the_model_bit_for_bit_and_fp64(R):
-    F = torch.nn.functional
-    n = 40
-    frames = _stacks(n, 3)
+@pytest.fixture(scope="module")
+def sms(R):
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def test_stem_forward_equals_the_model_bit_for_bit_and_fp64(R, sms):
+    """n = 40: one stack per CTA.  Every stack bit for bit against stem_model's device restatement and its numpy loops,
+    the constant stacks' tie rule, and against fp64 through check_stem's per-element bounds."""
+    frames = _stacks(40, 3)
+    _check_stem_forward(R, sms, frames, None)
+
+
+def test_stem_forward_loops_over_stacks_bit_for_bit_and_fp64(R, sms):
+    """n = 3 * (2 SMs) + 5, read through an idx that permutes the rows and repeats some: every CTA of the persistent
+    kernel (grid 2 SMs) loops over three or four stacks, so the raw_full barrier's parity, the prefetch of the next
+    stack into sRaw and the conv-row ring are reused across stacks.  Every stack bit for bit against stem_model's
+    device restatement, and against fp64 through check_stem's per-element bounds."""
+    n = 3 * 2 * sms + 5
+    rows = n - 2 * sms                                          # the idx repeats 2 * SMs of the rows
+    frames = _stacks(rows, 3)
+    g = torch.Generator(device="cuda").manual_seed(11)
+    perm = torch.randperm(rows, device="cuda", generator=g)
+    idx = torch.cat([perm, perm[torch.randint(0, rows, (n - rows,), device="cuda", generator=g)]])
+    _check_stem_forward(R, sms, frames, idx[torch.randperm(n, device="cuda", generator=g)].contiguous())
+
+
+def _check_stem_forward(R, sms, frames, idx):
+    n = len(frames) if idx is None else idx.numel()
     w = _weights(1)
     fr = torch.from_numpy(frames).cuda()
     pack = R.StemPack("cuda")
     pack.pack(w.cuda())
-    pooled, amax = R.stem_fused(fr, None, pack)
-    pooled2, amax2 = R.stem_fused(fr, None, pack)
+    pooled, amax = R.stem_fused(fr, idx, pack)
+    pooled2, amax2 = R.stem_fused(fr, idx, pack)
     torch.cuda.synchronize()
+    assert pooled.shape == (n, 16, 42, 42)
     assert torch.equal(pooled, pooled2) and torch.equal(amax, amax2)               # run to run
     q, scale = M.pack(w.numpy())
     assert np.array_equal(pack.scale.cpu().numpy(), scale)
     bq = pack.bq.cpu().numpy().reshape(4, 16, 12, 4)
     assert np.array_equal(bq[..., :3].reshape(4, 16, 36), q) and not bq[..., 3].any()
-    for lo in range(0, n, 8):                                                   # the model in pieces (memory)
-        y = M.conv(frames[lo:lo + 8], w.numpy())
-        want_p, want_a = M.pool(y)
-        assert np.array_equal(pooled[lo:lo + 8].cpu().numpy(), want_p), lo
-        assert np.array_equal(amax[lo:lo + 8].cpu().numpy(), want_a), lo
-    # fp64: values within conv_1's bound, and each argmax holds a value within that bound of its window's maximum
-    x64 = fr.double() / 255
-    y64 = F.conv2d(x64, w.cuda().double(), padding=1)
-    p64 = F.max_pool2d(y64, 3, 2, 1)
-    bound = 2e-6 * p64.abs().max().item()
-    assert (pooled.double() - p64).abs().max().item() <= bound
-    a = amax.long()
-    assert a.max().item() <= 8
-    py = torch.arange(42, device="cuda").view(42, 1)
-    px = torch.arange(42, device="cuda").view(1, 42)
-    yy, xx = 2 * py - 1 + a // 3, 2 * px - 1 + a % 3
-    assert ((yy >= 0) & (xx >= 0)).all()                                        # a padded position is never chosen
-    held = y64.view(n, 16, -1).gather(2, (yy * 84 + xx).view(n, 16, -1)).view(n, 16, 42, 42)
-    assert (held - p64).abs().max().item() <= bound
-    # constant stacks: windows of interior conv rows all tie -> position 0; windows on the border never pick a padded
-    # position (the conv output differs at the border: its patches reach into the zero padding)
-    for k in (1, 2, 3):
-        assert amax[k, :, 1:41, 1:41].max().item() == 0
-        assert amax[k, :, 0].min().item() >= 3 and amax[k, :, :, 0].remainder(3).min().item() >= 1
+    want_p, want_a = M.forward_t(fr, idx, w.cuda())
+    bad = ((pooled.view(torch.int32) != want_p.view(torch.int32)) | (amax != want_a)).flatten(1).any(1)
+    print(f"[bits] stem forward n={n}, grid {min(n, 2 * sms)}: {int(bad.sum())} of {n} stacks differ")
+    assert not bad.any(), f"stacks {bad.nonzero()[:8, 0].tolist()} differ from the device restatement"
+    if idx is None:
+        for lo in range(0, n, 8):                                               # the numpy loops in pieces (memory)
+            want_p, want_a = M.pool(M.conv(frames[lo:lo + 8], w.numpy()))
+            assert np.array_equal(pooled[lo:lo + 8].cpu().numpy(), want_p), lo
+            assert np.array_equal(amax[lo:lo + 8].cpu().numpy(), want_a), lo
+        # constant stacks: windows of interior conv rows all tie -> position 0; windows on the border never pick a
+        # padded position (the conv output differs at the border: its patches reach into the zero padding)
+        for k in (1, 2, 3):
+            assert amax[k, :, 1:41, 1:41].max().item() == 0
+            assert amax[k, :, 0].min().item() >= 3 and amax[k, :, :, 0].remainder(3).min().item() >= 1
+    check_stem(f"stem forward n={n}", fr, idx, w.cuda(), pooled, amax)
 
 
 def test_stem_wgrad_within_the_fp64_bound_and_deterministic(R):
+    """n = 300 > SMs: the weight gradient's CTAs (grid = SMs) loop over two or three stacks each.  Within one fp32 ulp
+    of stem_model's device restatement of the kernel's arithmetic, and against fp64 through check_stem_wgrad's
+    per-element bound, alone and accumulated into an existing gradient."""
     n = 300                                                 # more stacks than SMs: several per CTA
     frames = _stacks(n, 5)
     w = _weights(2)
@@ -110,28 +131,21 @@ def test_stem_wgrad_within_the_fp64_bound_and_deterministic(R):
     g = torch.Generator(device="cuda").manual_seed(3)
     gp = torch.randn(n, 16, 42, 42, device="cuda", generator=g)
     gp[7] *= 1e-3                                           # a stack of small gradients: its own digit scale
+    gp[8] *= 1e-33                                          # and one whose digit exponent clamps at 27
     dw = R.stem_wgrad(fr, None, gp, amax)
     dw2 = R.stem_wgrad(fr, None, gp, amax)
     acc = dw.clone()
     R.stem_wgrad(fr, None, gp, amax, out=acc, accumulate=True)
     torch.cuda.synchronize()
     assert torch.equal(dw, dw2)
-    # fp64: the pool's backward through the kernel's argmax (max_unpool's scatter, in fp64), then an fp64 wgrad
-    a = amax.long()
-    py = torch.arange(42, device="cuda").view(42, 1)
-    px = torch.arange(42, device="cuda").view(1, 42)
-    pos = ((2 * py - 1 + a // 3) * 84 + (2 * px - 1 + a % 3)).view(n, 16, -1)
-    gy = torch.zeros(n, 16, 84 * 84, dtype=torch.float64, device="cuda")
-    gy.scatter_add_(2, pos, gp.double().view(n, 16, -1))
-    ref = torch.nn.grad.conv2d_weight(fr.double() / 255, (16, 4, 3, 3), gy.view(n, 16, 84, 84), padding=1)
-    err = (dw.double() - ref).abs().max().item()
-    assert err <= 2e-6 * ref.abs().max().item(), err
+    want = M.wgrad_t(fr, None, gp, amax)
+    d = M.ulps(dw, want)
+    print(f"[bits] stem wgrad n={n}: {int((d > 0).sum())} of {d.numel()} elements one ulp from the restatement")
+    assert d.max().item() <= 1
+    assert M.ulps(acc, M.wgrad_t(fr, None, gp, amax, base=dw)).max().item() <= 1
+    check_stem_wgrad(f"stem wgrad n={n}", fr, None, gp, amax, dw)
+    check_stem_wgrad(f"stem wgrad n={n} accumulated", fr, None, gp, amax, acc, base=dw)
     assert (acc.double() - 2 * dw.double()).abs().max().item() <= 2 ** -22 * dw.abs().max().item()
-    # the per-stack arithmetic of the numpy model on a few stacks
-    sel = slice(0, 6)
-    want = M.wgrad(frames[sel], gp[sel].cpu().numpy(), amax[sel].cpu().numpy())
-    got = R.stem_wgrad(fr[sel], None, gp[sel].contiguous(), amax[sel].contiguous())
-    assert np.abs(got.cpu().numpy().reshape(16, 36) - want).max() <= 2 ** -23 * np.abs(want).max()
 
 
 def _rollout_cols(n, T, seed):

@@ -1,6 +1,7 @@
 """CPU tests of the IMPALA residual network (netCat RESCNN2D, impala.resnet_small_model): the node's layers, feature
-sizes and parameter count, the config round trip, the refusals that need no GPU, and the numpy restatement of the
-fused stem's arithmetic (tests/stem_model.py) at a tiny size against float64."""
+sizes and parameter count, the config round trip, the refusals that need no GPU, the numpy restatement of the
+fused stem's arithmetic (tests/stem_model.py) at a tiny size against float64, and its torch restatement against the
+numpy one."""
 import os
 import sys
 import types
@@ -180,3 +181,53 @@ def test_the_stem_entry_points_refuse_bad_arguments_before_any_launch():
     assert b"16-byte" in lib.b2rl_last_error()
     assert lib.b2rl_stem_pack(None, dummy, dummy, None) == -1
     assert lib.b2rl_launch_count() == n0
+
+
+def _edge_stacks(n, H, seed):
+    """n >= 7 stacks: random, constant 0, 255 and 77, flat 3x3 and 4x4 blocks (exact ties inside and across
+    windows), and random again."""
+    rng = np.random.default_rng(seed)
+    f = rng.integers(0, 256, size=(n, 4, H, H), dtype=np.uint8)
+    f[1], f[2], f[3] = 0, 255, 77
+    for k, b in ((4, 3), (5, 4)):
+        blocks = rng.integers(0, 256, size=(4, (H + b - 1) // b, (H + b - 1) // b), dtype=np.uint8)
+        f[k] = np.repeat(np.repeat(blocks, b, axis=1), b, axis=2)[:, :H, :H]
+    return f
+
+
+@pytest.mark.parametrize("H", [9, 10, 84])
+def test_the_torch_restatement_is_the_numpy_model(H):
+    """stem_model's torch functions (which the GPU tests run at 21 504 stacks) against its numpy loops: the forward's
+    pooled values and argmax bit for bit, in chunks and through a permuting, repeating idx; the fold bit for bit in
+    fp32 and fp64; the weight gradient within one fp32 ulp (the two sum the stacks in other float64 orders), with
+    stacks of small gradients (their own digit scale) and of gradients so small the digit exponent clamps at 27."""
+    n = 7
+    frames = _edge_stacks(n, H, seed=H)
+    w = np.random.default_rng(3).standard_normal((16, 4, 3, 3)).astype(np.float32) * 0.1
+    w[2] = 0.0
+    w[6, 1, 1, 1] = 2.0                                     # one dominant weight: the small ones live in the low digits
+    want_p, want_a = M.pool(M.conv(frames, w))
+    ft, wt = torch.from_numpy(frames), torch.from_numpy(w)
+    got_p, got_a = M.forward_t(ft, None, wt, chunk=3)
+    assert np.array_equal(got_p.numpy().view(np.uint32), want_p.view(np.uint32))
+    assert np.array_equal(got_a.numpy(), want_a)
+    idx = torch.tensor([6, 0, 4, 4, 1, 5, 2, 3, 0])
+    p_i, a_i = M.forward_t(ft, idx, wt, chunk=4)
+    assert torch.equal(p_i, got_p[idx]) and torch.equal(a_i, got_a[idx])
+
+    rng = np.random.default_rng(4)
+    gp = rng.standard_normal(want_p.shape).astype(np.float32)
+    gp[3] *= np.float32(1e-3)
+    gp[4] *= np.float32(1e-33)                               # 4 max|gp| / 127 below 2^-100: the exponent clamps
+    gp[5] = np.abs(gp[5]) * np.exp2(-rng.uniform(0, 30, size=gp[5].shape)).astype(np.float32)
+    assert M.digit_exponent(4 * np.abs(gp[4]).max(axis=(1, 2))).max() == 27
+    gt, at = torch.from_numpy(gp), torch.from_numpy(want_a)
+    for dt, ndt in ((torch.float32, np.float32), (torch.float64, np.float64)):
+        assert np.array_equal(M.fold_t(gt, at, H, H, dt).numpy(), M.fold(gp, want_a, H, H, ndt))
+    want = torch.from_numpy(M.wgrad(frames, gp, want_a))
+    got = M.wgrad_t(ft, None, gt, at, chunk=3)
+    assert M.ulps(got.view(16, 36), want.float()).max().item() <= 1
+    assert (got.double().view(16, 36) - want).abs().max().item() <= 2 ** -24 * want.abs().max().item()
+    base = torch.from_numpy(rng.standard_normal((16, 4, 3, 3)).astype(np.float32))
+    acc = M.wgrad_t(ft, None, gt, at, base=base)
+    assert M.ulps(acc.view(16, 36), (base.double().view(16, 36) + want).float()).max().item() <= 1
