@@ -79,6 +79,7 @@ SIGNATURES = {
     "b2rl_conv1_wgrad": (C.c_int, [C.POINTER(Frames), c_vp, c_i64, c_vp, c_vp, c_i32, c_vp, c_vp, c_i32, c_vp]),
     "b2rl_stem_pack": (C.c_int, [c_vp, c_vp, c_vp, c_vp]),
     "b2rl_stem_fused": (C.c_int, [C.POINTER(Frames), c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "b2rl_stem_fused_pair": (C.c_int, [C.POINTER(Frames), c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b2rl_stem_wgrad_workspace_doubles": (c_i64, []),
     "b2rl_stem_wgrad": (C.c_int, [C.POINTER(Frames), c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp]),
     "b2rl_dedup_attach": (C.c_int, [c_vp, c_i32, c_i64, c_i64, c_u64]),

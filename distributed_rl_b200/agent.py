@@ -9,8 +9,9 @@ much smaller interpreter for the node types the three shipped configs use
 
     CNN2D  MLP  LSTMNET  ViewV2  Add  Mean  Substract
 
-and RESCNN2D, the IMPALA paper's residual network (impala.resnet_small_model; no shipped config uses it), with the
-same call surface the learners rely on: forward([inputs]) -> tuple,
+and RESCNN2D, the IMPALA paper's residual network (impala.resnet_small_model, and r2d2.resnet_model in front of
+R2D2's LSTM; no shipped config uses it, a config selects it through its MODEL dict), with the same call surface the
+learners rely on: forward([inputs]) -> tuple,
 getParameters, updateParameter(other, tau), setCellState / detachCellState /
 zeroCellState, calculateNorm, clippingNorm, and state_dict() key names
 (`module00.conv_1.weight`, `module02.MLP_1.weight`, `module02.rnn.weight_ih_l0`,

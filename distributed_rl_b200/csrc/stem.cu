@@ -271,6 +271,171 @@ k_stem_fused(const __grid_constant__ FwdParams P) {
   }
 }
 
+// ---- the stem of two networks over the same rows (b2rl_stem_fused_pair) ----
+// k_stem_fused's per-stack work as functions.  k_stem_fused keeps its own inline copy: routed through these, nvcc
+// commutes a few address additions and its SASS would no longer be the one it has been measured and checked with.
+
+// weight fragments of one pack: n-tile j = columns 8j .. 8j + 7 (digit j / 2, channels 8 (j % 2) ..); b0 / b1 the k32
+// step's groups tig and tig + 4, b2 the k16 step's group 8 + tig
+__device__ __forceinline__ void load_weight_frags(const int8_t* bq, int gid, int tig, uint32_t (&bw)[8][3]) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const uint32_t* row = reinterpret_cast<const uint32_t*>(bq + (8 * j + gid) * K_PAD);
+    bw[j][0] = row[tig]; bw[j][1] = row[tig + 4]; bw[j][2] = row[tig + 8];
+  }
+}
+
+// One stack against one pack: the 14 bands of conv rows from the zero-bordered image into the ring, each band's three
+// pooled rows written to `pooled` (and, with ARGMAX, their argmax to `amax`).  Ends on a barrier: the ring is free.
+template <bool ARGMAX>
+__device__ __forceinline__ void conv_pool_stack(const uint8_t* sPad, float* sRing, const uint32_t (&bw)[8][3],
+                                                const int (&goff)[3], const float* s_scale, float* pooled,
+                                                uint8_t* amax, int warp, int gid, int tig) {
+#pragma unroll 1
+  for (int b = 0; b < BANDS; ++b) {
+    // ---- conv rows 6b .. 6b + 5 into the ring ----
+#pragma unroll 1
+    for (int t = warp; t < M_TILES; t += WARPS) {
+      int yy[2], xx[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int p = min(t * 16 + gid + 8 * h, BAND_POS - 1);   // rows past the band compute a copy, not stored
+        const int r = p / HW;
+        yy[h] = BAND * b + r, xx[h] = p - r * HW;
+      }
+      uint32_t a[4], a4, a5;
+      a[0] = pad_word(sPad + goff[0] + yy[0] * PAD_W, xx[0]);
+      a[1] = pad_word(sPad + goff[0] + yy[1] * PAD_W, xx[1]);
+      a[2] = pad_word(sPad + goff[1] + yy[0] * PAD_W, xx[0]);
+      a[3] = pad_word(sPad + goff[1] + yy[1] * PAD_W, xx[1]);
+      a4 = pad_word(sPad + goff[2] + yy[0] * PAD_W, xx[0]);
+      a5 = pad_word(sPad + goff[2] + yy[1] * PAD_W, xx[1]);
+      int32_t acc[8][4];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0;
+        mma_k32(acc[j], a, bw[j][0], bw[j][1]);
+        mma_k16(acc[j], a4, a5, bw[j][2]);
+      }
+      // fragment: acc[j][2h + c] = row gid + 8h, column 8j + 2 tig + c; digit d of channel co is column 16d + co,
+      // so tile j = 2d + (co >= 8) and this thread holds all four digits of channels 2tig + c and 8 + 2tig + c
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (t * 16 + gid + 8 * h >= BAND_POS) continue;
+        float* ring = sRing + ((yy[h] + 1) % RING) * (C_OUT * HW) + xx[h];
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int i = 2 * h + c;
+            const int32_t q0 = acc[half][i], q1 = acc[2 + half][i], q2 = acc[4 + half][i], q3 = acc[6 + half][i];
+            // conv1.cu's recombination: exact pairs, one fp32 rounding each, one FMA, the scale
+            const float fu = (float)(q0 * 128 + q1);
+            const float ft = (float)(q2 * 128 + q3);
+            const int co = 8 * half + 2 * tig + c;
+            ring[co * HW] = __fmaf_rn(ft, 1.0f / 16384.0f, fu) * s_scale[co];
+          }
+        }
+      }
+    }
+    __syncthreads();
+    // ---- pooled rows 3b .. 3b + 2 from conv rows 6b - 1 .. 6b + 5 ----
+    for (int e = threadIdx.x; e < C_OUT * 3 * PHW; e += THREADS) {
+      const int co = e / (3 * PHW), rem = e - co * (3 * PHW);
+      const int py = 3 * b + rem / PHW, px = rem % PHW;
+      float best = -INFINITY;
+      int bi = 0;
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        const int y = 2 * py - 1 + i;
+        if (y < 0) continue;                                     // padded row (y <= 83 always)
+        const float* ring = sRing + ((y + 1) % RING) * (C_OUT * HW) + co * HW;
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+          const int x = 2 * px - 1 + j;
+          if (x < 0) continue;                                   // padded column (x <= 83 always)
+          const float v = ring[x];
+          if (v > best || v != v) { best = v; bi = 3 * i + j; }  // first maximum, as max_pool2d (NaN wins)
+        }
+      }
+      const int o = co * (PHW * PHW) + py * PHW + px;
+      pooled[o] = best;
+      if (ARGMAX) amax[o] = (uint8_t)bi;
+    }
+    __syncthreads();
+  }
+}
+
+// this thread's A groups (c, ky): tig, tig + 4, tig + 8 -> byte offset of padded row ky of channel c
+__device__ __forceinline__ void group_offsets(int tig, int (&goff)[3]) {
+#pragma unroll
+  for (int q = 0; q < 3; ++q) {
+    const int g = tig + 4 * q;
+    goff[q] = (g / 3) * PAD_PLANE + (g % 3) * PAD_W;
+  }
+}
+
+constexpr int PACK_BYTES = N_COLS * K_PAD;         // 3 072: one network's packed digits
+
+struct PairParams {
+  FrameSource src;
+  const int64_t* idx;        // sampled rows, or nullptr for rows 0..n-1
+  int64_t n;
+  const int8_t* bq;          // [2][64][48]: net 0's pack, then net 1's
+  const float* scale;        // [2][16]
+  float* pooled;             // [2][n][16][42][42]
+  uint8_t* argmax;           // net 0's [n][16][42][42] (ARGMAX only)
+};
+
+// Both networks' stems over the same rows (R2D2's online and target nets): each stack is loaded and zero-bordered
+// once, then run through k_stem_fused's bands against net 0's digits and then net 1's, on the one ring (a second ring
+// would not leave two CTAs per SM).  Per net the arithmetic is k_stem_fused's, so each net's output is bit for bit a
+// single-net launch's with that net's pack.  ARGMAX: write net 0's argmax (net 1's is never needed).
+template <FrameKind KIND, bool ARGMAX>
+__global__ void __launch_bounds__(THREADS, 2)
+k_stem_fused_pair(const __grid_constant__ PairParams P) {
+  extern __shared__ __align__(128) uint8_t smem_raw[];
+  uint8_t* sRaw = smem_raw;
+  uint8_t* sPad = sRaw + RAW_BYTES;
+  float* sRing = reinterpret_cast<float*>(sPad + PAD_BYTES);   // [7][16][84]: conv row r in slot (r + 1) % 7
+  __shared__ __align__(8) uint64_t raw_full;
+  __shared__ float s_scale[2 * C_OUT];
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int gid = lane >> 2, tig = lane & 3;
+  if (threadIdx.x < 2 * C_OUT) s_scale[threadIdx.x] = P.scale[threadIdx.x] * (1.0f / 128.0f);   // exact
+  zero_pad(sPad);
+  if (threadIdx.x == 0) {
+    mbar_init(&raw_full, 1);
+    mbar_init_fence();
+  }
+  __syncthreads();
+  const uint8_t* frames = frame_base<KIND>(P.src);
+  if (threadIdx.x == 0 && blockIdx.x < P.n)
+    load_row<KIND>(P.src, frames, clamp_row(P.src, P.idx, blockIdx.x), sRaw, &raw_full);
+  int goff[3];
+  group_offsets(tig, goff);
+
+  int it = 0;
+  for (int64_t k = blockIdx.x; k < P.n; k += gridDim.x, ++it) {
+    mbar_wait(&raw_full, it & 1);
+    fill_pad(sRaw, sPad);
+    fence_async_smem();
+    __syncthreads();
+    if (threadIdx.x == 0 && k + gridDim.x < P.n)
+      load_row<KIND>(P.src, frames, clamp_row(P.src, P.idx, k + gridDim.x), sRaw, &raw_full);
+    // the fragments are reloaded per net (L1-resident 3 KB packs) rather than held for both: the same registers as
+    // k_stem_fused
+    uint32_t bw[8][3];
+    load_weight_frags(P.bq, gid, tig, bw);
+    conv_pool_stack<ARGMAX>(sPad, sRing, bw, goff, s_scale, P.pooled + k * POOLED, ARGMAX ? P.argmax + k * POOLED : nullptr,
+                            warp, gid, tig);
+    load_weight_frags(P.bq + PACK_BYTES, gid, tig, bw);
+    conv_pool_stack<false>(sPad, sRing, bw, goff, s_scale + C_OUT, P.pooled + (P.n + k) * POOLED, nullptr, warp, gid,
+                           tig);
+  }
+}
+
 struct WgradParams {
   FrameSource src;
   const int64_t* idx;
@@ -520,6 +685,45 @@ extern "C" int b2rl_stem_fused(const b2rl_frames* frames, const int64_t* idx_dev
       cudaError_t r = set_max_dynamic_smem<stem::k_stem_fused<KIND>>(dev, stem::FWD_SMEM);
       if (r != cudaSuccess) return r;
       stem::k_stem_fused<KIND><<<grid, stem::THREADS, stem::FWD_SMEM, st>>>(P);
+      return cudaSuccess;
+    }
+  });
+  B2RL_CUDA(e);
+  count_launch();
+  B2RL_CHECK_LAUNCH();
+  return B2RL_OK;
+}
+
+extern "C" int b2rl_stem_fused_pair(const b2rl_frames* frames, const int64_t* idx_dev, int64_t n, const int8_t* bq_dev,
+                                    const float* scale_dev, float* pooled_out_dev, uint8_t* argmax_out_dev,
+                                    void* stream) {
+  B2RL_REQUIRE(n >= 0, "negative n");
+  stem::PairParams P{};
+  FrameKind kind;
+  if (const int rc = stem::check_stem_frames(frames, P.src, kind)) return rc;
+  if (n == 0) return B2RL_OK;
+  B2RL_REQUIRE(bq_dev && scale_dev && pooled_out_dev, "null argument");
+  B2RL_REQUIRE((uintptr_t)bq_dev % 16 == 0, "packed weights must be 16-byte aligned");
+  int dev = 0, sms = 0;
+  B2RL_CUDA(cudaGetDevice(&dev));
+  B2RL_CUDA(sm_count(dev, &sms));
+  P.idx = idx_dev, P.n = n, P.bq = bq_dev, P.scale = scale_dev, P.pooled = pooled_out_dev, P.argmax = argmax_out_dev;
+  const unsigned grid = (unsigned)(n < 2 * (int64_t)sms ? n : 2 * (int64_t)sms);
+  cudaStream_t st = (cudaStream_t)stream;
+  const cudaError_t e = with_frame_kind(kind, [&](auto K) {
+    constexpr FrameKind KIND = decltype(K)::value;
+    if constexpr (KIND == FrameKind::CodedPlanes) {
+      return cudaErrorInvalidValue;                       // refused by check_stem_frames
+    } else {
+      if (argmax_out_dev) {
+        cudaError_t r = set_max_dynamic_smem<stem::k_stem_fused_pair<KIND, true>>(dev, stem::FWD_SMEM);
+        if (r != cudaSuccess) return r;
+        stem::k_stem_fused_pair<KIND, true><<<grid, stem::THREADS, stem::FWD_SMEM, st>>>(P);
+      } else {
+        cudaError_t r = set_max_dynamic_smem<stem::k_stem_fused_pair<KIND, false>>(dev, stem::FWD_SMEM);
+        if (r != cudaSuccess) return r;
+        stem::k_stem_fused_pair<KIND, false><<<grid, stem::THREADS, stem::FWD_SMEM, st>>>(P);
+      }
       return cudaSuccess;
     }
   });

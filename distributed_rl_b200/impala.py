@@ -13,7 +13,8 @@ import torch
 from . import replay as R
 from .agent import GraphAgent
 from .learner_common import (CapturedStep, Conv1Gathered, ReplayThread, StemGathered, _attach_replay,
-                             check_served_fused, conv1_packs, make_optimizer, publishers, time_major_rows)
+                             check_served_fused, conv1_packs, fused_first_layer, make_optimizer, publishers,
+                             time_major_rows)
 from .publish import ParamPublisher
 
 
@@ -230,7 +231,7 @@ class Learner(CapturedStep):
         T, B = c.UNROLL_STEP, c.BATCHSIZE
         dev = self.device
         state, action, mu, reward, done = [torch.as_tensor(x).to(dev) for x in transition]
-        fused = c.FUSED_CONV1 and state.dtype == torch.uint8 and _fused_first_layer(self.model)
+        fused = c.FUSED_CONV1 and state.dtype == torch.uint8 and fused_first_layer(self.model)
         if fused:   # the staged batch is the frame table: rows already are time-major
             frames = state.contiguous().view((T + 1) * B, 4, 84, 84)
             self._train_core(frames, None, action, mu, reward, done, step)
@@ -475,7 +476,7 @@ class _BoundRollouts:
     def __init__(self, L: "Learner"):
         c, dev = L.cfg, L.device
         T, B = c.UNROLL_STEP, c.BATCHSIZE
-        if not _fused_first_layer(L.model):
+        if not fused_first_layer(L.model):
             raise ValueError("SERVED_FUSED_STEP reads the ring slot's frames with the fused conv_1 or stem kernels: "
                              "the model's first node must be the Atari conv_1 or a RESCNN2D stem")
         self.stream = torch.cuda.Stream(dev)
@@ -498,7 +499,7 @@ class _DrawnRollouts:
     def __init__(self, L: "Learner"):
         c, dev = L.cfg, L.device
         T, B = c.UNROLL_STEP, c.BATCHSIZE
-        if not _fused_first_layer(L.model):
+        if not fused_first_layer(L.model):
             raise ValueError("fused_step(use_graph=True) reads the replay's frames with the fused conv_1 or stem "
                              "kernels: the model's first node must be the Atari conv_1 or a RESCNN2D stem")
         self.stream = torch.cuda.Stream(dev)
@@ -524,12 +525,6 @@ class _StagedRollouts:
 
     def stage(self, idx: torch.Tensor):
         return self.store.stage_frames(idx, self.buffers)
-
-
-def _fused_first_layer(model) -> bool:
-    """True if the model's first layer reads frames on libb2rl's kernels: the Atari conv_1, or the stem of a RESCNN2D
-    node."""
-    return model.first_conv_node() is not None or model.first_stem_node() is not None
 
 
 def _rollout_buffers(T: int, B: int, dev) -> dict:

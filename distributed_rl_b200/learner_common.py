@@ -247,6 +247,19 @@ class StemGathered(torch.autograd.Function):
         return (R.stem_wgrad(ctx.frames, idx, gp, argmax),) + (None,) * (len(ctx.needs_input_grad) - 1)
 
 
+def fused_first_layer(model) -> bool:
+    """True if the model's first layer reads frames on libb2rl's kernels: the Atari conv_1, or the stem of a RESCNN2D
+    node (GraphAgent.first_stem_node)."""
+    return model.first_conv_node() is not None or model.first_stem_node() is not None
+
+
+def require_fused_first_layer(model, what: str) -> None:
+    """ValueError naming `what` (the step that reads the frames in place) unless fused_first_layer(model)."""
+    if not fused_first_layer(model):
+        raise ValueError(f"{what} reads the frames with the fused conv_1 or stem kernels: the model's first node must be "
+                         "the Atari conv_1 or a RESCNN2D stem")
+
+
 def conv1_packs(model, device, *n_nets):
     """-> (name of `model`'s first conv node, one Conv1Pack per entry of `n_nets`): each pack holds the conv_1
     weights of that many networks (1: online; 2: online + target, run as one launch)."""
@@ -275,12 +288,13 @@ def publishers(model, log_w, *pubs):
 
 
 def check_served_fused(cfg, memory, fields=None) -> None:
-    """What SERVED_FUSED_STEP needs, checked before the learner builds anything: FUSED_CONV1 (conv_1 reads the ring
-    slot's frames through the frame table), a memory that binds ring slots (DeviceReplayClient.acquire / release), a
+    """What SERVED_FUSED_STEP needs, checked before the learner builds anything: FUSED_CONV1 (conv_1, or a RESCNN2D
+    model's stem, reads the ring slot's frames through the frame table; the model itself is checked when the step
+    state is built, require_fused_first_layer), a memory that binds ring slots (DeviceReplayClient.acquire / release), a
     ring whose minibatches hold BATCHSIZE records and, when `fields` is given, a ring that carries those fields."""
     if not cfg.FUSED_CONV1:
-        raise ValueError("SERVED_FUSED_STEP reads the frames in the ring slot with the fused conv_1 kernels: it "
-                         "needs FUSED_CONV1")
+        raise ValueError("SERVED_FUSED_STEP reads the frames in the ring slot with the fused conv_1 or stem kernels: "
+                         "it needs FUSED_CONV1")
     if not (hasattr(memory, "acquire") and hasattr(memory, "release")):
         raise TypeError("SERVED_FUSED_STEP needs a served memory that binds ring slots (DeviceReplayClient)")
     L = memory.ring.layout

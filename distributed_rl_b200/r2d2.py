@@ -16,8 +16,9 @@ import torch
 
 from . import replay as R
 from .agent import GraphAgent
-from .learner_common import (Conv1Gathered, MemoryView, ReplayThread, TargetNetLearner, _attach_replay,
-                             check_served_fused, conv1_packs, make_optimizer, time_major_rows)
+from .learner_common import (Conv1Gathered, MemoryView, ReplayThread, StemGathered, TargetNetLearner, _attach_replay,
+                             check_served_fused, conv1_packs, fused_first_layer, make_optimizer,
+                             require_fused_first_layer, time_major_rows)
 
 
 def default_r2d2_model() -> dict:
@@ -38,6 +39,19 @@ def default_r2d2_model() -> dict:
         "module05": {"netCat": "Substract", "prior": 5, "prevNodeNames": ["module04", "module04_1"],
                      "output": True},
     }
+
+
+def resnet_model() -> dict:
+    """default_r2d2_model() with the IMPALA paper's residual torso in front of the LSTM, the R2D2 paper's DMLab-30
+    agent (R2D2+): module00 is impala.resnet_small_model()'s RESCNN2D node (16, 32, 32 channels, two blocks per
+    section, 84 -> 11) and the LSTM takes its 3 872 features; the dueling heads are unchanged.  9 607 744 parameters.
+    R2D2Config(MODEL=resnet_model()) trains it; with FUSED_CONV1 its stem reads the sampled sequences' frames in place
+    for both networks (R.stem_fused_pair)."""
+    from .impala import resnet_small_model
+    m = default_r2d2_model()
+    m["module00"] = dict(resnet_small_model()["module00"])
+    m["module02"]["iSize"] = 3872
+    return m
 
 
 @dataclass
@@ -245,7 +259,7 @@ class Learner(TargetNetLearner):
         self.model.setCellState((h0, h1))                       # :86-87
         self.target_model.setCellState((h0, h1))
         state = torch.as_tensor(state).to(dev)
-        fused = c.FUSED_CONV1 and state.dtype == torch.uint8 and self.model.first_conv_node() is not None
+        fused = c.FUSED_CONV1 and state.dtype == torch.uint8 and fused_first_layer(self.model)
         if fused:
             strips = R.stacks_strips(state)
             if strips is not None:                              # the stack view of frame strips: read the windows
@@ -299,7 +313,10 @@ class Learner(TargetNetLearner):
     def _forward_fused(self, frames, tm_rows, T, MEM, B, A):
         """The forward passes with conv_1 on the tensor cores, reading `frames` (a uint8 (rows, 4, 84, 84) table:
         the staged batch or the replay payload itself, its stacks or the windows of its strips) IN PLACE: the (b, t) ->
-        time-major reordering and the uint8 -> /255 conversion are folded into the kernel's gather (`tm_rows`)."""
+        time-major reordering and the uint8 -> /255 conversion are folded into the kernel's gather (`tm_rows`).  A
+        RESCNN2D model runs its stem instead (_forward_stem)."""
+        if self.model.first_stem_node() is not None:
+            return self._forward_stem(frames, tm_rows, T, MEM, B, A)
         dev = self.device
         if not hasattr(self, "_pack2"):
             self._conv_name, self._pack2, self._pack1 = conv1_packs(self.model, dev, 2, 1)
@@ -322,6 +339,35 @@ class Learner(TargetNetLearner):
         q = self.model.forward_from_conv1(y, False, [shape])[0].view(L, B, A)             # :121
         with torch.no_grad():
             q_target = self.target_model.forward_from_conv1(torch.relu(y_tg_w), True, [shape])[0].view(L, B, A)
+        return q, q_target
+
+    def _forward_stem(self, frames, tm_rows, T, MEM, B, A):
+        """_forward_fused for a RESCNN2D model: the residual network's stem (3x3 conv + max-pool) of both networks in
+        one launch per pass (R.stem_fused_pair), reading `frames` in place through `tm_rows`.  The online net's grad
+        pass takes the window's pooled output through StemGathered, whose backward runs the stem's weight-gradient
+        kernel over the same rows; only that pass needs the argmax."""
+        if not hasattr(self, "_stem_packs"):
+            self._stem_packs = R.stem_pack_pair(self.device)
+        name = self.model.first_stem_node()
+        w_on = getattr(self.model, name).conv_1.weight
+        pack_on, pack_tg = self._stem_packs
+        pack_on.pack(w_on)
+        pack_tg.pack(getattr(self.target_model, name).conv_1.weight)
+        rows_burn, rows_win = tm_rows[:MEM * B], tm_rows[MEM * B:]
+        L = T - MEM
+        with torch.no_grad():                                   # burn-in, :99-104
+            p_on, p_tg, _ = R.stem_fused_pair(frames, rows_burn, pack_on, pack_tg, argmax=False)
+            shape = torch.tensor([MEM, B, -1])
+            self.model.forward_from_stem(p_on, [shape])
+            self.target_model.forward_from_stem(p_tg, [shape])
+            self.model.detachCellState()
+            self.target_model.detachCellState()
+            p_on_w, p_tg_w, a_on_w = R.stem_fused_pair(frames, rows_win, pack_on, pack_tg)
+        shape = torch.tensor([L, B, -1])
+        pooled = StemGathered.apply(w_on, frames, rows_win, p_on_w, a_on_w)
+        q = self.model.forward_from_stem(pooled, [shape])[0].view(L, B, A)              # :121
+        with torch.no_grad():
+            q_target = self.target_model.forward_from_stem(p_tg_w, [shape])[0].view(L, B, A)   # :132
         return q, q_target
 
     def fused_step(self, use_graph: bool = False):
@@ -452,12 +498,10 @@ class _StepState:
     def __init__(self, L: "Learner"):
         c, dev = L.cfg, L.device
         T, B = c.FIXED_TRAJECTORY, c.BATCHSIZE
+        require_fused_first_layer(L.model, "SERVED_FUSED_STEP" if L._served else "fused_step(use_graph=True)")
         self.stream = torch.cuda.Stream(dev)
         self.cur = self.frames = self.rows = None
         if L._served:
-            if L.model.first_conv_node() is None:
-                raise ValueError("SERVED_FUSED_STEP reads the ring slot's frames with the fused conv_1 kernels: the "
-                                 "model's first node must be the Atari conv_1")
             self.cur = dict(R.alloc_rows(R.r2d2_config_fields(c), B, dev, ("action", "reward", "h0", "h1", "notdone")),
                             idx=torch.empty(B, dtype=torch.int64, device=dev),
                             w=torch.empty(B, dtype=torch.float32, device=dev),

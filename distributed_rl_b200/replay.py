@@ -1079,10 +1079,13 @@ class StemPack:
     """Packed stem weights (the RESCNN2D node's first conv, 16 x 4 x 3 x 3) for b2rl_stem_fused: four signed 7-bit
     digits per weight and a per-channel scale, re-packed after every optimizer step (one tiny launch)."""
 
-    def __init__(self, device):
+    BYTES = STEM_OUT * 4 * 48          # 3 072
+
+    def __init__(self, device, bq: torch.Tensor | None = None, scale: torch.Tensor | None = None):
+        """`bq`, `scale`: storage to pack into (stem_pack_pair's views), else freshly allocated."""
         self.device = torch.device(device)
-        self.bq = torch.empty(STEM_OUT * 4 * 48, dtype=torch.int8, device=self.device)
-        self.scale = torch.empty(STEM_OUT, dtype=torch.float32, device=self.device)
+        self.bq = torch.empty(self.BYTES, dtype=torch.int8, device=self.device) if bq is None else bq
+        self.scale = torch.empty(STEM_OUT, dtype=torch.float32, device=self.device) if scale is None else scale
 
     def pack(self, weight: torch.Tensor) -> None:
         w = weight.detach().to(torch.float32).contiguous(memory_format=torch.contiguous_format)
@@ -1107,6 +1110,42 @@ def stem_fused(frames, idx, pack: StemPack, out=None):
     check(_lib.load().b2rl_stem_fused(src, None if idx is None else idx.data_ptr(), n, pack.bq.data_ptr(),
                                       pack.scale.data_ptr(), pooled.data_ptr(), amax.data_ptr(), _stream_ptr(dev)))
     return pooled, amax
+
+
+def stem_pack_pair(device) -> tuple:
+    """(online, target) StemPacks over one allocation, back to back as b2rl_stem_fused_pair reads them: a
+    stem_fused_pair of the two then passes their storage as it lies."""
+    bq = torch.empty(2 * StemPack.BYTES, dtype=torch.int8, device=device)
+    scale = torch.empty(2 * STEM_OUT, dtype=torch.float32, device=device)
+    return tuple(StemPack(device, bq[i * StemPack.BYTES:(i + 1) * StemPack.BYTES], scale[i * STEM_OUT:(i + 1) * STEM_OUT])
+                 for i in range(2))
+
+
+def stem_fused_pair(frames, idx, pack_online: StemPack, pack_target: StemPack, argmax: bool = True, out=None):
+    """stem_fused of two networks over the same rows in one launch (b2rl_stem_fused_pair): each stack is read and
+    zero-bordered once and run against both packs.  -> (online pooled, target pooled, online argmax or None), each
+    net's pooled output (n, 16, 42, 42) and the argmax bit for bit stem_fused's with that pack.  `argmax`: write the
+    online net's argmax (the grad pass needs it; the burn-in and the target never do).  Packs from stem_pack_pair are
+    read in place; any other two are first copied side by side.  `out`: a (pooled (2, n, 16, 42, 42), argmax or None)
+    pair to write into."""
+    src = _frame_source(frames)
+    n = src.rows if idx is None else idx.numel()
+    dev = frames.device
+    if out is None:
+        out = (torch.empty((2, n, STEM_OUT, STEM_HW, STEM_HW), dtype=torch.float32, device=dev),
+               torch.empty((n, STEM_OUT, STEM_HW, STEM_HW), dtype=torch.uint8, device=dev) if argmax else None)
+    pooled, amax = out
+    assert pooled.is_contiguous() and pooled.shape[:2] == (2, n) and (amax is None) == (not argmax)
+    assert amax is None or (amax.is_contiguous() and amax.shape[0] == n)
+    on, tg = pack_online, pack_target
+    if tg.bq.data_ptr() == on.bq.data_ptr() + StemPack.BYTES and tg.scale.data_ptr() == on.scale.data_ptr() + 4 * STEM_OUT:
+        bq, scale = on.bq, on.scale
+    else:
+        bq, scale = torch.cat([on.bq, tg.bq]), torch.cat([on.scale, tg.scale])
+    check(_lib.load().b2rl_stem_fused_pair(src, None if idx is None else idx.data_ptr(), n, bq.data_ptr(),
+                                           scale.data_ptr(), pooled.data_ptr(),
+                                           None if amax is None else amax.data_ptr(), _stream_ptr(dev)))
+    return pooled[0], pooled[1], amax
 
 
 _stem_ws = {}

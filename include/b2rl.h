@@ -496,12 +496,21 @@ int b2rl_conv1_wgrad(const b2rl_frames* frames, const int64_t* idx_dev, int64_t 
  *   b2rl_stem_fused  pooled_out_dev fp32 [n][16][42][42] (NCHW), argmax_out_dev uint8 [n][16][42][42]: 3i + j of
  *                    the window position (row 2py - 1 + i, column 2px - 1 + j) that holds the first maximum in
  *                    row-major window order, padded positions never chosen (torch's max_pool2d picks the same one)
+ *   b2rl_stem_fused_pair  b2rl_stem_fused of two networks over the same rows in one launch (R2D2's online and target
+ *                    nets, the burn-in and window forwards of R2D2/Learner.py:99-104,121,132): each stack is loaded
+ *                    and zero-bordered once and run against both packs.  bq_dev: the two nets' packs, 3 072 bytes
+ *                    each, back to back (16-byte aligned); scale_dev: 2 x 16 fp32; pooled_out_dev fp32
+ *                    [2][n][16][42][42] (net 0's n stacks, then net 1's); argmax_out_dev uint8 [n][16][42][42], net
+ *                    0's argmax, or NULL for none.  Each net's pooled output (and net 0's argmax) is bit for bit what
+ *                    b2rl_stem_fused writes with that net's pack.
  *   b2rl_stem_wgrad  gw[co][c][ky][kx] (+)= dL/dW from the same rows, the pooled gradient gpooled_dev fp32
  *                    [n][16][42][42] and the forward's argmax (16-byte aligned); workspace_dev:
  *                    b2rl_stem_wgrad_workspace_doubles() doubles of per-SM partial sums. */
 int b2rl_stem_pack(const float* w_dev, int8_t* bq_out_dev, float* scale_out_dev, void* stream);
 int b2rl_stem_fused(const b2rl_frames* frames, const int64_t* idx_dev, int64_t n, const int8_t* bq_dev,
                     const float* scale_dev, float* pooled_out_dev, uint8_t* argmax_out_dev, void* stream);
+int b2rl_stem_fused_pair(const b2rl_frames* frames, const int64_t* idx_dev, int64_t n, const int8_t* bq_dev,
+                         const float* scale_dev, float* pooled_out_dev, uint8_t* argmax_out_dev, void* stream);
 int64_t b2rl_stem_wgrad_workspace_doubles(void);
 int b2rl_stem_wgrad(const b2rl_frames* frames, const int64_t* idx_dev, int64_t n, const float* gpooled_dev,
                     const uint8_t* argmax_dev, double* workspace_dev, float* gw_dev, int32_t accumulate, void* stream);

@@ -1,6 +1,16 @@
-"""Measure IMPALA on the residual network (impala.resnet_small_model) on one GPU.
+"""Measure IMPALA, or R2D2, on the residual network (impala.resnet_small_model, r2d2.resnet_model) on one GPU.
 
     python tools/bench_impala_resnet.py [--steps 20] [--iters 20]
+    python tools/bench_impala_resnet.py --workload r2d2 [--steps 20] [--iters 20]
+
+--workload r2d2 prints, at B = 64, T = 80, MEM = 20 (1 280 burn-in and 3 840 window stacks per network):
+  - the two-network stem launch (R.stem_fused_pair) against two single-net launches (R.stem_fused) on the same rows,
+    at both stack counts, timed with CUDA events (burn-in: the pair without argmax; window: with the online argmax);
+  - captured in-process learner steps/s and peak device memory for r2d2.resnet_model() and for the default conv model;
+  - one eager residual-model step under torch.profiler: its kernels' device time split into stem, residual-block
+    convs, LSTM, dense heads and the rest.
+
+The default (IMPALA) workload:
 
 Prints, with the card's name and power limit read in the same run:
   - captured in-process learner steps/s at B = 32 and B = 1024 (T = 20), over a pushed stack store;
@@ -71,8 +81,9 @@ KERNEL_CLASSES = (                       # first match wins; names are the kerne
 )
 
 
-def profile_step(L) -> dict:
-    """One eager step of learner L under torch.profiler: device time of its kernels by class, and the largest six."""
+def profile_step(L, classes=KERNEL_CLASSES) -> dict:
+    """One eager step of learner L under torch.profiler: device time of its kernels by `classes`, and the largest
+    six."""
     from torch.profiler import ProfilerActivity, profile
     L.fused_step()
     torch.cuda.synchronize()
@@ -86,7 +97,7 @@ def profile_step(L) -> dict:
         per[e.name] = per.get(e.name, 0.0) + e.time_range.elapsed_us() / 1000.0
     split = {"total_ms": sum(per.values())}
     for name, ms in per.items():
-        cls = next((c for c, keys in KERNEL_CLASSES if any(k in name.lower() for k in keys)), "other")
+        cls = next((c for c, keys in classes if any(k in name.lower() for k in keys)), "other")
         split[cls] = split.get(cls, 0.0) + ms
     split["top"] = sorted(((ms, name[:90]) for name, ms in per.items()), reverse=True)[:6]
     return split
@@ -160,8 +171,138 @@ def stem_alone(iters: int, cols) -> dict:
     return out
 
 
+# ---- --workload r2d2 ---------------------------------------------------------------------------------------------
+R2D2_B, R2D2_T, R2D2_MEM, R2D2_N = 64, 80, 20, 160
+
+LSTM = "LSTM (cuDNN RNN, cuBLAS GEMMs)"
+R2D2_CLASSES = (                         # first match wins; names are the kernels' own
+    ("stem", ("k_stem",)),
+    ("dense heads (3xTF32, dueling tail)", ("k_gemm", "splitk", "dueling")),
+    (LSTM, ("rnn", "lstm", "elemwise")),
+    ("residual-block convs (cuDNN, with its layout transforms)",
+     ("fprop", "dgrad", "wgrad", "implicit", "convolve", "winograd", "fft", "conv", "nchwtonhwc", "nhwctonchw")),
+    (LSTM, ("gemm",)),                   # the only cuBLAS GEMMs left: the LSTM's input and recurrent projections
+)
+
+
+def r2d2_store(dev):
+    """A stack store of R2D2_N hashed sequences, valid small fields and a built tree."""
+    from distributed_rl_b200 import replay as R
+    st = R.DeviceReplay(R2D2_N, R.r2d2_fields(R2D2_T), dev)
+    fill_r2d2(st, 1)
+    return st
+
+
+def fill_r2d2(st, seed):
+    st.fill_hash(R2D2_N, seed=seed)
+    g = torch.Generator(device=st.device).manual_seed(seed)
+    st.field_view("action").random_(0, 6, generator=g)
+    st.field_view("reward").normal_(generator=g)
+    for name in ("h0", "h1"):
+        st.field_view(name).normal_(0.0, 0.1, generator=g)
+    st.field_view("notdone").bernoulli_(0.9, generator=g)
+    st.build(torch.rand(R2D2_N, generator=torch.Generator().manual_seed(seed)).to(st.device) + 0.05)
+
+
+def r2d2_stem_pair(iters: int) -> dict:
+    """The pair launch against two single-net launches over the rows of one B = 64 draw, burn-in and window."""
+    from distributed_rl_b200 import replay as R
+    from distributed_rl_b200.learner_common import time_major_rows
+    dev = torch.device("cuda:0")
+    st = r2d2_store(dev)
+    frames = st.field_view("state").view(-1, 4, 84, 84)
+    seq = torch.randperm(R2D2_N, device=dev)[:R2D2_B]
+    rows = time_major_rows(seq, torch.arange(R2D2_T, device=dev).view(R2D2_T, 1))
+    split = R2D2_MEM * R2D2_B
+    on, tg = R.stem_pack_pair(dev)
+    on.pack(torch.randn(16, 4, 3, 3, device=dev) * 0.1)
+    tg.pack(torch.randn(16, 4, 3, 3, device=dev) * 0.1)
+    out = {}
+    for name, r, amax in (("burn_in", rows[:split], False), ("window", rows[split:], True)):
+        n = r.numel()
+        single = [(torch.empty(n, 16, 42, 42, device=dev), torch.empty(n, 16, 42, 42, dtype=torch.uint8, device=dev))
+                  for _ in range(2)]
+        pair = (torch.empty(2, n, 16, 42, 42, device=dev),
+                torch.empty(n, 16, 42, 42, dtype=torch.uint8, device=dev) if amax else None)
+
+        def two_singles():
+            R.stem_fused(frames, r, on, out=single[0])
+            R.stem_fused(frames, r, tg, out=single[1])
+
+        def one_pair():
+            R.stem_fused_pair(frames, r, on, tg, argmax=amax, out=pair)
+
+        ms = {"two_singles": [], "pair": []}
+        for _ in range(3):                                   # alternated, so that both see the same clocks
+            ms["two_singles"].append(time_events(two_singles, iters))
+            ms["pair"].append(time_events(one_pair, iters))
+        torch.cuda.synchronize()
+        for k in range(2):
+            assert torch.equal(pair[0][k], single[k][0]), (name, k)
+        if amax:
+            assert torch.equal(pair[1], single[0][1]), name
+        out[name] = {"stacks": n, "argmax": amax, "two_singles_ms": ms["two_singles"], "pair_ms": ms["pair"]}
+    st.close()
+    return out
+
+
+def r2d2_steps(model: str, steps: int, profiled: bool) -> dict:
+    from distributed_rl_b200 import r2d2
+    dev = torch.device("cuda:0")
+    torch.cuda.empty_cache()
+    torch.cuda.reset_peak_memory_stats(dev)
+    torch.manual_seed(0)
+    cfg = r2d2.R2D2Config(BATCHSIZE=R2D2_B, FIXED_TRAJECTORY=R2D2_T, MEM=R2D2_MEM, REPLAY_MEMORY_LEN=R2D2_N,
+                          LEARNER_DEVICE="cuda:0",
+                          MODEL=r2d2.resnet_model() if model == "resnet" else r2d2.default_r2d2_model())
+    L = r2d2.Learner(cfg, start_replay=False)
+    fill_r2d2(L.memory.store, 1)
+    L.fused_step(use_graph=True)                         # 3 eager warm-ups + capture
+    for _ in range(3):
+        L.fused_step(use_graph=True)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(steps):
+        L.fused_step(use_graph=True)
+    torch.cuda.synchronize()
+    out = {"steps_per_s": steps / (time.perf_counter() - t0),
+           "peak_GB": torch.cuda.max_memory_allocated(dev) / 1e9,
+           "params": sum(p.numel() for p in L.model.parameters())}
+    if profiled:
+        L._graph = None                                  # eager steps from here on
+        out["eager_step_kernels"] = profile_step(L, R2D2_CLASSES)
+    L.memory.store.close()
+    del L
+    torch.cuda.empty_cache()
+    return out
+
+
+def main_r2d2(args, info):
+    res = dict(info, workload="r2d2", B=R2D2_B, T=R2D2_T, MEM=R2D2_MEM)
+    pair = r2d2_stem_pair(args.iters)
+    res["stem_pair"] = pair
+    for name, p in pair.items():
+        print(f"stem {name} ({p['stacks']} stacks per net, argmax {p['argmax']}): pair "
+              f"{min(p['pair_ms']):.3f}-{max(p['pair_ms']):.3f} ms, two single-net launches "
+              f"{min(p['two_singles_ms']):.3f}-{max(p['two_singles_ms']):.3f} ms")
+    for rep in range(2):                                 # alternated, twice: the spread of the step rates
+        for model in ("resnet", "conv"):
+            s = r2d2_steps(model, args.steps, profiled=model == "resnet" and rep == 1)
+            res.setdefault(f"{model}", []).append(s)
+            print(f"r2d2 {model} ({s['params']} parameters) captured step B={R2D2_B} T={R2D2_T}: "
+                  f"{s['steps_per_s']:.2f} steps/s, peak {s['peak_GB']:.2f} GB")
+            split = s.get("eager_step_kernels")
+            if split is not None:
+                parts = ", ".join(f"{k} {v:.1f} ms" for k, v in split.items() if k not in ("total_ms", "top"))
+                print(f"eager {model} step under torch.profiler: kernels {split['total_ms']:.1f} ms: {parts}")
+                for ms, name in split["top"]:
+                    print(f"    {ms:8.2f} ms  {name}")
+    print(json.dumps(res))
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--workload", choices=("impala", "r2d2"), default="impala")
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--iters", type=int, default=20)
     args = ap.parse_args()
@@ -169,6 +310,8 @@ def main():
         sys.exit("bench_impala_resnet needs a CUDA device")
     info = card()
     print(f"# {info['gpu']}, power limit {info['power_limit']}, max SM clock {info['max_sm_clock']}")
+    if args.workload == "r2d2":
+        return main_r2d2(args, info)
     cols = rollouts(1100, 0)
     res = dict(info)
     s = stem_alone(args.iters, cols)
